@@ -452,6 +452,8 @@ DEVI void tg_emit_lane_body(const TgBatchDev& b, const CfgDev& cfg, const EmitIn
     atomicAdd(in.counters + 1, (unsigned long long)bytes_in);
   }
 }
+// The lane emitter's residency is set by its shared memory (LaneShared: 2 CTAs per SM with LANE_STAGE 256, see
+// tg_lane.cuh); 3 here is the register budget (80 registers).
 #ifndef LB_LANE
 #define LB_LANE 3
 #endif

@@ -21,10 +21,15 @@
 
 namespace tgi {
 
+// Bytes staged per lane between two drains.  A drain writes each lane's staged run from an arbitrary 16-byte
+// boundary, so both ends of every run are partial 128-byte lines; a deeper row writes more whole lines per drain.
+// Measured on one H100 SXM at a 700 W power limit, lane-emitter CUDA-event time per 10 M config-2 messages
+// (tools/variants.sh, two runs each): 128: 23.65 ms at 3 resident CTAs per SM, 23.3 at 2 (TGI_LANE_MULT=2);
+// 256: 21.35 at 2 (what its shared memory admits).  More resident warps do not help this kernel (DESIGN.md §7).
 #ifndef LANE_STAGE
-#define LANE_STAGE 128
+#define LANE_STAGE 256
 #endif
-constexpr uint32_t LANE_STAGE_BYTES = LANE_STAGE;             // staged per lane between two drains (128 or 64)
+constexpr uint32_t LANE_STAGE_BYTES = LANE_STAGE;             // staged per lane between two drains (64, 128 or 256)
 constexpr uint32_t LANE_STAGE_ROW = LANE_STAGE_BYTES + 16;    // +16 spreads the lanes' rows over the banks
 
 struct LaneStream {

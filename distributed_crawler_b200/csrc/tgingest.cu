@@ -1148,7 +1148,7 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       for (int k = 0; k < 3; k++) ei.list[k] = s.d_lists.as<uint32_t>() + (size_t)k * n;
       ei.list_count = (uint32_t*)(dsc + SC_LISTS);
       ei.lane_text_max = LANE_TEXT_MAX;
-      // one LANE per record (tg_lane.cuh): 3 resident CTAs per SM by shared memory, persistent over the record groups
+      // one LANE per record (tg_lane.cuh): 2 resident CTAs per SM by shared memory, persistent over the record groups
       static const unsigned lane_mult = [] { const char* e = getenv("TGI_LANE_MULT"); return e && atoi(e) > 0 ? (unsigned)atoi(e) : 24u; }();  // H100: 12, 24 and 48 within 0.3 ms of each other
       unsigned gl = (unsigned)std::min<uint64_t>(ctas, (uint64_t)c->sms * lane_mult);
       tg_emit_lane_kernel<<<gl, CTA_THREADS, sizeof(LaneShared), st>>>(b, cfg, ei);
