@@ -11,6 +11,7 @@
 //   join_*                                 message-status join (SURVEY 8f)
 // yt_size_kernel is the warp-per-record predecessor of the YouTube lane sizer, kept as an A/B reference (TGI_YT_WARP).
 #pragma once
+#include "scalars.cuh"
 #include "tg_walk.cuh"
 #include "tg_lane.cuh"
 #include "yt_walk.cuh"
@@ -40,11 +41,6 @@ constexpr int CTA_THREADS = WARPS_PER_CTA * 32;
 #ifndef LB_YT
 #define LB_YT 4  // per 2 M config-4 records, same H100: 4: 31.6 ms, 5: 33.6, 6: 35.3, 7: 41.7, 8: 41.7 (tools/variants_yt.sh)
 #endif
-
-#define ERR_ARENA_OVERFLOW 1
-#define ERR_TOO_MANY_REACTIONS 2
-#define ERR_FRONTIER_FULL 4
-#define ERR_TOO_MANY_LINKS 8
 
 // ---- batch validation: every offset the kernels will follow stays inside its array ------------------------------
 // A malformed batch that crossed the C ABI must come back as TGI_E_ARG, not as an illegal address (or as foreign
@@ -681,7 +677,7 @@ DEVI void yt_emit_record(const YtBatchDev& b, const CfgDev& cfg, const YtOut& o,
   w.el[1] = o.esc_len[3 * r + 1];
   w.p = out + line_off[r];
   walk_yt_record(w, a);
-  if (lane_id() == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, 16);
+  if (lane_id() == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, ERR_LINE_MISMATCH);
   __syncwarp();
 }
 __global__ void __launch_bounds__(CTA_THREADS, LB_YT) yt_emit_kernel(YtBatchDev b, CfgDev cfg, YtOut o, const uint64_t* line_off, uint8_t* out, int* err,
@@ -720,7 +716,7 @@ __global__ void __launch_bounds__(CTA_THREADS, LB_YT) yt_emit_lane_kernel(YtBatc
       w.begin((uint64_t)(uintptr_t)out + line_off[r]);
       walk_yt_record(w, a);
       w.end();
-      if (w.s.pos != (uint64_t)(uintptr_t)out + line_off[r + 1]) atomicOr(err, 16);
+      if (w.s.pos != (uint64_t)(uintptr_t)out + line_off[r + 1]) atomicOr(err, ERR_LINE_MISMATCH);
     }
     __syncwarp();
     w.flush_pending(active);
@@ -792,7 +788,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 4) gm_emit_kernel(GmBatchDev b, C
     w.sc = &scs[wid];
     w.p = out + line_off[r];
     walk_gm_record(w, b, cfg, r);
-    if (l == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, 16);
+    if (l == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, ERR_LINE_MISMATCH);
   }
 }
 

@@ -28,8 +28,21 @@
 namespace tgi {
 namespace cg = cooperative_groups;
 
-#define ERR_PAGE_OVERFLOW 64
-constexpr int PAGE_TRACE_AT = 16, PAGE_PHASES = 7;  // scalars[16 .. 16 + 8): start, after each barrier, end
+// the offsets, the result block and the frontier of a page launch (both record kinds)
+struct PageResult {
+  uint64_t* scalars;       // SC_* (first bytes of the result block)
+  uint64_t* line_off;      // [n+1] result block
+  uint64_t* link_off;      // [n+1] scratch
+  uint32_t* link_off32;    // [n+1] result block
+  uint8_t* var;            // result block: links (36 bytes each), then the JSONL at the next 256-byte boundary
+  uint64_t var_cap;
+  uint64_t max_out;        // tgi_config.max_out_bytes (0 = no limit): a page over it falls back BEFORE the frontier is touched
+  FrontierDev fr;
+  FrontierBatch fb;
+  ExclusionDev excl;
+  uint64_t bslots;
+  uint64_t* new_off;       // [n+1]
+};
 
 struct PageArgs {
   TgBatchDev b;
@@ -43,22 +56,7 @@ struct PageArgs {
   uint64_t* chan_off;
   uint8_t* chan_blob;
   uint64_t chan_blob_cap;
-  // offsets and the result block
-  uint64_t* scalars;       // SC_* (first bytes of the result block)
-  uint64_t* line_off;      // [n+1] result block
-  uint64_t* link_off;      // [n+1] scratch
-  uint32_t* link_off32;    // [n+1] result block
-  uint8_t* var;            // result block: links (36 bytes each), then the JSONL at the next 256-byte boundary
-  uint64_t var_cap;
-  uint64_t max_out;        // tgi_config.max_out_bytes (0 = no limit): a page over it falls back BEFORE the frontier is touched
-  // frontier
-  FrontierDev fr;
-  FrontierBatch fb;
-  ExclusionDev excl;
-  uint64_t bslots;
-  uint64_t* new_off;       // [n+1]
-  // indices into `scalars`
-  int sc_chan_total, sc_line_total, sc_link_total, sc_new, sc_count;
+  PageResult res;
 };
 
 // exclusive scan u32[n] -> u64[n+1] by ONE CTA of CTA_THREADS threads (all of them call it)
@@ -126,21 +124,21 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) tg_page_kernel(const __grid_co
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      a.scalars[PAGE_TRACE_AT + phase] = t;
+      a.res.scalars[PAGE_TRACE_AT + phase] = t;
     }
     phase++;
   };
   stamp();
   // slowest record of the per-record phases: (cycles << 32 | record), atomicMax'd behind the phase clock
   auto slowest = [&](int k, long long t_begin, uint64_t r) {
-    if (l == 0) atomicMax((unsigned long long*)&a.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + k],
+    if (l == 0) atomicMax((unsigned long long*)&a.res.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + k],
                           ((unsigned long long)(clock64() - t_begin) << 32) | (unsigned long long)(r & 0xffffffffu));
   };
-  if (blockIdx.x == 0 && threadIdx.x < 3) a.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + threadIdx.x] = 0;
+  if (blockIdx.x == 0 && threadIdx.x < 3) a.res.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + threadIdx.x] = 0;
 
   // P0
-  if (blockIdx.x == 0 && (int)threadIdx.x < a.sc_count) a.scalars[threadIdx.x] = 0;
-  if (want_fr) grid_zero16(a.fb.btable, a.bslots * 8);
+  if (blockIdx.x == 0 && (int)threadIdx.x < SC_COUNT) a.res.scalars[threadIdx.x] = 0;
+  if (want_fr) grid_zero16(a.res.fb.btable, a.res.bslots * 8);
   if (want_json) {
     grid_zero16(a.chan_blob, a.chan_blob_cap);  // segment padding must read as zero
     tg_chan_size_body(a.b, a.chan_derived, a.chan_len);
@@ -167,14 +165,14 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) tg_page_kernel(const __grid_co
     slowest(0, tb, r);
   }
   if (want_json && blockIdx.x == last) {
-    cta_scan_u32(a.chan_len, a.b.n_chans, a.chan_off, a.scalars + a.sc_chan_total);
+    cta_scan_u32(a.chan_len, a.b.n_chans, a.chan_off, a.res.scalars + SC_CHAN_TOTAL);
     __syncthreads();
     for (uint32_t c = threadIdx.x; c < a.b.n_chans; c += blockDim.x) a.chan_derived[c].off = a.chan_off[c];
   }
   grid.sync();
   stamp();
   if (*(volatile int*)a.po.err & (ERR_ARENA_OVERFLOW | ERR_TOO_MANY_LINKS)) return;  // the host reruns the ordinary pipeline
-  if (want_json && a.scalars[a.sc_chan_total] > a.chan_blob_cap) {
+  if (want_json && a.res.scalars[SC_CHAN_TOTAL] > a.chan_blob_cap) {
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(a.po.err, ERR_PAGE_OVERFLOW);
     return;
   }
@@ -210,33 +208,33 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) tg_page_kernel(const __grid_co
     tg_chan_emit_body(a.b, a.chan_derived, a.chan_off, a.chan_blob, false);
   }
   const uint64_t t0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = (uint64_t)gridDim.x * blockDim.x;
-  if (want_fr) frontier_probe_body(n, a.po.link_start, a.po.link_count, a.po.arena, a.run_flags, a.fr, a.fb, a.excl, t0, nt);
+  if (want_fr) frontier_probe_body(n, a.po.link_start, a.po.link_count, a.po.arena, a.run_flags, a.res.fr, a.res.fb, a.res.excl, t0, nt);
   grid.sync();
   stamp();
 
   // P3
-  if (want_json && blockIdx.x == 0) cta_scan_u32(a.po.linelen, n, a.line_off, a.scalars + a.sc_line_total);
-  if (want_links && blockIdx.x == 1 % gridDim.x) cta_scan_u32(a.po.link_count, n, a.link_off, a.scalars + a.sc_link_total);
-  if (want_fr) frontier_count_body(n, a.po.link_start, a.po.link_count, a.fb, t0, nt);
+  if (want_json && blockIdx.x == 0) cta_scan_u32(a.po.linelen, n, a.res.line_off, a.res.scalars + SC_LINE_TOTAL);
+  if (want_links && blockIdx.x == 1 % gridDim.x) cta_scan_u32(a.po.link_count, n, a.res.link_off, a.res.scalars + SC_LINK_TOTAL);
+  if (want_fr) frontier_count_body(n, a.po.link_start, a.po.link_count, a.res.fb, t0, nt);
   grid.sync();
   stamp();
 
   // P4
   if (want_fr) {
-    if (blockIdx.x == last) cta_scan_u32(a.fb.rec_new, n, a.new_off, a.scalars + a.sc_new);
+    if (blockIdx.x == last) cta_scan_u32(a.res.fb.rec_new, n, a.res.new_off, a.res.scalars + SC_NEW);
     grid.sync();
   }
   stamp();
-  const uint64_t links_bytes = want_links ? (a.scalars[a.sc_link_total] * sizeof(tgi_link) + 255) & ~255ull : 0;
-  const uint64_t line_total = want_json ? a.scalars[a.sc_line_total] : 0;
-  if (links_bytes + line_total > a.var_cap || (a.max_out && line_total > a.max_out)) {
+  const uint64_t links_bytes = want_links ? (a.res.scalars[SC_LINK_TOTAL] * sizeof(tgi_link) + 255) & ~255ull : 0;
+  const uint64_t line_total = want_json ? a.res.scalars[SC_LINE_TOTAL] : 0;
+  if (links_bytes + line_total > a.res.var_cap || (a.res.max_out && line_total > a.res.max_out)) {
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(a.po.err, ERR_PAGE_OVERFLOW);
     return;
   }
 
   // P5
   if (want_json) {
-    uint8_t* out = a.var + links_bytes;
+    uint8_t* out = a.res.var + links_bytes;
     for (uint64_t r = w0; r < n; r += nwarps) {
       if (a.po.status[r] != TGI_ST_EMITTED) continue;
       const long long tb = clock64();
@@ -247,11 +245,11 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) tg_page_kernel(const __grid_co
       wa.v = load_rec_view(a.b, r);
       wa.links = nullptr;
       wa.n_links = 0;
-      const uint64_t lo = a.line_off[r];
+      const uint64_t lo = a.res.line_off[r];
       uint8_t* line = out + lo;
       const uint32_t* xlen_g = a.po.xlen + r * 8;
       uint32_t* xp = a.ei.xpos + r * 8;
-      emit_tg_fixed(line, &wss[wid], &cs, wa, (uint32_t)(a.line_off[r + 1] - lo), xlen_g, xp, a.po.err);
+      emit_tg_fixed(line, &wss[wid], &cs, wa, (uint32_t)(a.res.line_off[r + 1] - lo), xlen_g, xp, a.po.err);
       __syncwarp();  // the offsets of the variable pieces (xpos), written by their owning lanes
       emit_tg_escapes<ESC_ALL>(line, wa, xlen_g, xp, 0xffffffffu);  // every string: no lane emitter ran
       const uint32_t c0 = a.b.comment_off[r], c1 = a.b.comment_off[r + 1];
@@ -266,14 +264,14 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) tg_page_kernel(const __grid_co
     }
   }
   if (want_fr) {
-    frontier_append_body(n, a.po.link_start, a.po.link_count, a.po.arena, a.fr, a.fb, a.new_off, a.po.err, nullptr, t0, nt);
+    frontier_append_body(n, a.po.link_start, a.po.link_count, a.po.arena, a.res.fr, a.res.fb, a.res.new_off, a.po.err, nullptr, t0, nt);
     grid.sync();  // the NEW flags of the links
   }
   stamp();
 
   // P6
-  if (want_links) links_compact_body(n, a.po.link_start, a.po.link_count, a.link_off, a.po.arena, (tgi_link*)a.var, a.link_off32);
-  if (want_fr && blockIdx.x == last && threadIdx.x == 0) frontier_commit_body(a.fr, a.new_off, n, a.scalars + a.sc_new, a.po.err);
+  if (want_links) links_compact_body(n, a.po.link_start, a.po.link_count, a.res.link_off, a.po.arena, (tgi_link*)a.res.var, a.res.link_off32);
+  if (want_fr && blockIdx.x == last && threadIdx.x == 0) frontier_commit_body(a.res.fr, a.res.new_off, n, a.res.scalars + SC_NEW, a.po.err);
   stamp();  // block 0's own end of P6
 }
 

@@ -9,6 +9,7 @@
 #include <cstddef>
 
 #include "dev_common.cuh"
+#include "scalars.cuh"
 #include "tg_links.cuh"
 
 namespace tgi {
@@ -600,7 +601,7 @@ DEVI void emit_tg_fixed(uint8_t* line, WarpScratch* ws, const CtaShared* cs, con
     run += len[k];
   }
   if (__shfl_sync(FULL, incl, 31) != total) {  // sizing and emission disagree: never expected; the host reports it
-    if (l == 0) atomicOr(err, 16);
+    if (l == 0) atomicOr(err, ERR_LINE_MISMATCH);
     return;
   }
 #pragma unroll

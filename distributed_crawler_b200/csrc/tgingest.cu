@@ -58,6 +58,10 @@ struct HostBuf {  // pinned
   void* p = nullptr;
   size_t cap = 0;
   unsigned flags = cudaHostAllocDefault;
+  HostBuf() = default;
+  HostBuf(const HostBuf&) = delete;
+  HostBuf& operator=(const HostBuf&) = delete;
+  ~HostBuf() { release(); }
   cudaError_t ensure(size_t bytes) {
     if (bytes <= cap && p) return cudaSuccess;
     if (p) cudaFreeHost(p);
@@ -78,8 +82,19 @@ struct HostBuf {  // pinned
 
 enum JobKind { JOB_NONE = 0, JOB_TG, JOB_TG_RESIDENT, JOB_TG_UPLOAD, JOB_YT, JOB_YT_RESIDENT, JOB_YT_UPLOAD, JOB_GM, JOB_QUIT };
 
+// one batch's frontier phases: the batch hash table, per-link state, per-record NEW counts and their offsets
+struct FrontierScratch {
+  DevBuf btable, lstate, rec_new, new_off;
+};
+
 struct InsertScratch {
-  DevBuf arena, cnt, lstate, recnew, newoff, btable, tiles, sc;
+  DevBuf arena, cnt, tiles, sc;
+  FrontierScratch fs;
+};
+
+// the buffers behind one device key set (FrontierDev)
+struct SetBufs {
+  DevBuf pool, table, count, payload;
 };
 
 // the NCCL entry points the merge uses, resolved at run time
@@ -101,16 +116,16 @@ struct NcclApi {
 struct Slot {
   int idx = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr, ev_mid = nullptr, ev_p0 = nullptr, ev_p1 = nullptr, ev_e0 = nullptr, ev_e1 = nullptr, ev_f1 = nullptr, ev_fr0 = nullptr, ev_fr1 = nullptr;
+  cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr, ev_p0 = nullptr, ev_p1 = nullptr, ev_e0 = nullptr, ev_e1 = nullptr, ev_f1 = nullptr, ev_fr0 = nullptr, ev_fr1 = nullptr;
   // device inputs
   DevBuf d_recs, d_strs, d_ent_off, d_ents, d_react_off, d_reacts, d_comment_off, d_comments, d_aux,
       d_chans, d_chan_strs;
   // device intermediates / outputs
   DevBuf d_chan_derived, d_chan_len, d_chan_off, d_chan_blob, d_status, d_linelen, d_line_off,
-      d_link_start, d_link_count, d_xlen, d_xpos, d_lists, d_arena, d_lstate, d_rec_new, d_new_off, d_link_off, d_links_out,
-      d_link_off32, d_btable, d_tiles, d_scalars, d_jsonl, d_url_start, d_url_count, d_urls, d_ent_range;
+      d_link_start, d_link_count, d_xlen, d_xpos, d_lists, d_arena, d_link_off, d_links_out, d_link_off32, d_tiles, d_scalars, d_jsonl, d_url_start, d_url_count, d_urls, d_ent_range;
   // pinned host outputs
   HostBuf h_status, h_line_off, h_jsonl, h_link_off, h_links, h_scalars;
+  FrontierScratch fs;
   // page-sized Telegram batches (tg_page.cuh): the input arrays in ONE block / copy, the result arrays in one block / copy
   DevBuf d_page_in, d_page_out;
   HostBuf h_page_in, h_page_out;
@@ -163,7 +178,7 @@ struct tgi_ctx {
   CfgDev cfgdev{};
   std::mutex cfg_mu;
   // frontier: the local set (every key this GPU has seen)
-  DevBuf d_pool, d_table, d_fcount, d_err;
+  SetBufs fr_bufs;
   FrontierDev fr{};
   std::mutex fr_mu;
   cudaEvent_t fr_event = nullptr;
@@ -175,13 +190,13 @@ struct tgi_ctx {
   uint64_t tk_next = 0, tk_serving = 0;
   InsertScratch ins;  // scratch of tgi_frontier_insert* / the merge (under fr_mu)
   // frontier -> validator hand-off: resident exclusion sets (tgi_set_add)
-  DevBuf x_pool[2], x_table[2], x_count[2], x_payload;
+  SetBufs x_bufs[2];
   ExclusionDev excl{};
   // multi-GPU merge: communicator + this rank's partition of the global set
   NcclApi* nccl = nullptr;
   ncclComm_t comm = nullptr;
   int rank = 0, nranks = 1;
-  DevBuf o_pool, o_table, o_count, o_payload;
+  SetBufs o_bufs;
   FrontierDev owned{};
   uint64_t merged_upto = 0, merge_round = 0;
   DevBuf m_cnt, m_all, m_cursor, m_send_keys, m_send_pay, m_recv_keys, m_recv_pay, m_gsize;
@@ -334,28 +349,70 @@ uint64_t next_pow2(uint64_t v) {
   return p;
 }
 
-// exclusive scan u32[n] -> u64[n+1]; total also lands in *d_total
-int launch_scan(tgi_ctx* c, Slot& s, const uint32_t* in, uint64_t n, uint64_t* out, uint64_t* d_total, uint32_t& launches) {
-  if (n <= (uint64_t)SCAN_SMALL_MAX) {  // page-sized batch: one launch instead of three
-    scan_small_kernel<<<1, SCAN_SMALL_THREADS, 0, s.stream>>>(in, n, out, d_total);
+// exclusive scan u32[n] -> u64[n+1]; total also lands in *d_total.  A page-sized n takes one launch instead of three
+// unless `tiled` asks for the three-launch scan (over `tiles`) at every size.
+int launch_scan(tgi_ctx* c, cudaStream_t st, DevBuf& tiles, const uint32_t* in, uint64_t n, uint64_t* out, uint64_t* d_total,
+                uint32_t& launches, bool tiled = false) {
+  if (!tiled && n <= (uint64_t)SCAN_SMALL_MAX) {
+    scan_small_kernel<<<1, SCAN_SMALL_THREADS, 0, st>>>(in, n, out, d_total);
     launches += 1;
     CK(cudaGetLastError());
     return TGI_OK;
   }
   uint64_t ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
   if (ntiles == 0) ntiles = 1;
-  CK(s.d_tiles.ensure(ntiles * 8));
-  scan_tile_sums_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, s.stream>>>(in, n, s.d_tiles.as<uint64_t>());
-  scan_tiles_kernel<<<1, 1024, 0, s.stream>>>(s.d_tiles.as<uint64_t>(), ntiles, d_total);
-  scan_apply_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, s.stream>>>(in, n, s.d_tiles.as<uint64_t>(), d_total, out);
+  CK(tiles.ensure(ntiles * 8));
+  scan_tile_sums_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, st>>>(in, n, tiles.as<uint64_t>());
+  scan_tiles_kernel<<<1, 1024, 0, st>>>(tiles.as<uint64_t>(), ntiles, d_total);
+  scan_apply_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, st>>>(in, n, tiles.as<uint64_t>(), d_total, out);
   launches += 3;
   CK(cudaGetLastError());
   return TGI_OK;
 }
+int launch_scan(tgi_ctx* c, Slot& s, const uint32_t* in, uint64_t n, uint64_t* out, uint64_t* d_total, uint32_t& launches) {
+  return launch_scan(c, s.stream, s.d_tiles, in, n, out, d_total, launches);
+}
 
-template <class T>
-int h2d(tgi_ctx* c, Slot& s, DevBuf& d, const T* src, size_t count) {
-  size_t bytes = count * sizeof(T);
+// Sizes the frontier scratch for a batch of n records and `links` links (the hash table holds at least twice as many
+// slots, the per-link state covers `lstate_rows`) and returns the kernels' view of it.  The table is not zeroed.
+int frontier_scratch(tgi_ctx* c, FrontierScratch& z, uint64_t n, uint64_t links, uint64_t lstate_rows, FrontierBatch& fb) {
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * links, 1024));
+  CK(z.btable.ensure(bslots * 8));
+  CK(z.lstate.ensure((size_t)lstate_rows * 4));
+  CK(z.rec_new.ensure(n * 4));
+  CK(z.new_off.ensure((n + 1) * 8));
+  fb.btable = z.btable.as<uint64_t>();
+  fb.bmask = bslots - 1;
+  fb.lstate = z.lstate.as<uint32_t>();
+  fb.rec_new = z.rec_new.as<uint32_t>();
+  return TGI_OK;
+}
+
+// An empty device key set of `cap` keys in a table of `tslots` slots (with a u64 payload per key if asked), zeroed on
+// slot 0's stream; the caller synchronises.
+int set_alloc(tgi_ctx* c, SetBufs& m, uint64_t cap, uint64_t tslots, bool payload, FrontierDev& f) {
+  cudaStream_t st = c->slots[0].stream;
+  CK(m.pool.ensure(cap * 32));
+  CK(m.table.ensure(tslots * 8));
+  CK(m.count.ensure(16));
+  if (payload) CK(m.payload.ensure(cap * 8));
+  CK(cudaMemsetAsync(m.table.p, 0, tslots * 8, st));
+  CK(cudaMemsetAsync(m.count.p, 0, 16, st));
+  f.pool = m.pool.as<uint8_t>();
+  f.cap = cap;
+  f.table = m.table.as<uint64_t>();
+  f.tmask = tslots - 1;
+  f.count = m.count.as<uint64_t>();
+  f.payload = payload ? m.payload.as<uint64_t>() : nullptr;
+  return TGI_OK;
+}
+
+CfgDev cfg_snapshot(tgi_ctx* c) {
+  std::lock_guard<std::mutex> g(c->cfg_mu);
+  return c->cfgdev;
+}
+
+int h2d(tgi_ctx* c, Slot& s, DevBuf& d, const void* src, size_t bytes) {
   cudaStream_t st = s.stream;
   CK(d.ensure(bytes));
   if (bytes) CK(cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, st));
@@ -382,7 +439,6 @@ int publish(tgi_ctx* c, const void* d_src, HostBuf& h, int n_words, cudaStream_t
   return TGI_OK;
 }
 
-enum { SC_CHAN_TOTAL = 0, SC_LINE_TOTAL = 1, SC_CURSOR = 2, SC_NEW = 3, SC_FSIZE = 4, SC_LINK_TOTAL = 5, SC_LONG = 6, SC_URL_CURSOR = 7, SC_LANE_OUT = 8, SC_LANE_IN = 9, SC_LISTS = 10 /* 3 x u32 */, SC_COUNT = 12 };
 constexpr uint64_t HOST_VALIDATE_MAX = 1u << 16;  // batches up to this many elements are range-checked on the host
 
 // the checks of tg_validate_kernel, on the host (small batches: no extra launch / sync in a page-sized call)
@@ -450,73 +506,67 @@ unsigned grid_mult() {
   return v;
 }
 
-// ---- page-sized batches: one block in, one launch, one block out (tg_page.cuh) ---------------------------------------
+// ---- page-sized batches: one block in, one launch, one block out (tg_page.cuh, yt_page.cuh) ---------------------------
 constexpr uint64_t PAGE_MAX_RECS = 8192;          // the in-kernel scans are single-CTA
 constexpr uint64_t PAGE_MAX_IN_BYTES = 4u << 20;
 bool page_enabled() {
   return getenv("TGI_NO_PAGE") == nullptr;  // A/B switch (read per call): the ordinary pipeline for every size
 }
-struct PageInLayout {
-  size_t off[11], bytes[11], total;
-};
-PageInLayout page_in_layout(const tgi_tg_batch* in, uint64_t n_ents) {
-  const uint64_t n = in->n;
-  const size_t b[11] = {n * sizeof(tgi_tg_rec), in->strs_len, (n + 1) * 4, n_ents * sizeof(tgi_entity), (n + 1) * 4,
-                        in->n_reacts * sizeof(tgi_reaction), (n + 1) * 4, in->n_comments * sizeof(tgi_comment), in->aux_len,
-                        in->n_chans * sizeof(tgi_tg_chan), in->chan_strs_len};
-  PageInLayout L;
-  size_t o = 0;
-  for (int i = 0; i < 11; i++) {
-    L.off[i] = o;
-    L.bytes[i] = b[i];
-    o += (b[i] + PAD + 15) & ~(size_t)15;  // PAD readable zero bytes behind every array, as h2d() leaves them
-  }
-  L.total = o;
-  return L;
+// the size rule of the page kernels, for packing the input and for running it
+bool page_fits(uint64_t n, uint64_t n_chans, uint64_t in_bytes) {
+  return page_enabled() && n && n <= PAGE_MAX_RECS && n_chans <= PAGE_MAX_RECS && in_bytes <= PAGE_MAX_IN_BYTES;
 }
-bool page_sized(const tgi_tg_batch* in, uint64_t n_ents) {
-  if (!page_enabled() || in->n == 0 || in->n > PAGE_MAX_RECS || in->n_chans > PAGE_MAX_RECS) return false;
-  if (in->n + n_ents + in->n_reacts + in->n_comments + in->n_chans > HOST_VALIDATE_MAX) return false;  // validate_tg checked every offset
-  return page_in_layout(in, n_ents).total <= PAGE_MAX_IN_BYTES;
+bool page_run_ok(const Slot& s, uint64_t n, uint64_t n_chans, uint32_t flags) {
+  if (!page_fits(n, n_chans, s.in_bytes)) return false;
+  if (flags & TGI_RUN_NO_D2H) return false;  // a device-resident result keeps the ordinary buffers
+  return (flags & (TGI_RUN_JSONL | TGI_RUN_LINKS | TGI_RUN_FRONTIER)) != 0;
 }
 
-// The eleven input arrays packed into one pinned block and sent with ONE copy (eleven copies + eleven pad memsets are a
-// third of what a 100-message call costs otherwise).  The pack is a host memcpy of the page (tens of KB).
-int upload_tg_page(tgi_ctx* c, Slot& s, const tgi_tg_batch* in, uint64_t n_ents) {
-  const uint64_t n = in->n;
-  const PageInLayout L = page_in_layout(in, n_ents);
-  CK(s.h_page_in.ensure(L.total));
-  CK(s.d_page_in.ensure(L.total));
-  uint8_t* h = s.h_page_in.as<uint8_t>();
-  const void* src[11] = {in->recs, in->strs, in->ent_off, in->ents, in->react_off, in->reacts, in->comment_off, in->comments,
-                         in->aux, in->chans, in->chan_strs};
-  for (int i = 0; i < 11; i++) {
-    if (L.bytes[i]) memcpy(h + L.off[i], src[i], L.bytes[i]);
-    const size_t end = i + 1 < 11 ? L.off[i + 1] : L.total;
-    memset(h + L.off[i] + L.bytes[i], 0, end - L.off[i] - L.bytes[i]);
+// A batch's input arrays on their way to the device, each followed by PAD readable zero bytes.
+struct InArrays {
+  static constexpr int MAX = 11;
+  int k = 0;
+  const void* src[MAX];
+  size_t bytes[MAX];
+  DevBuf* buf[MAX];  // the array's own buffer (ordinary upload)
+  uint8_t* dev[MAX];  // where it landed
+  void add(DevBuf& b, const void* p, size_t n) {
+    buf[k] = &b;
+    src[k] = p;
+    bytes[k] = n;
+    k++;
   }
-  CK(cudaMemcpyAsync(s.d_page_in.p, h, L.total, cudaMemcpyHostToDevice, s.stream));
-  uint8_t* d = s.d_page_in.as<uint8_t>();
-  TgBatchDev& b = s.tg;
-  b.n = n;
-  b.recs = (const tgi_tg_rec*)(d + L.off[0]);
-  b.strs = d + L.off[1];
-  b.ent_off = (const uint32_t*)(d + L.off[2]);
-  b.ents = (const tgi_entity*)(d + L.off[3]);
-  b.react_off = (const uint32_t*)(d + L.off[4]);
-  b.reacts = (const tgi_reaction*)(d + L.off[5]);
-  b.comment_off = (const uint32_t*)(d + L.off[6]);
-  b.comments = (const tgi_comment*)(d + L.off[7]);
-  b.aux = d + L.off[8];
-  b.n_chans = in->n_chans;
-  b.chans = (const tgi_tg_chan*)(d + L.off[9]);
-  b.chan_strs = d + L.off[10];
-  s.n_ents = n_ents;
-  s.n_reacts = in->n_reacts;
-  s.n_comments = in->n_comments;
-  s.chan_strs_len = in->chan_strs_len;
-  for (int i = 0; i < 11; i++) s.in_bytes += L.bytes[i];
-  s.resident = true;  // the element count is below HOST_VALIDATE_MAX: validate_tg has range-checked every offset
+  static size_t packed_size(size_t b) { return (b + PAD + 15) & ~(size_t)15; }
+  size_t packed_total() const {
+    size_t o = 0;
+    for (int i = 0; i < k; i++) o += packed_size(bytes[i]);
+    return o;
+  }
+};
+// `packed`: all arrays in one pinned block and ONE copy (a page-sized batch: eleven copies + eleven pad copies are a
+// third of what a 100-message call costs otherwise; the pack is a host memcpy of tens of KB).  Otherwise one copy per array.
+int upload_arrays(tgi_ctx* c, Slot& s, InArrays& a, bool packed) {
+  if (!packed) {
+    for (int i = 0; i < a.k; i++) {
+      const int rc = h2d(c, s, *a.buf[i], a.src[i], a.bytes[i]);
+      if (rc) return rc;
+      a.dev[i] = a.buf[i]->as<uint8_t>();
+    }
+    return TGI_OK;
+  }
+  const size_t total = a.packed_total();
+  CK(s.h_page_in.ensure(total));
+  CK(s.d_page_in.ensure(total));
+  uint8_t* h = s.h_page_in.as<uint8_t>();
+  size_t o = 0;
+  for (int i = 0; i < a.k; i++) {
+    if (a.bytes[i]) memcpy(h + o, a.src[i], a.bytes[i]);
+    memset(h + o + a.bytes[i], 0, InArrays::packed_size(a.bytes[i]) - a.bytes[i]);
+    a.dev[i] = s.d_page_in.as<uint8_t>() + o;
+    s.in_bytes += a.bytes[i];
+    o += InArrays::packed_size(a.bytes[i]);
+  }
+  CK(cudaMemcpyAsync(s.d_page_in.p, h, total, cudaMemcpyHostToDevice, s.stream));
   return TGI_OK;
 }
 
@@ -527,41 +577,41 @@ int upload_tg(tgi_ctx* c, Slot& s, const tgi_tg_batch* in) {
   uint64_t n = in->n;
   s.in_bytes = 0;
   uint64_t n_ents = n ? in->ent_off[n] : 0;
-  if (page_sized(in, n_ents)) return upload_tg_page(c, s, in, n_ents);
-#define UP(buf, ptr, cnt)                      \
-  rc = h2d(c, s, s.buf, ptr, (size_t)(cnt));   \
+  InArrays a;
+  a.add(s.d_recs, in->recs, n * sizeof(tgi_tg_rec));
+  a.add(s.d_strs, in->strs, in->strs_len);
+  a.add(s.d_ent_off, in->ent_off, (n + 1) * 4);
+  a.add(s.d_ents, in->ents, n_ents * sizeof(tgi_entity));
+  a.add(s.d_react_off, in->react_off, (n + 1) * 4);
+  a.add(s.d_reacts, in->reacts, in->n_reacts * sizeof(tgi_reaction));
+  a.add(s.d_comment_off, in->comment_off, (n + 1) * 4);
+  a.add(s.d_comments, in->comments, in->n_comments * sizeof(tgi_comment));
+  a.add(s.d_aux, in->aux, in->aux_len);
+  a.add(s.d_chans, in->chans, in->n_chans * sizeof(tgi_tg_chan));
+  a.add(s.d_chan_strs, in->chan_strs, in->chan_strs_len);
+  // small batches were range-checked on the host by validate_tg; the others are checked on the device below
+  const bool host_checked = n + n_ents + in->n_reacts + in->n_comments + in->n_chans <= HOST_VALIDATE_MAX;
+  rc = upload_arrays(c, s, a, host_checked && page_fits(n, in->n_chans, a.packed_total()));
   if (rc) return rc;
-  UP(d_recs, in->recs, n);
-  UP(d_strs, in->strs, in->strs_len);
-  UP(d_ent_off, in->ent_off, n + 1);
-  UP(d_ents, in->ents, n_ents);
-  UP(d_react_off, in->react_off, n + 1);
-  UP(d_reacts, in->reacts, in->n_reacts);
-  UP(d_comment_off, in->comment_off, n + 1);
-  UP(d_comments, in->comments, in->n_comments);
-  UP(d_aux, in->aux, in->aux_len);
-  UP(d_chans, in->chans, in->n_chans);
-  UP(d_chan_strs, in->chan_strs, in->chan_strs_len);
-#undef UP
   TgBatchDev& b = s.tg;
   b.n = n;
-  b.recs = s.d_recs.as<tgi_tg_rec>();
-  b.strs = s.d_strs.as<uint8_t>();
-  b.ent_off = s.d_ent_off.as<uint32_t>();
-  b.ents = s.d_ents.as<tgi_entity>();
-  b.react_off = s.d_react_off.as<uint32_t>();
-  b.reacts = s.d_reacts.as<tgi_reaction>();
-  b.comment_off = s.d_comment_off.as<uint32_t>();
-  b.comments = s.d_comments.as<tgi_comment>();
-  b.aux = s.d_aux.as<uint8_t>();
+  b.recs = (const tgi_tg_rec*)a.dev[0];
+  b.strs = a.dev[1];
+  b.ent_off = (const uint32_t*)a.dev[2];
+  b.ents = (const tgi_entity*)a.dev[3];
+  b.react_off = (const uint32_t*)a.dev[4];
+  b.reacts = (const tgi_reaction*)a.dev[5];
+  b.comment_off = (const uint32_t*)a.dev[6];
+  b.comments = (const tgi_comment*)a.dev[7];
+  b.aux = a.dev[8];
   b.n_chans = in->n_chans;
-  b.chans = s.d_chans.as<tgi_tg_chan>();
-  b.chan_strs = s.d_chan_strs.as<uint8_t>();
+  b.chans = (const tgi_tg_chan*)a.dev[9];
+  b.chan_strs = a.dev[10];
   s.n_ents = n_ents;
   s.n_reacts = in->n_reacts;
   s.n_comments = in->n_comments;
   s.chan_strs_len = in->chan_strs_len;
-  if (n + n_ents + in->n_reacts + in->n_comments + in->n_chans > HOST_VALIDATE_MAX) {  // big batch: range-check on the device
+  if (!host_checked) {
     CK(s.d_scalars.ensure(SC_COUNT * 8));
     int* bad = (int*)s.d_scalars.p;
     CK(cudaMemsetAsync(bad, 0, 4, s.stream));
@@ -615,48 +665,160 @@ void turn_pass(tgi_ctx* c, Slot& s) {
   turn_end(c, s);
 }
 
-// scalars block (device + pinned mirror): [0] chan total, [1] line total, [2] cursor(u32)+err(int),
-// [3] n_new, [4] frontier size, [5] link total
+// ---- results ----------------------------------------------------------------------------------------------------------
+enum RecKind { REC_TG, REC_YT, REC_GM };
 
-// shared tail of the Telegram and YouTube pipelines: frontier phases, link compaction, D2H, result
-int finish_batch(tgi_ctx* c, Slot& s, uint64_t n, uint32_t flags, uint64_t line_total, uint32_t arena_used,
-                 uint64_t arena_cap, uint64_t var_bytes, uint32_t launches, tgi_result* out) {
+uint32_t sc_cursor(const uint64_t* hsc) { return ((const uint32_t*)(hsc + SC_CURSOR))[0]; }
+int sc_err(const uint64_t* hsc) { return ((const int*)(hsc + SC_CURSOR))[1]; }
+
+// the device errors that fail a batch once it has run to the end
+int check_dev_err(tgi_ctx* c, int err) {
+  if (err & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)c->fr.cap); return TGI_E_CAPACITY; }
+  if (err & ERR_LINE_MISMATCH) { set_err(c, "internal: sized and emitted line lengths disagree"); return TGI_E_STATE; }
+  return TGI_OK;
+}
+int check_max_out(tgi_ctx* c, uint64_t line_total) {
+  if (c->cfg.max_out_bytes && line_total > c->cfg.max_out_bytes) {
+    set_err(c, "JSONL output %llu bytes exceeds max_out_bytes", (unsigned long long)line_total);
+    return TGI_E_CAPACITY;
+  }
+  return TGI_OK;
+}
+
+struct ResultArrays {  // where a batch's result arrays are, on the host or on the device
+  const uint8_t* status;
+  const uint64_t* line_off;
+  const uint8_t* jsonl;
+  const uint32_t* link_off;
+  const tgi_link* links;
+};
+// Fills *out, the slot's device read-back pointers (tgi_result_read_*), its hand-off state (tgi_pending_edges) and the
+// context stats from a batch that has run to the end; hsc is its scalars block on the host.  `host` is nullptr when the
+// result stays on the device.
+void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, const uint64_t* hsc, uint64_t line_total,
+                 uint32_t launches, const ResultArrays* host, const ResultArrays& dev, tgi_result* out) {
+  const bool want_json = flags & TGI_RUN_JSONL, want_links = flags & TGI_RUN_LINKS, want_fr = flags & TGI_RUN_FRONTIER;
+  memset(out, 0, sizeof *out);
+  out->n = n;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, s.ev_k0, s.ev_k1);
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  out->slot = s.idx;
+  if (n && want_json) {
+    out->var_bytes = hsc[SC_LONG];
+    out->main_bytes_out = hsc[SC_LANE_OUT];
+    out->main_bytes_in = hsc[SC_LANE_IN];
+  }
+  out->jsonl_len = want_json ? line_total : 0;
+  out->n_links = want_links ? hsc[SC_LINK_TOTAL] : 0;
+  out->n_new = want_fr ? hsc[SC_NEW] : 0;
+  out->frontier_size = want_fr ? hsc[SC_FSIZE] : 0;
+  if (host) {
+    out->status = host->status;
+    if (want_json) {
+      out->jsonl = host->jsonl;
+      out->line_off = host->line_off;
+    }
+    if (want_links) {
+      out->link_off = host->link_off;
+      out->links = host->links;
+    }
+  }
+  s.dev_jsonl_len = out->jsonl_len;
+  s.dev_jsonl = dev.jsonl;
+  s.dev_status = dev.status;
+  s.dev_link_off = want_links ? dev.link_off : nullptr;
+  s.dev_links = want_links ? dev.links : nullptr;
+  s.dev_n_links = out->n_links;
+  s.last_n = n;
+  s.last_new = out->n_new;
+  s.last_frontier = want_fr && n;
+  s.last_yt = kind == REC_YT;
+  std::lock_guard<std::mutex> g(c->st_mu);
+  c->stats.records += n;
+  c->stats.bytes_in += s.in_bytes;
+  c->stats.bytes_out += out->jsonl_len;
+  c->stats.links += out->n_links;
+  c->stats.launches += launches;
+  c->stats.kernel_ms_total += ms;
+  if (want_fr) c->stats.frontier_size = out->frontier_size;
+}
+
+// ---- bulk batches -----------------------------------------------------------------------------------------------------
+// the scalars block (device + mapped pinned mirror) and the per-record arrays every bulk pipeline writes; starts the
+// batch's kernel clock and zeroes the scalars
+int bulk_prologue(tgi_ctx* c, Slot& s, uint64_t n) {
+  CK(s.d_scalars.ensure(SC_COUNT * 8));
+  CK(s.h_scalars.ensure(SC_COUNT * 8));
+  CK(s.d_status.ensure(n));
+  CK(s.d_linelen.ensure(n * 4));
+  CK(s.d_line_off.ensure((n + 1) * 8));
+  CK(s.d_link_start.ensure(n * 4));
+  CK(s.d_link_count.ensure(n * 4));
+  CK(cudaEventRecord(s.ev_k0, s.stream));
+  CK(cudaMemsetAsync(s.d_scalars.p, 0, SC_COUNT * 8, s.stream));
+  return TGI_OK;
+}
+
+struct Totals {
+  uint64_t line_total;
+  uint32_t cursor;  // the link arena's fill
+  int err;
+};
+// Between the size and the emit pass: scan the line lengths, publish the scalars block, wait for it and decode it.  An
+// arena overflow comes back in t.err for the caller to handle; the other device errors and max_out_bytes fail the batch.
+int bulk_totals(tgi_ctx* c, Slot& s, uint64_t n, bool want_json, uint32_t& launches, Totals& t) {
+  uint64_t* dsc = s.d_scalars.as<uint64_t>();
+  const uint64_t* hsc = s.h_scalars.as<uint64_t>();
+  if (want_json) {
+    const int rc = launch_scan(c, s, s.d_linelen.as<uint32_t>(), n, s.d_line_off.as<uint64_t>(), dsc + SC_LINE_TOTAL, launches);
+    if (rc) return rc;
+  }
+  CK(cudaGetLastError());
+  const int rc = publish(c, dsc, s.h_scalars, SC_COUNT, s.stream);
+  if (rc) return rc;
+  launches++;
+  trace_slot(s, "parse + size: enqueued");
+  CK(cudaStreamSynchronize(s.stream));
+  trace_slot(s, "parse + size: done");
+  t.line_total = hsc[SC_LINE_TOTAL];
+  t.cursor = sc_cursor(hsc);
+  t.err = sc_err(hsc);
+  if (t.err & ERR_ARENA_OVERFLOW) return TGI_OK;
+  if (t.err & ERR_TOO_MANY_LINKS) { set_err(c, "a record has 2^20 or more link candidates"); return TGI_E_ARG; }
+  return want_json ? check_max_out(c, t.line_total) : TGI_OK;
+}
+
+// shared tail of the bulk pipelines: frontier phases, link compaction, D2H, result
+int finish_batch(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, uint64_t line_total, uint32_t arena_used,
+                 uint64_t arena_cap, uint32_t launches, tgi_result* out) {
   cudaStream_t st = s.stream;
   const bool want_json = flags & TGI_RUN_JSONL, want_links = flags & TGI_RUN_LINKS, want_fr = flags & TGI_RUN_FRONTIER;
   uint64_t* dsc = s.d_scalars.as<uint64_t>();
   uint64_t* hsc = s.h_scalars.as<uint64_t>();
-  int dev_err = 0;
-  s.dev_jsonl_len = want_json ? line_total : 0;
-  s.dev_jsonl = s.d_jsonl.as<uint8_t>();
 
   if (want_fr && n) {
     // frontier phases of different slots are serialised in submission order (tickets)
     turn_begin(c, s);
     std::unique_lock<std::mutex> fg(c->fr_mu);
     if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-    uint64_t bslots = next_pow2(std::max<uint64_t>(2ull * arena_used, 1024));
-    CK(s.d_btable.ensure(bslots * 8));
-    CK(s.d_lstate.ensure((size_t)arena_cap * 4));
-    CK(s.d_rec_new.ensure(n * 4));
-    CK(s.d_new_off.ensure((n + 1) * 8));
-    CK(cudaEventRecord(s.ev_fr0, st));
-    CK(cudaMemsetAsync(s.d_btable.p, 0, bslots * 8, st));
     FrontierBatch fb;
-    fb.btable = s.d_btable.as<uint64_t>();
-    fb.bmask = bslots - 1;
-    fb.lstate = s.d_lstate.as<uint32_t>();
-    fb.rec_new = s.d_rec_new.as<uint32_t>();
+    int rc = frontier_scratch(c, s.fs, n, arena_used, arena_cap, fb);
+    if (rc) return rc;
+    CK(cudaEventRecord(s.ev_fr0, st));
+    CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
     unsigned g = (unsigned)((n + 255) / 256);
     frontier_probe_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
                                              s.d_arena.as<tgi_link>(), flags, c->fr, fb, c->excl);
     frontier_count_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(), fb);
     launches += 2;
-    int rc = launch_scan(c, s, fb.rec_new, n, s.d_new_off.as<uint64_t>(), dsc + SC_NEW, launches);
+    rc = launch_scan(c, s, fb.rec_new, n, s.fs.new_off.as<uint64_t>(), dsc + SC_NEW, launches);
     if (rc) return rc;
     int* derr = (int*)(dsc + SC_CURSOR) + 1;
     frontier_append_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
-                                              s.d_arena.as<tgi_link>(), c->fr, fb, s.d_new_off.as<uint64_t>(), derr);
-    frontier_commit_kernel<<<1, 1, 0, st>>>(c->fr, s.d_new_off.as<uint64_t>(), n, dsc + SC_NEW, derr);
+                                              s.d_arena.as<tgi_link>(), c->fr, fb, s.fs.new_off.as<uint64_t>(), derr);
+    frontier_commit_kernel<<<1, 1, 0, st>>>(c->fr, s.fs.new_off.as<uint64_t>(), n, dsc + SC_NEW, derr);
     launches += 2;
     CK(cudaGetLastError());
     CK(cudaEventRecord(s.ev_fr1, st));
@@ -681,10 +843,7 @@ int finish_batch(tgi_ctx* c, Slot& s, uint64_t n, uint32_t flags, uint64_t line_
   CK(cudaEventRecord(s.ev_k1, st));
   CK(cudaMemcpyAsync(hsc, dsc, SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
 
-  memset(out, 0, sizeof *out);
-  out->n = n;
   const bool d2h = !(flags & TGI_RUN_NO_D2H);
-  uint64_t n_links_total = 0;
   if (d2h) {
     CK(s.h_status.ensure(n + 1));
     CK(cudaMemcpyAsync(s.h_status.p, s.d_status.p, n, cudaMemcpyDeviceToHost, st));
@@ -706,74 +865,105 @@ int finish_batch(tgi_ctx* c, Slot& s, uint64_t n, uint32_t flags, uint64_t line_
   trace_slot(s, "emit + frontier + result copy: enqueued");
   CK(cudaStreamSynchronize(st));
   trace_slot(s, "result landed");
-  dev_err = ((int*)(hsc + SC_CURSOR))[1];
-  if (dev_err & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)c->fr.cap); return TGI_E_CAPACITY; }
-  if (dev_err & 16) { set_err(c, "internal: sized and emitted line lengths disagree"); return TGI_E_STATE; }
-  n_links_total = want_links ? hsc[SC_LINK_TOTAL] : 0;
-  if (n_links_total > arena_used) { set_err(c, "internal: more links than arena rows"); return TGI_E_STATE; }
-  s.dev_status = s.d_status.as<uint8_t>();
-  s.dev_link_off = want_links ? s.d_link_off32.as<uint32_t>() : nullptr;
-  s.dev_links = want_links ? s.d_links_out.as<tgi_link>() : nullptr;
-  s.dev_n_links = n_links_total;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, s.ev_k0, s.ev_k1);
-  out->kernel_ms = ms;
-  out->gpu_launches = launches;
-  out->slot = s.idx;
+  const int rc = check_dev_err(c, sc_err(hsc));
+  if (rc) return rc;
+  if (want_links && hsc[SC_LINK_TOTAL] > arena_used) { set_err(c, "internal: more links than arena rows"); return TGI_E_STATE; }
+  const ResultArrays dev{s.d_status.as<uint8_t>(), s.d_line_off.as<uint64_t>(), s.d_jsonl.as<uint8_t>(), s.d_link_off32.as<uint32_t>(),
+                         s.d_links_out.as<tgi_link>()};
+  const ResultArrays host{s.h_status.as<uint8_t>(), s.h_line_off.as<uint64_t>(), s.h_jsonl.as<uint8_t>(), s.h_link_off.as<uint32_t>(),
+                          s.h_links.as<tgi_link>()};
+  fill_result(c, s, kind, n, flags, hsc, line_total, launches, d2h ? &host : nullptr, dev, out);
   if (n) cudaEventElapsedTime(&out->parse_ms, s.ev_p0, s.ev_p1);
   if (n && want_json) {
     cudaEventElapsedTime(&out->emit_ms, s.ev_e0, s.ev_e1);
     cudaEventElapsedTime(&out->emit_main_ms, s.ev_e0, s.ev_f1);
-    out->var_bytes = var_bytes;
-    out->main_bytes_out = hsc[SC_LANE_OUT];
-    out->main_bytes_in = hsc[SC_LANE_IN];
   }
   if (want_fr && n) cudaEventElapsedTime(&out->frontier_ms, s.ev_fr0, s.ev_fr1);
-  out->jsonl_len = want_json ? line_total : 0;
-  out->n_links = n_links_total;
-  out->n_new = want_fr ? hsc[SC_NEW] : 0;
-  s.last_n = n;
-  s.last_new = out->n_new;
-  s.last_frontier = want_fr && n;
-  s.last_yt = s.tg.n == 0 && s.yt.n == n && n != 0;
-  out->frontier_size = want_fr ? hsc[SC_FSIZE] : 0;
-  if (d2h) {
-    out->status = s.h_status.as<uint8_t>();
-    if (want_json) {
-      out->jsonl = s.h_jsonl.as<uint8_t>();
-      out->line_off = s.h_line_off.as<uint64_t>();
-    }
-    if (want_links) {
-      out->link_off = s.h_link_off.as<uint32_t>();
-      out->links = s.h_links.as<tgi_link>();
-    }
-  }
-  {
-    std::lock_guard<std::mutex> g(c->st_mu);
-    c->stats.records += n;
-    c->stats.bytes_in += s.in_bytes;
-    c->stats.bytes_out += out->jsonl_len;
-    c->stats.links += n_links_total;
-    c->stats.launches += launches;
-    c->stats.kernel_ms_total += ms;
-    if (want_fr) c->stats.frontier_size = out->frontier_size;
-  }
   return TGI_OK;
 }
 
-// One cooperative launch and one result copy for a page-sized batch.  PAGE_FALLBACK: the batch did not fit the
-// estimate-sized result block or the link arena (nothing was committed): run_tg goes on with the ordinary pipeline.
-constexpr int PAGE_FALLBACK = -1000;
-bool page_run_ok(const Slot& s, uint32_t flags) {
-  if (!page_enabled() || s.tg.n == 0 || s.tg.n > PAGE_MAX_RECS || s.tg.n_chans > PAGE_MAX_RECS || s.in_bytes > PAGE_MAX_IN_BYTES) return false;
-  if (flags & TGI_RUN_NO_D2H) return false;  // a device-resident result keeps the ordinary buffers
-  return (flags & (TGI_RUN_JSONL | TGI_RUN_LINKS | TGI_RUN_FRONTIER)) != 0;
+// the outputs of the Telegram parse / size passes, for a link arena of arena_cap rows
+ParseOut tg_parse_out(Slot& s, uint8_t* status, uint64_t* dsc, uint64_t arena_cap) {
+  ParseOut po;
+  po.status = status;
+  po.linelen = s.d_linelen.as<uint32_t>();
+  po.link_start = s.d_link_start.as<uint32_t>();
+  po.link_count = s.d_link_count.as<uint32_t>();
+  po.xlen = s.d_xlen.as<uint32_t>();
+  po.var_total = (unsigned long long*)(dsc + SC_LONG);
+  po.arena = s.d_arena.as<tgi_link>();
+  po.arena_cap = (uint32_t)arena_cap;
+  po.cursor = (uint32_t*)(dsc + SC_CURSOR);
+  po.err = (int*)(dsc + SC_CURSOR) + 1;
+  po.ent_range = s.d_ent_range.as<int2>();
+  return po;
 }
-// ---- shared by the Telegram and the YouTube page paths ------------------------------------------------------------------
+// what the Telegram emit passes read and write besides the batch (ei.out: the caller's)
+EmitIn tg_emit_in(Slot& s, const ParseOut& po, const uint64_t* line_off, uint64_t* dsc, uint64_t n) {
+  EmitIn ei;
+  ei.status = po.status;
+  ei.line_off = line_off;
+  ei.link_start = po.link_start;
+  ei.link_count = po.link_count;
+  ei.xlen = po.xlen;
+  ei.xpos = s.d_xpos.as<uint32_t>();
+  ei.arena = po.arena;
+  ei.out = nullptr;
+  ei.err = po.err;
+  ei.lane_text_max = LANE_TEXT_MAX;
+  ei.counters = (unsigned long long*)(dsc + SC_LANE_OUT);
+  for (int k = 0; k < 3; k++) ei.list[k] = s.d_lists.as<uint32_t>() + (size_t)k * n;  // record indices: n < 2^32 checked at upload
+  ei.list_count = (uint32_t*)(dsc + SC_LISTS);
+  return ei;
+}
+// The outputs of the YouTube parse / size passes.  Upper bounds on the capacities: every URL needs "http://x"
+// (8 bytes), every channel link "youtube.com/" (12 bytes).
+uint64_t yt_arena_cap(const Slot& s) { return s.yt_desc_bytes / 12 + 1024; }
+int yt_parse_out(tgi_ctx* c, Slot& s, uint64_t n, uint8_t* status, uint64_t* dsc, YtOut& yo) {
+  const uint64_t urls_cap = s.yt_desc_bytes / 4 + 1024, arena_cap = yt_arena_cap(s);
+  CK(s.d_linelen.ensure(n * 4));
+  CK(s.d_link_start.ensure(n * 4));
+  CK(s.d_link_count.ensure(n * 4));
+  CK(s.d_url_start.ensure(n * 4));
+  CK(s.d_url_count.ensure(n * 4));
+  CK(s.d_urls.ensure(urls_cap * sizeof(YtUrl)));
+  CK(s.d_arena.ensure(arena_cap * sizeof(tgi_link)));
+  CK(s.d_xlen.ensure(n * 12));
+  yo.status = status;
+  yo.linelen = s.d_linelen.as<uint32_t>();
+  yo.esc_len = s.d_xlen.as<uint32_t>();
+  yo.url_start = s.d_url_start.as<uint32_t>();
+  yo.url_count = s.d_url_count.as<uint32_t>();
+  yo.urls = s.d_urls.as<YtUrl>();
+  yo.urls_cap = (uint32_t)std::min<uint64_t>(urls_cap, 0xFFFFFFFFu);
+  yo.url_cursor = (uint32_t*)(dsc + SC_URL_CURSOR);
+  yo.link_start = s.d_link_start.as<uint32_t>();
+  yo.link_count = s.d_link_count.as<uint32_t>();
+  yo.arena = s.d_arena.as<tgi_link>();
+  yo.arena_cap = (uint32_t)std::min<uint64_t>(arena_cap, 0xFFFFFFFFu);
+  yo.cursor = (uint32_t*)(dsc + SC_CURSOR);
+  yo.err = (int*)(dsc + SC_CURSOR) + 1;
+  return TGI_OK;
+}
+
+// ---- page batches: one cooperative launch and one result copy -----------------------------------------------------------
+// PAGE_FALLBACK: the batch did not fit the estimate-sized result block or the link arena (nothing was committed): the
+// caller goes on with the bulk pipeline on the same resident input.
+constexpr int PAGE_FALLBACK = -1000;
+int page_occupancy(const void* kernel) {  // resident CTAs per SM of a page kernel; 0: no page launches
+  int o = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kernel, CTA_THREADS, 0) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return o;
+}
 struct PageOut {  // the result block: scalars | status | line_off | link_off | links, JSONL
   uint64_t o_status, o_line_off, o_link_off, o_var, var_cap;
 };
-int page_out_prepare(tgi_ctx* c, Slot& s, uint64_t n, PageOut& L) {
+// Lays out and sizes the result block and the frontier scratch, and fills the kernel's result arguments but for the
+// frontier and the exclusion sets, which page_launch_and_read reads under the frontier lock.
+int page_prepare(tgi_ctx* c, Slot& s, uint64_t n, uint64_t arena_cap, uint32_t flags, PageOut& L, PageResult& r) {
   auto up = [](uint64_t v, uint64_t a) { return (v + a - 1) / a * a; };
   L.o_status = 256;
   L.o_line_off = L.o_status + up(n + 1, 16);
@@ -783,15 +973,29 @@ int page_out_prepare(tgi_ctx* c, Slot& s, uint64_t n, PageOut& L) {
   if (const char* v = getenv("TGI_PAGE_VAR_CAP")) L.var_cap = up(strtoull(v, nullptr, 10), 256);  // tests: force the fallback
   CK(s.d_page_out.ensure(L.o_var + L.var_cap));
   CK(s.h_page_out.ensure(L.o_var + L.var_cap));
+  CK(s.d_link_off.ensure((n + 1) * 8));
+  if (flags & TGI_RUN_FRONTIER) {
+    const int rc = frontier_scratch(c, s.fs, n, arena_cap, arena_cap, r.fb);
+    if (rc) return rc;
+    r.bslots = r.fb.bmask + 1;
+  }
+  uint8_t* d = s.d_page_out.as<uint8_t>();
+  r.scalars = (uint64_t*)d;
+  r.line_off = (uint64_t*)(d + L.o_line_off);
+  r.link_off = s.d_link_off.as<uint64_t>();
+  r.link_off32 = (uint32_t*)(d + L.o_link_off);
+  r.var = d + L.o_var;
+  r.var_cap = L.var_cap;
+  r.max_out = c->cfg.max_out_bytes;
+  r.new_off = s.fs.new_off.as<uint64_t>();
   return TGI_OK;
 }
 // launch (in the batch's frontier turn), ONE read of the result block, the result.  PAGE_FALLBACK: nothing was committed.
-int page_launch_and_read(tgi_ctx* c, Slot& s, uint32_t flags, uint64_t n, const void* kernel, void** kargs, int occ, const PageOut& L,
-                         FrontierDev* fr_arg, ExclusionDev* excl_arg, const char* name, bool is_yt, tgi_result* out) {
+int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint64_t n, const void* kernel, void** kargs, int occ,
+                         const PageOut& L, PageResult& r, const char* name, tgi_result* out) {
   cudaStream_t st = s.stream;
   const bool want_json = flags & TGI_RUN_JSONL, want_links = flags & TGI_RUN_LINKS, want_fr = flags & TGI_RUN_FRONTIER;
   auto up = [](uint64_t v, uint64_t a) { return (v + a - 1) / a * a; };
-  const uint64_t o_status = L.o_status, o_line_off = L.o_line_off, o_link_off = L.o_link_off, o_var = L.o_var, var_cap = L.var_cap;
   uint8_t* d = s.d_page_out.as<uint8_t>();
   uint8_t* h = s.h_page_out.as<uint8_t>();
   const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)c->sms * occ, std::max<uint64_t>(1, (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA));
@@ -802,8 +1006,8 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, uint32_t flags, uint64_t n, const 
       turn_begin(c, s);
       fg.lock();
       if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-      *fr_arg = c->fr;
-      *excl_arg = c->excl;
+      r.fr = c->fr;
+      r.excl = c->excl;
     }
     CK(cudaEventRecord(s.ev_k0, st));
     if (cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(CTA_THREADS), kargs, 0, st) != cudaSuccess) {
@@ -817,24 +1021,22 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, uint32_t flags, uint64_t n, const 
     }
   }
   // ONE read of the result block, sized by what the previous pages needed; a second one only for the rest of a bigger page
-  const uint64_t spec = std::min<uint64_t>(var_cap, up((uint64_t)s.page_bpr * n * 5 / 4 + 4096, 256));
-  CK(cudaMemcpyAsync(h, d, o_var + spec, cudaMemcpyDeviceToHost, st));
+  const uint64_t spec = std::min<uint64_t>(L.var_cap, up((uint64_t)s.page_bpr * n * 5 / 4 + 4096, 256));
+  CK(cudaMemcpyAsync(h, d, L.o_var + spec, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const uint64_t* hsc = (const uint64_t*)h;
-  const int dev_err = ((const int*)(hsc + SC_CURSOR))[1];
+  const int dev_err = sc_err(hsc);
   if (dev_err & (ERR_ARENA_OVERFLOW | ERR_TOO_MANY_LINKS | ERR_PAGE_OVERFLOW)) return PAGE_FALLBACK;  // keeps its turn
   turn_end(c, s);
-  if (dev_err & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)c->fr.cap); return TGI_E_CAPACITY; }
-  if (dev_err & 16) { set_err(c, "internal: sized and emitted line lengths disagree"); return TGI_E_STATE; }
+  int rc = check_dev_err(c, dev_err);
+  if (rc) return rc;
   const uint64_t line_total = want_json ? hsc[SC_LINE_TOTAL] : 0, n_links_total = want_links ? hsc[SC_LINK_TOTAL] : 0;
   const uint64_t links_bytes = want_links ? up(n_links_total * sizeof(tgi_link), 256) : 0;
-  if (want_json && c->cfg.max_out_bytes && line_total > c->cfg.max_out_bytes) {
-    set_err(c, "JSONL output %llu bytes exceeds max_out_bytes", (unsigned long long)line_total);
-    return TGI_E_CAPACITY;
-  }
+  rc = check_max_out(c, line_total);
+  if (rc) return rc;
   const uint64_t need = links_bytes + line_total;
   if (need > spec) {
-    CK(cudaMemcpyAsync(h + o_var + spec, d + o_var + spec, need - spec, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h + L.o_var + spec, d + L.o_var + spec, need - spec, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   if (getenv("TGI_PAGE_TRACE")) {
@@ -848,75 +1050,24 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, uint32_t flags, uint64_t n, const 
     fprintf(stderr, "\n");
   }
   s.page_bpr = (uint32_t)std::min<uint64_t>(1u << 20, (3ull * s.page_bpr + need / n + 1) / 4 + (need > spec ? need / n / 4 : 0));
-
-  memset(out, 0, sizeof *out);
-  out->n = n;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, s.ev_k0, s.ev_k1);
-  out->kernel_ms = ms;
-  out->gpu_launches = 1;
-  out->slot = s.idx;
-  if (want_json) {
-    out->var_bytes = hsc[SC_LONG];
-    out->main_bytes_out = hsc[SC_LANE_OUT];
-    out->main_bytes_in = hsc[SC_LANE_IN];
-  }
-  out->jsonl_len = line_total;
-  out->n_links = n_links_total;
-  out->n_new = want_fr ? hsc[SC_NEW] : 0;
-  out->frontier_size = want_fr ? hsc[SC_FSIZE] : 0;
-  out->status = h + o_status;
-  if (want_json) {
-    out->jsonl = h + o_var + links_bytes;
-    out->line_off = (const uint64_t*)(h + o_line_off);
-  }
-  if (want_links) {
-    out->link_off = (const uint32_t*)(h + o_link_off);
-    out->links = (const tgi_link*)(h + o_var);
-  }
-  s.dev_jsonl_len = line_total;
-  s.dev_jsonl = d + o_var + links_bytes;
-  s.dev_status = d + o_status;
-  s.dev_link_off = want_links ? (const uint32_t*)(d + o_link_off) : nullptr;
-  s.dev_links = want_links ? (const tgi_link*)(d + o_var) : nullptr;
-  s.dev_n_links = n_links_total;
-  s.last_n = n;
-  s.last_new = out->n_new;
-  s.last_frontier = want_fr;
-  s.last_yt = is_yt;
-  {
-    std::lock_guard<std::mutex> g(c->st_mu);
-    c->stats.records += n;
-    c->stats.bytes_in += s.in_bytes;
-    c->stats.bytes_out += out->jsonl_len;
-    c->stats.links += n_links_total;
-    c->stats.launches += 1;
-    c->stats.kernel_ms_total += ms;
-    if (want_fr) c->stats.frontier_size = out->frontier_size;
-  }
+  const ResultArrays dev{d + L.o_status, (const uint64_t*)(d + L.o_line_off), d + L.o_var + links_bytes, (const uint32_t*)(d + L.o_link_off),
+                         (const tgi_link*)(d + L.o_var)};
+  const ResultArrays host{h + L.o_status, (const uint64_t*)(h + L.o_line_off), h + L.o_var + links_bytes, (const uint32_t*)(h + L.o_link_off),
+                          (const tgi_link*)(h + L.o_var)};
+  fill_result(c, s, kind, n, flags, hsc, line_total, 1, &host, dev, out);
   return TGI_OK;
 }
-
 
 int run_tg_page(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   TgBatchDev& b = s.tg;
   const uint64_t n = b.n;
-  const bool want_fr = flags & TGI_RUN_FRONTIER;
-  static const int occ = [] {
-    int o = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, tg_page_kernel, CTA_THREADS, 0) != cudaSuccess) return 0;
-    return o;
-  }();
-  if (occ <= 0) { cudaGetLastError(); return PAGE_FALLBACK; }
+  static const int occ = page_occupancy((const void*)tg_page_kernel);
+  if (occ <= 0) return PAGE_FALLBACK;
   PageArgs pa{};
-  {
-    std::lock_guard<std::mutex> g(c->cfg_mu);
-    pa.cfg = c->cfgdev;
-  }
+  pa.cfg = cfg_snapshot(c);
   pa.run_flags = flags;
   const uint64_t arena_cap = s.n_ents + 2 * n + 1024;
   const uint64_t blob_cap = 8 * s.chan_strs_len + 1024ull * b.n_chans + 1024;
-  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * arena_cap, 1024));
   // scratch (the buffers of the ordinary pipeline, so that tgi_pending_edges finds the same arrays afterwards)
   CK(s.d_linelen.ensure(n * 4));
   CK(s.d_link_start.ensure(n * 4));
@@ -926,83 +1077,25 @@ int run_tg_page(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   CK(s.d_lists.ensure(3 * n * 4));
   CK(s.d_arena.ensure(arena_cap * sizeof(tgi_link)));
   CK(s.d_ent_range.ensure((size_t)s.n_ents * sizeof(int2)));
-  CK(s.d_link_off.ensure((n + 1) * 8));
   CK(s.d_chan_derived.ensure((size_t)b.n_chans * sizeof(ChanDerived)));
   CK(s.d_chan_len.ensure((size_t)b.n_chans * 4));
   CK(s.d_chan_off.ensure(((size_t)b.n_chans + 1) * 8));
   CK(s.d_chan_blob.ensure(blob_cap));
-  if (want_fr) {
-    CK(s.d_btable.ensure(bslots * 8));
-    CK(s.d_lstate.ensure((size_t)arena_cap * 4));
-    CK(s.d_rec_new.ensure(n * 4));
-    CK(s.d_new_off.ensure((n + 1) * 8));
-  }
   PageOut L;
-  {
-    const int rc = page_out_prepare(c, s, n, L);
-    if (rc) return rc;
-  }
-  const uint64_t o_status = L.o_status, o_line_off = L.o_line_off, o_link_off = L.o_link_off, o_var = L.o_var, var_cap = L.var_cap;
-  uint8_t* d = s.d_page_out.as<uint8_t>();
-  uint64_t* dsc = (uint64_t*)d;
-
+  const int rc = page_prepare(c, s, n, arena_cap, flags, L, pa.res);
+  if (rc) return rc;
   b.chan_derived = s.d_chan_derived.as<ChanDerived>();
   b.chan_blob = s.d_chan_blob.as<uint8_t>();
   pa.b = b;
-  ParseOut& po = pa.po;
-  po.status = d + o_status;
-  po.linelen = s.d_linelen.as<uint32_t>();
-  po.link_start = s.d_link_start.as<uint32_t>();
-  po.link_count = s.d_link_count.as<uint32_t>();
-  po.xlen = s.d_xlen.as<uint32_t>();
-  po.var_total = (unsigned long long*)(dsc + SC_LONG);
-  po.arena = s.d_arena.as<tgi_link>();
-  po.arena_cap = (uint32_t)arena_cap;
-  po.cursor = (uint32_t*)(dsc + SC_CURSOR);
-  po.err = (int*)(dsc + SC_CURSOR) + 1;
-  po.ent_range = s.d_ent_range.as<int2>();
-  EmitIn& ei = pa.ei;
-  ei.status = po.status;
-  ei.line_off = (const uint64_t*)(d + o_line_off);
-  ei.link_start = po.link_start;
-  ei.link_count = po.link_count;
-  ei.xlen = po.xlen;
-  ei.xpos = s.d_xpos.as<uint32_t>();
-  ei.arena = po.arena;
-  ei.out = nullptr;
-  ei.err = po.err;
-  ei.lane_text_max = LANE_TEXT_MAX;
-  ei.counters = (unsigned long long*)(dsc + SC_LANE_OUT);
-  for (int k = 0; k < 3; k++) ei.list[k] = s.d_lists.as<uint32_t>() + (size_t)k * n;
-  ei.list_count = (uint32_t*)(dsc + SC_LISTS);
+  pa.po = tg_parse_out(s, s.d_page_out.as<uint8_t>() + L.o_status, pa.res.scalars, arena_cap);
+  pa.ei = tg_emit_in(s, pa.po, pa.res.line_off, pa.res.scalars, n);
   pa.chan_derived = s.d_chan_derived.as<ChanDerived>();
   pa.chan_len = s.d_chan_len.as<uint32_t>();
   pa.chan_off = s.d_chan_off.as<uint64_t>();
   pa.chan_blob = s.d_chan_blob.as<uint8_t>();
   pa.chan_blob_cap = blob_cap;
-  pa.scalars = dsc;
-  pa.line_off = (uint64_t*)(d + o_line_off);
-  pa.link_off = s.d_link_off.as<uint64_t>();
-  pa.link_off32 = (uint32_t*)(d + o_link_off);
-  pa.var = d + o_var;
-  pa.var_cap = var_cap;
-  pa.max_out = c->cfg.max_out_bytes;
-  pa.fr = c->fr;
-  pa.fb.btable = s.d_btable.as<uint64_t>();
-  pa.fb.bmask = bslots - 1;
-  pa.fb.lstate = s.d_lstate.as<uint32_t>();
-  pa.fb.rec_new = s.d_rec_new.as<uint32_t>();
-  pa.excl = c->excl;
-  pa.bslots = bslots;
-  pa.new_off = s.d_new_off.as<uint64_t>();
-  pa.sc_chan_total = SC_CHAN_TOTAL;
-  pa.sc_line_total = SC_LINE_TOTAL;
-  pa.sc_link_total = SC_LINK_TOTAL;
-  pa.sc_new = SC_NEW;
-  pa.sc_count = SC_COUNT;
-
   void* kargs[] = {&pa};
-  return page_launch_and_read(c, s, flags, n, (const void*)tg_page_kernel, kargs, occ, L, &pa.fr, &pa.excl, "tg_page", false, out);
+  return page_launch_and_read(c, s, REC_TG, flags, n, (const void*)tg_page_kernel, kargs, occ, L, pa.res, "tg_page", out);
 }
 
 int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
@@ -1011,33 +1104,25 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   cudaStream_t st = s.stream;
   uint32_t launches = 0;
   const bool want_json = flags & TGI_RUN_JSONL;
-  CfgDev cfg;
-  {
-    std::lock_guard<std::mutex> g(c->cfg_mu);
-    cfg = c->cfgdev;
-  }
-  if (page_run_ok(s, flags)) {
+  if (page_run_ok(s, n, b.n_chans, flags)) {
     const int rc = run_tg_page(c, s, flags, out);
     if (rc != PAGE_FALLBACK) return rc;
   }
-  CK(s.d_scalars.ensure(SC_COUNT * 8));
-  CK(s.h_scalars.ensure(SC_COUNT * 8));
-  uint64_t* dsc = s.d_scalars.as<uint64_t>();
-  uint64_t* hsc = s.h_scalars.as<uint64_t>();
-  CK(s.d_status.ensure(n));
-  CK(s.d_linelen.ensure(n * 4));
-  CK(s.d_line_off.ensure((n + 1) * 8));
-  CK(s.d_link_start.ensure(n * 4));
-  CK(s.d_link_count.ensure(n * 4));
+  const CfgDev cfg = cfg_snapshot(c);
   CK(s.d_xlen.ensure(n * 32));
+  CK(s.d_ent_range.ensure((size_t)s.n_ents * sizeof(int2)));
   uint64_t arena_cap = s.n_ents + n / 2 + 1024;
   if (s.d_arena.cap / sizeof(tgi_link) > arena_cap + 8) arena_cap = (s.d_arena.cap - PAD) / sizeof(tgi_link);
+  int rc = bulk_prologue(c, s, n);
+  if (rc) return rc;
+  uint64_t* dsc = s.d_scalars.as<uint64_t>();
+  const uint64_t* hsc = s.h_scalars.as<uint64_t>();
 
-  CK(cudaEventRecord(s.ev_k0, st));
-  int dev_err = 0;
+  Totals t{};
+  ParseOut po{};
   for (int attempt = 0; attempt < 3; attempt++) {
+    if (attempt) CK(cudaMemsetAsync(dsc, 0, SC_COUNT * 8, st));  // the rerun starts from zeroed scalars
     CK(s.d_arena.ensure(arena_cap * sizeof(tgi_link)));
-    CK(cudaMemsetAsync(dsc, 0, SC_COUNT * 8, st));
     if (want_json) {
       CK(s.d_chan_derived.ensure((size_t)b.n_chans * sizeof(ChanDerived)));
       CK(s.d_chan_len.ensure((size_t)b.n_chans * 4));
@@ -1048,22 +1133,10 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
         tg_chan_size_kernel<<<g, CTA_THREADS, 0, st>>>(b, s.d_chan_derived.as<ChanDerived>(), s.d_chan_len.as<uint32_t>());
         launches++;
       }
-      int rc = launch_scan(c, s, s.d_chan_len.as<uint32_t>(), b.n_chans, s.d_chan_off.as<uint64_t>(), dsc + SC_CHAN_TOTAL, launches);
+      rc = launch_scan(c, s, s.d_chan_len.as<uint32_t>(), b.n_chans, s.d_chan_off.as<uint64_t>(), dsc + SC_CHAN_TOTAL, launches);
       if (rc) return rc;
     }
-    ParseOut po;
-    po.status = s.d_status.as<uint8_t>();
-    po.linelen = s.d_linelen.as<uint32_t>();
-    po.link_start = s.d_link_start.as<uint32_t>();
-    po.link_count = s.d_link_count.as<uint32_t>();
-    po.xlen = s.d_xlen.as<uint32_t>();
-    po.var_total = (unsigned long long*)(dsc + SC_LONG);
-    po.arena = s.d_arena.as<tgi_link>();
-    po.arena_cap = (uint32_t)arena_cap;
-    po.cursor = (uint32_t*)(dsc + SC_CURSOR);
-    po.err = (int*)(dsc + SC_CURSOR) + 1;
-    CK(s.d_ent_range.ensure((size_t)s.n_ents * sizeof(int2)));
-    po.ent_range = s.d_ent_range.as<int2>();
+    po = tg_parse_out(s, s.d_status.as<uint8_t>(), dsc, arena_cap);
     if (n) {
       uint64_t want = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
       unsigned g = (unsigned)std::min<uint64_t>(want, (uint64_t)c->sms * grid_mult());
@@ -1083,40 +1156,17 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       }
       CK(cudaEventRecord(s.ev_p1, st));
     }
-    if (want_json) {
-      int rc = launch_scan(c, s, s.d_linelen.as<uint32_t>(), n, s.d_line_off.as<uint64_t>(), dsc + SC_LINE_TOTAL, launches);
-      if (rc) return rc;
-    }
-    CK(cudaGetLastError());
-    {
-      const int rc = publish(c, dsc, s.h_scalars, SC_COUNT, st);
-      if (rc) return rc;
-      launches++;
-    }
-    trace_slot(s, "parse + size: enqueued");
-    CK(cudaStreamSynchronize(st));
-    trace_slot(s, "parse + size: done");
-    dev_err = ((int*)(hsc + SC_CURSOR))[1];
-    uint32_t cursor = ((uint32_t*)(hsc + SC_CURSOR))[0];
-    if (dev_err & ERR_ARENA_OVERFLOW) {
-      arena_cap = (uint64_t)cursor + 1024;  // exact demand is known now: rerun the parse
-      continue;
-    }
-    break;
+    rc = bulk_totals(c, s, n, want_json, launches, t);
+    if (rc) return rc;
+    if (!(t.err & ERR_ARENA_OVERFLOW)) break;
+    arena_cap = (uint64_t)t.cursor + 1024;  // exact demand is known now: rerun the parse
   }
-  if (dev_err & ERR_ARENA_OVERFLOW) { set_err(c, "link arena overflow persisted"); return TGI_E_CAPACITY; }
-  if (dev_err & ERR_TOO_MANY_LINKS) { set_err(c, "a record has 2^20 or more link candidates"); return TGI_E_ARG; }
-  uint64_t chan_total = hsc[SC_CHAN_TOTAL], line_total = hsc[SC_LINE_TOTAL];
-  uint32_t arena_used = ((uint32_t*)(hsc + SC_CURSOR))[0];
-  const uint64_t var_bytes = hsc[SC_LONG];
+  if (t.err & ERR_ARENA_OVERFLOW) { set_err(c, "link arena overflow persisted"); return TGI_E_CAPACITY; }
+  const uint64_t chan_total = hsc[SC_CHAN_TOTAL];
 
   if (want_json) {
-    if (c->cfg.max_out_bytes && line_total > c->cfg.max_out_bytes) {
-      set_err(c, "JSONL output %llu bytes exceeds max_out_bytes", (unsigned long long)line_total);
-      return TGI_E_CAPACITY;
-    }
     CK(s.d_chan_blob.ensure(chan_total));
-    CK(s.d_jsonl.ensure(line_total));
+    CK(s.d_jsonl.ensure(t.line_total));
     if (chan_total) CK(cudaMemsetAsync(s.d_chan_blob.p, 0, chan_total, st));  // segment padding must read as zero
     b.chan_blob = s.d_chan_blob.as<uint8_t>();
     unsigned g = (b.n_chans + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
@@ -1125,16 +1175,6 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       launches++;
     }
     if (n) {
-      EmitIn ei;
-      ei.status = s.d_status.as<uint8_t>();
-      ei.line_off = s.d_line_off.as<uint64_t>();
-      ei.link_start = s.d_link_start.as<uint32_t>();
-      ei.link_count = s.d_link_count.as<uint32_t>();
-      ei.xlen = s.d_xlen.as<uint32_t>();
-      ei.arena = s.d_arena.as<tgi_link>();
-      ei.out = s.d_jsonl.as<uint8_t>();
-      ei.err = (int*)(dsc + SC_CURSOR) + 1;
-      ei.counters = (unsigned long long*)(dsc + SC_LANE_OUT);
       static const bool attr_set = [] {
         return cudaFuncSetAttribute(tg_emit_lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LaneShared)) == cudaSuccess;
       }();
@@ -1143,33 +1183,25 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       const uint64_t ctas = (groups + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
       CK(cudaEventRecord(s.ev_e0, st));
       CK(s.d_xpos.ensure(n * 32));
-      ei.xpos = s.d_xpos.as<uint32_t>();
-      CK(s.d_lists.ensure(3 * n * 4));  // work lists of the clean-up kernels (record indices; n < 2^32 checked at upload)
-      for (int k = 0; k < 3; k++) ei.list[k] = s.d_lists.as<uint32_t>() + (size_t)k * n;
-      ei.list_count = (uint32_t*)(dsc + SC_LISTS);
-      ei.lane_text_max = LANE_TEXT_MAX;
+      CK(s.d_lists.ensure(3 * n * 4));  // work lists of the clean-up kernels
+      EmitIn ei = tg_emit_in(s, po, s.d_line_off.as<uint64_t>(), dsc, n);
+      ei.out = s.d_jsonl.as<uint8_t>();
       // one LANE per record (tg_lane.cuh): 2 resident CTAs per SM by shared memory, persistent over the record groups
       static const unsigned lane_mult = [] { const char* e = getenv("TGI_LANE_MULT"); return e && atoi(e) > 0 ? (unsigned)atoi(e) : 24u; }();  // H100: 12, 24 and 48 within 0.3 ms of each other
       unsigned gl = (unsigned)std::min<uint64_t>(ctas, (uint64_t)c->sms * lane_mult);
       tg_emit_lane_kernel<<<gl, CTA_THREADS, sizeof(LaneShared), st>>>(b, cfg, ei);
+      launches++;
       CK(cudaEventRecord(s.ev_f1, st));
       unsigned gg = (unsigned)std::min<uint64_t>(ctas, (uint64_t)c->sms * grid_mult());
-      static const bool one_esc = getenv("TGI_ESC_ONE") != nullptr;  // A/B: the round-1 single escape kernel
-      if (one_esc) {
-        tg_emit_esc_kernel<ESC_ALL><<<gg, CTA_THREADS, 0, st>>>(b, ei);
-        launches += 1;
-      } else {
-        tg_emit_esc_kernel<ESC_SPARSE><<<gg, CTA_THREADS, 0, st>>>(b, ei);  // descriptions with a few line breaks
-        tg_emit_esc_kernel<ESC_DENSE><<<gg, CTA_THREADS, 0, st>>>(b, ei);   // the other strings that need escaping or are long
-        launches += 2;
-      }
+      tg_emit_esc_kernel<ESC_SPARSE><<<gg, CTA_THREADS, 0, st>>>(b, ei);  // descriptions with a few line breaks
+      tg_emit_esc_kernel<ESC_DENSE><<<gg, CTA_THREADS, 0, st>>>(b, ei);   // the other strings that need escaping or are long
       tg_emit_maps_kernel<<<gg, CTA_THREADS, 0, st>>>(b, ei);  // comment lists, non-trivial maps, long outlink lists
-      launches += 2;
+      launches += 3;
       CK(cudaEventRecord(s.ev_e1, st));
     }
     CK(cudaGetLastError());
   }
-  return finish_batch(c, s, n, flags, line_total, arena_used, arena_cap, var_bytes, launches, out);
+  return finish_batch(c, s, REC_TG, n, flags, t.line_total, t.cursor, arena_cap, launches, out);
 }
 
 int upload_yt(tgi_ctx* c, Slot& s, const tgi_yt_batch* in) {
@@ -1192,42 +1224,18 @@ int upload_yt(tgi_ctx* c, Slot& s, const tgi_yt_batch* in) {
     if (e) { set_err(c, "youtube batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
   }
   s.in_bytes = 0;
-  int rc;
-  YtBatchDev& b = s.yt;
-  const size_t yb[4] = {in->n * sizeof(tgi_yt_rec), in->strs_len, in->n_chans * sizeof(tgi_yt_chan), in->chan_strs_len};
-  size_t yo[5] = {0, 0, 0, 0, 0};
-  for (int i = 0; i < 4; i++) yo[i + 1] = yo[i] + ((yb[i] + PAD + 15) & ~(size_t)15);
-  if (page_enabled() && in->n && in->n <= PAGE_MAX_RECS && in->n_chans <= PAGE_MAX_RECS && yo[4] <= PAGE_MAX_IN_BYTES) {
-    // page-sized: the four arrays in one pinned block, ONE copy (upload_tg_page)
-    CK(s.h_page_in.ensure(yo[4]));
-    CK(s.d_page_in.ensure(yo[4]));
-    uint8_t* h = s.h_page_in.as<uint8_t>();
-    const void* src[4] = {in->recs, in->strs, in->chans, in->chan_strs};
-    for (int i = 0; i < 4; i++) {
-      if (yb[i]) memcpy(h + yo[i], src[i], yb[i]);
-      memset(h + yo[i] + yb[i], 0, yo[i + 1] - yo[i] - yb[i]);
-      s.in_bytes += yb[i];
-    }
-    CK(cudaMemcpyAsync(s.d_page_in.p, h, yo[4], cudaMemcpyHostToDevice, s.stream));
-    uint8_t* d = s.d_page_in.as<uint8_t>();
-    b.recs = (const tgi_yt_rec*)(d + yo[0]);
-    b.strs = d + yo[1];
-    b.chans = (const tgi_yt_chan*)(d + yo[2]);
-    b.chan_strs = d + yo[3];
-  } else {
-#define UP(buf, ptr, cnt)                      \
-  rc = h2d(c, s, s.buf, ptr, (size_t)(cnt));   \
+  InArrays a;
+  a.add(s.d_recs, in->recs, in->n * sizeof(tgi_yt_rec));
+  a.add(s.d_strs, in->strs, in->strs_len);
+  a.add(s.d_chans, in->chans, in->n_chans * sizeof(tgi_yt_chan));
+  a.add(s.d_chan_strs, in->chan_strs, in->chan_strs_len);
+  const int rc = upload_arrays(c, s, a, page_fits(in->n, in->n_chans, a.packed_total()));
   if (rc) return rc;
-    UP(d_recs, in->recs, in->n);
-    UP(d_strs, in->strs, in->strs_len);
-    UP(d_chans, in->chans, in->n_chans);
-    UP(d_chan_strs, in->chan_strs, in->chan_strs_len);
-#undef UP
-    b.recs = s.d_recs.as<tgi_yt_rec>();
-    b.strs = s.d_strs.as<uint8_t>();
-    b.chans = s.d_chans.as<tgi_yt_chan>();
-    b.chan_strs = s.d_chan_strs.as<uint8_t>();
-  }
+  YtBatchDev& b = s.yt;
+  b.recs = (const tgi_yt_rec*)a.dev[0];
+  b.strs = a.dev[1];
+  b.chans = (const tgi_yt_chan*)a.dev[2];
+  b.chan_strs = a.dev[3];
   b.n = in->n;
   b.n_chans = in->n_chans;
   s.yt_desc_bytes = in->strs_len;
@@ -1238,83 +1246,20 @@ int upload_yt(tgi_ctx* c, Slot& s, const tgi_yt_batch* in) {
 
 // a page of the Data API (50 videos) in one cooperative launch (yt_page.cuh); PAGE_FALLBACK as in run_tg_page
 int run_yt_page(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
-  YtBatchDev& b = s.yt;
-  const uint64_t n = b.n;
-  const bool want_fr = flags & TGI_RUN_FRONTIER;
-  static const int occ = [] {
-    int o = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, yt_page_kernel, CTA_THREADS, 0) != cudaSuccess) return 0;
-    return o;
-  }();
-  if (occ <= 0) { cudaGetLastError(); return PAGE_FALLBACK; }
+  const uint64_t n = s.yt.n;
+  static const int occ = page_occupancy((const void*)yt_page_kernel);
+  if (occ <= 0) return PAGE_FALLBACK;
   YtPageArgs pa{};
-  {
-    std::lock_guard<std::mutex> g(c->cfg_mu);
-    pa.cfg = c->cfgdev;
-  }
+  pa.cfg = cfg_snapshot(c);
   pa.run_flags = flags;
-  pa.b = b;
-  // every URL needs "http://x" (8 bytes), every channel link "youtube.com/" (12 bytes): upper bounds, as in run_yt
-  const uint64_t urls_cap = s.yt_desc_bytes / 4 + 1024, arena_cap = s.yt_desc_bytes / 12 + 1024;
-  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * arena_cap, 1024));
-  CK(s.d_linelen.ensure(n * 4));
-  CK(s.d_link_start.ensure(n * 4));
-  CK(s.d_link_count.ensure(n * 4));
-  CK(s.d_url_start.ensure(n * 4));
-  CK(s.d_url_count.ensure(n * 4));
-  CK(s.d_urls.ensure(urls_cap * sizeof(YtUrl)));
-  CK(s.d_arena.ensure(arena_cap * sizeof(tgi_link)));
-  CK(s.d_xlen.ensure(n * 12));
-  CK(s.d_link_off.ensure((n + 1) * 8));
-  if (want_fr) {
-    CK(s.d_btable.ensure(bslots * 8));
-    CK(s.d_lstate.ensure((size_t)arena_cap * 4));
-    CK(s.d_rec_new.ensure(n * 4));
-    CK(s.d_new_off.ensure((n + 1) * 8));
-  }
+  pa.b = s.yt;
   PageOut L;
-  {
-    const int rc = page_out_prepare(c, s, n, L);
-    if (rc) return rc;
-  }
-  uint8_t* d = s.d_page_out.as<uint8_t>();
-  uint64_t* dsc = (uint64_t*)d;
-  YtOut& yo = pa.yo;
-  yo.status = d + L.o_status;
-  yo.linelen = s.d_linelen.as<uint32_t>();
-  yo.esc_len = s.d_xlen.as<uint32_t>();
-  yo.url_start = s.d_url_start.as<uint32_t>();
-  yo.url_count = s.d_url_count.as<uint32_t>();
-  yo.urls = s.d_urls.as<YtUrl>();
-  yo.urls_cap = (uint32_t)urls_cap;
-  yo.url_cursor = (uint32_t*)(dsc + SC_URL_CURSOR);
-  yo.link_start = s.d_link_start.as<uint32_t>();
-  yo.link_count = s.d_link_count.as<uint32_t>();
-  yo.arena = s.d_arena.as<tgi_link>();
-  yo.arena_cap = (uint32_t)arena_cap;
-  yo.cursor = (uint32_t*)(dsc + SC_CURSOR);
-  yo.err = (int*)(dsc + SC_CURSOR) + 1;
-  pa.scalars = dsc;
-  pa.line_off = (uint64_t*)(d + L.o_line_off);
-  pa.link_off = s.d_link_off.as<uint64_t>();
-  pa.link_off32 = (uint32_t*)(d + L.o_link_off);
-  pa.var = d + L.o_var;
-  pa.var_cap = L.var_cap;
-  pa.max_out = c->cfg.max_out_bytes;
-  pa.fr = c->fr;
-  pa.fb.btable = s.d_btable.as<uint64_t>();
-  pa.fb.bmask = bslots - 1;
-  pa.fb.lstate = s.d_lstate.as<uint32_t>();
-  pa.fb.rec_new = s.d_rec_new.as<uint32_t>();
-  pa.excl = c->excl;
-  pa.bslots = bslots;
-  pa.new_off = s.d_new_off.as<uint64_t>();
-  pa.sc_line_total = SC_LINE_TOTAL;
-  pa.sc_link_total = SC_LINK_TOTAL;
-  pa.sc_new = SC_NEW;
-  pa.sc_count = SC_COUNT;
+  int rc = page_prepare(c, s, n, yt_arena_cap(s), flags, L, pa.res);
+  if (rc) return rc;
+  rc = yt_parse_out(c, s, n, s.d_page_out.as<uint8_t>() + L.o_status, pa.res.scalars, pa.yo);
+  if (rc) return rc;
   void* kargs[] = {&pa};
-  return page_launch_and_read(c, s, flags, n, (const void*)yt_page_kernel, kargs, occ, L, &pa.fr, &pa.excl, "yt_page", true, out);
+  return page_launch_and_read(c, s, REC_YT, flags, n, (const void*)yt_page_kernel, kargs, occ, L, pa.res, "yt_page", out);
 }
 
 int run_yt(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
@@ -1323,56 +1268,24 @@ int run_yt(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   cudaStream_t st = s.stream;
   uint32_t launches = 0;
   const bool want_json = flags & TGI_RUN_JSONL;
-  if (page_enabled() && n && n <= PAGE_MAX_RECS && b.n_chans <= PAGE_MAX_RECS && s.in_bytes <= PAGE_MAX_IN_BYTES && !(flags & TGI_RUN_NO_D2H) &&
-      (flags & (TGI_RUN_JSONL | TGI_RUN_LINKS | TGI_RUN_FRONTIER))) {
+  if (page_run_ok(s, n, b.n_chans, flags)) {
     const int rc = run_yt_page(c, s, flags, out);
     if (rc != PAGE_FALLBACK) return rc;
   }
-  CfgDev cfg;
-  {
-    std::lock_guard<std::mutex> g(c->cfg_mu);
-    cfg = c->cfgdev;
-  }
-  CK(s.d_scalars.ensure(SC_COUNT * 8));
-  CK(s.h_scalars.ensure(SC_COUNT * 8));
+  const CfgDev cfg = cfg_snapshot(c);
+  int rc = bulk_prologue(c, s, n);
+  if (rc) return rc;
   uint64_t* dsc = s.d_scalars.as<uint64_t>();
-  uint64_t* hsc = s.h_scalars.as<uint64_t>();
-  CK(s.d_status.ensure(n));
-  CK(s.d_linelen.ensure(n * 4));
-  CK(s.d_line_off.ensure((n + 1) * 8));
-  CK(s.d_link_start.ensure(n * 4));
-  CK(s.d_link_count.ensure(n * 4));
-  CK(s.d_url_start.ensure(n * 4));
-  CK(s.d_url_count.ensure(n * 4));
-  // every URL needs "http://x" (8 bytes), every channel link "youtube.com/" (12 bytes)
-  uint64_t urls_cap = s.yt_desc_bytes / 4 + 1024, arena_cap = s.yt_desc_bytes / 12 + 1024;
-  CK(s.d_urls.ensure(urls_cap * sizeof(YtUrl)));
-  CK(s.d_arena.ensure(arena_cap * sizeof(tgi_link)));
-  CK(cudaEventRecord(s.ev_k0, st));
-  CK(cudaMemsetAsync(dsc, 0, SC_COUNT * 8, st));
   YtOut yo;
-  yo.status = s.d_status.as<uint8_t>();
-  yo.linelen = s.d_linelen.as<uint32_t>();
-  CK(s.d_xlen.ensure(n * 12));
-  yo.esc_len = s.d_xlen.as<uint32_t>();
-  yo.url_start = s.d_url_start.as<uint32_t>();
-  yo.url_count = s.d_url_count.as<uint32_t>();
-  yo.urls = s.d_urls.as<YtUrl>();
-  yo.urls_cap = (uint32_t)std::min<uint64_t>(urls_cap, 0xFFFFFFFFu);
-  yo.url_cursor = (uint32_t*)(dsc + SC_URL_CURSOR);
-  yo.link_start = s.d_link_start.as<uint32_t>();
-  yo.link_count = s.d_link_count.as<uint32_t>();
-  yo.arena = s.d_arena.as<tgi_link>();
-  yo.arena_cap = (uint32_t)std::min<uint64_t>(arena_cap, 0xFFFFFFFFu);
-  yo.cursor = (uint32_t*)(dsc + SC_CURSOR);
-  yo.err = (int*)(dsc + SC_CURSOR) + 1;
+  rc = yt_parse_out(c, s, n, s.d_status.as<uint8_t>(), dsc, yo);
+  if (rc) return rc;
   unsigned g = (unsigned)std::min<uint64_t>((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
+  static const bool yt_warp = getenv("TGI_YT_WARP") != nullptr;  // A/B switch: the warp sizer and writer for every record
   if (n) {
     CK(cudaEventRecord(s.ev_p0, st));
     yt_parse_kernel<<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, yo);
     launches++;
     if (want_json) {
-      static const bool yt_warp = getenv("TGI_YT_WARP") != nullptr;
       if (yt_warp) {
         yt_size_kernel<<<g, CTA_THREADS, 0, st>>>(b, cfg, yo);
       } else {
@@ -1384,31 +1297,14 @@ int run_yt(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
     }
     CK(cudaEventRecord(s.ev_p1, st));
   }
+  Totals t{};
+  rc = bulk_totals(c, s, n, want_json, launches, t);
+  if (rc) return rc;
+  if (t.err & ERR_ARENA_OVERFLOW) { set_err(c, "youtube url/link arena overflow (cannot happen: capacities are upper bounds)"); return TGI_E_CAPACITY; }
   if (want_json) {
-    int rc = launch_scan(c, s, s.d_linelen.as<uint32_t>(), n, s.d_line_off.as<uint64_t>(), dsc + SC_LINE_TOTAL, launches);
-    if (rc) return rc;
-  }
-  CK(cudaGetLastError());
-  {
-    const int rc = publish(c, dsc, s.h_scalars, SC_COUNT, st);
-    if (rc) return rc;
-    launches++;
-  }
-  CK(cudaStreamSynchronize(st));
-  int dev_err = ((int*)(hsc + SC_CURSOR))[1];
-  if (dev_err & ERR_ARENA_OVERFLOW) { set_err(c, "youtube url/link arena overflow (cannot happen: capacities are upper bounds)"); return TGI_E_CAPACITY; }
-  if (dev_err & ERR_TOO_MANY_LINKS) { set_err(c, "a record has 2^20 or more channel-link candidates"); return TGI_E_ARG; }
-  uint64_t line_total = hsc[SC_LINE_TOTAL];
-  uint32_t arena_used = ((uint32_t*)(hsc + SC_CURSOR))[0];
-  if (want_json) {
-    if (c->cfg.max_out_bytes && line_total > c->cfg.max_out_bytes) {
-      set_err(c, "JSONL output %llu bytes exceeds max_out_bytes", (unsigned long long)line_total);
-      return TGI_E_CAPACITY;
-    }
-    CK(s.d_jsonl.ensure(line_total));
+    CK(s.d_jsonl.ensure(t.line_total));
     if (n) {
       CK(cudaEventRecord(s.ev_e0, st));
-      static const bool yt_warp = getenv("TGI_YT_WARP") != nullptr;  // A/B switch: the warp writer for every record
       const uint64_t groups = (n + 31) / 32;
       unsigned gg = (unsigned)std::min<uint64_t>((groups + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
       if (!yt_warp) {
@@ -1422,7 +1318,7 @@ int run_yt(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
     }
     CK(cudaGetLastError());
   }
-  return finish_batch(c, s, n, flags, line_total, arena_used, arena_cap, 0, launches, out);
+  return finish_batch(c, s, REC_YT, n, flags, t.line_total, t.cursor, yt_arena_cap(s), launches, out);
 }
 
 // generic client.Message batch (a12): upload, size, scan, emit; no links
@@ -1446,47 +1342,32 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
   cudaStream_t st = s.stream;
   s.in_bytes = 0;
   s.resident = false;
-  int rc;
-#define UP(buf, ptr, cnt)                      \
-  rc = h2d(c, s, s.buf, ptr, (size_t)(cnt));   \
+  InArrays a;
+  a.add(s.d_recs, in->recs, n * sizeof(tgi_gm_rec));
+  a.add(s.d_strs, in->strs, in->strs_len);
+  a.add(s.d_react_off, in->react_off, in->react_off ? (n + 1) * 4 : 0);
+  a.add(s.d_reacts, in->reacts, in->n_reacts * sizeof(tgi_gm_reaction));
+  a.add(s.d_aux, in->aux, in->aux_len);
+  int rc = upload_arrays(c, s, a, false);
   if (rc) return rc;
-  UP(d_recs, in->recs, n);
-  UP(d_strs, in->strs, in->strs_len);
-  UP(d_react_off, in->react_off, in->react_off ? n + 1 : 0);
-  UP(d_reacts, in->reacts, in->n_reacts);
-  UP(d_aux, in->aux, in->aux_len);
-#undef UP
   GmBatchDev& b = s.gm;
   b.n = n;
-  b.recs = s.d_recs.as<tgi_gm_rec>();
-  b.strs = s.d_strs.as<uint8_t>();
-  b.react_off = in->react_off ? s.d_react_off.as<uint32_t>() : nullptr;
-  b.reacts = s.d_reacts.as<tgi_gm_reaction>();
-  b.aux = s.d_aux.as<uint8_t>();
+  b.recs = (const tgi_gm_rec*)a.dev[0];
+  b.strs = a.dev[1];
+  b.react_off = in->react_off ? (const uint32_t*)a.dev[2] : nullptr;
+  b.reacts = (const tgi_gm_reaction*)a.dev[3];
+  b.aux = a.dev[4];
   uint32_t launches = 0;
   const bool want_json = flags & TGI_RUN_JSONL;
-  CfgDev cfg;
-  {
-    std::lock_guard<std::mutex> g(c->cfg_mu);
-    cfg = c->cfgdev;
-  }
-  CK(s.d_scalars.ensure(SC_COUNT * 8));
-  CK(s.h_scalars.ensure(SC_COUNT * 8));
-  uint64_t* dsc = s.d_scalars.as<uint64_t>();
-  uint64_t* hsc = s.h_scalars.as<uint64_t>();
-  CK(s.d_status.ensure(n));
-  CK(s.d_linelen.ensure(n * 4));
-  CK(s.d_line_off.ensure((n + 1) * 8));
-  CK(s.d_link_start.ensure(n * 4));
-  CK(s.d_link_count.ensure(n * 4));
+  const CfgDev cfg = cfg_snapshot(c);
   CK(s.d_arena.ensure(1024 * sizeof(tgi_link)));
-  CK(cudaEventRecord(s.ev_k0, st));
-  CK(cudaMemsetAsync(dsc, 0, SC_COUNT * 8, st));
+  rc = bulk_prologue(c, s, n);
+  if (rc) return rc;
   if (n) {
     CK(cudaMemsetAsync(s.d_link_start.p, 0, n * 4, st));
     CK(cudaMemsetAsync(s.d_link_count.p, 0, n * 4, st));
   }
-  int* derr = (int*)(dsc + SC_CURSOR) + 1;
+  int* derr = (int*)(s.d_scalars.as<uint64_t>() + SC_CURSOR) + 1;
   unsigned g = (unsigned)std::min<uint64_t>((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
   CK(cudaEventRecord(s.ev_p0, st));
   if (n) {  // the status does not depend on TGI_RUN_JSONL: the size pass always runs
@@ -1494,20 +1375,11 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
     launches++;
   }
   CK(cudaEventRecord(s.ev_p1, st));
-  uint64_t line_total = 0;
+  Totals t{};
   if (want_json) {
-    rc = launch_scan(c, s, s.d_linelen.as<uint32_t>(), n, s.d_line_off.as<uint64_t>(), dsc + SC_LINE_TOTAL, launches);
+    rc = bulk_totals(c, s, n, want_json, launches, t);
     if (rc) return rc;
-    rc = publish(c, dsc, s.h_scalars, SC_COUNT, st);
-    if (rc) return rc;
-    launches++;
-    CK(cudaStreamSynchronize(st));
-    line_total = hsc[SC_LINE_TOTAL];
-    if (c->cfg.max_out_bytes && line_total > c->cfg.max_out_bytes) {
-      set_err(c, "JSONL output %llu bytes exceeds max_out_bytes", (unsigned long long)line_total);
-      return TGI_E_CAPACITY;
-    }
-    CK(s.d_jsonl.ensure(line_total));
+    CK(s.d_jsonl.ensure(t.line_total));
     CK(cudaEventRecord(s.ev_e0, st));
     if (n) {
       gm_emit_kernel<<<g, CTA_THREADS, 0, st>>>(b, cfg, s.d_status.as<uint8_t>(), s.d_line_off.as<uint64_t>(), s.d_jsonl.as<uint8_t>(), derr);
@@ -1517,7 +1389,24 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
     CK(cudaEventRecord(s.ev_e1, st));
     CK(cudaGetLastError());
   }
-  return finish_batch(c, s, n, flags & ~(uint32_t)TGI_RUN_FRONTIER, line_total, 0, 1024, 0, launches, out);
+  return finish_batch(c, s, REC_GM, n, flags & ~(uint32_t)TGI_RUN_FRONTIER, t.line_total, 0, 1024, launches, out);
+}
+
+// ---- jobs -------------------------------------------------------------------------------------------------------------
+// upload (for the kinds that carry a batch), synchronise (upload-only jobs), run; the inputs are the slot's in_* / run_flags
+int run_job(tgi_ctx* c, Slot& s, JobKind job) {
+  if (job == JOB_GM) return run_gm(c, s, s.in_gm, s.run_flags, &s.res);
+  const bool tg = job == JOB_TG || job == JOB_TG_RESIDENT || job == JOB_TG_UPLOAD;
+  const bool upload_only = job == JOB_TG_UPLOAD || job == JOB_YT_UPLOAD;
+  int rc = TGI_OK;
+  if (job != JOB_TG_RESIDENT && job != JOB_YT_RESIDENT) rc = tg ? upload_tg(c, s, s.in_tg) : upload_yt(c, s, s.in_yt);
+  if (rc != TGI_OK) return rc;
+  if (upload_only) {
+    cudaError_t e = cudaStreamSynchronize(s.stream);
+    if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); return TGI_E_CUDA; }
+    return TGI_OK;
+  }
+  return tg ? run_tg(c, s, s.run_flags, &s.res) : run_yt(c, s, s.run_flags, &s.res);
 }
 
 void worker_main(tgi_ctx* c, Slot* s) {
@@ -1530,20 +1419,7 @@ void worker_main(tgi_ctx* c, Slot* s) {
       job = s->job;
     }
     if (job == JOB_QUIT) return;
-    int rc = TGI_OK;
-    if (job == JOB_TG || job == JOB_TG_UPLOAD) rc = upload_tg(c, *s, s->in_tg);
-    if (rc == TGI_OK && job == JOB_TG_UPLOAD) {
-      cudaError_t e = cudaStreamSynchronize(s->stream);
-      if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); rc = TGI_E_CUDA; }
-    }
-    if (rc == TGI_OK && (job == JOB_TG || job == JOB_TG_RESIDENT)) rc = run_tg(c, *s, s->run_flags, &s->res);
-    if (job == JOB_YT || job == JOB_YT_UPLOAD) rc = upload_yt(c, *s, s->in_yt);
-    if (rc == TGI_OK && job == JOB_YT_UPLOAD) {
-      cudaError_t e = cudaStreamSynchronize(s->stream);
-      if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); rc = TGI_E_CUDA; }
-    }
-    if (rc == TGI_OK && (job == JOB_YT || job == JOB_YT_RESIDENT)) rc = run_yt(c, *s, s->run_flags, &s->res);
-    if (job == JOB_GM) rc = run_gm(c, *s, s->in_gm, s->run_flags, &s->res);
+    const int rc = run_job(c, *s, job);
     turn_pass(c, *s);
     {
       std::lock_guard<std::mutex> lk(s->mu);
@@ -1598,19 +1474,14 @@ int run_inline(tgi_ctx* c, int slot, JobKind kind, const tgi_tg_batch* in_tg, co
     if (s.busy) { set_err(c, "slot %d is busy", slot); return TGI_E_STATE; }
     s.busy = true;
     s.done = false;
+    s.in_tg = in_tg;
+    s.in_yt = in_yt;
+    s.in_gm = in_gm;
+    s.run_flags = flags;
   }
   take_ticket(c, s, kind, flags);
   cudaSetDevice(c->device);
-  int rc = TGI_OK;
-  if (kind == JOB_TG) {
-    rc = upload_tg(c, s, in_tg);
-    if (rc == TGI_OK) rc = run_tg(c, s, flags, &s.res);
-  } else if (kind == JOB_YT) {
-    rc = upload_yt(c, s, in_yt);
-    if (rc == TGI_OK) rc = run_yt(c, s, flags, &s.res);
-  } else {
-    rc = run_gm(c, s, in_gm, flags, &s.res);
-  }
+  const int rc = run_job(c, s, kind);
   turn_pass(c, s);
   {
     std::lock_guard<std::mutex> lk(s.mu);
@@ -1672,8 +1543,7 @@ int tgi_create(const tgi_config* cfg, tgi_ctx** out) {
         cudaEventCreate(&s.ev_k0) != cudaSuccess || cudaEventCreate(&s.ev_k1) != cudaSuccess ||
         cudaEventCreate(&s.ev_p0) != cudaSuccess || cudaEventCreate(&s.ev_p1) != cudaSuccess ||
         cudaEventCreate(&s.ev_e0) != cudaSuccess || cudaEventCreate(&s.ev_e1) != cudaSuccess || cudaEventCreate(&s.ev_f1) != cudaSuccess ||
-        cudaEventCreate(&s.ev_fr0) != cudaSuccess || cudaEventCreate(&s.ev_fr1) != cudaSuccess ||
-        cudaEventCreateWithFlags(&s.ev_mid, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreate(&s.ev_fr0) != cudaSuccess || cudaEventCreate(&s.ev_fr1) != cudaSuccess) {
       set_err(c, "stream/event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
       return fail(TGI_E_CUDA);
     }
@@ -1682,20 +1552,11 @@ int tgi_create(const tgi_config* cfg, tgi_ctx** out) {
   // frontier
   uint64_t fcap = cfg->frontier_capacity ? cfg->frontier_capacity : (1ull << 22);
   uint64_t tslots = next_pow2(2 * fcap);
-  if (ctx->d_pool.ensure(fcap * 32) != cudaSuccess || ctx->d_table.ensure(tslots * 8) != cudaSuccess ||
-      ctx->d_fcount.ensure(16) != cudaSuccess) {
+  if (set_alloc(ctx, ctx->fr_bufs, fcap, tslots, false, ctx->fr) != TGI_OK) {
     set_err(c, "frontier allocation failed (%llu keys)", (unsigned long long)fcap);
     return fail(TGI_E_NOMEM);
   }
-  cudaMemsetAsync(ctx->d_table.p, 0, tslots * 8, ctx->slots[0].stream);
-  cudaMemsetAsync(ctx->d_fcount.p, 0, 16, ctx->slots[0].stream);
   cudaStreamSynchronize(ctx->slots[0].stream);
-  ctx->fr.pool = ctx->d_pool.as<uint8_t>();
-  ctx->fr.cap = fcap;
-  ctx->fr.table = ctx->d_table.as<uint64_t>();
-  ctx->fr.tmask = tslots - 1;
-  ctx->fr.count = ctx->d_fcount.as<uint64_t>();
-  ctx->fr.payload = nullptr;
   int rc = build_cfg_blob(ctx);
   if (rc) return fail(rc);
   for (int i = 0; i < TGI_SLOTS; i++) ctx->slots[i].worker = std::thread(worker_main, ctx, &ctx->slots[i]);
@@ -1719,36 +1580,13 @@ void tgi_destroy(tgi_ctx* c) {
       s.worker.join();
     }
     if (s.stream) cudaStreamSynchronize(s.stream);
-    DevBuf* db[] = {&s.d_recs, &s.d_strs, &s.d_ent_off, &s.d_ents, &s.d_react_off, &s.d_reacts, &s.d_comment_off,
-                    &s.d_comments, &s.d_aux, &s.d_chans, &s.d_chan_strs, &s.d_chan_derived, &s.d_chan_len,
-                    &s.d_chan_off, &s.d_chan_blob, &s.d_status, &s.d_linelen, &s.d_line_off, &s.d_link_start,
-                    &s.d_link_count, &s.d_xlen, &s.d_xpos, &s.d_lists, &s.d_arena, &s.d_lstate, &s.d_rec_new, &s.d_new_off, &s.d_link_off,
-                    &s.d_links_out, &s.d_link_off32, &s.d_btable, &s.d_tiles, &s.d_scalars, &s.d_jsonl,
-                    &s.d_url_start, &s.d_url_count, &s.d_urls, &s.d_ent_range, &s.d_page_in, &s.d_page_out};
-    for (DevBuf* d : db) d->release();
-    HostBuf* hb[] = {&s.h_status, &s.h_line_off, &s.h_jsonl, &s.h_link_off, &s.h_links, &s.h_scalars, &s.h_page_in, &s.h_page_out};
-    for (HostBuf* h : hb) h->release();
-    if (s.ev_k0) cudaEventDestroy(s.ev_k0);
-    if (s.ev_k1) cudaEventDestroy(s.ev_k1);
-    if (s.ev_mid) cudaEventDestroy(s.ev_mid);
-    for (cudaEvent_t e : {s.ev_p0, s.ev_p1, s.ev_e0, s.ev_e1, s.ev_f1, s.ev_fr0, s.ev_fr1}) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : {s.ev_k0, s.ev_k1, s.ev_p0, s.ev_p1, s.ev_e0, s.ev_e1, s.ev_f1, s.ev_fr0, s.ev_fr1}) if (e) cudaEventDestroy(e);
     if (s.stream) cudaStreamDestroy(s.stream);
   }
   for (auto& f : c->stg_free) cudaFreeHost(f.second);
   for (auto& f : c->stg_live) cudaFreeHost(f.first);
-  c->stg_free.clear();
-  c->stg_live.clear();
-  c->h_zero.release();
-  c->m_host.release();
-  for (int k = 0; k < 2; k++) { c->x_pool[k].release(); c->x_table[k].release(); c->x_count[k].release(); }
-  c->x_payload.release();
-  c->d_cfg.release();
-  c->d_pool.release();
-  c->d_table.release();
-  c->d_fcount.release();
-  c->d_err.release();
   if (c->fr_event) cudaEventDestroy(c->fr_event);
-  delete c;
+  delete c;  // the device and pinned buffers free themselves
 }
 
 const char* tgi_last_error(tgi_ctx* c) {
@@ -1987,35 +1825,23 @@ static int frontier_insert_locked(tgi_ctx* c, FrontierDev& f, const void* d_keys
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
   CK(z.arena.ensure(n * sizeof(tgi_link)));
   CK(z.cnt.ensure(n * 4));
-  CK(z.lstate.ensure(n * 4));
-  CK(z.recnew.ensure(n * 4));
-  CK(z.newoff.ensure((n + 1) * 8));
   CK(z.sc.ensure(64));
-  uint64_t bslots = next_pow2(std::max<uint64_t>(2 * n, 1024));
-  CK(z.btable.ensure(bslots * 8));
-  CK(cudaMemsetAsync(z.btable.p, 0, bslots * 8, st));
+  FrontierBatch fb;
+  int rc = frontier_scratch(c, z.fs, n, n, n, fb);
+  if (rc) return rc;
+  CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
   CK(cudaMemsetAsync(z.sc.p, 0, 64, st));
   unsigned g = (unsigned)((n + 255) / 256);
   if (!g) g = 1;
   keys_to_links_kernel<<<g, 256, 0, st>>>((const uint8_t*)d_keys, n, z.arena.as<tgi_link>(), z.cnt.as<uint32_t>());
-  FrontierBatch fb;
-  fb.btable = z.btable.as<uint64_t>();
-  fb.bmask = bslots - 1;
-  fb.lstate = z.lstate.as<uint32_t>();
-  fb.rec_new = z.recnew.as<uint32_t>();
   frontier_probe_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), 0, f, fb, ExclusionDev{});
   frontier_count_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), fb);
-  {
-    uint64_t ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
-    if (!ntiles) ntiles = 1;
-    CK(z.tiles.ensure(ntiles * 8));
-    scan_tile_sums_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, st>>>(fb.rec_new, n, z.tiles.as<uint64_t>());
-    scan_tiles_kernel<<<1, 1024, 0, st>>>(z.tiles.as<uint64_t>(), ntiles, z.sc.as<uint64_t>());
-    scan_apply_kernel<<<(unsigned)ntiles, SCAN_THREADS, 0, st>>>(fb.rec_new, n, z.tiles.as<uint64_t>(), z.sc.as<uint64_t>(), z.newoff.as<uint64_t>());
-  }
+  uint32_t launches = 0;  // not reported by the insert API
+  rc = launch_scan(c, st, z.tiles, fb.rec_new, n, z.fs.new_off.as<uint64_t>(), z.sc.as<uint64_t>(), launches, true);
+  if (rc) return rc;
   int* derr = (int*)(z.sc.as<uint64_t>() + 4);
-  frontier_append_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), f, fb, z.newoff.as<uint64_t>(), derr, d_payload);
-  frontier_commit_kernel<<<1, 1, 0, st>>>(f, z.newoff.as<uint64_t>(), n, z.sc.as<uint64_t>() + 1, derr);
+  frontier_append_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), f, fb, z.fs.new_off.as<uint64_t>(), derr, d_payload);
+  frontier_commit_kernel<<<1, 1, 0, st>>>(f, z.fs.new_off.as<uint64_t>(), n, z.sc.as<uint64_t>() + 1, derr);
   if (d_is_new) links_new_flags_kernel<<<g, 256, 0, st>>>(z.arena.as<tgi_link>(), n, (uint8_t*)d_is_new);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->fr_event, st));
@@ -2148,19 +1974,8 @@ int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* sta
   cudaStream_t st = c->slots[0].stream;
   const int k = which == TGI_SET_INVALID ? 0 : 1;
   if (!f->table) {  // first use: same capacity as the dedup set
-    const uint64_t fcap = c->fr.cap, tslots = c->fr.tmask + 1;
-    CK(c->x_pool[k].ensure(fcap * 32));
-    CK(c->x_table[k].ensure(tslots * 8));
-    CK(c->x_count[k].ensure(16));
-    if (k == 0) CK(c->x_payload.ensure(fcap * 8));
-    CK(cudaMemsetAsync(c->x_table[k].p, 0, tslots * 8, st));
-    CK(cudaMemsetAsync(c->x_count[k].p, 0, 16, st));
-    f->pool = c->x_pool[k].as<uint8_t>();
-    f->cap = fcap;
-    f->table = c->x_table[k].as<uint64_t>();
-    f->tmask = tslots - 1;
-    f->count = c->x_count[k].as<uint64_t>();
-    f->payload = k == 0 ? c->x_payload.as<uint64_t>() : nullptr;
+    const int rc = set_alloc(c, c->x_bufs[k], c->fr.cap, c->fr.tmask + 1, k == 0, *f);
+    if (rc) return rc;
   }
   if (!n) return TGI_OK;
   DevBuf dk, dp;
@@ -2226,7 +2041,7 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
   const uint32_t* chan = s.last_yt ? &s.yt.recs->chan_idx : &s.tg.recs->chan_idx;
   const uint32_t stride = s.last_yt ? (uint32_t)sizeof(tgi_yt_rec) : (uint32_t)sizeof(tgi_tg_rec);
   edges_emit_kernel<<<(unsigned)((s.last_n + 255) / 256), 256, 0, st>>>(s.last_n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
-                                                                    s.d_arena.as<tgi_link>(), chan, stride, s.d_new_off.as<uint64_t>(), x,
+                                                                    s.d_arena.as<tgi_link>(), chan, stride, s.fs.new_off.as<uint64_t>(), x,
                                                                     drows.as<tgi_edge>(), m);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(rows, drows.p, m * sizeof(tgi_edge), cudaMemcpyDeviceToHost, st));
@@ -2330,20 +2145,9 @@ int tgi_comm_init(tgi_ctx* c, const uint8_t id[TGI_COMM_ID_BYTES], int rank, int
   c->nranks = nranks;
   // this rank's partition of the global set: sized like the local set (a skewed hash cannot overflow it before the
   // local sets do)
-  const uint64_t fcap = c->fr.cap, tslots = c->fr.tmask + 1;
-  CK(c->o_pool.ensure(fcap * 32));
-  CK(c->o_table.ensure(tslots * 8));
-  CK(c->o_count.ensure(16));
-  CK(c->o_payload.ensure(fcap * 8));
+  const int rc = set_alloc(c, c->o_bufs, c->fr.cap, c->fr.tmask + 1, true, c->owned);
+  if (rc) return rc;
   cudaStream_t st = c->slots[0].stream;
-  CK(cudaMemsetAsync(c->o_table.p, 0, tslots * 8, st));
-  CK(cudaMemsetAsync(c->o_count.p, 0, 16, st));
-  c->owned.pool = c->o_pool.as<uint8_t>();
-  c->owned.cap = fcap;
-  c->owned.table = c->o_table.as<uint64_t>();
-  c->owned.tmask = tslots - 1;
-  c->owned.count = c->o_count.as<uint64_t>();
-  c->owned.payload = c->o_payload.as<uint64_t>();
   CK(c->m_cnt.ensure(64 * 8));
   CK(c->m_all.ensure(64 * 64 * 8));
   CK(c->m_cursor.ensure(64 * 8));

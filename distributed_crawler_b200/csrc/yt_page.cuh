@@ -20,19 +20,7 @@ struct YtPageArgs {
   CfgDev cfg;
   uint32_t run_flags;
   YtOut yo;
-  uint64_t* scalars;
-  uint64_t* line_off;    // [n+1] result block
-  uint64_t* link_off;    // [n+1] scratch
-  uint32_t* link_off32;  // [n+1] result block
-  uint8_t* var;          // result block: links, then the JSONL at the next 256-byte boundary
-  uint64_t var_cap;
-  uint64_t max_out;      // as PageArgs.max_out
-  FrontierDev fr;
-  FrontierBatch fb;
-  ExclusionDev excl;
-  uint64_t bslots;
-  uint64_t* new_off;
-  int sc_line_total, sc_link_total, sc_new, sc_count;
+  PageResult res;
 };
 
 __global__ void __launch_bounds__(CTA_THREADS, 2) yt_page_kernel(const __grid_constant__ YtPageArgs a) {
@@ -49,16 +37,16 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) yt_page_kernel(const __grid_co
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      a.scalars[PAGE_TRACE_AT + phase] = t;
+      a.res.scalars[PAGE_TRACE_AT + phase] = t;
     }
     phase++;
   };
   stamp();
 
   // P0
-  if (blockIdx.x == 0 && (int)threadIdx.x < a.sc_count) a.scalars[threadIdx.x] = 0;
-  if (blockIdx.x == 0 && threadIdx.x < 3) a.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + threadIdx.x] = 0;
-  if (want_fr) grid_zero16(a.fb.btable, a.bslots * 8);
+  if (blockIdx.x == 0 && (int)threadIdx.x < SC_COUNT) a.res.scalars[threadIdx.x] = 0;
+  if (blockIdx.x == 0 && threadIdx.x < 3) a.res.scalars[PAGE_TRACE_AT + PAGE_PHASES + 1 + threadIdx.x] = 0;
+  if (want_fr) grid_zero16(a.res.fb.btable, a.res.bslots * 8);
   grid.sync();
   stamp();
 
@@ -72,45 +60,45 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) yt_page_kernel(const __grid_co
   if (want_json)
     for (uint64_t r = w0; r < n; r += nwarps)
       if (a.yo.status[r] == TGI_ST_EMITTED) yt_size_record(a.b, a.cfg, a.yo, r, &scs[wid]);
-  if (want_fr) frontier_probe_body(n, a.yo.link_start, a.yo.link_count, a.yo.arena, a.run_flags, a.fr, a.fb, a.excl, t0, nt);
+  if (want_fr) frontier_probe_body(n, a.yo.link_start, a.yo.link_count, a.yo.arena, a.run_flags, a.res.fr, a.res.fb, a.res.excl, t0, nt);
   grid.sync();
   stamp();
 
   // P3
-  if (want_json && blockIdx.x == 0) cta_scan_u32(a.yo.linelen, n, a.line_off, a.scalars + a.sc_line_total);
-  if (want_links && blockIdx.x == 1 % gridDim.x) cta_scan_u32(a.yo.link_count, n, a.link_off, a.scalars + a.sc_link_total);
-  if (want_fr) frontier_count_body(n, a.yo.link_start, a.yo.link_count, a.fb, t0, nt);
+  if (want_json && blockIdx.x == 0) cta_scan_u32(a.yo.linelen, n, a.res.line_off, a.res.scalars + SC_LINE_TOTAL);
+  if (want_links && blockIdx.x == 1 % gridDim.x) cta_scan_u32(a.yo.link_count, n, a.res.link_off, a.res.scalars + SC_LINK_TOTAL);
+  if (want_fr) frontier_count_body(n, a.yo.link_start, a.yo.link_count, a.res.fb, t0, nt);
   grid.sync();
   stamp();
 
   // P4
   if (want_fr) {
-    if (blockIdx.x == last) cta_scan_u32(a.fb.rec_new, n, a.new_off, a.scalars + a.sc_new);
+    if (blockIdx.x == last) cta_scan_u32(a.res.fb.rec_new, n, a.res.new_off, a.res.scalars + SC_NEW);
     grid.sync();
   }
   stamp();
-  const uint64_t links_bytes = want_links ? (a.scalars[a.sc_link_total] * sizeof(tgi_link) + 255) & ~255ull : 0;
-  const uint64_t line_total = want_json ? a.scalars[a.sc_line_total] : 0;
-  if (links_bytes + line_total > a.var_cap || (a.max_out && line_total > a.max_out)) {
+  const uint64_t links_bytes = want_links ? (a.res.scalars[SC_LINK_TOTAL] * sizeof(tgi_link) + 255) & ~255ull : 0;
+  const uint64_t line_total = want_json ? a.res.scalars[SC_LINE_TOTAL] : 0;
+  if (links_bytes + line_total > a.res.var_cap || (a.res.max_out && line_total > a.res.max_out)) {
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(a.yo.err, ERR_PAGE_OVERFLOW);
     return;
   }
 
   // P5
   if (want_json) {
-    uint8_t* out = a.var + links_bytes;
+    uint8_t* out = a.res.var + links_bytes;
     for (uint64_t r = w0; r < n; r += nwarps)
-      if (a.yo.status[r] == TGI_ST_EMITTED) yt_emit_record(a.b, a.cfg, a.yo, a.line_off, out, a.yo.err, r, &scs[wid]);
+      if (a.yo.status[r] == TGI_ST_EMITTED) yt_emit_record(a.b, a.cfg, a.yo, a.res.line_off, out, a.yo.err, r, &scs[wid]);
   }
   if (want_fr) {
-    frontier_append_body(n, a.yo.link_start, a.yo.link_count, a.yo.arena, a.fr, a.fb, a.new_off, a.yo.err, nullptr, t0, nt);
+    frontier_append_body(n, a.yo.link_start, a.yo.link_count, a.yo.arena, a.res.fr, a.res.fb, a.res.new_off, a.yo.err, nullptr, t0, nt);
     grid.sync();  // the NEW flags of the links
   }
   stamp();
 
   // P6
-  if (want_links) links_compact_body(n, a.yo.link_start, a.yo.link_count, a.link_off, a.yo.arena, (tgi_link*)a.var, a.link_off32);
-  if (want_fr && blockIdx.x == last && threadIdx.x == 0) frontier_commit_body(a.fr, a.new_off, n, a.scalars + a.sc_new, a.yo.err);
+  if (want_links) links_compact_body(n, a.yo.link_start, a.yo.link_count, a.res.link_off, a.yo.arena, (tgi_link*)a.res.var, a.res.link_off32);
+  if (want_fr && blockIdx.x == last && threadIdx.x == 0) frontier_commit_body(a.res.fr, a.res.new_off, n, a.res.scalars + SC_NEW, a.yo.err);
   stamp();
 }
 
