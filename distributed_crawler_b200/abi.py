@@ -76,7 +76,7 @@ assert EDGE.itemsize == 48
 APPEND_RUN = np.dtype([("chan_idx", "<u4"), ("n_lines", "<u4"), ("first", "<u8"), ("end", "<u8"), ("byte_begin", "<u8"),
                        ("byte_end", "<u8")])  # tgi_append_run
 assert APPEND_RUN.itemsize == 40
-SET_INVALID, SET_DISCOVERED = 1, 2
+SET_FRONTIER, SET_INVALID, SET_DISCOVERED, SET_OWNED = 0, 1, 2, 3  # tgi_set_info / tgi_set_add
 EDGE_PENDING, EDGE_DUPLICATE, EDGE_INVALID_CACHED = 0, 1, 2
 ROWS_STATUS, ROWS_LINK_OFF, ROWS_LINKS = 0, 1, 2  # tgi_result_read_rows
 RUN_SKIP_INVALID = 0x40
@@ -140,6 +140,10 @@ class MergeStatsC(C.Structure):
     _fields_ = [("merges", C.c_uint64), ("keys_sent", C.c_uint64), ("keys_received", C.c_uint64), ("keys_owned", C.c_uint64),
                 ("bytes_sent", C.c_uint64), ("bucket_ms", C.c_double), ("exchange_ms", C.c_double), ("insert_ms", C.c_double),
                 ("last_bucket_ms", C.c_double), ("last_exchange_ms", C.c_double), ("last_insert_ms", C.c_double)]
+
+
+class SetInfoC(C.Structure):  # tgi_set_info_t
+    _fields_ = [("count", C.c_uint64), ("capacity", C.c_uint64), ("table_slots", C.c_uint64), ("grows", C.c_uint64)]
 
 
 class StatsC(C.Structure):

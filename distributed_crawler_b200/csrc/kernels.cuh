@@ -1157,6 +1157,19 @@ __global__ void frontier_commit_kernel(FrontierDev f, const uint64_t* new_off, u
   frontier_commit_body(f, new_off, n, out_new, err);
 }
 
+// growth of a set (tgi_set_growth): index the first n keys of f.pool (already copied from the smaller set) in f.table,
+// zeroed.  Entry format and probe sequence are those of frontier_append_body; the pool order is untouched, so the
+// export order and the NEW flags of later batches are those of a set that was big enough from the start.
+__global__ void set_rehash_kernel(FrontierDev f, uint64_t n) {
+  const uint64_t pi = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pi >= n) return;
+  const uint64_t h = key_hash(load_key(f.pool + 32 * pi));
+  const uint64_t e = (pi + 1) | (((h >> 40) | 1ull) << 40);
+  for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
+    if (f.table[s] == 0 && atomicCAS((unsigned long long*)&f.table[s], 0ull, (unsigned long long)e) == 0) break;
+  }
+}
+
 // ---- multi-GPU merge (SURVEY 8e option A): bucket the new local keys by owner rank ----------------------------------
 DEVI uint32_t key_owner(const Key32& k, uint32_t nranks) { return (uint32_t)((key_hash(k) >> 17) % nranks); }
 __global__ void merge_count_kernel(const uint8_t* pool, uint64_t first, uint64_t m, uint32_t nranks, unsigned long long* cnt) {

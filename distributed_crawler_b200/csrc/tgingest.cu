@@ -51,6 +51,10 @@ struct DevBuf {
     p = nullptr;
     cap = 0;
   }
+  void swap(DevBuf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+  }
   template <class T>
   T* as() const { return (T*)p; }
 };
@@ -92,9 +96,11 @@ struct InsertScratch {
   FrontierScratch fs;
 };
 
-// the buffers behind one device key set (FrontierDev)
+// the buffers behind one device key set (FrontierDev), and what the host knows of its fill
 struct SetBufs {
   DevBuf pool, table, count, payload;
+  uint64_t bound = 0;  // upper bound of the set's count: the keys it held when last read plus every key enqueued since
+  uint64_t grows = 0;  // rehashes into bigger buffers (set_grow)
 };
 
 // the NCCL entry points the merge uses, resolved at run time
@@ -180,6 +186,8 @@ struct tgi_ctx {
   // frontier: the local set (every key this GPU has seen)
   SetBufs fr_bufs;
   FrontierDev fr{};
+  uint64_t fr_cap0 = 0;    // tgi_config.frontier_capacity: the size the dedup set started at
+  uint64_t grow_max = 0;   // tgi_set_growth: sets grow up to this many keys (0: fixed size)
   std::mutex fr_mu;
   cudaEvent_t fr_event = nullptr;
   bool fr_event_valid = false;
@@ -404,6 +412,58 @@ int set_alloc(tgi_ctx* c, SetBufs& m, uint64_t cap, uint64_t tslots, bool payloa
   f.tmask = tslots - 1;
   f.count = m.count.as<uint64_t>();
   f.payload = payload ? m.payload.as<uint64_t>() : nullptr;
+  m.bound = 0;
+  m.grows = 0;
+  return TGI_OK;
+}
+
+// Makes room for up to `need` more keys in set f (buffers m) before a caller inserts them on stream st, when growth is on
+// (tgi_set_growth).  Runs under fr_mu, inside the caller's frontier turn.  The host bound decides without a device round
+// trip; only when it says the set might overflow is the exact count read, and only when that overflows too does the set
+// move into buffers for next_pow2(count + need) keys (at most grow_max): the pool and payload are copied, the bigger
+// table is rebuilt by set_rehash_kernel.  Past grow_max the insert still fails with TGI_E_CAPACITY and leaves the set as
+// it was.
+//
+// Freeing the old buffers: kernels take FrontierDev / ExclusionDev by value, so a kernel enqueued earlier may still read
+// them.  Every such reader runs under fr_mu and either synchronises its stream before it lets go of the lock (inserts,
+// exports, the merge, tgi_pending_edges) or records fr_event behind its kernels (the batches' frontier phases, the page
+// kernels).  This function enqueues its work behind fr_event and synchronises st before it frees anything, so every
+// earlier reader has finished by then, and later ones see only the new buffers.
+int set_grow(tgi_ctx* c, FrontierDev& f, SetBufs& m, uint64_t need, cudaStream_t st) {
+  if (c->grow_max && f.cap < c->grow_max && m.bound + need > f.cap) {
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    uint64_t count = 0;
+    CK(cudaMemcpyAsync(&count, f.count, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    m.bound = count;
+    if (count + need > f.cap) {
+      const uint64_t cap = std::min(next_pow2(count + need), c->grow_max), tslots = next_pow2(2 * cap);
+      SetBufs nb;
+      CK(nb.pool.ensure(cap * 32));
+      CK(nb.table.ensure(tslots * 8));
+      if (f.payload) CK(nb.payload.ensure(cap * 8));
+      CK(cudaMemsetAsync(nb.table.p, 0, tslots * 8, st));
+      FrontierDev g = f;
+      g.pool = nb.pool.as<uint8_t>();
+      g.cap = cap;
+      g.table = nb.table.as<uint64_t>();
+      g.tmask = tslots - 1;
+      g.payload = f.payload ? nb.payload.as<uint64_t>() : nullptr;
+      if (count) {
+        CK(cudaMemcpyAsync(g.pool, f.pool, count * 32, cudaMemcpyDeviceToDevice, st));
+        if (f.payload) CK(cudaMemcpyAsync(g.payload, f.payload, count * 8, cudaMemcpyDeviceToDevice, st));
+        set_rehash_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(g, count);
+        CK(cudaGetLastError());
+      }
+      CK(cudaStreamSynchronize(st));
+      m.pool.swap(nb.pool);  // nb now holds the old buffers and frees them on return
+      m.table.swap(nb.table);
+      m.payload.swap(nb.payload);
+      f = g;
+      m.grows++;
+    }
+  }
+  m.bound += need;
   return TGI_OK;
 }
 
@@ -803,8 +863,10 @@ int finish_batch(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
     turn_begin(c, s);
     std::unique_lock<std::mutex> fg(c->fr_mu);
     if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    int rc = set_grow(c, c->fr, c->fr_bufs, arena_used, st);  // the batch adds at most one key per link
+    if (rc) return rc;
     FrontierBatch fb;
-    int rc = frontier_scratch(c, s.fs, n, arena_used, arena_cap, fb);
+    rc = frontier_scratch(c, s.fs, n, arena_used, arena_cap, fb);
     if (rc) return rc;
     CK(cudaEventRecord(s.ev_fr0, st));
     CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
@@ -960,6 +1022,7 @@ int page_occupancy(const void* kernel) {  // resident CTAs per SM of a page kern
 }
 struct PageOut {  // the result block: scalars | status | line_off | link_off | links, JSONL
   uint64_t o_status, o_line_off, o_link_off, o_var, var_cap;
+  uint64_t links_max;  // the link arena's capacity: an upper bound of the keys the page adds to the frontier
 };
 // Lays out and sizes the result block and the frontier scratch, and fills the kernel's result arguments but for the
 // frontier and the exclusion sets, which page_launch_and_read reads under the frontier lock.
@@ -970,6 +1033,7 @@ int page_prepare(tgi_ctx* c, Slot& s, uint64_t n, uint64_t arena_cap, uint32_t f
   L.o_link_off = L.o_line_off + (n + 1) * 8;
   L.o_var = up(L.o_link_off + (n + 1) * 4, 256);
   L.var_cap = up(6 * s.in_bytes + 3072 * n + 65536, 256);
+  L.links_max = arena_cap;
   if (const char* v = getenv("TGI_PAGE_VAR_CAP")) L.var_cap = up(strtoull(v, nullptr, 10), 256);  // tests: force the fallback
   CK(s.d_page_out.ensure(L.o_var + L.var_cap));
   CK(s.h_page_out.ensure(L.o_var + L.var_cap));
@@ -1008,6 +1072,7 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint
       if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
       r.fr = c->fr;
       r.excl = c->excl;
+      c->fr_bufs.bound += L.links_max;
     }
     CK(cudaEventRecord(s.ev_k0, st));
     if (cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(CTA_THREADS), kargs, 0, st) != cudaSuccess) {
@@ -1027,6 +1092,8 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint
   const uint64_t* hsc = (const uint64_t*)h;
   const int dev_err = sc_err(hsc);
   if (dev_err & (ERR_ARENA_OVERFLOW | ERR_TOO_MANY_LINKS | ERR_PAGE_OVERFLOW)) return PAGE_FALLBACK;  // keeps its turn
+  // a full frontier left the set untouched: with growth on, the bulk pipeline grows it and runs the page again
+  if ((dev_err & ERR_FRONTIER_FULL) && c->grow_max) return PAGE_FALLBACK;
   turn_end(c, s);
   int rc = check_dev_err(c, dev_err);
   if (rc) return rc;
@@ -1552,6 +1619,7 @@ int tgi_create(const tgi_config* cfg, tgi_ctx** out) {
   // frontier
   uint64_t fcap = cfg->frontier_capacity ? cfg->frontier_capacity : (1ull << 22);
   uint64_t tslots = next_pow2(2 * fcap);
+  ctx->fr_cap0 = fcap;
   if (set_alloc(ctx, ctx->fr_bufs, fcap, tslots, false, ctx->fr) != TGI_OK) {
     set_err(c, "frontier allocation failed (%llu keys)", (unsigned long long)fcap);
     return fail(TGI_E_NOMEM);
@@ -1856,7 +1924,9 @@ static int frontier_insert_check(tgi_ctx* c, const FrontierDev& f) {  // after a
 }
 static int frontier_insert_impl(tgi_ctx* c, const void* d_keys, uint64_t n, void* d_is_new) {
   std::unique_lock<std::mutex> fg(c->fr_mu);
-  int rc = frontier_insert_locked(c, c->fr, d_keys, nullptr, n, d_is_new);
+  int rc = set_grow(c, c->fr, c->fr_bufs, n, c->slots[0].stream);
+  if (rc) return rc;
+  rc = frontier_insert_locked(c, c->fr, d_keys, nullptr, n, d_is_new);
   if (rc) return rc;
   CK(cudaStreamSynchronize(c->slots[0].stream));
   return frontier_insert_check(c, c->fr);
@@ -1953,6 +2023,8 @@ int tgi_frontier_clear(tgi_ctx* c) {
   int rc = frontier_clear_set(c, c->fr);
   if (rc == TGI_OK && c->owned.table) rc = frontier_clear_set(c, c->owned);
   if (rc) return rc;
+  c->fr_bufs.bound = 0;
+  c->o_bufs.bound = 0;
   c->merged_upto = 0;
   CK(cudaEventRecord(c->fr_event, st));
   c->fr_event_valid = true;
@@ -1973,11 +2045,15 @@ int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* sta
   std::lock_guard<std::mutex> g(c->fr_mu);
   cudaStream_t st = c->slots[0].stream;
   const int k = which == TGI_SET_INVALID ? 0 : 1;
-  if (!f->table) {  // first use: same capacity as the dedup set
-    const int rc = set_alloc(c, c->x_bufs[k], c->fr.cap, c->fr.tmask + 1, k == 0, *f);
+  if (!f->table) {  // first use: same capacity as the dedup set, or at most 2^16 keys when the sets grow on their own
+    const uint64_t cap = std::min<uint64_t>(c->fr_cap0, 1u << 16);
+    const int rc = c->grow_max ? set_alloc(c, c->x_bufs[k], cap, next_pow2(2 * cap), k == 0, *f)
+                               : set_alloc(c, c->x_bufs[k], c->fr.cap, c->fr.tmask + 1, k == 0, *f);
     if (rc) return rc;
   }
   if (!n) return TGI_OK;
+  int rc = set_grow(c, *f, c->x_bufs[k], n, st);
+  if (rc) return rc;
   DevBuf dk, dp;
   CK(dk.ensure(n * 32));
   CK(cudaMemcpyAsync(dk.p, keys32, n * 32, cudaMemcpyHostToDevice, st));
@@ -1987,7 +2063,7 @@ int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* sta
     CK(cudaMemcpyAsync(dp.p, stamp_sec, n * 8, cudaMemcpyHostToDevice, st));
     pay = dp.as<uint64_t>();
   }
-  int rc = frontier_insert_locked(c, *f, dk.p, pay, n, nullptr);
+  rc = frontier_insert_locked(c, *f, dk.p, pay, n, nullptr);
   if (rc) return rc;
   CK(cudaStreamSynchronize(st));
   return frontier_insert_check(c, *f);
@@ -2003,6 +2079,7 @@ int tgi_set_clear(tgi_ctx* c, int which) {
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
   int rc = frontier_clear_set(c, *f);
   if (rc) return rc;
+  c->x_bufs[which == TGI_SET_INVALID ? 0 : 1].bound = 0;
   CK(cudaStreamSynchronize(st));
   return TGI_OK;
 }
@@ -2020,6 +2097,35 @@ int tgi_set_now(tgi_ctx* c, int64_t now_sec) {
   if (!c) return TGI_E_ARG;
   std::lock_guard<std::mutex> g(c->fr_mu);
   c->excl.now_sec = now_sec;
+  return TGI_OK;
+}
+int tgi_set_growth(tgi_ctx* c, uint64_t max_keys) {
+  if (!c) return TGI_E_ARG;
+  if (max_keys >= (1ull << 40)) { set_err(c, "tgi_set_growth: a set holds fewer than 2^40 keys"); return TGI_E_ARG; }
+  for (int i = 0; i < TGI_SLOTS; i++) {
+    std::lock_guard<std::mutex> lk(c->slots[i].mu);
+    if (c->slots[i].busy && !c->slots[i].done) { set_err(c, "tgi_set_growth while slot %d is in flight", i); return TGI_E_STATE; }
+  }
+  std::lock_guard<std::mutex> g(c->fr_mu);
+  c->grow_max = max_keys;
+  return TGI_OK;
+}
+int tgi_set_info(tgi_ctx* c, int which, tgi_set_info_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  FrontierDev* f = which == TGI_SET_FRONTIER ? &c->fr : which == TGI_SET_OWNED ? &c->owned : excl_set(c, which);
+  const SetBufs* m = which == TGI_SET_FRONTIER ? &c->fr_bufs : which == TGI_SET_OWNED ? &c->o_bufs
+                     : &c->x_bufs[which == TGI_SET_INVALID ? 0 : 1];
+  if (!f) { set_err(c, "tgi_set_info: unknown set %d", which); return TGI_E_ARG; }
+  cudaSetDevice(c->device);
+  std::lock_guard<std::mutex> g(c->fr_mu);
+  if (which == TGI_SET_OWNED && !c->comm) { set_err(c, "tgi_set_info: TGI_SET_OWNED needs tgi_comm_init first"); return TGI_E_STATE; }
+  memset(out, 0, sizeof *out);
+  if (!f->table) return TGI_OK;  // an exclusion set before its first tgi_set_add
+  const int rc = frontier_read_count(c, *f, &out->count);
+  if (rc) return rc;
+  out->capacity = f->cap;
+  out->table_slots = f->tmask + 1;
+  out->grows = m->grows;
   return TGI_OK;
 }
 int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uint64_t cap, uint64_t* n) {
@@ -2240,6 +2346,8 @@ int tgi_frontier_merge(tgi_ctx* c, uint64_t* global_size, uint64_t* owned) {
   CK(cudaEventRecord(c->m_ev[2], st));
   // 4. the owner inserts what it received (source-rank-major: the lowest rank's copy of a key wins)
   if (R) {
+    rc = set_grow(c, c->owned, c->o_bufs, R, st);
+    if (rc) return rc;
     rc = frontier_insert_locked(c, c->owned, c->m_recv_keys.p, c->m_recv_pay.as<uint64_t>(), R, nullptr);
     if (rc) return rc;
   }

@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = [
     "tgi_filter_usernames", "tgi_acquire_staging", "tgi_release_staging", "tgi_comm_unique_id", "tgi_comm_init",
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
+    "tgi_set_growth", "tgi_set_info",
 ]
 
 
@@ -93,6 +94,8 @@ def lib() -> C.CDLL:
         L.tgi_set_now.argtypes = [vp, C.c_int64]
         L.tgi_pending_edges.argtypes = [vp, i32, C.c_int64, vp, u64, C.POINTER(u64)]
         L.tgi_plan_channel_appends.argtypes = [vp, vp, u32, u64, vp, u64, C.POINTER(u64)]
+        L.tgi_set_growth.argtypes = [vp, u64]
+        L.tgi_set_info.argtypes = [vp, i32, C.POINTER(abi.SetInfoC)]
         _LIB = L
     return _LIB
 
@@ -153,7 +156,8 @@ class Result:
 
 
 class Engine:
-    def __init__(self, cfg: abi.ConfigC | None = None, **kw):
+    def __init__(self, cfg: abi.ConfigC | None = None, set_growth: int = 0, **kw):
+        """set_growth: let every resident set grow up to this many keys (see set_growth); 0 keeps them fixed"""
         self.cfg = cfg or abi.make_config(**kw)
         self.h = C.c_void_p()
         rc = lib().tgi_create(C.byref(self.cfg), C.byref(self.h))
@@ -162,6 +166,8 @@ class Engine:
             self.h = None
             raise EngineError(rc, msg)
         self._keep = {}
+        if set_growth:
+            self.set_growth(set_growth)
 
     def _check(self, rc: int):
         if rc != 0:
@@ -328,6 +334,17 @@ class Engine:
 
     def set_now(self, now_sec: int):
         self._check(lib().tgi_set_now(self.h, now_sec))
+
+    def set_growth(self, max_keys: int):
+        """let the dedup set, the exclusion sets and this rank's partition grow on demand up to max_keys keys each
+        (frontier_capacity becomes their initial size); 0 = fixed capacity.  Not while a job is in flight."""
+        self._check(lib().tgi_set_growth(self.h, max_keys))
+
+    def set_info(self, which: int) -> dict:
+        """count, capacity, table_slots and grows of one set (abi.SET_FRONTIER / SET_INVALID / SET_DISCOVERED / SET_OWNED)"""
+        s = abi.SetInfoC()
+        self._check(lib().tgi_set_info(self.h, which, C.byref(s)))
+        return {k: getattr(s, k) for k, _ in s._fields_}
 
     def pending_edges(self, slot: int, now_sec: int = 0) -> np.ndarray:
         """the new edges of the slot's last batch as packed pending_edges rows (call before release)"""

@@ -247,6 +247,16 @@ class MessageProcessor {
   void SetClock(int64_t created_sec, int32_t created_nsec, int64_t capture_sec, int32_t capture_nsec) {
     tgi_set_clock(ctx_, created_sec, created_nsec, capture_sec, capture_nsec);
   }
+  // Lets the resident sets grow on demand up to max_keys keys each, like the reference's maps (0: fixed capacity).
+  void SetGrowth(uint64_t max_keys) {
+    if (tgi_set_growth(ctx_, max_keys) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+  }
+  // count / capacity / table_slots / grows of one set (TGI_SET_FRONTIER, TGI_SET_INVALID, TGI_SET_DISCOVERED, TGI_SET_OWNED)
+  tgi_set_info_t SetInfo(int which) {
+    tgi_set_info_t s{};
+    if (tgi_set_info(ctx_, which, &s) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return s;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

@@ -37,7 +37,7 @@ extern "C" {
 #define TGI_E_ARG (-1)      /* bad argument / malformed batch                                     */
 #define TGI_E_CUDA (-2)     /* CUDA runtime error (message in tgi_last_error)                     */
 #define TGI_E_NOMEM (-3)    /* host or device allocation failed                                   */
-#define TGI_E_CAPACITY (-4) /* a fixed capacity from tgi_config was exceeded                      */
+#define TGI_E_CAPACITY (-4) /* a capacity from tgi_config (or the tgi_set_growth limit) exceeded  */
 #define TGI_E_NODEVICE (-5) /* no CUDA device: there is NO CPU fallback in the product            */
 #define TGI_E_STATE (-6)    /* call sequence error (slot busy, result not released, ...)          */
 
@@ -290,7 +290,8 @@ typedef struct tgi_config {
   uint32_t crawl_label_len;
   uint32_t reserved;
   const char* crawl_label; /* Post.CrawlLabel as the sink would see it (daprstate.go:1113-1115)   */
-  uint64_t frontier_capacity; /* max distinct names in the frontier set (0 = default 1<<22)       */
+  uint64_t frontier_capacity; /* max distinct names in the frontier set (0 = default 1<<22); with
+                                 tgi_set_growth the initial size of the resident sets           */
   uint64_t max_records;    /* per-call record capacity (0 = default 1<<20)                        */
   uint64_t max_in_bytes;   /* per-call input byte capacity, all arrays (0 = grow on demand)       */
   uint64_t max_out_bytes;  /* per-call JSONL capacity (0 = grow on demand)                        */
@@ -543,6 +544,30 @@ int tgi_set_size(tgi_ctx* ctx, int which, uint64_t* n);
 /* the clock tgi_*_batch uses for the invalid-channel TTL (TGI_RUN_SKIP_INVALID); default: never expire */
 int tgi_set_now(tgi_ctx* ctx, int64_t now_sec);
 int tgi_pending_edges(tgi_ctx* ctx, int slot, int64_t now_sec, tgi_edge* rows, uint64_t cap, uint64_t* n);
+
+/* Resident key sets that grow on demand, as the reference's maps do (seenInBatch, urlCache, existingURLs,
+ * DiscoveredChannels, invalidChannelCache grow without limit).
+ *   tgi_set_growth   every resident set (the dedup set, the two exclusion sets, this rank's partition of the global set)
+ *                    may grow up to max_keys keys (< 2^40); 0 = fixed capacity, the default.  tgi_config.frontier_capacity
+ *                    is then the initial capacity of the dedup set and the partition; the exclusion sets start at
+ *                    min(frontier_capacity, 1<<16) keys.  A batch or insert that brings more keys than fit moves the set
+ *                    into buffers for next_pow2(count + incoming) keys first: the keys keep their first-occurrence order,
+ *                    so every result and the export equal those of a set that was big enough from the start.  Device
+ *                    memory peaks at old + new buffers during the move.  Past max_keys the call fails with
+ *                    TGI_E_CAPACITY and leaves the set untouched.  Must not be called while a job is in flight on any
+ *                    slot (returns TGI_E_STATE).
+ *   tgi_set_info     count, capacity, table slots and number of growth steps of one set (all 0 for an exclusion set
+ *                    before its first tgi_set_add); TGI_SET_OWNED before tgi_comm_init returns TGI_E_STATE.          */
+#define TGI_SET_FRONTIER 0    /* the dedup set (tgi_frontier_*, TGI_RUN_FRONTIER)                  */
+#define TGI_SET_OWNED 3       /* this rank's partition of the global set (tgi_frontier_merge)      */
+typedef struct tgi_set_info_t {
+  uint64_t count;       /* keys in the set                                                        */
+  uint64_t capacity;    /* keys it holds before it grows (or fails with TGI_E_CAPACITY)           */
+  uint64_t table_slots; /* slots of its open-addressed hash table                                 */
+  uint64_t grows;       /* growth steps since it was created or last allocated                    */
+} tgi_set_info_t;
+int tgi_set_growth(tgi_ctx* ctx, uint64_t max_keys);
+int tgi_set_info(tgi_ctx* ctx, int which, tgi_set_info_t* out);
 
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
