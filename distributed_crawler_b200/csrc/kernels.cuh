@@ -965,6 +965,11 @@ DEVI Key32 load_key(const uint8_t* p) {  // 4-byte aligned
   for (int i = 0; i < 8; i++) k.w[i] = q[i];
   return k;
 }
+DEVI void store_key(uint8_t* p, const Key32& k) {  // 4-byte aligned
+  uint32_t* q = (uint32_t*)p;
+#pragma unroll
+  for (int i = 0; i < 8; i++) q[i] = k.w[i];
+}
 DEVI bool key_eq(const Key32& a, const Key32& b) {
   uint32_t d = 0;
 #pragma unroll
@@ -983,17 +988,30 @@ DEVI uint64_t key_hash(const Key32& k) {
   return h ^ (h >> 29);
 }
 
-// pool index of `key` in set f, or -1
-DEVI int64_t set_lookup(const FrontierDev& f, const Key32& key, uint64_t h) {
-  if (!f.table) return -1;
-  const uint64_t fp = (h >> 40) | 1ull;
+// whether set f holds `key` (hash h), and if so its pool index pi.  Table entry: (pool index + 1) | fingerprint << 40,
+// placed by set_place.
+DEVI bool set_probe(const FrontierDev& f, const Key32& key, uint64_t h, uint64_t& pi) {
+  const uint64_t fp = (h >> 40) | 1ull;  // 24-bit fingerprint, never 0
   for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
     const uint64_t e = f.table[s];
-    if (e == 0) return -1;
+    if (e == 0) return false;
     if ((e >> 40) == fp) {
-      const uint64_t pi = (e & 0xFFFFFFFFFFull) - 1;
-      if (key_eq(key, load_key(f.pool + 32 * pi))) return (int64_t)pi;
+      pi = (e & 0xFFFFFFFFFFull) - 1;
+      if (key_eq(key, load_key(f.pool + 32 * pi))) return true;
     }
+  }
+}
+// pool index of `key` in exclusion set f, or -1: before its first tgi_set_add a set has no table and holds nothing
+DEVI int64_t set_lookup(const FrontierDev& f, const Key32& key, uint64_t h) {
+  uint64_t pi;
+  return f.table && set_probe(f, key, h, pi) ? (int64_t)pi : -1;
+}
+// enters the key with hash h at pool index pi into f.table: the only writer of table entries, so the append and the
+// rehash of a growing set produce the same table
+DEVI void set_place(const FrontierDev& f, uint64_t pi, uint64_t h) {
+  const uint64_t e = (pi + 1) | (((h >> 40) | 1ull) << 40);
+  for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
+    if (f.table[s] == 0 && atomicCAS((unsigned long long*)&f.table[s], 0ull, (unsigned long long)e) == 0) break;
   }
 }
 // the resident exclusion sets of the frontier -> validator hand-off (tgi_set_add): invalid channels expire after
@@ -1041,20 +1059,8 @@ DEVI void frontier_probe_body(uint64_t n, const uint32_t* link_start, const uint
       fb.lstate[idx] = LS_INELIGIBLE;
       continue;
     }
-    uint64_t fp = (h >> 40) | 1ull;  // 24-bit fingerprint, never 0
-    bool known = false;
-    for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
-      uint64_t e = f.table[s];
-      if (e == 0) break;
-      if ((e >> 40) == fp) {
-        uint64_t pi = (e & 0xFFFFFFFFFFull) - 1;
-        if (key_eq(key, load_key(f.pool + 32 * pi))) {
-          known = true;
-          break;
-        }
-      }
-    }
-    if (known) {
+    uint64_t pi;
+    if (set_probe(f, key, h, pi)) {
       fb.lstate[idx] = LS_KNOWN;
       continue;
     }
@@ -1123,15 +1129,9 @@ DEVI void frontier_append_body(uint64_t n, const uint32_t* link_start, const uin
     if (fb.btable[st] != (((uint64_t)r << SEQ_ORD_BITS) | k) + 1) continue;
     tgi_link& lk = arena[ls + k];
     Key32 key = load_key(lk.name);
-    uint32_t* dst = (uint32_t*)(f.pool + 32 * pi);
-#pragma unroll
-    for (int i = 0; i < 8; i++) dst[i] = key.w[i];
+    store_key(f.pool + 32 * pi, key);
     if (f.payload) f.payload[pi] = payload_in ? payload_in[r] : 0ull;  // keys mode: one key per "record"
-    uint64_t h = key_hash(key);
-    uint64_t e = (pi + 1) | (((h >> 40) | 1ull) << 40);
-    for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
-      if (f.table[s] == 0 && atomicCAS((unsigned long long*)&f.table[s], 0ull, (unsigned long long)e) == 0) break;
-    }
+    set_place(f, pi, key_hash(key));
     lk.flags |= TGI_LF_NEW;
     pi++;
   }
@@ -1158,16 +1158,12 @@ __global__ void frontier_commit_kernel(FrontierDev f, const uint64_t* new_off, u
 }
 
 // growth of a set (tgi_set_growth): index the first n keys of f.pool (already copied from the smaller set) in f.table,
-// zeroed.  Entry format and probe sequence are those of frontier_append_body; the pool order is untouched, so the
-// export order and the NEW flags of later batches are those of a set that was big enough from the start.
+// zeroed.  The entries are placed by set_place, as in frontier_append_body; the pool order is untouched, so the export
+// order and the NEW flags of later batches are those of a set that was big enough from the start.
 __global__ void set_rehash_kernel(FrontierDev f, uint64_t n) {
   const uint64_t pi = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (pi >= n) return;
-  const uint64_t h = key_hash(load_key(f.pool + 32 * pi));
-  const uint64_t e = (pi + 1) | (((h >> 40) | 1ull) << 40);
-  for (uint64_t s = h & f.tmask;; s = (s + 1) & f.tmask) {
-    if (f.table[s] == 0 && atomicCAS((unsigned long long*)&f.table[s], 0ull, (unsigned long long)e) == 0) break;
-  }
+  set_place(f, pi, key_hash(load_key(f.pool + 32 * pi)));
 }
 
 // ---- multi-GPU merge (SURVEY 8e option A): bucket the new local keys by owner rank ----------------------------------
@@ -1189,9 +1185,7 @@ __global__ void merge_scatter_kernel(const uint8_t* pool, uint64_t first, uint64
   if (i >= m) return;
   const Key32 k = load_key(pool + 32 * (first + i));
   const unsigned long long pos = atomicAdd(&cursor[key_owner(k, nranks)], 1ull);
-  uint32_t* dst = (uint32_t*)(send_keys + 32 * pos);
-#pragma unroll
-  for (int j = 0; j < 8; j++) dst[j] = k.w[j];
+  store_key(send_keys + 32 * pos, k);
   send_pay[pos] = pay_base | (first + i);
 }
 
@@ -1213,9 +1207,7 @@ __global__ void edges_emit_kernel(uint64_t n, const uint32_t* link_start, const 
       const Key32 key = load_key(lk[k].name);
       const uint64_t h = key_hash(key);
       tgi_edge e;
-      uint32_t* d = (uint32_t*)e.destination;
-#pragma unroll
-      for (int i = 0; i < 8; i++) d[i] = key.w[i];
+      store_key(e.destination, key);
       e.record = r;
       e.chan_idx = chan_idx_of ? *(const uint32_t*)((const uint8_t*)chan_idx_of + (size_t)r * chan_stride) : 0u;
       e.dest_len = lk[k].len;

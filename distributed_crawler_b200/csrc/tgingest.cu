@@ -96,9 +96,10 @@ struct InsertScratch {
   FrontierScratch fs;
 };
 
-// the buffers behind one device key set (FrontierDev), and what the host knows of its fill
-struct SetBufs {
+// one device-resident key set: its buffers, the kernels' view of them, and what the host knows of its fill
+struct KeySet {
   DevBuf pool, table, count, payload;
+  FrontierDev dev{};   // dev.table == nullptr: not allocated (an exclusion set before its first tgi_set_add)
   uint64_t bound = 0;  // upper bound of the set's count: the keys it held when last read plus every key enqueued since
   uint64_t grows = 0;  // rehashes into bigger buffers (set_grow)
 };
@@ -183,9 +184,10 @@ struct tgi_ctx {
   DevBuf d_cfg;
   CfgDev cfgdev{};
   std::mutex cfg_mu;
-  // frontier: the local set (every key this GPU has seen)
-  SetBufs fr_bufs;
-  FrontierDev fr{};
+  // the resident key sets, indexed by TGI_SET_*: the dedup set (every key this GPU has seen), the exclusion sets of the
+  // frontier -> validator hand-off (tgi_set_add) and this rank's partition of the multi-GPU set (tgi_comm_init)
+  KeySet sets[4];
+  int64_t now_sec = 0;     // tgi_set_now: the clock the TTL of the invalid set is checked against
   uint64_t fr_cap0 = 0;    // tgi_config.frontier_capacity: the size the dedup set started at
   uint64_t grow_max = 0;   // tgi_set_growth: sets grow up to this many keys (0: fixed size)
   std::mutex fr_mu;
@@ -196,16 +198,11 @@ struct tgi_ctx {
   std::mutex tk_mu;
   std::condition_variable tk_cv;
   uint64_t tk_next = 0, tk_serving = 0;
-  InsertScratch ins;  // scratch of tgi_frontier_insert* / the merge (under fr_mu)
-  // frontier -> validator hand-off: resident exclusion sets (tgi_set_add)
-  SetBufs x_bufs[2];
-  ExclusionDev excl{};
-  // multi-GPU merge: communicator + this rank's partition of the global set
+  InsertScratch ins;  // scratch of tgi_frontier_insert* / tgi_set_add / the merge (under fr_mu)
+  // multi-GPU merge: communicator (this rank's partition is sets[TGI_SET_OWNED])
   NcclApi* nccl = nullptr;
   ncclComm_t comm = nullptr;
   int rank = 0, nranks = 1;
-  SetBufs o_bufs;
-  FrontierDev owned{};
   uint64_t merged_upto = 0, merge_round = 0;
   DevBuf m_cnt, m_all, m_cursor, m_send_keys, m_send_pay, m_recv_keys, m_recv_pay, m_gsize;
   HostBuf m_host;
@@ -396,28 +393,62 @@ int frontier_scratch(tgi_ctx* c, FrontierScratch& z, uint64_t n, uint64_t links,
   return TGI_OK;
 }
 
+// The set `which` (TGI_SET_*) names, or nullptr.  With exclusion_only, only the exclusion sets are named (the
+// tgi_set_add / _clear / _size family).
+KeySet* key_set(tgi_ctx* c, int which, bool exclusion_only) {
+  if (which == TGI_SET_INVALID || which == TGI_SET_DISCOVERED) return &c->sets[which];
+  if (!exclusion_only && (which == TGI_SET_FRONTIER || which == TGI_SET_OWNED)) return &c->sets[which];
+  return nullptr;
+}
+// the kernels' view of the exclusion sets, with the invalid set's TTL checked against now_sec
+ExclusionDev exclusion(const tgi_ctx* c, int64_t now_sec) {
+  return ExclusionDev{c->sets[TGI_SET_INVALID].dev, c->sets[TGI_SET_DISCOVERED].dev, (long long)now_sec};
+}
+
 // An empty device key set of `cap` keys in a table of `tslots` slots (with a u64 payload per key if asked), zeroed on
 // slot 0's stream; the caller synchronises.
-int set_alloc(tgi_ctx* c, SetBufs& m, uint64_t cap, uint64_t tslots, bool payload, FrontierDev& f) {
+int set_alloc(tgi_ctx* c, KeySet& k, uint64_t cap, uint64_t tslots, bool payload) {
   cudaStream_t st = c->slots[0].stream;
-  CK(m.pool.ensure(cap * 32));
-  CK(m.table.ensure(tslots * 8));
-  CK(m.count.ensure(16));
-  if (payload) CK(m.payload.ensure(cap * 8));
-  CK(cudaMemsetAsync(m.table.p, 0, tslots * 8, st));
-  CK(cudaMemsetAsync(m.count.p, 0, 16, st));
-  f.pool = m.pool.as<uint8_t>();
+  CK(k.pool.ensure(cap * 32));
+  CK(k.table.ensure(tslots * 8));
+  CK(k.count.ensure(16));
+  if (payload) CK(k.payload.ensure(cap * 8));
+  CK(cudaMemsetAsync(k.table.p, 0, tslots * 8, st));
+  CK(cudaMemsetAsync(k.count.p, 0, 16, st));
+  FrontierDev& f = k.dev;
+  f.pool = k.pool.as<uint8_t>();
   f.cap = cap;
-  f.table = m.table.as<uint64_t>();
+  f.table = k.table.as<uint64_t>();
   f.tmask = tslots - 1;
-  f.count = m.count.as<uint64_t>();
-  f.payload = payload ? m.payload.as<uint64_t>() : nullptr;
-  m.bound = 0;
-  m.grows = 0;
+  f.count = k.count.as<uint64_t>();
+  f.payload = payload ? k.payload.as<uint64_t>() : nullptr;
+  k.bound = 0;
+  k.grows = 0;
   return TGI_OK;
 }
 
-// Makes room for up to `need` more keys in set f (buffers m) before a caller inserts them on stream st, when growth is on
+// The number of keys in set k (0 while it is not allocated), under fr_mu.  Reads and clears of a set go through slot 0's
+// stream (the library's streams are non-blocking: work on the legacy default stream would not be ordered with them) and
+// are synchronised before the entry point returns.
+int set_count(tgi_ctx* c, const KeySet& k, uint64_t* n) {
+  *n = 0;
+  if (!k.dev.table) return TGI_OK;
+  cudaStream_t st = c->slots[0].stream;
+  if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+  CK(cudaMemcpyAsync(n, k.dev.count, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return TGI_OK;
+}
+// empties allocated set k but keeps its capacity and growth steps; the caller orders it behind fr_event and synchronises
+int set_clear(tgi_ctx* c, KeySet& k) {
+  cudaStream_t st = c->slots[0].stream;
+  CK(cudaMemsetAsync(k.dev.table, 0, (k.dev.tmask + 1) * 8, st));
+  CK(cudaMemsetAsync(k.dev.count, 0, 8, st));
+  k.bound = 0;
+  return TGI_OK;
+}
+
+// Makes room for up to `need` more keys in set k before a caller inserts them on stream st, when growth is on
 // (tgi_set_growth).  Runs under fr_mu, inside the caller's frontier turn.  The host bound decides without a device round
 // trip; only when it says the set might overflow is the exact count read, and only when that overflows too does the set
 // move into buffers for next_pow2(count + need) keys (at most grow_max): the pool and payload are copied, the bigger
@@ -429,16 +460,17 @@ int set_alloc(tgi_ctx* c, SetBufs& m, uint64_t cap, uint64_t tslots, bool payloa
 // exports, the merge, tgi_pending_edges) or records fr_event behind its kernels (the batches' frontier phases, the page
 // kernels).  This function enqueues its work behind fr_event and synchronises st before it frees anything, so every
 // earlier reader has finished by then, and later ones see only the new buffers.
-int set_grow(tgi_ctx* c, FrontierDev& f, SetBufs& m, uint64_t need, cudaStream_t st) {
-  if (c->grow_max && f.cap < c->grow_max && m.bound + need > f.cap) {
+int set_grow(tgi_ctx* c, KeySet& k, uint64_t need, cudaStream_t st) {
+  const FrontierDev& f = k.dev;
+  if (c->grow_max && f.cap < c->grow_max && k.bound + need > f.cap) {
     if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
     uint64_t count = 0;
     CK(cudaMemcpyAsync(&count, f.count, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    m.bound = count;
+    k.bound = count;
     if (count + need > f.cap) {
       const uint64_t cap = std::min(next_pow2(count + need), c->grow_max), tslots = next_pow2(2 * cap);
-      SetBufs nb;
+      KeySet nb;
       CK(nb.pool.ensure(cap * 32));
       CK(nb.table.ensure(tslots * 8));
       if (f.payload) CK(nb.payload.ensure(cap * 8));
@@ -456,14 +488,49 @@ int set_grow(tgi_ctx* c, FrontierDev& f, SetBufs& m, uint64_t need, cudaStream_t
         CK(cudaGetLastError());
       }
       CK(cudaStreamSynchronize(st));
-      m.pool.swap(nb.pool);  // nb now holds the old buffers and frees them on return
-      m.table.swap(nb.table);
-      m.payload.swap(nb.payload);
-      f = g;
-      m.grows++;
+      k.pool.swap(nb.pool);  // nb now holds the old buffers and frees them on return
+      k.table.swap(nb.table);
+      k.payload.swap(nb.payload);
+      k.dev = g;
+      k.grows++;
     }
   }
-  m.bound += need;
+  k.bound += need;
+  return TGI_OK;
+}
+
+// Enqueues the frontier phases that insert the keys of n records' links into set k on stream st, behind every earlier
+// user of the sets (fr_event): make room for `links` more keys (set_grow), size the scratch (a batch table for `links`
+// keys, per-link state for `lstate_rows` arena rows), zero the batch table, probe, count, scan, append, commit, and
+// record fr_event.  link_start == nullptr: record r is the one link arena[r], and payload[r] (if given) is its key's
+// payload.  out_new[0..1] receive the NEW count and the set's size; a full set is left untouched and sets
+// ERR_FRONTIER_FULL in *err.  The caller reads both after it synchronises st.  `tiled` asks launch_scan for the
+// three-launch scan at every size.  ev0 / ev1 (if given) time the phases.  Runs under fr_mu.
+int set_insert(tgi_ctx* c, KeySet& k, cudaStream_t st, uint64_t n, const uint32_t* link_start, const uint32_t* link_count,
+               tgi_link* arena, uint64_t links, uint64_t lstate_rows, uint32_t run_flags, const ExclusionDev& x,
+               FrontierScratch& z, DevBuf& tiles, bool tiled, uint64_t* out_new, int* err, const uint64_t* payload,
+               uint32_t& launches, cudaEvent_t ev0 = nullptr, cudaEvent_t ev1 = nullptr) {
+  if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+  int rc = set_grow(c, k, links, st);  // at most one new key per link
+  if (rc) return rc;
+  FrontierBatch fb;
+  rc = frontier_scratch(c, z, n, links, lstate_rows, fb);
+  if (rc) return rc;
+  if (ev0) CK(cudaEventRecord(ev0, st));
+  CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
+  const unsigned g = (unsigned)((n + 255) / 256);
+  frontier_probe_kernel<<<g, 256, 0, st>>>(n, link_start, link_count, arena, run_flags, k.dev, fb, x);
+  frontier_count_kernel<<<g, 256, 0, st>>>(n, link_start, link_count, fb);
+  launches += 2;
+  rc = launch_scan(c, st, tiles, fb.rec_new, n, z.new_off.as<uint64_t>(), out_new, launches, tiled);
+  if (rc) return rc;
+  frontier_append_kernel<<<g, 256, 0, st>>>(n, link_start, link_count, arena, k.dev, fb, z.new_off.as<uint64_t>(), err, payload);
+  frontier_commit_kernel<<<1, 1, 0, st>>>(k.dev, z.new_off.as<uint64_t>(), n, out_new, err);
+  launches += 2;
+  CK(cudaGetLastError());
+  if (ev1) CK(cudaEventRecord(ev1, st));
+  CK(cudaEventRecord(c->fr_event, st));
+  c->fr_event_valid = true;
   return TGI_OK;
 }
 
@@ -733,7 +800,7 @@ int sc_err(const uint64_t* hsc) { return ((const int*)(hsc + SC_CURSOR))[1]; }
 
 // the device errors that fail a batch once it has run to the end
 int check_dev_err(tgi_ctx* c, int err) {
-  if (err & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)c->fr.cap); return TGI_E_CAPACITY; }
+  if (err & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)c->sets[TGI_SET_FRONTIER].dev.cap); return TGI_E_CAPACITY; }
   if (err & ERR_LINE_MISMATCH) { set_err(c, "internal: sized and emitted line lengths disagree"); return TGI_E_STATE; }
   return TGI_OK;
 }
@@ -862,30 +929,10 @@ int finish_batch(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
     // frontier phases of different slots are serialised in submission order (tickets)
     turn_begin(c, s);
     std::unique_lock<std::mutex> fg(c->fr_mu);
-    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-    int rc = set_grow(c, c->fr, c->fr_bufs, arena_used, st);  // the batch adds at most one key per link
+    const int rc = set_insert(c, c->sets[TGI_SET_FRONTIER], st, n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
+                              s.d_arena.as<tgi_link>(), arena_used, arena_cap, flags, exclusion(c, c->now_sec), s.fs, s.d_tiles,
+                              false, dsc + SC_NEW, (int*)(dsc + SC_CURSOR) + 1, nullptr, launches, s.ev_fr0, s.ev_fr1);
     if (rc) return rc;
-    FrontierBatch fb;
-    rc = frontier_scratch(c, s.fs, n, arena_used, arena_cap, fb);
-    if (rc) return rc;
-    CK(cudaEventRecord(s.ev_fr0, st));
-    CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
-    unsigned g = (unsigned)((n + 255) / 256);
-    frontier_probe_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
-                                             s.d_arena.as<tgi_link>(), flags, c->fr, fb, c->excl);
-    frontier_count_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(), fb);
-    launches += 2;
-    rc = launch_scan(c, s, fb.rec_new, n, s.fs.new_off.as<uint64_t>(), dsc + SC_NEW, launches);
-    if (rc) return rc;
-    int* derr = (int*)(dsc + SC_CURSOR) + 1;
-    frontier_append_kernel<<<g, 256, 0, st>>>(n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
-                                              s.d_arena.as<tgi_link>(), c->fr, fb, s.fs.new_off.as<uint64_t>(), derr);
-    frontier_commit_kernel<<<1, 1, 0, st>>>(c->fr, s.fs.new_off.as<uint64_t>(), n, dsc + SC_NEW, derr);
-    launches += 2;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(s.ev_fr1, st));
-    CK(cudaEventRecord(c->fr_event, st));
-    c->fr_event_valid = true;
     fg.unlock();
     turn_end(c, s);
   }
@@ -1070,9 +1117,10 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint
       turn_begin(c, s);
       fg.lock();
       if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-      r.fr = c->fr;
-      r.excl = c->excl;
-      c->fr_bufs.bound += L.links_max;
+      KeySet& fr = c->sets[TGI_SET_FRONTIER];
+      r.fr = fr.dev;
+      r.excl = exclusion(c, c->now_sec);
+      fr.bound += L.links_max;
     }
     CK(cudaEventRecord(s.ev_k0, st));
     if (cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(CTA_THREADS), kargs, 0, st) != cudaSuccess) {
@@ -1620,7 +1668,7 @@ int tgi_create(const tgi_config* cfg, tgi_ctx** out) {
   uint64_t fcap = cfg->frontier_capacity ? cfg->frontier_capacity : (1ull << 22);
   uint64_t tslots = next_pow2(2 * fcap);
   ctx->fr_cap0 = fcap;
-  if (set_alloc(ctx, ctx->fr_bufs, fcap, tslots, false, ctx->fr) != TGI_OK) {
+  if (set_alloc(ctx, ctx->sets[TGI_SET_FRONTIER], fcap, tslots, false) != TGI_OK) {
     set_err(c, "frontier allocation failed (%llu keys)", (unsigned long long)fcap);
     return fail(TGI_E_NOMEM);
   }
@@ -1884,52 +1932,39 @@ int tgi_youtube_run_resident(tgi_ctx* c, int slot, uint32_t run_flags, tgi_resul
 }
 
 // ---- frontier host API ------------------------------------------------------------------------------
-// Inserts n device-resident 32-byte keys into set `f` (the local set, or this rank's partition of the global set).
-// Runs on slot 0's stream under the frontier lock (taken by the caller); the scratch lives in the context.
-static int frontier_insert_locked(tgi_ctx* c, FrontierDev& f, const void* d_keys, const uint64_t* d_payload, uint64_t n, void* d_is_new) {
-  Slot& s = c->slots[0];
-  cudaStream_t st = s.stream;
+// Enqueues the insert of n (> 0) device-resident 32-byte keys, each with its payload if d_payload is given, into set k
+// (the dedup set, an exclusion set, or this rank's partition of the global set), and their NEW flags into d_is_new if
+// given.  Runs on slot 0's stream under the frontier lock (taken by the caller); the scratch lives in the context.
+static int frontier_insert_enqueue(tgi_ctx* c, KeySet& k, const void* d_keys, const uint64_t* d_payload, uint64_t n, void* d_is_new) {
+  cudaStream_t st = c->slots[0].stream;
   InsertScratch& z = c->ins;
-  if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
   CK(z.arena.ensure(n * sizeof(tgi_link)));
   CK(z.cnt.ensure(n * 4));
   CK(z.sc.ensure(64));
-  FrontierBatch fb;
-  int rc = frontier_scratch(c, z.fs, n, n, n, fb);
-  if (rc) return rc;
-  CK(cudaMemsetAsync(fb.btable, 0, (fb.bmask + 1) * 8, st));
   CK(cudaMemsetAsync(z.sc.p, 0, 64, st));
-  unsigned g = (unsigned)((n + 255) / 256);
-  if (!g) g = 1;
+  const unsigned g = (unsigned)((n + 255) / 256);
   keys_to_links_kernel<<<g, 256, 0, st>>>((const uint8_t*)d_keys, n, z.arena.as<tgi_link>(), z.cnt.as<uint32_t>());
-  frontier_probe_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), 0, f, fb, ExclusionDev{});
-  frontier_count_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), fb);
   uint32_t launches = 0;  // not reported by the insert API
-  rc = launch_scan(c, st, z.tiles, fb.rec_new, n, z.fs.new_off.as<uint64_t>(), z.sc.as<uint64_t>(), launches, true);
+  const int rc = set_insert(c, k, st, n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), n, n, 0, ExclusionDev{}, z.fs,
+                            z.tiles, true, z.sc.as<uint64_t>(), (int*)(z.sc.as<uint64_t>() + 4), d_payload, launches);
   if (rc) return rc;
-  int* derr = (int*)(z.sc.as<uint64_t>() + 4);
-  frontier_append_kernel<<<g, 256, 0, st>>>(n, nullptr, z.cnt.as<uint32_t>(), z.arena.as<tgi_link>(), f, fb, z.fs.new_off.as<uint64_t>(), derr, d_payload);
-  frontier_commit_kernel<<<1, 1, 0, st>>>(f, z.fs.new_off.as<uint64_t>(), n, z.sc.as<uint64_t>() + 1, derr);
   if (d_is_new) links_new_flags_kernel<<<g, 256, 0, st>>>(z.arena.as<tgi_link>(), n, (uint8_t*)d_is_new);
   CK(cudaGetLastError());
-  CK(cudaEventRecord(c->fr_event, st));
-  c->fr_event_valid = true;
   return TGI_OK;
 }
-static int frontier_insert_check(tgi_ctx* c, const FrontierDev& f) {  // after a stream synchronize
+static int frontier_insert_check(tgi_ctx* c, const KeySet& k) {  // after a stream synchronize
   int herr = 0;
   CK(cudaMemcpy(&herr, (int*)(c->ins.sc.as<uint64_t>() + 4), 4, cudaMemcpyDeviceToHost));
-  if (herr & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)f.cap); return TGI_E_CAPACITY; }
+  if (herr & ERR_FRONTIER_FULL) { set_err(c, "frontier capacity %llu exceeded", (unsigned long long)k.dev.cap); return TGI_E_CAPACITY; }
   return TGI_OK;
 }
 static int frontier_insert_impl(tgi_ctx* c, const void* d_keys, uint64_t n, void* d_is_new) {
   std::unique_lock<std::mutex> fg(c->fr_mu);
-  int rc = set_grow(c, c->fr, c->fr_bufs, n, c->slots[0].stream);
-  if (rc) return rc;
-  rc = frontier_insert_locked(c, c->fr, d_keys, nullptr, n, d_is_new);
+  KeySet& fr = c->sets[TGI_SET_FRONTIER];
+  const int rc = frontier_insert_enqueue(c, fr, d_keys, nullptr, n, d_is_new);
   if (rc) return rc;
   CK(cudaStreamSynchronize(c->slots[0].stream));
-  return frontier_insert_check(c, c->fr);
+  return frontier_insert_check(c, fr);
 }
 
 int tgi_frontier_insert(tgi_ctx* c, const uint8_t* keys32, uint64_t n, uint8_t* is_new) {
@@ -1962,31 +1997,23 @@ int tgi_frontier_sync(tgi_ctx* c) {
   if (c->fr_event_valid) CK(cudaEventSynchronize(c->fr_event));
   return TGI_OK;
 }
-// all copies / memsets of the frontier go through slot 0's stream (the library's streams are non-blocking: work on
-// the legacy default stream would not be ordered with them) and are synchronised before returning
-static int frontier_read_count(tgi_ctx* c, const FrontierDev& f, uint64_t* n) {
-  cudaStream_t st = c->slots[0].stream;
-  if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-  CK(cudaMemcpyAsync(n, f.count, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return TGI_OK;
-}
 int tgi_frontier_size(tgi_ctx* c, uint64_t* n) {
   if (!c || !n) return TGI_E_ARG;
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
-  return frontier_read_count(c, c->fr, n);
+  return set_count(c, c->sets[TGI_SET_FRONTIER], n);
 }
 int tgi_frontier_export(tgi_ctx* c, uint8_t* keys32, uint64_t cap, uint64_t* n) {
   if (!c || !n) return TGI_E_ARG;
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
+  const KeySet& fr = c->sets[TGI_SET_FRONTIER];
   uint64_t sz = 0;
-  int rc = frontier_read_count(c, c->fr, &sz);
+  int rc = set_count(c, fr, &sz);
   if (rc) return rc;
   uint64_t m = sz < cap ? sz : cap;
   if (m && keys32) {
-    CK(cudaMemcpyAsync(keys32, c->fr.pool, m * 32, cudaMemcpyDeviceToHost, c->slots[0].stream));
+    CK(cudaMemcpyAsync(keys32, fr.dev.pool, m * 32, cudaMemcpyDeviceToHost, c->slots[0].stream));
     CK(cudaStreamSynchronize(c->slots[0].stream));
   }
   *n = sz;
@@ -1996,22 +2023,17 @@ int tgi_frontier_export_dev(tgi_ctx* c, void* d_keys32, uint64_t cap, uint64_t f
   if (!c || !n) return TGI_E_ARG;
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
+  const KeySet& fr = c->sets[TGI_SET_FRONTIER];
   uint64_t sz = 0;
-  int rc = frontier_read_count(c, c->fr, &sz);
+  int rc = set_count(c, fr, &sz);
   if (rc) return rc;
   uint64_t avail = first < sz ? sz - first : 0;
   uint64_t m = avail < cap ? avail : cap;
   if (m && d_keys32) {
-    CK(cudaMemcpyAsync(d_keys32, c->fr.pool + 32 * first, m * 32, cudaMemcpyDeviceToDevice, c->slots[0].stream));
+    CK(cudaMemcpyAsync(d_keys32, fr.dev.pool + 32 * first, m * 32, cudaMemcpyDeviceToDevice, c->slots[0].stream));
     CK(cudaStreamSynchronize(c->slots[0].stream));  // the caller's stream may read the keys as soon as this returns
   }
   *n = m;
-  return TGI_OK;
-}
-static int frontier_clear_set(tgi_ctx* c, FrontierDev& f) {
-  cudaStream_t st = c->slots[0].stream;
-  CK(cudaMemsetAsync(f.table, 0, (f.tmask + 1) * 8, st));
-  CK(cudaMemsetAsync(f.count, 0, 8, st));
   return TGI_OK;
 }
 int tgi_frontier_clear(tgi_ctx* c) {
@@ -2020,11 +2042,10 @@ int tgi_frontier_clear(tgi_ctx* c) {
   std::lock_guard<std::mutex> g(c->fr_mu);
   cudaStream_t st = c->slots[0].stream;
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-  int rc = frontier_clear_set(c, c->fr);
-  if (rc == TGI_OK && c->owned.table) rc = frontier_clear_set(c, c->owned);
+  KeySet& owned = c->sets[TGI_SET_OWNED];
+  int rc = set_clear(c, c->sets[TGI_SET_FRONTIER]);
+  if (rc == TGI_OK && owned.dev.table) rc = set_clear(c, owned);
   if (rc) return rc;
-  c->fr_bufs.bound = 0;
-  c->o_bufs.bound = 0;
   c->merged_upto = 0;
   CK(cudaEventRecord(c->fr_event, st));
   c->fr_event_valid = true;
@@ -2033,70 +2054,63 @@ int tgi_frontier_clear(tgi_ctx* c) {
 }
 
 // ---- frontier -> validator hand-off (SURVEY 8f rank 3) ------------------------------------------------------------
-static FrontierDev* excl_set(tgi_ctx* c, int which) {
-  return which == TGI_SET_INVALID ? &c->excl.invalid : which == TGI_SET_DISCOVERED ? &c->excl.discovered : nullptr;
-}
 int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* stamp_sec, uint64_t n) {
   if (!c || (n && !keys32)) return TGI_E_ARG;
-  FrontierDev* f = excl_set(c, which);
-  if (!f) { set_err(c, "tgi_set_add: unknown set %d", which); return TGI_E_ARG; }
+  KeySet* k = key_set(c, which, true);
+  if (!k) { set_err(c, "tgi_set_add: unknown set %d", which); return TGI_E_ARG; }
   if (n >= (1ull << 32)) { set_err(c, "too many keys in one call"); return TGI_E_ARG; }
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
   cudaStream_t st = c->slots[0].stream;
-  const int k = which == TGI_SET_INVALID ? 0 : 1;
-  if (!f->table) {  // first use: same capacity as the dedup set, or at most 2^16 keys when the sets grow on their own
+  const bool stamps = which == TGI_SET_INVALID;
+  if (!k->dev.table) {  // first use: same capacity as the dedup set, or at most 2^16 keys when the sets grow on their own
+    const FrontierDev& fr = c->sets[TGI_SET_FRONTIER].dev;
     const uint64_t cap = std::min<uint64_t>(c->fr_cap0, 1u << 16);
-    const int rc = c->grow_max ? set_alloc(c, c->x_bufs[k], cap, next_pow2(2 * cap), k == 0, *f)
-                               : set_alloc(c, c->x_bufs[k], c->fr.cap, c->fr.tmask + 1, k == 0, *f);
+    const int rc = c->grow_max ? set_alloc(c, *k, cap, next_pow2(2 * cap), stamps)
+                               : set_alloc(c, *k, fr.cap, fr.tmask + 1, stamps);
     if (rc) return rc;
   }
   if (!n) return TGI_OK;
-  int rc = set_grow(c, *f, c->x_bufs[k], n, st);
-  if (rc) return rc;
   DevBuf dk, dp;
   CK(dk.ensure(n * 32));
   CK(cudaMemcpyAsync(dk.p, keys32, n * 32, cudaMemcpyHostToDevice, st));
   const uint64_t* pay = nullptr;
-  if (k == 0 && stamp_sec) {
+  if (stamps && stamp_sec) {
     CK(dp.ensure(n * 8));
     CK(cudaMemcpyAsync(dp.p, stamp_sec, n * 8, cudaMemcpyHostToDevice, st));
     pay = dp.as<uint64_t>();
   }
-  rc = frontier_insert_locked(c, *f, dk.p, pay, n, nullptr);
+  const int rc = frontier_insert_enqueue(c, *k, dk.p, pay, n, nullptr);
   if (rc) return rc;
   CK(cudaStreamSynchronize(st));
-  return frontier_insert_check(c, *f);
+  return frontier_insert_check(c, *k);
 }
 int tgi_set_clear(tgi_ctx* c, int which) {
   if (!c) return TGI_E_ARG;
-  FrontierDev* f = excl_set(c, which);
-  if (!f) return TGI_E_ARG;
+  KeySet* k = key_set(c, which, true);
+  if (!k) return TGI_E_ARG;
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
-  if (!f->table) return TGI_OK;
+  if (!k->dev.table) return TGI_OK;
   cudaStream_t st = c->slots[0].stream;
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-  int rc = frontier_clear_set(c, *f);
+  const int rc = set_clear(c, *k);
   if (rc) return rc;
-  c->x_bufs[which == TGI_SET_INVALID ? 0 : 1].bound = 0;
   CK(cudaStreamSynchronize(st));
   return TGI_OK;
 }
 int tgi_set_size(tgi_ctx* c, int which, uint64_t* n) {
   if (!c || !n) return TGI_E_ARG;
-  FrontierDev* f = excl_set(c, which);
-  if (!f) return TGI_E_ARG;
+  KeySet* k = key_set(c, which, true);
+  if (!k) return TGI_E_ARG;
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
-  *n = 0;
-  if (!f->table) return TGI_OK;
-  return frontier_read_count(c, *f, n);
+  return set_count(c, *k, n);
 }
 int tgi_set_now(tgi_ctx* c, int64_t now_sec) {
   if (!c) return TGI_E_ARG;
   std::lock_guard<std::mutex> g(c->fr_mu);
-  c->excl.now_sec = now_sec;
+  c->now_sec = now_sec;
   return TGI_OK;
 }
 int tgi_set_growth(tgi_ctx* c, uint64_t max_keys) {
@@ -2112,20 +2126,18 @@ int tgi_set_growth(tgi_ctx* c, uint64_t max_keys) {
 }
 int tgi_set_info(tgi_ctx* c, int which, tgi_set_info_t* out) {
   if (!c || !out) return TGI_E_ARG;
-  FrontierDev* f = which == TGI_SET_FRONTIER ? &c->fr : which == TGI_SET_OWNED ? &c->owned : excl_set(c, which);
-  const SetBufs* m = which == TGI_SET_FRONTIER ? &c->fr_bufs : which == TGI_SET_OWNED ? &c->o_bufs
-                     : &c->x_bufs[which == TGI_SET_INVALID ? 0 : 1];
-  if (!f) { set_err(c, "tgi_set_info: unknown set %d", which); return TGI_E_ARG; }
+  const KeySet* k = key_set(c, which, false);
+  if (!k) { set_err(c, "tgi_set_info: unknown set %d", which); return TGI_E_ARG; }
   cudaSetDevice(c->device);
   std::lock_guard<std::mutex> g(c->fr_mu);
   if (which == TGI_SET_OWNED && !c->comm) { set_err(c, "tgi_set_info: TGI_SET_OWNED needs tgi_comm_init first"); return TGI_E_STATE; }
   memset(out, 0, sizeof *out);
-  if (!f->table) return TGI_OK;  // an exclusion set before its first tgi_set_add
-  const int rc = frontier_read_count(c, *f, &out->count);
+  if (!k->dev.table) return TGI_OK;  // an exclusion set before its first tgi_set_add
+  const int rc = set_count(c, *k, &out->count);
   if (rc) return rc;
-  out->capacity = f->cap;
-  out->table_slots = f->tmask + 1;
-  out->grows = m->grows;
+  out->capacity = k->dev.cap;
+  out->table_slots = k->dev.tmask + 1;
+  out->grows = k->grows;
   return TGI_OK;
 }
 int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uint64_t cap, uint64_t* n) {
@@ -2141,8 +2153,7 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
   DevBuf drows;
   CK(drows.ensure(m * sizeof(tgi_edge)));
-  ExclusionDev x = c->excl;
-  x.now_sec = now_sec;
+  const ExclusionDev x = exclusion(c, now_sec);
   // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
   const uint32_t* chan = s.last_yt ? &s.yt.recs->chan_idx : &s.tg.recs->chan_idx;
   const uint32_t stride = s.last_yt ? (uint32_t)sizeof(tgi_yt_rec) : (uint32_t)sizeof(tgi_tg_rec);
@@ -2251,7 +2262,8 @@ int tgi_comm_init(tgi_ctx* c, const uint8_t id[TGI_COMM_ID_BYTES], int rank, int
   c->nranks = nranks;
   // this rank's partition of the global set: sized like the local set (a skewed hash cannot overflow it before the
   // local sets do)
-  const int rc = set_alloc(c, c->o_bufs, c->fr.cap, c->fr.tmask + 1, true, c->owned);
+  const FrontierDev& fr = c->sets[TGI_SET_FRONTIER].dev;
+  const int rc = set_alloc(c, c->sets[TGI_SET_OWNED], fr.cap, fr.tmask + 1, true);
   if (rc) return rc;
   cudaStream_t st = c->slots[0].stream;
   CK(c->m_cnt.ensure(64 * 8));
@@ -2276,7 +2288,7 @@ int tgi_comm_destroy(tgi_ctx* c) {
     c->comm = nullptr;
   }
   for (auto& e : c->m_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
-  c->owned = FrontierDev{};
+  c->sets[TGI_SET_OWNED].dev = FrontierDev{};
   return TGI_OK;
 }
 
@@ -2289,14 +2301,16 @@ int tgi_frontier_merge(tgi_ctx* c, uint64_t* global_size, uint64_t* owned) {
   const int G = c->nranks, me = c->rank;
   cudaStream_t st = c->slots[0].stream;
   uint64_t* hb = c->m_host.as<uint64_t>();
+  const uint8_t* pool = c->sets[TGI_SET_FRONTIER].dev.pool;
+  KeySet& part = c->sets[TGI_SET_OWNED];  // this rank's partition
   uint64_t sz = 0;
-  int rc = frontier_read_count(c, c->fr, &sz);
+  int rc = set_count(c, c->sets[TGI_SET_FRONTIER], &sz);
   if (rc) return rc;
   const uint64_t first = c->merged_upto, m = sz > first ? sz - first : 0;
   // 1. how many of my new keys go to each owner; every rank learns every count
   CK(cudaEventRecord(c->m_ev[0], st));
   CK(cudaMemsetAsync(c->m_cnt.p, 0, 64 * 8, st));
-  if (m) merge_count_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(c->fr.pool, first, m, (uint32_t)G, c->m_cnt.as<unsigned long long>());
+  if (m) merge_count_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(pool, first, m, (uint32_t)G, c->m_cnt.as<unsigned long long>());
   CK(cudaGetLastError());
   NK(N.AllGather(c->m_cnt.p, c->m_all.p, (size_t)G, ncclUint64, c->comm, st));
   CK(cudaMemcpyAsync(hb, c->m_all.p, (size_t)G * G * 8, cudaMemcpyDeviceToHost, st));
@@ -2317,7 +2331,7 @@ int tgi_frontier_merge(tgi_ctx* c, uint64_t* global_size, uint64_t* owned) {
   for (int p = 0; p < G; p++) hcur[p] = send_off[p];
   CK(cudaMemcpyAsync(c->m_cursor.p, hcur, (size_t)G * 8, cudaMemcpyHostToDevice, st));
   const uint64_t pay_base = (c->merge_round << 52) | ((uint64_t)me << 44);
-  if (m) merge_scatter_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(c->fr.pool, first, m, (uint32_t)G, c->m_cursor.as<unsigned long long>(),
+  if (m) merge_scatter_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(pool, first, m, (uint32_t)G, c->m_cursor.as<unsigned long long>(),
                                                                       c->m_send_keys.as<uint8_t>(), c->m_send_pay.as<uint64_t>(), pay_base);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->m_ev[1], st));
@@ -2346,19 +2360,17 @@ int tgi_frontier_merge(tgi_ctx* c, uint64_t* global_size, uint64_t* owned) {
   CK(cudaEventRecord(c->m_ev[2], st));
   // 4. the owner inserts what it received (source-rank-major: the lowest rank's copy of a key wins)
   if (R) {
-    rc = set_grow(c, c->owned, c->o_bufs, R, st);
-    if (rc) return rc;
-    rc = frontier_insert_locked(c, c->owned, c->m_recv_keys.p, c->m_recv_pay.as<uint64_t>(), R, nullptr);
+    rc = frontier_insert_enqueue(c, part, c->m_recv_keys.p, c->m_recv_pay.as<uint64_t>(), R, nullptr);
     if (rc) return rc;
   }
   // 5. global size = sum of the partitions
-  NK(N.AllReduce(c->owned.count, c->m_gsize.p, 1, ncclUint64, ncclSum, c->comm, st));
+  NK(N.AllReduce(part.dev.count, c->m_gsize.p, 1, ncclUint64, ncclSum, c->comm, st));
   CK(cudaEventRecord(c->m_ev[3], st));
   CK(cudaMemcpyAsync(hb, c->m_gsize.p, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(hb + 1, c->owned.count, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(hb + 1, part.dev.count, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (R) {
-    rc = frontier_insert_check(c, c->owned);
+    rc = frontier_insert_check(c, part);
     if (rc) return rc;
   }
   if (global_size) *global_size = hb[0];
@@ -2399,8 +2411,9 @@ int tgi_frontier_global_export(tgi_ctx* c, uint8_t* keys32, uint64_t cap, uint64
   const int G = c->nranks;
   cudaStream_t st = c->slots[0].stream;
   uint64_t* hb = c->m_host.as<uint64_t>();
+  const FrontierDev& owned = c->sets[TGI_SET_OWNED].dev;
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-  NK(N.AllGather(c->owned.count, c->m_all.p, 1, ncclUint64, c->comm, st));
+  NK(N.AllGather(owned.count, c->m_all.p, 1, ncclUint64, c->comm, st));
   CK(cudaMemcpyAsync(hb, c->m_all.p, (size_t)G * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   std::vector<uint64_t> off(G + 1, 0);
@@ -2412,8 +2425,8 @@ int tgi_frontier_global_export(tgi_ctx* c, uint8_t* keys32, uint64_t cap, uint64
   for (int p = 0; p < G; p++) {
     const uint64_t cnt = off[p + 1] - off[p];
     if (!cnt) continue;
-    NK(N.Broadcast(c->owned.pool, dk.as<uint8_t>() + 32 * off[p], cnt * 32, ncclUint8, p, c->comm, st));
-    NK(N.Broadcast(c->owned.payload, dp.as<uint64_t>() + off[p], cnt, ncclUint64, p, c->comm, st));
+    NK(N.Broadcast(owned.pool, dk.as<uint8_t>() + 32 * off[p], cnt * 32, ncclUint8, p, c->comm, st));
+    NK(N.Broadcast(owned.payload, dp.as<uint64_t>() + off[p], cnt, ncclUint64, p, c->comm, st));
   }
   std::vector<uint8_t> hk(T * 32);
   std::vector<uint64_t> hp(T);
