@@ -80,6 +80,7 @@ SET_FRONTIER, SET_INVALID, SET_DISCOVERED, SET_OWNED = 0, 1, 2, 3  # tgi_set_inf
 EDGE_PENDING, EDGE_DUPLICATE, EDGE_INVALID_CACHED = 0, 1, 2
 ROWS_STATUS, ROWS_LINK_OFF, ROWS_LINKS = 0, 1, 2  # tgi_result_read_rows
 RUN_SKIP_INVALID = 0x40
+RUN_JSONL_DEVICE = 0x80  # with RUN_JSONL: the lines stay on the device (tgi_result.jsonl is NULL)
 LF_INVALID = 0x08
 
 assert TG_REC.itemsize == 64 and ENTITY.itemsize == 16 and REACTION.itemsize == 12
@@ -144,6 +145,12 @@ class MergeStatsC(C.Structure):
 
 class SetInfoC(C.Structure):  # tgi_set_info_t
     _fields_ = [("count", C.c_uint64), ("capacity", C.c_uint64), ("table_slots", C.c_uint64), ("grows", C.c_uint64)]
+
+
+class DaprPayloadsC(C.Structure):  # tgi_dapr_payloads_t
+    _fields_ = [("n", C.c_uint64), ("data", C.c_void_p), ("data_len", C.c_uint64), ("data_off", C.c_void_p),
+                ("path", C.c_void_p), ("path_len", C.c_uint64), ("path_off", C.c_void_p), ("kernel_ms", C.c_float),
+                ("gpu_launches", C.c_uint32)]
 
 
 class StatsC(C.Structure):

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "kernels.cuh"
+#include "dapr.cuh"
 #include "tg_page.cuh"
 #include "yt_page.cuh"
 
@@ -120,6 +121,12 @@ struct NcclApi {
   const char* (*GetErrorString)(ncclResult_t) = nullptr;
 };
 
+// tgi_dapr_payloads: its device scratch and outputs, and the pinned host copies it returns
+struct DaprBufs {
+  DevBuf prefix, lens, off, data, path, sc;
+  HostBuf h_off, h_data, h_path, h_sc;
+};
+
 struct Slot {
   int idx = 0;
   cudaStream_t stream = nullptr;
@@ -150,6 +157,10 @@ struct Slot {
   uint64_t n_ents = 0, n_reacts = 0, n_comments = 0, in_bytes = 0, chan_strs_len = 0;
   bool resident = false;
   uint64_t dev_jsonl_len = 0;
+  // what tgi_dapr_payloads needs from the slot's last result: its device line offsets (nullptr: no lines) and kind
+  const uint64_t* dev_line_off = nullptr;
+  bool last_gm = false;
+  DaprBufs dapr;
   // what tgi_pending_edges needs from the slot's last batch
   uint64_t last_n = 0, last_new = 0;
   bool last_frontier = false, last_yt = false;
@@ -844,7 +855,7 @@ void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
   if (host) {
     out->status = host->status;
     if (want_json) {
-      out->jsonl = host->jsonl;
+      out->jsonl = (flags & TGI_RUN_JSONL_DEVICE) ? nullptr : host->jsonl;
       out->line_off = host->line_off;
     }
     if (want_links) {
@@ -855,6 +866,8 @@ void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
   s.dev_jsonl_len = out->jsonl_len;
   s.dev_jsonl = dev.jsonl;
   s.dev_status = dev.status;
+  s.dev_line_off = want_json ? dev.line_off : nullptr;
+  s.last_gm = kind == REC_GM;
   s.dev_link_off = want_links ? dev.link_off : nullptr;
   s.dev_links = want_links ? dev.links : nullptr;
   s.dev_n_links = out->n_links;
@@ -958,9 +971,9 @@ int finish_batch(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
     CK(cudaMemcpyAsync(s.h_status.p, s.d_status.p, n, cudaMemcpyDeviceToHost, st));
     if (want_json) {
       CK(s.h_line_off.ensure((n + 1) * 8));
-      CK(s.h_jsonl.ensure(line_total + 1));
+      if (!(flags & TGI_RUN_JSONL_DEVICE)) CK(s.h_jsonl.ensure(line_total + 1));  // the lines may stay on the device
       CK(cudaMemcpyAsync(s.h_line_off.p, s.d_line_off.p, (n + 1) * 8, cudaMemcpyDeviceToHost, st));
-      if (line_total) CK(cudaMemcpyAsync(s.h_jsonl.p, s.d_jsonl.p, line_total, cudaMemcpyDeviceToHost, st));
+      if (line_total && !(flags & TGI_RUN_JSONL_DEVICE)) CK(cudaMemcpyAsync(s.h_jsonl.p, s.d_jsonl.p, line_total, cudaMemcpyDeviceToHost, st));
     }
     if (want_links) {
       // the exact link count is one more host round trip away (behind the other slots' bulk copies on the copy engine);
@@ -1149,7 +1162,7 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint
   const uint64_t links_bytes = want_links ? up(n_links_total * sizeof(tgi_link), 256) : 0;
   rc = check_max_out(c, line_total);
   if (rc) return rc;
-  const uint64_t need = links_bytes + line_total;
+  const uint64_t need = links_bytes + ((flags & TGI_RUN_JSONL_DEVICE) ? 0 : line_total);  // the lines may stay behind
   if (need > spec) {
     CK(cudaMemcpyAsync(h + L.o_var + spec, d + L.o_var + spec, need - spec, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1164,7 +1177,9 @@ int page_launch_and_read(tgi_ctx* c, Slot& s, RecKind kind, uint32_t flags, uint
       fprintf(stderr, " slowest %s: rec %u %.1f us", what[k], (unsigned)t[PAGE_PHASES + 1 + k], (double)(t[PAGE_PHASES + 1 + k] >> 32) / 1965.0);
     fprintf(stderr, "\n");
   }
-  s.page_bpr = (uint32_t)std::min<uint64_t>(1u << 20, (3ull * s.page_bpr + need / n + 1) / 4 + (need > spec ? need / n / 4 : 0));
+  // the estimate learns from whole results only: a result whose lines stayed behind would under-size the next read
+  if (!(flags & TGI_RUN_JSONL_DEVICE))
+    s.page_bpr = (uint32_t)std::min<uint64_t>(1u << 20, (3ull * s.page_bpr + need / n + 1) / 4 + (need > spec ? need / n / 4 : 0));
   const ResultArrays dev{d + L.o_status, (const uint64_t*)(d + L.o_line_off), d + L.o_var + links_bytes, (const uint32_t*)(d + L.o_link_off),
                          (const tgi_link*)(d + L.o_var)};
   const ResultArrays host{h + L.o_status, (const uint64_t*)(h + L.o_line_off), h + L.o_var + links_bytes, (const uint32_t*)(h + L.o_link_off),
@@ -1510,6 +1525,7 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
 // ---- jobs -------------------------------------------------------------------------------------------------------------
 // upload (for the kinds that carry a batch), synchronise (upload-only jobs), run; the inputs are the slot's in_* / run_flags
 int run_job(tgi_ctx* c, Slot& s, JobKind job) {
+  s.dev_line_off = nullptr;  // the slot's last result is gone from here on, and an upload replaces its batch descriptor
   if (job == JOB_GM) return run_gm(c, s, s.in_gm, s.run_flags, &s.res);
   const bool tg = job == JOB_TG || job == JOB_TG_RESIDENT || job == JOB_TG_UPLOAD;
   const bool upload_only = job == JOB_TG_UPLOAD || job == JOB_YT_UPLOAD;
@@ -1546,10 +1562,19 @@ void worker_main(tgi_ctx* c, Slot* s) {
   }
 }
 
+bool run_flags_ok(tgi_ctx* c, uint32_t flags) {
+  if ((flags & TGI_RUN_JSONL_DEVICE) && !(flags & TGI_RUN_JSONL)) {
+    set_err(c, "TGI_RUN_JSONL_DEVICE without TGI_RUN_JSONL");
+    return false;
+  }
+  return true;
+}
+
 int post_job(tgi_ctx* c, int slot, JobKind kind, const tgi_tg_batch* in, uint32_t flags, const tgi_yt_batch* in_yt = nullptr,
              const tgi_gm_batch* in_gm = nullptr) {
   if (!c) return TGI_E_ARG;
   if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "bad slot %d", slot); return TGI_E_ARG; }
+  if (!run_flags_ok(c, flags)) return TGI_E_ARG;
   Slot& s = c->slots[slot];
   std::lock_guard<std::mutex> lk(s.mu);
   if (s.busy) { set_err(c, "slot %d is busy (wait/release it first)", slot); return TGI_E_STATE; }
@@ -1583,6 +1608,7 @@ int wait_job(tgi_ctx* c, int slot, tgi_result* out) {
 // hand-offs per call are most of what a page-sized batch costs besides the launches themselves.
 int run_inline(tgi_ctx* c, int slot, JobKind kind, const tgi_tg_batch* in_tg, const tgi_yt_batch* in_yt, const tgi_gm_batch* in_gm,
                uint32_t flags, tgi_result* out) {
+  if (!run_flags_ok(c, flags)) return TGI_E_ARG;
   Slot& s = c->slots[slot];
   {
     std::lock_guard<std::mutex> lk(s.mu);
@@ -2163,6 +2189,103 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(rows, drows.p, m * sizeof(tgi_edge), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  return TGI_OK;
+}
+
+// Dapr sink payloads (dapr.cuh): size, two scans, one synchronise for the totals, write, the four copies, one synchronise.
+int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t prefix_len, tgi_dapr_payloads_t* out) {
+  if (!c || !out || !path_prefix || slot < 0 || slot >= TGI_SLOTS) return TGI_E_ARG;
+  cudaSetDevice(c->device);
+  Slot& s = c->slots[slot];
+  {
+    std::lock_guard<std::mutex> lk(s.mu);
+    if (s.busy && !s.done) { set_err(c, "tgi_dapr_payloads: slot %d is in flight", slot); return TGI_E_STATE; }
+  }
+  if (s.last_gm) { set_err(c, "tgi_dapr_payloads: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
+  if (!s.dev_line_off) { set_err(c, "tgi_dapr_payloads: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
+  DaprBufs& z = s.dapr;
+  cudaStream_t st = s.stream;
+  const uint64_t n = s.last_n;
+  memset(out, 0, sizeof *out);
+  out->n = n;
+  CK(z.h_off.ensure(2 * (n + 1) * 8));
+  uint64_t* h_off = z.h_off.as<uint64_t>();
+  out->data_off = h_off;
+  out->path_off = h_off + n + 1;
+  if (!n) {
+    h_off[0] = h_off[1] = 0;
+    return TGI_OK;
+  }
+  DaprSrc src{};
+  src.n = n;
+  src.status = s.dev_status;
+  src.line_off = s.dev_line_off;
+  src.jsonl = s.dev_jsonl;
+  src.yt = s.last_yt;
+  // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
+  if (s.last_yt) {
+    src.yt_recs = s.yt.recs, src.yt_chans = s.yt.chans, src.strs = s.yt.strs, src.chan_strs = s.yt.chan_strs;
+  } else {
+    src.tg_recs = s.tg.recs, src.tg_chans = s.tg.chans, src.strs = s.tg.strs, src.chan_strs = s.tg.chan_strs;
+  }
+  src.prefix_len = prefix_len;
+  CK(z.prefix.ensure(prefix_len));
+  if (prefix_len) CK(cudaMemcpyAsync(z.prefix.p, path_prefix, prefix_len, cudaMemcpyHostToDevice, st));
+  src.prefix = z.prefix.as<uint8_t>();
+  CK(z.lens.ensure(2 * n * 4));
+  CK(z.off.ensure(2 * (n + 1) * 8));
+  CK(z.sc.ensure(4 * 8));
+  CK(z.h_sc.ensure(4 * 8));
+  uint64_t* dsc = z.sc.as<uint64_t>();  // data total | path total | error word
+  DaprOut o{};
+  o.data_len = z.lens.as<uint32_t>();
+  o.path_len = o.data_len + n;
+  o.data_off = z.off.as<uint64_t>();
+  o.path_off = o.data_off + n + 1;
+  o.err = (int*)(dsc + 2);
+  uint32_t launches = 0;
+  // device time = [ev_p0, ev_p1] (size kernel, scans) + [ev_e0, ev_e1] (writer): the totals' read-back and the host's
+  // allocations between them are left out.  The batch's own times were read into its result already.
+  CK(cudaMemsetAsync(dsc, 0, 4 * 8, st));
+  CK(cudaEventRecord(s.ev_p0, st));
+  const unsigned gs = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
+  dapr_size_kernel<<<gs, 256, 0, st>>>(src, o);
+  launches++;
+  int rc = launch_scan(c, s, o.data_len, n, (uint64_t*)o.data_off, dsc, launches);
+  if (rc) return rc;
+  rc = launch_scan(c, s, o.path_len, n, (uint64_t*)o.path_off, dsc + 1, launches);
+  if (rc) return rc;
+  CK(cudaEventRecord(s.ev_p1, st));
+  CK(cudaMemcpyAsync(z.h_sc.p, dsc, 4 * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t* hsc = z.h_sc.as<uint64_t>();
+  if (hsc[2]) { set_err(c, "tgi_dapr_payloads: a payload or path of 4 GiB or more"); return TGI_E_CAPACITY; }
+  const uint64_t data_total = hsc[0], path_total = hsc[1];
+  CK(z.data.ensure(data_total));
+  CK(z.path.ensure(path_total));
+  CK(z.h_data.ensure(data_total + 1));
+  CK(z.h_path.ensure(path_total + 1));
+  o.data = z.data.as<uint8_t>();
+  o.path = z.path.as<uint8_t>();
+  const unsigned gw = (unsigned)std::min<uint64_t>((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * 32);  // 5 resident CTAs per SM
+  CK(cudaEventRecord(s.ev_e0, st));
+  dapr_write_kernel<<<gw, CTA_THREADS, 0, st>>>(src, o);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(s.ev_e1, st));
+  CK(cudaMemcpyAsync(h_off, o.data_off, 2 * (n + 1) * 8, cudaMemcpyDeviceToHost, st));
+  if (data_total) CK(cudaMemcpyAsync(z.h_data.p, o.data, data_total, cudaMemcpyDeviceToHost, st));
+  if (path_total) CK(cudaMemcpyAsync(z.h_path.p, o.path, path_total, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  out->data = z.h_data.as<uint8_t>();
+  out->data_len = data_total;
+  out->path = z.h_path.as<uint8_t>();
+  out->path_len = path_total;
+  float size_ms = 0, write_ms = 0;
+  cudaEventElapsedTime(&size_ms, s.ev_p0, s.ev_p1);
+  cudaEventElapsedTime(&write_ms, s.ev_e0, s.ev_e1);
+  out->kernel_ms = size_ms + write_ms;
+  out->gpu_launches = launches;
   return TGI_OK;
 }
 

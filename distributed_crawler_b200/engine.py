@@ -35,7 +35,7 @@ EXPORTED_SYMBOLS = [
     "tgi_filter_usernames", "tgi_acquire_staging", "tgi_release_staging", "tgi_comm_unique_id", "tgi_comm_init",
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
-    "tgi_set_growth", "tgi_set_info",
+    "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads",
 ]
 
 
@@ -96,6 +96,7 @@ def lib() -> C.CDLL:
         L.tgi_plan_channel_appends.argtypes = [vp, vp, u32, u64, vp, u64, C.POINTER(u64)]
         L.tgi_set_growth.argtypes = [vp, u64]
         L.tgi_set_info.argtypes = [vp, i32, C.POINTER(abi.SetInfoC)]
+        L.tgi_dapr_payloads.argtypes = [vp, i32, C.c_char_p, u32, C.POINTER(abi.DaprPayloadsC)]
         _LIB = L
     return _LIB
 
@@ -126,6 +127,7 @@ class Result:
         self.main_bytes_in = int(r.main_bytes_in)
         self.has_links = bool(r.link_off)
         self.has_jsonl = bool(r.line_off)
+        self.jsonl_on_device = self.has_jsonl and not r.jsonl and self.jsonl_len > 0  # RUN_JSONL_DEVICE: not copied
         self.gpu_launches = int(r.gpu_launches)
         self.slot = int(r.slot)
         if copy:
@@ -139,7 +141,7 @@ class Result:
         """bytes the library copied device -> pinned host for this result"""
         b = self.n + 80  # status + scalars
         if self.has_jsonl:
-            b += self.jsonl_len + 8 * (self.n + 1)
+            b += (0 if self.jsonl_on_device else self.jsonl_len) + 8 * (self.n + 1)
         if self.has_links:
             b += 4 * (self.n + 1) + 36 * self.n_links
         return b
@@ -153,6 +155,29 @@ class Result:
             l = self.links[k]
             out.append((l["name"][: int(l["len"])].tobytes(), abi.SRC_NAMES[int(l["src"])]))
         return out
+
+
+class DaprPayloads:
+    """Host copy of a tgi_dapr_payloads_t: record i's binding Data is data(i), its blob path path(i); both are empty
+    for records without a post."""
+
+    def __init__(self, r: abi.DaprPayloadsC):
+        n = int(r.n)
+        self.n = n
+        self.data_len = int(r.data_len)
+        self.path_len = int(r.path_len)
+        self.kernel_ms = float(r.kernel_ms)
+        self.gpu_launches = int(r.gpu_launches)
+        self.data_off = _copy(r.data_off, n + 1, np.uint64)
+        self.path_off = _copy(r.path_off, n + 1, np.uint64)
+        self.data_blob = _copy(r.data, self.data_len, np.uint8)
+        self.path_blob = _copy(r.path, self.path_len, np.uint8)
+
+    def data(self, i: int) -> bytes:
+        return self.data_blob[int(self.data_off[i]):int(self.data_off[i + 1])].tobytes()
+
+    def path(self, i: int) -> bytes:
+        return self.path_blob[int(self.path_off[i]):int(self.path_off[i + 1])].tobytes()
 
 
 class Engine:
@@ -354,6 +379,13 @@ class Engine:
         if n.value:
             self._check(lib().tgi_pending_edges(self.h, slot, now_sec, rows.ctypes.data, n.value, C.byref(n)))
         return rows
+
+    def dapr_payloads(self, slot: int, prefix: bytes) -> "DaprPayloads":
+        """host copies of the StorePost binding payloads of the slot's last Telegram / YouTube result (call before
+        release): the base64 of every line, and its blob path prefix | channelID | /posts/ | PostUID | .jsonl"""
+        out = abi.DaprPayloadsC()
+        self._check(lib().tgi_dapr_payloads(self.h, slot, prefix, len(prefix), C.byref(out)))
+        return DaprPayloads(out)
 
     # --- generic client.Message -> sparse Post (SURVEY a12) -------------------------------------
     def generic(self, batch, run_flags=abi.RUN_JSONL, copy=True) -> Result:

@@ -206,6 +206,14 @@ class Result {
     return v;
   }
   const tgi_result& Raw() const { return r_; }
+  // DaprStateManager.StorePost's binding payloads (state/daprstate.go:1141-1181) for every message of this result:
+  // base64 of its line and its blob path prefix|channelID|/posts/|PostUID|.jsonl; valid until the next call or the release
+  tgi_dapr_payloads_t DaprPayloads(std::string_view path_prefix) const {
+    tgi_dapr_payloads_t p{};
+    if (tgi_dapr_payloads(ctx_, r_.slot, path_prefix.data(), (uint32_t)path_prefix.size(), &p) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return p;
+  }
 
  private:
   tgi_ctx* ctx_;

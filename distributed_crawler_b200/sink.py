@@ -1,8 +1,13 @@
-"""Combined-blob sink (SURVEY §8f rank 1): groups the JSONL lines of one engine result into the blobs the reference's
+"""Sinks for the lines of an engine result.
+
+Combined-blob sink (SURVEY §8f rank 1): groups the JSONL lines of one engine result into the blobs the reference's
 chunk combiner would upload as combined_<ns>.jsonl (chunk/main.go:292-421), without one file per post.
 
 The grouping rule is libtgingest's tgi_plan_chunks (a restatement of Chunker.processBatches); the bytes of a group are
-a contiguous slice of the result's JSONL blob (minus lines dropped for exceeding the hard cap)."""
+a contiguous slice of the result's JSONL blob (minus lines dropped for exceeding the hard cap).
+
+Local sink: append_posts (LocalStateManager.StorePost).  Dapr sink: store_posts_dapr (DaprStateManager.StorePost outside
+combine mode), fed by Engine.dapr_payloads."""
 from __future__ import annotations
 
 import ctypes as C
@@ -77,3 +82,18 @@ def append_posts(jsonl: bytes | np.ndarray, line_off: np.ndarray, recs: np.ndarr
         with open(os.path.join(d, "posts.jsonl"), "ab") as f:
             f.write(buf[int(r["byte_begin"]): int(r["byte_end"])])
     return len(runs)
+
+
+def store_posts_dapr(invoke, payloads, binding: str, naming_key: str) -> int:
+    """DaprStateManager.StorePost outside combine mode (state/daprstate.go:1141-1181) for a whole result: one
+    invoke(binding, "create", data, metadata) per post, in record order, with data = the base64 of its line and metadata
+    {naming_key: blob path, "operation": "append"}; the path is raw bytes, as a Go string holds it.  `payloads` is Engine.dapr_payloads(slot, prefix); naming_key is
+    fetchFileNamingComponent's answer for the binding, resolved once per crawl.  Records without a post are skipped.
+    Returns the number of requests."""
+    k = 0
+    for i in range(payloads.n):
+        if payloads.data_off[i + 1] == payloads.data_off[i]:
+            continue
+        invoke(binding, "create", payloads.data(i), {naming_key: payloads.path(i), "operation": "append"})
+        k += 1
+    return k

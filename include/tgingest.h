@@ -306,6 +306,8 @@ typedef struct tgi_config {
 #define TGI_RUN_NO_D2H 0x20     /* bench only: leave results on the device (kernel-only timing)   */
 #define TGI_RUN_SKIP_INVALID 0x40 /* tandem mode: drop outlinks found in the resident invalid-channel set before they
                                    reach the dedup set (crawl/runner.go:1247 sm.IsInvalidChannel); link.flags INVALID */
+#define TGI_RUN_JSONL_DEVICE 0x80 /* with TGI_RUN_JSONL: lines are emitted but stay on the device; tgi_result.jsonl is
+                                     NULL, jsonl_len and line_off are filled (for tgi_dapr_payloads / tgi_result_read_jsonl) */
 
 #define TGI_LF_FILTER_OK 0x01 /* FilterUsername(name).Valid                                       */
 #define TGI_LF_NEW 0x02       /* first occurrence in the global frontier set                      */
@@ -425,6 +427,36 @@ typedef struct tgi_append_run {
 } tgi_append_run;
 int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uint32_t chan_stride, uint64_t n,
                              tgi_append_run* runs, uint64_t max_runs, uint64_t* n_runs);
+
+/* Dapr sink — DaprStateManager.StorePost outside combine mode (state/daprstate.go:1141-1181) sends, per post, ONE
+ * InvokeBinding with Operation "create", Data = base64.StdEncoding.EncodeToString(json.Marshal(post) + "\n") (:1159)
+ * and Metadata {<file naming key>: <blob path>, "operation": "append"} (:1150-1153, path format :2689-2698).
+ * tgi_dapr_payloads computes both byte strings on the device for every record of the slot's last Telegram or YouTube
+ * result, from the lines that are still resident (run the batch with TGI_RUN_JSONL_DEVICE to leave them there).
+ *   path_prefix  StorageRoot + "/" + CrawlID + "/" + CrawlExecutionID + "/", taken verbatim (prefix_len bytes).
+ *   data         record i's line, '\n' included, in Go's StdEncoding: A-Z a-z 0-9 + /, '=' padding, no line breaks,
+ *                4*ceil(len/3) bytes; data[data_off[i], data_off[i+1]).
+ *   path         prefix | channelID | "/posts/" | PostUID | ".jsonl", raw bytes (not JSON-escaped);
+ *                path[path_off[i], path_off[i+1]).  Telegram: channelID = the channel row's name (the channelName
+ *                argument, tdutils.go:725), PostUID = FormatInt(id / 1048576) + "-" + channelName (tdutils.go:416,636,
+ *                1008; truncating division).  YouTube: channelID = the channel row's id (video.ChannelID,
+ *                youtube_crawler.go:396), PostUID = the record's id (video.ID, :701).
+ * Only records with status TGI_ST_EMITTED get a payload; the others get empty ranges: a date-skipped message never
+ * reaches StorePost (tdutils.go:419-421), a failed one panicked before it, and a TGI_ST_NOLINE one failed json.Marshal
+ * before any binding call (daprstate.go:1141-1144).
+ * Call between tgi_*_wait / tgi_*_batch and tgi_result_release (like tgi_pending_edges); works after TGI_RUN_NO_D2H and
+ * TGI_RUN_JSONL_DEVICE.  Outputs live in library-owned pinned memory and stay valid until the release or the next call
+ * on that slot.  TGI_E_STATE: the last result is a tgi_generic_batch one (its posts go to SavePost,
+ * crawler/common/runner.go:55, which has no Dapr implementation) or ran without TGI_RUN_JSONL; TGI_E_ARG: bad slot or
+ * NULL prefix / out; TGI_E_NOMEM: allocation failed (the batch result stays valid).                                  */
+typedef struct tgi_dapr_payloads_t {
+  uint64_t n;
+  const uint8_t* data;  uint64_t data_len;  const uint64_t* data_off;  /* [n+1] base64 of record i's line          */
+  const uint8_t* path;  uint64_t path_len;  const uint64_t* path_off;  /* [n+1] blob path of record i               */
+  float kernel_ms;      /* device time of this call's kernels (sizes + scans, writer; not the read-back between) */
+  uint32_t gpu_launches;
+} tgi_dapr_payloads_t;
+int tgi_dapr_payloads(tgi_ctx* ctx, int slot, const char* path_prefix, uint32_t prefix_len, tgi_dapr_payloads_t* out);
 
 /* SURVEY §8f rank 2 — the message-status join.  The reference looks messages up by (ChatID, MessageID) with
  * string-keyed maps or linear scans: resampleMarker (crawl/runner.go:1572-1635), addNewMessages (:1650-1697), the

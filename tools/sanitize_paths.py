@@ -47,4 +47,11 @@ big = [msg("messageText", " ".join("t.me/chan_%05d" % i for i in range(3000)), r
 print("big", e.telegram(pack_telegram(big), f).n_links)
 e.comm_init(Engine.comm_unique_id(), 0, 1)
 print("merge", e.frontier_merge(), len(e.frontier_global_export()))
+# Dapr sink payloads after a bulk batch, a page and a YouTube page, with the lines left on the device
+for b, yt in ((Corpus(20000, profile=2, nthreads=4).batch, False), (Corpus(300, profile=3, nthreads=4).batch, False),
+              (make_youtube(50, seed=5)[0], True)):
+    (e.youtube_submit if yt else e.telegram_submit)(0, b, abi.RUN_JSONL | abi.RUN_JSONL_DEVICE)
+    (e.youtube_wait if yt else e.telegram_wait)(0)
+    print("dapr", e.dapr_payloads(0, b"root/crawl/exec/").data_len)
+    e.release(0)
 print("done")
