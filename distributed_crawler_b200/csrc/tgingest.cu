@@ -85,7 +85,33 @@ struct HostBuf {  // pinned
   T* as() const { return (T*)p; }
 };
 
-enum JobKind { JOB_NONE = 0, JOB_TG, JOB_TG_RESIDENT, JOB_TG_UPLOAD, JOB_YT, JOB_YT_RESIDENT, JOB_YT_UPLOAD, JOB_GM, JOB_QUIT };
+enum RecKind { REC_NONE, REC_TG, REC_YT, REC_GM };
+
+// One job on a staging slot: upload a batch (which becomes the slot's resident batch), run the resident batch, or both.
+enum JobStages : uint32_t { JOB_UPLOAD = 1, JOB_RUN = 2 };
+struct Job {
+  RecKind kind;
+  uint32_t stages;    // JOB_UPLOAD | JOB_RUN
+  const void* batch;  // JOB_UPLOAD: the tgi_tg_batch / tgi_yt_batch / tgi_gm_batch of `kind`
+  uint32_t flags;     // JOB_RUN: TGI_RUN_*
+};
+
+struct ResultArrays {  // where a batch's result arrays are, on the host or on the device
+  const uint8_t* status;
+  const uint64_t* line_off;
+  const uint8_t* jsonl;
+  const uint32_t* link_off;
+  const tgi_link* links;
+};
+// What the readers (tgi_result_read_*, tgi_pending_edges, tgi_dapr_payloads) read: the result of the slot's last job,
+// from its success until the next job is claimed on the slot.  kind == REC_NONE: the slot holds no result.
+struct LastResult {
+  RecKind kind = REC_NONE;
+  uint64_t n = 0;
+  uint32_t flags = 0;  // the run flags that shaped it
+  uint64_t n_new = 0, n_links = 0, jsonl_len = 0;
+  ResultArrays dev{};  // its arrays on the device; line_off / link_off / links are null when the run did not make them
+};
 
 // one batch's frontier phases: the batch hash table, per-link state, per-record NEW counts and their offsets
 struct FrontierScratch {
@@ -144,35 +170,21 @@ struct Slot {
   DevBuf d_page_in, d_page_out;
   HostBuf h_page_in, h_page_out;
   uint32_t page_bpr = 3072;              // running estimate of result bytes per record (sizes the speculative read)
-  const uint8_t* dev_jsonl = nullptr;    // where the last batch's JSONL lives on the device (tgi_result_read_jsonl)
-  const uint8_t* dev_status = nullptr;   // ... and its status, link offsets and link rows (tgi_result_read_rows)
-  const uint32_t* dev_link_off = nullptr;
-  const tgi_link* dev_links = nullptr;
-  uint64_t dev_n_links = 0;
-  // resident batch descriptor
+  // batch descriptors, filled by the uploads (`resident` says which one still describes the batch on the device)
   TgBatchDev tg{};
   YtBatchDev yt{};
   GmBatchDev gm{};
   uint64_t yt_desc_bytes = 0;
   uint64_t n_ents = 0, n_reacts = 0, n_comments = 0, in_bytes = 0, chan_strs_len = 0;
-  bool resident = false;
-  uint64_t dev_jsonl_len = 0;
-  // what tgi_dapr_payloads needs from the slot's last result: its device line offsets (nullptr: no lines) and kind
-  const uint64_t* dev_line_off = nullptr;
-  bool last_gm = false;
+  RecKind resident = REC_NONE;  // REC_TG / REC_YT: tg / yt describes the batch of the last successful upload
+  LastResult last;
   DaprBufs dapr;
-  // what tgi_pending_edges needs from the slot's last batch
-  uint64_t last_n = 0, last_new = 0;
-  bool last_frontier = false, last_yt = false;
-  // job hand-off
+  // job hand-off (under mu)
   std::mutex mu;
   std::condition_variable cv;
-  JobKind job = JOB_NONE;
+  enum { IDLE, QUEUED, QUIT } worker_state = IDLE;  // what the worker thread has to do: nothing, `job`, exit
+  Job job{};
   bool busy = false, done = false, claimed = false;
-  const tgi_tg_batch* in_tg = nullptr;
-  const tgi_yt_batch* in_yt = nullptr;
-  const tgi_gm_batch* in_gm = nullptr;
-  uint32_t run_flags = 0;
   uint64_t ticket = 0;
   bool has_ticket = false;
   int rc = 0;
@@ -764,24 +776,12 @@ int upload_tg(tgi_ctx* c, Slot& s, const tgi_tg_batch* in) {
     CK(cudaStreamSynchronize(s.stream));
     const int hbad = *s.h_scalars.as<int>();
     trace_slot(s, "upload: landed + validated");
-    if (hbad) {
-      s.resident = false;
-      set_err(c, "telegram batch: offsets outside their arrays (mask 0x%x)", hbad);
-      return TGI_E_ARG;
-    }
+    if (hbad) { set_err(c, "telegram batch: offsets outside their arrays (mask 0x%x)", hbad); return TGI_E_ARG; }
   }
-  s.resident = true;
   return TGI_OK;
 }
 
 // ---- frontier turns ---------------------------------------------------------------------------------------------------
-void take_ticket(tgi_ctx* c, Slot& s, JobKind kind, uint32_t flags) {
-  const bool runs = kind == JOB_TG || kind == JOB_TG_RESIDENT || kind == JOB_YT || kind == JOB_YT_RESIDENT;
-  if (!runs || !(flags & TGI_RUN_FRONTIER)) return;
-  std::lock_guard<std::mutex> g(c->tk_mu);
-  s.ticket = c->tk_next++;
-  s.has_ticket = true;
-}
 void turn_begin(tgi_ctx* c, Slot& s) {
   if (!s.has_ticket) return;
   std::unique_lock<std::mutex> lk(c->tk_mu);
@@ -804,8 +804,6 @@ void turn_pass(tgi_ctx* c, Slot& s) {
 }
 
 // ---- results ----------------------------------------------------------------------------------------------------------
-enum RecKind { REC_TG, REC_YT, REC_GM };
-
 uint32_t sc_cursor(const uint64_t* hsc) { return ((const uint32_t*)(hsc + SC_CURSOR))[0]; }
 int sc_err(const uint64_t* hsc) { return ((const int*)(hsc + SC_CURSOR))[1]; }
 
@@ -823,16 +821,8 @@ int check_max_out(tgi_ctx* c, uint64_t line_total) {
   return TGI_OK;
 }
 
-struct ResultArrays {  // where a batch's result arrays are, on the host or on the device
-  const uint8_t* status;
-  const uint64_t* line_off;
-  const uint8_t* jsonl;
-  const uint32_t* link_off;
-  const tgi_link* links;
-};
-// Fills *out, the slot's device read-back pointers (tgi_result_read_*), its hand-off state (tgi_pending_edges) and the
-// context stats from a batch that has run to the end; hsc is its scalars block on the host.  `host` is nullptr when the
-// result stays on the device.
+// Fills *out, the slot's last result (the readers') and the context stats from a batch that has run to the end; hsc is
+// its scalars block on the host.  `host` is nullptr when the result stays on the device.
 void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, const uint64_t* hsc, uint64_t line_total,
                  uint32_t launches, const ResultArrays* host, const ResultArrays& dev, tgi_result* out) {
   const bool want_json = flags & TGI_RUN_JSONL, want_links = flags & TGI_RUN_LINKS, want_fr = flags & TGI_RUN_FRONTIER;
@@ -863,18 +853,9 @@ void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
       out->links = host->links;
     }
   }
-  s.dev_jsonl_len = out->jsonl_len;
-  s.dev_jsonl = dev.jsonl;
-  s.dev_status = dev.status;
-  s.dev_line_off = want_json ? dev.line_off : nullptr;
-  s.last_gm = kind == REC_GM;
-  s.dev_link_off = want_links ? dev.link_off : nullptr;
-  s.dev_links = want_links ? dev.links : nullptr;
-  s.dev_n_links = out->n_links;
-  s.last_n = n;
-  s.last_new = out->n_new;
-  s.last_frontier = want_fr && n;
-  s.last_yt = kind == REC_YT;
+  s.last = LastResult{kind, n, flags, out->n_new, out->n_links, out->jsonl_len,
+                      {dev.status, want_json ? dev.line_off : nullptr, dev.jsonl, want_links ? dev.link_off : nullptr,
+                       want_links ? dev.links : nullptr}};
   std::lock_guard<std::mutex> g(c->st_mu);
   c->stats.records += n;
   c->stats.bytes_in += s.in_bytes;
@@ -1369,8 +1350,6 @@ int upload_yt(tgi_ctx* c, Slot& s, const tgi_yt_batch* in) {
   b.n = in->n;
   b.n_chans = in->n_chans;
   s.yt_desc_bytes = in->strs_len;
-  s.resident = true;
-  s.tg.n = 0;
   return TGI_OK;
 }
 
@@ -1451,8 +1430,8 @@ int run_yt(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   return finish_batch(c, s, REC_YT, n, flags, t.line_total, t.cursor, yt_arena_cap(s), launches, out);
 }
 
-// generic client.Message batch (a12): upload, size, scan, emit; no links
-int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_result* out) {
+// generic client.Message batch (a12): upload, then size, scan, emit; no links
+int upload_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in) {
   if (!in) { set_err(c, "null batch"); return TGI_E_ARG; }
   if (in->n && !in->recs) { set_err(c, "generic batch: recs must be non-null"); return TGI_E_ARG; }
   if (in->n >= (1ull << 40)) { set_err(c, "generic batch: too many records"); return TGI_E_ARG; }
@@ -1469,16 +1448,14 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
     if (e) { set_err(c, "generic batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
   }
   const uint64_t n = in->n;
-  cudaStream_t st = s.stream;
   s.in_bytes = 0;
-  s.resident = false;
   InArrays a;
   a.add(s.d_recs, in->recs, n * sizeof(tgi_gm_rec));
   a.add(s.d_strs, in->strs, in->strs_len);
   a.add(s.d_react_off, in->react_off, in->react_off ? (n + 1) * 4 : 0);
   a.add(s.d_reacts, in->reacts, in->n_reacts * sizeof(tgi_gm_reaction));
   a.add(s.d_aux, in->aux, in->aux_len);
-  int rc = upload_arrays(c, s, a, false);
+  const int rc = upload_arrays(c, s, a, false);
   if (rc) return rc;
   GmBatchDev& b = s.gm;
   b.n = n;
@@ -1487,11 +1464,18 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
   b.react_off = in->react_off ? (const uint32_t*)a.dev[2] : nullptr;
   b.reacts = (const tgi_gm_reaction*)a.dev[3];
   b.aux = a.dev[4];
+  return TGI_OK;
+}
+
+int run_gm(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
+  const GmBatchDev& b = s.gm;
+  const uint64_t n = b.n;
+  cudaStream_t st = s.stream;
   uint32_t launches = 0;
   const bool want_json = flags & TGI_RUN_JSONL;
   const CfgDev cfg = cfg_snapshot(c);
   CK(s.d_arena.ensure(1024 * sizeof(tgi_link)));
-  rc = bulk_prologue(c, s, n);
+  int rc = bulk_prologue(c, s, n);
   if (rc) return rc;
   if (n) {
     CK(cudaMemsetAsync(s.d_link_start.p, 0, n * 4, st));
@@ -1519,45 +1503,50 @@ int run_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in, uint32_t flags, tgi_resu
     CK(cudaEventRecord(s.ev_e1, st));
     CK(cudaGetLastError());
   }
-  return finish_batch(c, s, REC_GM, n, flags & ~(uint32_t)TGI_RUN_FRONTIER, t.line_total, 0, 1024, launches, out);
+  return finish_batch(c, s, REC_GM, n, flags, t.line_total, 0, 1024, launches, out);
 }
 
 // ---- jobs -------------------------------------------------------------------------------------------------------------
-// upload (for the kinds that carry a batch), synchronise (upload-only jobs), run; the inputs are the slot's in_* / run_flags
-int run_job(tgi_ctx* c, Slot& s, JobKind job) {
-  s.dev_line_off = nullptr;  // the slot's last result is gone from here on, and an upload replaces its batch descriptor
-  if (job == JOB_GM) return run_gm(c, s, s.in_gm, s.run_flags, &s.res);
-  const bool tg = job == JOB_TG || job == JOB_TG_RESIDENT || job == JOB_TG_UPLOAD;
-  const bool upload_only = job == JOB_TG_UPLOAD || job == JOB_YT_UPLOAD;
-  int rc = TGI_OK;
-  if (job != JOB_TG_RESIDENT && job != JOB_YT_RESIDENT) rc = tg ? upload_tg(c, s, s.in_tg) : upload_yt(c, s, s.in_yt);
-  if (rc != TGI_OK) return rc;
-  if (upload_only) {
-    cudaError_t e = cudaStreamSynchronize(s.stream);
-    if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); return TGI_E_CUDA; }
-    return TGI_OK;
+// Upload if the job uploads (an upload-only job waits for the copy to land), run if it runs.
+int run_job(tgi_ctx* c, Slot& s) {
+  const Job& j = s.job;
+  if (j.stages & JOB_UPLOAD) {
+    const int rc = j.kind == REC_TG   ? upload_tg(c, s, (const tgi_tg_batch*)j.batch)
+                   : j.kind == REC_YT ? upload_yt(c, s, (const tgi_yt_batch*)j.batch)
+                                      : upload_gm(c, s, (const tgi_gm_batch*)j.batch);
+    if (rc != TGI_OK) return rc;
+    if (!(j.stages & JOB_RUN)) {
+      const cudaError_t e = cudaStreamSynchronize(s.stream);
+      if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); return TGI_E_CUDA; }
+    }
+    if (j.kind != REC_GM) s.resident = j.kind;  // generic batches are not run resident
   }
-  return tg ? run_tg(c, s, s.run_flags, &s.res) : run_yt(c, s, s.run_flags, &s.res);
+  if (!(j.stages & JOB_RUN)) return TGI_OK;
+  return j.kind == REC_TG   ? run_tg(c, s, j.flags, &s.res)
+         : j.kind == REC_YT ? run_yt(c, s, j.flags, &s.res)
+                            : run_gm(c, s, j.flags, &s.res);
+}
+
+// runs the slot's claimed job to its end, on the worker thread or the caller's
+int do_job(tgi_ctx* c, Slot& s) {
+  const int rc = run_job(c, s);
+  turn_pass(c, s);
+  std::lock_guard<std::mutex> lk(s.mu);
+  s.rc = rc;
+  s.done = true;
+  return rc;
 }
 
 void worker_main(tgi_ctx* c, Slot* s) {
   cudaSetDevice(c->device);
   for (;;) {
-    JobKind job;
     {
       std::unique_lock<std::mutex> lk(s->mu);
-      s->cv.wait(lk, [&] { return s->job != JOB_NONE; });
-      job = s->job;
+      s->cv.wait(lk, [&] { return s->worker_state != Slot::IDLE; });
+      if (s->worker_state == Slot::QUIT) return;
+      s->worker_state = Slot::IDLE;
     }
-    if (job == JOB_QUIT) return;
-    const int rc = run_job(c, *s, job);
-    turn_pass(c, *s);
-    {
-      std::lock_guard<std::mutex> lk(s->mu);
-      s->rc = rc;
-      s->job = JOB_NONE;
-      s->done = true;
-    }
+    do_job(c, *s);
     s->cv.notify_all();
   }
 }
@@ -1570,23 +1559,38 @@ bool run_flags_ok(tgi_ctx* c, uint32_t flags) {
   return true;
 }
 
-int post_job(tgi_ctx* c, int slot, JobKind kind, const tgi_tg_batch* in, uint32_t flags, const tgi_yt_batch* in_yt = nullptr,
-             const tgi_gm_batch* in_gm = nullptr) {
-  if (!c) return TGI_E_ARG;
-  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "bad slot %d", slot); return TGI_E_ARG; }
-  if (!run_flags_ok(c, flags)) return TGI_E_ARG;
-  Slot& s = c->slots[slot];
+// Claims slot s for job j, all under s.mu: the run flags, the busy check, the resident check, the job, its frontier
+// ticket (frontier phases enter the dedup set in claim order), and the end of the slot's last result.  A job that
+// uploads also ends the slot's resident batch: only a successful upload sets it again (run_job).
+int claim_job(tgi_ctx* c, Slot& s, const Job& j) {
+  if (!run_flags_ok(c, j.flags)) return TGI_E_ARG;
   std::lock_guard<std::mutex> lk(s.mu);
-  if (s.busy) { set_err(c, "slot %d is busy (wait/release it first)", slot); return TGI_E_STATE; }
-  if ((kind == JOB_TG_RESIDENT || kind == JOB_YT_RESIDENT) && !s.resident) { set_err(c, "slot %d holds no resident batch", slot); return TGI_E_STATE; }
+  if (s.busy) { set_err(c, "slot %d is busy (wait/release it first)", s.idx); return TGI_E_STATE; }
+  if (!(j.stages & JOB_UPLOAD) && s.resident != j.kind) { set_err(c, "slot %d holds no resident batch of this kind", s.idx); return TGI_E_STATE; }
   s.busy = true;
   s.done = false;
-  s.in_tg = in;
-  s.in_yt = in_yt;
-  s.in_gm = in_gm;
-  s.run_flags = flags;
-  take_ticket(c, s, kind, flags);
-  s.job = kind;
+  s.job = j;
+  s.last = LastResult{};
+  if (j.stages & JOB_UPLOAD) s.resident = REC_NONE;
+  if ((j.stages & JOB_RUN) && (j.flags & TGI_RUN_FRONTIER)) {
+    std::lock_guard<std::mutex> g(c->tk_mu);
+    s.ticket = c->tk_next++;
+    s.has_ticket = true;
+  }
+  return TGI_OK;
+}
+
+// tgi_*_submit: the slot's worker thread runs the job, tgi_*_wait collects it
+int submit(tgi_ctx* c, int slot, const Job& j) {
+  if (!c) return TGI_E_ARG;
+  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "bad slot %d", slot); return TGI_E_ARG; }
+  Slot& s = c->slots[slot];
+  const int rc = claim_job(c, s, j);
+  if (rc != TGI_OK) return rc;
+  {
+    std::lock_guard<std::mutex> lk(s.mu);
+    s.worker_state = Slot::QUEUED;
+  }
   s.cv.notify_all();
   return TGI_OK;
 }
@@ -1604,33 +1608,12 @@ int wait_job(tgi_ctx* c, int slot, tgi_result* out) {
   return rc;
 }
 
-// Blocking entry points run the job on the CALLER's thread (the slot is claimed exclusively): two condition-variable
-// hand-offs per call are most of what a page-sized batch costs besides the launches themselves.
-int run_inline(tgi_ctx* c, int slot, JobKind kind, const tgi_tg_batch* in_tg, const tgi_yt_batch* in_yt, const tgi_gm_batch* in_gm,
-               uint32_t flags, tgi_result* out) {
-  if (!run_flags_ok(c, flags)) return TGI_E_ARG;
-  Slot& s = c->slots[slot];
-  {
-    std::lock_guard<std::mutex> lk(s.mu);
-    if (s.busy) { set_err(c, "slot %d is busy", slot); return TGI_E_STATE; }
-    s.busy = true;
-    s.done = false;
-    s.in_tg = in_tg;
-    s.in_yt = in_yt;
-    s.in_gm = in_gm;
-    s.run_flags = flags;
-  }
-  take_ticket(c, s, kind, flags);
-  cudaSetDevice(c->device);
-  const int rc = run_job(c, s, kind);
-  turn_pass(c, s);
-  {
-    std::lock_guard<std::mutex> lk(s.mu);
-    s.rc = rc;
-    s.done = true;
-    if (rc != TGI_OK) s.busy = false;
-  }
-  if (rc == TGI_OK && out) *out = s.res;
+// tgi_*_upload and tgi_*_run_resident: submit and wait.  The slot stays claimed only by a job that leaves a result.
+int submit_wait(tgi_ctx* c, int slot, const Job& j, tgi_result* out) {
+  int rc = submit(c, slot, j);
+  if (rc != TGI_OK) return rc;
+  rc = wait_job(c, slot, out);
+  if (rc != TGI_OK || !(j.stages & JOB_RUN)) tgi_result_release(c, slot);
   return rc;
 }
 
@@ -1644,6 +1627,47 @@ int claim_slot(tgi_ctx* c) {
     }
     c->alloc_cv.wait(lk);
   }
+}
+
+// Blocking calls run the job on the CALLER's thread in a free slot (claimed exclusively): two condition-variable
+// hand-offs per call are most of what a page-sized batch costs besides the launches themselves.  The result stays
+// valid until tgi_result_release(ctx, out->slot); a failed call releases the slot itself.
+int run_blocking(tgi_ctx* c, const Job& j, tgi_result* out) {
+  if (!c) return TGI_E_ARG;
+  const int slot = claim_slot(c);
+  Slot& s = c->slots[slot];
+  int rc = claim_job(c, s, j);
+  if (rc == TGI_OK) {
+    cudaSetDevice(c->device);
+    rc = do_job(c, s);
+  }
+  if (rc != TGI_OK) tgi_result_release(c, slot);
+  else if (out) *out = s.res;
+  return rc;
+}
+
+// a job is in flight on slot s: claimed and not finished (the caller holds s.mu)
+bool in_flight(const Slot& s) { return s.busy && !s.done; }
+
+// the first slot with a job in flight, or -1
+int slot_in_flight(tgi_ctx* c) {
+  for (int i = 0; i < TGI_SLOTS; i++) {
+    std::lock_guard<std::mutex> lk(c->slots[i].mu);
+    if (in_flight(c->slots[i])) return i;
+  }
+  return -1;
+}
+
+// The readers' view of slot `slot`: its last result.  TGI_E_ARG for a bad slot; TGI_E_STATE while a job is in flight on
+// it or when it holds no result (nothing has run there, or its last job failed or only uploaded).
+int slot_result(tgi_ctx* c, int slot, const char* who, LastResult* r) {
+  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
+  Slot& s = c->slots[slot];
+  std::lock_guard<std::mutex> lk(s.mu);
+  if (in_flight(s)) { set_err(c, "%s: slot %d is in flight", who, slot); return TGI_E_STATE; }
+  if (s.last.kind == REC_NONE) { set_err(c, "%s: slot %d holds no result", who, slot); return TGI_E_STATE; }
+  *r = s.last;
+  return TGI_OK;
 }
 
 }  // namespace
@@ -1715,8 +1739,8 @@ void tgi_destroy(tgi_ctx* c) {
     if (s.worker.joinable()) {
       {
         std::unique_lock<std::mutex> lk(s.mu);
-        s.cv.wait(lk, [&] { return s.job == JOB_NONE; });
-        s.job = JOB_QUIT;
+        s.cv.wait(lk, [&] { return s.worker_state == Slot::IDLE; });
+        s.worker_state = Slot::QUIT;
       }
       s.cv.notify_all();
       s.worker.join();
@@ -1746,10 +1770,7 @@ void tgi_get_stats(tgi_ctx* c, tgi_stats* out) {
 int tgi_set_clock(tgi_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec, int32_t capture_nsec) {
   if (!c) return TGI_E_ARG;
   cudaSetDevice(c->device);
-  for (int i = 0; i < TGI_SLOTS; i++) {
-    std::lock_guard<std::mutex> lk(c->slots[i].mu);
-    if (c->slots[i].busy && !c->slots[i].done) { set_err(c, "tgi_set_clock while slot %d is in flight", i); return TGI_E_STATE; }
-  }
+  if (const int i = slot_in_flight(c); i >= 0) { set_err(c, "tgi_set_clock while slot %d is in flight", i); return TGI_E_STATE; }
   std::lock_guard<std::mutex> g(c->cfg_mu);
   c->cfg.created_at_sec = created_at_sec;
   c->cfg.created_at_nsec = created_at_nsec;
@@ -1759,7 +1780,7 @@ int tgi_set_clock(tgi_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, i
 }
 
 int tgi_telegram_submit(tgi_ctx* c, int slot, const tgi_tg_batch* in, uint32_t run_flags) {
-  return post_job(c, slot, JOB_TG, in, run_flags);
+  return submit(c, slot, {REC_TG, JOB_UPLOAD | JOB_RUN, in, run_flags});
 }
 int tgi_telegram_wait(tgi_ctx* c, int slot, tgi_result* out) { return wait_job(c, slot, out); }
 
@@ -1778,64 +1799,49 @@ void tgi_result_release(tgi_ctx* c, int slot) {
 }
 
 int tgi_telegram_batch(tgi_ctx* c, const tgi_tg_batch* in, uint32_t run_flags, tgi_result* out) {
-  if (!c) return TGI_E_ARG;
-  int slot = claim_slot(c);
-  int rc = run_inline(c, slot, JOB_TG, in, nullptr, nullptr, run_flags, out);
-  if (rc != TGI_OK) {
-    tgi_result_release(c, slot);
-    return rc;
-  }
-  return TGI_OK;  // result stays valid until tgi_result_release(ctx, out->slot)
+  return run_blocking(c, {REC_TG, JOB_UPLOAD | JOB_RUN, in, run_flags}, out);
 }
 
 int tgi_telegram_upload(tgi_ctx* c, int slot, const tgi_tg_batch* in) {
-  int rc = post_job(c, slot, JOB_TG_UPLOAD, in, 0);
-  if (rc) return rc;
-  rc = wait_job(c, slot, nullptr);
-  tgi_result_release(c, slot);
-  return rc;
+  return submit_wait(c, slot, {REC_TG, JOB_UPLOAD, in, 0}, nullptr);
 }
 int tgi_telegram_run_resident(tgi_ctx* c, int slot, uint32_t run_flags, tgi_result* out) {
-  int rc = post_job(c, slot, JOB_TG_RESIDENT, nullptr, run_flags);
-  if (rc) return rc;
-  rc = wait_job(c, slot, out);
-  if (rc != TGI_OK) tgi_result_release(c, slot);
-  return rc;
+  return submit_wait(c, slot, {REC_TG, JOB_RUN, nullptr, run_flags}, out);
 }
 
 int tgi_result_read_jsonl(tgi_ctx* c, int slot, uint64_t off, uint64_t len, uint8_t* dst) {
-  if (!c || slot < 0 || slot >= TGI_SLOTS || !dst) return TGI_E_ARG;
+  if (!c || !dst) return TGI_E_ARG;
+  LastResult r;
+  const int rc = slot_result(c, slot, "read_jsonl", &r);
+  if (rc != TGI_OK) return rc;
   cudaSetDevice(c->device);
-  Slot& s = c->slots[slot];
-  if (off + len > s.dev_jsonl_len) { set_err(c, "read_jsonl out of range"); return TGI_E_ARG; }
-  CK(cudaMemcpy(dst, s.dev_jsonl + off, len, cudaMemcpyDeviceToHost));
+  if (off + len > r.jsonl_len) { set_err(c, "read_jsonl out of range"); return TGI_E_ARG; }
+  CK(cudaMemcpy(dst, r.dev.jsonl + off, len, cudaMemcpyDeviceToHost));
   return TGI_OK;
 }
 
 int tgi_result_read_rows(tgi_ctx* c, int slot, int which, uint64_t first, uint64_t count, void* dst) {
-  if (!c || slot < 0 || slot >= TGI_SLOTS || !dst) return TGI_E_ARG;
+  if (!c || !dst) return TGI_E_ARG;
+  LastResult r;
+  const int rc = slot_result(c, slot, "read_rows", &r);
+  if (rc != TGI_OK) return rc;
   cudaSetDevice(c->device);
-  Slot& s = c->slots[slot];
   const void* base = nullptr;
   uint64_t rows = 0, size = 0;
-  if (which == TGI_ROWS_STATUS) base = s.dev_status, rows = s.last_n, size = 1;
-  if (which == TGI_ROWS_LINK_OFF) base = s.dev_link_off, rows = s.last_n + 1, size = 4;
-  if (which == TGI_ROWS_LINKS) base = s.dev_links, rows = s.dev_n_links, size = sizeof(tgi_link);
+  if (which == TGI_ROWS_STATUS) base = r.dev.status, rows = r.n, size = 1;
+  if (which == TGI_ROWS_LINK_OFF) base = r.dev.link_off, rows = r.n + 1, size = 4;
+  if (which == TGI_ROWS_LINKS) base = r.dev.links, rows = r.n_links, size = sizeof(tgi_link);
   if (!base || first > rows || count > rows - first) { set_err(c, "read_rows: no such rows in the slot's last result"); return TGI_E_ARG; }
   CK(cudaMemcpy(dst, (const uint8_t*)base + first * size, count * size, cudaMemcpyDeviceToHost));
   return TGI_OK;
 }
 
 int tgi_youtube_submit(tgi_ctx* c, int slot, const tgi_yt_batch* in, uint32_t run_flags) {
-  return post_job(c, slot, JOB_YT, nullptr, run_flags, in);
+  return submit(c, slot, {REC_YT, JOB_UPLOAD | JOB_RUN, in, run_flags});
 }
 int tgi_youtube_wait(tgi_ctx* c, int slot, tgi_result* out) { return wait_job(c, slot, out); }
 int tgi_youtube_batch(tgi_ctx* c, const tgi_yt_batch* in, uint32_t run_flags, tgi_result* out) {
-  if (!c) return TGI_E_ARG;
-  int slot = claim_slot(c);
-  int rc = run_inline(c, slot, JOB_YT, nullptr, in, nullptr, run_flags, out);
-  if (rc != TGI_OK) tgi_result_release(c, slot);
-  return rc;
+  return run_blocking(c, {REC_YT, JOB_UPLOAD | JOB_RUN, in, run_flags}, out);
 }
 int tgi_key_join(tgi_ctx* c, const int64_t* a_keys, uint64_t na, const int64_t* b_keys, uint64_t nb, int64_t* b_index) {
   if (!c || (na && !a_keys) || (nb && (!b_keys || !b_index))) return TGI_E_ARG;
@@ -1936,25 +1942,14 @@ int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uin
 }
 
 int tgi_generic_batch(tgi_ctx* c, const tgi_gm_batch* in, uint32_t run_flags, tgi_result* out) {
-  if (!c) return TGI_E_ARG;
-  int slot = claim_slot(c);
-  int rc = run_inline(c, slot, JOB_GM, nullptr, nullptr, in, run_flags, out);
-  if (rc != TGI_OK) tgi_result_release(c, slot);
-  return rc;
+  // generic messages have no links: no frontier phase, no frontier turn
+  return run_blocking(c, {REC_GM, JOB_UPLOAD | JOB_RUN, in, run_flags & ~(uint32_t)TGI_RUN_FRONTIER}, out);
 }
 int tgi_youtube_upload(tgi_ctx* c, int slot, const tgi_yt_batch* in) {
-  int rc = post_job(c, slot, JOB_YT_UPLOAD, nullptr, 0, in);
-  if (rc) return rc;
-  rc = wait_job(c, slot, nullptr);
-  tgi_result_release(c, slot);
-  return rc;
+  return submit_wait(c, slot, {REC_YT, JOB_UPLOAD, in, 0}, nullptr);
 }
 int tgi_youtube_run_resident(tgi_ctx* c, int slot, uint32_t run_flags, tgi_result* out) {
-  int rc = post_job(c, slot, JOB_YT_RESIDENT, nullptr, run_flags);
-  if (rc) return rc;
-  rc = wait_job(c, slot, out);
-  if (rc != TGI_OK) tgi_result_release(c, slot);
-  return rc;
+  return submit_wait(c, slot, {REC_YT, JOB_RUN, nullptr, run_flags}, out);
 }
 
 // ---- frontier host API ------------------------------------------------------------------------------
@@ -2142,10 +2137,7 @@ int tgi_set_now(tgi_ctx* c, int64_t now_sec) {
 int tgi_set_growth(tgi_ctx* c, uint64_t max_keys) {
   if (!c) return TGI_E_ARG;
   if (max_keys >= (1ull << 40)) { set_err(c, "tgi_set_growth: a set holds fewer than 2^40 keys"); return TGI_E_ARG; }
-  for (int i = 0; i < TGI_SLOTS; i++) {
-    std::lock_guard<std::mutex> lk(c->slots[i].mu);
-    if (c->slots[i].busy && !c->slots[i].done) { set_err(c, "tgi_set_growth while slot %d is in flight", i); return TGI_E_STATE; }
-  }
+  if (const int i = slot_in_flight(c); i >= 0) { set_err(c, "tgi_set_growth while slot %d is in flight", i); return TGI_E_STATE; }
   std::lock_guard<std::mutex> g(c->fr_mu);
   c->grow_max = max_keys;
   return TGI_OK;
@@ -2167,13 +2159,17 @@ int tgi_set_info(tgi_ctx* c, int which, tgi_set_info_t* out) {
   return TGI_OK;
 }
 int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uint64_t cap, uint64_t* n) {
-  if (!c || !n || slot < 0 || slot >= TGI_SLOTS || (cap && !rows)) return TGI_E_ARG;
+  if (!c || !n || (cap && !rows)) return TGI_E_ARG;
+  *n = 0;
+  LastResult r;
+  const int rc = slot_result(c, slot, "tgi_pending_edges", &r);
+  if (rc != TGI_OK) return rc;
+  if (r.n && !(r.flags & TGI_RUN_FRONTIER)) { set_err(c, "tgi_pending_edges: the slot's last batch ran without TGI_RUN_FRONTIER"); return TGI_E_STATE; }
+  *n = r.n_new;
+  const uint64_t m = r.n_new < cap ? r.n_new : cap;
+  if (!m) return TGI_OK;
   cudaSetDevice(c->device);
   Slot& s = c->slots[slot];
-  if (!s.last_frontier) { *n = 0; if (s.last_n == 0) return TGI_OK; set_err(c, "tgi_pending_edges: the slot's last batch ran without TGI_RUN_FRONTIER"); return TGI_E_STATE; }
-  *n = s.last_new;
-  const uint64_t m = s.last_new < cap ? s.last_new : cap;
-  if (!m) return TGI_OK;
   std::lock_guard<std::mutex> g(c->fr_mu);
   cudaStream_t st = s.stream;
   if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
@@ -2181,11 +2177,11 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
   CK(drows.ensure(m * sizeof(tgi_edge)));
   const ExclusionDev x = exclusion(c, now_sec);
   // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
-  const uint32_t* chan = s.last_yt ? &s.yt.recs->chan_idx : &s.tg.recs->chan_idx;
-  const uint32_t stride = s.last_yt ? (uint32_t)sizeof(tgi_yt_rec) : (uint32_t)sizeof(tgi_tg_rec);
-  edges_emit_kernel<<<(unsigned)((s.last_n + 255) / 256), 256, 0, st>>>(s.last_n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
-                                                                    s.d_arena.as<tgi_link>(), chan, stride, s.fs.new_off.as<uint64_t>(), x,
-                                                                    drows.as<tgi_edge>(), m);
+  const uint32_t* chan = r.kind == REC_YT ? &s.yt.recs->chan_idx : &s.tg.recs->chan_idx;
+  const uint32_t stride = r.kind == REC_YT ? (uint32_t)sizeof(tgi_yt_rec) : (uint32_t)sizeof(tgi_tg_rec);
+  edges_emit_kernel<<<(unsigned)((r.n + 255) / 256), 256, 0, st>>>(r.n, s.d_link_start.as<uint32_t>(), s.d_link_count.as<uint32_t>(),
+                                                                  s.d_arena.as<tgi_link>(), chan, stride, s.fs.new_off.as<uint64_t>(), x,
+                                                                  drows.as<tgi_edge>(), m);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(rows, drows.p, m * sizeof(tgi_edge), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -2194,18 +2190,17 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
 
 // Dapr sink payloads (dapr.cuh): size, two scans, one synchronise for the totals, write, the four copies, one synchronise.
 int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t prefix_len, tgi_dapr_payloads_t* out) {
-  if (!c || !out || !path_prefix || slot < 0 || slot >= TGI_SLOTS) return TGI_E_ARG;
+  if (!c || !out || !path_prefix) return TGI_E_ARG;
+  LastResult r;
+  int rc = slot_result(c, slot, "tgi_dapr_payloads", &r);
+  if (rc != TGI_OK) return rc;
+  if (r.kind == REC_GM) { set_err(c, "tgi_dapr_payloads: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
+  if (!r.dev.line_off) { set_err(c, "tgi_dapr_payloads: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
   cudaSetDevice(c->device);
   Slot& s = c->slots[slot];
-  {
-    std::lock_guard<std::mutex> lk(s.mu);
-    if (s.busy && !s.done) { set_err(c, "tgi_dapr_payloads: slot %d is in flight", slot); return TGI_E_STATE; }
-  }
-  if (s.last_gm) { set_err(c, "tgi_dapr_payloads: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
-  if (!s.dev_line_off) { set_err(c, "tgi_dapr_payloads: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
   DaprBufs& z = s.dapr;
   cudaStream_t st = s.stream;
-  const uint64_t n = s.last_n;
+  const uint64_t n = r.n;
   memset(out, 0, sizeof *out);
   out->n = n;
   CK(z.h_off.ensure(2 * (n + 1) * 8));
@@ -2218,12 +2213,12 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   }
   DaprSrc src{};
   src.n = n;
-  src.status = s.dev_status;
-  src.line_off = s.dev_line_off;
-  src.jsonl = s.dev_jsonl;
-  src.yt = s.last_yt;
+  src.status = r.dev.status;
+  src.line_off = r.dev.line_off;
+  src.jsonl = r.dev.jsonl;
+  src.yt = r.kind == REC_YT;
   // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
-  if (s.last_yt) {
+  if (src.yt) {
     src.yt_recs = s.yt.recs, src.yt_chans = s.yt.chans, src.strs = s.yt.strs, src.chan_strs = s.yt.chan_strs;
   } else {
     src.tg_recs = s.tg.recs, src.tg_chans = s.tg.chans, src.strs = s.tg.strs, src.chan_strs = s.tg.chan_strs;
@@ -2251,7 +2246,7 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   const unsigned gs = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
   dapr_size_kernel<<<gs, 256, 0, st>>>(src, o);
   launches++;
-  int rc = launch_scan(c, s, o.data_len, n, (uint64_t*)o.data_off, dsc, launches);
+  rc = launch_scan(c, s, o.data_len, n, (uint64_t*)o.data_off, dsc, launches);
   if (rc) return rc;
   rc = launch_scan(c, s, o.path_len, n, (uint64_t*)o.path_off, dsc + 1, launches);
   if (rc) return rc;

@@ -446,9 +446,10 @@ int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uin
  * before any binding call (daprstate.go:1141-1144).
  * Call between tgi_*_wait / tgi_*_batch and tgi_result_release (like tgi_pending_edges); works after TGI_RUN_NO_D2H and
  * TGI_RUN_JSONL_DEVICE.  Outputs live in library-owned pinned memory and stay valid until the release or the next call
- * on that slot.  TGI_E_STATE: the last result is a tgi_generic_batch one (its posts go to SavePost,
- * crawler/common/runner.go:55, which has no Dapr implementation) or ran without TGI_RUN_JSONL; TGI_E_ARG: bad slot or
- * NULL prefix / out; TGI_E_NOMEM: allocation failed (the batch result stays valid).                                  */
+ * on that slot.  TGI_E_STATE: the slot holds no result (see tgi_result_read_jsonl), the last result is a
+ * tgi_generic_batch one (its posts go to SavePost, crawler/common/runner.go:55, which has no Dapr implementation) or
+ * ran without TGI_RUN_JSONL; TGI_E_ARG: bad slot or NULL prefix / out; TGI_E_NOMEM: allocation failed (the batch
+ * result stays valid).                                                                                                */
 typedef struct tgi_dapr_payloads_t {
   uint64_t n;
   const uint8_t* data;  uint64_t data_len;  const uint64_t* data_off;  /* [n+1] base64 of record i's line          */
@@ -474,15 +475,22 @@ int tgi_generic_batch(tgi_ctx* ctx, const tgi_gm_batch* in, uint32_t run_flags, 
 void tgi_result_release(tgi_ctx* ctx, int slot);
 
 /* Device-resident variant used for kernel-only measurement and by pipelines that already hold the
- * packed batch in HBM: upload once, run many times.  Same kernels as tgi_telegram_batch.         */
+ * packed batch in HBM: upload once, run many times.  Same kernels as tgi_telegram_batch.
+ * A slot's resident batch is the batch of its last successful upload (tgi_*_upload, tgi_*_submit or tgi_*_batch of
+ * Telegram or YouTube); tgi_telegram_run_resident / tgi_youtube_run_resident return TGI_E_STATE unless it is of their
+ * kind.  The upload call returns once the copy has landed.                                                           */
 int tgi_telegram_upload(tgi_ctx* ctx, int slot, const tgi_tg_batch* in);
 int tgi_telegram_run_resident(tgi_ctx* ctx, int slot, uint32_t run_flags, tgi_result* out);
 int tgi_youtube_upload(tgi_ctx* ctx, int slot, const tgi_yt_batch* in);
 int tgi_youtube_run_resident(tgi_ctx* ctx, int slot, uint32_t run_flags, tgi_result* out);
-/* copy [off, off+len) of the slot's device JSONL to dst (host); for spot checks of huge runs     */
+/* The readers (tgi_result_read_jsonl, tgi_result_read_rows, tgi_pending_edges, tgi_dapr_payloads) read a slot's last
+ * result, which lives from a successful job until the next job is claimed on the slot: after tgi_result_release too,
+ * but not after a failed or upload-only job.  A reader that finds no result, or a job in flight on the slot, returns
+ * TGI_E_STATE.
+ * tgi_result_read_jsonl: copy [off, off+len) of the slot's device JSONL to dst (host); for spot checks of huge runs */
 int tgi_result_read_jsonl(tgi_ctx* ctx, int slot, uint64_t off, uint64_t len, uint8_t* dst);
 /* copy rows [first, first+count) of the slot's last per-record status (uint8), link offsets (uint32, n+1) or link rows
- * (tgi_link) to dst (host): what a TGI_RUN_NO_D2H run left on the device                         */
+ * (tgi_link) to dst (host): what a TGI_RUN_NO_D2H run left on the device; TGI_E_ARG for rows the result does not have */
 enum { TGI_ROWS_STATUS = 0, TGI_ROWS_LINK_OFF = 1, TGI_ROWS_LINKS = 2 };
 int tgi_result_read_rows(tgi_ctx* ctx, int slot, int which, uint64_t first, uint64_t count, void* dst);
 
@@ -553,8 +561,10 @@ int tgi_merge_get_stats(tgi_ctx* ctx, tgi_merge_stats* out);
  *                     TGI_EDGE_PENDING (needs the HTTP check), TGI_EDGE_DUPLICATE (already discovered: validator.go:214-226),
  *                     TGI_EDGE_INVALID_CACHED (validator.go:205-212; only if the batch ran without TGI_RUN_SKIP_INVALID or
  *                     the channel was marked invalid in between).  Call between tgi_*_wait / tgi_*_batch and
- *                     tgi_result_release.  The per-batch constants of a row (batch_id, crawl_id, sequence_id, discovery_time)
- *                     stay with the caller; source_channel = the name of channel row `chan_idx`.                          */
+ *                     tgi_result_release.  0 rows for an empty batch; TGI_E_STATE for a slot that holds no result
+ *                     (see tgi_result_read_jsonl) or a non-empty one that ran without TGI_RUN_FRONTIER.  The per-batch
+ *                     constants of a row (batch_id, crawl_id, sequence_id, discovery_time) stay with the caller;
+ *                     source_channel = the name of channel row `chan_idx`.                                             */
 #define TGI_SET_INVALID 1     /* invalid_channels (state/daprstate.go:3489-3564)                  */
 #define TGI_SET_DISCOVERED 2  /* discovered_channels (state/base.go:522-528)                      */
 #define TGI_INVALID_TTL_SEC (30 * 24 * 3600)
