@@ -153,6 +153,17 @@ class DaprPayloadsC(C.Structure):  # tgi_dapr_payloads_t
                 ("gpu_launches", C.c_uint32)]
 
 
+class CombinedBlobC(C.Structure):  # tgi_combined_blob
+    _fields_ = [("data_off", C.c_uint64), ("data_len", C.c_uint64), ("path_off", C.c_uint64), ("path_len", C.c_uint64),
+                ("n_lines", C.c_uint64), ("raw_bytes", C.c_uint64), ("unix_nano", C.c_int64)]
+
+
+class CombinedC(C.Structure):  # tgi_combined_t
+    _fields_ = [("n_blobs", C.c_uint64), ("blobs", C.POINTER(CombinedBlobC)), ("data", C.c_void_p), ("path", C.c_void_p),
+                ("n_dropped", C.c_uint64), ("dropped", C.c_void_p), ("open_lines", C.c_uint64), ("open_bytes", C.c_uint64),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 class StatsC(C.Structure):
     _fields_ = [("records", C.c_uint64), ("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64),
                 ("links", C.c_uint64), ("frontier_size", C.c_uint64), ("launches", C.c_uint64),

@@ -21,6 +21,7 @@
 
 #include "kernels.cuh"
 #include "dapr.cuh"
+#include "combine.cuh"
 #include "tg_page.cuh"
 #include "yt_page.cuh"
 
@@ -111,6 +112,7 @@ struct LastResult {
   uint32_t flags = 0;  // the run flags that shaped it
   uint64_t n_new = 0, n_links = 0, jsonl_len = 0;
   ResultArrays dev{};  // its arrays on the device; line_off / link_off / links are null when the run did not make them
+  const uint64_t* host_line_off = nullptr;  // its line offsets in pinned host memory (null: TGI_RUN_NO_D2H or no lines)
 };
 
 // one batch's frontier phases: the batch hash table, per-link state, per-record NEW counts and their offsets
@@ -151,6 +153,25 @@ struct NcclApi {
 struct DaprBufs {
   DevBuf prefix, lens, off, data, path, sc;
   HostBuf h_off, h_data, h_path, h_sc;
+};
+
+// tgi_combine_*: the combiner's settings, its open group (encoded on the device, 0-2 bytes pending) and its scratch
+struct Combiner {
+  std::mutex mu;
+  bool open = false;
+  uint64_t trigger = 0, hard_cap = 0;
+  std::string prefix;
+  uint64_t open_lines = 0, open_bytes = 0;  // the open group: its posts and raw bytes; enc holds open_bytes / 3 words
+  DevBuf enc;        // the open blob's base64, 4*ceil(hard_cap/3) bytes
+  DevBuf pend;       // two 32-byte halves: the pending bytes (open_bytes % 3) in half `cur`, the next call's in the other
+  int cur = 0;
+  int64_t last_ns = 0;
+  bool any_ns = false;
+  cudaStream_t stream = nullptr;  // tgi_combine_flush's work (the adds run on their slot's stream)
+  cudaEvent_t ev = nullptr, t0 = nullptr, t1 = nullptr;  // ev: the last call's work; t0 / t1: its device time
+  bool ev_valid = false;
+  DevBuf out, tables, drops, counts;  // closed blobs past the first, task / segment tables, dropped lines, posts per group
+  HostBuf h_blobs, h_data, h_path, h_tables, h_drops, h_counts, h_line_off;
 };
 
 struct Slot {
@@ -222,6 +243,7 @@ struct tgi_ctx {
   std::condition_variable tk_cv;
   uint64_t tk_next = 0, tk_serving = 0;
   InsertScratch ins;  // scratch of tgi_frontier_insert* / tgi_set_add / the merge (under fr_mu)
+  Combiner cb;        // tgi_combine_*
   // multi-GPU merge: communicator (this rank's partition is sets[TGI_SET_OWNED])
   NcclApi* nccl = nullptr;
   ncclComm_t comm = nullptr;
@@ -855,7 +877,8 @@ void fill_result(tgi_ctx* c, Slot& s, RecKind kind, uint64_t n, uint32_t flags, 
   }
   s.last = LastResult{kind, n, flags, out->n_new, out->n_links, out->jsonl_len,
                       {dev.status, want_json ? dev.line_off : nullptr, dev.jsonl, want_links ? dev.link_off : nullptr,
-                       want_links ? dev.links : nullptr}};
+                       want_links ? dev.links : nullptr},
+                      host && want_json ? host->line_off : nullptr};
   std::lock_guard<std::mutex> g(c->st_mu);
   c->stats.records += n;
   c->stats.bytes_in += s.in_bytes;
@@ -1670,6 +1693,84 @@ int slot_result(tgi_ctx* c, int slot, const char* who, LastResult* r) {
   return TGI_OK;
 }
 
+// Chunker.processBatches (chunk/main.go:292-345) over lines [0, n) of one result, continuing a group that holds open_in
+// bytes of earlier results; drops are the sorted indices of the lines longer than hard_cap.  Every group the rule closes
+// goes to emit(begin, end) (false: stop with TGI_E_CAPACITY): lines [begin, end) minus the empty and dropped ones, begin
+// 0 for the group carried in.  The group left open holds *open_out bytes; its first line of this result is *open_begin.
+// K(i), the kept bytes before line i, is line_off[i] minus the dropped bytes before i: monotone, so every boundary is a
+// binary search and the walk costs O(groups * log n * log drops), not O(n).
+template <class Emit>
+int plan_groups(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t open_in,
+                const std::vector<uint64_t>& drops, Emit emit, uint64_t* open_out, uint64_t* open_begin) {
+  std::vector<uint64_t> dbytes(drops.size() + 1, 0);
+  for (size_t k = 0; k < drops.size(); k++) dbytes[k + 1] = dbytes[k] + (line_off[drops[k] + 1] - line_off[drops[k]]);
+  auto K = [&](uint64_t i) {
+    const size_t k = std::lower_bound(drops.begin(), drops.end(), i) - drops.begin();
+    return line_off[i] - line_off[0] - dbytes[k];
+  };
+  // the first m in (p, n] with K(m) - base > thr, or n + 1
+  auto first_over = [&](uint64_t p, uint64_t base, uint64_t thr) {
+    if (K(n) - base <= thr) return n + 1;
+    uint64_t lo = p + 1, hi = n;
+    while (lo < hi) {
+      const uint64_t mid = lo + (hi - lo) / 2;
+      if (K(mid) - base > thr) hi = mid;
+      else lo = mid + 1;
+    }
+    return lo;
+  };
+  uint64_t p = 0, size = open_in, begin = 0;
+  while (p < n) {
+    const uint64_t base = K(p);
+    // line mc - 1 would push the group over hard_cap (:324-327); line mt - 1 makes it reach trigger (:334-337)
+    const uint64_t mc = first_over(p, base, hard_cap - size);
+    const uint64_t mt = first_over(p, base, (trigger > size ? trigger - size : 1) - 1);
+    if (!size && K(n) > base) begin = first_over(p, base, 0) - 1;  // the group's first line
+    if (mc > n && mt > n) {  // every line left joins the open group
+      size += K(n) - base;
+      break;
+    }
+    if (mc <= mt) {  // close before line mc - 1, which starts the next group
+      if (!emit(begin, mc - 1)) return TGI_E_CAPACITY;
+      p = mc - 1;
+    } else {         // close after line mt - 1
+      if (!emit(begin, mt)) return TGI_E_CAPACITY;
+      p = mt;
+    }
+    size = 0;
+  }
+  *open_out = size;
+  *open_begin = size ? begin : n;
+  return TGI_OK;
+}
+
+// tgi_plan_chunks(_carry): the dropped lines by a scan, then plan_groups; `close` closes the group left open (:339-343)
+int plan_host(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t open_in, uint64_t* groups,
+              uint64_t max_groups, uint64_t* n_groups, uint8_t* dropped, uint64_t* open_out, bool close) {
+  std::vector<uint64_t> drops;
+  for (uint64_t i = 0; i < n; i++) {
+    const bool d = line_off[i + 1] - line_off[i] > hard_cap;
+    if (dropped) dropped[i] = d;
+    if (d) drops.push_back(i);
+  }
+  uint64_t g = 0, open_begin = 0;
+  auto emit = [&](uint64_t a, uint64_t b) {
+    if (g >= max_groups) return false;
+    groups[2 * g] = a;
+    groups[2 * g + 1] = b;
+    g++;
+    return true;
+  };
+  const int rc = plan_groups(line_off, n, trigger, hard_cap, open_in, drops, emit, open_out, &open_begin);
+  if (rc) return rc;
+  if (close && *open_out) {
+    if (!emit(open_begin, n)) return TGI_E_CAPACITY;
+    *open_out = 0;
+  }
+  *n_groups = g;
+  return TGI_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1752,6 +1853,11 @@ void tgi_destroy(tgi_ctx* c) {
   for (auto& f : c->stg_free) cudaFreeHost(f.second);
   for (auto& f : c->stg_live) cudaFreeHost(f.first);
   if (c->fr_event) cudaEventDestroy(c->fr_event);
+  if (c->cb.stream) {
+    cudaStreamSynchronize(c->cb.stream);
+    cudaStreamDestroy(c->cb.stream);
+  }
+  for (cudaEvent_t e : {c->cb.ev, c->cb.t0, c->cb.t1}) if (e) cudaEventDestroy(e);
   delete c;  // the device and pinned buffers free themselves
 }
 
@@ -1872,38 +1978,16 @@ int tgi_key_join(tgi_ctx* c, const int64_t* a_keys, uint64_t na, const int64_t* 
 int tgi_plan_chunks(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t* groups,
                     uint64_t max_groups, uint64_t* n_groups, uint8_t* dropped) {
   if (!line_off || !groups || !n_groups) return TGI_E_ARG;
-  uint64_t g = 0, size = 0, files = 0, begin = 0;
-  auto flush = [&](uint64_t end) -> bool {  // chunk/main.go:298-311; end = one past the last line of the group
-    if (!files) return true;
-    if (g >= max_groups) return false;
-    groups[2 * g] = begin;
-    groups[2 * g + 1] = end;
-    g++;
-    size = 0;
-    files = 0;
-    return true;
-  };
-  for (uint64_t i = 0; i < n; i++) {
-    const uint64_t len = line_off[i + 1] - line_off[i];
-    if (dropped) dropped[i] = 0;
-    if (len == 0) continue;  // no line for this record: no file
-    if (len > hard_cap) {    // :316-322
-      if (dropped) dropped[i] = 1;
-      continue;
-    }
-    if (size > 0 && size + len > hard_cap) {  // :324-327
-      if (!flush(i)) return TGI_E_CAPACITY;
-    }
-    if (!files) begin = i;
-    files++;
-    size += len;
-    if (size >= trigger) {  // :334-337
-      if (!flush(i + 1)) return TGI_E_CAPACITY;
-    }
-  }
-  if (!flush(n)) return TGI_E_CAPACITY;  // :339-343
-  *n_groups = g;
-  return TGI_OK;
+  uint64_t open_out = 0;
+  return plan_host(line_off, n, trigger, hard_cap, 0, groups, max_groups, n_groups, dropped, &open_out, true);
+}
+
+int tgi_plan_chunks_carry(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t open_bytes_in,
+                          uint64_t* groups, uint64_t max_groups, uint64_t* n_groups, uint8_t* dropped,
+                          uint64_t* open_bytes_out) {
+  if (!line_off || !n_groups || !open_bytes_out || (max_groups && !groups)) return TGI_E_ARG;
+  if (open_bytes_in > hard_cap || (open_bytes_in && open_bytes_in >= trigger)) return TGI_E_ARG;  // no group rests there
+  return plan_host(line_off, n, trigger, hard_cap, open_bytes_in, groups, max_groups, n_groups, dropped, open_bytes_out, false);
 }
 
 int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uint32_t chan_stride, uint64_t n, tgi_append_run* runs,
@@ -2283,6 +2367,335 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   out->gpu_launches = launches;
   return TGI_OK;
 }
+
+}  // extern "C"
+
+// ---- combine mode (combine.cuh) ---------------------------------------------------------------------------------------
+namespace {
+
+// one launch of combine_encode_kernel being built: its tasks and their segments
+struct CbPlan {
+  std::vector<CbTask> t;
+  std::vector<CbSeg> s;
+  uint64_t units = 0;
+  void add(uint8_t* dst, bool last, const std::vector<CbSeg>& segs) {
+    CbTask k{dst, 0, units, (uint32_t)s.size(), (uint32_t)segs.size(), last ? 1u : 0u};
+    for (const CbSeg& g : segs) k.bytes += g.len;
+    if (!k.bytes) return;
+    s.insert(s.end(), segs.begin(), segs.end());
+    units += cb_units(k);
+    t.push_back(k);
+  }
+};
+
+// the kept lines of [a, b) as segments of the result's JSONL behind stream position pos (a dropped line splits a run)
+void cb_runs(const uint64_t* off, const uint8_t* jsonl, uint64_t a, uint64_t b, const std::vector<uint64_t>& drops,
+             std::vector<CbSeg>& segs, uint64_t& pos) {
+  size_t k = std::lower_bound(drops.begin(), drops.end(), a) - drops.begin();
+  while (a < b) {
+    const bool d = k < drops.size() && drops[k] < b;
+    const uint64_t e = d ? drops[k] : b;
+    if (off[e] > off[a]) {
+      segs.push_back({pos, off[e] - off[a], jsonl + off[a]});
+      pos += off[e] - off[a];
+    }
+    a = d ? e + 1 : b;
+    k++;
+  }
+}
+
+// P's tasks: inline in the launch parameters, or in the device tables dt / ds
+int cb_launch(tgi_ctx* c, cudaStream_t st, const CbPlan& P, const CbTask* dt, const CbSeg* ds, uint8_t* pend_out,
+              uint32_t& launches) {
+  if (!P.units) return TGI_OK;
+  CbLaunch L{};
+  L.n_tasks = (uint32_t)P.t.size();
+  L.units = P.units;
+  L.pend_out = pend_out;
+  if (P.t.size() <= (size_t)CB_INLINE && P.s.size() <= (size_t)CB_INLINE) {
+    std::copy(P.t.begin(), P.t.end(), L.t);
+    std::copy(P.s.begin(), P.s.end(), L.s);
+  } else {
+    L.tasks = dt;
+    L.segs = ds;
+  }
+  const unsigned g = (unsigned)std::min<uint64_t>((P.units + 255) / 256, (uint64_t)c->sms * 16);
+  combine_encode_kernel<<<g, 256, 0, st>>>(L);
+  launches++;
+  CK(cudaGetLastError());
+  return TGI_OK;
+}
+
+std::string cb_path(const Combiner& z, int64_t ns) {
+  return z.prefix + "combined-posts/combined_" + std::to_string(ns) + ".jsonl";
+}
+
+// the next blob name: max(unix_nano, previous + 1)
+int64_t cb_next_ns(Combiner& z, int64_t unix_nano) {
+  const int64_t ns = z.any_ns && unix_nano <= z.last_ns ? z.last_ns + 1 : unix_nano;
+  z.last_ns = ns;
+  z.any_ns = true;
+  return ns;
+}
+
+// the paths of out's blobs, once their data is in place
+int cb_finish(tgi_ctx* c, Combiner& z, int64_t unix_nano, tgi_combined_blob* blobs, uint64_t k, tgi_combined_t* out) {
+  std::string paths;
+  for (uint64_t j = 0; j < k; j++) {
+    const std::string p = cb_path(z, cb_next_ns(z, unix_nano));
+    blobs[j].unix_nano = z.last_ns;
+    blobs[j].path_off = paths.size();
+    blobs[j].path_len = p.size();
+    paths += p;
+  }
+  CK(z.h_path.ensure(paths.size() + 1));
+  memcpy(z.h_path.p, paths.data(), paths.size());
+  out->n_blobs = k;
+  out->blobs = blobs;
+  out->data = z.h_data.as<uint8_t>();
+  out->path = z.h_path.as<uint8_t>();
+  return TGI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tgi_combine_open(tgi_ctx* c, uint64_t trigger, uint64_t hard_cap, const char* path_prefix, uint32_t prefix_len) {
+  if (!c || (prefix_len && !path_prefix)) return TGI_E_ARG;
+  Combiner& z = c->cb;
+  std::lock_guard<std::mutex> g(z.mu);
+  if (z.open && z.open_bytes) { set_err(c, "tgi_combine_open: the open group holds lines (tgi_combine_flush first)"); return TGI_E_STATE; }
+  if (hard_cap >= (1ull << 62)) { set_err(c, "tgi_combine_open: hard_cap %llu cannot be allocated", (unsigned long long)hard_cap); return TGI_E_NOMEM; }
+  cudaSetDevice(c->device);
+  if (!z.ev) {
+    CK(cudaStreamCreateWithFlags(&z.stream, cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(&z.ev, cudaEventDisableTiming));
+    CK(cudaEventCreate(&z.t0));
+    CK(cudaEventCreate(&z.t1));
+  }
+  if (z.ev_valid) CK(cudaEventSynchronize(z.ev));
+  z.open = false;
+  for (DevBuf* d : {&z.out, &z.tables, &z.drops, &z.counts}) d->release();  // a new stream starts with no scratch
+  for (HostBuf* h : {&z.h_blobs, &z.h_data, &z.h_path, &z.h_tables, &z.h_drops, &z.h_counts, &z.h_line_off}) h->release();
+  z.enc.release();  // exactly the largest blob: 4*ceil(hard_cap/3), plus the pad every device blob carries
+  const size_t enc = (hard_cap + 2) / 3 * 4 + PAD;
+  CK(cudaMalloc(&z.enc.p, enc));
+  z.enc.cap = enc;
+  CK(z.pend.ensure(64));
+  z.trigger = trigger;
+  z.hard_cap = hard_cap;
+  z.prefix.assign(path_prefix ? path_prefix : "", prefix_len);
+  z.open_lines = z.open_bytes = 0;
+  z.cur = 0;
+  z.open = true;
+  return TGI_OK;
+}
+
+// The fast path (the lines fit in the open group) enqueues one launch.  Otherwise: the dropped lines and, for a
+// TGI_RUN_NO_D2H result, the line offsets are read back; the host plans the groups; launch 1 encodes the blobs that
+// close (the first one behind the open group's encoded bytes) and the open group if none closes, the closed blobs are
+// copied to pinned memory, launch 2 encodes the new open group from the start of the (now copied) open buffer.
+int tgi_combine_add(tgi_ctx* c, int slot, int64_t unix_nano, tgi_combined_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  LastResult r;
+  int rc = slot_result(c, slot, "tgi_combine_add", &r);
+  if (rc != TGI_OK) return rc;
+  if (r.kind == REC_GM) { set_err(c, "tgi_combine_add: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
+  if (!r.dev.line_off) { set_err(c, "tgi_combine_add: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
+  Combiner& z = c->cb;
+  std::lock_guard<std::mutex> g(z.mu);
+  if (!z.open) { set_err(c, "tgi_combine_add: no combiner is open (tgi_combine_open)"); return TGI_E_STATE; }
+  cudaSetDevice(c->device);
+  memset(out, 0, sizeof *out);
+  cudaStream_t st = c->slots[slot].stream;
+  const uint64_t n = r.n, L = r.jsonl_len;
+  uint8_t* pend_in = z.pend.as<uint8_t>() + 32 * z.cur;
+  uint8_t* pend_out = z.pend.as<uint8_t>() + 32 * (1 - z.cur);
+  uint8_t* enc = z.enc.as<uint8_t>();
+  const uint64_t p0 = z.open_bytes % 3;
+  const CbSeg pend{0, p0, pend_in};  // the open blob's pending bytes: its continuation's input starts with them
+  uint32_t launches = 0;
+  if (z.ev_valid) CK(cudaStreamWaitEvent(st, z.ev, 0));
+  if (r.host_line_off && z.open_bytes + L < z.trigger && z.open_bytes + L <= z.hard_cap) {
+    if (L) {
+      const uint64_t* off = r.host_line_off;
+      uint64_t lines = 0;
+      for (uint64_t i = 0; i < n; i++) lines += off[i + 1] != off[i];
+      std::vector<CbSeg> segs;
+      if (p0) segs.push_back(pend);
+      segs.push_back({p0, L, r.dev.jsonl + off[0]});
+      CbPlan P;
+      P.add(enc + z.open_bytes / 3 * 4, false, segs);
+      rc = cb_launch(c, st, P, nullptr, nullptr, pend_out, launches);
+      if (rc) return rc;
+      CK(cudaEventRecord(z.ev, st));
+      z.ev_valid = true;
+      z.open_bytes += L;
+      z.open_lines += lines;
+      z.cur ^= 1;
+    }
+    out->open_lines = z.open_lines;
+    out->open_bytes = z.open_bytes;
+    out->gpu_launches = launches;
+    return TGI_OK;
+  }
+  // 1. the dropped lines (at most L / (hard_cap + 1) of them) and the line offsets on the host
+  const uint64_t max_drops = std::min<uint64_t>(n, L / (z.hard_cap + 1));
+  CK(z.drops.ensure(8 * (1 + max_drops)));
+  CK(z.h_drops.ensure(8 * (1 + max_drops)));
+  uint64_t* d_drops = z.drops.as<uint64_t>();
+  CK(cudaEventRecord(z.t0, st));
+  CK(cudaMemsetAsync(d_drops, 0, 8, st));
+  if (n && max_drops) {
+    const unsigned gd = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
+    combine_drops_kernel<<<gd, 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, d_drops + 1, max_drops, (unsigned long long*)d_drops);
+    launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(z.t1, st));
+  CK(cudaMemcpyAsync(z.h_drops.p, d_drops, 8 * (1 + max_drops), cudaMemcpyDeviceToHost, st));
+  const uint64_t* off = r.host_line_off;
+  if (!off) {
+    CK(z.h_line_off.ensure((n + 1) * 8));
+    CK(cudaMemcpyAsync(z.h_line_off.p, r.dev.line_off, (n + 1) * 8, cudaMemcpyDeviceToHost, st));
+    off = z.h_line_off.as<uint64_t>();
+  }
+  CK(cudaStreamSynchronize(st));
+  float ms0 = 0;
+  cudaEventElapsedTime(&ms0, z.t0, z.t1);
+  uint64_t* hd = z.h_drops.as<uint64_t>();
+  const uint64_t nd = std::min(hd[0], max_drops);
+  std::vector<uint64_t> drops(hd + 1, hd + 1 + nd);
+  std::sort(drops.begin(), drops.end());
+  // 2. the groups (the rule of tgi_plan_chunks)
+  std::vector<uint64_t> ends;
+  uint64_t open_out = 0, open_begin = 0;
+  rc = plan_groups(off, n, z.trigger, z.hard_cap, z.open_bytes, drops,
+                   [&](uint64_t, uint64_t e) { ends.push_back(e); return true; }, &open_out, &open_begin);
+  if (rc) return rc;
+  const uint64_t k = ends.size();
+  // 3. the tasks: closed group 0 continues the open blob in enc, closed groups 1.. go to `out` at 16-byte aligned
+  // offsets, the group left open (index k) continues enc (nothing closed: launch 1) or restarts it (launch 2)
+  std::vector<std::vector<CbSeg>> gsegs(k + 1);
+  std::vector<uint64_t> raw(k + 1), dev_off(k + 1, 0);
+  uint64_t out_bytes = 0;
+  for (uint64_t j = 0; j <= k; j++) {
+    if (!j && p0) gsegs[j].push_back(pend);
+    uint64_t pos = j ? 0 : p0;
+    cb_runs(off, r.dev.jsonl, j ? ends[j - 1] : 0, j < k ? ends[j] : n, drops, gsegs[j], pos);
+    raw[j] = pos + (j ? 0 : z.open_bytes - p0);
+    if (j && j < k) {
+      dev_off[j] = out_bytes;
+      out_bytes += ((raw[j] + 2) / 3 * 4 + 15) & ~15ull;
+    }
+  }
+  CK(z.out.ensure(out_bytes));
+  uint8_t* cont = enc + z.open_bytes / 3 * 4;  // where the open blob continues
+  CbPlan P1, P2;
+  for (uint64_t j = 0; j < k; j++) P1.add(j ? z.out.as<uint8_t>() + dev_off[j] : cont, true, gsegs[j]);
+  if (k) P2.add(enc, false, gsegs[k]);
+  else P1.add(cont, false, gsegs[0]);
+  // tables: ends | P1 tasks | P1 segs | P2 tasks | P2 segs, one copy
+  const size_t tb = 8 * k, t1b = sizeof(CbTask) * P1.t.size(), s1b = sizeof(CbSeg) * P1.s.size(),
+               t2b = sizeof(CbTask) * P2.t.size(), s2b = sizeof(CbSeg) * P2.s.size(), all = tb + t1b + s1b + t2b + s2b;
+  CK(z.tables.ensure(all));
+  CK(z.h_tables.ensure(all));
+  uint8_t* ht = z.h_tables.as<uint8_t>();
+  memcpy(ht, ends.data(), tb);
+  memcpy(ht + tb, P1.t.data(), t1b);
+  memcpy(ht + tb + t1b, P1.s.data(), s1b);
+  memcpy(ht + tb + t1b + s1b, P2.t.data(), t2b);
+  memcpy(ht + tb + t1b + s1b + t2b, P2.s.data(), s2b);
+  uint8_t* dtb = z.tables.as<uint8_t>();
+  if (all) CK(cudaMemcpyAsync(dtb, ht, all, cudaMemcpyHostToDevice, st));
+  CK(z.counts.ensure(8 * (k + 1)));
+  CK(z.h_counts.ensure(8 * (k + 1)));
+  uint64_t data_bytes = 0;
+  for (uint64_t j = 0; j < k; j++) data_bytes += (raw[j] + 2) / 3 * 4;
+  CK(z.h_data.ensure(data_bytes + 1));
+  CK(z.h_blobs.ensure(sizeof(tgi_combined_blob) * (k + 1)));
+  // 4. posts per group, launch 1, the copies of the closed blobs, launch 2
+  CK(cudaEventRecord(z.t0, st));
+  CK(cudaMemsetAsync(z.counts.p, 0, 8 * (k + 1), st));
+  if (n) {
+    const unsigned gc = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
+    combine_count_kernel<<<gc, 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, (const uint64_t*)dtb, (uint32_t)k,
+                                             z.counts.as<unsigned long long>());
+    launches++;
+    CK(cudaGetLastError());
+  }
+  rc = cb_launch(c, st, P1, (const CbTask*)(dtb + tb), (const CbSeg*)(dtb + tb + t1b), pend_out, launches);
+  if (rc) return rc;
+  CK(cudaEventRecord(z.t1, st));
+  tgi_combined_blob* blobs = z.h_blobs.as<tgi_combined_blob>();
+  uint64_t hoff = 0;
+  for (uint64_t j = 0; j < k; j++) {
+    const uint64_t len = (raw[j] + 2) / 3 * 4;
+    const uint8_t* src = j ? z.out.as<uint8_t>() + dev_off[j] : enc;
+    if (len) CK(cudaMemcpyAsync(z.h_data.as<uint8_t>() + hoff, src, len, cudaMemcpyDeviceToHost, st));
+    blobs[j] = tgi_combined_blob{hoff, len, 0, 0, 0, raw[j], 0};
+    hoff += len;
+  }
+  rc = cb_launch(c, st, P2, (const CbTask*)(dtb + tb + t1b + s1b), (const CbSeg*)(dtb + tb + t1b + s1b + t2b), pend_out, launches);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(z.h_counts.p, z.counts.p, 8 * (k + 1), cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(z.ev, st));
+  z.ev_valid = true;
+  CK(cudaStreamSynchronize(st));
+  float ms1 = 0;
+  cudaEventElapsedTime(&ms1, z.t0, z.t1);
+  const uint64_t* cnt = z.h_counts.as<uint64_t>();
+  for (uint64_t j = 0; j < k; j++) blobs[j].n_lines = cnt[j] + (j ? 0 : z.open_lines);
+  z.open_lines = cnt[k] + (k ? 0 : z.open_lines);
+  z.open_bytes = open_out;
+  z.cur ^= 1;
+  rc = cb_finish(c, z, unix_nano, blobs, k, out);
+  if (rc) return rc;
+  out->n_dropped = nd;
+  memcpy(hd + 1, drops.data(), 8 * nd);
+  out->dropped = hd + 1;
+  out->open_lines = z.open_lines;
+  out->open_bytes = z.open_bytes;
+  out->kernel_ms = ms0 + ms1;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+int tgi_combine_flush(tgi_ctx* c, int64_t unix_nano, tgi_combined_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  Combiner& z = c->cb;
+  std::lock_guard<std::mutex> g(z.mu);
+  if (!z.open) { set_err(c, "tgi_combine_flush: no combiner is open (tgi_combine_open)"); return TGI_E_STATE; }
+  cudaSetDevice(c->device);
+  memset(out, 0, sizeof *out);
+  if (!z.open_bytes) return TGI_OK;
+  cudaStream_t st = z.stream;
+  const uint64_t p0 = z.open_bytes % 3, len = (z.open_bytes + 2) / 3 * 4;
+  uint32_t launches = 0;
+  if (z.ev_valid) CK(cudaStreamWaitEvent(st, z.ev, 0));
+  CbPlan P;
+  P.add(z.enc.as<uint8_t>() + z.open_bytes / 3 * 4, true, {{0, p0, z.pend.as<uint8_t>() + 32 * z.cur}});
+  CK(cudaEventRecord(z.t0, st));
+  int rc = cb_launch(c, st, P, nullptr, nullptr, nullptr, launches);
+  if (rc) return rc;
+  CK(cudaEventRecord(z.t1, st));
+  CK(z.h_data.ensure(len + 1));
+  CK(z.h_blobs.ensure(sizeof(tgi_combined_blob)));
+  CK(cudaMemcpyAsync(z.h_data.p, z.enc.p, len, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(z.ev, st));
+  z.ev_valid = true;
+  CK(cudaStreamSynchronize(st));
+  tgi_combined_blob* blobs = z.h_blobs.as<tgi_combined_blob>();
+  blobs[0] = tgi_combined_blob{0, len, 0, 0, z.open_lines, z.open_bytes, 0};
+  z.open_lines = z.open_bytes = 0;
+  rc = cb_finish(c, z, unix_nano, blobs, 1, out);
+  if (rc) return rc;
+  cudaEventElapsedTime(&out->kernel_ms, z.t0, z.t1);
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
 
 // ---- pinned input staging ---------------------------------------------------------------------------------
 int tgi_acquire_staging(tgi_ctx* c, uint64_t bytes, void** out) {

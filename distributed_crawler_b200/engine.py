@@ -35,7 +35,8 @@ EXPORTED_SYMBOLS = [
     "tgi_filter_usernames", "tgi_acquire_staging", "tgi_release_staging", "tgi_comm_unique_id", "tgi_comm_init",
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
-    "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads",
+    "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
+    "tgi_combine_flush",
 ]
 
 
@@ -97,6 +98,10 @@ def lib() -> C.CDLL:
         L.tgi_set_growth.argtypes = [vp, u64]
         L.tgi_set_info.argtypes = [vp, i32, C.POINTER(abi.SetInfoC)]
         L.tgi_dapr_payloads.argtypes = [vp, i32, C.c_char_p, u32, C.POINTER(abi.DaprPayloadsC)]
+        L.tgi_plan_chunks_carry.argtypes = [vp, u64, u64, u64, u64, vp, u64, C.POINTER(u64), vp, C.POINTER(u64)]
+        L.tgi_combine_open.argtypes = [vp, u64, u64, C.c_char_p, u32]
+        L.tgi_combine_add.argtypes = [vp, i32, C.c_int64, C.POINTER(abi.CombinedC)]
+        L.tgi_combine_flush.argtypes = [vp, C.c_int64, C.POINTER(abi.CombinedC)]
         _LIB = L
     return _LIB
 
@@ -178,6 +183,36 @@ class DaprPayloads:
 
     def path(self, i: int) -> bytes:
         return self.path_blob[int(self.path_off[i]):int(self.path_off[i + 1])].tobytes()
+
+
+class CombinedBlobs:
+    """Host copy of a tgi_combined_t: the combined-posts blobs one combine call closed.  Blob j's binding Data is
+    blob(j), its path path(j); blobs[j] holds its n_lines, raw_bytes and unix_nano."""
+
+    def __init__(self, r: abi.CombinedC):
+        k = int(r.n_blobs)
+        self.n_blobs = k
+        self.blobs = [{f: getattr(r.blobs[j], f) for f, _ in abi.CombinedBlobC._fields_} for j in range(k)]
+        data_len = max((b["data_off"] + b["data_len"] for b in self.blobs), default=0)
+        path_len = max((b["path_off"] + b["path_len"] for b in self.blobs), default=0)
+        self.data_blob = _copy(r.data, data_len, np.uint8)
+        self.path_blob = _copy(r.path, path_len, np.uint8)
+        self.dropped = _copy(r.dropped, int(r.n_dropped), np.uint64)
+        self.open_lines = int(r.open_lines)
+        self.open_bytes = int(r.open_bytes)
+        self.kernel_ms = float(r.kernel_ms)
+        self.gpu_launches = int(r.gpu_launches)
+
+    def __len__(self):
+        return self.n_blobs
+
+    def blob(self, j: int) -> bytes:
+        b = self.blobs[j]
+        return self.data_blob[b["data_off"]:b["data_off"] + b["data_len"]].tobytes()
+
+    def path(self, j: int) -> bytes:
+        b = self.blobs[j]
+        return self.path_blob[b["path_off"]:b["path_off"] + b["path_len"]].tobytes()
 
 
 class Engine:
@@ -386,6 +421,23 @@ class Engine:
         out = abi.DaprPayloadsC()
         self._check(lib().tgi_dapr_payloads(self.h, slot, prefix, len(prefix), C.byref(out)))
         return DaprPayloads(out)
+
+    # --- combine mode: combined-posts blobs (SURVEY §8f rank 1) -----------------------------------
+    def combine_open(self, trigger: int, hard_cap: int, prefix: bytes):
+        """(re)configure the combiner: processBatches' trigger / hard cap and the blob path prefix"""
+        self._check(lib().tgi_combine_open(self.h, trigger, hard_cap, prefix, len(prefix)))
+
+    def combine_add(self, slot: int, unix_nano: int) -> CombinedBlobs:
+        """pass the lines of the slot's last Telegram / YouTube result to the combiner; the blobs this closes"""
+        out = abi.CombinedC()
+        self._check(lib().tgi_combine_add(self.h, slot, unix_nano, C.byref(out)))
+        return CombinedBlobs(out)
+
+    def combine_flush(self, unix_nano: int) -> CombinedBlobs:
+        """close the open group (Chunker shutdown)"""
+        out = abi.CombinedC()
+        self._check(lib().tgi_combine_flush(self.h, unix_nano, C.byref(out)))
+        return CombinedBlobs(out)
 
     # --- generic client.Message -> sparse Post (SURVEY a12) -------------------------------------
     def generic(self, batch, run_flags=abi.RUN_JSONL, copy=True) -> Result:

@@ -265,6 +265,22 @@ class MessageProcessor {
     if (tgi_set_info(ctx_, which, &s) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
     return s;
   }
+  // Combine mode (chunk/main.go:292-421, UploadCombinedFile): the combiner's trigger, hard cap and blob path prefix
+  void CombineOpen(uint64_t trigger, uint64_t hard_cap, std::string_view path_prefix) {
+    if (tgi_combine_open(ctx_, trigger, hard_cap, path_prefix.data(), (uint32_t)path_prefix.size()) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+  }
+  // the lines of a result go to the combiner; the blobs this closes, valid until the next combine call
+  tgi_combined_t CombineAdd(const Result& r, int64_t unix_nano) {
+    tgi_combined_t o{};
+    if (tgi_combine_add(ctx_, r.Raw().slot, unix_nano, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  tgi_combined_t CombineFlush(int64_t unix_nano) {  // Chunker shutdown
+    tgi_combined_t o{};
+    if (tgi_combine_flush(ctx_, unix_nano, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

@@ -7,7 +7,8 @@ The grouping rule is libtgingest's tgi_plan_chunks (a restatement of Chunker.pro
 a contiguous slice of the result's JSONL blob (minus lines dropped for exceeding the hard cap).
 
 Local sink: append_posts (LocalStateManager.StorePost).  Dapr sink: store_posts_dapr (DaprStateManager.StorePost outside
-combine mode), fed by Engine.dapr_payloads."""
+combine mode), fed by Engine.dapr_payloads; in combine mode upload_combined_dapr (UploadCombinedFile), fed by
+Engine.combine_add / combine_flush, which group and encode the lines on the device across results."""
 from __future__ import annotations
 
 import ctypes as C
@@ -35,6 +36,23 @@ def plan_chunks(line_off: np.ndarray, trigger: int = TRIGGER_DEFAULT, hard_cap: 
         raise RuntimeError(f"tgi_plan_chunks: {rc}")
     g = groups[: 2 * ng.value].reshape(-1, 2)
     return [(int(a), int(b)) for a, b in g], dropped[:n]
+
+
+def plan_chunks_carry(line_off: np.ndarray, open_bytes: int, trigger: int = TRIGGER_DEFAULT, hard_cap: int = HARD_CAP_DEFAULT):
+    """the streaming form (tgi_plan_chunks_carry): the lines of one result continue a group of open_bytes bytes
+    -> (closed groups [(begin, end)], dropped uint8[n], open bytes after the result)"""
+    line_off = np.ascontiguousarray(line_off, dtype=np.uint64)
+    n = len(line_off) - 1
+    cap = max(n + 1, 1)
+    groups = np.zeros(2 * cap, np.uint64)
+    dropped = np.zeros(max(n, 1), np.uint8)
+    ng, ob = C.c_uint64(), C.c_uint64()
+    rc = engine.lib().tgi_plan_chunks_carry(line_off.ctypes.data, n, trigger, hard_cap, open_bytes, groups.ctypes.data, cap,
+                                            C.byref(ng), dropped.ctypes.data, C.byref(ob))
+    if rc:
+        raise RuntimeError(f"tgi_plan_chunks_carry: {rc}")
+    g = groups[: 2 * ng.value].reshape(-1, 2)
+    return [(int(a), int(b)) for a, b in g], dropped[:n], ob.value
 
 
 def write_combined(jsonl: bytes | np.ndarray, line_off: np.ndarray, combine_dir: str, trigger: int = TRIGGER_DEFAULT,
@@ -97,3 +115,13 @@ def store_posts_dapr(invoke, payloads, binding: str, naming_key: str) -> int:
         invoke(binding, "create", payloads.data(i), {naming_key: payloads.path(i), "operation": "append"})
         k += 1
     return k
+
+
+def upload_combined_dapr(invoke, blobs, binding: str, naming_key: str) -> int:
+    """DaprStateManager.UploadCombinedFile (state/daprstate.go:3734-3777) for every blob a combine call closed: one
+    invoke(binding, "create", data, {naming_key: path, "operation": "append"}) per blob, in order, with data = the base64
+    of the combined lines and path = <prefix>combined-posts/combined_<ns>.jsonl.  `blobs` is Engine.combine_add /
+    combine_flush.  Returns the number of requests."""
+    for j in range(blobs.n_blobs):
+        invoke(binding, "create", blobs.blob(j), {naming_key: blobs.path(j), "operation": "append"})
+    return blobs.n_blobs

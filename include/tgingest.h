@@ -413,6 +413,66 @@ int tgi_youtube_batch(tgi_ctx* ctx, const tgi_yt_batch* in, uint32_t run_flags, 
  * max_groups groups are needed.                                                                        */
 int tgi_plan_chunks(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t* groups,
                     uint64_t max_groups, uint64_t* n_groups, uint8_t* dropped);
+/* The same rule as a stream: the lines of one result continue a group that already holds open_bytes_in bytes of earlier
+ * results (0: none), and the group left open at the end is NOT closed: its bytes go to *open_bytes_out.  groups gets
+ * the groups this call closes; the first one has begin 0 when it is the group carried in (it may then hold no line of
+ * this result: the carried group closes before line `end` that would push it over hard_cap).  The open group's lines
+ * of this result are the kept ones behind the last closed group.  Chaining the calls over the results of a stream, then
+ * closing what is left, gives the groups of tgi_plan_chunks over the whole stream; tgi_plan_chunks is the case
+ * open_bytes_in = 0 plus that last close.  TGI_E_ARG: open_bytes_in above hard_cap, or above 0 and not below
+ * trigger (no group rests there).  Each boundary is a binary search over line_off; only the scan for dropped lines is linear. */
+int tgi_plan_chunks_carry(const uint64_t* line_off, uint64_t n, uint64_t trigger, uint64_t hard_cap, uint64_t open_bytes_in,
+                          uint64_t* groups, uint64_t max_groups, uint64_t* n_groups, uint8_t* dropped,
+                          uint64_t* open_bytes_out);
+
+/* Combine mode on the device — with --combine-files (dapr/standalone.go:256-264) DaprStateManager.StorePost writes one
+ * temp file per post into a watch directory (state/daprstate.go:1117-1138); Chunker.processBatches (chunk/main.go:
+ * 292-345) groups those files, combineFiles concatenates each group into combined_<unixnano>.jsonl (:386-421) and
+ * UploadCombinedFile (daprstate.go:3734-3777) sends ONE InvokeBinding per file, with Data = its base64 and the path
+ * <prefix>combined-posts/combined_<ns>.jsonl.  The combiner is context state that takes the lines of each result in
+ * call order and returns, for every blob a call closes, that Data and that path.  The lines never leave the device.
+ *   Rule     processBatches over the stream of every line passed so far.  Records without a line (length 0: skipped,
+ *            failed, TGI_ST_NOLINE) are not files and are ignored.  A line longer than hard_cap is dropped and its
+ *            record index reported in `dropped` (:316-322).  A group closes BEFORE a line that would push it over
+ *            hard_cap (:324-327) and AFTER the line that makes it reach trigger (:334-337).  tgi_combine_flush closes the
+ *            open group if it holds a line (:339-343, Chunker shutdown).  Any trigger / hard_cap is accepted, trigger >
+ *            hard_cap included.
+ *   Data     base64.StdEncoding of the blob's concatenated lines: '=' padding, no line breaks, 4*ceil(raw_bytes/3)
+ *            bytes, data[data_off, data_off + data_len).
+ *   Path     path_prefix verbatim, then "combined-posts/combined_<ns>.jsonl" (generateCrawlExecutableStoragePath,
+ *            daprstate.go:2689-2698, :3743-3746): path[path_off, path_off + path_len).  <ns> = max(unix_nano, previous
+ *            <ns> + 1) for every blob, so names are unique and increase when one call closes several blobs.
+ *   Inputs   tgi_combine_add takes the slot's last result (Telegram or YouTube, bulk or page) like tgi_dapr_payloads,
+ *            also after TGI_RUN_JSONL_DEVICE and TGI_RUN_NO_D2H.  TGI_E_STATE: no combiner is open, the slot holds no
+ *            result, the result ran without TGI_RUN_JSONL, or it is a tgi_generic_batch one (SavePost has no Dapr
+ *            implementation).  The open group never points into the slot: once tgi_combine_add returns, the slot may
+ *            be released and reused.
+ *   Open     tgi_combine_open allocates the open blob's encoded buffer (4*ceil(hard_cap/3) bytes on the device).  On an
+ *            open combiner it reconfigures it, and returns TGI_E_STATE while the open group holds lines.  prefix is
+ *            copied.  tgi_destroy frees everything.
+ *   Order    Calls are serialised by a combiner lock and apply in call order, whatever their slots.  A call whose lines
+ *            all fit in the open group (open_bytes + jsonl_len below trigger and at most hard_cap) and whose line
+ *            offsets are on the host (not TGI_RUN_NO_D2H) only enqueues on the slot's stream and records an event that
+ *            the next call waits on: it does not synchronise, and reports kernel_ms = 0.  Other calls synchronise once
+ *            to plan, and once when their blobs are in host memory.
+ * Outputs live in library-owned pinned memory and stay valid until the next combine call.                             */
+typedef struct tgi_combined_blob {
+  uint64_t data_off, data_len;  /* base64 of the blob in tgi_combined_t.data                                */
+  uint64_t path_off, path_len;  /* its blob path in tgi_combined_t.path                                     */
+  uint64_t n_lines, raw_bytes;  /* posts in it and their bytes (Chunker.postsUploaded / totalUploadSize)    */
+  int64_t unix_nano;            /* the <ns> of combined_<ns>.jsonl                                          */
+} tgi_combined_blob;
+typedef struct tgi_combined_t {
+  uint64_t n_blobs;  const tgi_combined_blob* blobs;  /* blobs CLOSED by this call, in order                  */
+  const uint8_t* data;  const uint8_t* path;          /* library-owned pinned memory                          */
+  uint64_t n_dropped;  const uint64_t* dropped;       /* record indices of this result's lines > hard_cap     */
+  uint64_t open_lines, open_bytes;                    /* the group still open after the call                  */
+  float kernel_ms;                                    /* device time of this call's launches (0: not waited)  */
+  uint32_t gpu_launches;
+} tgi_combined_t;
+int tgi_combine_open(tgi_ctx* ctx, uint64_t trigger, uint64_t hard_cap, const char* path_prefix, uint32_t prefix_len);
+int tgi_combine_add(tgi_ctx* ctx, int slot, int64_t unix_nano, tgi_combined_t* out);  /* the slot's last result        */
+int tgi_combine_flush(tgi_ctx* ctx, int64_t unix_nano, tgi_combined_t* out);           /* Chunker shutdown: :339-343     */
 
 /* SURVEY 8f rank 1, local sink — LocalStateManager.StorePost opens, appends to and closes <crawl>/<channel>/posts/posts.jsonl
  * once per POST (state/storageproviders.go:39-53,275-298).  The lines of consecutive records of one channel are contiguous

@@ -54,4 +54,13 @@ for b, yt in ((Corpus(20000, profile=2, nthreads=4).batch, False), (Corpus(300, 
     (e.youtube_wait if yt else e.telegram_wait)(0)
     print("dapr", e.dapr_payloads(0, b"root/crawl/exec/").data_len)
     e.release(0)
+# combine mode: a page that stays in the open group, a bulk batch run without copies that closes blobs, the flush
+e.combine_open(1_000_000, 1_500_000, b"root/crawl/exec/")
+for b, flags in ((Corpus(100, profile=2, nthreads=4).batch, abi.RUN_JSONL), (Corpus(20000, profile=3, nthreads=4).batch,
+                                                                             abi.RUN_JSONL | abi.RUN_NO_D2H)):
+    e.telegram_submit(0, b, flags)
+    e.telegram_wait(0)
+    print("combine", e.combine_add(0, 1).n_blobs)
+    e.release(0)
+print("combine flush", e.combine_flush(2).n_blobs)
 print("done")
