@@ -164,6 +164,16 @@ class CombinedC(C.Structure):  # tgi_combined_t
                 ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+CHANNEL_GROUP = np.dtype([("chan_idx", "<u4"), ("reserved", "<u4"), ("n_lines", "<u8"), ("first_record", "<u8"),
+                          ("byte_off", "<u8"), ("byte_len", "<u8")])  # tgi_channel_group
+assert CHANNEL_GROUP.itemsize == 40
+
+
+class ChannelAppendsC(C.Structure):  # tgi_channel_appends_t
+    _fields_ = [("n_groups", C.c_uint64), ("groups", C.c_void_p), ("data", C.c_void_p), ("data_len", C.c_uint64),
+                ("order", C.c_void_p), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 class StatsC(C.Structure):
     _fields_ = [("records", C.c_uint64), ("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64),
                 ("links", C.c_uint64), ("frontier_size", C.c_uint64), ("launches", C.c_uint64),

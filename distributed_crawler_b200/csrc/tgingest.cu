@@ -22,6 +22,7 @@
 #include "kernels.cuh"
 #include "dapr.cuh"
 #include "combine.cuh"
+#include "local_appends.cuh"
 #include "tg_page.cuh"
 #include "yt_page.cuh"
 
@@ -155,6 +156,13 @@ struct DaprBufs {
   HostBuf h_off, h_data, h_path, h_sc;
 };
 
+// tgi_channel_appends: the channelID table and row map, the per-record / per-line / per-run arrays (u32s, u64s), the
+// radix counts and their scan, its outputs and the pinned host copies it returns
+struct LocalBufs {
+  DevBuf table, rows, u32s, u64s, counts, roff, groups, order, data, sc;
+  HostBuf h_groups, h_order, h_data, h_sc;
+};
+
 // tgi_combine_*: the combiner's settings, its open group (encoded on the device, 0-2 bytes pending) and its scratch
 struct Combiner {
   std::mutex mu;
@@ -200,6 +208,7 @@ struct Slot {
   RecKind resident = REC_NONE;  // REC_TG / REC_YT: tg / yt describes the batch of the last successful upload
   LastResult last;
   DaprBufs dapr;
+  LocalBufs local;
   // job hand-off (under mu)
   std::mutex mu;
   std::condition_variable cv;
@@ -2364,6 +2373,147 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   cudaEventElapsedTime(&size_ms, s.ev_p0, s.ev_p1);
   cudaEventElapsedTime(&write_ms, s.ev_e0, s.ev_e1);
   out->kernel_ms = size_ms + write_ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// Local sink appends (local_appends.cuh): every kernel and scan is sized by upper bounds the host knows (records,
+// channel rows, the result's JSONL bytes) and reads the exact counts from the device, so the whole pipeline and the
+// read-back are enqueued at once and the call synchronises once.
+int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  LastResult r;
+  int rc = slot_result(c, slot, "tgi_channel_appends", &r);
+  if (rc != TGI_OK) return rc;
+  if (r.kind == REC_GM) { set_err(c, "tgi_channel_appends: generic posts go to SavePost, not StorePost"); return TGI_E_STATE; }
+  if (!r.dev.line_off) { set_err(c, "tgi_channel_appends: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
+  memset(out, 0, sizeof *out);
+  const uint64_t n = r.n, total = r.jsonl_len;  // every byte of the JSONL belongs to a line that takes part
+  if (!n || !total) return TGI_OK;
+  if (n > 0xFFFFFFF0ull) { set_err(c, "tgi_channel_appends: %llu records (at most 2^32 - 16)", (unsigned long long)n); return TGI_E_CAPACITY; }
+  cudaSetDevice(c->device);
+  Slot& s = c->slots[slot];
+  LocalBufs& z = s.local;
+  cudaStream_t st = s.stream;
+  LaSrc src{};
+  src.n = n;
+  src.status = r.dev.status;
+  src.line_off = r.dev.line_off;
+  src.jsonl = r.dev.jsonl;
+  src.yt = r.kind == REC_YT;
+  // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
+  if (src.yt) {
+    src.yt_recs = s.yt.recs, src.yt_chans = s.yt.chans, src.chan_strs = s.yt.chan_strs, src.n_chans = s.yt.n_chans;
+  } else {
+    src.tg_recs = s.tg.recs, src.tg_chans = s.tg.chans, src.chan_strs = s.tg.chan_strs, src.n_chans = s.tg.n_chans;
+  }
+  const uint64_t nc = src.n_chans, n2 = n + 2;
+  const uint64_t gmax = std::min<uint64_t>(n, nc);  // groups: at most one per record and one per row
+  const uint64_t tslots = next_pow2(std::max<uint64_t>(2 * nc, 64));
+  // radix passes over the bits of the largest group id, 8 bits or fewer each
+  uint32_t bits = 0;
+  while (bits < 32 && (gmax - 1) >> bits) bits++;
+  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
+  const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;
+  CK(z.table.ensure(tslots * 4));
+  CK(z.rows.ensure(2 * nc * 4));
+  CK(z.u32s.ensure(11 * n2 * 4));
+  CK(z.u64s.ensure(7 * n2 * 8));
+  CK(z.counts.ensure(radix * ntiles * 4));
+  CK(z.roff.ensure((radix * ntiles + 1) * 8));
+  CK(z.groups.ensure(gmax * sizeof(tgi_channel_group)));
+  CK(z.order.ensure(n * 8));
+  CK(z.data.ensure(total));
+  CK(z.sc.ensure(LA_SC_COUNT * 8));
+  CK(z.h_groups.ensure(gmax * sizeof(tgi_channel_group)));
+  CK(z.h_order.ensure(n * 8));
+  CK(z.h_data.ensure(total + 1));
+  CK(z.h_sc.ensure(LA_SC_COUNT * 8));
+  LaWork w{};
+  w.sc = z.sc.as<uint64_t>();
+  w.table = z.table.as<uint32_t>();
+  w.tmask = tslots - 1;
+  w.canon = z.rows.as<uint32_t>();
+  w.first_line = w.canon + nc;
+  uint32_t* u = z.u32s.as<uint32_t>();
+  uint32_t** u32_arrays[] = {&w.flag, &w.gflag, &w.lrec, &w.lkey, &w.run_start, &w.keys[0], &w.keys[1], &w.vals[0],
+                             &w.vals[1], &w.cnt, &w.inv};
+  for (size_t k = 0; k < sizeof u32_arrays / sizeof *u32_arrays; k++) *u32_arrays[k] = u + k * n2;
+  uint64_t* v = z.u64s.as<uint64_t>();
+  uint64_t** u64_arrays[] = {&w.pos, &w.rpos, &w.gpos, &w.lpos, &w.goff, &w.rsrc, &w.rdst};
+  for (size_t k = 0; k < sizeof u64_arrays / sizeof *u64_arrays; k++) *u64_arrays[k] = v + k * n2;
+  w.groups = z.groups.as<tgi_channel_group>();
+  w.order = z.order.as<uint64_t>();
+  w.data = z.data.as<uint8_t>();
+  uint32_t launches = 0;
+  auto grid = [&](uint64_t items) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((items + LA_THREADS - 1) / LA_THREADS, (uint64_t)c->sms * 16)); };
+  CK(cudaMemsetAsync(w.table, 0xFF, tslots * 4, st));
+  CK(cudaMemsetAsync(w.first_line, 0xFF, nc * 4, st));
+  CK(cudaMemsetAsync(w.sc, 0, LA_SC_COUNT * 8, st));
+  CK(cudaEventRecord(s.ev_p0, st));
+  la_canon_insert_kernel<<<grid(nc), LA_THREADS, 0, st>>>(src, w);
+  la_canon_flag_kernel<<<grid(std::max(n, nc)), LA_THREADS, 0, st>>>(src, w);
+  launches += 2;
+  if ((rc = launch_scan(c, s, w.flag, n, w.pos, w.sc + LA_SC_LINES, launches))) return rc;
+  la_compact_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w);
+  la_flags_kernel<<<grid(n), LA_THREADS, 0, st>>>(n, w);
+  launches += 2;
+  if ((rc = launch_scan(c, s, w.flag, n, w.rpos, w.sc + LA_SC_RUNS, launches))) return rc;
+  if ((rc = launch_scan(c, s, w.gflag, n, w.gpos, w.sc + LA_SC_GROUPS, launches))) return rc;
+  la_runs_kernel<<<grid(n), LA_THREADS, 0, st>>>(n, w);
+  launches++;
+  int cur = 0;  // the ping-pong side that holds the sorted pairs
+  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
+    const uint32_t shift = p * width;
+    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(w.keys[cur], w.sc + LA_SC_RUNS, shift, radix,
+                                                                     (uint32_t)ntiles, z.counts.as<uint32_t>());
+    launches++;
+    if ((rc = launch_scan(c, s, z.counts.as<uint32_t>(), radix * ntiles, z.roff.as<uint64_t>(), w.sc + LA_SC_RADIX, launches))) return rc;
+    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(w.keys[cur], w.vals[cur], w.keys[cur ^ 1],
+                                                                        w.vals[cur ^ 1], w.sc + LA_SC_RUNS, shift, radix,
+                                                                        (uint32_t)ntiles, z.roff.as<uint64_t>());
+    launches++;
+  }
+  const uint32_t* sorted = w.vals[cur];
+  la_sorted_counts_kernel<<<grid(n), LA_THREADS, 0, st>>>(n, sorted, w);
+  launches++;
+  if ((rc = launch_scan(c, s, w.cnt, n, w.lpos, w.sc + LA_SC_SORTED_LINES, launches))) return rc;
+  la_inverse_kernel<<<grid(n), LA_THREADS, 0, st>>>(sorted, w);
+  la_order_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w);
+  launches += 2;
+  if ((rc = launch_scan(c, s, w.cnt, n, w.goff, w.sc + LA_SC_BYTES, launches))) return rc;
+  la_tables_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w.keys[cur], sorted, w);
+  const uint64_t vec_steps = ((total + 15) / 16 + LA_GATHER_ITEMS * LA_THREADS - 1) / (LA_GATHER_ITEMS * LA_THREADS);
+  la_gather_kernel<<<(unsigned)std::min<uint64_t>(vec_steps, (uint64_t)c->sms * 8), LA_THREADS, 0, st>>>(src, w, total);
+  launches += 2;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(s.ev_p1, st));
+  // the read-back: the scalars, the group table and `order` at their upper bounds, the grouped bytes exactly
+  CK(cudaMemcpyAsync(z.h_sc.p, w.sc, LA_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(z.h_groups.p, w.groups, gmax * sizeof(tgi_channel_group), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(z.h_order.p, w.order, n * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(z.h_data.p, w.data, total, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t* hsc = z.h_sc.as<uint64_t>();
+  const uint64_t lines = hsc[LA_SC_LINES], n_groups = hsc[LA_SC_GROUPS];
+  if (hsc[LA_SC_BYTES] != total || hsc[LA_SC_SORTED_LINES] != lines || n_groups > gmax) {
+    set_err(c, "tgi_channel_appends: %llu grouped bytes of %llu, %llu grouped lines of %llu", (unsigned long long)hsc[LA_SC_BYTES],
+            (unsigned long long)total, (unsigned long long)hsc[LA_SC_SORTED_LINES], (unsigned long long)lines);
+    return TGI_E_CUDA;
+  }
+  // the device left every group's first grouped line in n_lines and its first byte in byte_off: the next group's start
+  // (or the end) turns them into counts
+  tgi_channel_group* g = z.h_groups.as<tgi_channel_group>();
+  for (uint64_t k = 0; k < n_groups; k++) {
+    g[k].n_lines = (k + 1 < n_groups ? g[k + 1].n_lines : lines) - g[k].n_lines;
+    g[k].byte_len = (k + 1 < n_groups ? g[k + 1].byte_off : total) - g[k].byte_off;
+  }
+  out->n_groups = n_groups;
+  out->groups = g;
+  out->data = z.h_data.as<uint8_t>();
+  out->data_len = total;
+  out->order = z.h_order.as<uint64_t>();
+  cudaEventElapsedTime(&out->kernel_ms, s.ev_p0, s.ev_p1);
   out->gpu_launches = launches;
   return TGI_OK;
 }

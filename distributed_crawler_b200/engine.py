@@ -36,7 +36,7 @@ EXPORTED_SYMBOLS = [
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
     "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
-    "tgi_combine_flush",
+    "tgi_combine_flush", "tgi_channel_appends",
 ]
 
 
@@ -102,6 +102,7 @@ def lib() -> C.CDLL:
         L.tgi_combine_open.argtypes = [vp, u64, u64, C.c_char_p, u32]
         L.tgi_combine_add.argtypes = [vp, i32, C.c_int64, C.POINTER(abi.CombinedC)]
         L.tgi_combine_flush.argtypes = [vp, C.c_int64, C.POINTER(abi.CombinedC)]
+        L.tgi_channel_appends.argtypes = [vp, i32, C.POINTER(abi.ChannelAppendsC)]
         _LIB = L
     return _LIB
 
@@ -183,6 +184,35 @@ class DaprPayloads:
 
     def path(self, i: int) -> bytes:
         return self.path_blob[int(self.path_off[i]):int(self.path_off[i + 1])].tobytes()
+
+
+class ChannelAppends:
+    """A tgi_channel_appends_t: the lines of one result grouped by channel.  groups is an abi.CHANNEL_GROUP array
+    (copied); data and order are views of the library's pinned memory, valid until the release or the next call on the
+    slot.  Group k's bytes are group(k)."""
+
+    def __init__(self, r: abi.ChannelAppendsC):
+        self.n_groups = int(r.n_groups)
+        self.data_len = int(r.data_len)
+        self.kernel_ms = float(r.kernel_ms)
+        self.gpu_launches = int(r.gpu_launches)
+        self.groups = _copy(r.groups, self.n_groups, abi.CHANNEL_GROUP)
+        self.n_lines = int(self.groups["n_lines"].sum())
+        self.data = _view(r.data, self.data_len, np.uint8)
+        self.order = _view(r.order, self.n_lines, np.uint64)
+
+    def __len__(self):
+        return self.n_groups
+
+    def group(self, k: int) -> memoryview:
+        g = self.groups[k]
+        return memoryview(self.data[int(g["byte_off"]):int(g["byte_off"]) + int(g["byte_len"])])
+
+
+def _view(p, n, dt):
+    if not n or not p:
+        return np.zeros(0, dt)
+    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * np.dtype(dt).itemsize,)).view(dt)
 
 
 class CombinedBlobs:
@@ -421,6 +451,13 @@ class Engine:
         out = abi.DaprPayloadsC()
         self._check(lib().tgi_dapr_payloads(self.h, slot, prefix, len(prefix), C.byref(out)))
         return DaprPayloads(out)
+
+    def channel_appends(self, slot: int) -> ChannelAppends:
+        """the lines of the slot's last Telegram / YouTube result grouped by channelID on the device (call before
+        release): one group per posts.jsonl file, each group's lines in record order, groups by first line"""
+        out = abi.ChannelAppendsC()
+        self._check(lib().tgi_channel_appends(self.h, slot, C.byref(out)))
+        return ChannelAppends(out)
 
     # --- combine mode: combined-posts blobs (SURVEY §8f rank 1) -----------------------------------
     def combine_open(self, trigger: int, hard_cap: int, prefix: bytes):

@@ -214,6 +214,13 @@ class Result {
       throw std::runtime_error(tgi_last_error(ctx_));
     return p;
   }
+  // LocalStateManager.StorePost (state/storageproviders.go:275-298) with one append per channel file: this result's lines
+  // grouped by channelID on the device, each group's in record order; valid until the next call or the release
+  tgi_channel_appends_t ChannelAppends() const {
+    tgi_channel_appends_t a{};
+    if (tgi_channel_appends(ctx_, r_.slot, &a) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return a;
+  }
 
  private:
   tgi_ctx* ctx_;

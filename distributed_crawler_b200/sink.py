@@ -6,7 +6,9 @@ chunk combiner would upload as combined_<ns>.jsonl (chunk/main.go:292-421), with
 The grouping rule is libtgingest's tgi_plan_chunks (a restatement of Chunker.processBatches); the bytes of a group are
 a contiguous slice of the result's JSONL blob (minus lines dropped for exceeding the hard cap).
 
-Local sink: append_posts (LocalStateManager.StorePost).  Dapr sink: store_posts_dapr (DaprStateManager.StorePost outside
+Local sink: append_posts (LocalStateManager.StorePost) over a result's host JSONL, one append per run of consecutive
+lines of a channel; append_posts_grouped, fed by Engine.channel_appends, one append per channel file, also when the
+lines stayed on the device or the channels interleave.  Dapr sink: store_posts_dapr (DaprStateManager.StorePost outside
 combine mode), fed by Engine.dapr_payloads; in combine mode upload_combined_dapr (UploadCombinedFile), fed by
 Engine.combine_add / combine_flush, which group and encode the lines on the device across results."""
 from __future__ import annotations
@@ -100,6 +102,49 @@ def append_posts(jsonl: bytes | np.ndarray, line_off: np.ndarray, recs: np.ndarr
         with open(os.path.join(d, "posts.jsonl"), "ab") as f:
             f.write(buf[int(r["byte_begin"]): int(r["byte_end"])])
     return len(runs)
+
+
+def go_clean(p: bytes) -> bytes:
+    """Go's filepath.Clean on a Unix path: repeated separators become one, "." elements go, ".." removes the element
+    before it (a rooted path drops a leading ".."), no trailing separator; the empty result is "." ("/" if rooted).
+    Unlike os.path.normpath, a leading "//" becomes "/"."""
+    rooted = p.startswith(b"/")
+    out: list[bytes] = []
+    for e in p.split(b"/"):
+        if e in (b"", b"."):
+            continue
+        if e == b"..":
+            if out and out[-1] != b"..":
+                out.pop()
+            elif not rooted:
+                out.append(e)
+            continue
+        out.append(e)
+    s = b"/".join(out)
+    return (b"/" + s) if rooted else (s or b".")
+
+
+def go_join(*elems: bytes) -> bytes:
+    """Go's filepath.Join: the non-empty elements joined with "/", then Clean; "" when every element is empty"""
+    parts = [e for e in elems if e]
+    return go_clean(b"/".join(parts)) if parts else b""
+
+
+def append_posts_grouped(engine, slot: int, channel_ids, base_path, crawl_id) -> int:
+    """LocalStateManager.StorePost for the slot's last Telegram / YouTube result (state/storageproviders.go:275-298),
+    one append per channel file: filepath.Join(base, crawl, channelID, "posts")/posts.jsonl gets the channel's lines in
+    record order, grouped on the device by Engine.channel_appends (call before release).  channel_ids[row] is the
+    channelID of channel row `row` (str or bytes; the group's lowest row stands for every row with the same bytes).
+    Returns the number of appends."""
+    enc = lambda x: x if isinstance(x, bytes) else os.fsencode(x)
+    ca = engine.channel_appends(slot)
+    base, crawl = enc(base_path), enc(crawl_id)
+    for k in range(ca.n_groups):
+        d = go_join(base, crawl, enc(channel_ids[int(ca.groups[k]["chan_idx"])]), b"posts")
+        os.makedirs(d, exist_ok=True)
+        with open(go_join(d, b"posts.jsonl"), "ab") as f:
+            f.write(ca.group(k))
+    return ca.n_groups
 
 
 def store_posts_dapr(invoke, payloads, binding: str, naming_key: str) -> int:

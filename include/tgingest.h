@@ -488,6 +488,42 @@ typedef struct tgi_append_run {
 int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uint32_t chan_stride, uint64_t n,
                              tgi_append_run* runs, uint64_t max_runs, uint64_t* n_runs);
 
+/* Local sink on the device — the same posts.jsonl files as one LocalStateManager.StorePost per post, written with ONE
+ * append per channel file per result, also when the result's lines stay on the device and when one channel's lines are
+ * interleaved with other channels' (a YouTube batch, several channels' pages in one bulk call).  tgi_channel_appends
+ * groups the lines of the slot's last result by channel on the device and returns every group's bytes, contiguous.
+ *   Input    the slot's last Telegram or YouTube result, bulk or page, like tgi_dapr_payloads: also after
+ *            TGI_RUN_JSONL_DEVICE (this call is then the only time the lines cross PCIe) and TGI_RUN_NO_D2H.
+ *   Lines    only records with status TGI_ST_EMITTED and a non-empty line take part.  Skipped, failed and
+ *            TGI_ST_NOLINE records never reach StorePost: they neither start nor break a group.
+ *   Channel  channelID as tgi_dapr_payloads reads it: Telegram = the channel row's name (tdutils.go:725), YouTube = the
+ *            channel row's id (youtube_crawler.go:396).  Rows whose channelID bytes are equal are ONE channel (one file,
+ *            so one group); chan_idx is the lowest such row.  IDs that differ as bytes but that filepath.Clean maps to
+ *            one path (e.g. "a" and "a/") are distinct groups: real usernames are [A-Za-z0-9_] and channel ids
+ *            [A-Za-z0-9_-], so this cannot happen with real data.
+ *   Order    inside a group, lines in record order: what the per-post appends leave in the file.  Groups are ordered by
+ *            their first line.  order[] lists the record index of every grouped line, group after group.
+ *   Errors   TGI_E_STATE: the slot holds no result (see tgi_result_read_jsonl), the result ran without TGI_RUN_JSONL,
+ *            or it is a tgi_generic_batch one (its posts go to SavePost).  TGI_E_ARG: bad slot or NULL out.
+ *            TGI_E_NOMEM: allocation failed (the batch result stays valid).  TGI_E_CAPACITY: 2^32 - 16 records or more.
+ * The call synchronises once.  Outputs live in library-owned pinned memory and stay valid until the release or the
+ * next call on that slot.  The batch's tgi_result is not changed.                                                     */
+typedef struct tgi_channel_group {
+  uint32_t chan_idx;      /* first channel row (lowest index) carrying this channelID                              */
+  uint32_t reserved;
+  uint64_t n_lines;       /* posts of this channel in the result                                                   */
+  uint64_t first_record;  /* record index of its first line                                                        */
+  uint64_t byte_off, byte_len; /* its lines, in record order, in tgi_channel_appends_t.data                        */
+} tgi_channel_group;
+typedef struct tgi_channel_appends_t {
+  uint64_t n_groups;  const tgi_channel_group* groups; /* ordered by first_record                                  */
+  const uint8_t* data; uint64_t data_len;              /* all emitted lines, grouped (pinned)                     */
+  const uint64_t* order;                               /* [n_lines total] record index of each grouped line        */
+  float kernel_ms;      /* device time of this call's kernels and scans (not the read-back)                        */
+  uint32_t gpu_launches;
+} tgi_channel_appends_t;
+int tgi_channel_appends(tgi_ctx* ctx, int slot, tgi_channel_appends_t* out);
+
 /* Dapr sink — DaprStateManager.StorePost outside combine mode (state/daprstate.go:1141-1181) sends, per post, ONE
  * InvokeBinding with Operation "create", Data = base64.StdEncoding.EncodeToString(json.Marshal(post) + "\n") (:1159)
  * and Metadata {<file naming key>: <blob path>, "operation": "append"} (:1150-1153, path format :2689-2698).

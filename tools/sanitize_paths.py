@@ -53,6 +53,7 @@ for b, yt in ((Corpus(20000, profile=2, nthreads=4).batch, False), (Corpus(300, 
     (e.youtube_submit if yt else e.telegram_submit)(0, b, abi.RUN_JSONL | abi.RUN_JSONL_DEVICE)
     (e.youtube_wait if yt else e.telegram_wait)(0)
     print("dapr", e.dapr_payloads(0, b"root/crawl/exec/").data_len)
+    print("local appends", len(e.channel_appends(0)))
     e.release(0)
 # combine mode: a page that stays in the open group, a bulk batch run without copies that closes blobs, the flush
 e.combine_open(1_000_000, 1_500_000, b"root/crawl/exec/")
