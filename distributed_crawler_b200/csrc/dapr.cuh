@@ -7,7 +7,7 @@
 // Two kernels: dapr_size_kernel measures both per record (the host scans them into u64 offsets with launch_scan),
 // dapr_write_kernel encodes each line once, a warp per record, and writes its path.
 #pragma once
-#include "kernels.cuh"
+#include "sink_src.cuh"
 
 namespace tgi {
 
@@ -18,23 +18,6 @@ constexpr int DAPR_ERR_TOO_LONG = 1;        // a payload or a path of 2^32 bytes
 constexpr uint64_t DAPR_POSTS = 0x2f7374736f702full;  // "/posts/"
 constexpr uint64_t DAPR_JSONL = 0x6c6e6f736a2eull;    // ".jsonl"
 
-// where a record's channelID and PostUID come from
-struct DaprSrc {
-  uint64_t n;
-  const uint8_t* status;    // the batch result's status [n]
-  const uint64_t* line_off; // ... its line offsets [n+1] and lines
-  const uint8_t* jsonl;
-  bool yt;
-  const tgi_tg_rec* tg_recs;  // Telegram: channelID = channel row's name (tdutils.go:725), PostUID = id/2^20 "-" name
-  const tgi_tg_chan* tg_chans;
-  const tgi_yt_rec* yt_recs;  // YouTube: channelID = channel row's id (youtube_crawler.go:396), PostUID = video id (:701)
-  const tgi_yt_chan* yt_chans;
-  const uint8_t* strs;
-  const uint8_t* chan_strs;
-  const uint8_t* prefix;      // StorageRoot/CrawlID/CrawlExecutionID/, verbatim
-  uint32_t prefix_len;
-};
-
 struct DaprOut {
   uint32_t* data_len;  // [n] sizes (dapr_size_kernel)
   uint32_t* path_len;
@@ -43,6 +26,8 @@ struct DaprOut {
   uint8_t* data;
   uint8_t* path;
   int* err;
+  const uint8_t* prefix;  // StorageRoot/CrawlID/CrawlExecutionID/, verbatim
+  uint32_t prefix_len;
 };
 
 struct DaprPath {
@@ -54,41 +39,38 @@ struct DaprPath {
   uint32_t num_len;     // digits of num, 0 for YouTube
 };
 
-DEVI DaprPath dapr_path(const DaprSrc& s, uint64_t i) {
+// PostUID: Telegram id/2^20 "-" channel name (tdutils.go:1008), YouTube the video id (youtube_crawler.go:701)
+DEVI DaprPath dapr_path(const SinkSrc& s, uint64_t i) {
   DaprPath p;
   if (s.yt) {
     const tgi_yt_rec& r = s.yt_recs[i];
-    const tgi_yt_chan& ch = s.yt_chans[r.chan_idx];
-    p.chan = s.chan_strs + ch.str_off;
-    p.chan_len = ch.id_len;
+    p.chan = sink_chan_id(s, r.chan_idx, p.chan_len);
     p.uid = s.strs + r.str_off;
     p.uid_len = r.id_len;
     p.num = 0;
     p.num_len = 0;
   } else {
     const tgi_tg_rec& r = s.tg_recs[i];
-    const tgi_tg_chan& ch = s.tg_chans[r.chan_idx];
-    p.chan = s.chan_strs + ch.str_off + ch.title_len;
-    p.chan_len = ch.name_len;
+    p.chan = sink_chan_id(s, r.chan_idx, p.chan_len);
     p.uid = p.chan;
-    p.uid_len = ch.name_len;
+    p.uid_len = p.chan_len;
     p.num = r.id / 1048576;
     p.num_len = ndigits_i64(p.num) + 1;  // the number and its '-'
   }
   return p;
 }
-DEVI uint64_t dapr_path_len(const DaprSrc& s, const DaprPath& p) {
-  return (uint64_t)s.prefix_len + p.chan_len + 7 + p.num_len + p.uid_len + 6;  // "/posts/" ... ".jsonl"
+DEVI uint64_t dapr_path_len(const DaprOut& o, const DaprPath& p) {
+  return (uint64_t)o.prefix_len + p.chan_len + 7 + p.num_len + p.uid_len + 6;  // "/posts/" ... ".jsonl"
 }
 
 // one thread per record: base64 length 4*ceil(len/3) of its line and the length of its path; 0 for records without a
 // post (skipped, failed, TGI_ST_NOLINE: the reference calls no binding for them)
-__global__ void dapr_size_kernel(DaprSrc s, DaprOut o) {
+__global__ void dapr_size_kernel(SinkSrc s, DaprOut o) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < s.n; i += (uint64_t)gridDim.x * blockDim.x) {
     uint64_t d = 0, p = 0;
     if (s.status[i] == TGI_ST_EMITTED) {
       d = (s.line_off[i + 1] - s.line_off[i] + 2) / 3 * 4;
-      p = dapr_path_len(s, dapr_path(s, i));
+      p = dapr_path_len(o, dapr_path(s, i));
     }
     if ((d | p) >> 32) {
       atomicOr(o.err, DAPR_ERR_TOO_LONG);
@@ -97,11 +79,6 @@ __global__ void dapr_size_kernel(DaprSrc s, DaprOut o) {
     o.data_len[i] = (uint32_t)d;
     o.path_len[i] = (uint32_t)p;
   }
-}
-
-// one base64 character of a 6-bit value: A-Z a-z 0-9 + / (StdEncoding)
-DEVI uint32_t b64_char(uint32_t v) {
-  return v + (v < 26 ? 'A' : v < 52 ? 'a' - 26 : v < 62 ? (uint32_t)('0' - 52) : v == 62 ? (uint32_t)('+' - 62) : (uint32_t)('/' - 63));
 }
 
 struct DaprShared {
@@ -113,7 +90,7 @@ struct DaprShared {
 // 16-byte words that cover the chunk in shared memory (lines start at any byte; the loads stay within 15 bytes of the
 // line's end, inside the PAD bytes every device blob carries), then lane l encodes output words l, l+32, ...: 3 line
 // bytes -> one 4-byte word, stored at a 4-byte aligned address (payload lengths are multiples of 4), coalesced.
-__global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(DaprSrc s, DaprOut o) {
+__global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(SinkSrc s, DaprOut o) {
   __shared__ DaprShared sh;
   const int l = lane_id(), w = threadIdx.x >> 5;
   const uint8_t* sm = (const uint8_t*)sh.line[w];
@@ -140,6 +117,8 @@ __global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(DaprSrc s, D
       for (int k = 0; k < DAPR_CHUNK / 96; k++) {
         const uint32_t q = l + 32 * k;
         if (q < words) {
+          // written out rather than through b64_word: with its byte count m - 3q the compiler cannot rule out the
+          // wrap-around, and this loop grows by 16 instructions
           const uint32_t b = 3 * q;
           const uint32_t x = ((uint32_t)sm[shift + b] << 16) | (b + 1 < m ? (uint32_t)sm[shift + b + 1] << 8 : 0u) |
                              (b + 2 < m ? (uint32_t)sm[shift + b + 2] : 0u);
@@ -158,11 +137,11 @@ __global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(DaprSrc s, D
     }
     __syncwarp();
     uint8_t* dp = o.path + o.path_off[i];
-    const uint64_t e0 = s.prefix_len, e1 = e0 + p.chan_len, e2 = e1 + 7, e3 = e2 + p.num_len, e4 = e3 + p.uid_len,
+    const uint64_t e0 = o.prefix_len, e1 = e0 + p.chan_len, e2 = e1 + 7, e3 = e2 + p.num_len, e4 = e3 + p.uid_len,
                    e5 = e4 + 6;
     for (uint64_t j = l; j < e5; j += 32) {
       uint32_t c;
-      if (j < e0) c = ldb(s.prefix + j);
+      if (j < e0) c = ldb(o.prefix + j);
       else if (j < e1) c = ldb(p.chan + (j - e0));
       else if (j < e2) c = (uint32_t)(DAPR_POSTS >> (8 * (j - e1))) & 0xFF;
       else if (j < e3) c = sh.num[w][j - e2];

@@ -31,6 +31,19 @@ DEVI uint32_t ld_u32_unaligned(const uint8_t* p) {
   return __funnelshift_r(lo, hi, sh);
 }
 
+// 16 bytes at arbitrary alignment as four little-endian words: the two aligned 16-byte words that cover them and
+// funnel shifts.  Reads [q & ~15, (q & ~15) + 32), at most 16 bytes past q+15 (device blobs carry PAD bytes).
+DEVI uint4 ld16_unaligned(const uint8_t* q) {
+  const uint32_t sa = (uint32_t)(uintptr_t)q & 15u, sh = (sa & 3u) * 8u, qw = sa >> 2;
+  const uint4 a = __ldg((const uint4*)(q - sa)), c = __ldg((const uint4*)(q - sa) + 1);
+  uint32_t v0, v1, v2, v3, v4;
+  if (qw == 0) { v0 = a.x; v1 = a.y; v2 = a.z; v3 = a.w; v4 = c.x; }
+  else if (qw == 1) { v0 = a.y; v1 = a.z; v2 = a.w; v3 = c.x; v4 = c.y; }
+  else if (qw == 2) { v0 = a.z; v1 = a.w; v2 = c.x; v3 = c.y; v4 = c.z; }
+  else { v0 = a.w; v1 = c.x; v2 = c.y; v3 = c.z; v4 = c.w; }
+  return make_uint4(__funnelshift_r(v0, v1, sh), __funnelshift_r(v1, v2, sh), __funnelshift_r(v2, v3, sh), __funnelshift_r(v3, v4, sh));
+}
+
 // ---- character classes ---------------------------------------------------------------------------
 DEVI bool is_letter(uint32_t c) { return ((c | 32u) - 'a') < 26u; }
 DEVI bool is_word(uint32_t c) { return is_letter(c) || (c - '0') < 10u || c == '_'; }

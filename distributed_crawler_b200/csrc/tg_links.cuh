@@ -96,23 +96,11 @@ DEVI uint32_t warp_word_run(const uint8_t* p, const uint8_t* end) {
 // A strip for the link scan = 512 bytes, 16 per lane (no UTF-8 bookkeeping is needed to find "t.me/").
 // Returns the lane's 16-bit mask: bit k set if s[p0+k] is the '/' of a "t.me/" (p0 = base + 16*lane).
 // '/' is rare in message text, so almost every strip ends after four SWAR compares per lane.
-// the lane's 16 bytes s[p0 .. p0+16) as four little-endian words (p0 = base + 16*lane; every lane has the same
-// misalignment: two aligned 16-byte loads + one funnel; the blob padding covers the over-read)
-DEVI uint4 load16_lane(const uint8_t* q) {
-  const uint32_t sa = (uint32_t)(uintptr_t)q & 15u, sh = (sa & 3u) * 8u, qw = sa >> 2;
-  const uint4 a = __ldg((const uint4*)(q - sa)), c = __ldg((const uint4*)(q - sa) + 1);
-  uint32_t v0, v1, v2, v3, v4;
-  if (qw == 0) { v0 = a.x; v1 = a.y; v2 = a.z; v3 = a.w; v4 = c.x; }
-  else if (qw == 1) { v0 = a.y; v1 = a.z; v2 = a.w; v3 = c.x; v4 = c.y; }
-  else if (qw == 2) { v0 = a.z; v1 = a.w; v2 = c.x; v3 = c.y; v4 = c.z; }
-  else { v0 = a.w; v1 = c.x; v2 = c.y; v3 = c.z; v4 = c.w; }
-  return make_uint4(__funnelshift_r(v0, v1, sh), __funnelshift_r(v1, v2, sh), __funnelshift_r(v2, v3, sh), __funnelshift_r(v3, v4, sh));
-}
 DEVI uint32_t strip16_tme(const uint8_t* s, int64_t base, int64_t n) {
   const int64_t p0 = base + 16 * lane_id();
   if (p0 >= n) return 0;
   const uint8_t* q = s + p0;
-  const uint4 w = load16_lane(q);
+  const uint4 w = ld16_unaligned(q);
   const uint32_t s0 = swar_eq(w.x, '/'), s1 = swar_eq(w.y, '/'), s2 = swar_eq(w.z, '/'), s3 = swar_eq(w.w, '/');
   if (!(s0 | s1 | s2 | s3)) return 0;
   uint32_t m = swar_movemask(s0) | (swar_movemask(s1) << 4) | (swar_movemask(s2) << 8) | (swar_movemask(s3) << 12);
@@ -133,7 +121,7 @@ DEVI int64_t warp_first_non_ascii(const uint8_t* s, int64_t n) {
     const int64_t p0 = base + 16 * lane_id();
     uint32_t m = 0;
     if (p0 < n) {
-      const uint4 w = load16_lane(s + p0);
+      const uint4 w = ld16_unaligned(s + p0);
       m = swar_movemask(w.x & 0x80808080u) | (swar_movemask(w.y & 0x80808080u) << 4) | (swar_movemask(w.z & 0x80808080u) << 8) |
           (swar_movemask(w.w & 0x80808080u) << 12);
       const int64_t rem = n - p0;

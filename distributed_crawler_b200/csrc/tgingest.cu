@@ -30,7 +30,7 @@ using namespace tgi;
 
 namespace {
 
-constexpr size_t PAD = 64;  // zero bytes behind every device blob (kernels over-read <= 16 bytes)
+constexpr size_t PAD = 64;  // zero bytes behind every device blob (kernels over-read <= 31 bytes)
 
 struct DevBuf {
   void* p = nullptr;
@@ -1702,6 +1702,38 @@ int slot_result(tgi_ctx* c, int slot, const char* who, LastResult* r) {
   return TGI_OK;
 }
 
+// The sinks' view of slot `slot`: its last result, which must be a Telegram or YouTube one with lines; with src, also
+// the device arrays the sink kernels read (sink_src.cuh).  Selects the context's device.
+int sink_source(tgi_ctx* c, int slot, const char* who, LastResult& r, SinkSrc* src) {
+  const int rc = slot_result(c, slot, who, &r);
+  if (rc != TGI_OK) return rc;
+  if (r.kind == REC_GM) { set_err(c, "%s: generic posts go to SavePost, not to the StorePost sinks", who); return TGI_E_STATE; }
+  if (!r.dev.line_off) { set_err(c, "%s: the slot's last result has no lines (run it with TGI_RUN_JSONL)", who); return TGI_E_STATE; }
+  cudaSetDevice(c->device);
+  if (!src) return TGI_OK;
+  const Slot& s = c->slots[slot];
+  *src = SinkSrc{};
+  src->n = r.n;
+  src->status = r.dev.status;
+  src->line_off = r.dev.line_off;
+  src->jsonl = r.dev.jsonl;
+  src->yt = r.kind == REC_YT;
+  // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
+  if (src->yt) {
+    src->yt_recs = s.yt.recs, src->yt_chans = s.yt.chans, src->strs = s.yt.strs, src->chan_strs = s.yt.chan_strs;
+    src->n_chans = s.yt.n_chans;
+  } else {
+    src->tg_recs = s.tg.recs, src->tg_chans = s.tg.chans, src->strs = s.tg.strs, src->chan_strs = s.tg.chan_strs;
+    src->n_chans = s.tg.n_chans;
+  }
+  return TGI_OK;
+}
+
+// the grid of a grid-stride sink launch: one CTA per per_cta items, at most per_sm CTAs per SM
+unsigned sink_grid(const tgi_ctx* c, uint64_t items, uint64_t per_cta, uint64_t per_sm) {
+  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((items + per_cta - 1) / per_cta, (uint64_t)c->sms * per_sm));
+}
+
 // Chunker.processBatches (chunk/main.go:292-345) over lines [0, n) of one result, continuing a group that holds open_in
 // bytes of earlier results; drops are the sorted indices of the lines longer than hard_cap.  Every group the rule closes
 // goes to emit(begin, end) (false: stop with TGI_E_CAPACITY): lines [begin, end) minus the empty and dropped ones, begin
@@ -2285,11 +2317,9 @@ int tgi_pending_edges(tgi_ctx* c, int slot, int64_t now_sec, tgi_edge* rows, uin
 int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t prefix_len, tgi_dapr_payloads_t* out) {
   if (!c || !out || !path_prefix) return TGI_E_ARG;
   LastResult r;
-  int rc = slot_result(c, slot, "tgi_dapr_payloads", &r);
+  SinkSrc src;
+  int rc = sink_source(c, slot, "tgi_dapr_payloads", r, &src);
   if (rc != TGI_OK) return rc;
-  if (r.kind == REC_GM) { set_err(c, "tgi_dapr_payloads: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
-  if (!r.dev.line_off) { set_err(c, "tgi_dapr_payloads: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
-  cudaSetDevice(c->device);
   Slot& s = c->slots[slot];
   DaprBufs& z = s.dapr;
   cudaStream_t st = s.stream;
@@ -2304,22 +2334,8 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
     h_off[0] = h_off[1] = 0;
     return TGI_OK;
   }
-  DaprSrc src{};
-  src.n = n;
-  src.status = r.dev.status;
-  src.line_off = r.dev.line_off;
-  src.jsonl = r.dev.jsonl;
-  src.yt = r.kind == REC_YT;
-  // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
-  if (src.yt) {
-    src.yt_recs = s.yt.recs, src.yt_chans = s.yt.chans, src.strs = s.yt.strs, src.chan_strs = s.yt.chan_strs;
-  } else {
-    src.tg_recs = s.tg.recs, src.tg_chans = s.tg.chans, src.strs = s.tg.strs, src.chan_strs = s.tg.chan_strs;
-  }
-  src.prefix_len = prefix_len;
   CK(z.prefix.ensure(prefix_len));
   if (prefix_len) CK(cudaMemcpyAsync(z.prefix.p, path_prefix, prefix_len, cudaMemcpyHostToDevice, st));
-  src.prefix = z.prefix.as<uint8_t>();
   CK(z.lens.ensure(2 * n * 4));
   CK(z.off.ensure(2 * (n + 1) * 8));
   CK(z.sc.ensure(4 * 8));
@@ -2331,13 +2347,14 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   o.data_off = z.off.as<uint64_t>();
   o.path_off = o.data_off + n + 1;
   o.err = (int*)(dsc + 2);
+  o.prefix = z.prefix.as<uint8_t>();
+  o.prefix_len = prefix_len;
   uint32_t launches = 0;
   // device time = [ev_p0, ev_p1] (size kernel, scans) + [ev_e0, ev_e1] (writer): the totals' read-back and the host's
   // allocations between them are left out.  The batch's own times were read into its result already.
   CK(cudaMemsetAsync(dsc, 0, 4 * 8, st));
   CK(cudaEventRecord(s.ev_p0, st));
-  const unsigned gs = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
-  dapr_size_kernel<<<gs, 256, 0, st>>>(src, o);
+  dapr_size_kernel<<<sink_grid(c, n, 256, 16), 256, 0, st>>>(src, o);
   launches++;
   rc = launch_scan(c, s, o.data_len, n, (uint64_t*)o.data_off, dsc, launches);
   if (rc) return rc;
@@ -2355,9 +2372,8 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   CK(z.h_path.ensure(path_total + 1));
   o.data = z.data.as<uint8_t>();
   o.path = z.path.as<uint8_t>();
-  const unsigned gw = (unsigned)std::min<uint64_t>((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * 32);  // 5 resident CTAs per SM
   CK(cudaEventRecord(s.ev_e0, st));
-  dapr_write_kernel<<<gw, CTA_THREADS, 0, st>>>(src, o);
+  dapr_write_kernel<<<sink_grid(c, n, WARPS_PER_CTA, 32), CTA_THREADS, 0, st>>>(src, o);  // 5 resident CTAs per SM
   launches++;
   CK(cudaGetLastError());
   CK(cudaEventRecord(s.ev_e1, st));
@@ -2383,30 +2399,16 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
 int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   if (!c || !out) return TGI_E_ARG;
   LastResult r;
-  int rc = slot_result(c, slot, "tgi_channel_appends", &r);
+  SinkSrc src;
+  int rc = sink_source(c, slot, "tgi_channel_appends", r, &src);
   if (rc != TGI_OK) return rc;
-  if (r.kind == REC_GM) { set_err(c, "tgi_channel_appends: generic posts go to SavePost, not StorePost"); return TGI_E_STATE; }
-  if (!r.dev.line_off) { set_err(c, "tgi_channel_appends: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
   memset(out, 0, sizeof *out);
   const uint64_t n = r.n, total = r.jsonl_len;  // every byte of the JSONL belongs to a line that takes part
   if (!n || !total) return TGI_OK;
   if (n > 0xFFFFFFF0ull) { set_err(c, "tgi_channel_appends: %llu records (at most 2^32 - 16)", (unsigned long long)n); return TGI_E_CAPACITY; }
-  cudaSetDevice(c->device);
   Slot& s = c->slots[slot];
   LocalBufs& z = s.local;
   cudaStream_t st = s.stream;
-  LaSrc src{};
-  src.n = n;
-  src.status = r.dev.status;
-  src.line_off = r.dev.line_off;
-  src.jsonl = r.dev.jsonl;
-  src.yt = r.kind == REC_YT;
-  // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
-  if (src.yt) {
-    src.yt_recs = s.yt.recs, src.yt_chans = s.yt.chans, src.chan_strs = s.yt.chan_strs, src.n_chans = s.yt.n_chans;
-  } else {
-    src.tg_recs = s.tg.recs, src.tg_chans = s.tg.chans, src.chan_strs = s.tg.chan_strs, src.n_chans = s.tg.n_chans;
-  }
   const uint64_t nc = src.n_chans, n2 = n + 2;
   const uint64_t gmax = std::min<uint64_t>(n, nc);  // groups: at most one per record and one per row
   const uint64_t tslots = next_pow2(std::max<uint64_t>(2 * nc, 64));
@@ -2446,7 +2448,7 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   w.order = z.order.as<uint64_t>();
   w.data = z.data.as<uint8_t>();
   uint32_t launches = 0;
-  auto grid = [&](uint64_t items) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((items + LA_THREADS - 1) / LA_THREADS, (uint64_t)c->sms * 16)); };
+  auto grid = [&](uint64_t items) { return sink_grid(c, items, LA_THREADS, 16); };
   CK(cudaMemsetAsync(w.table, 0xFF, tslots * 4, st));
   CK(cudaMemsetAsync(w.first_line, 0xFF, nc * 4, st));
   CK(cudaMemsetAsync(w.sc, 0, LA_SC_COUNT * 8, st));
@@ -2483,8 +2485,7 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   launches += 2;
   if ((rc = launch_scan(c, s, w.cnt, n, w.goff, w.sc + LA_SC_BYTES, launches))) return rc;
   la_tables_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w.keys[cur], sorted, w);
-  const uint64_t vec_steps = ((total + 15) / 16 + LA_GATHER_ITEMS * LA_THREADS - 1) / (LA_GATHER_ITEMS * LA_THREADS);
-  la_gather_kernel<<<(unsigned)std::min<uint64_t>(vec_steps, (uint64_t)c->sms * 8), LA_THREADS, 0, st>>>(src, w, total);
+  la_gather_kernel<<<sink_grid(c, (total + 15) / 16, LA_GATHER_ITEMS * LA_THREADS, 8), LA_THREADS, 0, st>>>(src, w, total);
   launches += 2;
   CK(cudaGetLastError());
   CK(cudaEventRecord(s.ev_p1, st));
@@ -2569,8 +2570,7 @@ int cb_launch(tgi_ctx* c, cudaStream_t st, const CbPlan& P, const CbTask* dt, co
     L.tasks = dt;
     L.segs = ds;
   }
-  const unsigned g = (unsigned)std::min<uint64_t>((P.units + 255) / 256, (uint64_t)c->sms * 16);
-  combine_encode_kernel<<<g, 256, 0, st>>>(L);
+  combine_encode_kernel<<<sink_grid(c, P.units, 256, 16), 256, 0, st>>>(L);
   launches++;
   CK(cudaGetLastError());
   return TGI_OK;
@@ -2649,14 +2649,11 @@ int tgi_combine_open(tgi_ctx* c, uint64_t trigger, uint64_t hard_cap, const char
 int tgi_combine_add(tgi_ctx* c, int slot, int64_t unix_nano, tgi_combined_t* out) {
   if (!c || !out) return TGI_E_ARG;
   LastResult r;
-  int rc = slot_result(c, slot, "tgi_combine_add", &r);
+  int rc = sink_source(c, slot, "tgi_combine_add", r, nullptr);
   if (rc != TGI_OK) return rc;
-  if (r.kind == REC_GM) { set_err(c, "tgi_combine_add: generic posts go to SavePost, which has no Dapr implementation"); return TGI_E_STATE; }
-  if (!r.dev.line_off) { set_err(c, "tgi_combine_add: the slot's last result has no lines (run it with TGI_RUN_JSONL)"); return TGI_E_STATE; }
   Combiner& z = c->cb;
   std::lock_guard<std::mutex> g(z.mu);
   if (!z.open) { set_err(c, "tgi_combine_add: no combiner is open (tgi_combine_open)"); return TGI_E_STATE; }
-  cudaSetDevice(c->device);
   memset(out, 0, sizeof *out);
   cudaStream_t st = c->slots[slot].stream;
   const uint64_t n = r.n, L = r.jsonl_len;
@@ -2698,8 +2695,7 @@ int tgi_combine_add(tgi_ctx* c, int slot, int64_t unix_nano, tgi_combined_t* out
   CK(cudaEventRecord(z.t0, st));
   CK(cudaMemsetAsync(d_drops, 0, 8, st));
   if (n && max_drops) {
-    const unsigned gd = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
-    combine_drops_kernel<<<gd, 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, d_drops + 1, max_drops, (unsigned long long*)d_drops);
+    combine_drops_kernel<<<sink_grid(c, n, 256, 16), 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, d_drops + 1, max_drops, (unsigned long long*)d_drops);
     launches++;
     CK(cudaGetLastError());
   }
@@ -2769,9 +2765,8 @@ int tgi_combine_add(tgi_ctx* c, int slot, int64_t unix_nano, tgi_combined_t* out
   CK(cudaEventRecord(z.t0, st));
   CK(cudaMemsetAsync(z.counts.p, 0, 8 * (k + 1), st));
   if (n) {
-    const unsigned gc = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
-    combine_count_kernel<<<gc, 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, (const uint64_t*)dtb, (uint32_t)k,
-                                             z.counts.as<unsigned long long>());
+    combine_count_kernel<<<sink_grid(c, n, 256, 16), 256, 0, st>>>(r.dev.line_off, n, z.hard_cap, (const uint64_t*)dtb,
+                                                                   (uint32_t)k, z.counts.as<unsigned long long>());
     launches++;
     CK(cudaGetLastError());
   }

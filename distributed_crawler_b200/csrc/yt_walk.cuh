@@ -265,7 +265,7 @@ __device__ __noinline__ uint32_t yt_sanitize(const uint8_t* s, uint32_t n, uint8
 DEVI uint32_t yt_strip16_scheme(const uint8_t* s, uint32_t base, uint32_t n) {
   const uint32_t p0 = base + 16u * (uint32_t)lane_id();
   if (p0 >= n) return 0;
-  const uint4 w = load16_lane(s + p0);
+  const uint4 w = ld16_unaligned(s + p0);
   const uint32_t c0 = swar_eq(w.x, ':'), c1 = swar_eq(w.y, ':'), c2 = swar_eq(w.z, ':'), c3 = swar_eq(w.w, ':');
   if (!(c0 | c1 | c2 | c3)) return 0;
   uint32_t m = swar_movemask(c0) | (swar_movemask(c1) << 4) | (swar_movemask(c2) << 8) | (swar_movemask(c3) << 12);
@@ -351,7 +351,7 @@ DEVI bool yt_is_handle_char(uint32_t c) { return is_word(c) || c == '-' || c == 
 DEVI uint32_t yt_strip16_ytcom(const uint8_t* s, uint32_t base, uint32_t n) {
   const uint32_t p0 = base + 16u * (uint32_t)lane_id();
   if (p0 >= n) return 0;
-  const uint4 w = load16_lane(s + p0);
+  const uint4 w = ld16_unaligned(s + p0);
   const uint32_t c0 = swar_eq(w.x, '/'), c1 = swar_eq(w.y, '/'), c2 = swar_eq(w.z, '/'), c3 = swar_eq(w.w, '/');
   if (!(c0 | c1 | c2 | c3)) return 0;
   uint32_t m = swar_movemask(c0) | (swar_movemask(c1) << 4) | (swar_movemask(c2) << 8) | (swar_movemask(c3) << 12);

@@ -107,10 +107,14 @@ def lib() -> C.CDLL:
     return _LIB
 
 
-def _copy(p, n, dt):
+def _view(p, n, dt):
     if not n or not p:
         return np.zeros(0, dt)
-    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * np.dtype(dt).itemsize,)).view(dt).copy()
+    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * np.dtype(dt).itemsize,)).view(dt)
+
+
+def _copy(p, n, dt):
+    return _view(p, n, dt).copy()
 
 
 class Result:
@@ -207,12 +211,6 @@ class ChannelAppends:
     def group(self, k: int) -> memoryview:
         g = self.groups[k]
         return memoryview(self.data[int(g["byte_off"]):int(g["byte_off"]) + int(g["byte_len"])])
-
-
-def _view(p, n, dt):
-    if not n or not p:
-        return np.zeros(0, dt)
-    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * np.dtype(dt).itemsize,)).view(dt)
 
 
 class CombinedBlobs:

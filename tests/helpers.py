@@ -8,7 +8,7 @@ import os
 import numpy as np
 
 from distributed_crawler_b200 import abi
-from distributed_crawler_b200.pack import Channel, FormattedText, Message, TextEntity, pack_telegram
+from distributed_crawler_b200.pack import Channel, Comment, FormattedText, Message, TextEntity, pack_telegram
 
 
 def ft(text, entities=()):
@@ -60,3 +60,73 @@ def no_page():
         yield
     finally:
         del os.environ["TGI_NO_PAGE"]
+
+
+# ---- the result sinks (Dapr payloads, combine mode, local appends) ----------------------------------------------------
+PREFIX = b"/data/crawls/crawl-7/exec-2024-01-01/"
+J = abi.RUN_JSONL
+JL = ALL
+DEV = abi.RUN_JSONL_DEVICE
+
+
+def channel_ids(batch, yt: bool) -> list[bytes]:
+    """channelID of every channel row: Telegram the row's name (tdutils.go:725), YouTube the row's id
+    (youtube_crawler.go:396)"""
+    out = []
+    for ch in batch.chans:
+        o = int(ch["str_off"])
+        if yt:
+            out.append(batch.chan_strs[o:o + int(ch["id_len"])].tobytes())
+        else:
+            o += int(ch["title_len"])
+            out.append(batch.chan_strs[o:o + int(ch["name_len"])].tobytes())
+    return out
+
+
+def post_uid_tg(msg_id: int, channel_name: bytes) -> bytes:
+    """tdutils.go:416,636,1008: fmt.Sprintf("%d-%s", message.Id/1048576, channelName); Go's / truncates toward zero"""
+    q = -((-msg_id) // 1048576) if msg_id < 0 else msg_id // 1048576
+    return b"%d-" % q + channel_name
+
+
+def edge_batch():
+    """escaped, non-UTF-8 and empty channel names, ids of both signs around multiples of 2^20, lines of 2-20 KB,
+    skipped (min_post_date 1 600 000 000) and failed records"""
+    names = [b'a"b', b"<tag>&x", "канал-é✓".encode(), b"bad\xff\xfeutf8\xc0", b"", b"plain_name"]
+    chans = [Channel(title="T%d" % k, name=nm, username="u%d" % k) for k, nm in enumerate(names)]
+    ids = [-(1 << 20) + 1, -1, -(1 << 20), -(1 << 20) - 1, -(5 << 20) - 3, 0, 1 << 20, (1 << 20) - 1, (1 << 62) + 12345,
+           -(1 << 62), 7 << 20]
+    ms = []
+    for k in range(420):
+        long_ = k % 37 == 5
+        text = ("x" * (2000 + 97 * k) + " t.me/longchan") if long_ else ("m%d " % k) + "é" * (k % 23) + "y" * (k % 17)
+        comments = [Comment(text="c" * (200 + k), handle="h%d" % j, view_count=j) for j in range(40)] if k % 53 == 7 else []
+        ms.append(msg("messageText", text, id=ids[k % len(ids)], channel=k % len(chans), date=1_700_000_000 + k,
+                      reactions=[("r%03d" % j, j) for j in range(k % 7 * 60)], comments=comments,
+                      panics=k % 41 == 3))
+    ms[10].date = 1_500_000_000  # before min_post_date: skipped (tdutils.go:419-421)
+    ms[11].date = 1_400_000_000
+    return pack_telegram(ms, chans)
+
+
+def mem_available() -> int:
+    """the host's MemAvailable in bytes, 0 if unknown"""
+    try:
+        with open("/proc/meminfo") as f:
+            for line in f:
+                if line.startswith("MemAvailable:"):
+                    return int(line.split()[1]) * 1024
+    except OSError:
+        pass
+    return 0
+
+
+def on_slot(e, batch, flags, yt, slot, call):
+    """one batch on `slot`: submit, wait, call(slot), release; returns the batch's result (copied) and what call
+    returned, which must not point into the slot's buffers"""
+    (e.youtube_submit if yt else e.telegram_submit)(slot, batch, flags)
+    try:
+        r = (e.youtube_wait if yt else e.telegram_wait)(slot, copy=True)
+        return r, call(slot)
+    finally:
+        e.release(slot)

@@ -15,14 +15,11 @@ from distributed_crawler_b200 import abi, sink
 from distributed_crawler_b200.corpus import Corpus, YtCorpus
 from distributed_crawler_b200.engine import Engine, EngineError, lib
 from distributed_crawler_b200.pack import Channel, pack_telegram, pack_youtube
-from helpers import msg, no_page
+from helpers import DEV, J, JL, channel_ids, mem_available, msg, no_page, on_slot
 from oracle.pyoracle import Oracle
 from yt_corpus import make_youtube, make_youtube_config4
 
 pytestmark = pytest.mark.gpu
-J = abi.RUN_JSONL
-JL = abi.RUN_JSONL | abi.RUN_LINKS | abi.RUN_FRONTIER | abi.RUN_SKIP_SELF
-DEV = abi.RUN_JSONL_DEVICE
 CRAWL = b"crawl-7"
 
 
@@ -34,19 +31,6 @@ def filepath_join(*elems: bytes) -> bytes:
         return b""
     p = posixpath.normpath(b"/".join(parts))
     return p[1:] if p.startswith(b"//") and not p.startswith(b"///") else p
-
-
-def channel_ids(batch, yt: bool) -> list[bytes]:
-    """channelID of every channel row: Telegram the row's name (tdutils.go:725), YouTube the row's id (:396)"""
-    out = []
-    for ch in batch.chans:
-        o = int(ch["str_off"])
-        if yt:
-            out.append(batch.chan_strs[o:o + int(ch["id_len"])].tobytes())
-        else:
-            o += int(ch["title_len"])
-            out.append(batch.chan_strs[o:o + int(ch["name_len"])].tobytes())
-    return out
 
 
 def store_post_loop(batch, yt, ro):
@@ -94,12 +78,7 @@ class Snapshot:
 
 def run(e, batch, flags, yt=False, slot=0):
     """one batch on `slot`, its channel appends, release"""
-    (e.youtube_submit if yt else e.telegram_submit)(slot, batch, flags)
-    try:
-        (e.youtube_wait if yt else e.telegram_wait)(slot)
-        return Snapshot(e.channel_appends(slot))
-    finally:
-        e.release(slot)
+    return on_slot(e, batch, flags, yt, slot, lambda s: Snapshot(e.channel_appends(s)))[1]
 
 
 def tree(root: bytes) -> dict:
@@ -122,12 +101,8 @@ def check_tree(tmp_path, e, batch, yt, ro, flags, slot=0):
             os.makedirs(d, exist_ok=True)
             with open(filepath_join(d, b"posts.jsonl"), "ab") as f:
                 f.write(ro.line(i))
-    (e.youtube_submit if yt else e.telegram_submit)(slot, batch, flags)
-    (e.youtube_wait if yt else e.telegram_wait)(slot)
-    try:
-        k = sink.append_posts_grouped(e, slot, [x.decode("utf-8", "surrogateescape") for x in ids], b, CRAWL)
-    finally:
-        e.release(slot)
+    names = [x.decode("utf-8", "surrogateescape") for x in ids]
+    _, k = on_slot(e, batch, flags, yt, slot, lambda s: sink.append_posts_grouped(e, s, names, b, CRAWL))
     want = tree(a)
     assert k == len(want) and tree(b) == want
 
@@ -331,23 +306,12 @@ def test_slot_rules():
     e.close()
 
 
-def _mem_available() -> int:
-    try:
-        with open("/proc/meminfo") as f:
-            for line in f:
-                if line.startswith("MemAvailable:"):
-                    return int(line.split()[1]) * 1024
-    except OSError:
-        pass
-    return 0
-
-
 LARGE_N = 2_000_000  # config-4 videos over 1 000 channels: a new channel almost every record
 LARGE_HOST_BYTES = 24 << 30
 
 
 def test_config4_batch_of_two_million_videos():
-    if _mem_available() < LARGE_HOST_BYTES:
+    if mem_available() < LARGE_HOST_BYTES:
         pytest.skip(f"needs {LARGE_HOST_BYTES >> 30} GiB of available host memory")
     yc = YtCorpus(LARGE_N)
     b = yc.batch

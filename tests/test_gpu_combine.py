@@ -12,16 +12,12 @@ import pytest
 from distributed_crawler_b200 import abi, sink
 from distributed_crawler_b200.corpus import Corpus
 from distributed_crawler_b200.engine import Engine, EngineError, lib
+from helpers import DEV, J, JL, PREFIX, edge_batch, on_slot
 from oracle.pyoracle import Oracle
-from test_gpu_dapr_payloads import edge_batch
 from test_sink import process_batches
 from yt_corpus import make_youtube
 
 pytestmark = pytest.mark.gpu
-PREFIX = b"/data/crawls/crawl-7/exec-2024-01-01/"
-J = abi.RUN_JSONL
-JL = abi.RUN_JSONL | abi.RUN_LINKS | abi.RUN_FRONTIER | abi.RUN_SKIP_SELF
-DEV = abi.RUN_JSONL_DEVICE
 
 
 class Chain:
@@ -97,12 +93,7 @@ def open_state(chain):
 def add(e, chain, batch, flags, slot, ns, yt=False, ro=None):
     """one batch on `slot`, tgi_combine_add, release; checks the closed blobs and the open group against the chain"""
     ro = ro or (Oracle().youtube(batch, J) if yt else Oracle().telegram(batch, J))
-    (e.youtube_submit if yt else e.telegram_submit)(slot, batch, flags)
-    try:
-        r = (e.youtube_wait if yt else e.telegram_wait)(slot)
-        got = e.combine_add(slot, ns)
-    finally:
-        e.release(slot)
+    r, got = on_slot(e, batch, flags, yt, slot, lambda s: e.combine_add(s, ns))
     same(got, chain.add(lines_of(ro), ns), f"slot {slot} flags {flags:#x} n {ro.n}")
     assert (got.open_lines, got.open_bytes) == open_state(chain)
     return r, got

@@ -12,52 +12,39 @@ import pytest
 
 from distributed_crawler_b200 import abi, sink
 from distributed_crawler_b200.corpus import Corpus
-from distributed_crawler_b200.engine import Engine, EngineError, lib
-from distributed_crawler_b200.pack import Channel, Comment, YouTubeChannel, YouTubeVideo, pack_telegram, pack_youtube
-from helpers import msg
+from distributed_crawler_b200.engine import Engine, EngineError, _view, lib
+from distributed_crawler_b200.pack import pack_telegram, pack_youtube
+from helpers import J, JL, PREFIX, channel_ids, edge_batch, mem_available, on_slot, post_uid_tg
 from oracle.pyoracle import Oracle
 from yt_corpus import make_youtube
 
 pytestmark = pytest.mark.gpu
-PREFIX = b"/data/crawls/crawl-7/exec-2024-01-01/"
-J = abi.RUN_JSONL
-JL = abi.RUN_JSONL | abi.RUN_LINKS | abi.RUN_FRONTIER | abi.RUN_SKIP_SELF
 
 
-def _blob(a, off, n):
-    return a[off: off + n].tobytes()
-
-
-def post_uid_tg(msg_id: int, channel_name: bytes) -> bytes:
-    """tdutils.go:416,636,1008: fmt.Sprintf("%d-%s", message.Id/1048576, channelName); Go's / truncates toward zero"""
-    q = -((-msg_id) // 1048576) if msg_id < 0 else msg_id // 1048576
-    return b"%d-" % q + channel_name
-
-
-def channel_and_uid(batch, yt: bool, i: int):
+def channel_and_uid(batch, yt: bool, i: int, ids):
+    """channelID and PostUID of record i; ids = channel_ids(batch, yt)"""
     r = batch.recs[i]
+    chan = ids[int(r["chan_idx"])]
     if yt:
-        ch = batch.chans[int(r["chan_idx"])]
-        chan = _blob(batch.chan_strs, int(ch["str_off"]), int(ch["id_len"]))  # video.ChannelID (youtube_crawler.go:396)
-        return chan, _blob(batch.strs, int(r["str_off"]), int(r["id_len"]))  # video.ID (:701)
-    ch = batch.chans[int(r["chan_idx"])]
-    name = _blob(batch.chan_strs, int(ch["str_off"]) + int(ch["title_len"]), int(ch["name_len"]))  # tdutils.go:725
-    return name, post_uid_tg(int(r["id"]), name)
+        o = int(r["str_off"])
+        return chan, batch.strs[o:o + int(r["id_len"])].tobytes()  # video.ID (youtube_crawler.go:701)
+    return chan, post_uid_tg(int(r["id"]), chan)
 
 
-def expected(batch, yt, ro, prefix, i):
+def expected(batch, yt, ro, prefix, i, ids):
     """(Data, blob path) of record i, or (b"", b"") where the reference stores nothing"""
     if ro.status[i] != abi.ST_EMITTED:
         return b"", b""
-    chan, uid = channel_and_uid(batch, yt, i)
+    chan, uid = channel_and_uid(batch, yt, i, ids)
     return base64.b64encode(ro.line(i)), prefix + chan + b"/posts/" + uid + b".jsonl"
 
 
 def check(batch, yt, ro, pay, prefix=PREFIX, label=""):
     assert pay.n == ro.n
     assert pay.data_off[0] == 0 and pay.path_off[0] == 0
+    ids = channel_ids(batch, yt)
     for i in range(ro.n):
-        d, p = expected(batch, yt, ro, prefix, i)
+        d, p = expected(batch, yt, ro, prefix, i, ids)
         assert pay.data(i) == d, f"{label}: record {i}: data differs"
         assert pay.path(i) == p, f"{label}: record {i}: path {pay.path(i)!r} != {p!r}"
     assert pay.data_len == int(pay.data_off[-1]) and pay.path_len == int(pay.path_off[-1])
@@ -65,13 +52,7 @@ def check(batch, yt, ro, pay, prefix=PREFIX, label=""):
 
 def run(e, batch, flags, yt=False, slot=0, prefix=PREFIX):
     """one batch on `slot`, its payloads, release"""
-    (e.youtube_submit if yt else e.telegram_submit)(slot, batch, flags)
-    try:
-        r = (e.youtube_wait if yt else e.telegram_wait)(slot, copy=True)
-        pay = e.dapr_payloads(slot, prefix)
-    finally:
-        e.release(slot)
-    return r, pay
+    return on_slot(e, batch, flags, yt, slot, lambda s: e.dapr_payloads(s, prefix))
 
 
 def same_result(a, b):
@@ -151,24 +132,6 @@ def test_youtube_bulk_and_pages():
             assert r.gpu_launches == 1
             check(page, True, rp, pay, label=f"youtube page {k}")
     e.close()
-
-
-def edge_batch():
-    names = [b'a"b', b"<tag>&x", "канал-é✓".encode(), b"bad\xff\xfeutf8\xc0", b"", b"plain_name"]
-    chans = [Channel(title="T%d" % k, name=nm, username="u%d" % k) for k, nm in enumerate(names)]
-    ids = [-(1 << 20) + 1, -1, -(1 << 20), -(1 << 20) - 1, -(5 << 20) - 3, 0, 1 << 20, (1 << 20) - 1, (1 << 62) + 12345,
-           -(1 << 62), 7 << 20]
-    ms = []
-    for k in range(420):
-        long_ = k % 37 == 5
-        text = ("x" * (2000 + 97 * k) + " t.me/longchan") if long_ else ("m%d " % k) + "é" * (k % 23) + "y" * (k % 17)
-        comments = [Comment(text="c" * (200 + k), handle="h%d" % j, view_count=j) for j in range(40)] if k % 53 == 7 else []
-        ms.append(msg("messageText", text, id=ids[k % len(ids)], channel=k % len(chans), date=1_700_000_000 + k,
-                      reactions=[("r%03d" % j, j) for j in range(k % 7 * 60)], comments=comments,
-                      panics=k % 41 == 3))
-    ms[10].date = 1_500_000_000  # before min_post_date: skipped (tdutils.go:419-421)
-    ms[11].date = 1_400_000_000
-    return pack_telegram(ms, chans)
 
 
 @pytest.mark.parametrize("prefix", [b"", PREFIX, b"root/" + bytes(range(32, 127)) * 43 + b"/"])
@@ -273,9 +236,10 @@ def test_store_posts_dapr_end_to_end():
     c = Corpus(5000, profile=2, first=777)
     ro = Oracle().telegram(c.batch, J)
     want = []
+    ids = channel_ids(c.batch, False)
     for i in range(ro.n):
         if ro.status[i] == abi.ST_EMITTED:
-            chan, uid = channel_and_uid(c.batch, False, i)
+            chan, uid = channel_and_uid(c.batch, False, i, ids)
             want.append(store_post_restated(ro.line(i), chan, uid, PREFIX, "telegramstorage", "blobName"))
     got = []
     e = Engine()
@@ -283,21 +247,6 @@ def test_store_posts_dapr_end_to_end():
     assert sink.store_posts_dapr(lambda *req: got.append(req), pay, "telegramstorage", "blobName") == len(want)
     assert got == want
     e.close()
-
-
-def _mem_available() -> int:
-    try:
-        with open("/proc/meminfo") as f:
-            for line in f:
-                if line.startswith("MemAvailable:"):
-                    return int(line.split()[1]) * 1024
-    except OSError:
-        pass
-    return 0
-
-
-def _view(p, n, dt=np.uint8):
-    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * np.dtype(dt).itemsize,)).view(dt) if n else np.zeros(0, dt)
 
 
 LARGE_N = 2_100_000  # config-2 messages: about 4.75 GB of JSONL
@@ -308,7 +257,7 @@ def test_batch_with_more_than_4gib_of_jsonl():
     """One batch whose JSONL passes 4 GiB, every payload compared.  The host holds the packed input, the library's pinned
     payloads (6.4 GB) and the oracle's lines (4.8 GB) once each: nothing is copied into Python objects but the small
     arrays the paths need, and the comparison reads both sides in place."""
-    if _mem_available() < LARGE_HOST_BYTES:
+    if mem_available() < LARGE_HOST_BYTES:
         pytest.skip(f"needs {LARGE_HOST_BYTES >> 30} GiB of available host memory")
     import resource
     from types import SimpleNamespace
@@ -330,20 +279,21 @@ def test_batch_with_more_than_4gib_of_jsonl():
     del d, b
     c.close()
     n = LARGE_N
-    o_status, o_off = _view(ro.status, n), _view(ro.line_off, n + 1, np.uint64)
-    o_jsonl = _view(ro.jsonl, int(ro.jsonl_len))
+    o_status, o_off = _view(ro.status, n, np.uint8), _view(ro.line_off, n + 1, np.uint64)
+    o_jsonl = _view(ro.jsonl, int(ro.jsonl_len), np.uint8)
     assert np.array_equal(o_off, _view(r.line_off, n + 1, np.uint64))
-    assert np.array_equal(o_status, _view(r.status, n))
+    assert np.array_equal(o_status, _view(r.status, n, np.uint8))
     do, po = _view(pay.data_off, n + 1, np.uint64), _view(pay.path_off, n + 1, np.uint64)
-    data, path = _view(pay.data, int(pay.data_len)), _view(pay.path, int(pay.path_len))
+    data, path = _view(pay.data, int(pay.data_len), np.uint8), _view(pay.path, int(pay.path_len), np.uint8)
     assert do[0] == 0 and po[0] == 0 and do[n] == pay.data_len and po[n] == pay.path_len
+    ids = channel_ids(small, False)
     for i in range(n):
         if o_status[i] != abi.ST_EMITTED:
             assert do[i + 1] == do[i] and po[i + 1] == po[i], i
             continue
         want = base64.b64encode(o_jsonl[int(o_off[i]):int(o_off[i + 1])].tobytes())
         assert data[int(do[i]):int(do[i + 1])].tobytes() == want, i
-        chan, uid = channel_and_uid(small, False, i)
+        chan, uid = channel_and_uid(small, False, i, ids)
         assert path[int(po[i]):int(po[i + 1])].tobytes() == PREFIX + chan + b"/posts/" + uid + b".jsonl", i
     print(f"peak RSS {resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 2**20:.1f} GiB")
     lib().tgi_result_release(e.h, 0)

@@ -22,6 +22,7 @@ import numpy as np  # noqa: E402
 from distributed_crawler_b200 import abi, sink  # noqa: E402
 from distributed_crawler_b200.corpus import Corpus, YtCorpus  # noqa: E402
 from distributed_crawler_b200.engine import Engine, EngineError, lib  # noqa: E402
+from helpers import channel_ids  # noqa: E402
 from yt_corpus import make_youtube_config4  # noqa: E402
 
 HBM = 3.35e12  # H100 SXM data sheet
@@ -37,14 +38,6 @@ def appends_call(e, slot):
     if rc:
         raise EngineError(rc, lib().tgi_last_error(e.h).decode())
     return p, ms
-
-
-def channel_ids(batch, yt):
-    out = []
-    for ch in batch.chans:
-        o = int(ch["str_off"]) + (0 if yt else int(ch["title_len"]))
-        out.append(batch.chan_strs[o:o + int(ch["id_len" if yt else "name_len"])].tobytes().decode("utf-8", "surrogateescape"))
-    return out
 
 
 def measure(label, batch, yt, n, reps, tmp):
@@ -81,7 +74,7 @@ def measure(label, batch, yt, n, reps, tmp):
     e.release(0)
     runs = sink.plan_channel_appends(rc.line_off, batch.recs)
     print(f"  groups {p.n_groups} vs tgi_plan_channel_appends runs {len(runs)}: {len(runs) / max(p.n_groups, 1):.1f}x fewer appends")
-    ids = channel_ids(batch, yt)
+    ids = [x.decode("utf-8", "surrogateescape") for x in channel_ids(batch, yt)]
     walls = {}
     for way in ("runs", "grouped", "runs", "grouped"):
         d = tempfile.mkdtemp(dir=tmp)
