@@ -339,6 +339,7 @@ def youtube_post_line(v, ch, *, crawl_label=b"", created=(1_750_000_000, 0), cap
     churl = (b"https://www.youtube.com/" if chid[:1] == b"@" else b"https://www.youtube.com/channel/") + chid
     # int(LikeCount + CommentCount + ViewCount/100): Go's integer division truncates toward zero (:561)
     engagement = v.like_count + v.comment_count + (abs(v.view_count) // 100) * (1 if v.view_count >= 0 else -1)
+    engagement = (engagement + 2 ** 63) % 2 ** 64 - 2 ** 63  # an int64 sum in Go: wraps
     th = {k: _bs(x) for k, x in v.thumbnails.items()}
     thumb = b""
     for k in ("maxres", "high", "medium", "default"):
