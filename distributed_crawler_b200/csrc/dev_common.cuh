@@ -288,6 +288,49 @@ __device__ __noinline__ uint32_t warp_esc_len(const uint8_t* s, int64_t n, bool*
   return warp_sum(tot);
 }
 
+// ---- a message text measured 16 bytes per lane (the link count of the parse kernels, tg_links.cuh) ----------------
+// A text is "clean" when it is valid UTF-8 without C0/C1, bytes >= 0xF4 or E2 80 (U+2000..U+203F, which holds
+// U+2028/9): every strip of it takes warp_load_strip's fast path, warp_esc_len reports no exact path, and its
+// escaped length is n + #('"', '\\', \b \t \n \f \r) + 5 * #(other bytes < 0x20, '<', '>', '&').  The test is
+// stricter than warp_load_strip (it also rejects valid F4 sequences and every E2 80 xx), never looser.
+
+// bit 7 of every byte of w that makes the text not clean; pw = the 4 bytes in front of w (bytes past the text's end
+// are read as ' ', so a sequence left open at the end is a mismatch)
+DEVI uint32_t utf8_unclean4(uint32_t pw, uint32_t w) {
+  const uint32_t M = 0x80808080u;
+  const uint32_t p1 = __funnelshift_l(pw, w, 8), p2 = __funnelshift_l(pw, w, 16), p3 = __funnelshift_l(pw, w, 24);
+  const uint32_t cont = w & ~(w << 1);  // 10xxxxxx
+  const uint32_t due = (p1 & (p1 << 1)) | (p2 & (p2 << 1) & (p2 << 2)) | (p3 & (p3 << 1) & (p3 << 2) & (p3 << 3));
+  uint32_t bad = (cont ^ due) | (((w & 0x7F7F7F7Fu) + 0x0C0C0C0Cu) & w) | swar_eq(w & 0xFEFEFEFEu, 0xC0);  // >= F4, C0/C1
+  if (p1 & (p1 << 1) & (p1 << 2) & M)  // a 3- or 4-byte lead in front of a byte of w: that byte's range
+    bad |= (swar_eq(p1, 0xE0) & ~(w << 2)) | (swar_eq(p1, 0xED) & (w << 2)) |
+           (swar_eq(p1, 0xF0) & ~((w & 0x30303030u) + 0x70707070u)) | (swar_eq(p1, 0xE2) & swar_eq(w, 0x80));
+  return bad & M;
+}
+
+// escaped length minus 1 summed over the ASCII bytes of w (the other bytes of a clean text are copied as they are)
+DEVI uint32_t esc_extra4(uint32_t w) {
+  // an "any" test: < 0x20, '<' / '>' (0x3C | 2 = 0x3E), '"' / '&' (0x22 | 4 = 0x26), '\\'
+  const uint32_t special = ((w - 0x20202020u) & ~w & 0x80808080u) | swar_has_byte(w | 0x02020202u, 0x3E) |
+                           swar_has_byte(w | 0x04040404u, 0x26) | swar_has_byte(w, 0x5C);
+  if (!special) return 0;
+  uint32_t x = 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const uint32_t b = (w >> (8 * k)) & 0xFF;
+    x += b < 0x80 ? ascii_esc_len(b) - 1u : 0u;
+  }
+  return x;
+}
+
+// w with its bytes k.. read as ' '
+DEVI uint32_t blank_from(uint32_t w, int64_t k) {
+  if (k >= 4) return w;
+  if (k <= 0) return 0x20202020u;
+  const uint32_t lo = (1u << (8 * k)) - 1u;
+  return (w & lo) | (0x20202020u & ~lo);
+}
+
 // ---- single-thread number / time rendering (different lanes render different fields) ------------
 DEVI uint32_t ndigits_u32(uint32_t v) {
   return 1u + (v >= 10u) + (v >= 100u) + (v >= 1000u) + (v >= 10000u) + (v >= 100000u) + (v >= 1000000u) +

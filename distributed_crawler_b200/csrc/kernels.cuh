@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(CTA_THREADS) tg_chan_emit_kernel(TgBatchDev b,
 // ---- parse: status + links + line length ---------------------------------------------------------
 struct ParseOut {
   uint8_t* status;       // [n]
-  uint32_t* linelen;     // [n]
+  uint32_t* linelen;     // [n] line length; until the size pass, the message text's escaped length if the parse measured it
   uint32_t* link_start;  // [n] arena index of the record's first link
   uint32_t* link_count;  // [n]
   uint32_t* xlen;        // [n][8] emitted lengths of the variable pieces (XL_*)
@@ -144,18 +144,20 @@ DEVI TgRecView load_rec_view(const TgBatchDev& b, uint64_t r) {
 }
 
 // One record.  ENTITIES == false: the record has no entities, so the whole UTF-16 offset machinery
-// (warp_utf16_to_bytes, the exact UTF-8 path) is compiled out.
-template <bool ENTITIES>
+// (warp_utf16_to_bytes, the exact UTF-8 path) is compiled out.  MEASURE (JSONL runs of the multi-kernel pipeline): the
+// link count also measures the message text, and linelen[r] carries its escaped length to tg_size_lane_body (0: not
+// measured, the size pass measures it itself).
+template <bool ENTITIES, bool MEASURE = false>
 DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOut& o, uint64_t r, TgRecView v) {
   const int l = lane_id();
-  uint32_t status = TGI_ST_EMITTED, nlinks = 0, lstart = 0;
+  uint32_t status = TGI_ST_EMITTED, nlinks = 0, lstart = 0, text_esc = 0;
   if ((cfg.flags & TGI_CFG_HAS_MIN_POST_DATE) && (int64_t)v.rec->date < cfg.min_post_date) {
     status = TGI_ST_SKIPPED;  // tdutils.go:419-421
   } else if (v.flags & TGI_RF_PANIC) {
     status = TGI_ST_FAILED;
   } else {
     if (!ENTITIES) v.e1 = v.e0;
-    uint32_t ub = warp_link_upper_bound(v, b.ents);
+    uint32_t ub = warp_link_upper_bound<MEASURE>(v, b.ents, text_esc);
     if (ub >= (1u << 20)) {  // seq packing of the frontier needs ordinal < 2^20 (SEQ_ORD_BITS)
       if (l == 0) atomicOr(o.err, ERR_TOO_MANY_LINKS);
       ub = 0;
@@ -185,7 +187,7 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
   }
   if (l == 0) {
     o.status[r] = (uint8_t)status;
-    o.linelen[r] = 0;
+    o.linelen[r] = MEASURE && status == TGI_ST_EMITTED ? text_esc : 0u;  // the size pass overwrites the emitted ones
     o.link_start[r] = lstart;
     o.link_count[r] = nlinks;
   }
@@ -197,6 +199,7 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
 // entities (lanes pick them out of groups of 32), tg_size_lane_kernel = line lengths.  Fusing them was tried twice
 // (one parse kernel; parse + size in ONE pass over the text, fewer instructions in all): both fused kernels stalled on
 // instruction fetch and were slower than the split ones.
+template <bool MEASURE>
 DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_flags, const ParseOut& o) {
   int wid = threadIdx.x >> 5;
   uint64_t nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
@@ -212,14 +215,17 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
       asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(nx_len) : "l"(&b.recs[rn].text_len));
     }
     if (b.ent_off[r + 1] == b.ent_off[r])  // the others: tg_parse_ent_kernel
-      parse_one_record<false>(b, cfg, o, r, load_rec_view(b, r));
+      parse_one_record<false, MEASURE>(b, cfg, o, r, load_rec_view(b, r));
     if (rn < b.n) {
       const uint32_t off = (uint32_t)lane_id() * 128u;
       if (off < nx_len + 127u && off < 2048u) asm volatile("prefetch.global.L1 [%0];" ::"l"(b.strs + nx_off + off));
     }
   }
 }
-__global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_kernel(TgBatchDev b, CfgDev cfg, uint32_t run_flags, ParseOut o) { tg_parse_body(b, cfg, run_flags, o); }
+template <bool MEASURE>
+__global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_kernel(TgBatchDev b, CfgDev cfg, uint32_t run_flags, ParseOut o) {
+  tg_parse_body<MEASURE>(b, cfg, run_flags, o);
+}
 DEVI void tg_ent_map_body(const TgBatchDev& b, const ParseOut& o) {
   const int wid = threadIdx.x >> 5, l = lane_id();
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
@@ -234,6 +240,7 @@ DEVI void tg_ent_map_body(const TgBatchDev& b, const ParseOut& o) {
   }
 }
 __global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_ent_map_kernel(TgBatchDev b, ParseOut o) { tg_ent_map_body(b, o); }
+template <bool MEASURE>
 DEVI void tg_parse_ent_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_flags, const ParseOut& o) {
   const int wid = threadIdx.x >> 5, l = lane_id();
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
@@ -243,18 +250,19 @@ DEVI void tg_parse_ent_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run
     while (todo) {
       const uint64_t r = g * 32 + (uint32_t)(__ffs(todo) - 1);
       todo &= todo - 1;
-      parse_one_record<true>(b, cfg, o, r, load_rec_view(b, r));
+      parse_one_record<true, MEASURE>(b, cfg, o, r, load_rec_view(b, r));
     }
   }
 }
+template <bool MEASURE>
 __global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_ent_kernel(TgBatchDev b, CfgDev cfg, uint32_t run_flags, ParseOut o) {
-  tg_parse_ent_body(b, cfg, run_flags, o);
+  tg_parse_ent_body<MEASURE>(b, cfg, run_flags, o);
 }
 
 // The same sizes, 32 records per warp: every lane sizes the small pieces of its own record (numbers,
-// handle / media strings, comments, reactions, outlinks); only the message text, the one long string,
-// is measured by the whole warp, record after record; the rare complicated pieces (a comment list, a
-// reactions map that is not "simple") go through the warp-wide routines as well.
+// handle / media strings, comments, reactions, outlinks); the description, the one long string, is measured by the
+// whole warp, record after record, unless it is a message text the parse already measured (linelen); the rare
+// complicated pieces (a comment list, a reactions map that is not "simple") go through the warp-wide routines as well.
 DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseOut& o) {
   const int wid = threadIdx.x >> 5, l = lane_id();
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
@@ -279,6 +287,10 @@ DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseO
     uint32_t tot = 0;
     bool warp_comments = false, warp_map = false;
     const uint32_t r0 = b.react_off[r], nr = b.react_off[r + 1] - r0;
+    // the parse's measurement (parse_one_record), != 0 only for a text of >= 1 byte: then alt != text, and d.desc == text
+    // says the description is the message text
+    const uint32_t text_esc = active ? o.linelen[r] : 0u;
+    const bool measured = text_esc != 0 && d.desc == a.v.text;
     if (active && !(cfg.flags & CFGDEV_CLOCK_INVALID)) {
       uint32_t L[8] = {ndigits_i64(rec->id / 1048576), ndigits_i64(rec->chat_id), ndigits_i64(rec->view_count),
                        ndigits_i64(rec->share_count), ndigits_i64(d.ncomments), cfg.tz == 0 ? 22u : 27u, 0, 0};
@@ -286,6 +298,7 @@ DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseO
       uint32_t cf[4] = {cfg.label_len, cfg.created_tg_len, cfg.created_yt_len, cfg.capture_len};
       tot = tg_size_fixed(L, chan, cf, d.has_user, d.album);
       tot += a.v.ct == TGI_CT_OTHER ? 0u : (uint32_t)kPostTypeLen[a.v.ct];
+      if (measured) xl[XL_DESC] = text_esc;
       if (a.v.ct == TGI_CT_OTHER) xl[XL_ALT] = thread_esc_len(a.v.alt, a.v.alt_len);
       if (d.has_media) xl[XL_MEDIA] = thread_esc_len(a.v.media, a.v.media_len);
       xl[XL_HANDLE] = thread_esc_len(a.v.handle, a.v.handle_len);
@@ -328,9 +341,9 @@ DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseO
         xl[XL_OUTLINKS] = s;
       }
     }
-    // the message text (or the other description sources), one record at a time, all lanes
+    // the other descriptions (and the texts the parse did not measure), one record at a time, all lanes
     const bool sized = active && !(cfg.flags & CFGDEV_CLOCK_INVALID);
-    uint32_t todo = __ballot_sync(FULL, sized && d.desc_len != 0);
+    uint32_t todo = __ballot_sync(FULL, sized && d.desc_len != 0 && !measured);
     while (todo) {
       const int src = __ffs(todo) - 1;
       todo &= todo - 1;

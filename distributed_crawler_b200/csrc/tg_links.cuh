@@ -96,11 +96,9 @@ DEVI uint32_t warp_word_run(const uint8_t* p, const uint8_t* end) {
 // A strip for the link scan = 512 bytes, 16 per lane (no UTF-8 bookkeeping is needed to find "t.me/").
 // Returns the lane's 16-bit mask: bit k set if s[p0+k] is the '/' of a "t.me/" (p0 = base + 16*lane).
 // '/' is rare in message text, so almost every strip ends after four SWAR compares per lane.
-DEVI uint32_t strip16_tme(const uint8_t* s, int64_t base, int64_t n) {
-  const int64_t p0 = base + 16 * lane_id();
-  if (p0 >= n) return 0;
+// tme16 computes it from the lane's bytes w = s[p0..p0+16), p0 < n.
+DEVI uint32_t tme16(const uint8_t* s, int64_t p0, int64_t n, const uint4 w) {
   const uint8_t* q = s + p0;
-  const uint4 w = ld16_unaligned(q);
   const uint32_t s0 = swar_eq(w.x, '/'), s1 = swar_eq(w.y, '/'), s2 = swar_eq(w.z, '/'), s3 = swar_eq(w.w, '/');
   if (!(s0 | s1 | s2 | s3)) return 0;
   uint32_t m = swar_movemask(s0) | (swar_movemask(s1) << 4) | (swar_movemask(s2) << 8) | (swar_movemask(s3) << 12);
@@ -113,6 +111,11 @@ DEVI uint32_t strip16_tme(const uint8_t* s, int64_t base, int64_t n) {
     if (p0 + k >= 4 && ld_u32_unaligned(q + k - 4) == 0x656D2E74u) out |= 1u << k;  // "t.me"
   }
   return out;
+}
+DEVI uint32_t strip16_tme(const uint8_t* s, int64_t base, int64_t n) {
+  const int64_t p0 = base + 16 * lane_id();
+  if (p0 >= n) return 0;
+  return tme16(s, p0, n, ld16_unaligned(s + p0));
 }
 
 // index of the first byte >= 0x80 of s[0..n), n if there is none.  In front of it UTF-16 offsets are byte offsets.
@@ -140,6 +143,39 @@ DEVI int64_t warp_first_non_ascii(const uint8_t* s, int64_t n) {
 DEVI uint32_t warp_count_tme(const uint8_t* s, int64_t n) {
   uint32_t cnt = 0;
   for (int64_t base = 0; base < n; base += 512) cnt += __popc(strip16_tme(s, base, n));
+  return warp_sum(cnt);
+}
+
+// The same count, and the text measured from the same 16 bytes per lane (JSONL runs): esc_len = its JSON-escaped length
+// if it is clean (utf8_unclean4), 0 if not (or if n == 0).  The lane's 4 bytes in front come from the lane below, or
+// for lane 0 from the previous strip's last lane.
+DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len) {
+  const int l = lane_id();
+  const uint32_t SP = 0x20202020u;
+  uint32_t cnt = 0, extra = 0, bad = 0, tail = SP;  // tail: the last 4 bytes of the previous strip
+  for (int64_t base = 0; base < n; base += 512) {
+    const int64_t p0 = base + 16 * l, rem = n - p0;
+    uint4 w = make_uint4(SP, SP, SP, SP);
+    if (rem > 0) {
+      w = ld16_unaligned(s + p0);
+      cnt += __popc(tme16(s, p0, n, w));
+      if (rem < 16) w = make_uint4(blank_from(w.x, rem), blank_from(w.y, rem - 4), blank_from(w.z, rem - 8), blank_from(w.w, rem - 12));
+    }
+    const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
+    uint32_t pw = l == 0 ? tail : below;
+    tail = __shfl_sync(FULL, w.w, 31);
+    const bool ascii = ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) == 0;
+#pragma unroll 1
+    for (int k = 0; k < 4; k++) {  // a word at a time: the parse kernels' code has to stay small (instruction cache)
+      if (!ascii) bad |= utf8_unclean4(pw, w.x);
+      extra += esc_extra4(w.x);
+      pw = w.x;
+      w = make_uint4(w.y, w.z, w.w, w.x);
+    }
+  }
+  bad |= utf8_unclean4(tail, SP);  // a text that ends with its last strip: a sequence open at the end
+  const uint32_t e = (uint32_t)n + warp_sum(extra);
+  esc_len = __any_sync(FULL, bad != 0) ? 0u : e;
   return warp_sum(cnt);
 }
 
@@ -268,12 +304,15 @@ DEVI bool ct_carries_links(uint32_t ct) {  // extractFormattedTextFromMessage td
          ct == TGI_CT_ANIMATION || ct == TGI_CT_AUDIO || ct == TGI_CT_VOICE_NOTE;
 }
 
-// upper bound on the number of links of this record (entities of the three kinds + "t.me/" hits)
-DEVI uint32_t warp_link_upper_bound(const TgRecView& v, const tgi_entity* ents) {
+// upper bound on the number of links of this record (entities of the three kinds + "t.me/" hits).  MEASURE: text_esc =
+// the text's escaped length if the count found it clean, else 0 (warp_count_tme_esc); 0 for a record it does not scan.
+template <bool MEASURE>
+DEVI uint32_t warp_link_upper_bound(const TgRecView& v, const tgi_entity* ents, uint32_t& text_esc) {
+  text_esc = 0;
   if (!ct_carries_links(v.ct) || !(v.flags & TGI_RF_HAS_TEXT)) return 0;
   uint32_t c = 0;
   for (uint32_t e = v.e0 + lane_id(); e < v.e1; e += 32) c += ents[e].type != TGI_ENT_OTHER;
-  return warp_sum(c) + warp_count_tme(v.text, v.text_len);
+  return warp_sum(c) + (MEASURE ? warp_count_tme_esc(v.text, v.text_len, text_esc) : warp_count_tme(v.text, v.text_len));
 }
 
 // utf16OffsetToBytes for every mention / url entity of the record -> ranges[e - v.e0... absolute e] = (start, end)

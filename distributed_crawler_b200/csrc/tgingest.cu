@@ -693,6 +693,9 @@ constexpr uint64_t PAGE_MAX_IN_BYTES = 4u << 20;
 bool page_enabled() {
   return getenv("TGI_NO_PAGE") == nullptr;  // A/B switch (read per call): the ordinary pipeline for every size
 }
+bool size_text_in_parse() {
+  return getenv("TGI_SIZE_TEXT_WARP") == nullptr;  // A/B switch (read per call): the size pass measures every text itself
+}
 // the size rule of the page kernels, for packing the input and for running it
 bool page_fits(uint64_t n, uint64_t n_chans, uint64_t in_bytes) {
   return page_enabled() && n && n <= PAGE_MAX_RECS && n_chans <= PAGE_MAX_RECS && in_bytes <= PAGE_MAX_IN_BYTES;
@@ -1286,12 +1289,17 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       CK(cudaEventRecord(s.ev_p0, st));
       const uint64_t groups = (n + 31) / 32;
       unsigned ge = (unsigned)std::min<uint64_t>((groups + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
+      // JSONL: the link count measures the message texts as well (the size pass then skips the clean ones); runs without
+      // JSONL take the instances without that code
+      const bool measure = want_json && size_text_in_parse();
       if (s.n_ents) {  // records with entities first: status + links (two kernels by instruction footprint)
         tg_ent_map_kernel<<<ge, CTA_THREADS, 0, st>>>(b, po);
-        tg_parse_ent_kernel<<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
+        if (measure) tg_parse_ent_kernel<true><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
+        else tg_parse_ent_kernel<false><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
         launches += 2;
       }
-      tg_parse_kernel<<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, po);  // records without entities
+      if (measure) tg_parse_kernel<true><<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, po);  // records without entities
+      else tg_parse_kernel<false><<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
       launches++;
       if (want_json) {
         tg_size_lane_kernel<<<ge, CTA_THREADS, 0, st>>>(b, cfg, po);

@@ -385,7 +385,9 @@ int tgi_set_clock(tgi_ctx* ctx, int64_t created_at_sec, int32_t created_at_nsec,
  * Diagnostics (environment, read per call or at first use; none changes results): TGI_NO_PAGE=1 the
  * multi-kernel pipeline for every size; TGI_PAGE_TRACE=1 phase clock of the page kernels on
  * stderr; TGI_TRACE_SLOTS=1 host-side timeline of the slots' synchronisation points;
- * TGI_GRID_MULT / TGI_LANE_MULT grid sizes in CTAs per SM (defaults 128 / 24).                    */
+ * TGI_GRID_MULT / TGI_LANE_MULT grid sizes in CTAs per SM (defaults 128 / 24); TGI_SIZE_TEXT_WARP=1
+ * the multi-kernel pipeline's parse leaves the message texts unmeasured and the size pass measures
+ * every one of them (the path before the parse measured them).                                    */
 #define TGI_SLOTS 3
 int tgi_telegram_submit(tgi_ctx* ctx, int slot, const tgi_tg_batch* in, uint32_t run_flags);
 int tgi_telegram_wait(tgi_ctx* ctx, int slot, tgi_result* out);
