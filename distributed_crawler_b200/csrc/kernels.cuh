@@ -1281,10 +1281,7 @@ __global__ void filter_usernames_kernel(const uint8_t* names, const uint32_t* of
   int l = lane_id();
   uint32_t a = off[i], len = off[i + 1] - a;
   uint32_t c = ((uint32_t)l < len) ? ldb(names + a + l) : 0u;
-  uint32_t res = warp_filter_username(c, len);
-  if (res == TGI_FU_INVALID_CHAR || res == TGI_FU_VALID || res == TGI_FU_BOT_SUFFIX) {
-    // names longer than a warp cannot reach here (len > 32 -> too_long)
-  }
+  uint32_t res = warp_filter_username(c, len);  // names longer than a warp stop at too_long
   if (l == 0) reason[i] = (uint8_t)res;
 }
 

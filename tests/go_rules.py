@@ -91,10 +91,12 @@ _RESERVED = {b"joinchat", b"addlist", b"addstickers", b"addtheme", b"setlanguage
              b"iv", b"proxy", b"socks", b"login", b"confirm", b"bg"}
 
 
-def extract_links(text: bytes | None, entities, aux_urls=None):
+def extract_links(text: bytes | None, entities, aux_urls=None, utf16=None):
     """tdutils.go:897-949 with python's `re` standing in for Go's regexp (both leftmost, greedy; the
     patterns have no alternation whose priority could differ).  Returns [(name, src)] in first-
-    insertion order, or None where Go would panic."""
+    insertion order, or None where Go would panic.  utf16(text, off, len) replaces utf16_offset_to_bytes
+    (a table lookup for callers that map many entities over one text)."""
+    utf16 = utf16 or utf16_offset_to_bytes
     out, seen = [], set()
 
     def add(name, src):
@@ -113,7 +115,7 @@ def extract_links(text: bytes | None, entities, aux_urls=None):
         if typ == "text_url":
             chan(_CHANNEL_RE.search(url.encode() if isinstance(url, str) else url), "text_url")
         elif typ in ("mention", "url"):
-            st, en = utf16_offset_to_bytes(text, off, ln)
+            st, en = utf16(text, off, ln)
             if st < en and en <= len(text):
                 if st < 0:
                     return None
