@@ -38,6 +38,7 @@ CFG_HAS_MIN_POST_DATE, CFG_SKIP_MEDIA = 1, 2
 RUN_JSONL, RUN_LINKS, RUN_FRONTIER, RUN_FILTER, RUN_SKIP_SELF, RUN_NO_D2H = 1, 2, 4, 8, 16, 32
 LF_FILTER_OK, LF_NEW, LF_SELF = 1, 2, 4
 SLOTS = 3
+ZONE_MAX = 4096  # entries of a tgi_set_zone table
 YT_THUMB_ABSENT = 0xFFFF
 YT_THUMB_KEYS = ["default", "medium", "high", "standard", "maxres"]
 

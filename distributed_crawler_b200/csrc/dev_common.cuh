@@ -449,6 +449,38 @@ __device__ __noinline__ int render_time(uint8_t* dst, int64_t sec, int32_t nsec,
   return o;
 }
 
+// ---- the local zone as a transition table (tgi_set_zone) -----------------------------------------
+struct ZoneEnt {  // 16 bytes, so one probe is one load
+  int64_t start;  // first instant (unix seconds) of this offset
+  int32_t off;    // seconds east of UTC
+  int32_t pad;
+};
+// offset of the last entry with start <= t; entry 0 before the first start.  n >= 1.
+__device__ __noinline__ int32_t zone_lookup(const ZoneEnt* z, uint32_t n, int64_t t) {
+  uint32_t lo = 0;
+  int32_t off = __ldg(&z[0].off);
+  while (n > 1) {
+    const uint32_t half = n >> 1;
+    const longlong2 e = __ldg((const longlong2*)(z + lo + half));
+    if (e.x <= t) {
+      lo += half;
+      off = (int32_t)e.y;
+    }
+    n -= half;
+  }
+  return off;
+}
+// time.Time.MarshalJSON in the zone z[n], or at the fixed offset tz when n == 0 (render_time as it is).  In a zone the
+// offset suffix follows Go's appendFormatRFC3339: minutes = offset / 60 truncated, signed by the minutes, so an offset
+// of -1..-59 s is "+00:00" where the fixed-offset rule writes "-00:00".  Every other offset renders the same either way.
+__device__ __noinline__ int render_zone_time(uint8_t* dst, int64_t sec, int32_t nsec, const ZoneEnt* z, uint32_t n, int32_t tz) {
+  if (n == 0) return render_time(dst, sec, nsec, tz);
+  const int32_t off = zone_lookup(z, n, sec);
+  const int o = render_time(dst, sec, nsec, off);
+  if (o && off < 0 && off > -60) dst[o - 7] = '+';  // "-00:00\"" -> "+00:00\""
+  return o;
+}
+
 // ---- shared-memory access by 32-bit shared-space address ------------------------------------------
 DEVI uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 DEVI void sts8(uint32_t a, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(a), "r"(v)); }

@@ -27,7 +27,7 @@ DEVI bool walk_gm_record(W& w, const GmBatchDev& b, const CfgDev& cfg, uint64_t 
   const int l = lane_id();
   uint32_t tl = 0;
   __syncwarp();
-  if (l == 0) tl = (uint32_t)render_time(w.sc->num, v.ts_sec, v.ts_nsec, cfg.tz);  // :187 GetTimestamp()
+  if (l == 0) tl = (uint32_t)render_zone_time(w.sc->num, v.ts_sec, v.ts_nsec, cfg.zone, cfg.zone_n, cfg.tz);  // :187 GetTimestamp()
   __syncwarp();
   const uint32_t pub_len = __shfl_sync(FULL, tl, 0);
   if (pub_len == 0 || (cfg.flags & CFGDEV_CLOCK_INVALID) || cfg.created_yt_len == 0) return false;

@@ -293,7 +293,7 @@ DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseO
     const bool measured = text_esc != 0 && d.desc == a.v.text;
     if (active && !(cfg.flags & CFGDEV_CLOCK_INVALID)) {
       uint32_t L[8] = {ndigits_i64(rec->id / 1048576), ndigits_i64(rec->chat_id), ndigits_i64(rec->view_count),
-                       ndigits_i64(rec->share_count), ndigits_i64(d.ncomments), cfg.tz == 0 ? 22u : 27u, 0, 0};
+                       ndigits_i64(rec->share_count), ndigits_i64(d.ncomments), zone_offset(cfg, rec->date) == 0 ? 22u : 27u, 0, 0};
       uint32_t chan[4] = {cd.user_len, cd.name_len, cd.title_len, cd.cdata_len};
       uint32_t cf[4] = {cfg.label_len, cfg.created_tg_len, cfg.created_yt_len, cfg.capture_len};
       tot = tg_size_fixed(L, chan, cf, d.has_user, d.album);

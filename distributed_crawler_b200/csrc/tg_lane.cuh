@@ -243,7 +243,7 @@ DEVI void emit_tg_lane(LaneShared& sh, uint32_t* row, LaneStream& s, const TgBat
     const uint32_t fo = f ? 16u + (f >= 2 ? 16u * f : 0u) : 0u;
     rb[128 + f] = (uint8_t)render_i64(rb + fo, v);
   }
-  rb[128 + F_TIME] = (uint8_t)render_time(rb + 96, rec->date, 0, cfg.tz);  // tdutils.go:417
+  rb[128 + F_TIME] = (uint8_t)render_zone_time(rb + 96, rec->date, 0, cfg.zone, cfg.zone_n, cfg.tz);  // tdutils.go:417
 
   const uint64_t line_start = (uint64_t)(uintptr_t)out + line_off[r];
   const uint32_t total = (uint32_t)(line_off[r + 1] - line_off[r]);

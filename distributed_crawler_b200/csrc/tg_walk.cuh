@@ -54,8 +54,13 @@ struct CfgDev {             // per-context constants in a small device blob
   uint32_t flags;           // TGI_CFG_*; bit 31: injected clock not representable (Marshal error)
   int32_t tz;
   int64_t min_post_date;
+  const ZoneEnt* zone;      // tgi_set_zone: the local zone's transitions, replacing tz while zone_n != 0
+  uint32_t zone_n;
 };
 #define CFGDEV_CLOCK_INVALID 0x80000000u
+
+// offset of the local zone at instant t: the one rule behind both the size and the bytes of a zoned time field
+DEVI int32_t zone_offset(const CfgDev& cfg, int64_t t) { return cfg.zone_n ? zone_lookup(cfg.zone, cfg.zone_n, t) : cfg.tz; }
 
 __device__ const char kPostType[TGI_CT__COUNT][28] = {
     "unknown",          "messageText",          "messageVideo",           "messagePhoto",
@@ -493,7 +498,7 @@ DEVI uint32_t size_tg_record(const TgWalkArgs& a, uint32_t* xl) {
   if (cfg.flags & CFGDEV_CLOCK_INVALID) return 0;
   // int32 dates are always inside year [0,9999]: RFC3339 with quotes, 'Z' or a +hh:mm offset
   uint32_t L[8] = {ndigits_i64(rec->id / 1048576), ndigits_i64(rec->chat_id), ndigits_i64(rec->view_count),
-                   ndigits_i64(rec->share_count), ndigits_i64(d.ncomments), cfg.tz == 0 ? 22u : 27u, 0, 0};
+                   ndigits_i64(rec->share_count), ndigits_i64(d.ncomments), zone_offset(cfg, rec->date) == 0 ? 22u : 27u, 0, 0};
   uint32_t chan[4] = {cd.user_len, cd.name_len, cd.title_len, cd.cdata_len};
   uint32_t cf[4] = {cfg.label_len, cfg.created_tg_len, cfg.created_yt_len, cfg.capture_len};
   uint32_t tot = tg_size_fixed(L, chan, cf, d.has_user, d.album);
@@ -527,7 +532,7 @@ DEVI void emit_tg_prologue(WarpScratch* ws, const TgWalkArgs& a, const ChanDeriv
                                          : l == 3 ? (int64_t)rec->share_count : d.ncomments;
     ws->flen[l] = (uint32_t)render_i64(ws->field[l], v);
   } else if (l == 5) {
-    ws->flen[5] = (uint32_t)render_time(ws->field[5], rec->date, 0, cfg.tz);  // :417
+    ws->flen[5] = (uint32_t)render_zone_time(ws->field[5], rec->date, 0, cfg.zone, cfg.zone_n, cfg.tz);  // :417
   } else if (l == 6) {  // MessageContentType() string (28-byte rows, 4-byte aligned)
     const uint32_t* src = (const uint32_t*)kPostType[a.v.ct];
     uint32_t* dst = (uint32_t*)ws->field[F_POSTTYPE];

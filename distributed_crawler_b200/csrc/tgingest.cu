@@ -237,6 +237,8 @@ struct tgi_ctx {
   DevBuf d_cfg;
   CfgDev cfgdev{};
   std::mutex cfg_mu;
+  std::vector<ZoneEnt> zone;  // tgi_set_zone (empty: tz_offset_sec) and its device copy
+  DevBuf d_zone;
   // the resident key sets, indexed by TGI_SET_*: the dedup set (every key this GPU has seen), the exclusion sets of the
   // frontier -> validator hand-off (tgi_set_add) and this rank's partition of the multi-GPU set (tgi_comm_init)
   KeySet sets[4];
@@ -346,6 +348,15 @@ int host_render_time(char* dst, int64_t sec, int32_t nsec, int32_t tz) {
   dst[o++] = '"';
   return o;
 }
+// the same in the zone table z (render_zone_time on the device); an empty table is the fixed offset tz
+int host_render_zone_time(char* dst, int64_t sec, int32_t nsec, const std::vector<ZoneEnt>& z, int32_t tz) {
+  if (z.empty()) return host_render_time(dst, sec, nsec, tz);
+  const auto it = std::upper_bound(z.begin(), z.end(), sec, [](int64_t t, const ZoneEnt& e) { return t < e.start; });
+  const int32_t off = (it == z.begin() ? z.front() : it[-1]).off;
+  const int o = host_render_time(dst, sec, nsec, off);
+  if (o && off < 0 && off > -60) dst[o - 7] = '+';
+  return o;
+}
 
 // Builds the per-context constant blob (escaped label + clock strings) and uploads it.  The label
 // is JSON-escaped ON THE DEVICE by the same Emitter code that escapes everything else.
@@ -359,8 +370,8 @@ int build_cfg_blob(tgi_ctx* c) {
   const tgi_config& cfg = c->cfg;
   char t_tg[48], t_yt[48], t_cap[48];
   int n_tg = host_render_time(t_tg, cfg.created_at_sec, 0, 0);
-  int n_yt = host_render_time(t_yt, cfg.created_at_sec, cfg.created_at_nsec, cfg.tz_offset_sec);
-  int n_cap = host_render_time(t_cap, cfg.capture_sec, cfg.capture_nsec, cfg.tz_offset_sec);
+  int n_yt = host_render_zone_time(t_yt, cfg.created_at_sec, cfg.created_at_nsec, c->zone, cfg.tz_offset_sec);
+  int n_cap = host_render_zone_time(t_cap, cfg.capture_sec, cfg.capture_nsec, c->zone, cfg.tz_offset_sec);
   cudaStream_t s = c->slots[0].stream;
   uint32_t n = (uint32_t)c->label.size();
   DevBuf raw, len;
@@ -398,6 +409,8 @@ int build_cfg_blob(tgi_ctx* c) {
   d.flags = cfg.flags | ((n_tg == 0 || n_cap == 0) ? CFGDEV_CLOCK_INVALID : 0);
   d.tz = cfg.tz_offset_sec;
   d.min_post_date = cfg.min_post_date;
+  d.zone = c->zone.empty() ? nullptr : c->d_zone.as<ZoneEnt>();
+  d.zone_n = (uint32_t)c->zone.size();
   c->cfgdev = d;
   return TGI_OK;
 }
@@ -1932,6 +1945,35 @@ int tgi_set_clock(tgi_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, i
   c->cfg.capture_sec = capture_sec;
   c->cfg.capture_nsec = capture_nsec;
   return build_cfg_blob(c);
+}
+
+int tgi_set_zone(tgi_ctx* c, const int64_t* start_sec, const int32_t* offset_sec, uint32_t n) {
+  if (!c) return TGI_E_ARG;
+  if (n > TGI_ZONE_MAX) { set_err(c, "tgi_set_zone: %u entries (at most %d)", n, TGI_ZONE_MAX); return TGI_E_ARG; }
+  if (n && (!start_sec || !offset_sec)) { set_err(c, "tgi_set_zone: NULL table"); return TGI_E_ARG; }
+  std::vector<ZoneEnt> z(n);
+  for (uint32_t i = 0; i < n; i++) {
+    if (offset_sec[i] <= -86400 || offset_sec[i] >= 86400) { set_err(c, "tgi_set_zone: offset %d of entry %u is a day or more", offset_sec[i], i); return TGI_E_ARG; }
+    if (i && start_sec[i] <= start_sec[i - 1]) { set_err(c, "tgi_set_zone: start of entry %u is not after entry %u", i, i - 1); return TGI_E_ARG; }
+    z[i] = ZoneEnt{start_sec[i], offset_sec[i], 0};
+  }
+  cudaSetDevice(c->device);
+  if (const int i = slot_in_flight(c); i >= 0) { set_err(c, "tgi_set_zone while slot %d is in flight", i); return TGI_E_STATE; }
+  DevBuf d;
+  if (n) {
+    CK(d.ensure(n * sizeof(ZoneEnt)));
+    CK(cudaMemcpy(d.p, z.data(), n * sizeof(ZoneEnt), cudaMemcpyHostToDevice));
+  }
+  std::lock_guard<std::mutex> g(c->cfg_mu);
+  c->zone.swap(z);
+  c->d_zone.swap(d);
+  const int rc = build_cfg_blob(c);
+  if (rc) {  // the previous table stays in effect
+    c->zone.swap(z);
+    c->d_zone.swap(d);
+    build_cfg_blob(c);
+  }
+  return rc;
 }
 
 int tgi_telegram_submit(tgi_ctx* c, int slot, const tgi_tg_batch* in, uint32_t run_flags) {

@@ -36,7 +36,7 @@ EXPORTED_SYMBOLS = [
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
     "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
-    "tgi_combine_flush", "tgi_channel_appends",
+    "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone",
 ]
 
 
@@ -103,6 +103,7 @@ def lib() -> C.CDLL:
         L.tgi_combine_add.argtypes = [vp, i32, C.c_int64, C.POINTER(abi.CombinedC)]
         L.tgi_combine_flush.argtypes = [vp, C.c_int64, C.POINTER(abi.CombinedC)]
         L.tgi_channel_appends.argtypes = [vp, i32, C.POINTER(abi.ChannelAppendsC)]
+        L.tgi_set_zone.argtypes = [vp, vp, vp, u32]
         _LIB = L
     return _LIB
 
@@ -270,6 +271,15 @@ class Engine:
 
     def set_clock(self, created_at_sec, created_at_nsec, capture_sec, capture_nsec):
         self._check(lib().tgi_set_clock(self.h, created_at_sec, created_at_nsec, capture_sec, capture_nsec))
+
+    def set_zone(self, starts, offsets):
+        """the local zone as transitions (tgi_set_zone): instant t takes offsets[i] of the last starts[i] <= t; an empty
+        table goes back to the fixed tz_offset_sec"""
+        s = np.ascontiguousarray(starts, np.int64)
+        o = np.ascontiguousarray(offsets, np.int32)
+        if len(s) != len(o):
+            raise ValueError("starts and offsets differ in length")
+        self._check(lib().tgi_set_zone(self.h, s.ctypes.data if len(s) else None, o.ctypes.data if len(o) else None, len(s)))
 
     # --- Telegram -------------------------------------------------------------------------------
     def telegram(self, batch, run_flags=abi.RUN_JSONL | abi.RUN_LINKS, copy=True) -> Result:

@@ -262,6 +262,13 @@ class MessageProcessor {
   void SetClock(int64_t created_sec, int32_t created_nsec, int64_t capture_sec, int32_t capture_nsec) {
     tgi_set_clock(ctx_, created_sec, created_nsec, capture_sec, capture_nsec);
   }
+  // time.Local as transitions (tgi_set_zone): instant t takes offset_sec[i] of the last start_sec[i] <= t; empty
+  // vectors go back to Config::TzOffsetSec.
+  void SetZone(const std::vector<int64_t>& start_sec, const std::vector<int32_t>& offset_sec) {
+    if (start_sec.size() != offset_sec.size()) throw std::invalid_argument("SetZone: starts and offsets differ in length");
+    if (tgi_set_zone(ctx_, start_sec.data(), offset_sec.data(), (uint32_t)start_sec.size()) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+  }
   // Lets the resident sets grow on demand up to max_keys keys each, like the reference's maps (0: fixed capacity).
   void SetGrowth(uint64_t max_keys) {
     if (tgi_set_growth(ctx_, max_keys) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));

@@ -363,6 +363,30 @@ void tgi_get_stats(tgi_ctx* ctx, tgi_stats* out);
 int tgi_set_clock(tgi_ctx* ctx, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec,
                   int32_t capture_nsec);
 
+/* The local zone with its transitions — time.Local of a natively built crawler is the host's zone (e.g.
+ * America/New_York, with DST), which tz_offset_sec can only model as one fixed offset.  The table is n entries;
+ * start_sec is strictly increasing, and instant t is shown at offset_sec[i] of the last entry with start_sec[i] <= t
+ * (entry 0 before start_sec[0]).  While a table is set it replaces tz_offset_sec everywhere time.Local is used:
+ * Telegram published_at (time.Unix(message.Date, 0), tdutils.go:417) and generic published_at (GetTimestamp()) per
+ * record; YouTube and generic created_at and every capture_time, rendered at tgi_create / tgi_set_clock /
+ * tgi_set_zone.  Telegram created_at stays UTC (tdutils.go:611) and YouTube published_at keeps the zone of the API
+ * value (UTC).
+ *   Format   Go's appendFormatRFC3339 / appendStrictRFC3339: the local fields come from t + offset, seconds of the offset
+ *            included; 'Z' only when the offset is exactly 0; otherwise minutes = offset / 60 truncated toward zero and
+ *            the sign is that of the minutes (-30 s is "+00:00", -75 s is "-00:01", +00:19:32 is "+00:19").  A local year
+ *            outside [0, 9999] is TGI_ST_NOLINE, with the offset in effect at that record.  Zones whose offset is 0 for
+ *            part of the year (Europe/London) change the line length with it: line_off and the sinks follow.
+ *   Clearing n == 0 removes the table: tz_offset_sec applies again, byte for byte as without a table.
+ *   Errors   TGI_E_STATE while a job is in flight on any slot (as tgi_set_clock).  TGI_E_ARG: a NULL array with n > 0,
+ *            starts that are not strictly increasing, |offset| >= 86400, or n > TGI_ZONE_MAX.  A rejected call leaves
+ *            the previous table in effect.
+ *   Go shim  LocalZoneTable() (INTEGRATION.md) walks time.Local with Time.ZoneBounds() from time.Unix(math.MinInt32, 0)
+ *            (Telegram's Date is an int32) to a horizon, one entry per zone period, and calls tgi_set_zone once after
+ *            tgi_create.  Beyond the horizon the last entry applies, so int64 generic timestamps past it are exact only
+ *            up to the horizon.  Every tzdata zone has a few hundred transitions over that range.                  */
+#define TGI_ZONE_MAX 4096
+int tgi_set_zone(tgi_ctx* ctx, const int64_t* start_sec, const int32_t* offset_sec, uint32_t n);
+
 /* Telegram: replaces the loop body crawl/runner.go:1161-1244 -> processMessage (:1720) ->
  * telegramhelper.ParseMessage (tdutils.go:380-732) -> extractChannelLinksFromMessage (:989) ->
  * json.Marshal+'\n' (state/storageproviders.go:276-282, state/daprstate.go:1118-1120) for a whole
