@@ -175,6 +175,23 @@ class ChannelAppendsC(C.Structure):  # tgi_channel_appends_t
                 ("order", C.c_void_p), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+# crawl progress state (tgi_state_*)
+STATE_NO_PAGE = 0xFFFFFFFF
+STATE_TS_LOCAL = 0x7FFFFFFF  # tgi_state_page.ts_off of a time.Now() page: rendered in the context's local zone
+STATE_STRINGS = ("id", "url", "status", "error", "platform", "parentId", "LastConnectionID", "sequenceId", "crawlId")
+STATE_CODES = ("", "unfetched", "fetched", "failed", "deleted", "resample")  # preset status / platform codes
+STATE_PAGE = np.dtype([("str_off", "<u8"), ("str_len", "<u4", (9,)), ("ts_off", "<i4"), ("depth", "<i8"),
+                       ("ts_sec", "<i8"), ("ts_nsec", "<i4"), ("n_msgs", "<u4")])
+STATE_MSG = np.dtype([("chat_id", "<i8"), ("message_id", "<i8"), ("page_id", "<u4"), ("status", "<u2"), ("platform", "<u2")])
+STATE_UPDATE = np.dtype([("chat_id", "<i8"), ("message_id", "<i8"), ("row", "<u4"), ("status", "<u2"), ("reserved", "<u2")])
+STATE_LAYER = np.dtype([("depth", "<i8"), ("n_pages", "<u8")])
+assert (STATE_PAGE.itemsize, STATE_MSG.itemsize, STATE_UPDATE.itemsize, STATE_LAYER.itemsize) == (72, 24, 24, 16)
+
+
+class StateJsonC(C.Structure):  # tgi_state_json_t
+    _fields_ = [("data", C.c_void_p), ("len", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 class StatsC(C.Structure):
     _fields_ = [("records", C.c_uint64), ("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64),
                 ("links", C.c_uint64), ("frontier_size", C.c_uint64), ("launches", C.c_uint64),

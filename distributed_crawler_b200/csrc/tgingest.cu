@@ -17,12 +17,14 @@
 #include <map>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "kernels.cuh"
 #include "dapr.cuh"
 #include "combine.cuh"
 #include "local_appends.cuh"
+#include "state.cuh"
 #include "tg_page.cuh"
 #include "yt_page.cuh"
 
@@ -182,6 +184,32 @@ struct Combiner {
   HostBuf h_blobs, h_data, h_path, h_tables, h_drops, h_counts, h_line_off;
 };
 
+// tgi_state_*: the crawl progress state (state.cuh).  The host keeps the layers, the page rows (a mirror of the device
+// rows and their strings), the id and URL maps of AddLayer / UpdatePage and the string table; the messages and the
+// lookup table live on the device only.
+struct CrawlState {
+  std::mutex mu;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t t0 = nullptr, t1 = nullptr, t2 = nullptr, t3 = nullptr;  // the render's size pass and emit
+  std::vector<tgi_state_page> rows;  // str_off into blob
+  std::string blob;
+  std::vector<uint32_t> gen;         // mirror of row_gen
+  std::unordered_map<std::string, uint32_t> by_id;   // pageMap: id -> row
+  std::unordered_map<std::string, uint64_t> urls;    // URL -> pages of pageMap with it (AddLayer's existingURLs)
+  uint64_t deadends = 0;                             // pages with status "deadend"
+  std::map<int64_t, std::vector<uint32_t>> layers;   // layerMap, ascending depth
+  std::vector<std::string> codes;
+  std::unordered_map<std::string, uint16_t> code_of;
+  bool codes_dirty = true;
+  uint64_t rows_synced = 0, blob_synced = 0;         // rows / blob bytes already on the device
+  uint64_t n_msgs = 0, n_dead = 0;                   // message rows on the device, and how many are tombstones
+  uint64_t tslots = 0;
+  DevBuf pages, dblob, row_gen, row_cnt, msgs, table, code_blob, code_off;
+  DevBuf upd, bfirst, blast, slot_of, flag, pos, tiles, sc, spare;  // scratch
+  DevBuf entries, keys, vals, row_base, msize, moff, e32, e64, counts, roff, out;
+  HostBuf h_out, h_sc, h_read;
+};
+
 struct Slot {
   int idx = 0;
   cudaStream_t stream = nullptr;
@@ -255,6 +283,7 @@ struct tgi_ctx {
   uint64_t tk_next = 0, tk_serving = 0;
   InsertScratch ins;  // scratch of tgi_frontier_insert* / tgi_set_add / the merge (under fr_mu)
   Combiner cb;        // tgi_combine_*
+  CrawlState state;   // tgi_state_*
   // multi-GPU merge: communicator (this rank's partition is sets[TGI_SET_OWNED])
   NcclApi* nccl = nullptr;
   ncclComm_t comm = nullptr;
@@ -1920,6 +1949,11 @@ void tgi_destroy(tgi_ctx* c) {
     cudaStreamDestroy(c->cb.stream);
   }
   for (cudaEvent_t e : {c->cb.ev, c->cb.t0, c->cb.t1}) if (e) cudaEventDestroy(e);
+  if (c->state.stream) {
+    cudaStreamSynchronize(c->state.stream);
+    cudaStreamDestroy(c->state.stream);
+  }
+  for (cudaEvent_t e : {c->state.t0, c->state.t1, c->state.t2, c->state.t3}) if (e) cudaEventDestroy(e);
   delete c;  // the device and pinned buffers free themselves
 }
 
@@ -3190,6 +3224,636 @@ int tgi_filter_usernames(tgi_ctx* c, const uint8_t* names, const uint32_t* off, 
   dn.release();
   doff.release();
   dr.release();
+  return TGI_OK;
+}
+
+}  // extern "C"
+
+// ---- crawl progress state (state.cuh) ---------------------------------------------------------------------------------
+namespace {
+
+const char* const kPresetCodes[] = {"", "unfetched", "fetched", "failed", "deleted", "resample"};
+
+std::string st_field(const CrawlState& S, const tgi_state_page& p, int f) {
+  uint64_t o = p.str_off;
+  for (int k = 0; k < f; k++) o += p.str_len[k];
+  return S.blob.substr(o, p.str_len[f]);
+}
+std::string in_field(const tgi_state_page& p, const uint8_t* strs, int f) {
+  uint64_t o = p.str_off;
+  for (int k = 0; k < f; k++) o += p.str_len[k];
+  return std::string((const char*)strs + o, p.str_len[f]);
+}
+uint64_t page_str_bytes(const tgi_state_page& p) {
+  uint64_t t = 0;
+  for (int k = 0; k < TGI_PS_COUNT; k++) t += p.str_len[k];
+  return t;
+}
+bool page_ok(tgi_ctx* c, const tgi_state_page& p, const uint8_t* strs, uint64_t strs_len, const char* who) {
+  const uint64_t t = page_str_bytes(p);
+  if ((t && !strs) || p.str_off > strs_len || t > strs_len - p.str_off) { set_err(c, "%s: page strings outside strs", who); return false; }
+  if (p.ts_nsec < 0 || p.ts_nsec >= 1000000000) { set_err(c, "%s: ts_nsec %d out of range", who, p.ts_nsec); return false; }
+  if (p.ts_off != TGI_STATE_TS_LOCAL && (p.ts_off <= -86400 || p.ts_off >= 86400)) { set_err(c, "%s: ts_off %d is a day or more", who, p.ts_off); return false; }
+  return true;
+}
+
+// the state's stream, events, preset codes and minimal buffers, on first use (under S.mu)
+int st_init(tgi_ctx* c, CrawlState& S) {
+  cudaSetDevice(c->device);
+  if (S.stream) return TGI_OK;
+  CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
+  CK(cudaEventCreate(&S.t0));
+  CK(cudaEventCreate(&S.t1));
+  CK(cudaEventCreate(&S.t2));
+  CK(cudaEventCreate(&S.t3));
+  for (const char* s : kPresetCodes) {
+    S.code_of[s] = (uint16_t)S.codes.size();
+    S.codes.push_back(s);
+  }
+  for (DevBuf* b : {&S.pages, &S.dblob, &S.row_gen, &S.row_cnt, &S.msgs}) CK(b->ensure(64));
+  S.tslots = 1024;
+  CK(S.table.ensure(S.tslots * 4));
+  CK(cudaMemsetAsync(S.table.p, 0xFF, S.tslots * 4, S.stream));
+  return TGI_OK;
+}
+
+// b holds `used` bytes that must survive; make room for `need`
+int st_grow(tgi_ctx* c, CrawlState& S, DevBuf& b, size_t used, size_t need) {
+  if (need + PAD <= b.cap) return TGI_OK;
+  DevBuf n;
+  CK(n.ensure(std::max(need, 2 * used)));
+  if (used) CK(cudaMemcpyAsync(n.p, b.p, used, cudaMemcpyDeviceToDevice, S.stream));
+  CK(cudaStreamSynchronize(S.stream));
+  b.swap(n);
+  return TGI_OK;
+}
+
+StDev st_dev(const CrawlState& S) {
+  StDev d{};
+  d.pages = S.pages.as<tgi_state_page>();
+  d.blob = S.dblob.as<uint8_t>();
+  d.row_gen = S.row_gen.as<uint32_t>();
+  d.row_cnt = S.row_cnt.as<uint32_t>();
+  d.msgs = S.msgs.as<StMsg>();
+  d.table = S.table.as<uint32_t>();
+  d.tmask = S.tslots - 1;
+  d.codes = StCodes{S.code_blob.as<uint8_t>(), S.code_off.as<uint32_t>()};
+  return d;
+}
+unsigned st_grid(const tgi_ctx* c, uint64_t n) { return sink_grid(c, n, ST_THREADS, 16); }
+
+// writes row r (a new row when r == rows.size()) from page p, its strings appended to the blob; keeps the id / URL maps
+// and the deadend count
+void st_put_row(CrawlState& S, uint32_t r, const tgi_state_page& p, const uint8_t* strs) {
+  if (r < S.rows.size()) {
+    const std::string url = st_field(S, S.rows[r], TGI_PS_URL);
+    if (--S.urls[url] == 0) S.urls.erase(url);
+    if (st_field(S, S.rows[r], TGI_PS_STATUS) == "deadend") S.deadends--;
+  }
+  tgi_state_page q = p;
+  q.str_off = S.blob.size();
+  q.n_msgs = 0;
+  S.blob.append((const char*)strs + p.str_off, page_str_bytes(p));
+  S.urls[in_field(p, strs, TGI_PS_URL)]++;
+  if (in_field(p, strs, TGI_PS_STATUS) == "deadend") S.deadends++;
+  if (r == S.rows.size()) {
+    S.rows.push_back(q);
+    S.gen.push_back(0);
+    S.by_id[in_field(p, strs, TGI_PS_ID)] = r;
+  } else {
+    S.rows[r] = q;
+  }
+}
+
+// the rows and strings the device does not have yet, and the rewritten rows in `dirty` (their gen too; their message
+// count is set to 0, as for new rows)
+int st_sync_rows(tgi_ctx* c, CrawlState& S, const std::vector<uint32_t>& dirty) {
+  cudaStream_t st = S.stream;
+  const uint64_t nr = S.rows.size(), r0 = S.rows_synced;
+  int rc;
+  if ((rc = st_grow(c, S, S.dblob, S.blob_synced, S.blob.size()))) return rc;
+  if (S.blob.size() > S.blob_synced)
+    CK(cudaMemcpyAsync(S.dblob.as<uint8_t>() + S.blob_synced, S.blob.data() + S.blob_synced, S.blob.size() - S.blob_synced,
+                       cudaMemcpyHostToDevice, st));
+  S.blob_synced = S.blob.size();
+  if ((rc = st_grow(c, S, S.pages, r0 * sizeof(tgi_state_page), nr * sizeof(tgi_state_page)))) return rc;
+  if ((rc = st_grow(c, S, S.row_gen, r0 * 4, nr * 4))) return rc;
+  if ((rc = st_grow(c, S, S.row_cnt, r0 * 4, (nr + 1) * 4))) return rc;
+  if (nr > r0) {
+    CK(cudaMemcpyAsync(S.pages.as<tgi_state_page>() + r0, S.rows.data() + r0, (nr - r0) * sizeof(tgi_state_page), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(S.row_gen.as<uint32_t>() + r0, S.gen.data() + r0, (nr - r0) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(S.row_cnt.as<uint32_t>() + r0, 0, (nr - r0) * 4, st));
+  }
+  for (uint32_t r : dirty) {
+    if (r >= r0) continue;
+    CK(cudaMemcpyAsync(S.pages.as<tgi_state_page>() + r, &S.rows[r], sizeof(tgi_state_page), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(S.row_gen.as<uint32_t>() + r, &S.gen[r], 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(S.row_cnt.as<uint32_t>() + r, 0, 4, st));
+  }
+  S.rows_synced = nr;
+  CK(cudaStreamSynchronize(st));  // the host rows may move once this returns
+  return TGI_OK;
+}
+
+int st_row_count(tgi_ctx* c, CrawlState& S, uint32_t r, uint32_t* n) {
+  CK(cudaMemcpyAsync(n, S.row_cnt.as<uint32_t>() + r, 4, cudaMemcpyDeviceToHost, S.stream));
+  CK(cudaStreamSynchronize(S.stream));
+  return TGI_OK;
+}
+
+// the lookup table at `slots` slots, rebuilt from the live messages
+int st_rebuild_table(tgi_ctx* c, CrawlState& S, uint64_t slots) {
+  if (slots != S.tslots) {
+    CK(cudaStreamSynchronize(S.stream));
+    CK(S.table.ensure(slots * 4));
+    S.tslots = slots;
+  }
+  CK(cudaMemsetAsync(S.table.p, 0xFF, slots * 4, S.stream));
+  if (S.n_msgs) st_table_insert_kernel<<<st_grid(c, S.n_msgs), ST_THREADS, 0, S.stream>>>(st_dev(S), 0, S.n_msgs);
+  CK(cudaGetLastError());
+  return TGI_OK;
+}
+
+// room for `extra` more message rows, in the buffer and at a table load of at most one half
+int st_reserve(tgi_ctx* c, CrawlState& S, uint64_t extra) {
+  const uint64_t need = S.n_msgs + extra;
+  if (need >= 0xFFFFFFFEull) { set_err(c, "state: %llu message rows (at most 2^32 - 2)", (unsigned long long)need); return TGI_E_CAPACITY; }
+  int rc;
+  if ((rc = st_grow(c, S, S.msgs, S.n_msgs * sizeof(StMsg), need * sizeof(StMsg)))) return rc;
+  if (2 * need > S.tslots) return st_rebuild_table(c, S, next_pow2(std::max<uint64_t>(4 * need, 1024)));
+  return TGI_OK;
+}
+
+// the live messages moved to the front in storage order once the tombstones outnumber them, and the table rebuilt
+int st_compact(tgi_ctx* c, CrawlState& S) {
+  const uint64_t n = S.n_msgs, live = n - S.n_dead;
+  if (S.n_dead <= live) return TGI_OK;
+  cudaStream_t st = S.stream;
+  CK(S.flag.ensure(n * 4));
+  CK(S.pos.ensure((n + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.spare.ensure(std::max<uint64_t>(live, 1) * sizeof(StMsg)));
+  const StDev d = st_dev(S);
+  st_live_flag_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(d, n, ST_NONE, S.flag.as<uint32_t>());
+  uint32_t launches = 0;
+  int rc;
+  if ((rc = launch_scan(c, st, S.tiles, S.flag.as<uint32_t>(), n, S.pos.as<uint64_t>(), S.sc.as<uint64_t>(), launches))) return rc;
+  st_compact_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(d, n, S.flag.as<uint32_t>(), S.pos.as<uint64_t>(), S.spare.as<StMsg>());
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  S.msgs.swap(S.spare);
+  S.n_msgs = live;
+  S.n_dead = 0;
+  return st_rebuild_table(c, S, S.tslots);
+}
+
+// message rows of the host form, uploaded behind the existing ones and entered in the table
+int st_append_msgs(tgi_ctx* c, CrawlState& S, const std::vector<StMsg>& m) {
+  if (m.empty()) return TGI_OK;
+  int rc;
+  if ((rc = st_reserve(c, S, m.size()))) return rc;
+  CK(cudaMemcpyAsync(S.msgs.as<StMsg>() + S.n_msgs, m.data(), m.size() * sizeof(StMsg), cudaMemcpyHostToDevice, S.stream));
+  st_table_insert_kernel<<<st_grid(c, m.size()), ST_THREADS, 0, S.stream>>>(st_dev(S), S.n_msgs, S.n_msgs + m.size());
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(S.stream));
+  S.n_msgs += m.size();
+  return TGI_OK;
+}
+
+int st_upload_codes(tgi_ctx* c, CrawlState& S) {
+  if (!S.codes_dirty) return TGI_OK;
+  std::string blob;
+  std::vector<uint32_t> off(1, 0);
+  for (const std::string& s : S.codes) {
+    blob += s;
+    off.push_back((uint32_t)blob.size());
+  }
+  CK(S.code_blob.ensure(blob.size()));
+  CK(S.code_off.ensure(off.size() * 4));
+  CK(cudaMemsetAsync(S.code_blob.p, 0, blob.size() + PAD, S.stream));
+  if (!blob.empty()) CK(cudaMemcpyAsync(S.code_blob.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, S.stream));
+  CK(cudaMemcpyAsync(S.code_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, S.stream));
+  CK(cudaStreamSynchronize(S.stream));
+  S.codes_dirty = false;
+  return TGI_OK;
+}
+
+// the row's message generation moves on: its messages become tombstones
+int st_drop_messages(tgi_ctx* c, CrawlState& S, uint32_t r) {
+  uint32_t cnt = 0;
+  int rc;
+  if ((rc = st_row_count(c, S, r, &cnt))) return rc;
+  S.n_dead += cnt;
+  S.gen[r]++;
+  return TGI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tgi_state_code(tgi_ctx* c, const char* s, uint32_t len, uint16_t* code) {
+  if (!c || (len && !s) || !code) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  const std::string k(s ? s : "", len);
+  const auto it = S.code_of.find(k);
+  if (it != S.code_of.end()) {
+    *code = it->second;
+    return TGI_OK;
+  }
+  if (S.codes.size() >= 0xFFFF) { set_err(c, "tgi_state_code: 65535 codes registered"); return TGI_E_CAPACITY; }
+  *code = (uint16_t)S.codes.size();
+  S.code_of[k] = *code;
+  S.codes.push_back(k);
+  S.codes_dirty = true;
+  return TGI_OK;
+}
+
+int tgi_state_set(tgi_ctx* c, const tgi_state_layer* layers, uint32_t n_layers, const tgi_state_page* pages, uint64_t n_pages,
+                  const uint8_t* strs, uint64_t strs_len, const tgi_state_msg* msgs, uint64_t n_msgs, uint32_t* rows) {
+  if (!c || (n_layers && !layers) || (n_pages && !pages) || (n_msgs && !msgs)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  uint64_t in_layers = 0, owned = 0;
+  for (uint32_t k = 0; k < n_layers; k++) in_layers += layers[k].n_pages;
+  if (in_layers != n_pages) { set_err(c, "tgi_state_set: the layers hold %llu pages, not %llu", (unsigned long long)in_layers, (unsigned long long)n_pages); return TGI_E_ARG; }
+  for (uint64_t i = 0; i < n_pages; i++) {
+    if (!page_ok(c, pages[i], strs, strs_len, "tgi_state_set")) return TGI_E_ARG;
+    owned += pages[i].n_msgs;
+  }
+  if (owned != n_msgs) { set_err(c, "tgi_state_set: the pages own %llu messages, not %llu", (unsigned long long)owned, (unsigned long long)n_msgs); return TGI_E_ARG; }
+  if (n_msgs >= 0xFFFFFFFEull) { set_err(c, "tgi_state_set: %llu messages (at most 2^32 - 2)", (unsigned long long)n_msgs); return TGI_E_CAPACITY; }
+  for (uint64_t j = 0; j < n_msgs; j++)
+    if (msgs[j].page_id >= n_pages || msgs[j].status >= S.codes.size() || msgs[j].platform >= S.codes.size()) {
+      set_err(c, "tgi_state_set: message %llu names an unknown page or code", (unsigned long long)j);
+      return TGI_E_ARG;
+    }
+  // SetState: new maps, layer by layer; a later page with the same id replaces the row (and its messages)
+  S.rows.clear();
+  S.blob.clear();
+  S.gen.clear();
+  S.by_id.clear();
+  S.urls.clear();
+  S.layers.clear();
+  S.deadends = 0;
+  S.rows_synced = S.blob_synced = 0;
+  S.n_msgs = S.n_dead = 0;
+  std::vector<uint32_t> row_of(n_pages);
+  std::vector<uint64_t> winner;  // the page whose messages a row keeps
+  uint64_t i = 0;
+  for (uint32_t k = 0; k < n_layers; k++) {
+    std::vector<uint32_t>& L = S.layers[layers[k].depth];
+    L.clear();
+    for (uint64_t q = 0; q < layers[k].n_pages; q++, i++) {
+      const auto it = S.by_id.find(in_field(pages[i], strs, TGI_PS_ID));
+      const uint32_t r = it == S.by_id.end() ? (uint32_t)S.rows.size() : it->second;
+      st_put_row(S, r, pages[i], strs);
+      if (r == winner.size()) winner.push_back(i);
+      else winner[r] = i;
+      row_of[i] = r;
+      L.push_back(r);
+    }
+  }
+  std::vector<StMsg> m;
+  std::vector<uint32_t> cnt(S.rows.size(), 0);
+  uint64_t j = 0;
+  for (i = 0; i < n_pages; i++) {
+    const uint32_t r = row_of[i];
+    for (uint32_t q = 0; q < pages[i].n_msgs; q++, j++) {
+      if (winner[r] != i) continue;
+      const tgi_state_msg& x = msgs[j];
+      m.push_back(StMsg{(long long)x.chat_id, (long long)x.message_id, r, 0, row_of[x.page_id], x.status, x.platform});
+      cnt[r]++;
+    }
+  }
+  rc = st_sync_rows(c, S, std::vector<uint32_t>());
+  if (rc) return rc;
+  if (!cnt.empty()) CK(cudaMemcpyAsync(S.row_cnt.p, cnt.data(), cnt.size() * 4, cudaMemcpyHostToDevice, S.stream));
+  if ((rc = st_rebuild_table(c, S, next_pow2(std::max<uint64_t>(4 * m.size(), 1024))))) return rc;
+  if ((rc = st_append_msgs(c, S, m))) return rc;
+  if (rows) memcpy(rows, row_of.data(), n_pages * 4);
+  return TGI_OK;
+}
+
+int tgi_state_add_layer(tgi_ctx* c, const tgi_state_page* pages, uint64_t n, const uint8_t* strs, uint64_t strs_len,
+                        int64_t max_pages, uint32_t* rows) {
+  if (!c || (n && !pages)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if (!n) return TGI_OK;  // base.go:220-222: no layer is created
+  for (uint64_t i = 0; i < n; i++) {
+    if (!page_ok(c, pages[i], strs, strs_len, "tgi_state_add_layer")) return TGI_E_ARG;
+    if (pages[i].n_msgs) { set_err(c, "tgi_state_add_layer: page %llu carries messages", (unsigned long long)i); return TGI_E_ARG; }
+  }
+  const bool reached = max_pages > 0 && (int64_t)S.rows.size() >= max_pages;
+  int64_t replacements = (int64_t)S.deadends;
+  std::vector<uint32_t>& L = S.layers[pages[0].depth];
+  std::vector<uint32_t> dirty;
+  std::unordered_map<std::string, int> gone;  // URLs of overwritten pages: still in existingURLs for this call
+  for (uint64_t i = 0; i < n; i++) {
+    if (rows) rows[i] = TGI_STATE_NO_PAGE;
+    const std::string url = in_field(pages[i], strs, TGI_PS_URL);
+    if (S.urls.count(url) || gone.count(url)) continue;
+    if (reached) {
+      if (replacements <= 0) continue;
+      replacements--;
+    }
+    const auto it = S.by_id.find(in_field(pages[i], strs, TGI_PS_ID));
+    uint32_t r = (uint32_t)S.rows.size();
+    if (it != S.by_id.end()) {  // pageMap[id] = page: the old page and its messages go
+      r = it->second;
+      gone[st_field(S, S.rows[r], TGI_PS_URL)] = 1;
+      if (std::find(dirty.begin(), dirty.end(), r) == dirty.end()) {  // the device count is read once per call
+        if (r < S.rows_synced && (rc = st_drop_messages(c, S, r))) return rc;
+        dirty.push_back(r);
+      }
+    }
+    st_put_row(S, r, pages[i], strs);
+    L.push_back(r);
+    if (rows) rows[i] = r;
+  }
+  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  return st_compact(c, S);
+}
+
+int tgi_state_update_page(tgi_ctx* c, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                          const tgi_state_msg* msgs, uint32_t* row) {
+  if (!c || !page || (page->n_msgs && !msgs)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if (!page_ok(c, *page, strs, strs_len, "tgi_state_update_page")) return TGI_E_ARG;
+  for (uint32_t j = 0; j < page->n_msgs; j++)
+    if ((msgs[j].page_id != TGI_STATE_NO_PAGE && msgs[j].page_id >= S.rows.size()) || msgs[j].status >= S.codes.size() ||
+        msgs[j].platform >= S.codes.size()) {
+      set_err(c, "tgi_state_update_page: message %u names an unknown row or code", j);
+      return TGI_E_ARG;
+    }
+  if (S.n_msgs + page->n_msgs >= 0xFFFFFFFEull) { set_err(c, "tgi_state_update_page: more than 2^32 - 2 message rows"); return TGI_E_CAPACITY; }
+  const auto it = S.by_id.find(in_field(*page, strs, TGI_PS_ID));
+  uint32_t r = (uint32_t)S.rows.size();
+  std::vector<uint32_t> dirty;
+  if (it != S.by_id.end()) {
+    r = it->second;
+    if ((rc = st_drop_messages(c, S, r))) return rc;
+    dirty.push_back(r);
+  }
+  st_put_row(S, r, *page, strs);
+  // base.go:131-146: appended only to a layer of its depth that exists and does not hold it yet
+  const auto lit = S.layers.find(page->depth);
+  if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), r) == lit->second.end()) lit->second.push_back(r);
+  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  std::vector<StMsg> m(page->n_msgs);
+  for (uint32_t j = 0; j < page->n_msgs; j++)
+    m[j] = StMsg{(long long)msgs[j].chat_id, (long long)msgs[j].message_id, r, S.gen[r],
+                 msgs[j].page_id == TGI_STATE_NO_PAGE ? r : msgs[j].page_id, msgs[j].status, msgs[j].platform};
+  const uint32_t cnt = page->n_msgs;
+  CK(cudaMemcpyAsync(S.row_cnt.as<uint32_t>() + r, &cnt, 4, cudaMemcpyHostToDevice, S.stream));
+  if ((rc = st_append_msgs(c, S, m))) return rc;
+  CK(cudaStreamSynchronize(S.stream));
+  if (row) *row = r;
+  return st_compact(c, S);
+}
+
+int tgi_state_update_messages(tgi_ctx* c, const tgi_state_update* ups, uint64_t n, uint64_t* skipped) {
+  if (!c || (n && !ups)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  std::vector<tgi_state_update> u;
+  u.reserve(n);
+  uint64_t skip = 0;
+  for (uint64_t j = 0; j < n; j++) {
+    if (ups[j].row == TGI_STATE_NO_PAGE) {
+      skip++;
+      continue;
+    }
+    if (ups[j].row >= S.rows.size() || ups[j].status >= S.codes.size()) {
+      set_err(c, "tgi_state_update_messages: update %llu names an unknown row or code", (unsigned long long)j);
+      return TGI_E_ARG;
+    }
+    u.push_back(ups[j]);
+  }
+  if (skipped) *skipped = skip;
+  const uint64_t m = u.size();
+  if (!m) return TGI_OK;
+  if ((rc = st_reserve(c, S, m))) return rc;
+  cudaStream_t st = S.stream;
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * m, 64));
+  CK(S.upd.ensure(m * sizeof(tgi_state_update)));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.blast.ensure(bslots * 4));
+  CK(S.slot_of.ensure(m * 4));
+  CK(S.flag.ensure(m * 4));
+  CK(S.pos.ensure((m + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(cudaMemcpyAsync(S.upd.p, u.data(), m * sizeof(tgi_state_update), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(S.bfirst.p, 0xFF, bslots * 4, st));
+  CK(cudaMemsetAsync(S.blast.p, 0, bslots * 4, st));
+  StUpd w{};
+  w.u = S.upd.as<tgi_state_update>();
+  w.n = m;
+  w.bfirst = S.bfirst.as<uint32_t>();
+  w.blast = S.blast.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.slot_of.as<uint32_t>();
+  w.flag = S.flag.as<uint32_t>();
+  w.pos = S.pos.as<uint64_t>();
+  w.n_msgs = S.n_msgs;
+  const StDev d = st_dev(S);
+  uint32_t launches = 0;
+  st_upd_build_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(w);
+  st_upd_resolve_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
+  if ((rc = launch_scan(c, st, S.tiles, w.flag, m, w.pos, S.sc.as<uint64_t>(), launches))) return rc;
+  st_upd_append_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t added = *S.h_sc.as<uint64_t>();
+  if (added) st_table_insert_kernel<<<st_grid(c, added), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + added);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  S.n_msgs += added;
+  return TGI_OK;
+}
+
+int tgi_state_read_page(tgi_ctx* c, uint32_t row, tgi_state_msg* out, uint64_t cap, uint64_t* n) {
+  if (!c || !n) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if (row >= S.rows.size()) { set_err(c, "tgi_state_read_page: no row %u", row); return TGI_E_ARG; }
+  uint32_t cnt = 0;
+  if ((rc = st_row_count(c, S, row, &cnt))) return rc;
+  *n = cnt;
+  if (!out || cap < cnt || !cnt) return TGI_OK;
+  cudaStream_t st = S.stream;
+  const uint64_t nm = S.n_msgs;
+  CK(S.flag.ensure(nm * 4));
+  CK(S.pos.ensure((nm + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.spare.ensure(cnt * sizeof(tgi_state_msg)));
+  const StDev d = st_dev(S);
+  uint32_t launches = 0;
+  st_live_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, row, S.flag.as<uint32_t>());
+  if ((rc = launch_scan(c, st, S.tiles, S.flag.as<uint32_t>(), nm, S.pos.as<uint64_t>(), S.sc.as<uint64_t>(), launches))) return rc;
+  st_read_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, S.flag.as<uint32_t>(), S.pos.as<uint64_t>(), S.spare.as<tgi_state_msg>());
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, S.spare.p, cnt * sizeof(tgi_state_msg), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return TGI_OK;
+}
+
+// json.Marshal(GetState()): the layers' bytes on the device (two passes), the frame and the spliced values on the host
+int tgi_state_render(tgi_ctx* c, const uint8_t* metadata, uint64_t metadata_len, const uint8_t* last_updated,
+                     uint64_t last_updated_len, tgi_state_json_t* out) {
+  if (!c || !out || (metadata_len && !metadata) || (last_updated_len && !last_updated)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if ((rc = st_upload_codes(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  std::vector<StEntry> E;
+  for (const auto& [depth, L] : S.layers) {
+    const uint32_t fl = E.empty() ? (uint32_t)ST_E_FIRST_LAYER : 0u;
+    if (L.empty()) E.push_back(StEntry{(long long)depth, ST_NONE, ST_E_FIRST | ST_E_LAST | fl});
+    for (size_t k = 0; k < L.size(); k++)
+      E.push_back(StEntry{(long long)depth, L[k], (k == 0 ? ST_E_FIRST | fl : 0u) | (k + 1 == L.size() ? (uint32_t)ST_E_LAST : 0u)});
+  }
+  static const char kHead[] = "{\"layers\":[", kMeta[] = "],\"metadata\":", kLast[] = ",\"lastUpdated\":";
+  const uint64_t ne = E.size(), nr = S.rows.size(), nm = S.n_msgs, live = nm - S.n_dead;
+  cudaStream_t st = S.stream;
+  uint32_t launches = 0;
+  uint64_t body = 0;
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  // the zone table must not change under the kernels that read it (tgi_set_zone swaps it under cfg_mu)
+  std::lock_guard<std::mutex> zg(c->cfg_mu);
+  if (ne) {
+    CK(S.flag.ensure(nm * 4));
+    CK(S.pos.ensure((nm + 1) * 8));
+    CK(S.keys.ensure(2 * live * 4));
+    CK(S.vals.ensure(2 * live * 4));
+    CK(S.row_base.ensure((nr + 1) * 8));
+    CK(S.msize.ensure(live * 4));
+    CK(S.moff.ensure((live + 1) * 8));
+    CK(S.entries.ensure(ne * sizeof(StEntry)));
+    CK(S.e32.ensure(4 * ne * 4));
+    CK(S.e64.ensure(2 * (ne + 1) * 8));
+    StRender r{};
+    r.entries = S.entries.as<StEntry>();
+    r.n_entries = ne;
+    r.zone = c->cfgdev.zone;
+    r.zone_n = c->cfgdev.zone_n;
+    r.tz = c->cfgdev.tz;
+    r.sc = S.sc.as<uint64_t>();
+    r.flag = S.flag.as<uint32_t>();
+    r.pos = S.pos.as<uint64_t>();
+    r.keys[0] = S.keys.as<uint32_t>();
+    r.keys[1] = r.keys[0] + live;
+    r.vals[0] = S.vals.as<uint32_t>();
+    r.vals[1] = r.vals[0] + live;
+    r.row_base = S.row_base.as<uint64_t>();
+    r.msize = S.msize.as<uint32_t>();
+    r.moff = S.moff.as<uint64_t>();
+    r.esize_lo = S.e32.as<uint32_t>();
+    r.ebytes = r.esize_lo + ne;
+    r.ecnt = r.ebytes + ne;
+    r.esz = r.ecnt + ne;
+    r.eoff = S.e64.as<uint64_t>();
+    r.eslot = r.eoff + ne + 1;
+    // radix passes over the bits of the largest row
+    uint32_t bits = 0;
+    while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
+    const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
+    const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
+    CK(S.counts.ensure(radix * ntiles * 4));
+    CK(S.roff.ensure((radix * ntiles + 1) * 8));
+    const StDev d = st_dev(S);
+    CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+    CK(cudaEventRecord(S.t0, st));
+    st_render_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, r.sc + ST_SC_LIVE, launches))) return rc;
+    st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+    launches++;
+    int cur = 0;
+    for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
+      const uint32_t shift = p * width;
+      la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                     S.counts.as<uint32_t>());
+      launches++;
+      if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), r.sc + ST_SC_RADIX, launches))) return rc;
+      la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.vals[cur], r.keys[cur ^ 1], r.vals[cur ^ 1],
+                                                                        r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                        S.roff.as<uint64_t>());
+      launches++;
+    }
+    if ((rc = launch_scan(c, st, S.tiles, d.row_cnt, nr, r.row_base, r.sc + ST_SC_ROWS, launches))) return rc;
+    st_msg_size_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, r, r.vals[cur], r.keys[cur], live);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.msize, live, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
+    st_entry_size_kernel<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.esz, ne, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
+    if ((rc = launch_scan(c, st, S.tiles, r.ecnt, ne, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t1, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint64_t* h = S.h_sc.as<uint64_t>();
+    if (h[ST_SC_LIVE] != live) { set_err(c, "tgi_state_render: %llu live messages, expected %llu", (unsigned long long)h[ST_SC_LIVE], (unsigned long long)live); return TGI_E_CUDA; }
+    if (h[ST_SC_ERR]) { set_err(c, "tgi_state_render: a page timestamp's year is outside [0, 9999] (json.Marshal fails)"); return TGI_E_ARG; }
+    if (h[ST_SC_BIG]) { set_err(c, "tgi_state_render: a page renders to 4 GiB or more"); return TGI_E_CAPACITY; }
+    body = h[ST_SC_BYTES];
+    const uint64_t slots = h[ST_SC_SLOTS];
+    float size_ms = 0, emit_ms = 0;
+    cudaEventElapsedTime(&size_ms, S.t0, S.t1);
+    CK(S.out.ensure(body));
+    CK(S.h_out.ensure(sizeof kHead + body + sizeof kMeta + metadata_len + sizeof kLast + last_updated_len + 2));
+    r.out = S.out.as<uint8_t>();
+    CK(cudaEventRecord(S.t2, st));
+    st_entry_emit_kernel<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
+    if (slots) st_msg_emit_kernel<<<st_grid(c, slots), ST_THREADS, 0, st>>>(d, r, r.vals[cur]);
+    launches += 1 + (slots != 0);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t3, st));
+    CK(cudaMemcpyAsync(S.h_out.as<uint8_t>() + sizeof kHead - 1, S.out.p, body, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
+    out->kernel_ms = size_ms + emit_ms;
+  } else {
+    CK(S.h_out.ensure(sizeof kHead + sizeof kMeta + metadata_len + sizeof kLast + last_updated_len + 2));
+  }
+  uint8_t* o = S.h_out.as<uint8_t>();
+  uint64_t k = 0;
+  memcpy(o, kHead, sizeof kHead - 1);
+  k = sizeof kHead - 1 + body;
+  memcpy(o + k, kMeta, sizeof kMeta - 1);
+  k += sizeof kMeta - 1;
+  if (metadata_len) memcpy(o + k, metadata, metadata_len);
+  k += metadata_len;
+  memcpy(o + k, kLast, sizeof kLast - 1);
+  k += sizeof kLast - 1;
+  if (last_updated_len) memcpy(o + k, last_updated, last_updated_len);
+  k += last_updated_len;
+  o[k++] = '}';
+  out->data = o;
+  out->len = k;
+  out->gpu_launches = launches;
   return TGI_OK;
 }
 

@@ -36,7 +36,8 @@ EXPORTED_SYMBOLS = [
     "tgi_comm_destroy", "tgi_frontier_merge", "tgi_frontier_global_export", "tgi_merge_get_stats",
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
     "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
-    "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone",
+    "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
+    "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render",
 ]
 
 
@@ -104,6 +105,13 @@ def lib() -> C.CDLL:
         L.tgi_combine_flush.argtypes = [vp, C.c_int64, C.POINTER(abi.CombinedC)]
         L.tgi_channel_appends.argtypes = [vp, i32, C.POINTER(abi.ChannelAppendsC)]
         L.tgi_set_zone.argtypes = [vp, vp, vp, u32]
+        L.tgi_state_code.argtypes = [vp, C.c_char_p, u32, C.POINTER(C.c_uint16)]
+        L.tgi_state_set.argtypes = [vp, vp, u32, vp, u64, vp, u64, vp, u64, vp]
+        L.tgi_state_add_layer.argtypes = [vp, vp, u64, vp, u64, C.c_int64, vp]
+        L.tgi_state_update_page.argtypes = [vp, vp, vp, u64, vp, C.POINTER(u32)]
+        L.tgi_state_update_messages.argtypes = [vp, vp, u64, C.POINTER(u64)]
+        L.tgi_state_read_page.argtypes = [vp, u32, vp, u64, C.POINTER(u64)]
+        L.tgi_state_render.argtypes = [vp, vp, u64, vp, u64, C.POINTER(abi.StateJsonC)]
         _LIB = L
     return _LIB
 
@@ -501,6 +509,123 @@ class Engine:
         out = np.full(len(b), -1, np.int64)
         self._check(lib().tgi_key_join(self.h, a.ctypes.data, len(a), b.ctypes.data, len(b), out.ctypes.data))
         return out
+
+    # --- crawl progress state (tgi_state_*): pages as state_pack dicts, rows as the library returns them ----------------
+    def state_code(self, s: bytes) -> int:
+        """the string-table code of a message status / platform (registered on first use)"""
+        codes = self.__dict__.setdefault("_st_codes", {c.encode(): i for i, c in enumerate(abi.STATE_CODES)})
+        if s not in codes:
+            v = C.c_uint16()
+            self._check(lib().tgi_state_code(self.h, s, len(s), C.byref(v)))
+            codes[s] = v.value
+        return codes[s]
+
+    def _st_rows(self):
+        return self.__dict__.setdefault("_st_row_of", {})
+
+    def _st_note_rows(self, pages, rows):
+        ids = self.__dict__.setdefault("_st_ids", [])
+        for p, r in zip(pages, rows):
+            if r != abi.STATE_NO_PAGE:
+                self._st_rows()[p.get("id", b"")] = int(r)
+                ids.extend([b""] * (int(r) + 1 - len(ids)))
+                ids[int(r)] = p.get("id", b"")
+
+    def state_set_arrays(self, layers, recs, strs, msgs) -> np.ndarray:
+        """tgi_state_set on packed arrays (abi.STATE_LAYER, STATE_PAGE, bytes, STATE_MSG): the rows of the pages"""
+        layers = np.ascontiguousarray(layers, abi.STATE_LAYER)
+        recs = np.ascontiguousarray(recs, abi.STATE_PAGE)
+        strs = np.ascontiguousarray(strs, np.uint8)
+        msgs = np.ascontiguousarray(msgs, abi.STATE_MSG)
+        rows = np.zeros(max(len(recs), 1), np.uint32)
+        self._check(lib().tgi_state_set(self.h, layers.ctypes.data, len(layers), recs.ctypes.data, len(recs), strs.ctypes.data,
+                                        len(strs), msgs.ctypes.data, len(msgs), rows.ctypes.data))
+        return rows[:len(recs)]
+
+    def state_set(self, layers) -> list[int]:
+        """SetState: layers = [(depth, [page, ...]), ...]; a message's pageId names a page of the call"""
+        from .state_pack import pack_pages
+        pages = [p for _, ps in layers for p in ps]
+        index = {p.get("id", b""): i for i, p in enumerate(pages)}
+
+        def msg_page(pid, i):
+            if pid not in index:
+                raise ValueError(f"pageId {pid!r} names no page of the state")
+            return index[pid]
+        recs, strs, msgs = pack_pages(pages, self.state_code, msg_page)
+        lay = np.array([(d, len(ps)) for d, ps in layers], abi.STATE_LAYER)
+        rows = self.state_set_arrays(lay, recs, strs, msgs)
+        self.__dict__["_st_row_of"], self.__dict__["_st_ids"] = {}, []
+        self._st_note_rows(pages, rows)
+        return [int(r) for r in rows]
+
+    def state_add_layer(self, pages, max_pages: int = 0) -> list[int]:
+        """AddLayer (pages without messages, ids and timestamps filled): each page's row, or abi.STATE_NO_PAGE"""
+        from .state_pack import pack_pages
+        recs, strs, _ = pack_pages(pages, self.state_code, lambda pid, i: i)  # messages are refused by the library
+        rows = np.zeros(max(len(pages), 1), np.uint32)
+        self._check(lib().tgi_state_add_layer(self.h, recs.ctypes.data, len(recs), strs.ctypes.data, len(strs), max_pages,
+                                              rows.ctypes.data))
+        self._st_note_rows(pages, rows[:len(pages)])
+        return [int(r) for r in rows[:len(pages)]]
+
+    def state_update_page(self, page) -> int:
+        """UpdatePage: the page's row"""
+        from .state_pack import pack_pages
+        own = page.get("id", b"")
+
+        def msg_page(pid, i):
+            if pid == own:
+                return abi.STATE_NO_PAGE
+            if pid not in self._st_rows():
+                raise ValueError(f"pageId {pid!r} names no page of the state")
+            return self._st_rows()[pid]
+        recs, strs, msgs = pack_pages([page], self.state_code, msg_page)
+        row = C.c_uint32()
+        self._check(lib().tgi_state_update_page(self.h, recs.ctypes.data, strs.ctypes.data, len(strs),
+                                                msgs.ctypes.data if len(msgs) else None, C.byref(row)))
+        self._st_note_rows([page], [row.value])
+        return row.value
+
+    def state_update_messages(self, updates) -> int:
+        """UpdateMessage once per (row, chat_id, message_id, status bytes), in order; returns the updates skipped for
+        naming no page (row abi.STATE_NO_PAGE)"""
+        u = np.zeros(max(len(updates), 1), abi.STATE_UPDATE)
+        for j, (row, chat, msg, st) in enumerate(updates):
+            u[j] = (chat, msg, row, self.state_code(st), 0)
+        return self.state_update_arrays(u[:len(updates)])
+
+    def state_update_arrays(self, u) -> int:
+        u = np.ascontiguousarray(u, abi.STATE_UPDATE)
+        skipped = C.c_uint64()
+        self._check(lib().tgi_state_update_messages(self.h, u.ctypes.data, len(u), C.byref(skipped)))
+        return skipped.value
+
+    def state_read_page_arrays(self, row: int) -> np.ndarray:
+        n = C.c_uint64()
+        self._check(lib().tgi_state_read_page(self.h, row, None, 0, C.byref(n)))
+        out = np.zeros(max(n.value, 1), abi.STATE_MSG)
+        self._check(lib().tgi_state_read_page(self.h, row, out.ctypes.data, n.value, C.byref(n)))
+        return out[:n.value]
+
+    def state_read_page(self, row: int) -> list[dict]:
+        """GetPage(id).Messages of a row"""
+        names = {v: k for k, v in self.__dict__.get("_st_codes", {}).items()}
+        names.update({i: c.encode() for i, c in enumerate(abi.STATE_CODES)})
+        ids = self.__dict__.get("_st_ids", [])
+        return [{"chatId": int(m["chat_id"]), "messageId": int(m["message_id"]), "status": names[int(m["status"])],
+                 "pageId": ids[int(m["page_id"])], "platform": names[int(m["platform"])]}
+                for m in self.state_read_page_arrays(row)]
+
+    def state_render(self, metadata: bytes, last_updated: bytes, copy: bool = True):
+        """json.Marshal(GetState()) with the shim's marshalled metadata and lastUpdated spliced in (copy=False: a view of
+        the library's pinned bytes, valid until the next state call); the device time of the call is left in
+        self.state_render_ms"""
+        out = abi.StateJsonC()
+        self._check(lib().tgi_state_render(self.h, metadata, len(metadata), last_updated, len(last_updated), C.byref(out)))
+        self.state_render_ms = float(out.kernel_ms)
+        self.state_render_launches = int(out.gpu_launches)
+        return C.string_at(out.data, out.len) if copy else _view(out.data, out.len, np.uint8)
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

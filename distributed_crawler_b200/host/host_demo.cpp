@@ -2,6 +2,7 @@
 //   host_demo --pack   prints an FNV-1a hash of every packed array (no GPU needed): tests/test_host_cpp.py
 //                      packs the same messages with pack.py and compares
 //   host_demo --run    processes them on the GPU and prints status, outlinks and the JSONL lines
+//   host_demo --state  the same, then a one-page crawl state (StateSet) rendered as state.json (StateRender)
 #include <cstdio>
 #include <cstring>
 
@@ -89,6 +90,15 @@ int main(int argc, char** argv) {
       for (const std::string& l : r.Outlinks(i)) printf(" %s", l.c_str());
       printf("\n");
       fwrite(r.Line(i).data(), 1, r.Line(i).size(), stdout);
+    }
+    if (argc > 1 && !strcmp(argv[1], "--state")) {  // one seed page with one message, as state.json
+      tgi_state_page pg{};
+      pg.str_len[TGI_PS_ID] = 2, pg.str_len[TGI_PS_URL] = 11, pg.str_len[TGI_PS_STATUS] = 9;
+      pg.ts_off = TGI_STATE_TS_LOCAL, pg.ts_sec = 1750000000, pg.n_msgs = 1;
+      proc.StateSet({{0, 1}}, {pg}, "p1testchannelunfetched", {{-1001234567890ll, 5ll << 20, 0, 1, 0}});
+      const std::string_view js = proc.StateRender("{}", "\"2025-06-15T15:06:40Z\"");
+      fwrite(js.data(), 1, js.size(), stdout);
+      printf("\n");
     }
   } catch (const std::exception& e) {
     fprintf(stderr, "error: %s\n", e.what());

@@ -295,6 +295,25 @@ class MessageProcessor {
     if (tgi_combine_flush(ctx_, unix_nano, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
     return o;
   }
+  // SetState / Initialize on the device-resident crawl state (tgi_state_set): layers[k] takes the next
+  // layers[k].n_pages pages, pages[i] the next pages[i].n_msgs messages; returns every page's row
+  std::vector<uint32_t> StateSet(const std::vector<tgi_state_layer>& layers, const std::vector<tgi_state_page>& pages,
+                                 std::string_view strs, const std::vector<tgi_state_msg>& msgs) {
+    std::vector<uint32_t> rows(pages.size());
+    if (tgi_state_set(ctx_, layers.data(), (uint32_t)layers.size(), pages.data(), pages.size(), (const uint8_t*)strs.data(),
+                      strs.size(), msgs.data(), msgs.size(), rows.data()) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return rows;
+  }
+  // json.Marshal(GetState()): state.json with the caller's marshalled metadata and lastUpdated spliced in; the view
+  // stays valid until the next state call
+  std::string_view StateRender(std::string_view metadata_json, std::string_view last_updated_json) {
+    tgi_state_json_t o{};
+    if (tgi_state_render(ctx_, (const uint8_t*)metadata_json.data(), metadata_json.size(), (const uint8_t*)last_updated_json.data(),
+                         last_updated_json.size(), &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return std::string_view((const char*)o.data, o.len);
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

@@ -733,6 +733,94 @@ typedef struct tgi_set_info_t {
 int tgi_set_growth(tgi_ctx* ctx, uint64_t max_keys);
 int tgi_set_info(tgi_ctx* ctx, int which, tgi_set_info_t* out);
 
+/* Crawl progress state on the device — BaseStateManager's pageMap / layerMap (state/base.go) with state.Page and
+ * state.Message (state/datamodels.go:41-71), so LocalStateManager can write state.json ONCE per page (or per channel)
+ * instead of after every UpdateMessage / UpdatePage / AddLayer (state/storageproviders.go:246-272, 431-464).  The state
+ * has its own lock; every call applies atomically in call order and a rejected call leaves the state unchanged.
+ *   Rows     one page row per page id (pageMap).  The calls that create rows return them; a row stays valid until the
+ *            next tgi_state_set.  TGI_STATE_NO_PAGE names no page.
+ *   Pages    tgi_state_page: the nine strings (TGI_PS_*, in that order, back to back at strs[str_off]), depth, and the
+ *            timestamp: ts_sec / ts_nsec (0 <= nsec < 1e9) with ts_off = seconds east of UTC (|ts_off| < 86400; a
+ *            page reloaded from state.json keeps the offset it was written with; the zero time is -62135596800, 0, 0)
+ *            or TGI_STATE_TS_LOCAL (time.Now(): rendered in the context's local zone, tgi_set_zone / tz_offset_sec,
+ *            at render time).
+ *   Codes    message status and platform are indices into a string table: 0 "", 1 "unfetched", 2 "fetched",
+ *            3 "failed", 4 "deleted", 5 "resample"; tgi_state_code registers others (or returns the existing code).
+ *   Messages tgi_state_msg.page_id is the row whose id is the message's pageId (normally its own page's).
+ *            tgi_state_set: an index into that call's pages; tgi_state_update_page: a row, or TGI_STATE_NO_PAGE for
+ *            the page being written.  A pageId that names no page of the state cannot be expressed.
+ *   Set      tgi_state_set = SetState (base.go:375-398) / Initialize (:54-93): replaces everything.  layers[k] takes
+ *            the next layers[k].n_pages pages; pages[i] owns the next pages[i].n_msgs messages.  A later layer of the
+ *            same depth replaces the earlier list; a later page with the same id replaces the earlier one (pageMap),
+ *            messages included.  rows (optional, n_pages) gets each page's row.  The resume path: the shim parses
+ *            state.json itself and hands it over.
+ *   AddLayer tgi_state_add_layer = AddLayer (base.go:219-322) for pages without messages: skips URLs already in the
+ *            state or earlier in the call; max_pages > 0 caps the state at max_pages pages, past which only as many
+ *            pages as there were "deadend" pages at the call's start are added; every page goes to the layer of
+ *            pages[0].depth (created even if nothing is added).  The caller fills empty ids and zero timestamps
+ *            beforehand (uuid.New(), time.Now()).  rows (optional) gets each page's row or TGI_STATE_NO_PAGE (skipped).
+ *   Update   tgi_state_update_page = UpdatePage (base.go:123-149): replaces the page with that id (a new row if none)
+ *            and its whole message list; the row is appended to the layer of its depth only if that layer exists and
+ *            does not hold it.
+ *   Messages tgi_state_update_messages = UpdateMessage (base.go:182-215) once per update, in order: the first message
+ *            of the row with that (chat_id, message_id) takes the status, an unknown key is appended as {chat, msg,
+ *            status, pageId = the page} and later updates of it hit the appended message.  An update whose row is
+ *            TGI_STATE_NO_PAGE is skipped and counted in *skipped (the reference returns an error its caller ignores).
+ *   Read     tgi_state_read_page = GetPage(id).Messages: *n = the row's message count; the messages are written
+ *            when cap >= *n.
+ *   Render   tgi_state_render = json.Marshal(GetState()) (base.go:345-372), byte for byte: {"layers":[...],
+ *            "metadata":<metadata>,"lastUpdated":<last_updated>} where the two spliced values are the shim's own
+ *            json.Marshal of CrawlMetadata and of the time.  Layers in ascending depth (Go iterates layerMap in
+ *            random order: every order is a valid json.Marshal output, this one is fixed); omitempty strings and
+ *            empty message lists are left out; strings use encoding/json's HTML-safe escaping.  A timestamp whose
+ *            year leaves [0, 9999] is TGI_E_ARG (json.Marshal's error).  The bytes live in library-owned pinned
+ *            memory until the next state call.
+ *   Errors   TGI_E_ARG: malformed input (string ranges, layer / message counts, an unknown code, a row that is
+ *            neither a row nor TGI_STATE_NO_PAGE, nsec / offset out of range, messages in tgi_state_add_layer);
+ *            TGI_E_NOMEM.  More than 2^32 - 2 message rows is TGI_E_CAPACITY.                                     */
+#define TGI_STATE_NO_PAGE 0xFFFFFFFFu
+#define TGI_STATE_TS_LOCAL 0x7FFFFFFF
+enum { TGI_PS_ID, TGI_PS_URL, TGI_PS_STATUS, TGI_PS_ERROR, TGI_PS_PLATFORM, TGI_PS_PARENT, TGI_PS_CONN, TGI_PS_SEQ,
+       TGI_PS_CRAWL, TGI_PS_COUNT };
+typedef struct tgi_state_page { /* 72 bytes: one state.Page without its messages */
+  uint64_t str_off;                  /* id | url | status | error | platform | parentId | LastConnectionID |
+                                        sequenceId | crawlId, back to back                                     */
+  uint32_t str_len[TGI_PS_COUNT];
+  int32_t ts_off;                    /* seconds east of UTC, or TGI_STATE_TS_LOCAL                             */
+  int64_t depth;
+  int64_t ts_sec;
+  int32_t ts_nsec;
+  uint32_t n_msgs;                   /* tgi_state_set / tgi_state_update_page: its messages                    */
+} tgi_state_page;
+typedef struct tgi_state_msg { /* 24 bytes: one state.Message */
+  int64_t chat_id, message_id;
+  uint32_t page_id;                  /* see Messages above                                                     */
+  uint16_t status, platform;         /* codes                                                                  */
+} tgi_state_msg;
+typedef struct tgi_state_update { /* 24 bytes: the arguments of one UpdateMessage */
+  int64_t chat_id, message_id;
+  uint32_t row;                      /* the page (TGI_STATE_NO_PAGE: not found)                                */
+  uint16_t status, reserved;
+} tgi_state_update;
+typedef struct tgi_state_layer { int64_t depth; uint64_t n_pages; } tgi_state_layer;
+typedef struct tgi_state_json_t {
+  const uint8_t* data;  uint64_t len;  /* state.json, pinned                                                    */
+  float kernel_ms;                     /* device time of the render's kernels and scans (not the read-back)     */
+  uint32_t gpu_launches;
+} tgi_state_json_t;
+int tgi_state_code(tgi_ctx* ctx, const char* s, uint32_t len, uint16_t* code);
+int tgi_state_set(tgi_ctx* ctx, const tgi_state_layer* layers, uint32_t n_layers, const tgi_state_page* pages,
+                  uint64_t n_pages, const uint8_t* strs, uint64_t strs_len, const tgi_state_msg* msgs, uint64_t n_msgs,
+                  uint32_t* rows);
+int tgi_state_add_layer(tgi_ctx* ctx, const tgi_state_page* pages, uint64_t n, const uint8_t* strs, uint64_t strs_len,
+                        int64_t max_pages, uint32_t* rows);
+int tgi_state_update_page(tgi_ctx* ctx, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                          const tgi_state_msg* msgs, uint32_t* row);
+int tgi_state_update_messages(tgi_ctx* ctx, const tgi_state_update* ups, uint64_t n, uint64_t* skipped);
+int tgi_state_read_page(tgi_ctx* ctx, uint32_t row, tgi_state_msg* out, uint64_t cap, uint64_t* n);
+int tgi_state_render(tgi_ctx* ctx, const uint8_t* metadata, uint64_t metadata_len, const uint8_t* last_updated,
+                     uint64_t last_updated_len, tgi_state_json_t* out);
+
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
                          uint8_t* reason);
