@@ -192,6 +192,17 @@ class StateJsonC(C.Structure):  # tgi_state_json_t
     _fields_ = [("data", C.c_void_p), ("len", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+E_NOPAGES = -7  # tgi_state_export: the layer map holds no page ("no pages found to export")
+STATE_EXPORT_DAPR, STATE_EXPORT_LOCAL = 0, 1
+STATE_EXPORT_CHUNK_DEFAULT = 100 * 1024 * 1024  # exportChunkSizeBytes (state/daprstate.go:2909)
+
+
+class StateExportC(C.Structure):  # tgi_state_export_t
+    _fields_ = [("data", C.c_void_p), ("off", C.POINTER(C.c_uint64)), ("len", C.POINTER(C.c_uint64)),
+                ("raw_len", C.POINTER(C.c_uint64)), ("n_chunks", C.c_uint64), ("n_pages", C.c_uint64),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 class StatsC(C.Structure):
     _fields_ = [("records", C.c_uint64), ("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64),
                 ("links", C.c_uint64), ("frontier_size", C.c_uint64), ("launches", C.c_uint64),

@@ -15,6 +15,9 @@
 // inside a row = storage order); a thread per message sizes it, a warp per entry (a page of a layer, or an empty layer)
 // sizes the page around its messages, scans place both, and the emit writes every byte at its final offset: a warp per
 // entry for the page's fields, a thread per (entry, message) slot for the messages.
+//
+// DaprStateManager's side: the exports (daprstate.go:2911-3012, storageproviders.go:550-587) run the same passes with
+// st_entry in line mode, one {page}\n per entry; json.Marshal(layerMap) (daprstate.go:947) is a thread per listed id.
 #pragma once
 #include "local_appends.cuh"
 
@@ -299,8 +302,10 @@ __global__ void st_msg_size_kernel(StDev d, StRender r, const uint32_t* sorted, 
 }
 
 // one entry, sized or written by a warp (lane 0 writes the literals, the warp escapes the strings).  Returns the bytes
-// of part A (framing and fields up to the first message) in *a and of the whole entry without messages.
-template <bool EMIT>
+// of part A (framing and fields up to the first message) in *a and of the whole entry without messages.  LINE: the
+// page alone as one JSONL line, {page}\n, without layer framing (the exports).  A template parameter rather than an
+// entry flag: the flag cost the render's emit kernel 8 bytes of spills.
+template <bool EMIT, bool LINE = false>
 DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint32_t cnt, uint8_t* dst, uint64_t msg_bytes,
                        uint32_t* a, bool* bad) {
   const bool l0 = lane_id() == 0;
@@ -319,7 +324,8 @@ DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint
     const uint8_t* s = st_str(d, p, f, n);
     o += EMIT ? esc_to_global(dst + o, s, n) : warp_esc_len(s, n);
   };
-  if (e.flags & ST_E_FIRST) {
+  if (LINE) {
+  } else if (e.flags & ST_E_FIRST) {
     if (!(e.flags & ST_E_FIRST_LAYER)) lit(",", 1);
     lit("{\"depth\":", 9);
     num(e.depth);
@@ -375,14 +381,16 @@ DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint
   } else {
     *a = (uint32_t)o;
   }
-  if (e.flags & ST_E_LAST) lit("]}", 2);
+  if (LINE) lit("\n", 1);
+  else if (e.flags & ST_E_LAST) lit("]}", 2);
   return (uint32_t)(o - msg_bytes);
 }
 
 constexpr int ST_WARPS = 8;  // warps per CTA of the warp-per-entry kernels
 
 // size pass, a warp per entry: the entry's bytes around its messages, its message count and message bytes
-__global__ void __launch_bounds__(ST_WARPS * 32) st_entry_size_kernel(StDev d, StRender r) {
+template <bool LINE>
+DEVI void st_entry_size(const StDev& d, const StRender& r) {
   const uint64_t w0 = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5, nw = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   for (uint64_t e = w0; e < r.n_entries; e += nw) {
     const StEntry en = r.entries[e];
@@ -395,7 +403,7 @@ __global__ void __launch_bounds__(ST_WARPS * 32) st_entry_size_kernel(StDev d, S
     }
     uint32_t a;
     bool bad = false;
-    const uint32_t sz = st_entry<false>(d, r, en, cnt, nullptr, mb, &a, &bad);
+    const uint32_t sz = st_entry<false, LINE>(d, r, en, cnt, nullptr, mb, &a, &bad);
     if (lane_id() == 0) {
       r.esize_lo[e] = a;
       r.ebytes[e] = sz;
@@ -408,7 +416,8 @@ __global__ void __launch_bounds__(ST_WARPS * 32) st_entry_size_kernel(StDev d, S
 }
 
 // emit, a warp per entry: everything but the messages
-__global__ void __launch_bounds__(ST_WARPS * 32) st_entry_emit_kernel(StDev d, StRender r) {
+template <bool LINE>
+DEVI void st_entry_emit(const StDev& d, const StRender& r) {
   const uint64_t w0 = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5, nw = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   for (uint64_t e = w0; e < r.n_entries; e += nw) {
     const StEntry en = r.entries[e];
@@ -416,10 +425,16 @@ __global__ void __launch_bounds__(ST_WARPS * 32) st_entry_emit_kernel(StDev d, S
     const uint64_t mb = r.eoff[e + 1] - off - r.ebytes[e];
     uint32_t a;
     bool bad = false;
-    st_entry<true>(d, r, en, r.ecnt[e], r.out + off, mb, &a, &bad);
+    st_entry<true, LINE>(d, r, en, r.ecnt[e], r.out + off, mb, &a, &bad);
     __syncwarp();
   }
 }
+
+__global__ void __launch_bounds__(ST_WARPS * 32) st_entry_size_kernel(StDev d, StRender r) { st_entry_size<false>(d, r); }
+__global__ void __launch_bounds__(ST_WARPS * 32) st_entry_emit_kernel(StDev d, StRender r) { st_entry_emit<false>(d, r); }
+// the same for the exports' JSONL lines
+__global__ void __launch_bounds__(ST_WARPS * 32) st_line_size_kernel(StDev d, StRender r) { st_entry_size<true>(d, r); }
+__global__ void __launch_bounds__(ST_WARPS * 32) st_line_emit_kernel(StDev d, StRender r) { st_entry_emit<true>(d, r); }
 
 // emit, a thread per message slot of the output: slot t is message k of entry e (binary search over eslot)
 __global__ void st_msg_emit_kernel(StDev d, StRender r, const uint32_t* sorted) {
@@ -435,6 +450,54 @@ __global__ void st_msg_emit_kernel(StDev d, StRender r, const uint32_t* sorted) 
     const uint64_t b = r.row_base[r.entries[e].row], q = b + k;
     st_message<true>(d, d.msgs[sorted[q]], k != 0, r.out + r.eoff[e] + r.esize_lo[e] + (r.moff[q] - r.moff[b]));
   }
+}
+
+// ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------
+struct StLmEntry {  // one id of a layer, or an empty layer (row == ST_NONE)
+  uint32_t row;
+  uint32_t pre;      // the layer's opening [,]"<depth>":[ in StLm::keys, written by its first entry
+  uint32_t pre_len;  // 0: not the layer's first entry
+  uint32_t last;     // 1: the entry closes the layer with ]
+};
+struct StLm {
+  const StLmEntry* entries;
+  uint64_t n;
+  const uint8_t* keys;
+  uint32_t* size;  // [n] bytes of entry e
+  uint64_t* off;   // [n+1] their scan
+  uint8_t* out;
+};
+
+// one entry, sized (EMIT false) or written: [opening][,]"<escaped id>"[]]
+template <bool EMIT>
+DEVI uint32_t st_lm_entry(const StDev& d, const StLm& L, const StLmEntry& e, uint8_t* dst) {
+  uint32_t o = 0;
+  auto ch = [&](uint32_t c) {
+    if (EMIT) dst[o] = (uint8_t)c;
+    o++;
+  };
+  if (EMIT)
+    for (uint32_t k = 0; k < e.pre_len; k++) dst[k] = L.keys[e.pre + k];
+  o += e.pre_len;
+  if (e.row != ST_NONE) {
+    if (!e.pre_len) ch(',');
+    ch('"');
+    uint32_t il;
+    const uint8_t* id = st_str(d, d.pages[e.row], TGI_PS_ID, il);
+    o += EMIT ? st_thread_esc(dst + o, id, il) : thread_esc_len(id, il);
+    ch('"');
+  }
+  if (e.last) ch(']');
+  return o;
+}
+
+__global__ void st_lm_size_kernel(StDev d, StLm L) {
+  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < L.n; e += (uint64_t)gridDim.x * blockDim.x)
+    L.size[e] = st_lm_entry<false>(d, L, L.entries[e], nullptr);
+}
+__global__ void st_lm_emit_kernel(StDev d, StLm L) {
+  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < L.n; e += (uint64_t)gridDim.x * blockDim.x)
+    st_lm_entry<true>(d, L, L.entries[e], L.out + L.off[e]);
 }
 
 }  // namespace tgi

@@ -191,6 +191,7 @@ struct CrawlState {
   std::mutex mu;
   cudaStream_t stream = nullptr;
   cudaEvent_t t0 = nullptr, t1 = nullptr, t2 = nullptr, t3 = nullptr;  // the render's size pass and emit
+  cudaEvent_t t4 = nullptr, t5 = nullptr;                              // the export's base64 encode
   std::vector<tgi_state_page> rows;  // str_off into blob
   std::string blob;
   std::vector<uint32_t> gen;         // mirror of row_gen
@@ -207,7 +208,8 @@ struct CrawlState {
   DevBuf pages, dblob, row_gen, row_cnt, msgs, table, code_blob, code_off;
   DevBuf upd, bfirst, blast, slot_of, flag, pos, tiles, sc, spare;  // scratch
   DevBuf entries, keys, vals, row_base, msize, moff, e32, e64, counts, roff, out;
-  HostBuf h_out, h_sc, h_read;
+  DevBuf lm_keys, cb_tasks, cb_segs, b64;  // the layer map's openings; the export's encode tasks and output
+  HostBuf h_out, h_sc, h_read, h_chunks;
 };
 
 struct Slot {
@@ -1953,7 +1955,7 @@ void tgi_destroy(tgi_ctx* c) {
     cudaStreamSynchronize(c->state.stream);
     cudaStreamDestroy(c->state.stream);
   }
-  for (cudaEvent_t e : {c->state.t0, c->state.t1, c->state.t2, c->state.t3}) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : {c->state.t0, c->state.t1, c->state.t2, c->state.t3, c->state.t4, c->state.t5}) if (e) cudaEventDestroy(e);
   delete c;  // the device and pinned buffers free themselves
 }
 
@@ -3266,6 +3268,8 @@ int st_init(tgi_ctx* c, CrawlState& S) {
   CK(cudaEventCreate(&S.t1));
   CK(cudaEventCreate(&S.t2));
   CK(cudaEventCreate(&S.t3));
+  CK(cudaEventCreate(&S.t4));
+  CK(cudaEventCreate(&S.t5));
   for (const char* s : kPresetCodes) {
     S.code_of[s] = (uint16_t)S.codes.size();
     S.codes.push_back(s);
@@ -3445,6 +3449,105 @@ int st_drop_messages(tgi_ctx* c, CrawlState& S, uint32_t r) {
   if ((rc = st_row_count(c, S, r, &cnt))) return rc;
   S.n_dead += cnt;
   S.gen[r]++;
+  return TGI_OK;
+}
+
+// the entries' bytes in S.out by the render's two passes, their offsets in S.e64 ([ne+1]); *body = their length,
+// *size_ms = the size pass.  The emit is enqueued behind S.t2 and ends at S.t3, not waited for.
+int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bool lines, const char* who, uint64_t* body,
+                    float* size_ms, uint32_t& launches) {
+  const uint64_t ne = E.size(), nr = S.rows.size(), nm = S.n_msgs, live = nm - S.n_dead;
+  cudaStream_t st = S.stream;
+  int rc;
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.flag.ensure(nm * 4));
+  CK(S.pos.ensure((nm + 1) * 8));
+  CK(S.keys.ensure(2 * live * 4));
+  CK(S.vals.ensure(2 * live * 4));
+  CK(S.row_base.ensure((nr + 1) * 8));
+  CK(S.msize.ensure(live * 4));
+  CK(S.moff.ensure((live + 1) * 8));
+  CK(S.entries.ensure(ne * sizeof(StEntry)));
+  CK(S.e32.ensure(4 * ne * 4));
+  CK(S.e64.ensure(2 * (ne + 1) * 8));
+  StRender r{};
+  r.entries = S.entries.as<StEntry>();
+  r.n_entries = ne;
+  r.zone = c->cfgdev.zone;
+  r.zone_n = c->cfgdev.zone_n;
+  r.tz = c->cfgdev.tz;
+  r.sc = S.sc.as<uint64_t>();
+  r.flag = S.flag.as<uint32_t>();
+  r.pos = S.pos.as<uint64_t>();
+  r.keys[0] = S.keys.as<uint32_t>();
+  r.keys[1] = r.keys[0] + live;
+  r.vals[0] = S.vals.as<uint32_t>();
+  r.vals[1] = r.vals[0] + live;
+  r.row_base = S.row_base.as<uint64_t>();
+  r.msize = S.msize.as<uint32_t>();
+  r.moff = S.moff.as<uint64_t>();
+  r.esize_lo = S.e32.as<uint32_t>();
+  r.ebytes = r.esize_lo + ne;
+  r.ecnt = r.ebytes + ne;
+  r.esz = r.ecnt + ne;
+  r.eoff = S.e64.as<uint64_t>();
+  r.eslot = r.eoff + ne + 1;
+  // radix passes over the bits of the largest row
+  uint32_t bits = 0;
+  while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
+  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
+  const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
+  CK(S.counts.ensure(radix * ntiles * 4));
+  CK(S.roff.ensure((radix * ntiles + 1) * 8));
+  const StDev d = st_dev(S);
+  CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+  CK(cudaEventRecord(S.t0, st));
+  st_render_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, r.sc + ST_SC_LIVE, launches))) return rc;
+  st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+  launches++;
+  int cur = 0;
+  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
+    const uint32_t shift = p * width;
+    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                   S.counts.as<uint32_t>());
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), r.sc + ST_SC_RADIX, launches))) return rc;
+    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.vals[cur], r.keys[cur ^ 1], r.vals[cur ^ 1],
+                                                                      r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                      S.roff.as<uint64_t>());
+    launches++;
+  }
+  if ((rc = launch_scan(c, st, S.tiles, d.row_cnt, nr, r.row_base, r.sc + ST_SC_ROWS, launches))) return rc;
+  st_msg_size_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, r, r.vals[cur], r.keys[cur], live);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, r.msize, live, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
+  (lines ? st_line_size_kernel : st_entry_size_kernel)<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, r.esz, ne, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, r.ecnt, ne, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t* h = S.h_sc.as<uint64_t>();
+  if (h[ST_SC_LIVE] != live) { set_err(c, "%s: %llu live messages, expected %llu", who, (unsigned long long)h[ST_SC_LIVE], (unsigned long long)live); return TGI_E_CUDA; }
+  if (h[ST_SC_ERR]) { set_err(c, "%s: a page timestamp's year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  if (h[ST_SC_BIG]) { set_err(c, "%s: a page renders to 4 GiB or more", who); return TGI_E_CAPACITY; }
+  *body = h[ST_SC_BYTES];
+  const uint64_t slots = h[ST_SC_SLOTS];
+  cudaEventElapsedTime(size_ms, S.t0, S.t1);
+  CK(S.out.ensure(*body));
+  r.out = S.out.as<uint8_t>();
+  CK(cudaEventRecord(S.t2, st));
+  (lines ? st_line_emit_kernel : st_entry_emit_kernel)<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
+  if (slots) st_msg_emit_kernel<<<st_grid(c, slots), ST_THREADS, 0, st>>>(d, r, r.vals[cur]);
+  launches += 1 + (slots != 0);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
   return TGI_OK;
 }
 
@@ -3733,104 +3836,15 @@ int tgi_state_render(tgi_ctx* c, const uint8_t* metadata, uint64_t metadata_len,
       E.push_back(StEntry{(long long)depth, L[k], (k == 0 ? ST_E_FIRST | fl : 0u) | (k + 1 == L.size() ? (uint32_t)ST_E_LAST : 0u)});
   }
   static const char kHead[] = "{\"layers\":[", kMeta[] = "],\"metadata\":", kLast[] = ",\"lastUpdated\":";
-  const uint64_t ne = E.size(), nr = S.rows.size(), nm = S.n_msgs, live = nm - S.n_dead;
   cudaStream_t st = S.stream;
   uint32_t launches = 0;
   uint64_t body = 0;
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
   // the zone table must not change under the kernels that read it (tgi_set_zone swaps it under cfg_mu)
   std::lock_guard<std::mutex> zg(c->cfg_mu);
-  if (ne) {
-    CK(S.flag.ensure(nm * 4));
-    CK(S.pos.ensure((nm + 1) * 8));
-    CK(S.keys.ensure(2 * live * 4));
-    CK(S.vals.ensure(2 * live * 4));
-    CK(S.row_base.ensure((nr + 1) * 8));
-    CK(S.msize.ensure(live * 4));
-    CK(S.moff.ensure((live + 1) * 8));
-    CK(S.entries.ensure(ne * sizeof(StEntry)));
-    CK(S.e32.ensure(4 * ne * 4));
-    CK(S.e64.ensure(2 * (ne + 1) * 8));
-    StRender r{};
-    r.entries = S.entries.as<StEntry>();
-    r.n_entries = ne;
-    r.zone = c->cfgdev.zone;
-    r.zone_n = c->cfgdev.zone_n;
-    r.tz = c->cfgdev.tz;
-    r.sc = S.sc.as<uint64_t>();
-    r.flag = S.flag.as<uint32_t>();
-    r.pos = S.pos.as<uint64_t>();
-    r.keys[0] = S.keys.as<uint32_t>();
-    r.keys[1] = r.keys[0] + live;
-    r.vals[0] = S.vals.as<uint32_t>();
-    r.vals[1] = r.vals[0] + live;
-    r.row_base = S.row_base.as<uint64_t>();
-    r.msize = S.msize.as<uint32_t>();
-    r.moff = S.moff.as<uint64_t>();
-    r.esize_lo = S.e32.as<uint32_t>();
-    r.ebytes = r.esize_lo + ne;
-    r.ecnt = r.ebytes + ne;
-    r.esz = r.ecnt + ne;
-    r.eoff = S.e64.as<uint64_t>();
-    r.eslot = r.eoff + ne + 1;
-    // radix passes over the bits of the largest row
-    uint32_t bits = 0;
-    while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
-    const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
-    const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
-    CK(S.counts.ensure(radix * ntiles * 4));
-    CK(S.roff.ensure((radix * ntiles + 1) * 8));
-    const StDev d = st_dev(S);
-    CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-    CK(cudaEventRecord(S.t0, st));
-    st_render_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, r.sc + ST_SC_LIVE, launches))) return rc;
-    st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
-    launches++;
-    int cur = 0;
-    for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
-      const uint32_t shift = p * width;
-      la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                     S.counts.as<uint32_t>());
-      launches++;
-      if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), r.sc + ST_SC_RADIX, launches))) return rc;
-      la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.vals[cur], r.keys[cur ^ 1], r.vals[cur ^ 1],
-                                                                        r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                        S.roff.as<uint64_t>());
-      launches++;
-    }
-    if ((rc = launch_scan(c, st, S.tiles, d.row_cnt, nr, r.row_base, r.sc + ST_SC_ROWS, launches))) return rc;
-    st_msg_size_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, r, r.vals[cur], r.keys[cur], live);
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, r.msize, live, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
-    st_entry_size_kernel<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, r.esz, ne, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
-    if ((rc = launch_scan(c, st, S.tiles, r.ecnt, ne, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(S.t1, st));
-    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const uint64_t* h = S.h_sc.as<uint64_t>();
-    if (h[ST_SC_LIVE] != live) { set_err(c, "tgi_state_render: %llu live messages, expected %llu", (unsigned long long)h[ST_SC_LIVE], (unsigned long long)live); return TGI_E_CUDA; }
-    if (h[ST_SC_ERR]) { set_err(c, "tgi_state_render: a page timestamp's year is outside [0, 9999] (json.Marshal fails)"); return TGI_E_ARG; }
-    if (h[ST_SC_BIG]) { set_err(c, "tgi_state_render: a page renders to 4 GiB or more"); return TGI_E_CAPACITY; }
-    body = h[ST_SC_BYTES];
-    const uint64_t slots = h[ST_SC_SLOTS];
+  if (!E.empty()) {
     float size_ms = 0, emit_ms = 0;
-    cudaEventElapsedTime(&size_ms, S.t0, S.t1);
-    CK(S.out.ensure(body));
+    if ((rc = st_emit_entries(c, S, E, false, "tgi_state_render", &body, &size_ms, launches))) return rc;
     CK(S.h_out.ensure(sizeof kHead + body + sizeof kMeta + metadata_len + sizeof kLast + last_updated_len + 2));
-    r.out = S.out.as<uint8_t>();
-    CK(cudaEventRecord(S.t2, st));
-    st_entry_emit_kernel<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
-    if (slots) st_msg_emit_kernel<<<st_grid(c, slots), ST_THREADS, 0, st>>>(d, r, r.vals[cur]);
-    launches += 1 + (slots != 0);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(S.t3, st));
     CK(cudaMemcpyAsync(S.h_out.as<uint8_t>() + sizeof kHead - 1, S.out.p, body, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
@@ -3853,6 +3867,203 @@ int tgi_state_render(tgi_ctx* c, const uint8_t* metadata, uint64_t metadata_len,
   o[k++] = '}';
   out->data = o;
   out->len = k;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// Dapr's AddLayer after the caller's urlCache test (daprstate.go:625-780): pageMap[id] = page, the row appended to the
+// layer `depth`; the URL map and the deadend count stay right for later tgi_state_add_layer calls
+int tgi_state_add_pages(tgi_ctx* c, int64_t depth, const tgi_state_page* pages, uint64_t n, const uint8_t* strs,
+                        uint64_t strs_len, uint32_t* rows) {
+  if (!c || (n && !pages)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if (!n) return TGI_OK;  // daprstate.go:658-662: every page was a duplicate, no layer is created
+  for (uint64_t i = 0; i < n; i++) {
+    if (!page_ok(c, pages[i], strs, strs_len, "tgi_state_add_pages")) return TGI_E_ARG;
+    if (pages[i].n_msgs) { set_err(c, "tgi_state_add_pages: page %llu carries messages", (unsigned long long)i); return TGI_E_ARG; }
+  }
+  std::vector<uint32_t>& L = S.layers[depth];
+  std::vector<uint32_t> dirty;
+  for (uint64_t i = 0; i < n; i++) {
+    const auto it = S.by_id.find(in_field(pages[i], strs, TGI_PS_ID));
+    uint32_t r = (uint32_t)S.rows.size();
+    if (it != S.by_id.end()) {  // the old page and its messages go
+      r = it->second;
+      if (std::find(dirty.begin(), dirty.end(), r) == dirty.end()) {
+        if (r < S.rows_synced && (rc = st_drop_messages(c, S, r))) return rc;
+        dirty.push_back(r);
+      }
+    }
+    st_put_row(S, r, pages[i], strs);
+    L.push_back(r);
+    if (rows) rows[i] = r;
+  }
+  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  return st_compact(c, S);
+}
+
+// json.Marshal(map[int][]string): the keys' order and the layers' openings on the host, every id sized and written by
+// one thread on the device
+int tgi_state_layer_map(tgi_ctx* c, tgi_state_json_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  std::vector<std::pair<std::string, const std::vector<uint32_t>*>> K;
+  for (const auto& [depth, L] : S.layers) K.emplace_back(std::to_string(depth), &L);
+  std::sort(K.begin(), K.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  std::string keys;
+  std::vector<StLmEntry> E;
+  for (const auto& [key, L] : K) {
+    const uint32_t pre = (uint32_t)keys.size();
+    keys += (pre ? ",\"" : "\"") + key + "\":[";
+    const uint32_t pl = (uint32_t)keys.size() - pre;
+    if (L->empty()) E.push_back(StLmEntry{ST_NONE, pre, pl, 1});
+    for (size_t k = 0; k < L->size(); k++) E.push_back(StLmEntry{(*L)[k], pre, k ? 0u : pl, k + 1 == L->size() ? 1u : 0u});
+  }
+  const uint64_t ne = E.size();
+  cudaStream_t st = S.stream;
+  uint32_t launches = 0;
+  uint64_t body = 0;
+  if (ne) {
+    CK(S.entries.ensure(ne * sizeof(StLmEntry)));
+    CK(S.lm_keys.ensure(keys.size()));
+    CK(S.e32.ensure(ne * 4));
+    CK(S.e64.ensure((ne + 1) * 8));
+    CK(S.sc.ensure(ST_SC_COUNT * 8));
+    CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+    StLm L{};
+    L.entries = S.entries.as<StLmEntry>();
+    L.n = ne;
+    L.keys = S.lm_keys.as<uint8_t>();
+    L.size = S.e32.as<uint32_t>();
+    L.off = S.e64.as<uint64_t>();
+    const StDev d = st_dev(S);
+    CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StLmEntry), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(S.lm_keys.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(S.t0, st));
+    st_lm_size_kernel<<<st_grid(c, ne), ST_THREADS, 0, st>>>(d, L);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, L.size, ne, L.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t1, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.as<uint64_t>() + ST_SC_BYTES, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    body = *S.h_sc.as<uint64_t>();
+    CK(S.out.ensure(body));
+    CK(S.h_out.ensure(body + 2));
+    L.out = S.out.as<uint8_t>();
+    CK(cudaEventRecord(S.t2, st));
+    st_lm_emit_kernel<<<st_grid(c, ne), ST_THREADS, 0, st>>>(d, L);
+    launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t3, st));
+    CK(cudaMemcpyAsync(S.h_out.as<uint8_t>() + 1, S.out.p, body, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    float size_ms = 0, emit_ms = 0;
+    cudaEventElapsedTime(&size_ms, S.t0, S.t1);
+    cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
+    out->kernel_ms = size_ms + emit_ms;
+  } else {
+    CK(S.h_out.ensure(2));
+  }
+  uint8_t* o = S.h_out.as<uint8_t>();
+  o[0] = '{';
+  o[body + 1] = '}';
+  out->data = o;
+  out->len = body + 2;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// the pages as JSONL lines by the render's passes (st_entry in line mode); Dapr mode cuts them into chunks at the
+// line ends on the host and base64-encodes every chunk with the combiner's encoder, each into its own 16-byte aligned
+// range of the output
+int tgi_state_export(tgi_ctx* c, int mode, uint64_t chunk_bytes, tgi_state_export_t* out) {
+  if (!c || !out || (mode != TGI_STATE_EXPORT_DAPR && mode != TGI_STATE_EXPORT_LOCAL)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if ((rc = st_upload_codes(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  std::vector<StEntry> E;
+  if (mode == TGI_STATE_EXPORT_DAPR) {
+    for (const auto& [depth, L] : S.layers)
+      for (uint32_t r : L) E.push_back(StEntry{(long long)depth, r, 0});
+    if (E.empty()) { set_err(c, "tgi_state_export: no pages found to export"); return TGI_E_NOPAGES; }
+  } else {
+    for (uint32_t r = 0; r < (uint32_t)S.rows.size(); r++) E.push_back(StEntry{S.rows[r].depth, r, 0});
+  }
+  const uint64_t ne = E.size();
+  cudaStream_t st = S.stream;
+  uint32_t launches = 0;
+  uint64_t body = 0;
+  float size_ms = 0, emit_ms = 0, enc_ms = 0;
+  std::lock_guard<std::mutex> zg(c->cfg_mu);  // the zone table, as in tgi_state_render
+  if (ne && (rc = st_emit_entries(c, S, E, true, "tgi_state_export", &body, &size_ms, launches))) return rc;
+  // chunk k's raw bytes are [start[k], start[k+1]) of S.out
+  std::vector<uint64_t> start(1, 0);
+  if (mode == TGI_STATE_EXPORT_DAPR) {
+    std::vector<uint64_t> eoff(ne + 1);
+    CK(cudaMemcpyAsync(eoff.data(), S.e64.p, (ne + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (uint64_t s = 0; s < body;) {  // the first line end at or past s + chunk_bytes (every line is longer than 0)
+      const uint64_t want = chunk_bytes > body - s ? body + 1 : std::max<uint64_t>(s + chunk_bytes, s + 1);
+      const auto it = std::lower_bound(eoff.begin() + 1, eoff.end(), want);
+      s = it == eoff.end() ? body : *it;
+      start.push_back(s);
+    }
+  } else {
+    start.push_back(body);
+  }
+  const uint64_t nc = start.size() - 1;
+  CK(S.h_chunks.ensure(3 * nc * 8 + 8));
+  uint64_t* off = S.h_chunks.as<uint64_t>();
+  uint64_t *len = off + nc, *raw = len + nc, total = 0;
+  const bool enc = mode == TGI_STATE_EXPORT_DAPR;
+  for (uint64_t k = 0; k < nc; k++) {
+    raw[k] = start[k + 1] - start[k];
+    len[k] = enc ? (raw[k] + 2) / 3 * 4 : raw[k];
+    off[k] = total;
+    total = enc ? (total + len[k] + 15) & ~15ull : total + len[k];
+  }
+  CK(S.h_out.ensure(total));
+  if (enc) {
+    CK(S.b64.ensure(total));
+    CbPlan P;
+    for (uint64_t k = 0; k < nc; k++)
+      P.add(S.b64.as<uint8_t>() + off[k], true, {CbSeg{0, raw[k], S.out.as<uint8_t>() + start[k]}});
+    const bool tables = P.t.size() > (size_t)CB_INLINE || P.s.size() > (size_t)CB_INLINE;
+    if (tables) {
+      CK(S.cb_tasks.ensure(P.t.size() * sizeof(CbTask)));
+      CK(S.cb_segs.ensure(P.s.size() * sizeof(CbSeg)));
+      CK(cudaMemcpyAsync(S.cb_tasks.p, P.t.data(), P.t.size() * sizeof(CbTask), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(S.cb_segs.p, P.s.data(), P.s.size() * sizeof(CbSeg), cudaMemcpyHostToDevice, st));
+    }
+    CK(cudaEventRecord(S.t4, st));
+    if ((rc = cb_launch(c, st, P, S.cb_tasks.as<CbTask>(), S.cb_segs.as<CbSeg>(), nullptr, launches))) return rc;
+    CK(cudaEventRecord(S.t5, st));
+    if (total) CK(cudaMemcpyAsync(S.h_out.p, S.b64.p, total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));  // also keeps P's inline tasks alive until the launch has read them
+    cudaEventElapsedTime(&enc_ms, S.t4, S.t5);
+  } else if (total) {
+    CK(cudaMemcpyAsync(S.h_out.p, S.out.p, total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  if (ne) cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
+  out->data = S.h_out.as<uint8_t>();
+  out->off = off;
+  out->len = len;
+  out->raw_len = raw;
+  out->n_chunks = nc;
+  out->n_pages = ne;
+  out->kernel_ms = size_ms + emit_ms + enc_ms;
   out->gpu_launches = launches;
   return TGI_OK;
 }

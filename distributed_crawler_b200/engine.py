@@ -37,7 +37,8 @@ EXPORTED_SYMBOLS = [
     "tgi_set_add", "tgi_set_clear", "tgi_set_size", "tgi_set_now", "tgi_pending_edges", "tgi_plan_channel_appends",
     "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
     "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
-    "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render",
+    "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
+    "tgi_state_add_pages", "tgi_state_export",
 ]
 
 
@@ -112,6 +113,9 @@ def lib() -> C.CDLL:
         L.tgi_state_update_messages.argtypes = [vp, vp, u64, C.POINTER(u64)]
         L.tgi_state_read_page.argtypes = [vp, u32, vp, u64, C.POINTER(u64)]
         L.tgi_state_render.argtypes = [vp, vp, u64, vp, u64, C.POINTER(abi.StateJsonC)]
+        L.tgi_state_layer_map.argtypes = [vp, C.POINTER(abi.StateJsonC)]
+        L.tgi_state_add_pages.argtypes = [vp, C.c_int64, vp, u64, vp, u64, vp]
+        L.tgi_state_export.argtypes = [vp, i32, u64, C.POINTER(abi.StateExportC)]
         _LIB = L
     return _LIB
 
@@ -626,6 +630,39 @@ class Engine:
         self.state_render_ms = float(out.kernel_ms)
         self.state_render_launches = int(out.gpu_launches)
         return C.string_at(out.data, out.len) if copy else _view(out.data, out.len, np.uint8)
+
+    def state_layer_map(self) -> bytes:
+        """json.Marshal(layerMap) of DaprStateManager.SaveState; the device time of the call is left in
+        self.state_layer_map_ms"""
+        out = abi.StateJsonC()
+        self._check(lib().tgi_state_layer_map(self.h, C.byref(out)))
+        self.state_layer_map_ms = float(out.kernel_ms)
+        self.state_layer_map_launches = int(out.gpu_launches)
+        return C.string_at(out.data, out.len)
+
+    def state_add_pages(self, depth: int, pages) -> list[int]:
+        """Dapr's AddLayer once the caller has dropped the pages its urlCache holds: every page stored and appended to
+        the layer `depth` (pages[0]'s depth before the filtering); each page's row"""
+        from .state_pack import pack_pages
+        recs, strs, _ = pack_pages(pages, self.state_code, lambda pid, i: i)  # messages are refused by the library
+        rows = np.zeros(max(len(pages), 1), np.uint32)
+        self._check(lib().tgi_state_add_pages(self.h, depth, recs.ctypes.data, len(recs), strs.ctypes.data, len(strs),
+                                              rows.ctypes.data))
+        self._st_note_rows(pages, rows[:len(pages)])
+        return [int(r) for r in rows[:len(pages)]]
+
+    def state_export(self, mode: int = abi.STATE_EXPORT_DAPR, chunk_bytes: int = abi.STATE_EXPORT_CHUNK_DEFAULT):
+        """the pages as JSONL chunks: [(data, raw JSONL length), ...], data base64 (abi.STATE_EXPORT_DAPR,
+        ExportPagesToBinding's chunks) or the raw JSONL (abi.STATE_EXPORT_LOCAL, one chunk).  A Dapr export of a layer
+        map without pages raises EngineError with code abi.E_NOPAGES.  The device time is left in
+        self.state_export_ms"""
+        out = abi.StateExportC()
+        self._check(lib().tgi_state_export(self.h, mode, chunk_bytes, C.byref(out)))
+        self.state_export_ms = float(out.kernel_ms)
+        self.state_export_launches = int(out.gpu_launches)
+        self.state_export_pages = int(out.n_pages)
+        return [(C.string_at(out.data + out.off[k], out.len[k]) if out.len[k] else b"", int(out.raw_len[k]))
+                for k in range(out.n_chunks)]
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

@@ -3,6 +3,8 @@
 //                      packs the same messages with pack.py and compares
 //   host_demo --run    processes them on the GPU and prints status, outlinks and the JSONL lines
 //   host_demo --state  the same, then a one-page crawl state (StateSet) rendered as state.json (StateRender)
+//   host_demo --state-dapr  the same state, then a Dapr AddLayer of two pages at depth -1 (StateAddPages), the layer
+//                      map (StateLayerMap) and ExportPagesToBinding's base64 chunks of 100 bytes (StateExport)
 #include <cstdio>
 #include <cstring>
 
@@ -91,7 +93,8 @@ int main(int argc, char** argv) {
       printf("\n");
       fwrite(r.Line(i).data(), 1, r.Line(i).size(), stdout);
     }
-    if (argc > 1 && !strcmp(argv[1], "--state")) {  // one seed page with one message, as state.json
+    const bool dapr = argc > 1 && !strcmp(argv[1], "--state-dapr");
+    if (argc > 1 && (!strcmp(argv[1], "--state") || dapr)) {  // one seed page with one message, as state.json
       tgi_state_page pg{};
       pg.str_len[TGI_PS_ID] = 2, pg.str_len[TGI_PS_URL] = 11, pg.str_len[TGI_PS_STATUS] = 9;
       pg.ts_off = TGI_STATE_TS_LOCAL, pg.ts_sec = 1750000000, pg.n_msgs = 1;
@@ -99,6 +102,20 @@ int main(int argc, char** argv) {
       const std::string_view js = proc.StateRender("{}", "\"2025-06-15T15:06:40Z\"");
       fwrite(js.data(), 1, js.size(), stdout);
       printf("\n");
+    }
+    if (dapr) {
+      tgi_state_page a{}, b{};
+      a.str_len[TGI_PS_ID] = 2, a.str_len[TGI_PS_URL] = 5;
+      b = a;
+      b.str_off = 7;
+      proc.StateAddPages(-1, {a, b}, "p2url-2p3url-3");
+      const std::string_view lm = proc.StateLayerMap();
+      fwrite(lm.data(), 1, lm.size(), stdout);
+      printf("\n");
+      for (std::string_view chunk : proc.StateExport(TGI_STATE_EXPORT_DAPR, 100)) {
+        fwrite(chunk.data(), 1, chunk.size(), stdout);
+        printf("\n");
+      }
     }
   } catch (const std::exception& e) {
     fprintf(stderr, "error: %s\n", e.what());

@@ -314,6 +314,30 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return std::string_view((const char*)o.data, o.len);
   }
+  // DaprStateManager.SaveState's json.Marshal(layerMap); the view stays valid until the next state call
+  std::string_view StateLayerMap() {
+    tgi_state_json_t o{};
+    if (tgi_state_layer_map(ctx_, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return std::string_view((const char*)o.data, o.len);
+  }
+  // Dapr's AddLayer for the pages that passed the caller's urlCache test, into the layer `depth` (pages[0].Depth
+  // before that test); returns every page's row
+  std::vector<uint32_t> StateAddPages(int64_t depth, const std::vector<tgi_state_page>& pages, std::string_view strs) {
+    std::vector<uint32_t> rows(pages.size());
+    if (tgi_state_add_pages(ctx_, depth, pages.data(), pages.size(), (const uint8_t*)strs.data(), strs.size(), rows.data()) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return rows;
+  }
+  // ExportPagesToBinding's chunks (TGI_STATE_EXPORT_DAPR: base64, chunk_bytes as exportChunkSizeBytes) or the local
+  // export's one raw JSONL chunk; the views stay valid until the next state call.  TGI_E_NOPAGES (Dapr: no page in the
+  // layer map) throws like every other error.
+  std::vector<std::string_view> StateExport(int mode, uint64_t chunk_bytes) {
+    tgi_state_export_t o{};
+    if (tgi_state_export(ctx_, mode, chunk_bytes, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    std::vector<std::string_view> v;
+    for (uint64_t k = 0; k < o.n_chunks; k++) v.emplace_back((const char*)o.data + o.off[k], o.len[k]);
+    return v;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

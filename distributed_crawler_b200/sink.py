@@ -170,3 +170,19 @@ def upload_combined_dapr(invoke, blobs, binding: str, naming_key: str) -> int:
     for j in range(blobs.n_blobs):
         invoke(binding, "create", blobs.blob(j), {naming_key: blobs.path(j), "operation": "append"})
     return blobs.n_blobs
+
+
+def export_path(storage_root: str, crawl_cfg_id: str, crawl_id: str, ts: str, part: int) -> str:
+    """ExportPagesToBinding's blob path (state/daprstate.go:2922-2928, generateStoragePath :2669-2677): the directory
+    takes config.CrawlID, the file name the crawlID argument; ts is time.Now().Format("20060102-150405")"""
+    return "%s/%s/analysis/channels/channel-pages-%s-%s-part%d.jsonl" % (storage_root, crawl_cfg_id, crawl_id, ts, part)
+
+
+def export_pages_dapr(eng, storage_root: str, crawl_cfg_id: str, crawl_id: str, ts: str,
+                      chunk_bytes: int = 100 * 1024 * 1024) -> list[tuple[str, bytes]]:
+    """DaprStateManager.ExportPagesToBinding (state/daprstate.go:2911-3012) over the engine's resident state: one
+    (path, base64 data) pair per InvokeBinding call, in order.  Raises EngineError with code abi.E_NOPAGES when the layer
+    map holds no page (the reference's "no pages found to export")."""
+    from . import abi
+    chunks = eng.state_export(abi.STATE_EXPORT_DAPR, chunk_bytes)
+    return [(export_path(storage_root, crawl_cfg_id, crawl_id, ts, k), data) for k, (data, _) in enumerate(chunks)]

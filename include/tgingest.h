@@ -821,6 +821,49 @@ int tgi_state_read_page(tgi_ctx* ctx, uint32_t row, tgi_state_msg* out, uint64_t
 int tgi_state_render(tgi_ctx* ctx, const uint8_t* metadata, uint64_t metadata_len, const uint8_t* last_updated,
                      uint64_t last_updated_len, tgi_state_json_t* out);
 
+/* The same state for DaprStateManager (state/daprstate.go), whose SaveState marshals the whole layer map after every
+ * channel and whose ExportPagesToBinding marshals every page at the end of a crawl.
+ *   LayerMap tgi_state_layer_map = json.Marshal(layerMap), a map[int][]string (daprstate.go:947), byte for byte: the
+ *            keys are the decimal depths sorted as strings (-1, 0, 10, 2), as encoding/json sorts integer map keys; an
+ *            empty layer is [] and an empty map {}; ids use the HTML-safe escaper and a row listed twice is listed
+ *            twice.  Pinned bytes in out, like tgi_state_render's.
+ *   AddPages tgi_state_add_pages = the in-memory part of Dapr's AddLayer (daprstate.go:625-780) once the caller has
+ *            dropped the pages whose URL is in its urlCache (or dropped none, in random-walk mode): every page is
+ *            stored as pageMap[id] = page (an existing id keeps its row and loses its messages) and its row appended to
+ *            the layer `depth`, created if missing; depth is pages[0].Depth BEFORE that filtering.  No URL dedup, no
+ *            max_pages; n = 0 changes nothing (Dapr creates no layer when every page was a duplicate).  rows
+ *            (optional, n) gets each page's row.  Pages carrying messages are TGI_E_ARG.
+ *   Export   tgi_state_export renders every page as one JSONL line, json.Marshal(page) + '\n':
+ *            TGI_STATE_EXPORT_DAPR = DaprStateManager.ExportPagesToBinding (daprstate.go:2911-3012): the pages of the
+ *              layer map in its order (layers in ascending depth, as tgi_state_render), cut into chunks: a chunk
+ *              closes right after the line that brings it to chunk_bytes or more (0: one page per chunk), the last
+ *              chunk is the rest.  Each chunk is base64.StdEncoding-encoded on the device; chunk k is len[k] bytes at
+ *              data + off[k] (off[k] % 16 == 0) and encodes raw_len[k] JSONL bytes.  A layer map without pages is
+ *              TGI_E_NOPAGES (the reference's "no pages found to export").  The shim names chunk k
+ *              <StorageRoot>/<config CrawlID>/analysis/channels/channel-pages-<crawlID>-<ts>-part<k>.jsonl.
+ *            TGI_STATE_EXPORT_LOCAL = LocalStateManager.ExportPagesToBinding (storageproviders.go:550-587): every page
+ *              of pageMap once, in row order (Go's map order is random), raw JSONL in one chunk (empty without pages).
+ *            Timestamps, omitempty fields and message lists are those of tgi_state_render; a timestamp whose year
+ *            leaves [0, 9999] is TGI_E_ARG (where Go logs the marshal error and skips the page).  The output lives in
+ *            library-owned pinned memory until the next state call. */
+#define TGI_E_NOPAGES (-7)  /* tgi_state_export: the layer map holds no page                                */
+#define TGI_STATE_EXPORT_DAPR 0
+#define TGI_STATE_EXPORT_LOCAL 1
+typedef struct tgi_state_export_t {
+  const uint8_t* data;       /* the chunks: base64 (Dapr) or raw JSONL (local), pinned                         */
+  const uint64_t* off;       /* [n_chunks] chunk k starts at data + off[k]                                     */
+  const uint64_t* len;       /* [n_chunks] its bytes in data                                                   */
+  const uint64_t* raw_len;   /* [n_chunks] its JSONL bytes before encoding                                     */
+  uint64_t n_chunks;
+  uint64_t n_pages;          /* lines exported                                                                 */
+  float kernel_ms;           /* device time of the kernels and scans (not the read-back)                      */
+  uint32_t gpu_launches;
+} tgi_state_export_t;
+int tgi_state_layer_map(tgi_ctx* ctx, tgi_state_json_t* out);
+int tgi_state_add_pages(tgi_ctx* ctx, int64_t depth, const tgi_state_page* pages, uint64_t n, const uint8_t* strs,
+                        uint64_t strs_len, uint32_t* rows);
+int tgi_state_export(tgi_ctx* ctx, int mode, uint64_t chunk_bytes, tgi_state_export_t* out);
+
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
                          uint8_t* reason);
