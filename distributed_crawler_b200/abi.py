@@ -193,6 +193,15 @@ class StateJsonC(C.Structure):  # tgi_state_json_t
 
 
 E_NOPAGES = -7  # tgi_state_export: the layer map holds no page ("no pages found to export")
+TURN_PAGE_JSON = 1  # tgi_state_page_begin: also json.Marshal(page), the value Dapr's UpdatePage saves
+
+
+class StateTurnC(C.Structure):  # tgi_state_turn_t
+    _fields_ = [("turn", C.c_uint32), ("row", C.c_uint32), ("n_work", C.c_uint64), ("work", C.POINTER(C.c_uint32)),
+                ("page_json", C.c_void_p), ("page_json_len", C.c_uint64), ("kernel_ms", C.c_float),
+                ("gpu_launches", C.c_uint32)]
+
+
 STATE_EXPORT_DAPR, STATE_EXPORT_LOCAL = 0, 1
 STATE_EXPORT_CHUNK_DEFAULT = 100 * 1024 * 1024  # exportChunkSizeBytes (state/daprstate.go:2909)
 

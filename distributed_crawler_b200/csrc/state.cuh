@@ -18,6 +18,10 @@
 //
 // DaprStateManager's side: the exports (daprstate.go:2911-3012, storageproviders.go:550-587) run the same passes with
 // st_entry in line mode, one {page}\n per entry; json.Marshal(layerMap) (daprstate.go:947) is a thread per listed id.
+//
+// Page turns (crawl/runner.go:1132-1211): a thread per fetched key probes the table at the row's current generation and
+// records the first fetched index of its message id; the new keys become the row's next generation, and the one page
+// renders through the export's line passes over that fresh contiguous segment.  Nothing reads another row's messages.
 #pragma once
 #include "local_appends.cuh"
 
@@ -147,6 +151,81 @@ __global__ void st_upd_append_kernel(StDev d, StUpd w) {
     m.platform = 0;
     d.msgs[w.n_msgs + w.pos[j]] = m;
     atomicAdd(d.row_cnt + k.row, 1u);
+  }
+}
+
+// ---- page turns: processAllMessagesWithProcessor's bookkeeping (crawl/runner.go:1132-1147, 1161-1211) ---------------
+struct StTurn {
+  const long long* fetched;  // [n][2] chat_id, message_id in fetch order
+  uint64_t n;
+  uint32_t row, gen;  // the page, and the generation its new list takes
+  uint32_t* bfirst;   // batch table keyed by message id: lowest fetched index, ST_NONE = empty
+  uint64_t bmask;
+  uint32_t* flag;     // [n] 1: fetched key j is not in the page's list (addNewMessages keeps it)
+  uint64_t* pos;      // [n+1] scan of flag
+  uint64_t n_msgs;    // message rows before the new list
+  long long* keys;    // [n_new][2] the new list's keys: the turn's owner messages
+  uint32_t* work;     // [n_new] fetched index of each owner message's discMessage
+  uint32_t* sorted;   // [n_new] message index of each owner message (the one-page render's grouped order)
+  uint32_t* rows;     // [n_new] its row
+};
+
+DEVI uint64_t st_turn_slot(const StTurn& t, long long msg) { return st_hash(0, 0, 0, msg) & t.bmask; }
+
+// 1. addNewMessages' test against the page's current list, and the first fetched index of every message id
+__global__ void st_turn_probe_kernel(StDev d, StTurn t) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < t.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const long long chat = t.fetched[2 * j], msg = t.fetched[2 * j + 1];
+    t.flag[j] = st_lookup(d, t.row, d.row_gen[t.row], chat, msg) == ST_NONE;
+    for (uint64_t s = st_turn_slot(t, msg);; s = (s + 1) & t.bmask) {
+      const uint32_t cur = atomicCAS(t.bfirst + s, ST_NONE, (uint32_t)j);
+      if (cur == ST_NONE) break;
+      if (t.fetched[2 * cur + 1] == msg) {
+        atomicMin(t.bfirst + s, (uint32_t)j);
+        break;
+      }
+    }
+  }
+}
+
+// 2. the new list in fetch order, appended as the row's live messages: status "resample", no platform, pageId = the
+// page; each owner message's discMessage is the first fetched message with its message id (the chat id is ignored)
+__global__ void st_turn_append_kernel(StDev d, StTurn t) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < t.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!t.flag[j]) continue;
+    const uint64_t p = t.pos[j];
+    const long long chat = t.fetched[2 * j], msg = t.fetched[2 * j + 1];
+    uint64_t s = st_turn_slot(t, msg);
+    while (t.fetched[2 * t.bfirst[s] + 1] != msg) s = (s + 1) & t.bmask;
+    t.work[p] = t.bfirst[s];
+    t.keys[2 * p] = chat;
+    t.keys[2 * p + 1] = msg;
+    StMsg m;
+    m.chat = chat;
+    m.msg = msg;
+    m.row = t.row;
+    m.gen = t.gen;
+    m.pid = t.row;
+    m.status = 5;  // "resample"
+    m.platform = 0;
+    d.msgs[t.n_msgs + p] = m;
+    t.sorted[p] = (uint32_t)(t.n_msgs + p);
+    t.rows[p] = t.row;
+  }
+}
+
+// the loop's UpdateMessage calls: owner message j updates the key (message id, chat id), swapped as the reference passes
+// them, with "failed" for a record that failed and "fetched" otherwise
+__global__ void st_turn_updates_kernel(const long long* keys, const uint8_t* status, uint64_t n, uint32_t row,
+                                       tgi_state_update* u) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    tgi_state_update v;
+    v.chat_id = keys[2 * j + 1];
+    v.message_id = keys[2 * j];
+    v.row = row;
+    v.status = status[j] == TGI_ST_FAILED ? 3 : 2;  // "failed" : "fetched"
+    v.reserved = 0;
+    u[j] = v;
   }
 }
 

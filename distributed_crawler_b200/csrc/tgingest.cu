@@ -15,6 +15,7 @@
 #include <cstring>
 #include <mutex>
 #include <map>
+#include <memory>
 #include <string>
 #include <thread>
 #include <unordered_map>
@@ -210,6 +211,19 @@ struct CrawlState {
   DevBuf entries, keys, vals, row_base, msize, moff, e32, e64, counts, roff, out;
   DevBuf lm_keys, cb_tasks, cb_segs, b64;  // the layer map's openings; the export's encode tasks and output
   HostBuf h_out, h_sc, h_read, h_chunks;
+  // page turns (tgi_state_page_begin / _end): each open turn's row and owner keys, by handle; the key buffers of
+  // closed turns are kept for the next ones
+  struct Turn {
+    uint32_t row = 0;
+    uint64_t n_work = 0;
+    std::unique_ptr<DevBuf> keys;  // [n_work][2] chat_id, message_id
+  };
+  std::map<uint32_t, Turn> turns;
+  std::vector<std::unique_ptr<DevBuf>> turn_pool;
+  uint32_t next_turn = 1;
+  cudaEvent_t ev_slot = nullptr;  // tgi_state_page_end: the slot's work the state stream waits for
+  DevBuf turn_in;                 // the fetched keys of tgi_state_page_begin
+  HostBuf h_work;
 };
 
 struct Slot {
@@ -1955,7 +1969,7 @@ void tgi_destroy(tgi_ctx* c) {
     cudaStreamSynchronize(c->state.stream);
     cudaStreamDestroy(c->state.stream);
   }
-  for (cudaEvent_t e : {c->state.t0, c->state.t1, c->state.t2, c->state.t3, c->state.t4, c->state.t5}) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : {c->state.t0, c->state.t1, c->state.t2, c->state.t3, c->state.t4, c->state.t5, c->state.ev_slot}) if (e) cudaEventDestroy(e);
   delete c;  // the device and pinned buffers free themselves
 }
 
@@ -3270,6 +3284,7 @@ int st_init(tgi_ctx* c, CrawlState& S) {
   CK(cudaEventCreate(&S.t3));
   CK(cudaEventCreate(&S.t4));
   CK(cudaEventCreate(&S.t5));
+  CK(cudaEventCreateWithFlags(&S.ev_slot, cudaEventDisableTiming));
   for (const char* s : kPresetCodes) {
     S.code_of[s] = (uint16_t)S.codes.size();
     S.codes.push_back(s);
@@ -3551,6 +3566,48 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
   return TGI_OK;
 }
 
+// the m UpdateMessage calls in S.upd, in order (rows valid, st_reserve(m) done): the batch table, one probe per distinct
+// key, the new keys appended in first-occurrence order and entered in the table
+int st_apply_updates(tgi_ctx* c, CrawlState& S, uint64_t m) {
+  cudaStream_t st = S.stream;
+  int rc;
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * m, 64));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.blast.ensure(bslots * 4));
+  CK(S.slot_of.ensure(m * 4));
+  CK(S.flag.ensure(m * 4));
+  CK(S.pos.ensure((m + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(cudaMemsetAsync(S.bfirst.p, 0xFF, bslots * 4, st));
+  CK(cudaMemsetAsync(S.blast.p, 0, bslots * 4, st));
+  StUpd w{};
+  w.u = S.upd.as<tgi_state_update>();
+  w.n = m;
+  w.bfirst = S.bfirst.as<uint32_t>();
+  w.blast = S.blast.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.slot_of.as<uint32_t>();
+  w.flag = S.flag.as<uint32_t>();
+  w.pos = S.pos.as<uint64_t>();
+  w.n_msgs = S.n_msgs;
+  const StDev d = st_dev(S);
+  uint32_t launches = 0;
+  st_upd_build_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(w);
+  st_upd_resolve_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
+  if ((rc = launch_scan(c, st, S.tiles, w.flag, m, w.pos, S.sc.as<uint64_t>(), launches))) return rc;
+  st_upd_append_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t added = *S.h_sc.as<uint64_t>();
+  if (added) st_table_insert_kernel<<<st_grid(c, added), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + added);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  S.n_msgs += added;
+  return TGI_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -3596,7 +3653,10 @@ int tgi_state_set(tgi_ctx* c, const tgi_state_layer* layers, uint32_t n_layers, 
       set_err(c, "tgi_state_set: message %llu names an unknown page or code", (unsigned long long)j);
       return TGI_E_ARG;
     }
-  // SetState: new maps, layer by layer; a later page with the same id replaces the row (and its messages)
+  // SetState: new maps, layer by layer; a later page with the same id replaces the row (and its messages).  The rows
+  // are renumbered, so the open turns go.
+  for (auto& [h, T] : S.turns) S.turn_pool.push_back(std::move(T.keys));
+  S.turns.clear();
   S.rows.clear();
   S.blob.clear();
   S.gen.clear();
@@ -3750,44 +3810,9 @@ int tgi_state_update_messages(tgi_ctx* c, const tgi_state_update* ups, uint64_t 
   const uint64_t m = u.size();
   if (!m) return TGI_OK;
   if ((rc = st_reserve(c, S, m))) return rc;
-  cudaStream_t st = S.stream;
-  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * m, 64));
   CK(S.upd.ensure(m * sizeof(tgi_state_update)));
-  CK(S.bfirst.ensure(bslots * 4));
-  CK(S.blast.ensure(bslots * 4));
-  CK(S.slot_of.ensure(m * 4));
-  CK(S.flag.ensure(m * 4));
-  CK(S.pos.ensure((m + 1) * 8));
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
-  CK(cudaMemcpyAsync(S.upd.p, u.data(), m * sizeof(tgi_state_update), cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(S.bfirst.p, 0xFF, bslots * 4, st));
-  CK(cudaMemsetAsync(S.blast.p, 0, bslots * 4, st));
-  StUpd w{};
-  w.u = S.upd.as<tgi_state_update>();
-  w.n = m;
-  w.bfirst = S.bfirst.as<uint32_t>();
-  w.blast = S.blast.as<uint32_t>();
-  w.bmask = bslots - 1;
-  w.slot_of = S.slot_of.as<uint32_t>();
-  w.flag = S.flag.as<uint32_t>();
-  w.pos = S.pos.as<uint64_t>();
-  w.n_msgs = S.n_msgs;
-  const StDev d = st_dev(S);
-  uint32_t launches = 0;
-  st_upd_build_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(w);
-  st_upd_resolve_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
-  if ((rc = launch_scan(c, st, S.tiles, w.flag, m, w.pos, S.sc.as<uint64_t>(), launches))) return rc;
-  st_upd_append_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  const uint64_t added = *S.h_sc.as<uint64_t>();
-  if (added) st_table_insert_kernel<<<st_grid(c, added), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + added);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(st));
-  S.n_msgs += added;
-  return TGI_OK;
+  CK(cudaMemcpyAsync(S.upd.p, u.data(), m * sizeof(tgi_state_update), cudaMemcpyHostToDevice, S.stream));
+  return st_apply_updates(c, S, m);
 }
 
 int tgi_state_read_page(tgi_ctx* c, uint32_t row, tgi_state_msg* out, uint64_t cap, uint64_t* n) {
@@ -4065,6 +4090,245 @@ int tgi_state_export(tgi_ctx* c, int mode, uint64_t chunk_bytes, tgi_state_expor
   out->n_pages = ne;
   out->kernel_ms = size_ms + emit_ms + enc_ms;
   out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// addNewMessages + resampleMarker + UpdatePage for one page (crawl/runner.go:1132-1147), touching only the page's own
+// messages: the fetched keys are probed against the page's list in the resident table, the new ones compacted in fetch
+// order and appended as the row's new list.  Three synchronises: the new list's length (and the old one's, for the
+// tombstone count), the row upload, and the work list; with TGI_TURN_PAGE_JSON the page's size comes back with the work
+// list and one more synchronise brings its bytes.
+int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out) {
+  if (!c || !out || (n && !fetched)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  if (flags & ~TGI_TURN_PAGE_JSON) { set_err(c, "tgi_state_page_begin: unknown flags 0x%x", flags); return TGI_E_ARG; }
+  if (row >= S.rows.size()) { set_err(c, "tgi_state_page_begin: no row %u", row); return TGI_E_ARG; }
+  if (page) {
+    if (!page_ok(c, *page, strs, strs_len, "tgi_state_page_begin")) return TGI_E_ARG;
+    if (page->n_msgs) { set_err(c, "tgi_state_page_begin: the page carries messages (its list comes from the fetch)"); return TGI_E_ARG; }
+    if (in_field(*page, strs, TGI_PS_ID) != st_field(S, S.rows[row], TGI_PS_ID)) { set_err(c, "tgi_state_page_begin: the page's id is not row %u's", row); return TGI_E_ARG; }
+  }
+  if ((rc = st_upload_codes(c, S))) return rc;
+  if ((rc = st_reserve(c, S, n))) return rc;
+  cudaStream_t st = S.stream;
+  const bool json = flags & TGI_TURN_PAGE_JSON;
+  std::unique_ptr<DevBuf> keys;
+  if (S.turn_pool.empty()) {
+    keys = std::make_unique<DevBuf>();
+  } else {
+    keys = std::move(S.turn_pool.back());
+    S.turn_pool.pop_back();
+  }
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * n, 64));
+  CK(keys->ensure(n * 16));
+  CK(S.turn_in.ensure(n * 16));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.flag.ensure(n * 4));
+  CK(S.pos.ensure((n + 1) * 8));
+  CK(S.slot_of.ensure(n * 4));
+  CK(S.vals.ensure(n * 4));
+  CK(S.keys.ensure(n * 4));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_work.ensure(n * 4));
+  StTurn t{};
+  t.fetched = S.turn_in.as<long long>();
+  t.n = n;
+  t.row = row;
+  t.gen = S.gen[row] + 1;
+  t.bfirst = S.bfirst.as<uint32_t>();
+  t.bmask = bslots - 1;
+  t.flag = S.flag.as<uint32_t>();
+  t.pos = S.pos.as<uint64_t>();
+  t.n_msgs = S.n_msgs;
+  t.keys = keys->as<long long>();
+  t.work = S.slot_of.as<uint32_t>();
+  t.sorted = S.vals.as<uint32_t>();
+  t.rows = S.keys.as<uint32_t>();
+  uint64_t* hs = S.h_sc.as<uint64_t>();
+  hs[0] = hs[1] = 0;
+  uint32_t launches = 0;
+  // 1. which fetched keys the page's list lacks, and the old list's length
+  CK(cudaEventRecord(S.t0, st));
+  if (n) {
+    CK(cudaMemcpyAsync(S.turn_in.p, fetched, n * 16, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(S.bfirst.p, 0xFF, bslots * 4, st));
+    st_turn_probe_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(st_dev(S), t);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, t.flag, n, t.pos, S.sc.as<uint64_t>(), launches))) return rc;
+    CK(cudaMemcpyAsync(hs, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaMemcpyAsync(hs + 1, S.row_cnt.as<uint32_t>() + row, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t n_new = hs[0];
+  // 2. UpdatePage(*owner): the old list becomes tombstones; the row takes the page's fields and joins the layer of its
+  // depth if that layer exists and does not hold it (base.go:131-146)
+  S.n_dead += hs[1];
+  S.gen[row]++;
+  if (page) st_put_row(S, row, *page, strs);
+  const auto lit = S.layers.find(S.rows[row].depth);
+  if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), row) == lit->second.end()) lit->second.push_back(row);
+  const std::vector<uint32_t> dirty(1, row);
+  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  const uint32_t cnt = (uint32_t)n_new;
+  CK(cudaMemcpyAsync(S.row_cnt.as<uint32_t>() + row, &cnt, 4, cudaMemcpyHostToDevice, st));
+  const StDev d = st_dev(S);
+  CK(cudaEventRecord(S.t2, st));
+  if (n_new) {
+    st_turn_append_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(d, t);
+    st_table_insert_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + n_new);
+    launches += 2;
+  }
+  S.n_msgs += n_new;
+  // 3. json.Marshal(page) by the export's line passes over this one row, its new list being the fresh segment
+  StRender r{};
+  std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
+  if (json) {
+    zg.lock();
+    CK(S.entries.ensure(sizeof(StEntry)));
+    CK(S.row_base.ensure((S.rows.size() + 1) * 8));
+    CK(S.msize.ensure(n_new * 4));
+    CK(S.moff.ensure((n_new + 1) * 8));
+    CK(S.e32.ensure(4 * 4));
+    CK(S.e64.ensure(2 * 2 * 8));
+    r.entries = S.entries.as<StEntry>();
+    r.n_entries = 1;
+    r.zone = c->cfgdev.zone;
+    r.zone_n = c->cfgdev.zone_n;
+    r.tz = c->cfgdev.tz;
+    r.sc = S.sc.as<uint64_t>();
+    r.row_base = S.row_base.as<uint64_t>();  // only row_base[row] = 0 is read
+    r.msize = S.msize.as<uint32_t>();
+    r.moff = S.moff.as<uint64_t>();
+    r.esize_lo = S.e32.as<uint32_t>();
+    r.ebytes = r.esize_lo + 1;
+    r.ecnt = r.ebytes + 1;
+    r.esz = r.ecnt + 1;
+    r.eoff = S.e64.as<uint64_t>();
+    r.eslot = r.eoff + 2;
+    const StEntry e{(long long)S.rows[row].depth, row, 0};
+    CK(cudaMemcpyAsync(S.entries.p, &e, sizeof e, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(r.row_base + row, 0, 8, st));
+    CK(cudaMemsetAsync(r.moff, 0, 8, st));
+    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+    if (n_new) {
+      st_msg_size_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, r, t.sorted, t.rows, n_new);
+      launches++;
+      if ((rc = launch_scan(c, st, S.tiles, r.msize, n_new, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
+    }
+    st_line_size_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.esz, 1, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
+    if ((rc = launch_scan(c, st, S.tiles, r.ecnt, 1, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+    CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  if (n_new) CK(cudaMemcpyAsync(S.h_work.p, t.work, n_new * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms0 = 0, ms1 = 0, ms2 = 0;
+  cudaEventElapsedTime(&ms0, S.t0, S.t1);
+  cudaEventElapsedTime(&ms1, S.t2, S.t3);
+  if (json) {
+    // Dapr's UpdatePage has changed pageMap before json.Marshal fails (daprstate.go:1378-1387): the new list stays, no
+    // turn opens, as the reference returns before its loop
+    if (hs[ST_SC_ERR]) {
+      rc = st_compact(c, S);
+      if (!rc) set_err(c, "tgi_state_page_begin: the page's timestamp year is outside [0, 9999] (json.Marshal fails)");
+      return rc ? rc : TGI_E_ARG;
+    }
+    if (hs[ST_SC_BIG]) {
+      rc = st_compact(c, S);
+      if (!rc) set_err(c, "tgi_state_page_begin: the page renders to 4 GiB or more");
+      return rc ? rc : TGI_E_CAPACITY;
+    }
+    const uint64_t body = hs[ST_SC_BYTES];
+    CK(S.out.ensure(body));
+    CK(S.h_out.ensure(body));
+    r.out = S.out.as<uint8_t>();
+    CK(cudaEventRecord(S.t4, st));
+    st_line_emit_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+    if (n_new) st_msg_emit_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, r, t.sorted);
+    launches += 1 + (n_new != 0);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t5, st));
+    CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&ms2, S.t4, S.t5);
+    out->page_json = S.h_out.as<uint8_t>();
+    out->page_json_len = body - 1;  // the line without its '\n'
+  }
+  if ((rc = st_compact(c, S))) return rc;
+  const uint32_t h = S.next_turn++;
+  if (!S.next_turn) S.next_turn = 1;
+  CrawlState::Turn& T = S.turns[h];
+  T.row = row;
+  T.n_work = n_new;
+  T.keys = std::move(keys);
+  out->turn = h;
+  out->row = row;
+  out->n_work = n_new;
+  out->work = S.h_work.as<uint32_t>();
+  out->kernel_ms = ms0 + ms1 + ms2;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// the loop's first n_done UpdateMessage calls (crawl/runner.go:1161-1211) as one tgi_state_update_messages batch, built
+// on the device from the turn's keys and the statuses.  Lock order: the slot, then the state; no other entry point holds
+// both.  The slot's lock is held until the kernels that read its status array have finished.
+int tgi_state_page_end(tgi_ctx* c, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended) {
+  if (!c || (slot < 0 && n_done && !status)) return TGI_E_ARG;
+  if (slot >= TGI_SLOTS) { set_err(c, "tgi_state_page_end: bad slot %d", slot); return TGI_E_ARG; }
+  Slot* s = slot >= 0 ? &c->slots[slot] : nullptr;
+  std::unique_lock<std::mutex> sl;
+  if (s) {
+    sl = std::unique_lock<std::mutex>(s->mu);
+    if (in_flight(*s)) { set_err(c, "tgi_state_page_end: slot %d is in flight", slot); return TGI_E_STATE; }
+    if (!s->busy || s->last.kind == REC_NONE) { set_err(c, "tgi_state_page_end: slot %d holds no result (released or none)", slot); return TGI_E_ARG; }
+    if (s->last.kind != REC_TG || !s->last.dev.status) { set_err(c, "tgi_state_page_end: slot %d's result is not a Telegram one", slot); return TGI_E_ARG; }
+  }
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  const auto it = S.turns.find(turn);
+  if (it == S.turns.end()) { set_err(c, "tgi_state_page_end: no open turn %u", turn); return TGI_E_ARG; }
+  CrawlState::Turn& T = it->second;
+  if (s && s->last.n != T.n_work) {
+    set_err(c, "tgi_state_page_end: the slot's result holds %llu records, the turn %llu", (unsigned long long)s->last.n, (unsigned long long)T.n_work);
+    return TGI_E_ARG;
+  }
+  if (n_done > T.n_work) { set_err(c, "tgi_state_page_end: n_done %llu > n_work %llu", (unsigned long long)n_done, (unsigned long long)T.n_work); return TGI_E_ARG; }
+  const uint64_t before = S.n_msgs;
+  if (n_done) {
+    if ((rc = st_reserve(c, S, n_done))) return rc;
+    cudaStream_t st = S.stream;
+    const uint8_t* d_status;
+    CK(S.upd.ensure(n_done * sizeof(tgi_state_update)));
+    if (s) {
+      CK(cudaEventRecord(S.ev_slot, s->stream));
+      CK(cudaStreamWaitEvent(st, S.ev_slot, 0));
+      d_status = s->last.dev.status;
+    } else {
+      CK(S.turn_in.ensure(n_done));
+      CK(cudaMemcpyAsync(S.turn_in.p, status, n_done, cudaMemcpyHostToDevice, st));
+      d_status = S.turn_in.as<uint8_t>();
+    }
+    st_turn_updates_kernel<<<st_grid(c, n_done), ST_THREADS, 0, st>>>(T.keys->as<long long>(), d_status, n_done, T.row,
+                                                                      S.upd.as<tgi_state_update>());
+    CK(cudaGetLastError());
+    if ((rc = st_apply_updates(c, S, n_done))) return rc;
+  }
+  if (appended) *appended = S.n_msgs - before;
+  S.turn_pool.push_back(std::move(T.keys));
+  S.turns.erase(it);
   return TGI_OK;
 }
 

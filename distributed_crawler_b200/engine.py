@@ -38,7 +38,7 @@ EXPORTED_SYMBOLS = [
     "tgi_set_growth", "tgi_set_info", "tgi_dapr_payloads", "tgi_plan_chunks_carry", "tgi_combine_open", "tgi_combine_add",
     "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
-    "tgi_state_add_pages", "tgi_state_export",
+    "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
 ]
 
 
@@ -116,6 +116,8 @@ def lib() -> C.CDLL:
         L.tgi_state_layer_map.argtypes = [vp, C.POINTER(abi.StateJsonC)]
         L.tgi_state_add_pages.argtypes = [vp, C.c_int64, vp, u64, vp, u64, vp]
         L.tgi_state_export.argtypes = [vp, i32, u64, C.POINTER(abi.StateExportC)]
+        L.tgi_state_page_begin.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, C.POINTER(abi.StateTurnC)]
+        L.tgi_state_page_end.argtypes = [vp, u32, i32, vp, u64, C.POINTER(u64)]
         _LIB = L
     return _LIB
 
@@ -663,6 +665,37 @@ class Engine:
         self.state_export_pages = int(out.n_pages)
         return [(C.string_at(out.data + out.off[k], out.len[k]) if out.len[k] else b"", int(out.raw_len[k]))
                 for k in range(out.n_chunks)]
+
+    def state_page_begin(self, row: int, fetched, page=None, page_json: bool = False):
+        """addNewMessages + resampleMarker + UpdatePage for a fetched page: fetched = (chat_id, message_id) pairs in
+        fetch order, page = a state_pack dict without messages that replaces the row's fields (None: keep them).
+        Returns (turn, work, page_json): work[i] indexes fetched for owner message i's discMessage; page_json is
+        json.Marshal(page) when asked for, else None.  The device time of the call is left in self.state_turn_ms"""
+        f = np.ascontiguousarray(fetched, np.int64).reshape(-1, 2)
+        recs = strs = None
+        if page is not None:
+            from .state_pack import pack_pages
+            if page.get("messages"):
+                raise ValueError("the page's message list comes from the fetch")
+            recs, strs, _ = pack_pages([page], self.state_code, lambda pid, i: i)
+        out = abi.StateTurnC()
+        self._check(lib().tgi_state_page_begin(
+            self.h, row, recs.ctypes.data if recs is not None else None, strs.ctypes.data if strs is not None else None,
+            len(strs) if strs is not None else 0, f.ctypes.data if len(f) else None, len(f),
+            abi.TURN_PAGE_JSON if page_json else 0, C.byref(out)))
+        self.state_turn_ms = float(out.kernel_ms)
+        self.state_turn_launches = int(out.gpu_launches)
+        work = np.ctypeslib.as_array(out.work, (out.n_work,)).copy() if out.n_work else np.zeros(0, np.uint32)
+        return int(out.turn), work, C.string_at(out.page_json, out.page_json_len) if out.page_json else None
+
+    def state_page_end(self, turn: int, n_done: int, slot: int = -1, status=None) -> int:
+        """the loop's first n_done UpdateMessage calls of a turn, with the statuses of the slot's last Telegram result
+        (slot >= 0) or of `status` (abi.ST_* per owner message, slot < 0); returns the messages appended"""
+        st = None if status is None else np.ascontiguousarray(status, np.uint8)
+        appended = C.c_uint64()
+        self._check(lib().tgi_state_page_end(self.h, turn, slot, st.ctypes.data if st is not None and len(st) else None,
+                                             n_done, C.byref(appended)))
+        return appended.value
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

@@ -338,6 +338,23 @@ class MessageProcessor {
     for (uint64_t k = 0; k < o.n_chunks; k++) v.emplace_back((const char*)o.data + o.off[k], o.len[k]);
     return v;
   }
+  // A page turn of processAllMessagesWithProcessor: addNewMessages + resampleMarker + UpdatePage for the fetched
+  // (chat_id, message_id) pairs (page: the owner's new fields, or nullptr); pack the batch as fetched[work[i]], run it,
+  // then StatePageEnd(turn, slot, n_done) makes the loop's UpdateMessage calls from the slot's result.  work and
+  // page_json stay valid until the next state call.
+  tgi_state_turn_t StatePageBegin(uint32_t row, const std::vector<int64_t>& fetched, bool page_json,
+                                  const tgi_state_page* page = nullptr, std::string_view strs = {}) {
+    tgi_state_turn_t t{};
+    if (tgi_state_page_begin(ctx_, row, page, (const uint8_t*)strs.data(), strs.size(), fetched.data(), fetched.size() / 2,
+                             page_json ? TGI_TURN_PAGE_JSON : 0u, &t) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return t;
+  }
+  uint64_t StatePageEnd(uint32_t turn, int slot, uint64_t n_done) {
+    uint64_t appended = 0;
+    if (tgi_state_page_end(ctx_, turn, slot, nullptr, n_done, &appended) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return appended;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

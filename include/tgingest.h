@@ -864,6 +864,51 @@ int tgi_state_add_pages(tgi_ctx* ctx, int64_t depth, const tgi_state_page* pages
                         uint64_t strs_len, uint32_t* rows);
 int tgi_state_export(tgi_ctx* ctx, int mode, uint64_t chunk_bytes, tgi_state_export_t* out);
 
+/* Page turns — the bookkeeping processAllMessagesWithProcessor runs once per fetched page (crawl/runner.go:1132-1147,
+ * 1161-1211), in two calls that touch only that page's messages (no call reads every message row of the state).  The
+ * caller's `owner` is the state's own page (row), with no other update of it between its GetPage and the turn.
+ *   Begin    tgi_state_page_begin = addNewMessages + resampleMarker + UpdatePage(*owner).  fetched holds the page's
+ *            fetched messages, chat_id and message_id, in fetch order (n = 0 empties the list, as the reference does).
+ *            The page's list becomes the fetched keys that were NOT in its list before, in fetch order, a key fetched
+ *            twice kept twice; the earlier messages are dropped.  Every new message is {chat, msg, "resample", pageId =
+ *            the page, no platform}: all came from the fetch, so resampleMarker marks each one.  page (optional) replaces
+ *            the row's fields as tgi_state_update_page does; its id must be the row's and it carries no messages (NULL:
+ *            the fields as stored).  Either way the row joins the layer of its depth if that layer exists and does not
+ *            hold it (UpdatePage's rule).
+ *            out->work[i] (n_work entries, pinned) is the index into fetched of owner message i's discMessage: the FIRST
+ *            fetched message with the same message id, the chat id ignored (:1171-1176).  It always exists, so the
+ *            loop's "deleted" branch (:1185) cannot be reached from this flow.  The caller packs its batch as
+ *            fetched[work[i]] in that order and processes it.
+ *            TGI_TURN_PAGE_JSON: out->page_json = json.Marshal(page) after UpdatePage, the value DaprStateManager's
+ *            UpdatePage saves (daprstate.go:1370-1407); the same bytes as the page's tgi_state_export line without its
+ *            '\n'.  A timestamp whose year leaves [0, 9999] is then TGI_E_ARG AFTER the update (Dapr changes pageMap
+ *            before its marshal fails) and no turn opens.  work and page_json live until the next state call.
+ *   End      tgi_state_page_end = the loop's first n_done UpdateMessage calls, in order, against the state as it is at
+ *            the call: exactly tgi_state_update_messages with owner message i's key SWAPPED, (message_id, chat_id) as
+ *            the reference passes them, and status "failed" for TGI_ST_FAILED, "fetched" for TGI_ST_EMITTED,
+ *            TGI_ST_SKIPPED and TGI_ST_NOLINE.  The swapped key usually misses and appends {msg, chat, s, pageId = the
+ *            page}; later updates of the same swapped key hit that message.  n_done < n_work: the loop stopped early
+ *            (the random-walk FLOOD_WAIT retire, :1333-1338).  The statuses are the resident status array of the slot's
+ *            last result, not read back (slot >= 0), or status[n_done] from the host (slot < 0).  *appended (optional)
+ *            gets the messages appended.  A handle is consumed once; tgi_state_set drops every open turn.
+ *   Errors   TGI_E_ARG, the state unchanged: no such row, a page whose id is not the row's; an unknown or consumed
+ *            handle, a slot result that is not Telegram, has been released or holds another record count than n_work,
+ *            n_done > n_work.  TGI_E_STATE: a job in flight on the slot.                                              */
+#define TGI_TURN_PAGE_JSON 1u
+typedef struct tgi_state_turn_t {
+  uint32_t turn;              /* handle for tgi_state_page_end (never 0)                                        */
+  uint32_t row;
+  uint64_t n_work;            /* len(owner.Messages) after addNewMessages: the records the loop processes        */
+  const uint32_t* work;       /* [n_work] index into fetched of each owner message's discMessage (pinned)        */
+  const uint8_t* page_json;   /* json.Marshal(page) with TGI_TURN_PAGE_JSON, else NULL (pinned)                  */
+  uint64_t page_json_len;
+  float kernel_ms;            /* device time of the call's kernels and scans (not the copies between them)       */
+  uint32_t gpu_launches;
+} tgi_state_turn_t;
+int tgi_state_page_begin(tgi_ctx* ctx, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out);
+int tgi_state_page_end(tgi_ctx* ctx, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended);
+
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
                          uint8_t* reason);
