@@ -78,6 +78,7 @@ APPEND_RUN = np.dtype([("chan_idx", "<u4"), ("n_lines", "<u4"), ("first", "<u8")
                        ("byte_end", "<u8")])  # tgi_append_run
 assert APPEND_RUN.itemsize == 40
 SET_FRONTIER, SET_INVALID, SET_DISCOVERED, SET_OWNED = 0, 1, 2, 3  # tgi_set_info / tgi_set_add
+SET_URLS = 4  # Dapr's urlCache (tgi_state_discover): seeded with tgi_set_add
 EDGE_PENDING, EDGE_DUPLICATE, EDGE_INVALID_CACHED = 0, 1, 2
 ROWS_STATUS, ROWS_LINK_OFF, ROWS_LINKS = 0, 1, 2  # tgi_result_read_rows
 RUN_SKIP_INVALID = 0x40
@@ -200,6 +201,18 @@ class StateTurnC(C.Structure):  # tgi_state_turn_t
     _fields_ = [("turn", C.c_uint32), ("row", C.c_uint32), ("n_work", C.c_uint64), ("work", C.POINTER(C.c_uint32)),
                 ("page_json", C.c_void_p), ("page_json_len", C.c_uint64), ("kernel_ms", C.c_float),
                 ("gpu_launches", C.c_uint32)]
+
+
+DISCOVER_NOW = 1        # tgi_state_discover: AddLayer per span now (else the candidates go to the pending list)
+DISCOVER_DAPR = 2       # DaprStateManager.AddLayer's rules instead of BaseStateManager's
+DISCOVER_PAGE_JSON = 4  # json.Marshal of every added page (Dapr's per-page SaveState value)
+STATE_SPAN = np.dtype([("row", "<u4"), ("reserved", "<u4"), ("first", "<u8"), ("n_records", "<u8"), ("n_done", "<u8")])
+
+
+class StateAddedC(C.Structure):  # tgi_state_added_t
+    _fields_ = [("n_candidates", C.c_uint64), ("n_added", C.c_uint64), ("rows", C.POINTER(C.c_uint32)),
+                ("ids", C.c_void_p), ("page_json", C.c_void_p), ("json_off", C.POINTER(C.c_uint64)),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
 STATE_EXPORT_DAPR, STATE_EXPORT_LOCAL = 0, 1

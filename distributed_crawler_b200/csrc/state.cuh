@@ -531,6 +531,188 @@ __global__ void st_msg_emit_kernel(StDev d, StRender r, const uint32_t* sorted) 
   }
 }
 
+// ---- snowball discovery (crawl/runner.go:1199-1244, standalone/runner.go:835-850, dapr/standalone.go:645-688) -------
+struct StCand {      // 48 bytes: one candidate page of the next layer (and one entry of the pending list)
+  uint8_t name[32];  // the outlink, zero padded: a key of the resident sets
+  uint32_t len;
+  uint32_t parent;   // the owner row
+  uint32_t span;     // the span that found it (unused in the pending list)
+  uint32_t reserved;
+};
+
+struct StDisc {
+  const tgi_state_span* spans;
+  uint32_t n_spans;
+  const uint8_t* status;     // the slot's resident result
+  const uint32_t* link_off;  // [n+1]
+  const tgi_link* links;
+  const uint64_t* soff;      // [n_spans+1] scan of the spans' processed link rows
+  uint64_t bound;            // gather threads: at least soff[n_spans]
+  uint32_t* flag;            // [bound] 1: link row i of the spans is a candidate
+  uint32_t* lnk;             // [bound] its link row in the result
+  uint32_t* spn;             // [bound] its span
+  uint64_t* pos;             // [bound+1] scan of flag
+  StCand* out;               // candidate k at out[k]
+  uint64_t* coff;            // [n_spans+1] first candidate of every span
+};
+
+// the link rows of span k's processed records
+__global__ void st_disc_count_kernel(StDisc g, uint32_t* cnt) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < g.n_spans; k += (uint64_t)gridDim.x * blockDim.x) {
+    const tgi_state_span s = g.spans[k];
+    cnt[k] = g.link_off[s.first + s.n_done] - g.link_off[s.first];
+  }
+}
+
+// a thread per processed link row: a candidate when its record was processed without error (a failed record returned an
+// error, a date-skipped one an empty Post) and its name is not byte-equal to the owner's URL (runner.go:1231)
+__global__ void st_disc_flag_kernel(StDev d, StDisc g) {
+  const uint64_t total = g.soff[g.n_spans];
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < g.bound; i += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t f = 0;
+    if (i < total) {
+      uint32_t lo = 0, hi = g.n_spans - 1;  // the last span with soff <= i (empty spans share their offset)
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (g.soff[mid] <= i) lo = mid;
+        else hi = mid - 1;
+      }
+      const tgi_state_span s = g.spans[lo];
+      const uint32_t L = g.link_off[s.first] + (uint32_t)(i - g.soff[lo]);
+      uint64_t a = s.first, b = s.first + s.n_done - 1;  // the record that holds link row L
+      while (a < b) {
+        const uint64_t mid = (a + b + 1) >> 1;
+        if (g.link_off[mid] <= L) a = mid;
+        else b = mid - 1;
+      }
+      const uint8_t st = g.status[a];
+      if (st == TGI_ST_EMITTED || st == TGI_ST_NOLINE) {
+        uint32_t ul;
+        const uint8_t* u = st_str(d, d.pages[s.row], TGI_PS_URL, ul);
+        const tgi_link& lk = g.links[L];
+        bool self = ul == lk.len;
+        for (uint32_t k = 0; self && k < ul; k++) self = u[k] == lk.name[k];
+        f = !self;
+      }
+      g.lnk[i] = L;
+      g.spn[i] = lo;
+    }
+    g.flag[i] = f;
+  }
+}
+
+// the candidates in (span, record, link) order, and every span's first candidate
+__global__ void st_disc_emit_kernel(StDisc g) {
+  const uint64_t total = g.soff[g.n_spans];
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+    if (!g.flag[i]) continue;
+    const tgi_link& lk = g.links[g.lnk[i]];
+    StCand& c = g.out[g.pos[i]];
+    store_key(c.name, load_key(lk.name));
+    c.len = lk.len;
+    c.parent = g.spans[g.spn[i]].row;
+    c.span = g.spn[i];
+    c.reserved = 0;
+  }
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k <= g.n_spans; k += (uint64_t)gridDim.x * blockDim.x)
+    g.coff[k] = g.pos[g.soff[k]];
+}
+
+// first occurrence per URL (per span, or over the list) and Dapr's urlCache test, over candidates [0, *n)
+struct StFirst {
+  const StCand* c;
+  const uint64_t* n;  // device count
+  uint64_t bound;     // threads: at least *n
+  bool per_span;      // first occurrence within each span (Base rules per page)
+  bool dedup;         // false: Dapr's AddLayer keeps a page's repeated URLs
+  FrontierDev urls;   // TGI_SET_URLS (table == nullptr: empty, or not tested)
+  uint32_t* bfirst;   // batch table: lowest candidate index of the slot's key, ST_NONE = empty
+  uint64_t bmask;
+  uint32_t* slot_of;  // [bound]
+  uint32_t* flag;     // [bound] 1: the candidate survives
+  uint64_t* pos;      // [bound+1] scan of flag
+  StCand* out;        // the survivors in candidate order
+};
+
+DEVI bool st_same_cand(const StFirst& w, const StCand& a, const StCand& b) {
+  return (!w.per_span || a.span == b.span) && key_eq(load_key(a.name), load_key(b.name));
+}
+
+__global__ void st_first_kernel(StFirst w) {
+  const uint64_t n = *w.n;
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const StCand& c = w.c[j];
+    const uint64_t h = key_hash(load_key(c.name)) ^ (w.per_span ? c.span * 0x9E3779B97F4A7C15ull : 0ull);
+    uint64_t s = (h >> 7) & w.bmask;
+    for (;; s = (s + 1) & w.bmask) {
+      const uint32_t cur = atomicCAS(w.bfirst + s, ST_NONE, (uint32_t)j);
+      if (cur == ST_NONE) break;
+      if (st_same_cand(w, w.c[cur], c)) {
+        atomicMin(w.bfirst + s, (uint32_t)j);
+        break;
+      }
+    }
+    w.slot_of[j] = (uint32_t)s;
+  }
+}
+
+__global__ void st_keep_kernel(StFirst w) {
+  const uint64_t n = *w.n;
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < w.bound; j += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t f = 0;
+    if (j < n) {
+      f = !w.dedup || w.bfirst[w.slot_of[j]] == (uint32_t)j;
+      if (f && w.urls.table) {
+        const Key32 k = load_key(w.c[j].name);
+        f = set_lookup(w.urls, k, key_hash(k)) < 0;
+      }
+    }
+    w.flag[j] = f;
+  }
+}
+
+__global__ void st_survivors_kernel(StFirst w) {
+  const uint64_t n = *w.n;
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+    if (w.flag[j]) w.out[w.pos[j]] = w.c[j];
+}
+
+// Philox4x32-10 (Salmon et al., SC'11): ten rounds over the counter, the key bumped between them
+DEVI void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
+  for (int r = 0; r < 10; r++) {
+    if (r) {
+      k0 += 0x9E3779B9u;
+      k1 += 0xBB67AE85u;
+    }
+    const uint32_t lo0 = 0xD2511F53u * c[0], hi0 = __umulhi(0xD2511F53u, c[0]);
+    const uint32_t lo1 = 0xCD9E8D57u * c[2], hi1 = __umulhi(0xCD9E8D57u, c[2]);
+    const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
+    c[0] = n0;
+    c[1] = lo1;
+    c[2] = n2;
+    c[3] = lo0;
+  }
+}
+
+// ids n0 .. n0+n-1 of the seed as version-4 uuid strings, 36 bytes each
+__global__ void st_uuid_kernel(uint64_t seed, uint64_t n0, uint64_t n, uint8_t* out) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t ctr = n0 + k;
+    uint32_t c[4] = {(uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u};
+    philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+    uint8_t b[16];
+    for (int q = 0; q < 16; q++) b[q] = (uint8_t)(c[q >> 2] >> (8 * (q & 3)));
+    b[6] = (b[6] & 0x0F) | 0x40;
+    b[8] = (b[8] & 0x3F) | 0x80;
+    uint8_t* o = out + 36 * k;
+    for (int q = 0, p = 0; q < 16; q++) {
+      if (q == 4 || q == 6 || q == 8 || q == 10) o[p++] = '-';
+      o[p++] = "0123456789abcdef"[b[q] >> 4];
+      o[p++] = "0123456789abcdef"[b[q] & 15];
+    }
+  }
+}
+
 // ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------
 struct StLmEntry {  // one id of a layer, or an empty layer (row == ST_NONE)
   uint32_t row;

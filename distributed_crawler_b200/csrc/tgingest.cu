@@ -19,6 +19,7 @@
 #include <string>
 #include <thread>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "kernels.cuh"
@@ -224,6 +225,13 @@ struct CrawlState {
   cudaEvent_t ev_slot = nullptr;  // tgi_state_page_end: the slot's work the state stream waits for
   DevBuf turn_in;                 // the fetched keys of tgi_state_page_begin
   HostBuf h_work;
+  // snowball discovery (tgi_state_discover / _next_layer): the pending next-layer list (StCand, grown on demand), the
+  // id generator's key and next counter, and the scratch of the candidates and survivors
+  DevBuf pend, cand, surv, spans, cnt, soff, coff, lnk, spn, uuids, url_keys;
+  uint64_t n_pend = 0;
+  uint64_t id_seed = 0, id_next = 0;
+  bool seeded = false;
+  HostBuf h_surv, h_coff, h_ids, h_rows, h_json_off;
 };
 
 struct Slot {
@@ -284,8 +292,9 @@ struct tgi_ctx {
   std::vector<ZoneEnt> zone;  // tgi_set_zone (empty: tz_offset_sec) and its device copy
   DevBuf d_zone;
   // the resident key sets, indexed by TGI_SET_*: the dedup set (every key this GPU has seen), the exclusion sets of the
-  // frontier -> validator hand-off (tgi_set_add) and this rank's partition of the multi-GPU set (tgi_comm_init)
-  KeySet sets[4];
+  // frontier -> validator hand-off (tgi_set_add), this rank's partition of the multi-GPU set (tgi_comm_init) and Dapr's
+  // urlCache (tgi_state_discover)
+  KeySet sets[5];
   int64_t now_sec = 0;     // tgi_set_now: the clock the TTL of the invalid set is checked against
   uint64_t fr_cap0 = 0;    // tgi_config.frontier_capacity: the size the dedup set started at
   uint64_t grow_max = 0;   // tgi_set_growth: sets grow up to this many keys (0: fixed size)
@@ -505,10 +514,10 @@ int frontier_scratch(tgi_ctx* c, FrontierScratch& z, uint64_t n, uint64_t links,
   return TGI_OK;
 }
 
-// The set `which` (TGI_SET_*) names, or nullptr.  With exclusion_only, only the exclusion sets are named (the
-// tgi_set_add / _clear / _size family).
+// The set `which` (TGI_SET_*) names, or nullptr.  With exclusion_only, only the sets the caller fills are named (the
+// tgi_set_add / _clear / _size family: the exclusion sets and the urlCache).
 KeySet* key_set(tgi_ctx* c, int which, bool exclusion_only) {
-  if (which == TGI_SET_INVALID || which == TGI_SET_DISCOVERED) return &c->sets[which];
+  if (which == TGI_SET_INVALID || which == TGI_SET_DISCOVERED || which == TGI_SET_URLS) return &c->sets[which];
   if (!exclusion_only && (which == TGI_SET_FRONTIER || which == TGI_SET_OWNED)) return &c->sets[which];
   return nullptr;
 }
@@ -2300,6 +2309,18 @@ int tgi_frontier_clear(tgi_ctx* c) {
 }
 
 // ---- frontier -> validator hand-off (SURVEY 8f rank 3) ------------------------------------------------------------
+}  // extern "C"
+namespace {
+// a caller-filled set on first use (under fr_mu): the dedup set's capacity, or at most 2^16 keys when the sets grow on
+// their own
+int set_first_use(tgi_ctx* c, KeySet& k, bool stamps) {
+  if (k.dev.table) return TGI_OK;
+  const FrontierDev& fr = c->sets[TGI_SET_FRONTIER].dev;
+  const uint64_t cap = std::min<uint64_t>(c->fr_cap0, 1u << 16);
+  return c->grow_max ? set_alloc(c, k, cap, next_pow2(2 * cap), stamps) : set_alloc(c, k, fr.cap, fr.tmask + 1, stamps);
+}
+}  // namespace
+extern "C" {
 int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* stamp_sec, uint64_t n) {
   if (!c || (n && !keys32)) return TGI_E_ARG;
   KeySet* k = key_set(c, which, true);
@@ -2309,13 +2330,7 @@ int tgi_set_add(tgi_ctx* c, int which, const uint8_t* keys32, const int64_t* sta
   std::lock_guard<std::mutex> g(c->fr_mu);
   cudaStream_t st = c->slots[0].stream;
   const bool stamps = which == TGI_SET_INVALID;
-  if (!k->dev.table) {  // first use: same capacity as the dedup set, or at most 2^16 keys when the sets grow on their own
-    const FrontierDev& fr = c->sets[TGI_SET_FRONTIER].dev;
-    const uint64_t cap = std::min<uint64_t>(c->fr_cap0, 1u << 16);
-    const int rc = c->grow_max ? set_alloc(c, *k, cap, next_pow2(2 * cap), stamps)
-                               : set_alloc(c, *k, fr.cap, fr.tmask + 1, stamps);
-    if (rc) return rc;
-  }
+  if (const int rc = set_first_use(c, *k, stamps)) return rc;
   if (!n) return TGI_OK;
   DevBuf dk, dp;
   CK(dk.ensure(n * 32));
@@ -3657,6 +3672,7 @@ int tgi_state_set(tgi_ctx* c, const tgi_state_layer* layers, uint32_t n_layers, 
   // are renumbered, so the open turns go.
   for (auto& [h, T] : S.turns) S.turn_pool.push_back(std::move(T.keys));
   S.turns.clear();
+  S.n_pend = 0;  // the pending next-layer list names rows
   S.rows.clear();
   S.blob.clear();
   S.gen.clear();
@@ -4329,6 +4345,468 @@ int tgi_state_page_end(tgi_ctx* c, uint32_t turn, int slot, const uint8_t* statu
   if (appended) *appended = S.n_msgs - before;
   S.turn_pool.push_back(std::move(T.keys));
   S.turns.erase(it);
+  return TGI_OK;
+}
+
+}  // extern "C"
+
+// ---- snowball discovery (state.cuh) -----------------------------------------------------------------------------------
+namespace {
+
+// one AddLayer of a discovery call: its depth, whether the call has a page at all (Base rules create the layer then),
+// and its survivors [s0, s1) of S.h_surv
+struct DiscGroup {
+  int64_t depth;
+  bool any;
+  uint64_t s0, s1;
+};
+
+// the checks both discovery calls share; with TGI_DISCOVER_PAGE_JSON the clock must render (json.Marshal's year rule)
+int disc_args(tgi_ctx* c, uint32_t flags, uint32_t allowed, int64_t now_sec, int32_t now_nsec, const char* who) {
+  if (flags & ~allowed) { set_err(c, "%s: unknown flags 0x%x", who, flags); return TGI_E_ARG; }
+  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
+  if (flags & TGI_DISCOVER_PAGE_JSON) {
+    char b[48];
+    std::lock_guard<std::mutex> zg(c->cfg_mu);
+    if (!host_render_zone_time(b, now_sec, now_nsec, c->zone, c->cfgdev.tz)) {
+      set_err(c, "%s: the clock's year is outside [0, 9999] (json.Marshal fails)", who);
+      return TGI_E_ARG;
+    }
+  }
+  return TGI_OK;
+}
+
+// the page-JSON outputs of a call that adds nothing: json_off = {0}
+int disc_json_empty(tgi_ctx* c, CrawlState& S, tgi_state_added_t* out) {
+  CK(S.h_json_off.ensure(8));
+  CK(S.h_out.ensure(1));
+  S.h_json_off.as<uint64_t>()[0] = 0;
+  out->json_off = S.h_json_off.as<uint64_t>();
+  out->page_json = S.h_out.as<uint8_t>();
+  return TGI_OK;
+}
+
+// First occurrences (per span, or over the list) and Dapr's urlCache test over the candidates at d_cands (count d_n on
+// the device, at most bound), compacted into S.surv; the survivors come back to S.h_surv with one id each from counter
+// id_next on (S.h_ids).  Two synchronises: the survivors' count, then their rows and ids.
+int st_survivors(tgi_ctx* c, CrawlState& S, const StCand* d_cands, const uint64_t* d_n, uint64_t bound, bool per_span,
+                 bool dedup, const FrontierDev& urls, uint64_t* n_surv, float* ms, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * bound, 64));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.slot_of.ensure(bound * 4));
+  CK(S.flag.ensure(bound * 4));
+  CK(S.pos.ensure((bound + 1) * 8));
+  CK(S.surv.ensure(bound * sizeof(StCand)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  StFirst w{};
+  w.c = d_cands;
+  w.n = d_n;
+  w.bound = bound;
+  w.per_span = per_span;
+  w.dedup = dedup;
+  w.urls = urls;
+  w.bfirst = S.bfirst.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.slot_of.as<uint32_t>();
+  w.flag = S.flag.as<uint32_t>();
+  w.pos = S.pos.as<uint64_t>();
+  w.out = S.surv.as<StCand>();
+  int rc;
+  CK(cudaEventRecord(S.t2, st));
+  if (dedup) {
+    CK(cudaMemsetAsync(w.bfirst, 0xFF, bslots * 4, st));
+    st_first_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(w);
+    launches++;
+  }
+  st_keep_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(w);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, w.flag, bound, w.pos, S.sc.as<uint64_t>(), launches))) return rc;
+  st_survivors_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(w);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t m = *S.h_sc.as<uint64_t>();
+  float t = 0;
+  cudaEventElapsedTime(&t, S.t2, S.t3);
+  *ms += t;
+  CK(S.h_surv.ensure(m * sizeof(StCand)));
+  CK(S.h_ids.ensure(m * 36));
+  if (m) {
+    CK(S.uuids.ensure(m * 36));
+    CK(cudaMemcpyAsync(S.h_surv.p, S.surv.p, m * sizeof(StCand), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(S.t2, st));
+    st_uuid_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(S.id_seed, S.id_next, m, S.uuids.as<uint8_t>());
+    launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t3, st));
+    CK(cudaMemcpyAsync(S.h_ids.p, S.uuids.p, m * 36, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&t, S.t2, S.t3);
+    *ms += t;
+  }
+  *n_surv = m;
+  return TGI_OK;
+}
+
+// AddLayer of every group in order under Base's or Dapr's rules, on the survivors in S.h_surv and their ids in S.h_ids.
+// The host mirror's URL map decides which pages go in (pageMap changes under UpdatePage / AddLayer overwrites, which a
+// key set cannot follow); nothing changes before every check has passed.
+int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G, bool dapr, bool json, int64_t now_sec,
+                      int32_t now_nsec, int64_t max_pages, const char* who, tgi_state_added_t* out, float* ms,
+                      uint32_t& launches) {
+  const StCand* sv = S.h_surv.as<StCand>();
+  auto url_of = [&](const StCand& k) { return std::string((const char*)k.name, k.len); };
+  // 1. the pages each AddLayer adds, in append order
+  std::vector<uint64_t> pick;
+  std::vector<size_t> gend;
+  std::unordered_set<std::string> seen;  // URLs added earlier in the call: in pageMap (Base) or in the urlCache (Dapr)
+  uint64_t rows = S.rows.size();
+  for (const DiscGroup& g : G) {
+    const bool reached = max_pages > 0 && (int64_t)rows >= max_pages;
+    int64_t replacements = (int64_t)S.deadends;
+    std::vector<std::string> added;
+    for (uint64_t j = g.s0; j < g.s1; j++) {
+      std::string u = url_of(sv[j]);
+      if (seen.count(u)) continue;
+      if (!dapr) {
+        if (S.urls.count(u)) continue;
+        if (reached) {
+          if (replacements <= 0) continue;
+          replacements--;
+        }
+        seen.insert(std::move(u));
+      } else {
+        added.push_back(std::move(u));  // Dapr's urlCache takes the URLs after its loop: a repeat within the page stays
+      }
+      pick.push_back(j);
+      rows++;
+    }
+    for (std::string& u : added) seen.insert(std::move(u));
+    gend.push_back(pick.size());
+  }
+  const uint64_t n_add = pick.size();
+  if (n_add && !S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
+  int rc;
+  // 2. Dapr: the added URLs enter the urlCache first.  The insert is all or nothing (a full set is left untouched,
+  // frontier_append_body), so a set that cannot take them leaves the state as it was
+  if (dapr && n_add) {
+    std::vector<uint8_t> keys(n_add * 32);
+    for (uint64_t k = 0; k < n_add; k++) memcpy(keys.data() + 32 * k, sv[pick[k]].name, 32);
+    std::lock_guard<std::mutex> fg(c->fr_mu);
+    KeySet& U = c->sets[TGI_SET_URLS];
+    if ((rc = set_first_use(c, U, false))) return rc;
+    cudaStream_t st0 = c->slots[0].stream;
+    CK(S.url_keys.ensure(n_add * 32));
+    CK(cudaMemcpyAsync(S.url_keys.p, keys.data(), n_add * 32, cudaMemcpyHostToDevice, st0));
+    if ((rc = frontier_insert_enqueue(c, U, S.url_keys.p, nullptr, n_add, nullptr))) return rc;
+    CK(cudaStreamSynchronize(st0));
+    if ((rc = frontier_insert_check(c, U))) return rc;
+  }
+  // 3. the pages {id, URL, "unfetched", ParentID = the owner's id, depth, the clock in time.Local} on their layers
+  CK(S.h_rows.ensure(n_add * 4 + 4));
+  uint32_t* hr = S.h_rows.as<uint32_t>();
+  const uint8_t* ids = S.h_ids.as<uint8_t>();
+  std::vector<uint32_t> dirty;
+  std::string strs;
+  size_t k = 0;
+  for (size_t gi = 0; gi < G.size(); gi++) {
+    const size_t k1 = gend[gi];
+    if (dapr ? k1 == k : !G[gi].any) continue;  // Dapr creates no layer when nothing is added
+    std::vector<uint32_t>& L = S.layers[G[gi].depth];
+    for (; k < k1; k++) {
+      const StCand& cd = sv[pick[k]];
+      const std::string parent = st_field(S, S.rows[cd.parent], TGI_PS_ID);
+      strs.assign((const char*)ids + 36 * k, 36);
+      strs.append((const char*)cd.name, cd.len);
+      strs += "unfetched";
+      strs += parent;
+      tgi_state_page p{};
+      p.str_len[TGI_PS_ID] = 36;
+      p.str_len[TGI_PS_URL] = cd.len;
+      p.str_len[TGI_PS_STATUS] = 9;
+      p.str_len[TGI_PS_PARENT] = (uint32_t)parent.size();
+      p.ts_off = TGI_STATE_TS_LOCAL;
+      p.depth = G[gi].depth;
+      p.ts_sec = now_sec;
+      p.ts_nsec = now_nsec;
+      const auto it = S.by_id.find(strs.substr(0, 36));
+      uint32_t r = (uint32_t)S.rows.size();
+      if (it != S.by_id.end()) {  // pageMap[id] = page: the old page and its messages go, as in AddLayer
+        r = it->second;
+        if (std::find(dirty.begin(), dirty.end(), r) == dirty.end()) {
+          if (r < S.rows_synced && (rc = st_drop_messages(c, S, r))) return rc;
+          dirty.push_back(r);
+        }
+      }
+      st_put_row(S, r, p, (const uint8_t*)strs.data());
+      L.push_back(r);
+      hr[k] = r;
+    }
+  }
+  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  if ((rc = st_compact(c, S))) return rc;
+  S.id_next += n_add;
+  out->n_added = n_add;
+  out->rows = hr;
+  out->ids = ids;
+  if (!json) return TGI_OK;
+  // 4. json.Marshal of every added page: the export's line passes over the added rows, which hold no messages
+  if (!n_add) return disc_json_empty(c, S, out);
+  CK(S.h_json_off.ensure((n_add + 1) * 8));
+  if ((rc = st_upload_codes(c, S))) return rc;
+  std::lock_guard<std::mutex> zg(c->cfg_mu);  // the zone table, as in tgi_state_render
+  cudaStream_t st = S.stream;
+  const uint64_t ne = n_add, nr = S.rows.size();
+  CK(S.entries.ensure(ne * sizeof(StEntry)));
+  CK(S.row_base.ensure((nr + 1) * 8));
+  CK(S.moff.ensure(8));
+  CK(S.msize.ensure(4));
+  CK(S.e32.ensure(4 * ne * 4));
+  CK(S.e64.ensure(2 * (ne + 1) * 8));
+  StRender r{};
+  r.entries = S.entries.as<StEntry>();
+  r.n_entries = ne;
+  r.zone = c->cfgdev.zone;
+  r.zone_n = c->cfgdev.zone_n;
+  r.tz = c->cfgdev.tz;
+  r.sc = S.sc.as<uint64_t>();
+  r.row_base = S.row_base.as<uint64_t>();  // every row at 0: the added rows count no messages
+  r.msize = S.msize.as<uint32_t>();
+  r.moff = S.moff.as<uint64_t>();
+  r.esize_lo = S.e32.as<uint32_t>();
+  r.ebytes = r.esize_lo + ne;
+  r.ecnt = r.ebytes + ne;
+  r.esz = r.ecnt + ne;
+  r.eoff = S.e64.as<uint64_t>();
+  r.eslot = r.eoff + ne + 1;
+  std::vector<StEntry> E(ne);
+  for (uint64_t q = 0; q < ne; q++) E[q] = StEntry{(long long)S.rows[hr[q]].depth, hr[q], 0};
+  const StDev d = st_dev(S);
+  uint64_t* hs = S.h_sc.as<uint64_t>();
+  CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(r.row_base, 0, (nr + 1) * 8, st));
+  CK(cudaMemsetAsync(r.moff, 0, 8, st));
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+  const unsigned grid = sink_grid(c, ne, ST_WARPS, 16);
+  CK(cudaEventRecord(S.t4, st));
+  st_line_size_kernel<<<grid, ST_WARPS * 32, 0, st>>>(d, r);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, r.esz, ne, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t5, st));
+  CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float t = 0;
+  cudaEventElapsedTime(&t, S.t4, S.t5);
+  *ms += t;
+  if (hs[ST_SC_ERR]) { set_err(c, "%s: a page timestamp's year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  const uint64_t body = hs[ST_SC_BYTES];
+  CK(S.out.ensure(body));
+  CK(S.h_out.ensure(body));
+  r.out = S.out.as<uint8_t>();
+  CK(cudaEventRecord(S.t4, st));
+  st_line_emit_kernel<<<grid, ST_WARPS * 32, 0, st>>>(d, r);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t5, st));
+  CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_json_off.p, r.eoff, (ne + 1) * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&t, S.t4, S.t5);
+  *ms += t;
+  out->page_json = S.h_out.as<uint8_t>();
+  out->json_off = S.h_json_off.as<uint64_t>();
+  return TGI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tgi_state_id_seed(tgi_ctx* c, uint64_t seed) {
+  if (!c) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  S.id_seed = seed;
+  S.seeded = true;
+  return TGI_OK;
+}
+
+// The candidates of the spans gathered from the slot's resident result (a thread per processed link row, a scan, the
+// compaction), then either appended to the pending list or deduplicated per span, tested against the urlCache and read
+// back as survivors for the AddLayers.  Lock order: the slot, then the state (as tgi_state_page_end); the slot's lock is
+// held until the kernels that read its result have finished.
+int tgi_state_discover(tgi_ctx* c, int slot, const tgi_state_span* spans, uint32_t n_spans, uint32_t flags, int64_t now_sec,
+                       int32_t now_nsec, int64_t max_pages, tgi_state_added_t* out) {
+  static const char* const who = "tgi_state_discover";
+  if (!c || !out || (n_spans && !spans)) return TGI_E_ARG;
+  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
+  Slot& s = c->slots[slot];
+  std::lock_guard<std::mutex> sl(s.mu);
+  if (in_flight(s)) { set_err(c, "%s: slot %d is in flight", who, slot); return TGI_E_STATE; }
+  if (!s.busy || s.last.kind == REC_NONE) { set_err(c, "%s: slot %d holds no result (released or none)", who, slot); return TGI_E_STATE; }
+  if (s.last.kind != REC_TG) { set_err(c, "%s: slot %d's result is not a Telegram one", who, slot); return TGI_E_STATE; }
+  if (!s.last.dev.link_off || !s.last.dev.links) { set_err(c, "%s: slot %d's result has no links (run it with TGI_RUN_LINKS)", who, slot); return TGI_E_STATE; }
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  if ((rc = disc_args(c, flags, TGI_DISCOVER_NOW | TGI_DISCOVER_DAPR | TGI_DISCOVER_PAGE_JSON, now_sec, now_nsec, who))) return rc;
+  if ((flags & TGI_DISCOVER_PAGE_JSON) && (rc = disc_json_empty(c, S, out))) return rc;
+  const uint64_t n = s.last.n;
+  std::vector<std::pair<uint64_t, int>> ev;  // the processed records' intervals: the gather's bound
+  for (uint32_t k = 0; k < n_spans; k++) {
+    const tgi_state_span& sp = spans[k];
+    if (sp.row >= S.rows.size()) { set_err(c, "%s: span %u: no row %u", who, k, sp.row); return TGI_E_ARG; }
+    if (sp.first > n || sp.n_records > n - sp.first) { set_err(c, "%s: span %u lies outside the result's %llu records", who, k, (unsigned long long)n); return TGI_E_ARG; }
+    if (sp.n_done > sp.n_records) { set_err(c, "%s: span %u: n_done %llu > n_records %llu", who, k, (unsigned long long)sp.n_done, (unsigned long long)sp.n_records); return TGI_E_ARG; }
+    if (sp.n_done) {
+      ev.emplace_back(sp.first, 1);
+      ev.emplace_back(sp.first + sp.n_done, -1);
+    }
+  }
+  std::sort(ev.begin(), ev.end(), [](const auto& a, const auto& b) { return a.first != b.first ? a.first < b.first : a.second < b.second; });
+  int64_t cover = 0, most = 0;
+  for (const auto& e : ev) most = std::max(most, cover += e.second);
+  const uint64_t bound = (uint64_t)most * s.last.n_links;  // link rows over the spans' processed records, at most
+  const bool now = flags & TGI_DISCOVER_NOW, dapr = flags & TGI_DISCOVER_DAPR, json = flags & TGI_DISCOVER_PAGE_JSON;
+  if (!bound) return TGI_OK;  // no candidate: no AddLayer call, nothing pending
+  if (!now && (rc = st_grow(c, S, S.pend, S.n_pend * sizeof(StCand), (S.n_pend + bound) * sizeof(StCand)))) return rc;
+  cudaStream_t st = S.stream;
+  CK(S.spans.ensure(n_spans * sizeof(tgi_state_span)));
+  CK(S.cnt.ensure(n_spans * 4));
+  CK(S.soff.ensure((n_spans + 1) * 8));
+  CK(S.coff.ensure((n_spans + 1) * 8));
+  CK(S.lnk.ensure(bound * 4));
+  CK(S.spn.ensure(bound * 4));
+  CK(S.flag.ensure(bound * 4));
+  CK(S.pos.ensure((bound + 1) * 8));
+  if (now) CK(S.cand.ensure(bound * sizeof(StCand)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_coff.ensure((n_spans + 1) * 8));
+  StDisc gd{};
+  gd.spans = S.spans.as<tgi_state_span>();
+  gd.n_spans = n_spans;
+  gd.status = s.last.dev.status;
+  gd.link_off = s.last.dev.link_off;
+  gd.links = s.last.dev.links;
+  gd.soff = S.soff.as<uint64_t>();
+  gd.bound = bound;
+  gd.flag = S.flag.as<uint32_t>();
+  gd.lnk = S.lnk.as<uint32_t>();
+  gd.spn = S.spn.as<uint32_t>();
+  gd.pos = S.pos.as<uint64_t>();
+  gd.out = now ? S.cand.as<StCand>() : S.pend.as<StCand>() + S.n_pend;
+  gd.coff = S.coff.as<uint64_t>();
+  uint32_t launches = 0;
+  float ms = 0;
+  CK(cudaMemcpyAsync(S.spans.p, spans, n_spans * sizeof(tgi_state_span), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(S.ev_slot, s.stream));  // the result is complete on the slot's stream
+  CK(cudaStreamWaitEvent(st, S.ev_slot, 0));
+  CK(cudaEventRecord(S.t0, st));
+  st_disc_count_kernel<<<st_grid(c, n_spans), ST_THREADS, 0, st>>>(gd, S.cnt.as<uint32_t>());
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, S.cnt.as<uint32_t>(), n_spans, S.soff.as<uint64_t>(), S.sc.as<uint64_t>() + 1, launches))) return rc;
+  st_disc_flag_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(st_dev(S), gd);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, gd.flag, bound, gd.pos, S.sc.as<uint64_t>() + 2, launches))) return rc;
+  st_disc_emit_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(gd);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_coff.p, gd.coff, (n_spans + 1) * 8, cudaMemcpyDeviceToHost, st));
+  const uint64_t* coff = S.h_coff.as<uint64_t>();
+  if (!now) {
+    CK(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&ms, S.t0, S.t1);
+    S.n_pend += coff[n_spans];
+    out->n_candidates = coff[n_spans];
+    out->kernel_ms = ms;
+    out->gpu_launches = launches;
+    return TGI_OK;
+  }
+  // per span: first occurrences under Base's rules (none under Dapr's) and Dapr's urlCache test
+  uint64_t n_surv = 0;
+  {
+    std::unique_lock<std::mutex> fg(c->fr_mu, std::defer_lock);
+    FrontierDev urls{};
+    if (dapr) {
+      fg.lock();
+      if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+      urls = c->sets[TGI_SET_URLS].dev;
+    }
+    if ((rc = st_survivors(c, S, S.cand.as<StCand>(), gd.coff + n_spans, bound, true, !dapr, urls, &n_surv, &ms, launches))) return rc;
+  }
+  float gather_ms = 0;
+  cudaEventElapsedTime(&gather_ms, S.t0, S.t1);
+  ms += gather_ms;
+  const StCand* sv = S.h_surv.as<StCand>();
+  std::vector<DiscGroup> G(n_spans);
+  uint64_t j = 0;
+  for (uint32_t k = 0; k < n_spans; k++) {
+    G[k].depth = S.rows[spans[k].row].depth + 1;
+    G[k].any = coff[k + 1] > coff[k];
+    G[k].s0 = j;
+    while (j < n_surv && sv[j].span == k) j++;
+    G[k].s1 = j;
+  }
+  out->n_candidates = coff[n_spans];
+  if ((rc = st_discover_apply(c, S, G, dapr, json, now_sec, now_nsec, max_pages, who, out, &ms, launches))) {
+    out->n_candidates = 0;
+    return rc;
+  }
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The layer end of dapr/standalone.go:647-688 over the pending list: first occurrences over the whole list, Dapr's
+// urlCache test, the survivors read back for one AddLayer at layer_depth + 1; the list is emptied once it applied.
+int tgi_state_next_layer(tgi_ctx* c, int64_t layer_depth, uint32_t flags, int64_t now_sec, int32_t now_nsec,
+                         int64_t max_pages, tgi_state_added_t* out) {
+  static const char* const who = "tgi_state_next_layer";
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  if ((rc = disc_args(c, flags, TGI_DISCOVER_DAPR | TGI_DISCOVER_PAGE_JSON, now_sec, now_nsec, who))) return rc;
+  if ((flags & TGI_DISCOVER_PAGE_JSON) && (rc = disc_json_empty(c, S, out))) return rc;
+  if (!S.n_pend) return TGI_OK;
+  const bool dapr = flags & TGI_DISCOVER_DAPR, json = flags & TGI_DISCOVER_PAGE_JSON;
+  const uint64_t m = S.n_pend;
+  cudaStream_t st = S.stream;
+  CK(S.h_coff.ensure(8));
+  CK(S.coff.ensure(8));
+  *S.h_coff.as<uint64_t>() = m;
+  CK(cudaMemcpyAsync(S.coff.p, S.h_coff.p, 8, cudaMemcpyHostToDevice, st));
+  uint32_t launches = 0;
+  float ms = 0;
+  uint64_t n_surv = 0;
+  {
+    std::unique_lock<std::mutex> fg(c->fr_mu, std::defer_lock);
+    FrontierDev urls{};
+    if (dapr) {
+      fg.lock();
+      if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+      urls = c->sets[TGI_SET_URLS].dev;
+    }
+    if ((rc = st_survivors(c, S, S.pend.as<StCand>(), S.coff.as<uint64_t>(), m, false, true, urls, &n_surv, &ms, launches))) return rc;
+  }
+  const std::vector<DiscGroup> G(1, DiscGroup{layer_depth + 1, true, 0, n_surv});
+  if ((rc = st_discover_apply(c, S, G, dapr, json, now_sec, now_nsec, max_pages, who, out, &ms, launches))) return rc;
+  S.n_pend = 0;
+  out->n_candidates = m;
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
   return TGI_OK;
 }
 

@@ -39,6 +39,7 @@ EXPORTED_SYMBOLS = [
     "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
+    "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer",
 ]
 
 
@@ -118,6 +119,9 @@ def lib() -> C.CDLL:
         L.tgi_state_export.argtypes = [vp, i32, u64, C.POINTER(abi.StateExportC)]
         L.tgi_state_page_begin.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, C.POINTER(abi.StateTurnC)]
         L.tgi_state_page_end.argtypes = [vp, u32, i32, vp, u64, C.POINTER(u64)]
+        L.tgi_state_id_seed.argtypes = [vp, u64]
+        L.tgi_state_discover.argtypes = [vp, i32, vp, u32, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
+        L.tgi_state_next_layer.argtypes = [vp, C.c_int64, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         _LIB = L
     return _LIB
 
@@ -696,6 +700,46 @@ class Engine:
         self._check(lib().tgi_state_page_end(self.h, turn, slot, st.ctypes.data if st is not None and len(st) else None,
                                              n_done, C.byref(appended)))
         return appended.value
+
+    # --- snowball discovery: outlinks of processed pages as next-layer pages ---------------------------------------
+    def state_id_seed(self, seed: int):
+        """the key of the page-id generator (Philox4x32-10); no page is added before it is set"""
+        self._check(lib().tgi_state_id_seed(self.h, seed))
+
+    def _st_added(self, out: abi.StateAddedC, json: bool) -> dict:
+        n = int(out.n_added)
+        rows = np.ctypeslib.as_array(out.rows, (n,)).tolist() if n else []
+        blob = C.string_at(out.ids, 36 * n) if n else b""
+        ids = [blob[36 * k:36 * k + 36] for k in range(n)]
+        self._st_note_rows([{"id": i} for i in ids], rows)
+        self.state_discover_ms = float(out.kernel_ms)
+        self.state_discover_launches = int(out.gpu_launches)
+        res = {"n_candidates": int(out.n_candidates), "rows": rows, "ids": ids, "page_json": None}
+        if json:
+            off = np.ctypeslib.as_array(out.json_off, (n + 1,)).tolist()
+            lines = C.string_at(out.page_json, off[n]) if off[n] else b""
+            res["page_json"] = [lines[off[k]:off[k + 1] - 1] for k in range(n)]  # each value without its '\n'
+        return res
+
+    def state_discover(self, slot: int, spans, flags: int = abi.DISCOVER_NOW, now=(0, 0), max_pages: int = 0) -> dict:
+        """the outlinks of the slot's last Telegram result as next-layer pages: spans = (row, first, n_records, n_done)
+        per owner page; flags = abi.DISCOVER_*; now = (sec, nsec) of the added pages.  Returns {"n_candidates", "rows",
+        "ids", "page_json"} (page_json: json.Marshal of every added page with abi.DISCOVER_PAGE_JSON, else None).  The
+        device time is left in self.state_discover_ms"""
+        sp = np.zeros(max(len(spans), 1), abi.STATE_SPAN)
+        for k, (row, first, n_records, n_done) in enumerate(spans):
+            sp[k] = (row, 0, first, n_records, n_done)
+        out = abi.StateAddedC()
+        self._check(lib().tgi_state_discover(self.h, slot, sp.ctypes.data, len(spans), flags, now[0], now[1], max_pages,
+                                             C.byref(out)))
+        return self._st_added(out, bool(flags & abi.DISCOVER_PAGE_JSON))
+
+    def state_next_layer(self, layer_depth: int, flags: int = 0, now=(0, 0), max_pages: int = 0) -> dict:
+        """the layer end over the pending list (first occurrence per URL, Depth = layer_depth + 1, then AddLayer under
+        abi.DISCOVER_DAPR's rules or Base's); returns what state_discover returns"""
+        out = abi.StateAddedC()
+        self._check(lib().tgi_state_next_layer(self.h, layer_depth, flags, now[0], now[1], max_pages, C.byref(out)))
+        return self._st_added(out, bool(flags & abi.DISCOVER_PAGE_JSON))
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

@@ -355,6 +355,25 @@ class MessageProcessor {
     if (tgi_state_page_end(ctx_, turn, slot, nullptr, n_done, &appended) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
     return appended;
   }
+  // Snowball discovery: the outlinks of the slot's Telegram result as next-layer pages.  StateDiscover with
+  // TGI_DISCOVER_NOW is the standalone runner's AddLayer per page; without it the candidates wait in the pending list
+  // for StateNextLayer, the Dapr runner's layer end.  The returned arrays stay valid until the next state call.
+  void StateIdSeed(uint64_t seed) {
+    if (tgi_state_id_seed(ctx_, seed) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+  }
+  tgi_state_added_t StateDiscover(int slot, const std::vector<tgi_state_span>& spans, uint32_t flags, int64_t now_sec,
+                                  int32_t now_nsec, int64_t max_pages = 0) {
+    tgi_state_added_t a{};
+    if (tgi_state_discover(ctx_, slot, spans.data(), (uint32_t)spans.size(), flags, now_sec, now_nsec, max_pages, &a) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return a;
+  }
+  tgi_state_added_t StateNextLayer(int64_t layer_depth, uint32_t flags, int64_t now_sec, int32_t now_nsec, int64_t max_pages = 0) {
+    tgi_state_added_t a{};
+    if (tgi_state_next_layer(ctx_, layer_depth, flags, now_sec, now_nsec, max_pages, &a) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return a;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

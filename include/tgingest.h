@@ -909,6 +909,81 @@ int tgi_state_page_begin(tgi_ctx* ctx, uint32_t row, const tgi_state_page* page,
                          const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out);
 int tgi_state_page_end(tgi_ctx* ctx, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended);
 
+/* Snowball discovery — the outlinks of processed pages become the next layer's pages (crawl/runner.go:1199-1244 outside
+ * random-walk, then standalone/runner.go:835-850 or dapr/standalone.go:612-616, 645-688), read straight from a slot's
+ * resident Telegram result: nothing is read back before the dedup, so it works after TGI_RUN_JSONL_DEVICE and
+ * TGI_RUN_NO_D2H, and only the deduplicated survivors (name, parent) cross to the host.
+ *   Candidates  span k names one owner page (row) and its records [first, first+n_records) of the result, of which the
+ *            loop processed the first n_done.  Every link row of a processed record whose status is TGI_ST_EMITTED or
+ *            TGI_ST_NOLINE is a candidate (a failed record returned an error and a date-skipped one an empty Post: no
+ *            outlinks), unless its name is byte-equal to the owner row's URL as the state holds it (`o == owner.URL`,
+ *            case-sensitive: not TGI_LF_SELF, which compares with the record's channel name).  Candidate order is
+ *            (span, record, link row); Go ranges over a per-message map, so every order inside a message is a valid
+ *            output and this one is fixed.  TGI_RUN_FILTER / SKIP_SELF / SKIP_INVALID only gate the dedup-set insert;
+ *            the link rows stay whole.  Each candidate becomes {URL: name, Status: "unfetched", ParentID: owner.ID,
+ *            Depth: owner.Depth + 1} with the owner as it is at the call.
+ *   Discover tgi_state_discover.  TGI_DISCOVER_NOW: each span with at least one candidate is one AddLayer, in span
+ *            order, under BaseStateManager's rules (base.go:219-322, as tgi_state_add_layer: first occurrence per URL
+ *            within the span, URLs already in the state skipped, max_pages with the deadend budget, the layer of
+ *            owner.Depth + 1 created even if every page is skipped) or with TGI_DISCOVER_DAPR DaprStateManager's
+ *            (daprstate.go:625-780: a URL in the urlCache set TGI_SET_URLS is skipped, NO dedup within the call, so a
+ *            page that mentions a channel twice adds it twice; no max_pages; no layer when nothing is added; the added
+ *            URLs then enter TGI_SET_URLS).  A span without candidates makes no call and creates no layer.  Without
+ *            TGI_DISCOVER_NOW the candidates (name, owner row) are appended to the state's pending next-layer list on
+ *            the device and the state is otherwise unchanged.
+ *   Layer end tgi_state_next_layer = the layer end of dapr/standalone.go:647-688 over the pending list: the first
+ *            occurrence of every URL, its ParentID included, with Depth = layer_depth + 1, then AddLayer under the
+ *            chosen rules, then the list is emptied.  An empty list changes nothing.  tgi_state_set drops the list.
+ *   Pages    every added page gets an id and the timestamp (now_sec, now_nsec) in time.Local (TGI_STATE_TS_LOCAL): one
+ *            clock reading per call, where Go reads it per page.  out->rows / ids list the added pages in the order
+ *            AddLayer appended them.  TGI_DISCOVER_PAGE_JSON: page_json holds json.Marshal(page) + '\n' of every added
+ *            page (its tgi_state_export line), page k's value being [json_off[k], json_off[k+1] - 1): the values of
+ *            Dapr's per-page SaveState("<execID>/page/<id>").  All of out lives until the next state call.
+ *   Ids      uuid.New() is random; the library makes its own version-4 ids.  The n-th page added under the context (n
+ *            counts added pages only, and tgi_state_set does not reset it) takes the id from Philox4x32-10 with counter
+ *            (n_lo, n_hi, 0, 0) and key (seed_lo, seed_hi): the four words little-endian as 16 bytes, then
+ *            b[6] = b[6]&0x0f|0x40 and b[8] = b[8]&0x3f|0x80, as lowercase 8-4-4-4-12 hex.  Philox is a bijection of the
+ *            counter and only the 6 version / variant bits are overwritten, so two ids of one seed collide as often as
+ *            two random v4 uuids.  tgi_state_id_seed sets the key (the shim seeds it once from crypto/rand); without it a
+ *            call that would add a page returns TGI_E_STATE: a built-in seed would repeat ids across processes.
+ *   urlCache TGI_SET_URLS is Dapr's urlCache on the device: the shim seeds it with tgi_set_add from initializeURLCache
+ *            / loadURLsForCrawl, skipping URLs longer than 32 bytes (a key holds 32; an outlink name is 5-32 bytes and
+ *            can never equal them); Dapr-rule AddLayers grow it, as tgi_set_growth lets every set grow.
+ *   Cost     the call sizes its scratch (flags, scans, the batch table) by the result's link rows times the largest
+ *            number of spans that share a record, without reading anything back: pass all the spans of one result in
+ *            one call (a page-sized result: its one span), not one call per page of a bulk result.
+ *   Errors   a rejected call (TGI_E_ARG, TGI_E_STATE, and TGI_E_CAPACITY when TGI_SET_URLS cannot take the added URLs:
+ *            the set's insert is all or nothing) leaves the state, the pending list and TGI_SET_URLS unchanged; after
+ *            TGI_E_CUDA or TGI_E_NOMEM the added URLs may be in TGI_SET_URLS without their pages.  TGI_E_ARG: an unknown row, a span outside
+ *            the result, n_done > n_records, now_nsec outside [0, 1e9), unknown flags, and with
+ *            TGI_DISCOVER_PAGE_JSON a clock whose year leaves [0, 9999].  TGI_E_STATE: no, a released or a non-Telegram
+ *            result, a result run without TGI_RUN_LINKS, a job in flight on the slot, no seed.  Lock order: the slot,
+ *            then the state (as tgi_state_page_end).                                                                */
+#define TGI_SET_URLS 4              /* Dapr's urlCache (daprstate.go:646-658): seeded with tgi_set_add            */
+#define TGI_DISCOVER_NOW 1u         /* AddLayer per span now (standalone/runner.go:835-850); else append to pending */
+#define TGI_DISCOVER_DAPR 2u        /* DaprStateManager.AddLayer's rules instead of BaseStateManager's            */
+#define TGI_DISCOVER_PAGE_JSON 4u   /* json.Marshal of every added page (Dapr's per-page SaveState value)         */
+typedef struct tgi_state_span {     /* 32 bytes: one owner page's records in the slot's result                    */
+  uint32_t row;                     /* the owner page: its URL, id and depth at the call                          */
+  uint32_t reserved;
+  uint64_t first, n_records, n_done;
+} tgi_state_span;
+typedef struct tgi_state_added_t {
+  uint64_t n_candidates;            /* outlinks considered after the self test                                   */
+  uint64_t n_added;
+  const uint32_t* rows;             /* [n_added] the new rows, in the order AddLayer appended them (pinned)      */
+  const uint8_t* ids;               /* [n_added][36] their uuid strings (pinned)                                 */
+  const uint8_t* page_json;         /* with TGI_DISCOVER_PAGE_JSON: the added pages' lines, else NULL (pinned)   */
+  const uint64_t* json_off;         /* [n_added+1] line k is [json_off[k], json_off[k+1]), its '\n' last         */
+  float kernel_ms;                  /* device time of the call's kernels and scans (not the copies between them) */
+  uint32_t gpu_launches;
+} tgi_state_added_t;
+int tgi_state_id_seed(tgi_ctx* ctx, uint64_t seed);
+int tgi_state_discover(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint32_t n_spans, uint32_t flags,
+                       int64_t now_sec, int32_t now_nsec, int64_t max_pages, tgi_state_added_t* out);
+int tgi_state_next_layer(tgi_ctx* ctx, int64_t layer_depth, uint32_t flags, int64_t now_sec, int32_t now_nsec,
+                         int64_t max_pages, tgi_state_added_t* out);
+
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
                          uint8_t* reason);
