@@ -194,7 +194,7 @@ class StateJsonC(C.Structure):  # tgi_state_json_t
 
 
 E_NOPAGES = -7  # tgi_state_export: the layer map holds no page ("no pages found to export")
-TURN_PAGE_JSON = 1  # tgi_state_page_begin: also json.Marshal(page), the value Dapr's UpdatePage saves
+TURN_PAGE_JSON = 1  # tgi_state_page_begin / _close: also json.Marshal(page), the value Dapr's UpdatePage saves
 
 
 class StateTurnC(C.Structure):  # tgi_state_turn_t

@@ -22,6 +22,7 @@
 // Page turns (crawl/runner.go:1132-1211): a thread per fetched key probes the table at the row's current generation and
 // records the first fetched index of its message id; the new keys become the row's next generation, and the one page
 // renders through the export's line passes over that fresh contiguous segment.  Nothing reads another row's messages.
+// The turn's owner keys stay as the row's owner view; the close appends the view as the row's next generation.
 #pragma once
 #include "local_appends.cuh"
 
@@ -226,6 +227,82 @@ __global__ void st_turn_updates_kernel(const long long* keys, const uint8_t* sta
     v.status = status[j] == TGI_ST_FAILED ? 3 : 2;  // "failed" : "fetched"
     v.reserved = 0;
     u[j] = v;
+  }
+}
+
+// ---- page close: UpdatePage(*owner) (crawl/runner.go:1543-1544) over the row's owner view ---------------------------
+// The view is the turn's k owner messages: their keys and a status code each, 0 while no hit of the end reached the
+// owner (the message is still "resample").  Go's owner shares its backing array with pageMap's page until an append
+// reallocates it; the array counts as full, so an UpdateMessage of the end reaches the owner only before the end's first
+// append, and then the first owner message with the key takes the status.
+struct StView {
+  const long long* keys;  // [k][2] chat_id, message_id of owner message p
+  uint16_t* status;       // [k]
+  uint64_t k;
+  uint32_t* vfirst;       // batch table keyed by the owner's keys: lowest owner index, ST_NONE = empty
+  uint64_t vmask;
+  uint32_t* last;         // [k] 1 + the last update that reached owner message p (0: none); [k]: the end's first append
+};
+
+DEVI uint64_t st_view_slot(const StView& v, long long chat, long long msg) { return st_hash(0, 0, chat, msg) & v.vmask; }
+
+// 1. the owner's keys by first owner index, and the first update of the end that appended (the lowest flagged leader)
+__global__ void st_view_build_kernel(StView v, const uint32_t* flag, uint64_t n) {
+  const uint64_t m = v.k > n ? v.k : n;
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < m; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (j < n && flag[j]) atomicMin(v.last + v.k, (uint32_t)j);
+    if (j >= v.k) continue;
+    const long long chat = v.keys[2 * j], msg = v.keys[2 * j + 1];
+    for (uint64_t s = st_view_slot(v, chat, msg);; s = (s + 1) & v.vmask) {
+      const uint32_t cur = atomicCAS(v.vfirst + s, ST_NONE, (uint32_t)j);
+      if (cur == ST_NONE) break;
+      if (v.keys[2 * cur] == chat && v.keys[2 * cur + 1] == msg) {
+        atomicMin(v.vfirst + s, (uint32_t)j);
+        break;
+      }
+    }
+  }
+}
+
+// 2. every update before the first append whose key is an owner key reaches that key's first owner message
+__global__ void st_view_hit_kernel(StView v, const tgi_state_update* u, uint64_t n) {
+  const uint32_t a = v.last[v.k];
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n && j < a; j += (uint64_t)gridDim.x * blockDim.x) {
+    const long long chat = u[j].chat_id, msg = u[j].message_id;
+    for (uint64_t s = st_view_slot(v, chat, msg);; s = (s + 1) & v.vmask) {
+      const uint32_t cur = v.vfirst[s];
+      if (cur == ST_NONE) break;
+      if (v.keys[2 * cur] == chat && v.keys[2 * cur + 1] == msg) {
+        atomicMax(v.last + cur, (uint32_t)j + 1);
+        break;
+      }
+    }
+  }
+}
+
+// 3. the last such update's status, in update order
+__global__ void st_view_status_kernel(StView v, const tgi_state_update* u) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < v.k; p += (uint64_t)gridDim.x * blockDim.x)
+    if (v.last[p]) v.status[p] = u[v.last[p] - 1].status;
+}
+
+// the close: the view's messages appended as the row's live list of generation gen, at n0 (pageId = the page, no
+// platform), and the row's count; sorted / rows are the one-page render's grouped order
+__global__ void st_view_append_kernel(StDev d, StView v, uint32_t row, uint32_t gen, uint64_t n0, uint32_t* sorted,
+                                      uint32_t* rows) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < v.k; p += (uint64_t)gridDim.x * blockDim.x) {
+    StMsg m;
+    m.chat = v.keys[2 * p];
+    m.msg = v.keys[2 * p + 1];
+    m.row = row;
+    m.gen = gen;
+    m.pid = row;
+    m.status = v.status[p] ? v.status[p] : 5;  // "resample"
+    m.platform = 0;
+    d.msgs[n0 + p] = m;
+    sorted[p] = (uint32_t)(n0 + p);
+    rows[p] = row;
+    if (p == 0) d.row_cnt[row] = (uint32_t)v.k;
   }
 }
 

@@ -212,15 +212,21 @@ struct CrawlState {
   DevBuf entries, keys, vals, row_base, msize, moff, e32, e64, counts, roff, out;
   DevBuf lm_keys, cb_tasks, cb_segs, b64;  // the layer map's openings; the export's encode tasks and output
   HostBuf h_out, h_sc, h_read, h_chunks;
-  // page turns (tgi_state_page_begin / _end): each open turn's row and owner keys, by handle; the key buffers of
-  // closed turns are kept for the next ones
+  // page turns (tgi_state_page_begin / _end / _close): each open turn's row and owner keys, by handle, and each row's
+  // owner view (tgi_state_page_close): the last begin's owner keys and their statuses, in the same buffer as that
+  // turn's keys.  A buffer neither a turn nor a view holds is kept for the next begins.
   struct Turn {
     uint32_t row = 0;
     uint64_t n_work = 0;
-    std::unique_ptr<DevBuf> keys;  // [n_work][2] chat_id, message_id
+    std::shared_ptr<DevBuf> keys;  // [n_work][2] chat_id, message_id, then the view's uint16 statuses [n_work]
+  };
+  struct View {
+    uint64_t k = 0;
+    std::shared_ptr<DevBuf> keys;  // as Turn::keys
   };
   std::map<uint32_t, Turn> turns;
-  std::vector<std::unique_ptr<DevBuf>> turn_pool;
+  std::unordered_map<uint32_t, View> views;  // by row
+  std::vector<std::shared_ptr<DevBuf>> turn_pool;
   uint32_t next_turn = 1;
   cudaEvent_t ev_slot = nullptr;  // tgi_state_page_end: the slot's work the state stream waits for
   DevBuf turn_in;                 // the fetched keys of tgi_state_page_begin
@@ -3472,13 +3478,125 @@ int st_upload_codes(tgi_ctx* c, CrawlState& S) {
   return TGI_OK;
 }
 
-// the row's message generation moves on: its messages become tombstones
+// a key buffer of a turn or a view lets go; the last holder returns it to the pool
+void st_release(CrawlState& S, std::shared_ptr<DevBuf>& b) {
+  if (b && b.use_count() == 1) S.turn_pool.push_back(std::move(b));
+  b.reset();
+}
+
+void st_drop_view(CrawlState& S, uint32_t r) {
+  const auto it = S.views.find(r);
+  if (it == S.views.end()) return;
+  st_release(S, it->second.keys);
+  S.views.erase(it);
+}
+
+// the row's message generation moves on: its messages become tombstones, and a page that replaces the row (UpdatePage,
+// an overwriting AddLayer) ends its owner view
 int st_drop_messages(tgi_ctx* c, CrawlState& S, uint32_t r) {
   uint32_t cnt = 0;
   int rc;
   if ((rc = st_row_count(c, S, r, &cnt))) return rc;
   S.n_dead += cnt;
   S.gen[r]++;
+  st_drop_view(S, r);
+  return TGI_OK;
+}
+
+// UpdatePage's fields for a turn's row (base.go:123-149): page (optional) replaces the row's fields and the host maps
+// follow; the row joins the layer of its depth if that layer exists and does not hold it.  new_list: the row's
+// generation has moved on, and its count goes to 0 for the caller to set; otherwise the list stays as it is.
+int st_page_fields(tgi_ctx* c, CrawlState& S, uint32_t row, const tgi_state_page* page, const uint8_t* strs, bool new_list) {
+  if (page) st_put_row(S, row, *page, strs);
+  const auto lit = S.layers.find(S.rows[row].depth);
+  if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), row) == lit->second.end()) lit->second.push_back(row);
+  const std::vector<uint32_t> dirty(new_list ? 1 : 0, row);
+  const int rc = st_sync_rows(c, S, dirty);
+  if (rc) return rc;
+  if (!new_list) CK(cudaMemcpyAsync(S.pages.as<tgi_state_page>() + row, &S.rows[row], sizeof(tgi_state_page), cudaMemcpyHostToDevice, S.stream));
+  return TGI_OK;
+}
+
+// json.Marshal(page) of one row by the export's line passes: its cnt messages are sorted[0, cnt) (message indices in
+// list order; rows[] holds the row for each).  The size pass is enqueued into r (no synchronise); once the host has
+// S.sc in hs, st_page_json_emit writes the bytes and brings them back.
+int st_page_json_size(tgi_ctx* c, CrawlState& S, uint32_t row, const uint32_t* sorted, const uint32_t* rows, uint64_t cnt,
+                      StRender& r, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  int rc;
+  CK(S.entries.ensure(sizeof(StEntry)));
+  CK(S.row_base.ensure((S.rows.size() + 1) * 8));
+  CK(S.msize.ensure(cnt * 4));
+  CK(S.moff.ensure((cnt + 1) * 8));
+  CK(S.e32.ensure(4 * 4));
+  CK(S.e64.ensure(2 * 2 * 8));
+  r.entries = S.entries.as<StEntry>();
+  r.n_entries = 1;
+  r.zone = c->cfgdev.zone;
+  r.zone_n = c->cfgdev.zone_n;
+  r.tz = c->cfgdev.tz;
+  r.sc = S.sc.as<uint64_t>();
+  r.row_base = S.row_base.as<uint64_t>();  // only row_base[row] = 0 is read
+  r.msize = S.msize.as<uint32_t>();
+  r.moff = S.moff.as<uint64_t>();
+  r.esize_lo = S.e32.as<uint32_t>();
+  r.ebytes = r.esize_lo + 1;
+  r.ecnt = r.ebytes + 1;
+  r.esz = r.ecnt + 1;
+  r.eoff = S.e64.as<uint64_t>();
+  r.eslot = r.eoff + 2;
+  const StDev d = st_dev(S);
+  const StEntry e{(long long)S.rows[row].depth, row, 0};
+  CK(cudaMemcpyAsync(S.entries.p, &e, sizeof e, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(r.row_base + row, 0, 8, st));
+  CK(cudaMemsetAsync(r.moff, 0, 8, st));
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+  if (cnt) {
+    st_msg_size_kernel<<<st_grid(c, cnt), ST_THREADS, 0, st>>>(d, r, sorted, rows, cnt);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.msize, cnt, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
+  }
+  st_line_size_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, r.esz, 1, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, r.ecnt, 1, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+  CK(cudaGetLastError());
+  return TGI_OK;
+}
+
+// the page's bytes after its size pass (hs = the size pass's S.sc).  Dapr's UpdatePage has changed pageMap before
+// json.Marshal fails (daprstate.go:1378-1387): a timestamp that does not render, or a page of 4 GiB or more, fails the
+// call after the update.
+int st_page_json_emit(tgi_ctx* c, CrawlState& S, StRender& r, const uint32_t* sorted, uint64_t cnt, const uint64_t* hs,
+                      const char* who, const uint8_t** data, uint64_t* len, float* ms, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  int rc;
+  if (hs[ST_SC_ERR]) {
+    rc = st_compact(c, S);
+    if (!rc) set_err(c, "%s: the page's timestamp year is outside [0, 9999] (json.Marshal fails)", who);
+    return rc ? rc : TGI_E_ARG;
+  }
+  if (hs[ST_SC_BIG]) {
+    rc = st_compact(c, S);
+    if (!rc) set_err(c, "%s: the page renders to 4 GiB or more", who);
+    return rc ? rc : TGI_E_CAPACITY;
+  }
+  const uint64_t body = hs[ST_SC_BYTES];
+  CK(S.out.ensure(body));
+  CK(S.h_out.ensure(body));
+  r.out = S.out.as<uint8_t>();
+  const StDev d = st_dev(S);
+  CK(cudaEventRecord(S.t4, st));
+  st_line_emit_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+  if (cnt) st_msg_emit_kernel<<<st_grid(c, cnt), ST_THREADS, 0, st>>>(d, r, sorted);
+  launches += 1 + (cnt != 0);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t5, st));
+  CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(ms, S.t4, S.t5);
+  *data = S.h_out.as<uint8_t>();
+  *len = body - 1;  // the line without its '\n'
   return TGI_OK;
 }
 
@@ -3669,9 +3787,11 @@ int tgi_state_set(tgi_ctx* c, const tgi_state_layer* layers, uint32_t n_layers, 
       return TGI_E_ARG;
     }
   // SetState: new maps, layer by layer; a later page with the same id replaces the row (and its messages).  The rows
-  // are renumbered, so the open turns go.
-  for (auto& [h, T] : S.turns) S.turn_pool.push_back(std::move(T.keys));
+  // are renumbered, so the open turns and the owner views go.
+  for (auto& [h, T] : S.turns) st_release(S, T.keys);
+  for (auto& [r, V] : S.views) st_release(S, V.keys);
   S.turns.clear();
+  S.views.clear();
   S.n_pend = 0;  // the pending next-layer list names rows
   S.rows.clear();
   S.blob.clear();
@@ -4133,15 +4253,15 @@ int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   if ((rc = st_reserve(c, S, n))) return rc;
   cudaStream_t st = S.stream;
   const bool json = flags & TGI_TURN_PAGE_JSON;
-  std::unique_ptr<DevBuf> keys;
+  std::shared_ptr<DevBuf> keys;
   if (S.turn_pool.empty()) {
-    keys = std::make_unique<DevBuf>();
+    keys = std::make_shared<DevBuf>();
   } else {
     keys = std::move(S.turn_pool.back());
     S.turn_pool.pop_back();
   }
   const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * n, 64));
-  CK(keys->ensure(n * 16));
+  CK(keys->ensure(n * 18));
   CK(S.turn_in.ensure(n * 16));
   CK(S.bfirst.ensure(bslots * 4));
   CK(S.flag.ensure(n * 4));
@@ -4184,16 +4304,16 @@ int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   CK(cudaStreamSynchronize(st));
   const uint64_t n_new = hs[0];
   // 2. UpdatePage(*owner): the old list becomes tombstones; the row takes the page's fields and joins the layer of its
-  // depth if that layer exists and does not hold it (base.go:131-146)
+  // depth if that layer exists and does not hold it (base.go:131-146).  The new list is the row's owner view, its
+  // statuses "resample" (0) until the end's hits.
   S.n_dead += hs[1];
   S.gen[row]++;
-  if (page) st_put_row(S, row, *page, strs);
-  const auto lit = S.layers.find(S.rows[row].depth);
-  if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), row) == lit->second.end()) lit->second.push_back(row);
-  const std::vector<uint32_t> dirty(1, row);
-  if ((rc = st_sync_rows(c, S, dirty))) return rc;
+  if ((rc = st_page_fields(c, S, row, page, strs, true))) return rc;
+  st_drop_view(S, row);
+  S.views[row] = CrawlState::View{n_new, keys};
   const uint32_t cnt = (uint32_t)n_new;
   CK(cudaMemcpyAsync(S.row_cnt.as<uint32_t>() + row, &cnt, 4, cudaMemcpyHostToDevice, st));
+  if (n_new) CK(cudaMemsetAsync(keys->as<uint8_t>() + 16 * n_new, 0, 2 * n_new, st));
   const StDev d = st_dev(S);
   CK(cudaEventRecord(S.t2, st));
   if (n_new) {
@@ -4207,41 +4327,7 @@ int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
   if (json) {
     zg.lock();
-    CK(S.entries.ensure(sizeof(StEntry)));
-    CK(S.row_base.ensure((S.rows.size() + 1) * 8));
-    CK(S.msize.ensure(n_new * 4));
-    CK(S.moff.ensure((n_new + 1) * 8));
-    CK(S.e32.ensure(4 * 4));
-    CK(S.e64.ensure(2 * 2 * 8));
-    r.entries = S.entries.as<StEntry>();
-    r.n_entries = 1;
-    r.zone = c->cfgdev.zone;
-    r.zone_n = c->cfgdev.zone_n;
-    r.tz = c->cfgdev.tz;
-    r.sc = S.sc.as<uint64_t>();
-    r.row_base = S.row_base.as<uint64_t>();  // only row_base[row] = 0 is read
-    r.msize = S.msize.as<uint32_t>();
-    r.moff = S.moff.as<uint64_t>();
-    r.esize_lo = S.e32.as<uint32_t>();
-    r.ebytes = r.esize_lo + 1;
-    r.ecnt = r.ebytes + 1;
-    r.esz = r.ecnt + 1;
-    r.eoff = S.e64.as<uint64_t>();
-    r.eslot = r.eoff + 2;
-    const StEntry e{(long long)S.rows[row].depth, row, 0};
-    CK(cudaMemcpyAsync(S.entries.p, &e, sizeof e, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(r.row_base + row, 0, 8, st));
-    CK(cudaMemsetAsync(r.moff, 0, 8, st));
-    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-    if (n_new) {
-      st_msg_size_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, r, t.sorted, t.rows, n_new);
-      launches++;
-      if ((rc = launch_scan(c, st, S.tiles, r.msize, n_new, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
-    }
-    st_line_size_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, r.esz, 1, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
-    if ((rc = launch_scan(c, st, S.tiles, r.ecnt, 1, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+    if ((rc = st_page_json_size(c, S, row, t.sorted, t.rows, n_new, r, launches))) return rc;
     CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaGetLastError());
@@ -4251,35 +4337,10 @@ int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   float ms0 = 0, ms1 = 0, ms2 = 0;
   cudaEventElapsedTime(&ms0, S.t0, S.t1);
   cudaEventElapsedTime(&ms1, S.t2, S.t3);
-  if (json) {
-    // Dapr's UpdatePage has changed pageMap before json.Marshal fails (daprstate.go:1378-1387): the new list stays, no
-    // turn opens, as the reference returns before its loop
-    if (hs[ST_SC_ERR]) {
-      rc = st_compact(c, S);
-      if (!rc) set_err(c, "tgi_state_page_begin: the page's timestamp year is outside [0, 9999] (json.Marshal fails)");
-      return rc ? rc : TGI_E_ARG;
-    }
-    if (hs[ST_SC_BIG]) {
-      rc = st_compact(c, S);
-      if (!rc) set_err(c, "tgi_state_page_begin: the page renders to 4 GiB or more");
-      return rc ? rc : TGI_E_CAPACITY;
-    }
-    const uint64_t body = hs[ST_SC_BYTES];
-    CK(S.out.ensure(body));
-    CK(S.h_out.ensure(body));
-    r.out = S.out.as<uint8_t>();
-    CK(cudaEventRecord(S.t4, st));
-    st_line_emit_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
-    if (n_new) st_msg_emit_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, r, t.sorted);
-    launches += 1 + (n_new != 0);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(S.t5, st));
-    CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    cudaEventElapsedTime(&ms2, S.t4, S.t5);
-    out->page_json = S.h_out.as<uint8_t>();
-    out->page_json_len = body - 1;  // the line without its '\n'
-  }
+  // a page that does not marshal: the new list and its view stay, no turn opens, as the reference returns before its loop
+  if (json && (rc = st_page_json_emit(c, S, r, t.sorted, n_new, hs, "tgi_state_page_begin", &out->page_json,
+                                      &out->page_json_len, &ms2, launches)))
+    return rc;
   if ((rc = st_compact(c, S))) return rc;
   const uint32_t h = S.next_turn++;
   if (!S.next_turn) S.next_turn = 1;
@@ -4341,10 +4402,145 @@ int tgi_state_page_end(tgi_ctx* c, uint32_t turn, int slot, const uint8_t* statu
                                                                       S.upd.as<tgi_state_update>());
     CK(cudaGetLastError());
     if ((rc = st_apply_updates(c, S, n_done))) return rc;
+    // the owner's side of the updates, while this turn's keys are still the row's owner view
+    const auto vit = S.views.find(T.row);
+    if (vit != S.views.end() && vit->second.keys == T.keys && T.n_work) {
+      const uint64_t k = T.n_work, vslots = next_pow2(std::max<uint64_t>(2 * k, 64));
+      CK(S.bfirst.ensure(vslots * 4));
+      CK(S.blast.ensure((k + 1) * 4));
+      StView v{};
+      v.keys = T.keys->as<long long>();
+      v.status = (uint16_t*)(T.keys->as<uint8_t>() + 16 * k);
+      v.k = k;
+      v.vfirst = S.bfirst.as<uint32_t>();
+      v.vmask = vslots - 1;
+      v.last = S.blast.as<uint32_t>();
+      CK(cudaMemsetAsync(v.vfirst, 0xFF, vslots * 4, st));
+      CK(cudaMemsetAsync(v.last, 0, k * 4, st));
+      CK(cudaMemsetAsync(v.last + k, 0xFF, 4, st));
+      const tgi_state_update* u = S.upd.as<tgi_state_update>();
+      st_view_build_kernel<<<st_grid(c, std::max(k, n_done)), ST_THREADS, 0, st>>>(v, S.flag.as<uint32_t>(), n_done);
+      st_view_hit_kernel<<<st_grid(c, n_done), ST_THREADS, 0, st>>>(v, u, n_done);
+      st_view_status_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(v, u);
+      CK(cudaGetLastError());
+    }
   }
   if (appended) *appended = S.n_msgs - before;
-  S.turn_pool.push_back(std::move(T.keys));
+  st_release(S, T.keys);
   S.turns.erase(it);
+  return TGI_OK;
+}
+
+// UpdatePage(*owner) for a page whose list came from a page turn (crawl/runner.go:1543-1544, dapr/standalone.go:589-609):
+// the page's fields replace the row's; with an owner view the row's list becomes the view, appended as its next
+// generation by one kernel.  The row upload synchronises, as every row rewrite does; beyond it the call waits only for
+// the page's read-back (TGI_TURN_PAGE_JSON; without a view, also the row's count) or, given out, for its kernels' time.
+int tgi_state_page_close(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         uint32_t flags, tgi_state_json_t* out) {
+  static const char* const who = "tgi_state_page_close";
+  if (!c || !page || (!out && (flags & TGI_TURN_PAGE_JSON))) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if (out) memset(out, 0, sizeof *out);
+  if (flags & ~TGI_TURN_PAGE_JSON) { set_err(c, "%s: unknown flags 0x%x", who, flags); return TGI_E_ARG; }
+  if (row >= S.rows.size()) { set_err(c, "%s: no row %u", who, row); return TGI_E_ARG; }
+  if (!page_ok(c, *page, strs, strs_len, who)) return TGI_E_ARG;
+  if (page->n_msgs) { set_err(c, "%s: the page carries messages (its list is the owner view)", who); return TGI_E_ARG; }
+  if (in_field(*page, strs, TGI_PS_ID) != st_field(S, S.rows[row], TGI_PS_ID)) { set_err(c, "%s: the page's id is not row %u's", who, row); return TGI_E_ARG; }
+  const bool json = flags & TGI_TURN_PAGE_JSON;
+  if (json && (rc = st_upload_codes(c, S))) return rc;
+  const auto vit = S.views.find(row);
+  const bool view = vit != S.views.end();
+  const uint64_t k = view ? vit->second.k : 0;
+  if (view && (rc = st_reserve(c, S, k))) return rc;
+  cudaStream_t st = S.stream;
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.vals.ensure(k * 4));
+  CK(S.keys.ensure(k * 4));
+  // no UpdateMessage of the loop follows: the row's open turns end here
+  for (auto it = S.turns.begin(); it != S.turns.end();) {
+    if (it->second.row != row) {
+      ++it;
+      continue;
+    }
+    st_release(S, it->second.keys);
+    it = S.turns.erase(it);
+  }
+  uint64_t* hs = S.h_sc.as<uint64_t>();
+  hs[1] = 0;
+  uint32_t launches = 0;
+  if (view) {  // the old list's length, brought back by the row upload's synchronise
+    CK(cudaMemcpyAsync(hs + 1, S.row_cnt.as<uint32_t>() + row, 4, cudaMemcpyDeviceToHost, st));
+    S.gen[row]++;
+  }
+  if ((rc = st_page_fields(c, S, row, page, strs, view))) return rc;
+  const uint64_t n0 = S.n_msgs;
+  const uint32_t* sorted = S.vals.as<uint32_t>();
+  const uint32_t* rows = S.keys.as<uint32_t>();
+  uint64_t cnt = k;
+  CK(cudaEventRecord(S.t2, st));
+  if (view) {
+    S.n_dead += hs[1];
+    const StDev d = st_dev(S);
+    StView v{};
+    v.keys = vit->second.keys->as<long long>();
+    v.status = (uint16_t*)(vit->second.keys->as<uint8_t>() + 16 * k);
+    v.k = k;
+    if (k) {
+      st_view_append_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(d, v, row, S.gen[row], n0, S.vals.as<uint32_t>(), S.keys.as<uint32_t>());
+      st_table_insert_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(d, n0, n0 + k);
+      launches += 2;
+    }
+    S.n_msgs += k;
+  } else if (json) {  // no view: the row's list as it is, found by a scan of the message rows
+    uint32_t n = 0;
+    if ((rc = st_row_count(c, S, row, &n))) return rc;
+    cnt = n;
+    const uint64_t nm = S.n_msgs;
+    CK(S.flag.ensure(nm * 4));
+    CK(S.pos.ensure((nm + 1) * 8));
+    CK(S.vals.ensure(cnt * 4));
+    CK(S.keys.ensure(cnt * 4));
+    sorted = S.vals.as<uint32_t>();
+    rows = S.keys.as<uint32_t>();
+    StRender r{};
+    r.flag = S.flag.as<uint32_t>();
+    r.pos = S.pos.as<uint64_t>();
+    r.keys[0] = S.keys.as<uint32_t>();
+    r.vals[0] = S.vals.as<uint32_t>();
+    const StDev d = st_dev(S);
+    st_live_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, row, r.flag);
+    if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, S.sc.as<uint64_t>(), launches))) return rc;
+    st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+    launches += 2;
+  }
+  float ms1 = 0, ms2 = 0;
+  StRender r{};
+  std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
+  if (json) {
+    zg.lock();
+    if ((rc = st_page_json_size(c, S, row, sorted, rows, cnt, r, launches))) return rc;
+    CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  if (json) {
+    CK(cudaStreamSynchronize(st));
+    cudaEventElapsedTime(&ms1, S.t2, S.t3);
+    if ((rc = st_page_json_emit(c, S, r, sorted, cnt, hs, who, &out->data, &out->len, &ms2, launches))) return rc;
+  }
+  if ((rc = st_compact(c, S))) return rc;
+  if (out) {
+    if (!json) {
+      CK(cudaEventSynchronize(S.t3));
+      cudaEventElapsedTime(&ms1, S.t2, S.t3);
+    }
+    out->kernel_ms = ms1 + ms2;
+    out->gpu_launches = launches;
+  }
   return TGI_OK;
 }
 

@@ -39,7 +39,7 @@ EXPORTED_SYMBOLS = [
     "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
-    "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer",
+    "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer",
 ]
 
 
@@ -119,6 +119,7 @@ def lib() -> C.CDLL:
         L.tgi_state_export.argtypes = [vp, i32, u64, C.POINTER(abi.StateExportC)]
         L.tgi_state_page_begin.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, C.POINTER(abi.StateTurnC)]
         L.tgi_state_page_end.argtypes = [vp, u32, i32, vp, u64, C.POINTER(u64)]
+        L.tgi_state_page_close.argtypes = [vp, u32, vp, vp, u64, u32, C.POINTER(abi.StateJsonC)]
         L.tgi_state_id_seed.argtypes = [vp, u64]
         L.tgi_state_discover.argtypes = [vp, i32, vp, u32, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         L.tgi_state_next_layer.argtypes = [vp, C.c_int64, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
@@ -700,6 +701,21 @@ class Engine:
         self._check(lib().tgi_state_page_end(self.h, turn, slot, st.ctypes.data if st is not None and len(st) else None,
                                              n_done, C.byref(appended)))
         return appended.value
+
+    def state_page_close(self, row: int, page, page_json: bool = False):
+        """UpdatePage(*owner) after a turn: page = a state_pack dict without messages whose fields replace the row's;
+        the row's list becomes its owner view (the last begin's owner messages with the end's hits) while it holds one.
+        Returns json.Marshal(page) when asked for, else None.  The device time is left in self.state_close_ms"""
+        from .state_pack import pack_pages
+        if page.get("messages"):
+            raise ValueError("the page's message list is the owner view")
+        recs, strs, _ = pack_pages([page], self.state_code, lambda pid, i: i)
+        out = abi.StateJsonC()
+        self._check(lib().tgi_state_page_close(self.h, row, recs.ctypes.data, strs.ctypes.data, len(strs),
+                                               abi.TURN_PAGE_JSON if page_json else 0, C.byref(out)))
+        self.state_close_ms = float(out.kernel_ms)
+        self.state_close_launches = int(out.gpu_launches)
+        return C.string_at(out.data, out.len) if page_json else None
 
     # --- snowball discovery: outlinks of processed pages as next-layer pages ---------------------------------------
     def state_id_seed(self, seed: int):

@@ -355,6 +355,16 @@ class MessageProcessor {
     if (tgi_state_page_end(ctx_, turn, slot, nullptr, n_done, &appended) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
     return appended;
   }
+  // UpdatePage(*owner) after the loop, and the Dapr runner's UpdatePage(page) after it: page's fields replace the
+  // row's, and the row's list becomes the last begin's owner view while it holds one.  With page_json the view of
+  // json.Marshal(page) stays valid until the next state call; else it is empty.
+  std::string_view StatePageClose(uint32_t row, const tgi_state_page& page, std::string_view strs, bool page_json) {
+    tgi_state_json_t o{};
+    if (tgi_state_page_close(ctx_, row, &page, (const uint8_t*)strs.data(), strs.size(), page_json ? TGI_TURN_PAGE_JSON : 0u,
+                             &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return page_json ? std::string_view((const char*)o.data, o.len) : std::string_view();
+  }
   // Snowball discovery: the outlinks of the slot's Telegram result as next-layer pages.  StateDiscover with
   // TGI_DISCOVER_NOW is the standalone runner's AddLayer per page; without it the candidates wait in the pending list
   // for StateNextLayer, the Dapr runner's layer end.  The returned arrays stay valid until the next state call.

@@ -909,6 +909,34 @@ int tgi_state_page_begin(tgi_ctx* ctx, uint32_t row, const tgi_state_page* page,
                          const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out);
 int tgi_state_page_end(tgi_ctx* ctx, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended);
 
+/* Page close — UpdatePage(*owner) at the end of the loop (crawl/runner.go:1543-1544, owner.Status = "fetched") and the
+ * Dapr runner's UpdatePage(page) after it (dapr/standalone.go:589-609, "fetched", or "error" with Error set).
+ *   Fields   page (required, no messages, its id the row's) replaces the row's fields exactly as
+ *            tgi_state_update_page does, the timestamp included; the row joins the layer of its depth if that layer
+ *            exists and does not hold it.
+ *   Owner    tgi_state_page_begin leaves the row an owner view: the turn's n_work owner messages in fetch order with
+ *            their keys, "resample", pageId = the page, no platform.  The view lives until the row's next begin, a
+ *            tgi_state_update_page of the row, a tgi_state_add_layer / tgi_state_add_pages / discovery that overwrites
+ *            the row, or tgi_state_set.  With a view the close makes the row's list exactly the view: the swapped-key
+ *            messages the end appended, and anything else appended since the begin, are dropped (Go's owner slice
+ *            still has its begin-time length).  Without one the list stays as it is and only the fields change.  A
+ *            second close of the same view gives the same list.  The close ends every open turn of the row: a later
+ *            tgi_state_page_end of it is TGI_E_ARG.
+ *   Hits     parity unpinned: Go's owner shares its backing array with pageMap's page until an append reallocates
+ *            it, which depends on cap(owner.Messages) (growslice and malloc size classes).  The library counts the
+ *            array as full: an UpdateMessage of tgi_state_page_end that hits an owner message BEFORE the end's first
+ *            append gives that status to the first owner message with the key (the last such hit wins); later hits
+ *            do not reach the owner.  With Telegram's keys this never happens: the swapped key has a positive chat id
+ *            and a channel's chat ids are negative.
+ *   JSON     TGI_TURN_PAGE_JSON: out->data / len = json.Marshal(page) after the close (Dapr's UpdatePage value), as
+ *            tgi_state_page_begin renders it; a timestamp whose year leaves [0, 9999] is then TGI_E_ARG AFTER the
+ *            update.  out may be NULL without the flag; else it gets kernel_ms / gpu_launches and the bytes live until
+ *            the next state call.
+ *   Errors   TGI_E_ARG, the state unchanged: no such row, an id that is not the row's, messages in page, unknown
+ *            flags, strings outside strs.                                                                            */
+int tgi_state_page_close(tgi_ctx* ctx, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         uint32_t flags, tgi_state_json_t* out);
+
 /* Snowball discovery — the outlinks of processed pages become the next layer's pages (crawl/runner.go:1199-1244 outside
  * random-walk, then standalone/runner.go:835-850 or dapr/standalone.go:612-616, 645-688), read straight from a slot's
  * resident Telegram result: nothing is read back before the dedup, so it works after TGI_RUN_JSONL_DEVICE and
