@@ -203,7 +203,17 @@ class StateTurnC(C.Structure):  # tgi_state_turn_t
                 ("gpu_launches", C.c_uint32)]
 
 
-DISCOVER_NOW = 1        # tgi_state_discover: AddLayer per span now (else the candidates go to the pending list)
+class StatePagesC(C.Structure):  # tgi_state_pages_t
+    _fields_ = [("turn", C.c_uint32), ("n_pages", C.c_uint32), ("n_work", C.c_uint64), ("work", C.POINTER(C.c_uint32)),
+                ("work_off", C.POINTER(C.c_uint64)), ("page_json", C.c_void_p), ("json_off", C.POINTER(C.c_uint64)),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
+class StateEndC(C.Structure):  # tgi_state_end_t
+    _fields_ = [("appended", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
+DISCOVER_NOW = 1       # tgi_state_discover: AddLayer per span now (else the candidates go to the pending list)
 DISCOVER_DAPR = 2       # DaprStateManager.AddLayer's rules instead of BaseStateManager's
 DISCOVER_PAGE_JSON = 4  # json.Marshal of every added page (Dapr's per-page SaveState value)
 STATE_SPAN = np.dtype([("row", "<u4"), ("reserved", "<u4"), ("first", "<u8"), ("n_records", "<u8"), ("n_done", "<u8")])

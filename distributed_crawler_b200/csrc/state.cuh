@@ -156,32 +156,54 @@ __global__ void st_upd_append_kernel(StDev d, StUpd w) {
 }
 
 // ---- page turns: processAllMessagesWithProcessor's bookkeeping (crawl/runner.go:1132-1147, 1161-1211) ---------------
+// A call covers P pages (distinct rows); page k owns the segment [off[k], off[k+1]) of each of the call's arrays.
+
+// the segment of item i: the last k with off[k] <= i (empty segments share their offset, so this one holds i)
+DEVI uint32_t st_seg(const uint64_t* off, uint32_t n_seg, uint64_t i) {
+  uint32_t lo = 0, hi = n_seg - 1;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= i) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
 struct StTurn {
-  const long long* fetched;  // [n][2] chat_id, message_id in fetch order
+  const long long* fetched;  // [n][2] chat_id, message_id in fetch order, page after page
   uint64_t n;
-  uint32_t row, gen;  // the page, and the generation its new list takes
-  uint32_t* bfirst;   // batch table keyed by message id: lowest fetched index, ST_NONE = empty
+  const uint64_t* foff;      // [P+1] page k's fetched keys
+  const uint32_t* prow;      // [P] page k's row
+  uint32_t P;
+  uint32_t* pg;       // [n] the page of fetched key j
+  uint32_t* bfirst;   // batch table keyed by (page, message id): lowest fetched index, ST_NONE = empty
   uint64_t bmask;
-  uint32_t* flag;     // [n] 1: fetched key j is not in the page's list (addNewMessages keeps it)
-  uint64_t* pos;      // [n+1] scan of flag
-  uint64_t n_msgs;    // message rows before the new list
-  long long* keys;    // [n_new][2] the new list's keys: the turn's owner messages
+  uint32_t* flag;     // [n] 1: fetched key j is not in its page's list (addNewMessages keeps it)
+  uint64_t* pos;      // [n+1] scan of flag: the call's new lists, in (page, fetch) order
+  uint64_t* woff;     // [P+1] page k's new list is [woff[k], woff[k+1]) of it
+  uint64_t n_msgs;    // message rows before the new lists
+  long long* keys;    // [n_new][2] the new lists' keys: the turn's owner messages
   uint32_t* work;     // [n_new] fetched index of each owner message's discMessage
-  uint32_t* sorted;   // [n_new] message index of each owner message (the one-page render's grouped order)
+  uint32_t* sorted;   // [n_new] message index of each owner message (the render's grouped order)
   uint32_t* rows;     // [n_new] its row
 };
 
-DEVI uint64_t st_turn_slot(const StTurn& t, long long msg) { return st_hash(0, 0, 0, msg) & t.bmask; }
+DEVI uint64_t st_turn_slot(const StTurn& t, uint32_t k, long long msg) { return st_hash(k, 0, 0, msg) & t.bmask; }
+DEVI bool st_turn_same(const StTurn& t, uint32_t k, uint32_t cur, long long msg) {
+  return cur >= t.foff[k] && cur < t.foff[k + 1] && t.fetched[2 * cur + 1] == msg;
+}
 
-// 1. addNewMessages' test against the page's current list, and the first fetched index of every message id
+// 1. addNewMessages' test against the page's current list, and the first fetched index of every message id of a page
 __global__ void st_turn_probe_kernel(StDev d, StTurn t) {
   for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < t.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t k = st_seg(t.foff, t.P, j), row = t.prow[k];
     const long long chat = t.fetched[2 * j], msg = t.fetched[2 * j + 1];
-    t.flag[j] = st_lookup(d, t.row, d.row_gen[t.row], chat, msg) == ST_NONE;
-    for (uint64_t s = st_turn_slot(t, msg);; s = (s + 1) & t.bmask) {
+    t.pg[j] = k;
+    t.flag[j] = st_lookup(d, row, d.row_gen[row], chat, msg) == ST_NONE;
+    for (uint64_t s = st_turn_slot(t, k, msg);; s = (s + 1) & t.bmask) {
       const uint32_t cur = atomicCAS(t.bfirst + s, ST_NONE, (uint32_t)j);
       if (cur == ST_NONE) break;
-      if (t.fetched[2 * cur + 1] == msg) {
+      if (st_turn_same(t, k, cur, msg)) {
         atomicMin(t.bfirst + s, (uint32_t)j);
         break;
       }
@@ -189,74 +211,124 @@ __global__ void st_turn_probe_kernel(StDev d, StTurn t) {
   }
 }
 
-// 2. the new list in fetch order, appended as the row's live messages: status "resample", no platform, pageId = the
-// page; each owner message's discMessage is the first fetched message with its message id (the chat id is ignored)
+// every page's new list in the call's list (woff, nullptr pos: all empty), and every row's message count before the
+// call (old, optional)
+__global__ void st_turn_meta_kernel(const uint32_t* row_cnt, const uint32_t* prow, uint32_t P, const uint64_t* foff,
+                                    const uint64_t* pos, uint64_t* woff, uint32_t* old) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k <= P; k += (uint64_t)gridDim.x * blockDim.x) {
+    if (woff) woff[k] = pos ? pos[foff[k]] : 0;
+    if (k < P && old) old[k] = row_cnt[prow[k]];
+  }
+}
+
+// 2. the new lists in fetch order, appended as their rows' live messages of the generation the rows now hold: status
+// "resample", no platform, pageId = the page; each owner message's discMessage is the first fetched message of its page
+// with its message id (the chat id is ignored)
 __global__ void st_turn_append_kernel(StDev d, StTurn t) {
   for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < t.n; j += (uint64_t)gridDim.x * blockDim.x) {
     if (!t.flag[j]) continue;
     const uint64_t p = t.pos[j];
+    const uint32_t k = t.pg[j], row = t.prow[k];
     const long long chat = t.fetched[2 * j], msg = t.fetched[2 * j + 1];
-    uint64_t s = st_turn_slot(t, msg);
-    while (t.fetched[2 * t.bfirst[s] + 1] != msg) s = (s + 1) & t.bmask;
+    uint64_t s = st_turn_slot(t, k, msg);
+    while (!st_turn_same(t, k, t.bfirst[s], msg)) s = (s + 1) & t.bmask;
     t.work[p] = t.bfirst[s];
     t.keys[2 * p] = chat;
     t.keys[2 * p + 1] = msg;
     StMsg m;
     m.chat = chat;
     m.msg = msg;
-    m.row = t.row;
-    m.gen = t.gen;
-    m.pid = t.row;
+    m.row = row;
+    m.gen = d.row_gen[row];
+    m.pid = row;
     m.status = 5;  // "resample"
     m.platform = 0;
     d.msgs[t.n_msgs + p] = m;
     t.sorted[p] = (uint32_t)(t.n_msgs + p);
-    t.rows[p] = t.row;
+    t.rows[p] = row;
   }
 }
 
-// the loop's UpdateMessage calls: owner message j updates the key (message id, chat id), swapped as the reference passes
-// them, with "failed" for a record that failed and "fetched" otherwise
-__global__ void st_turn_updates_kernel(const long long* keys, const uint8_t* status, uint64_t n, uint32_t row,
-                                       tgi_state_update* u) {
-  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+// a row's new fields in one upload: the page row, and with a new list its generation and count; base (ST_NO_BASE: left)
+// is its first message in the render's grouped order
+constexpr uint64_t ST_NO_BASE = ~0ull;
+struct StRowPut {
+  tgi_state_page page;
+  uint32_t row, gen, cnt, list;
+  uint64_t base;
+};
+__global__ void st_rows_put_kernel(tgi_state_page* pages, uint32_t* row_gen, uint32_t* row_cnt, const StRowPut* in, uint32_t P,
+                                   uint64_t* row_base) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < P; k += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t r = in[k].row;
+    pages[r] = in[k].page;
+    if (in[k].list) {
+      row_gen[r] = in[k].gen;
+      row_cnt[r] = in[k].cnt;
+    }
+    if (in[k].base != ST_NO_BASE) row_base[r] = in[k].base;
+  }
+}
+
+// the loop's UpdateMessage calls of every page: update q is owner message woff[k] + (q - uoff[k]) of page k, whose first
+// n_done[k] records were processed; it updates the key (message id, chat id), swapped as the reference passes them, with
+// "failed" for a record that failed and "fetched" otherwise (status: the turn's records, owner message j at status[j])
+struct StEnd {
+  const long long* keys;  // [n_work][2] the turn's owner keys
+  const uint8_t* status;
+  const uint32_t* prow;   // [P]
+  const uint64_t* woff;   // [P+1] page k's owner messages
+  const uint64_t* uoff;   // [P+1] page k's updates (scan of n_done)
+  const uint32_t* live;   // [P] 1: page k's row still holds this turn's owner view
+  uint32_t P;
+};
+__global__ void st_turn_updates_kernel(StEnd e, uint64_t m, tgi_state_update* u) {
+  for (uint64_t q = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; q < m; q += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t k = st_seg(e.uoff, e.P, q);
+    const uint64_t j = e.woff[k] + (q - e.uoff[k]);
     tgi_state_update v;
-    v.chat_id = keys[2 * j + 1];
-    v.message_id = keys[2 * j];
-    v.row = row;
-    v.status = status[j] == TGI_ST_FAILED ? 3 : 2;  // "failed" : "fetched"
+    v.chat_id = e.keys[2 * j + 1];
+    v.message_id = e.keys[2 * j];
+    v.row = e.prow[k];
+    v.status = e.status[j] == TGI_ST_FAILED ? 3 : 2;  // "failed" : "fetched"
     v.reserved = 0;
-    u[j] = v;
+    u[q] = v;
   }
 }
 
 // ---- page close: UpdatePage(*owner) (crawl/runner.go:1543-1544) over the row's owner view ---------------------------
-// The view is the turn's k owner messages: their keys and a status code each, 0 while no hit of the end reached the
-// owner (the message is still "resample").  Go's owner shares its backing array with pageMap's page until an append
-// reallocates it; the array counts as full, so an UpdateMessage of the end reaches the owner only before the end's first
-// append, and then the first owner message with the key takes the status.
+// The view is the turn's owner messages of the row: their keys and a status code each, 0 while no hit of the end
+// reached the owner (the message is still "resample").  Go's owner shares its backing array with pageMap's page until an
+// append reallocates it; the array counts as full, so an UpdateMessage of the end reaches the owner only before the
+// end's first append to that page, and then the first owner message of the page with the key takes the status.
 struct StView {
-  const long long* keys;  // [k][2] chat_id, message_id of owner message p
-  uint16_t* status;       // [k]
-  uint64_t k;
-  uint32_t* vfirst;       // batch table keyed by the owner's keys: lowest owner index, ST_NONE = empty
+  StEnd e;                // the turn's pages, their owner messages and updates
+  uint16_t* status;       // [k] the owner messages' statuses
+  uint64_t k;             // owner messages of the turn
+  uint32_t* vfirst;       // batch table keyed by (page, owner key): lowest owner index, ST_NONE = empty
   uint64_t vmask;
-  uint32_t* last;         // [k] 1 + the last update that reached owner message p (0: none); [k]: the end's first append
+  uint32_t* last;         // [k] 1 + the last update that reached owner message p (0: none)
+  uint32_t* app;          // [P] the first update of page k that appended (ST_NONE: none)
 };
 
-DEVI uint64_t st_view_slot(const StView& v, long long chat, long long msg) { return st_hash(0, 0, chat, msg) & v.vmask; }
+DEVI uint64_t st_view_slot(const StView& v, uint32_t pg, long long chat, long long msg) {
+  return st_hash(pg, 0, chat, msg) & v.vmask;
+}
 
-// 1. the owner's keys by first owner index, and the first update of the end that appended (the lowest flagged leader)
+// 1. the owner keys of the pages whose view is the turn's, by first owner index, and each page's first update that
+// appended (the lowest flagged leader of its segment)
 __global__ void st_view_build_kernel(StView v, const uint32_t* flag, uint64_t n) {
   const uint64_t m = v.k > n ? v.k : n;
   for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < m; j += (uint64_t)gridDim.x * blockDim.x) {
-    if (j < n && flag[j]) atomicMin(v.last + v.k, (uint32_t)j);
+    if (j < n && flag[j]) atomicMin(v.app + st_seg(v.e.uoff, v.e.P, j), (uint32_t)j);
     if (j >= v.k) continue;
-    const long long chat = v.keys[2 * j], msg = v.keys[2 * j + 1];
-    for (uint64_t s = st_view_slot(v, chat, msg);; s = (s + 1) & v.vmask) {
+    const uint32_t pg = st_seg(v.e.woff, v.e.P, j);
+    if (!v.e.live[pg]) continue;
+    const long long chat = v.e.keys[2 * j], msg = v.e.keys[2 * j + 1];
+    for (uint64_t s = st_view_slot(v, pg, chat, msg);; s = (s + 1) & v.vmask) {
       const uint32_t cur = atomicCAS(v.vfirst + s, ST_NONE, (uint32_t)j);
       if (cur == ST_NONE) break;
-      if (v.keys[2 * cur] == chat && v.keys[2 * cur + 1] == msg) {
+      if (cur >= v.e.woff[pg] && cur < v.e.woff[pg + 1] && v.e.keys[2 * cur] == chat && v.e.keys[2 * cur + 1] == msg) {
         atomicMin(v.vfirst + s, (uint32_t)j);
         break;
       }
@@ -264,15 +336,17 @@ __global__ void st_view_build_kernel(StView v, const uint32_t* flag, uint64_t n)
   }
 }
 
-// 2. every update before the first append whose key is an owner key reaches that key's first owner message
+// 2. every update before its page's first append whose key is an owner key of the page reaches that key's first owner
+// message
 __global__ void st_view_hit_kernel(StView v, const tgi_state_update* u, uint64_t n) {
-  const uint32_t a = v.last[v.k];
-  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n && j < a; j += (uint64_t)gridDim.x * blockDim.x) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t pg = st_seg(v.e.uoff, v.e.P, j);
+    if (j >= v.app[pg] || !v.e.live[pg]) continue;
     const long long chat = u[j].chat_id, msg = u[j].message_id;
-    for (uint64_t s = st_view_slot(v, chat, msg);; s = (s + 1) & v.vmask) {
+    for (uint64_t s = st_view_slot(v, pg, chat, msg);; s = (s + 1) & v.vmask) {
       const uint32_t cur = v.vfirst[s];
       if (cur == ST_NONE) break;
-      if (v.keys[2 * cur] == chat && v.keys[2 * cur + 1] == msg) {
+      if (cur >= v.e.woff[pg] && cur < v.e.woff[pg + 1] && v.e.keys[2 * cur] == chat && v.e.keys[2 * cur + 1] == msg) {
         atomicMax(v.last + cur, (uint32_t)j + 1);
         break;
       }
@@ -286,24 +360,60 @@ __global__ void st_view_status_kernel(StView v, const tgi_state_update* u) {
     if (v.last[p]) v.status[p] = u[v.last[p] - 1].status;
 }
 
-// the close: the view's messages appended as the row's live list of generation gen, at n0 (pageId = the page, no
-// platform), and the row's count; sorted / rows are the one-page render's grouped order
-__global__ void st_view_append_kernel(StDev d, StView v, uint32_t row, uint32_t gen, uint64_t n0, uint32_t* sorted,
+// one owner view of a close: its messages are [off, next off) of the close's appended list
+struct StViewSeg {
+  const long long* keys;   // [k][2]
+  const uint16_t* status;  // [k]
+  uint64_t off;
+  uint32_t row, reserved;
+};
+
+// the close: every view's messages appended at n0 as its row's live list of the generation the row now holds (pageId =
+// the page, no platform); sorted / rows are the render's grouped order
+__global__ void st_view_append_kernel(StDev d, const StViewSeg* seg, uint32_t Q, uint64_t K, uint64_t n0, uint32_t* sorted,
                                       uint32_t* rows) {
-  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < v.k; p += (uint64_t)gridDim.x * blockDim.x) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < K; p += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = Q - 1;  // the last view with off <= p
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi + 1) >> 1;
+      if (seg[mid].off <= p) lo = mid;
+      else hi = mid - 1;
+    }
+    const StViewSeg& v = seg[lo];
+    const uint64_t i = p - v.off;
     StMsg m;
-    m.chat = v.keys[2 * p];
-    m.msg = v.keys[2 * p + 1];
-    m.row = row;
-    m.gen = gen;
-    m.pid = row;
-    m.status = v.status[p] ? v.status[p] : 5;  // "resample"
+    m.chat = v.keys[2 * i];
+    m.msg = v.keys[2 * i + 1];
+    m.row = v.row;
+    m.gen = d.row_gen[v.row];
+    m.pid = v.row;
+    m.status = v.status[i] ? v.status[i] : 5;  // "resample"
     m.platform = 0;
     d.msgs[n0 + p] = m;
     sorted[p] = (uint32_t)(n0 + p);
-    rows[p] = row;
-    if (p == 0) d.row_cnt[row] = (uint32_t)v.k;
+    rows[p] = v.row;
   }
+}
+
+// flag[i] = message i is a live message of one of the rows in set (ascending, n_set > 0)
+__global__ void st_rows_flag_kernel(StDev d, uint64_t n, const uint32_t* set, uint32_t n_set, uint32_t* flag) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const StMsg m = d.msgs[i];
+    uint32_t lo = 0, hi = n_set - 1;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (set[mid] < m.row) lo = mid + 1;
+      else hi = mid;
+    }
+    flag[i] = set[lo] == m.row && st_live(d, m);
+  }
+}
+
+// the first grouped message of every row in rows[0, n) (grouped by row), at base + its position
+__global__ void st_row_starts_kernel(const uint32_t* rows, const uint64_t* n, uint64_t base, uint64_t* row_base) {
+  const uint64_t m = *n;
+  for (uint64_t q = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; q < m; q += (uint64_t)gridDim.x * blockDim.x)
+    if (q == 0 || rows[q - 1] != rows[q]) row_base[rows[q]] = base + q;
 }
 
 // ---- compaction / read-back -------------------------------------------------------------------------------------

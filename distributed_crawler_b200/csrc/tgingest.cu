@@ -212,25 +212,31 @@ struct CrawlState {
   DevBuf entries, keys, vals, row_base, msize, moff, e32, e64, counts, roff, out;
   DevBuf lm_keys, cb_tasks, cb_segs, b64;  // the layer map's openings; the export's encode tasks and output
   HostBuf h_out, h_sc, h_read, h_chunks;
-  // page turns (tgi_state_page_begin / _end / _close): each open turn's row and owner keys, by handle, and each row's
-  // owner view (tgi_state_page_close): the last begin's owner keys and their statuses, in the same buffer as that
-  // turn's keys.  A buffer neither a turn nor a view holds is kept for the next begins.
+  // page turns (tgi_state_pages_begin / _end / _close): each open turn's rows and owner keys, by handle, and each row's
+  // owner view (tgi_state_pages_close): the last begin's owner keys of the row and their statuses, a slice of the
+  // buffer of that begin's call.  A buffer neither a turn nor a view holds is kept for the next begins.
   struct Turn {
-    uint32_t row = 0;
-    uint64_t n_work = 0;
-    std::shared_ptr<DevBuf> keys;  // [n_work][2] chat_id, message_id, then the view's uint16 statuses [n_work]
+    std::vector<uint32_t> rows;    // [P] the pages
+    std::vector<uint64_t> off;     // [P+1] page k's owner messages are [off[k], off[k+1])
+    std::shared_ptr<DevBuf> keys;  // [n_work][2] chat_id, message_id, then the views' uint16 statuses [n_work]
+    uint64_t n_work() const { return off.back(); }
   };
   struct View {
-    uint64_t k = 0;
-    std::shared_ptr<DevBuf> keys;  // as Turn::keys
+    uint64_t off = 0, k = 0, total = 0;  // owner messages [off, off + k) of a buffer that holds `total`
+    std::shared_ptr<DevBuf> keys;        // as Turn::keys
+    const long long* key_ptr() const { return keys->as<long long>() + 2 * off; }
+    uint16_t* status_ptr() const { return (uint16_t*)(keys->as<uint8_t>() + 16 * total) + off; }
   };
   std::map<uint32_t, Turn> turns;
   std::unordered_map<uint32_t, View> views;  // by row
   std::vector<std::shared_ptr<DevBuf>> turn_pool;
   uint32_t next_turn = 1;
-  cudaEvent_t ev_slot = nullptr;  // tgi_state_page_end: the slot's work the state stream waits for
-  DevBuf turn_in;                 // the fetched keys of tgi_state_page_begin
-  HostBuf h_work;
+  cudaEvent_t ev_slot = nullptr;  // tgi_state_pages_end: the slot's work the state stream waits for
+  cudaEvent_t ev_seg = nullptr;   // the last upload from h_seg: a call that rewrites h_seg waits for it first
+  DevBuf turn_in;                 // the fetched keys of tgi_state_pages_begin
+  DevBuf seg, pg;                 // the pages' arrays of a turn call (rows, offsets, row puts, views); each key's page
+  HostBuf h_work, h_woff, h_seg, h_old;
+  std::vector<uint8_t> row_mark;  // st_join_layers' marks, a byte per row, all 0 between calls
   // snowball discovery (tgi_state_discover / _next_layer): the pending next-layer list (StCand, grown on demand), the
   // id generator's key and next counter, and the scratch of the candidates and survivors
   DevBuf pend, cand, surv, spans, cnt, soff, coff, lnk, spn, uuids, url_keys;
@@ -3306,6 +3312,7 @@ int st_init(tgi_ctx* c, CrawlState& S) {
   CK(cudaEventCreate(&S.t4));
   CK(cudaEventCreate(&S.t5));
   CK(cudaEventCreateWithFlags(&S.ev_slot, cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&S.ev_seg, cudaEventDisableTiming));
   for (const char* s : kPresetCodes) {
     S.code_of[s] = (uint16_t)S.codes.size();
     S.codes.push_back(s);
@@ -3503,72 +3510,60 @@ int st_drop_messages(tgi_ctx* c, CrawlState& S, uint32_t r) {
   return TGI_OK;
 }
 
-// UpdatePage's fields for a turn's row (base.go:123-149): page (optional) replaces the row's fields and the host maps
-// follow; the row joins the layer of its depth if that layer exists and does not hold it.  new_list: the row's
-// generation has moved on, and its count goes to 0 for the caller to set; otherwise the list stays as it is.
-int st_page_fields(tgi_ctx* c, CrawlState& S, uint32_t row, const tgi_state_page* page, const uint8_t* strs, bool new_list) {
-  if (page) st_put_row(S, row, *page, strs);
-  const auto lit = S.layers.find(S.rows[row].depth);
-  if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), row) == lit->second.end()) lit->second.push_back(row);
-  const std::vector<uint32_t> dirty(new_list ? 1 : 0, row);
-  const int rc = st_sync_rows(c, S, dirty);
-  if (rc) return rc;
-  if (!new_list) CK(cudaMemcpyAsync(S.pages.as<tgi_state_page>() + row, &S.rows[row], sizeof(tgi_state_page), cudaMemcpyHostToDevice, S.stream));
-  return TGI_OK;
-}
-
-// json.Marshal(page) of one row by the export's line passes: its cnt messages are sorted[0, cnt) (message indices in
-// list order; rows[] holds the row for each).  The size pass is enqueued into r (no synchronise); once the host has
-// S.sc in hs, st_page_json_emit writes the bytes and brings them back.
-int st_page_json_size(tgi_ctx* c, CrawlState& S, uint32_t row, const uint32_t* sorted, const uint32_t* rows, uint64_t cnt,
-                      StRender& r, uint32_t& launches) {
+// json.Marshal(page) of the P rows by the export's line passes: their cnt messages are sorted[0, cnt) (message indices
+// grouped by row, each row's in list order; srows[] holds the row of each), and the caller has set row_base[row] for
+// every listed row (its first grouped message; any value for a row without messages).  The size pass is enqueued into
+// r (no synchronise); once the host has S.sc in hs, st_page_json_emit writes the lines and brings them back.  tiled:
+// the scans take their multi-launch form whatever their length, so the launch count does not depend on P.
+int st_page_json_size(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, const uint32_t* sorted, const uint32_t* srows,
+                      uint64_t cnt, bool tiled, StRender& r, uint32_t& launches) {
   cudaStream_t st = S.stream;
   int rc;
-  CK(S.entries.ensure(sizeof(StEntry)));
-  CK(S.row_base.ensure((S.rows.size() + 1) * 8));
+  CK(S.entries.ensure(P * sizeof(StEntry)));
   CK(S.msize.ensure(cnt * 4));
   CK(S.moff.ensure((cnt + 1) * 8));
-  CK(S.e32.ensure(4 * 4));
-  CK(S.e64.ensure(2 * 2 * 8));
+  CK(S.e32.ensure(4 * P * 4));
+  CK(S.e64.ensure(2 * (P + 1) * 8));
   r.entries = S.entries.as<StEntry>();
-  r.n_entries = 1;
+  r.n_entries = P;
   r.zone = c->cfgdev.zone;
   r.zone_n = c->cfgdev.zone_n;
   r.tz = c->cfgdev.tz;
   r.sc = S.sc.as<uint64_t>();
-  r.row_base = S.row_base.as<uint64_t>();  // only row_base[row] = 0 is read
+  r.row_base = S.row_base.as<uint64_t>();
   r.msize = S.msize.as<uint32_t>();
   r.moff = S.moff.as<uint64_t>();
   r.esize_lo = S.e32.as<uint32_t>();
-  r.ebytes = r.esize_lo + 1;
-  r.ecnt = r.ebytes + 1;
-  r.esz = r.ecnt + 1;
+  r.ebytes = r.esize_lo + P;
+  r.ecnt = r.ebytes + P;
+  r.esz = r.ecnt + P;
   r.eoff = S.e64.as<uint64_t>();
-  r.eslot = r.eoff + 2;
+  r.eslot = r.eoff + P + 1;
   const StDev d = st_dev(S);
-  const StEntry e{(long long)S.rows[row].depth, row, 0};
-  CK(cudaMemcpyAsync(S.entries.p, &e, sizeof e, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(r.row_base + row, 0, 8, st));
+  std::vector<StEntry> E(P);
+  for (uint32_t k = 0; k < P; k++) E[k] = StEntry{(long long)S.rows[rows[k]].depth, rows[k], 0};
+  CK(cudaMemcpyAsync(S.entries.p, E.data(), P * sizeof(StEntry), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(r.moff, 0, 8, st));
   CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
   if (cnt) {
-    st_msg_size_kernel<<<st_grid(c, cnt), ST_THREADS, 0, st>>>(d, r, sorted, rows, cnt);
+    st_msg_size_kernel<<<st_grid(c, cnt), ST_THREADS, 0, st>>>(d, r, sorted, srows, cnt);
     launches++;
-    if ((rc = launch_scan(c, st, S.tiles, r.msize, cnt, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
+    if ((rc = launch_scan(c, st, S.tiles, r.msize, cnt, r.moff, r.sc + ST_SC_MBYTES, launches, tiled))) return rc;
   }
-  st_line_size_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+  st_line_size_kernel<<<sink_grid(c, P, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
   launches++;
-  if ((rc = launch_scan(c, st, S.tiles, r.esz, 1, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
-  if ((rc = launch_scan(c, st, S.tiles, r.ecnt, 1, r.eslot, r.sc + ST_SC_SLOTS, launches))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, r.esz, P, r.eoff, r.sc + ST_SC_BYTES, launches, tiled))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, r.ecnt, P, r.eslot, r.sc + ST_SC_SLOTS, launches, tiled))) return rc;
   CK(cudaGetLastError());
   return TGI_OK;
 }
 
-// the page's bytes after its size pass (hs = the size pass's S.sc).  Dapr's UpdatePage has changed pageMap before
-// json.Marshal fails (daprstate.go:1378-1387): a timestamp that does not render, or a page of 4 GiB or more, fails the
-// call after the update.
+// the pages' lines after their size pass (hs = the size pass's S.sc): *data holds json.Marshal(page) + '\n' of each,
+// page k's line being [(*json_off)[k], (*json_off)[k+1]).  Dapr's UpdatePage has changed pageMap before json.Marshal
+// fails (daprstate.go:1378-1387): a timestamp that does not render, or a page of 4 GiB or more, fails the call after the
+// update.
 int st_page_json_emit(tgi_ctx* c, CrawlState& S, StRender& r, const uint32_t* sorted, uint64_t cnt, const uint64_t* hs,
-                      const char* who, const uint8_t** data, uint64_t* len, float* ms, uint32_t& launches) {
+                      const char* who, const uint8_t** data, const uint64_t** json_off, float* ms, uint32_t& launches) {
   cudaStream_t st = S.stream;
   int rc;
   if (hs[ST_SC_ERR]) {
@@ -3581,22 +3576,24 @@ int st_page_json_emit(tgi_ctx* c, CrawlState& S, StRender& r, const uint32_t* so
     if (!rc) set_err(c, "%s: the page renders to 4 GiB or more", who);
     return rc ? rc : TGI_E_CAPACITY;
   }
-  const uint64_t body = hs[ST_SC_BYTES];
+  const uint64_t body = hs[ST_SC_BYTES], ne = r.n_entries;
   CK(S.out.ensure(body));
   CK(S.h_out.ensure(body));
+  CK(S.h_json_off.ensure((ne + 1) * 8));
   r.out = S.out.as<uint8_t>();
   const StDev d = st_dev(S);
   CK(cudaEventRecord(S.t4, st));
-  st_line_emit_kernel<<<1, ST_WARPS * 32, 0, st>>>(d, r);
+  st_line_emit_kernel<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
   if (cnt) st_msg_emit_kernel<<<st_grid(c, cnt), ST_THREADS, 0, st>>>(d, r, sorted);
   launches += 1 + (cnt != 0);
   CK(cudaGetLastError());
   CK(cudaEventRecord(S.t5, st));
   CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_json_off.p, r.eoff, (ne + 1) * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   cudaEventElapsedTime(ms, S.t4, S.t5);
   *data = S.h_out.as<uint8_t>();
-  *len = body - 1;  // the line without its '\n'
+  *json_off = S.h_json_off.as<uint64_t>();
   return TGI_OK;
 }
 
@@ -3700,8 +3697,9 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
 }
 
 // the m UpdateMessage calls in S.upd, in order (rows valid, st_reserve(m) done): the batch table, one probe per distinct
-// key, the new keys appended in first-occurrence order and entered in the table
-int st_apply_updates(tgi_ctx* c, CrawlState& S, uint64_t m) {
+// key, the new keys appended in first-occurrence order and entered in the table.  launches counts the kernels; tiled:
+// the scan takes its multi-launch form whatever m; ms (optional) gets the kernels' device time.
+int st_apply_updates(tgi_ctx* c, CrawlState& S, uint64_t m, uint32_t& launches, bool tiled = false, float* ms = nullptr) {
   cudaStream_t st = S.stream;
   int rc;
   const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * m, 64));
@@ -3725,18 +3723,33 @@ int st_apply_updates(tgi_ctx* c, CrawlState& S, uint64_t m) {
   w.pos = S.pos.as<uint64_t>();
   w.n_msgs = S.n_msgs;
   const StDev d = st_dev(S);
-  uint32_t launches = 0;
+  if (ms) CK(cudaEventRecord(S.t4, st));
   st_upd_build_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(w);
   st_upd_resolve_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
-  if ((rc = launch_scan(c, st, S.tiles, w.flag, m, w.pos, S.sc.as<uint64_t>(), launches))) return rc;
+  launches += 2;
+  if ((rc = launch_scan(c, st, S.tiles, w.flag, m, w.pos, S.sc.as<uint64_t>(), launches, tiled))) return rc;
   st_upd_append_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(d, w);
+  launches++;
   CK(cudaGetLastError());
+  if (ms) CK(cudaEventRecord(S.t5, st));
   CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  float t = 0;
+  if (ms) {
+    cudaEventElapsedTime(&t, S.t4, S.t5);
+    *ms += t;
+    CK(cudaEventRecord(S.t4, st));
+  }
   const uint64_t added = *S.h_sc.as<uint64_t>();
   if (added) st_table_insert_kernel<<<st_grid(c, added), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + added);
+  launches += added != 0;
   CK(cudaGetLastError());
+  if (ms) CK(cudaEventRecord(S.t5, st));
   CK(cudaStreamSynchronize(st));
+  if (ms) {
+    cudaEventElapsedTime(&t, S.t4, S.t5);
+    *ms += t;
+  }
   S.n_msgs += added;
   return TGI_OK;
 }
@@ -3948,7 +3961,8 @@ int tgi_state_update_messages(tgi_ctx* c, const tgi_state_update* ups, uint64_t 
   if ((rc = st_reserve(c, S, m))) return rc;
   CK(S.upd.ensure(m * sizeof(tgi_state_update)));
   CK(cudaMemcpyAsync(S.upd.p, u.data(), m * sizeof(tgi_state_update), cudaMemcpyHostToDevice, S.stream));
-  return st_apply_updates(c, S, m);
+  uint32_t launches = 0;
+  return st_apply_updates(c, S, m, launches);
 }
 
 int tgi_state_read_page(tgi_ctx* c, uint32_t row, tgi_state_msg* out, uint64_t cap, uint64_t* n) {
@@ -4229,105 +4243,217 @@ int tgi_state_export(tgi_ctx* c, int mode, uint64_t chunk_bytes, tgi_state_expor
   return TGI_OK;
 }
 
-// addNewMessages + resampleMarker + UpdatePage for one page (crawl/runner.go:1132-1147), touching only the page's own
-// messages: the fetched keys are probed against the page's list in the resident table, the new ones compacted in fetch
-// order and appended as the row's new list.  Three synchronises: the new list's length (and the old one's, for the
-// tombstone count), the row upload, and the work list; with TGI_TURN_PAGE_JSON the page's size comes back with the work
-// list and one more synchronise brings its bytes.
-int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
-                         const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out) {
-  if (!c || !out || (n && !fetched)) return TGI_E_ARG;
-  CrawlState& S = c->state;
-  std::lock_guard<std::mutex> g(S.mu);
+}  // extern "C"
+
+// ---- page turns over P pages (state.cuh): tgi_state_pages_begin / _end / _close, and the one-page calls as P = 1 ------
+namespace {
+
+// the rows of a turn call: at least one, each known, none listed twice
+int st_check_rows(tgi_ctx* c, const CrawlState& S, const uint32_t* rows, uint32_t P, const char* who) {
+  if (!P) { set_err(c, "%s: no pages", who); return TGI_E_ARG; }
+  std::unordered_set<uint32_t> seen;
+  for (uint32_t k = 0; k < P; k++) {
+    if (rows[k] >= S.rows.size()) { set_err(c, "%s: no row %u", who, rows[k]); return TGI_E_ARG; }
+    if (!seen.insert(rows[k]).second) { set_err(c, "%s: row %u is listed twice", who, rows[k]); return TGI_E_ARG; }
+  }
+  return TGI_OK;
+}
+
+// a page whose fields replace row r's: strings inside strs, no messages (`list` says where the list comes from), the
+// row's id
+bool st_check_page(tgi_ctx* c, const CrawlState& S, uint32_t r, const tgi_state_page& p, const uint8_t* strs,
+                   uint64_t strs_len, const char* who, const char* list) {
+  if (!page_ok(c, p, strs, strs_len, who)) return false;
+  if (p.n_msgs) { set_err(c, "%s: the page carries messages (%s)", who, list); return false; }
+  if (in_field(p, strs, TGI_PS_ID) != st_field(S, S.rows[r], TGI_PS_ID)) { set_err(c, "%s: the page's id is not row %u's", who, r); return false; }
+  return true;
+}
+
+// UpdatePage's layer rule for every row of the call (base.go:131-146): the row joins the layer of its depth if that
+// layer exists and does not hold it.  The rows of one depth are marked in a byte per row and the layer is read once,
+// so a call costs one pass over each layer it touches, whatever P, and allocates nothing once the marks have grown.
+void st_join_layers(CrawlState& S, const uint32_t* rows, uint32_t P) {
+  if (P == 1) {  // one row: the search stops where it finds the row
+    const auto lit = S.layers.find(S.rows[rows[0]].depth);
+    if (lit != S.layers.end() && std::find(lit->second.begin(), lit->second.end(), rows[0]) == lit->second.end())
+      lit->second.push_back(rows[0]);
+    return;
+  }
+  std::vector<uint8_t>& mark = S.row_mark;  // all 0 between calls
+  if (mark.size() < S.rows.size()) mark.resize(S.rows.size(), 0);
+  std::vector<std::pair<int64_t, uint32_t>> by_depth(P);
+  for (uint32_t k = 0; k < P; k++) by_depth[k] = {S.rows[rows[k]].depth, k};
+  std::sort(by_depth.begin(), by_depth.end());
+  for (size_t i = 0; i < by_depth.size();) {
+    size_t j = i;
+    while (j < by_depth.size() && by_depth[j].first == by_depth[i].first) j++;
+    const auto lit = S.layers.find(by_depth[i].first);
+    if (lit != S.layers.end()) {
+      std::vector<uint32_t>& L = lit->second;
+      for (size_t q = i; q < j; q++) mark[rows[by_depth[q].second]] = 1;
+      for (uint32_t r : L) mark[r] = 0;  // held already
+      for (size_t q = i; q < j; q++) {   // in call order, as P UpdatePage calls append them
+        const uint32_t r = rows[by_depth[q].second];
+        if (mark[r]) L.push_back(r);
+        mark[r] = 0;
+      }
+    }
+    i = j;
+  }
+}
+
+std::shared_ptr<DevBuf> st_take_keys(CrawlState& S) {
+  if (S.turn_pool.empty()) return std::make_shared<DevBuf>();
+  std::shared_ptr<DevBuf> b = std::move(S.turn_pool.back());
+  S.turn_pool.pop_back();
+  return b;
+}
+
+size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+// the pinned staging of a turn call's page arrays, `bytes` of it.  Its uploads are asynchronous and a call may return
+// before they have run (a close without TGI_TURN_PAGE_JSON and without out), so the buffer is reused, or regrown, only
+// once the last upload from it has finished; st_seg_upload records that upload.
+int st_seg_host(tgi_ctx* c, CrawlState& S, size_t bytes, uint8_t** h) {
+  CK(cudaEventSynchronize(S.ev_seg));
+  CK(S.h_seg.ensure(bytes));
+  *h = S.h_seg.as<uint8_t>();
+  return TGI_OK;
+}
+int st_seg_upload(tgi_ctx* c, CrawlState& S, size_t off, size_t bytes) {
+  CK(cudaMemcpyAsync(S.seg.as<uint8_t>() + off, S.h_seg.as<uint8_t>() + off, bytes, cudaMemcpyHostToDevice, S.stream));
+  CK(cudaEventRecord(S.ev_seg, S.stream));
+  return TGI_OK;
+}
+
+// addNewMessages + resampleMarker + UpdatePage for P pages (crawl/runner.go:1132-1147), touching only the pages' own
+// messages: a thread per fetched key probes its page's list in the resident table, one scan lays the new lists out in
+// (page, fetch) order, and each page's segment is appended as its row's next generation.  Three synchronises whatever
+// P: the new lists' lengths (and the old ones', for the tombstone count), the row strings' upload, and the work list;
+// with TGI_TURN_PAGE_JSON the pages' sizes come back with the work list and one more synchronise brings their lines.
+int st_pages_begin(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, const tgi_state_page* pages, const uint8_t* strs,
+                   uint64_t strs_len, const int64_t* fetched, uint64_t n, const uint64_t* foff, uint32_t flags, const char* who,
+                   tgi_state_pages_t* out) {
   int rc;
   if ((rc = st_init(c, S))) return rc;
   memset(out, 0, sizeof *out);
-  if (flags & ~TGI_TURN_PAGE_JSON) { set_err(c, "tgi_state_page_begin: unknown flags 0x%x", flags); return TGI_E_ARG; }
-  if (row >= S.rows.size()) { set_err(c, "tgi_state_page_begin: no row %u", row); return TGI_E_ARG; }
-  if (page) {
-    if (!page_ok(c, *page, strs, strs_len, "tgi_state_page_begin")) return TGI_E_ARG;
-    if (page->n_msgs) { set_err(c, "tgi_state_page_begin: the page carries messages (its list comes from the fetch)"); return TGI_E_ARG; }
-    if (in_field(*page, strs, TGI_PS_ID) != st_field(S, S.rows[row], TGI_PS_ID)) { set_err(c, "tgi_state_page_begin: the page's id is not row %u's", row); return TGI_E_ARG; }
-  }
+  if (flags & ~TGI_TURN_PAGE_JSON) { set_err(c, "%s: unknown flags 0x%x", who, flags); return TGI_E_ARG; }
+  if ((rc = st_check_rows(c, S, rows, P, who))) return rc;
+  if (foff[0] != 0 || foff[P] != n) { set_err(c, "%s: fetched_off runs from %llu to %llu, not 0 to n = %llu", who, (unsigned long long)foff[0], (unsigned long long)foff[P], (unsigned long long)n); return TGI_E_ARG; }
+  for (uint32_t k = 0; k < P; k++)
+    if (foff[k + 1] < foff[k]) { set_err(c, "%s: fetched_off decreases at page %u", who, k); return TGI_E_ARG; }
+  if (pages)
+    for (uint32_t k = 0; k < P; k++)
+      if (!st_check_page(c, S, rows[k], pages[k], strs, strs_len, who, "its list comes from the fetch")) return TGI_E_ARG;
   if ((rc = st_upload_codes(c, S))) return rc;
   if ((rc = st_reserve(c, S, n))) return rc;
   cudaStream_t st = S.stream;
-  const bool json = flags & TGI_TURN_PAGE_JSON;
-  std::shared_ptr<DevBuf> keys;
-  if (S.turn_pool.empty()) {
-    keys = std::make_shared<DevBuf>();
-  } else {
-    keys = std::move(S.turn_pool.back());
-    S.turn_pool.pop_back();
-  }
+  const bool json = flags & TGI_TURN_PAGE_JSON, tiled = P > 1;
+  std::shared_ptr<DevBuf> keys = st_take_keys(S);
   const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * n, 64));
+  // S.seg: foff [P+1] | woff [P+1] | prow [P] | old [P] | row puts [P]
+  const size_t o_woff = (P + 1) * 8ull, o_prow = 2 * o_woff, o_old = o_prow + 4ull * P, o_put = align16(o_old + 4ull * P);
+  const size_t seg_bytes = o_put + P * sizeof(StRowPut);
   CK(keys->ensure(n * 18));
   CK(S.turn_in.ensure(n * 16));
+  CK(S.seg.ensure(seg_bytes));
+  uint8_t* hseg;
+  if ((rc = st_seg_host(c, S, seg_bytes, &hseg))) return rc;
+  CK(S.pg.ensure(n * 4));
   CK(S.bfirst.ensure(bslots * 4));
   CK(S.flag.ensure(n * 4));
   CK(S.pos.ensure((n + 1) * 8));
   CK(S.slot_of.ensure(n * 4));
   CK(S.vals.ensure(n * 4));
   CK(S.keys.ensure(n * 4));
+  CK(S.row_base.ensure((S.rows.size() + 1) * 8));
   CK(S.sc.ensure(ST_SC_COUNT * 8));
   CK(S.h_sc.ensure(ST_SC_COUNT * 8));
   CK(S.h_work.ensure(n * 4));
+  CK(S.h_woff.ensure((P + 1) * 8));
+  CK(S.h_old.ensure(P * 4));
+  uint8_t* dseg = S.seg.as<uint8_t>();
+  memcpy(hseg, foff, (P + 1) * 8);
+  memcpy(hseg + o_prow, rows, P * 4);
   StTurn t{};
   t.fetched = S.turn_in.as<long long>();
   t.n = n;
-  t.row = row;
-  t.gen = S.gen[row] + 1;
+  t.foff = (const uint64_t*)dseg;
+  t.prow = (const uint32_t*)(dseg + o_prow);
+  t.P = P;
+  t.pg = S.pg.as<uint32_t>();
   t.bfirst = S.bfirst.as<uint32_t>();
   t.bmask = bslots - 1;
   t.flag = S.flag.as<uint32_t>();
   t.pos = S.pos.as<uint64_t>();
+  t.woff = (uint64_t*)(dseg + o_woff);
   t.n_msgs = S.n_msgs;
   t.keys = keys->as<long long>();
   t.work = S.slot_of.as<uint32_t>();
   t.sorted = S.vals.as<uint32_t>();
   t.rows = S.keys.as<uint32_t>();
-  uint64_t* hs = S.h_sc.as<uint64_t>();
-  hs[0] = hs[1] = 0;
+  uint32_t* d_old = (uint32_t*)(dseg + o_old);
   uint32_t launches = 0;
-  // 1. which fetched keys the page's list lacks, and the old list's length
+  // 1. which fetched keys their pages' lists lack, every page's segment of the new lists, and the old lists' lengths
   CK(cudaEventRecord(S.t0, st));
+  if ((rc = st_seg_upload(c, S, 0, o_old))) return rc;
   if (n) {
     CK(cudaMemcpyAsync(S.turn_in.p, fetched, n * 16, cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(S.bfirst.p, 0xFF, bslots * 4, st));
     st_turn_probe_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(st_dev(S), t);
     launches++;
-    if ((rc = launch_scan(c, st, S.tiles, t.flag, n, t.pos, S.sc.as<uint64_t>(), launches))) return rc;
-    CK(cudaMemcpyAsync(hs, S.sc.p, 8, cudaMemcpyDeviceToHost, st));
+    if ((rc = launch_scan(c, st, S.tiles, t.flag, n, t.pos, S.sc.as<uint64_t>(), launches, tiled))) return rc;
   }
-  CK(cudaMemcpyAsync(hs + 1, S.row_cnt.as<uint32_t>() + row, 4, cudaMemcpyDeviceToHost, st));
+  st_turn_meta_kernel<<<st_grid(c, P + 1), ST_THREADS, 0, st>>>(S.row_cnt.as<uint32_t>(), t.prow, P, t.foff, n ? t.pos : nullptr,
+                                                                 t.woff, d_old);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(S.h_woff.p, t.woff, (P + 1) * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_old.p, d_old, P * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(S.t1, st));
   CK(cudaStreamSynchronize(st));
-  const uint64_t n_new = hs[0];
-  // 2. UpdatePage(*owner): the old list becomes tombstones; the row takes the page's fields and joins the layer of its
-  // depth if that layer exists and does not hold it (base.go:131-146).  The new list is the row's owner view, its
-  // statuses "resample" (0) until the end's hits.
-  S.n_dead += hs[1];
-  S.gen[row]++;
-  if ((rc = st_page_fields(c, S, row, page, strs, true))) return rc;
-  st_drop_view(S, row);
-  S.views[row] = CrawlState::View{n_new, keys};
-  const uint32_t cnt = (uint32_t)n_new;
-  CK(cudaMemcpyAsync(S.row_cnt.as<uint32_t>() + row, &cnt, 4, cudaMemcpyHostToDevice, st));
+  const uint64_t* wo = S.h_woff.as<uint64_t>();
+  const uint32_t* old = S.h_old.as<uint32_t>();
+  const uint64_t n_new = wo[P];
+  // 2. UpdatePage(*owner) of every page: the old lists become tombstones; each row takes its page's fields and joins the
+  // layer of its depth if that layer exists and does not hold it (base.go:131-146).  Each new list is its row's owner
+  // view, a slice of this call's key buffer, its statuses "resample" (0) until the end's hits.
+  for (uint32_t k = 0; k < P; k++) {
+    S.n_dead += old[k];
+    S.gen[rows[k]]++;
+    if (pages) st_put_row(S, rows[k], pages[k], strs);
+  }
+  st_join_layers(S, rows, P);
+  rc = st_sync_rows(c, S, std::vector<uint32_t>());  // the new strings
+  if (rc) return rc;
+  StRowPut* put = (StRowPut*)(hseg + o_put);
+  for (uint32_t k = 0; k < P; k++) {
+    const uint32_t r = rows[k];
+    put[k] = StRowPut{S.rows[r], r, S.gen[r], (uint32_t)(wo[k + 1] - wo[k]), 1u, json ? wo[k] : ST_NO_BASE};
+    st_drop_view(S, r);
+    S.views[r] = CrawlState::View{wo[k], wo[k + 1] - wo[k], n_new, keys};
+  }
+  if ((rc = st_seg_upload(c, S, o_put, P * sizeof(StRowPut)))) return rc;
   if (n_new) CK(cudaMemsetAsync(keys->as<uint8_t>() + 16 * n_new, 0, 2 * n_new, st));
   const StDev d = st_dev(S);
   CK(cudaEventRecord(S.t2, st));
+  st_rows_put_kernel<<<st_grid(c, P), ST_THREADS, 0, st>>>(S.pages.as<tgi_state_page>(), d.row_gen, d.row_cnt,
+                                                           (const StRowPut*)(dseg + o_put), P, S.row_base.as<uint64_t>());
+  launches++;
   if (n_new) {
     st_turn_append_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(d, t);
     st_table_insert_kernel<<<st_grid(c, n_new), ST_THREADS, 0, st>>>(d, S.n_msgs, S.n_msgs + n_new);
     launches += 2;
   }
   S.n_msgs += n_new;
-  // 3. json.Marshal(page) by the export's line passes over this one row, its new list being the fresh segment
+  // 3. json.Marshal(page) of every page by the export's line passes over the rows, their new lists being the fresh
+  // segments in the call's order
   StRender r{};
+  uint64_t* hs = S.h_sc.as<uint64_t>();
   std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
   if (json) {
     zg.lock();
-    if ((rc = st_page_json_size(c, S, row, t.sorted, t.rows, n_new, r, launches))) return rc;
+    if ((rc = st_page_json_size(c, S, rows, P, t.sorted, t.rows, n_new, tiled, r, launches))) return rc;
     CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaGetLastError());
@@ -4337,192 +4463,325 @@ int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   float ms0 = 0, ms1 = 0, ms2 = 0;
   cudaEventElapsedTime(&ms0, S.t0, S.t1);
   cudaEventElapsedTime(&ms1, S.t2, S.t3);
-  // a page that does not marshal: the new list and its view stay, no turn opens, as the reference returns before its loop
-  if (json && (rc = st_page_json_emit(c, S, r, t.sorted, n_new, hs, "tgi_state_page_begin", &out->page_json,
-                                      &out->page_json_len, &ms2, launches)))
+  // a page that does not marshal: the new lists and their views stay, no turn opens, as the reference returns before
+  // its loop
+  if (json && (rc = st_page_json_emit(c, S, r, t.sorted, n_new, hs, who, &out->page_json, &out->json_off, &ms2, launches)))
     return rc;
   if ((rc = st_compact(c, S))) return rc;
   const uint32_t h = S.next_turn++;
   if (!S.next_turn) S.next_turn = 1;
   CrawlState::Turn& T = S.turns[h];
-  T.row = row;
-  T.n_work = n_new;
+  T.rows.assign(rows, rows + P);
+  T.off.assign(wo, wo + P + 1);
   T.keys = std::move(keys);
   out->turn = h;
-  out->row = row;
+  out->n_pages = P;
   out->n_work = n_new;
   out->work = S.h_work.as<uint32_t>();
+  out->work_off = wo;
   out->kernel_ms = ms0 + ms1 + ms2;
   out->gpu_launches = launches;
   return TGI_OK;
 }
 
-// the loop's first n_done UpdateMessage calls (crawl/runner.go:1161-1211) as one tgi_state_update_messages batch, built
-// on the device from the turn's keys and the statuses.  Lock order: the slot, then the state; no other entry point holds
-// both.  The slot's lock is held until the kernels that read its status array have finished.
-int tgi_state_page_end(tgi_ctx* c, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended) {
-  if (!c || (slot < 0 && n_done && !status)) return TGI_E_ARG;
-  if (slot >= TGI_SLOTS) { set_err(c, "tgi_state_page_end: bad slot %d", slot); return TGI_E_ARG; }
+// the loop's first n_done[k] UpdateMessage calls of every page k of a turn (crawl/runner.go:1161-1211), in page order,
+// as one tgi_state_update_messages batch built on the device from the turn's keys and the statuses; then the owner
+// views' hits, a segment per page.  one: tgi_state_page_end (a one-page turn, a result of exactly its records).  Lock
+// order: the slot, then the state; no other entry point holds both.  The slot's lock is held until the kernels that
+// read its status array have finished.
+int st_pages_end(tgi_ctx* c, uint32_t turn, int slot, uint64_t first, const uint8_t* status, const uint64_t* n_done, bool one,
+                 uint64_t* appended, tgi_state_end_t* out) {
+  const char* const who = one ? "tgi_state_page_end" : "tgi_state_pages_end";
+  if (slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
   Slot* s = slot >= 0 ? &c->slots[slot] : nullptr;
   std::unique_lock<std::mutex> sl;
   if (s) {
     sl = std::unique_lock<std::mutex>(s->mu);
-    if (in_flight(*s)) { set_err(c, "tgi_state_page_end: slot %d is in flight", slot); return TGI_E_STATE; }
-    if (!s->busy || s->last.kind == REC_NONE) { set_err(c, "tgi_state_page_end: slot %d holds no result (released or none)", slot); return TGI_E_ARG; }
-    if (s->last.kind != REC_TG || !s->last.dev.status) { set_err(c, "tgi_state_page_end: slot %d's result is not a Telegram one", slot); return TGI_E_ARG; }
+    if (in_flight(*s)) { set_err(c, "%s: slot %d is in flight", who, slot); return TGI_E_STATE; }
+    if (!s->busy || s->last.kind == REC_NONE) { set_err(c, "%s: slot %d holds no result (released or none)", who, slot); return TGI_E_ARG; }
+    if (s->last.kind != REC_TG || !s->last.dev.status) { set_err(c, "%s: slot %d's result is not a Telegram one", who, slot); return TGI_E_ARG; }
   }
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
   int rc;
   if ((rc = st_init(c, S))) return rc;
   const auto it = S.turns.find(turn);
-  if (it == S.turns.end()) { set_err(c, "tgi_state_page_end: no open turn %u", turn); return TGI_E_ARG; }
+  if (it == S.turns.end()) { set_err(c, "%s: no open turn %u", who, turn); return TGI_E_ARG; }
   CrawlState::Turn& T = it->second;
-  if (s && s->last.n != T.n_work) {
-    set_err(c, "tgi_state_page_end: the slot's result holds %llu records, the turn %llu", (unsigned long long)s->last.n, (unsigned long long)T.n_work);
+  const uint32_t P = (uint32_t)T.rows.size();
+  const uint64_t N = T.n_work();
+  if (one && P != 1) { set_err(c, "%s: turn %u covers %u pages (tgi_state_pages_end)", who, turn, P); return TGI_E_ARG; }
+  if (s && one && s->last.n != N) {
+    set_err(c, "%s: the slot's result holds %llu records, the turn %llu", who, (unsigned long long)s->last.n, (unsigned long long)N);
     return TGI_E_ARG;
   }
-  if (n_done > T.n_work) { set_err(c, "tgi_state_page_end: n_done %llu > n_work %llu", (unsigned long long)n_done, (unsigned long long)T.n_work); return TGI_E_ARG; }
+  if (s && (first > s->last.n || N > s->last.n - first)) {
+    set_err(c, "%s: records [%llu, %llu + %llu) lie outside the result's %llu", who, (unsigned long long)first, (unsigned long long)first,
+            (unsigned long long)N, (unsigned long long)s->last.n);
+    return TGI_E_ARG;
+  }
+  std::vector<uint64_t> uoff(P + 1, 0);
+  uint64_t reach = 0;  // statuses read: [0, reach) of the turn's records
+  for (uint32_t k = 0; k < P; k++) {
+    const uint64_t cnt = T.off[k + 1] - T.off[k], nd = n_done ? n_done[k] : cnt;
+    if (nd > cnt) { set_err(c, "%s: page %u: n_done %llu > n_work %llu", who, k, (unsigned long long)nd, (unsigned long long)cnt); return TGI_E_ARG; }
+    uoff[k + 1] = uoff[k] + nd;
+    if (nd) reach = T.off[k] + nd;
+  }
+  const uint64_t m = uoff[P];
+  if (!s && m && !status) { set_err(c, "%s: no statuses (slot < 0 takes them from the host)", who); return TGI_E_ARG; }
   const uint64_t before = S.n_msgs;
-  if (n_done) {
-    if ((rc = st_reserve(c, S, n_done))) return rc;
+  uint32_t launches = 0;
+  float ms = 0;
+  if (m) {
+    if ((rc = st_reserve(c, S, m))) return rc;
     cudaStream_t st = S.stream;
-    const uint8_t* d_status;
-    CK(S.upd.ensure(n_done * sizeof(tgi_state_update)));
+    // S.seg: woff [P+1] | uoff [P+1] | prow [P] | live [P] | app [P]
+    const size_t o_uoff = (P + 1) * 8ull, o_prow = 2 * o_uoff, o_live = o_prow + 4ull * P, o_app = o_live + 4ull * P;
+    const size_t seg_bytes = o_app + 4ull * P;
+    CK(S.seg.ensure(seg_bytes));
+    uint8_t* hseg;
+    if ((rc = st_seg_host(c, S, seg_bytes, &hseg))) return rc;
+    CK(S.upd.ensure(m * sizeof(tgi_state_update)));
+    uint8_t* dseg = S.seg.as<uint8_t>();
+    memcpy(hseg, T.off.data(), (P + 1) * 8);
+    memcpy(hseg + o_uoff, uoff.data(), (P + 1) * 8);
+    memcpy(hseg + o_prow, T.rows.data(), P * 4);
+    uint32_t* live = (uint32_t*)(hseg + o_live);
+    bool any = false;
+    for (uint32_t k = 0; k < P; k++) {  // the pages whose row still holds this turn's keys as its owner view
+      const auto vit = S.views.find(T.rows[k]);
+      live[k] = vit != S.views.end() && vit->second.keys == T.keys && vit->second.off == T.off[k] && T.off[k + 1] > T.off[k];
+      any = any || live[k];
+    }
+    if ((rc = st_seg_upload(c, S, 0, o_app))) return rc;
+    StEnd e{};
+    e.keys = T.keys->as<long long>();
+    e.woff = (const uint64_t*)dseg;
+    e.uoff = (const uint64_t*)(dseg + o_uoff);
+    e.prow = (const uint32_t*)(dseg + o_prow);
+    e.live = (const uint32_t*)(dseg + o_live);
+    e.P = P;
     if (s) {
       CK(cudaEventRecord(S.ev_slot, s->stream));
       CK(cudaStreamWaitEvent(st, S.ev_slot, 0));
-      d_status = s->last.dev.status;
+      e.status = s->last.dev.status + first;
     } else {
-      CK(S.turn_in.ensure(n_done));
-      CK(cudaMemcpyAsync(S.turn_in.p, status, n_done, cudaMemcpyHostToDevice, st));
-      d_status = S.turn_in.as<uint8_t>();
+      CK(S.turn_in.ensure(reach));
+      CK(cudaMemcpyAsync(S.turn_in.p, status, reach, cudaMemcpyHostToDevice, st));
+      e.status = S.turn_in.as<uint8_t>();
     }
-    st_turn_updates_kernel<<<st_grid(c, n_done), ST_THREADS, 0, st>>>(T.keys->as<long long>(), d_status, n_done, T.row,
-                                                                      S.upd.as<tgi_state_update>());
+    // the device time is taken only when out asks for it: the one-page end pays no event
+    if (out) CK(cudaEventRecord(S.t0, st));
+    st_turn_updates_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(e, m, S.upd.as<tgi_state_update>());
+    launches++;
     CK(cudaGetLastError());
-    if ((rc = st_apply_updates(c, S, n_done))) return rc;
-    // the owner's side of the updates, while this turn's keys are still the row's owner view
-    const auto vit = S.views.find(T.row);
-    if (vit != S.views.end() && vit->second.keys == T.keys && T.n_work) {
-      const uint64_t k = T.n_work, vslots = next_pow2(std::max<uint64_t>(2 * k, 64));
+    if (out) CK(cudaEventRecord(S.t1, st));
+    if ((rc = st_apply_updates(c, S, m, launches, P > 1, out ? &ms : nullptr))) return rc;  // synchronises
+    float t = 0;
+    if (out) {
+      cudaEventElapsedTime(&t, S.t0, S.t1);
+      ms += t;
+    }
+    // the owner's side of the updates, on the pages whose views are still this turn's keys
+    if (any) {
+      const uint64_t vslots = next_pow2(std::max<uint64_t>(2 * N, 64));
       CK(S.bfirst.ensure(vslots * 4));
-      CK(S.blast.ensure((k + 1) * 4));
+      CK(S.blast.ensure(N * 4));
       StView v{};
-      v.keys = T.keys->as<long long>();
-      v.status = (uint16_t*)(T.keys->as<uint8_t>() + 16 * k);
-      v.k = k;
+      v.e = e;
+      v.status = (uint16_t*)(T.keys->as<uint8_t>() + 16 * N);
+      v.k = N;
       v.vfirst = S.bfirst.as<uint32_t>();
       v.vmask = vslots - 1;
       v.last = S.blast.as<uint32_t>();
+      v.app = (uint32_t*)(dseg + o_app);
       CK(cudaMemsetAsync(v.vfirst, 0xFF, vslots * 4, st));
-      CK(cudaMemsetAsync(v.last, 0, k * 4, st));
-      CK(cudaMemsetAsync(v.last + k, 0xFF, 4, st));
+      CK(cudaMemsetAsync(v.last, 0, N * 4, st));
+      CK(cudaMemsetAsync(v.app, 0xFF, P * 4, st));
       const tgi_state_update* u = S.upd.as<tgi_state_update>();
-      st_view_build_kernel<<<st_grid(c, std::max(k, n_done)), ST_THREADS, 0, st>>>(v, S.flag.as<uint32_t>(), n_done);
-      st_view_hit_kernel<<<st_grid(c, n_done), ST_THREADS, 0, st>>>(v, u, n_done);
-      st_view_status_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(v, u);
+      if (out) CK(cudaEventRecord(S.t2, st));
+      st_view_build_kernel<<<st_grid(c, std::max(N, m)), ST_THREADS, 0, st>>>(v, S.flag.as<uint32_t>(), m);
+      st_view_hit_kernel<<<st_grid(c, m), ST_THREADS, 0, st>>>(v, u, m);
+      st_view_status_kernel<<<st_grid(c, N), ST_THREADS, 0, st>>>(v, u);
+      launches += 3;
       CK(cudaGetLastError());
+      if (out) {
+        CK(cudaEventRecord(S.t3, st));
+        CK(cudaEventSynchronize(S.t3));
+        cudaEventElapsedTime(&t, S.t2, S.t3);
+        ms += t;
+      }
     }
   }
   if (appended) *appended = S.n_msgs - before;
+  if (out) {
+    out->appended = S.n_msgs - before;
+    out->kernel_ms = ms;
+    out->gpu_launches = launches;
+  }
   st_release(S, T.keys);
   S.turns.erase(it);
   return TGI_OK;
 }
 
-// UpdatePage(*owner) for a page whose list came from a page turn (crawl/runner.go:1543-1544, dapr/standalone.go:589-609):
-// the page's fields replace the row's; with an owner view the row's list becomes the view, appended as its next
-// generation by one kernel.  The row upload synchronises, as every row rewrite does; beyond it the call waits only for
-// the page's read-back (TGI_TURN_PAGE_JSON; without a view, also the row's count) or, given out, for its kernels' time.
-int tgi_state_page_close(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
-                         uint32_t flags, tgi_state_json_t* out) {
-  static const char* const who = "tgi_state_page_close";
-  if (!c || !page || (!out && (flags & TGI_TURN_PAGE_JSON))) return TGI_E_ARG;
-  CrawlState& S = c->state;
-  std::lock_guard<std::mutex> g(S.mu);
+// UpdatePage(*owner) for P pages whose lists came from page turns (crawl/runner.go:1543-1544, dapr/standalone.go:589-609):
+// each page's fields replace its row's; a row with an owner view makes the view its list, appended as its next
+// generation.  All rows' fields go up in one upload and one kernel, every view is appended by one kernel.  The row
+// strings' upload synchronises, as every row rewrite does; beyond it the call waits only for the pages' read-back
+// (TGI_TURN_PAGE_JSON) or, given out, for its kernels' time.
+int st_pages_close(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, const tgi_state_page* pages, const uint8_t* strs,
+                   uint64_t strs_len, uint32_t flags, const char* who, tgi_state_pages_t* out) {
   int rc;
   if ((rc = st_init(c, S))) return rc;
   if (out) memset(out, 0, sizeof *out);
   if (flags & ~TGI_TURN_PAGE_JSON) { set_err(c, "%s: unknown flags 0x%x", who, flags); return TGI_E_ARG; }
-  if (row >= S.rows.size()) { set_err(c, "%s: no row %u", who, row); return TGI_E_ARG; }
-  if (!page_ok(c, *page, strs, strs_len, who)) return TGI_E_ARG;
-  if (page->n_msgs) { set_err(c, "%s: the page carries messages (its list is the owner view)", who); return TGI_E_ARG; }
-  if (in_field(*page, strs, TGI_PS_ID) != st_field(S, S.rows[row], TGI_PS_ID)) { set_err(c, "%s: the page's id is not row %u's", who, row); return TGI_E_ARG; }
-  const bool json = flags & TGI_TURN_PAGE_JSON;
+  if ((rc = st_check_rows(c, S, rows, P, who))) return rc;
+  for (uint32_t k = 0; k < P; k++)
+    if (!st_check_page(c, S, rows[k], pages[k], strs, strs_len, who, "its list is the owner view")) return TGI_E_ARG;
+  const bool json = flags & TGI_TURN_PAGE_JSON, tiled = P > 1;
   if (json && (rc = st_upload_codes(c, S))) return rc;
-  const auto vit = S.views.find(row);
-  const bool view = vit != S.views.end();
-  const uint64_t k = view ? vit->second.k : 0;
-  if (view && (rc = st_reserve(c, S, k))) return rc;
-  cudaStream_t st = S.stream;
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
-  CK(S.vals.ensure(k * 4));
-  CK(S.keys.ensure(k * 4));
-  // no UpdateMessage of the loop follows: the row's open turns end here
-  for (auto it = S.turns.begin(); it != S.turns.end();) {
-    if (it->second.row != row) {
-      ++it;
+  std::vector<const CrawlState::View*> view(P, nullptr);
+  std::vector<uint32_t> bare;  // the rows without a view, ascending
+  uint64_t K = 0;
+  uint32_t Q = 0;
+  for (uint32_t k = 0; k < P; k++) {
+    const auto vit = S.views.find(rows[k]);
+    if (vit == S.views.end()) {
+      bare.push_back(rows[k]);
       continue;
     }
-    st_release(S, it->second.keys);
-    it = S.turns.erase(it);
+    view[k] = &vit->second;
+    K += vit->second.k;
+    Q++;
   }
-  uint64_t* hs = S.h_sc.as<uint64_t>();
-  hs[1] = 0;
-  uint32_t launches = 0;
-  if (view) {  // the old list's length, brought back by the row upload's synchronise
-    CK(cudaMemcpyAsync(hs + 1, S.row_cnt.as<uint32_t>() + row, 4, cudaMemcpyDeviceToHost, st));
-    S.gen[row]++;
-  }
-  if ((rc = st_page_fields(c, S, row, page, strs, view))) return rc;
-  const uint64_t n0 = S.n_msgs;
-  const uint32_t* sorted = S.vals.as<uint32_t>();
-  const uint32_t* rows = S.keys.as<uint32_t>();
-  uint64_t cnt = k;
-  CK(cudaEventRecord(S.t2, st));
-  if (view) {
-    S.n_dead += hs[1];
-    const StDev d = st_dev(S);
-    StView v{};
-    v.keys = vit->second.keys->as<long long>();
-    v.status = (uint16_t*)(vit->second.keys->as<uint8_t>() + 16 * k);
-    v.k = k;
-    if (k) {
-      st_view_append_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(d, v, row, S.gen[row], n0, S.vals.as<uint32_t>(), S.keys.as<uint32_t>());
-      st_table_insert_kernel<<<st_grid(c, k), ST_THREADS, 0, st>>>(d, n0, n0 + k);
-      launches += 2;
+  std::sort(bare.begin(), bare.end());
+  if (K && (rc = st_reserve(c, S, K))) return rc;
+  cudaStream_t st = S.stream;
+  // S.seg: prow [P] | old [P] | bare rows [P] | row puts [P] | views [Q]
+  const size_t o_old = 4ull * P, o_bare = 8ull * P, o_put = align16(12ull * P), o_view = o_put + P * sizeof(StRowPut);
+  const size_t seg_bytes = o_view + Q * sizeof(StViewSeg);
+  CK(S.seg.ensure(seg_bytes));
+  uint8_t* hseg;
+  if ((rc = st_seg_host(c, S, seg_bytes, &hseg))) return rc;
+  CK(S.h_old.ensure(P * 4));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.row_base.ensure((S.rows.size() + 1) * 8));
+  // no UpdateMessage of the loop follows: every open turn that lists one of the rows ends here
+  {
+    const std::unordered_set<uint32_t> closing(rows, rows + P);
+    for (auto it = S.turns.begin(); it != S.turns.end();) {
+      if (std::none_of(it->second.rows.begin(), it->second.rows.end(), [&](uint32_t r) { return closing.count(r) > 0; })) {
+        ++it;
+        continue;
+      }
+      st_release(S, it->second.keys);
+      it = S.turns.erase(it);
     }
-    S.n_msgs += k;
-  } else if (json) {  // no view: the row's list as it is, found by a scan of the message rows
-    uint32_t n = 0;
-    if ((rc = st_row_count(c, S, row, &n))) return rc;
-    cnt = n;
-    const uint64_t nm = S.n_msgs;
-    CK(S.flag.ensure(nm * 4));
-    CK(S.pos.ensure((nm + 1) * 8));
-    CK(S.vals.ensure(cnt * 4));
-    CK(S.keys.ensure(cnt * 4));
-    sorted = S.vals.as<uint32_t>();
-    rows = S.keys.as<uint32_t>();
-    StRender r{};
-    r.flag = S.flag.as<uint32_t>();
-    r.pos = S.pos.as<uint64_t>();
-    r.keys[0] = S.keys.as<uint32_t>();
-    r.vals[0] = S.vals.as<uint32_t>();
-    const StDev d = st_dev(S);
-    st_live_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, row, r.flag);
-    if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, S.sc.as<uint64_t>(), launches))) return rc;
-    st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
+  }
+  uint8_t* dseg = S.seg.as<uint8_t>();
+  const uint32_t* d_rows = (const uint32_t*)dseg;
+  uint32_t* d_old = (uint32_t*)(dseg + o_old);
+  memcpy(hseg, rows, P * 4);
+  memcpy(hseg + o_bare, bare.data(), bare.size() * 4);
+  uint32_t launches = 0;
+  // the old lists' lengths, brought back by the row strings' synchronise
+  if ((rc = st_seg_upload(c, S, 0, o_put))) return rc;
+  st_turn_meta_kernel<<<st_grid(c, P + 1), ST_THREADS, 0, st>>>(S.row_cnt.as<uint32_t>(), d_rows, P, nullptr, nullptr, nullptr, d_old);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(S.h_old.p, d_old, P * 4, cudaMemcpyDeviceToHost, st));
+  for (uint32_t k = 0; k < P; k++) {
+    st_put_row(S, rows[k], pages[k], strs);
+    if (view[k]) S.gen[rows[k]]++;
+  }
+  st_join_layers(S, rows, P);
+  rc = st_sync_rows(c, S, std::vector<uint32_t>());  // the new strings
+  if (rc) return rc;
+  const uint32_t* old = S.h_old.as<uint32_t>();
+  uint64_t M = 0;  // messages of the rows without a view
+  StRowPut* put = (StRowPut*)(hseg + o_put);
+  StViewSeg* vs = (StViewSeg*)(hseg + o_view);
+  for (uint32_t k = 0, q = 0, voff = 0; k < P; k++) {
+    const uint32_t r = rows[k];
+    if (!view[k]) M += old[k];
+    else S.n_dead += old[k];
+    put[k] = StRowPut{S.rows[r], r, S.gen[r], view[k] ? (uint32_t)view[k]->k : 0u, view[k] ? 1u : 0u,
+                      json ? (view[k] ? voff : 0) : ST_NO_BASE};
+    if (view[k]) {
+      vs[q++] = StViewSeg{view[k]->key_ptr(), view[k]->status_ptr(), voff, r, 0};
+      voff += (uint32_t)view[k]->k;
+    }
+  }
+  // the grouped order: the views' K messages, then (TGI_TURN_PAGE_JSON) the M of the rows without a view and the radix
+  // passes' other buffer
+  const uint64_t grouped = K + (json ? 2 * M : 0);
+  CK(S.vals.ensure(grouped * 4));
+  CK(S.keys.ensure(grouped * 4));
+  if ((rc = st_seg_upload(c, S, o_put, seg_bytes - o_put))) return rc;
+  const uint64_t n0 = S.n_msgs;
+  const StDev d = st_dev(S);
+  CK(cudaEventRecord(S.t2, st));
+  st_rows_put_kernel<<<st_grid(c, P), ST_THREADS, 0, st>>>(S.pages.as<tgi_state_page>(), d.row_gen, d.row_cnt,
+                                                           (const StRowPut*)(dseg + o_put), P, S.row_base.as<uint64_t>());
+  launches++;
+  if (K) {
+    st_view_append_kernel<<<st_grid(c, K), ST_THREADS, 0, st>>>(d, (const StViewSeg*)(dseg + o_view), Q, K, n0, S.vals.as<uint32_t>(),
+                                                                S.keys.as<uint32_t>());
+    st_table_insert_kernel<<<st_grid(c, K), ST_THREADS, 0, st>>>(d, n0, n0 + K);
     launches += 2;
   }
+  S.n_msgs += K;
+  CK(cudaGetLastError());
   float ms1 = 0, ms2 = 0;
   StRender r{};
+  uint64_t* hs = S.h_sc.as<uint64_t>();
   std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
   if (json) {
+    // the rows without a view render their lists as they are: their live messages, found by a scan of the message rows
+    // and grouped by row with the render's stable radix passes, follow the views' K messages
+    if (M) {
+      const uint64_t nm = S.n_msgs, nr = S.rows.size();
+      uint32_t bits = 0;
+      while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
+      const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0,
+                     radix = 1u << width;
+      const uint64_t ntiles = std::max<uint64_t>((M + RS_TILE - 1) / RS_TILE, 1);
+      CK(S.flag.ensure(nm * 4));
+      CK(S.pos.ensure((nm + 1) * 8));
+      CK(S.counts.ensure(radix * ntiles * 4));
+      CK(S.roff.ensure((radix * ntiles + 1) * 8));
+      StRender g{};
+      g.flag = S.flag.as<uint32_t>();
+      g.pos = S.pos.as<uint64_t>();
+      const int fin = passes & 1;  // the buffer the last pass writes: right behind the views' messages
+      g.keys[fin] = S.keys.as<uint32_t>() + K;
+      g.keys[fin ^ 1] = S.keys.as<uint32_t>() + K + M;
+      g.vals[fin] = S.vals.as<uint32_t>() + K;
+      g.vals[fin ^ 1] = S.vals.as<uint32_t>() + K + M;
+      uint64_t* cnt = S.sc.as<uint64_t>() + ST_SC_LIVE;
+      st_rows_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, (const uint32_t*)(dseg + o_bare), (uint32_t)bare.size(), g.flag);
+      launches++;
+      if ((rc = launch_scan(c, st, S.tiles, g.flag, nm, g.pos, cnt, launches, tiled))) return rc;
+      st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, g);
+      launches++;
+      for (uint32_t p = 0, cur = 0; p < passes; p++, cur ^= 1) {
+        const uint32_t shift = p * width;
+        la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], cnt, shift, radix, (uint32_t)ntiles,
+                                                                       S.counts.as<uint32_t>());
+        launches++;
+        if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), S.sc.as<uint64_t>() + ST_SC_RADIX, launches, tiled))) return rc;
+        la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], g.vals[cur], g.keys[cur ^ 1], g.vals[cur ^ 1], cnt,
+                                                                          shift, radix, (uint32_t)ntiles, S.roff.as<uint64_t>());
+        launches++;
+      }
+      st_row_starts_kernel<<<st_grid(c, M), ST_THREADS, 0, st>>>(g.keys[fin], cnt, K, S.row_base.as<uint64_t>());
+      launches++;
+      CK(cudaGetLastError());
+    }
     zg.lock();
-    if ((rc = st_page_json_size(c, S, row, sorted, rows, cnt, r, launches))) return rc;
+    if ((rc = st_page_json_size(c, S, rows, P, S.vals.as<uint32_t>(), S.keys.as<uint32_t>(), K + M, tiled, r, launches))) return rc;
     CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaGetLastError());
@@ -4530,7 +4789,8 @@ int tgi_state_page_close(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
   if (json) {
     CK(cudaStreamSynchronize(st));
     cudaEventElapsedTime(&ms1, S.t2, S.t3);
-    if ((rc = st_page_json_emit(c, S, r, sorted, cnt, hs, who, &out->data, &out->len, &ms2, launches))) return rc;
+    if ((rc = st_page_json_emit(c, S, r, S.vals.as<uint32_t>(), K + M, hs, who, &out->page_json, &out->json_off, &ms2, launches)))
+      return rc;
   }
   if ((rc = st_compact(c, S))) return rc;
   if (out) {
@@ -4538,9 +4798,81 @@ int tgi_state_page_close(tgi_ctx* c, uint32_t row, const tgi_state_page* page, c
       CK(cudaEventSynchronize(S.t3));
       cudaEventElapsedTime(&ms1, S.t2, S.t3);
     }
+    out->n_pages = P;
     out->kernel_ms = ms1 + ms2;
     out->gpu_launches = launches;
   }
+  return TGI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tgi_state_pages_begin(tgi_ctx* c, const uint32_t* rows, uint32_t n_pages, const tgi_state_page* pages, const uint8_t* strs,
+                          uint64_t strs_len, const int64_t* fetched, uint64_t n, const uint64_t* fetched_off, uint32_t flags,
+                          tgi_state_pages_t* out) {
+  if (!c || !out || (n_pages && !rows) || !fetched_off || (n && !fetched)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  return st_pages_begin(c, S, rows, n_pages, pages, strs, strs_len, fetched, n, fetched_off, flags, "tgi_state_pages_begin", out);
+}
+
+int tgi_state_pages_end(tgi_ctx* c, uint32_t turn, int slot, uint64_t first, const uint8_t* status, const uint64_t* n_done,
+                        tgi_state_end_t* out) {
+  if (!c) return TGI_E_ARG;
+  if (out) memset(out, 0, sizeof *out);
+  return st_pages_end(c, turn, slot, first, status, n_done, false, nullptr, out);
+}
+
+int tgi_state_pages_close(tgi_ctx* c, const uint32_t* rows, uint32_t n_pages, const tgi_state_page* pages, const uint8_t* strs,
+                          uint64_t strs_len, uint32_t flags, tgi_state_pages_t* out) {
+  if (!c || (n_pages && (!rows || !pages)) || (!out && (flags & TGI_TURN_PAGE_JSON))) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  return st_pages_close(c, S, rows, n_pages, pages, strs, strs_len, flags, "tgi_state_pages_close", out);
+}
+
+// the one-page calls: P = 1 of the calls above
+int tgi_state_page_begin(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         const int64_t* fetched, uint64_t n, uint32_t flags, tgi_state_turn_t* out) {
+  if (!c || !out || (n && !fetched)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  memset(out, 0, sizeof *out);
+  const uint64_t foff[2] = {0, n};
+  tgi_state_pages_t o;
+  const int rc = st_pages_begin(c, S, &row, 1, page, strs, strs_len, fetched, n, foff, flags, "tgi_state_page_begin", &o);
+  if (rc) return rc;
+  out->turn = o.turn;
+  out->row = row;
+  out->n_work = o.n_work;
+  out->work = o.work;
+  out->page_json = o.page_json;
+  out->page_json_len = o.page_json ? o.json_off[1] - 1 : 0;  // the line without its '\n'
+  out->kernel_ms = o.kernel_ms;
+  out->gpu_launches = o.gpu_launches;
+  return TGI_OK;
+}
+
+int tgi_state_page_end(tgi_ctx* c, uint32_t turn, int slot, const uint8_t* status, uint64_t n_done, uint64_t* appended) {
+  if (!c || (slot < 0 && n_done && !status)) return TGI_E_ARG;
+  return st_pages_end(c, turn, slot, 0, status, &n_done, true, appended, nullptr);
+}
+
+int tgi_state_page_close(tgi_ctx* c, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
+                         uint32_t flags, tgi_state_json_t* out) {
+  if (!c || !page || (!out && (flags & TGI_TURN_PAGE_JSON))) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  if (out) memset(out, 0, sizeof *out);
+  tgi_state_pages_t o;
+  const int rc = st_pages_close(c, S, &row, 1, page, strs, strs_len, flags, "tgi_state_page_close", out ? &o : nullptr);
+  if (rc || !out) return rc;
+  out->data = o.page_json;
+  out->len = o.page_json ? o.json_off[1] - 1 : 0;
+  out->kernel_ms = o.kernel_ms;
+  out->gpu_launches = o.gpu_launches;
   return TGI_OK;
 }
 

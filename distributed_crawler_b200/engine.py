@@ -39,7 +39,8 @@ EXPORTED_SYMBOLS = [
     "tgi_combine_flush", "tgi_channel_appends", "tgi_set_zone", "tgi_state_code", "tgi_state_set", "tgi_state_add_layer",
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
-    "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer",
+    "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
+    "tgi_state_pages_end", "tgi_state_pages_close",
 ]
 
 
@@ -120,6 +121,9 @@ def lib() -> C.CDLL:
         L.tgi_state_page_begin.argtypes = [vp, u32, vp, vp, u64, vp, u64, u32, C.POINTER(abi.StateTurnC)]
         L.tgi_state_page_end.argtypes = [vp, u32, i32, vp, u64, C.POINTER(u64)]
         L.tgi_state_page_close.argtypes = [vp, u32, vp, vp, u64, u32, C.POINTER(abi.StateJsonC)]
+        L.tgi_state_pages_begin.argtypes = [vp, vp, u32, vp, vp, u64, vp, u64, vp, u32, C.POINTER(abi.StatePagesC)]
+        L.tgi_state_pages_end.argtypes = [vp, u32, i32, u64, vp, vp, C.POINTER(abi.StateEndC)]
+        L.tgi_state_pages_close.argtypes = [vp, vp, u32, vp, vp, u64, u32, C.POINTER(abi.StatePagesC)]
         L.tgi_state_id_seed.argtypes = [vp, u64]
         L.tgi_state_discover.argtypes = [vp, i32, vp, u32, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         L.tgi_state_next_layer.argtypes = [vp, C.c_int64, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
@@ -716,6 +720,71 @@ class Engine:
         self.state_close_ms = float(out.kernel_ms)
         self.state_close_launches = int(out.gpu_launches)
         return C.string_at(out.data, out.len) if page_json else None
+
+    # --- multi-page turns: the bookkeeping of many channels' pages in one call per step -----------------------------
+    def _st_lines(self, out: abi.StatePagesC) -> list[bytes]:
+        n = int(out.n_pages)
+        off = np.ctypeslib.as_array(out.json_off, (n + 1,)).tolist()
+        lines = C.string_at(out.page_json, off[n]) if off[n] else b""
+        return [lines[off[k]:off[k + 1] - 1] for k in range(n)]  # each value without its '\n'
+
+    def state_pages_begin(self, rows, fetched, pages=None, page_json: bool = False):
+        """state_page_begin of every row in order, in one call: fetched = one list of (chat_id, message_id) pairs per
+        row, pages = None or one state_pack dict per row.  Returns (turn, work, work_off, page_json): work indexes the
+        concatenated fetched keys, page k's owner messages are work[work_off[k]:work_off[k+1]]; page_json is the list of
+        json.Marshal(page) when asked for, else None.  The device time is left in self.state_pages_ms"""
+        rows = np.ascontiguousarray(rows, np.uint32)
+        parts = [np.ascontiguousarray(f, np.int64).reshape(-1, 2) for f in fetched]
+        foff = np.zeros(len(parts) + 1, np.uint64)
+        foff[1:] = np.cumsum([len(f) for f in parts])
+        f = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 2), np.int64))
+        recs = strs = None
+        if pages is not None:
+            from .state_pack import pack_pages
+            if any(p.get("messages") for p in pages):
+                raise ValueError("the pages' message lists come from the fetch")
+            recs, strs, _ = pack_pages(pages, self.state_code, lambda pid, i: i)
+        out = abi.StatePagesC()
+        self._check(lib().tgi_state_pages_begin(
+            self.h, rows.ctypes.data, len(rows), recs.ctypes.data if recs is not None else None,
+            strs.ctypes.data if strs is not None else None, len(strs) if strs is not None else 0,
+            f.ctypes.data if len(f) else None, len(f), foff.ctypes.data, abi.TURN_PAGE_JSON if page_json else 0,
+            C.byref(out)))
+        self.state_pages_ms = float(out.kernel_ms)
+        self.state_pages_launches = int(out.gpu_launches)
+        n = int(out.n_work)
+        work = np.ctypeslib.as_array(out.work, (n,)).copy() if n else np.zeros(0, np.uint32)
+        work_off = np.ctypeslib.as_array(out.work_off, (len(rows) + 1,)).copy()
+        return int(out.turn), work, work_off, self._st_lines(out) if page_json else None
+
+    def state_pages_end(self, turn: int, n_done=None, slot: int = -1, first: int = 0, status=None) -> int:
+        """state_page_end of every page of a turn: n_done = None (every record) or one count per page; the statuses are
+        records [first, first + n_work) of the slot's last Telegram result (slot >= 0) or `status` (abi.ST_* per owner
+        message of the turn, slot < 0); returns the messages appended.  The device time is left in self.state_pages_ms"""
+        st = None if status is None else np.ascontiguousarray(status, np.uint8)
+        nd = None if n_done is None else np.ascontiguousarray(n_done, np.uint64)
+        out = abi.StateEndC()
+        self._check(lib().tgi_state_pages_end(self.h, turn, slot, first, st.ctypes.data if st is not None and len(st) else None,
+                                              nd.ctypes.data if nd is not None else None, C.byref(out)))
+        self.state_pages_ms = float(out.kernel_ms)
+        self.state_pages_launches = int(out.gpu_launches)
+        return int(out.appended)
+
+    def state_pages_close(self, rows, pages, page_json: bool = False):
+        """state_page_close of every row in order with its page (state_pack dicts without messages), in one call;
+        returns the list of json.Marshal(page) when asked for, else None.  The device time is left in
+        self.state_pages_ms"""
+        from .state_pack import pack_pages
+        if any(p.get("messages") for p in pages):
+            raise ValueError("the pages' message lists are the owner views")
+        rows = np.ascontiguousarray(rows, np.uint32)
+        recs, strs, _ = pack_pages(pages, self.state_code, lambda pid, i: i)
+        out = abi.StatePagesC()
+        self._check(lib().tgi_state_pages_close(self.h, rows.ctypes.data, len(rows), recs.ctypes.data, strs.ctypes.data,
+                                                len(strs), abi.TURN_PAGE_JSON if page_json else 0, C.byref(out)))
+        self.state_pages_ms = float(out.kernel_ms)
+        self.state_pages_launches = int(out.gpu_launches)
+        return self._st_lines(out) if page_json else None
 
     # --- snowball discovery: outlinks of processed pages as next-layer pages ---------------------------------------
     def state_id_seed(self, seed: int):

@@ -365,6 +365,34 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return page_json ? std::string_view((const char*)o.data, o.len) : std::string_view();
   }
+  // Multi-page turns: the pages of many channels in one call per step.  Page k's fetched keys are
+  // fetched[2*fetched_off[k] .. 2*fetched_off[k+1]); work indexes the whole fetched array, so the caller packs every
+  // page's work into one batch, runs it, and ends the turn from records [first, first + n_work) of that result.  The
+  // returned arrays stay valid until the next state call.
+  tgi_state_pages_t StatePagesBegin(const std::vector<uint32_t>& rows, const std::vector<int64_t>& fetched,
+                                    const std::vector<uint64_t>& fetched_off, bool page_json,
+                                    const tgi_state_page* pages = nullptr, std::string_view strs = {}) {
+    tgi_state_pages_t t{};
+    if (tgi_state_pages_begin(ctx_, rows.data(), (uint32_t)rows.size(), pages, (const uint8_t*)strs.data(), strs.size(),
+                              fetched.data(), fetched.size() / 2, fetched_off.data(), page_json ? TGI_TURN_PAGE_JSON : 0u,
+                              &t) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return t;
+  }
+  tgi_state_end_t StatePagesEnd(uint32_t turn, int slot, uint64_t first, const std::vector<uint64_t>& n_done = {}) {
+    tgi_state_end_t o{};
+    if (tgi_state_pages_end(ctx_, turn, slot, first, nullptr, n_done.empty() ? nullptr : n_done.data(), &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  tgi_state_pages_t StatePagesClose(const std::vector<uint32_t>& rows, const std::vector<tgi_state_page>& pages,
+                                    std::string_view strs, bool page_json) {
+    tgi_state_pages_t o{};
+    if (tgi_state_pages_close(ctx_, rows.data(), (uint32_t)rows.size(), pages.data(), (const uint8_t*)strs.data(), strs.size(),
+                              page_json ? TGI_TURN_PAGE_JSON : 0u, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Snowball discovery: the outlinks of the slot's Telegram result as next-layer pages.  StateDiscover with
   // TGI_DISCOVER_NOW is the standalone runner's AddLayer per page; without it the candidates wait in the pending list
   // for StateNextLayer, the Dapr runner's layer end.  The returned arrays stay valid until the next state call.

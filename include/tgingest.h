@@ -937,6 +937,64 @@ int tgi_state_page_end(tgi_ctx* ctx, uint32_t turn, int slot, const uint8_t* sta
 int tgi_state_page_close(tgi_ctx* ctx, uint32_t row, const tgi_state_page* page, const uint8_t* strs, uint64_t strs_len,
                          uint32_t flags, tgi_state_json_t* out);
 
+/* Multi-page turns — the bookkeeping of P pages (crawl/runner.go:1132-1211, 1543-1544, dapr/standalone.go:589-609) in
+ * one call per step, so that the pages of a worker's channels share one bulk batch: begin them all, pack every work list
+ * into one batch and run it (TGI_RUN_JSONL_DEVICE keeps the statuses on the device), end them all from that result,
+ * close them all.  For the same flags a call's synchronises, and its launches from P = 2 on, do not depend on P (a
+ * one-page call keeps the one-launch scans); the one-page calls above are its P = 1 case.  The launches still follow the
+ * data in two places: an end launches nothing without a processed record and its view passes only for pages whose row
+ * still holds the turn's view, and a TGI_TURN_PAGE_JSON close of any row without an owner view adds one scan of the
+ * message rows and the render's radix passes, whose number is set by the state's row count.
+ *   Begin    tgi_state_pages_begin = tgi_state_page_begin of rows[0], rows[1], ... in that order, each with its own
+ *            fetched keys fetched[fetched_off[k] .. fetched_off[k+1]) (fetched_off[0] = 0, ascending, fetched_off[P] = n)
+ *            and pages[k] (pages NULL: every row keeps its fields).  One handle covers the P pages.  Page k's owner
+ *            messages are work[work_off[k] .. work_off[k+1]) of out->work[n_work]; work[i] indexes the call's whole
+ *            fetched array, so the caller packs fetched[work[i]] for i = 0 .. n_work-1 as one batch.  Each page's
+ *            equal message ids are matched within the page only.  TGI_TURN_PAGE_JSON: page_json holds
+ *            json.Marshal(page) + '\n' of every page in call order, page k's line being [json_off[k], json_off[k+1]),
+ *            as tgi_state_discover returns its pages.
+ *   End      tgi_state_pages_end = tgi_state_page_end of every page in page order, page k with its first n_done[k]
+ *            records (n_done NULL: all of them).  The turn's n_work records are [first, first + n_work) of the slot's
+ *            last Telegram result, which may hold other records before and after them (slot >= 0), or status[n_work]
+ *            from the host (slot < 0; records past a page's n_done are not read).  The owner views' hits follow the
+ *            close's rules, page by page.  tgi_state_pages_end takes a one-page handle; tgi_state_page_end of a handle
+ *            that covers more than one page is TGI_E_ARG.  out (optional) gets the messages appended, the device time
+ *            and the launches; with out the call waits for its kernels.
+ *   Close    tgi_state_pages_close = tgi_state_page_close of rows[0], rows[1], ... with pages[k] (required), in that
+ *            order.  TGI_TURN_PAGE_JSON: out->page_json / json_off as the begin's.  Closing any row of an open turn
+ *            ends that whole turn: a later end of it is TGI_E_ARG.  out may be NULL without the flag.
+ *   Errors   every check runs before anything changes, so a rejected call leaves the state, the open turns and the
+ *            views unchanged.  TGI_E_ARG: no pages, a row unknown or listed twice, a page whose id is not its row's,
+ *            that carries messages or whose strings lie outside strs, a fetched_off that decreases or does not run
+ *            from 0 to n, unknown flags; an unknown or consumed handle, a slot result that is released, not Telegram
+ *            or shorter than first + n_work, n_done[k] greater than page k's work, no host statuses with slot < 0.
+ *            TGI_E_STATE: a job in flight on the slot.  As with the one-page calls, a timestamp whose year leaves
+ *            [0, 9999] fails a TGI_TURN_PAGE_JSON call after the update (the begin then opens no turn).
+ *            tgi_state_set drops every open turn.  All of out lives until the next state call.                         */
+typedef struct tgi_state_pages_t {
+  uint32_t turn;              /* handle for tgi_state_pages_end (never 0); 0 from a close                         */
+  uint32_t n_pages;
+  uint64_t n_work;            /* owner messages of all pages: the records the loops process                       */
+  const uint32_t* work;       /* [n_work] index into fetched of each owner message's discMessage (pinned)         */
+  const uint64_t* work_off;   /* [n_pages+1] page k's owner messages are [work_off[k], work_off[k+1])             */
+  const uint8_t* page_json;   /* with TGI_TURN_PAGE_JSON: the pages' lines, else NULL (pinned)                     */
+  const uint64_t* json_off;   /* [n_pages+1] page k's line is [json_off[k], json_off[k+1]), its '\n' last          */
+  float kernel_ms;            /* device time of the call's kernels and scans (not the copies between them)        */
+  uint32_t gpu_launches;
+} tgi_state_pages_t;
+int tgi_state_pages_begin(tgi_ctx* ctx, const uint32_t* rows, uint32_t n_pages, const tgi_state_page* pages,
+                          const uint8_t* strs, uint64_t strs_len, const int64_t* fetched, uint64_t n,
+                          const uint64_t* fetched_off, uint32_t flags, tgi_state_pages_t* out);
+typedef struct tgi_state_end_t {
+  uint64_t appended;          /* messages the ends appended                                                       */
+  float kernel_ms;            /* device time of the call's kernels and scans (not the copies between them)        */
+  uint32_t gpu_launches;
+} tgi_state_end_t;
+int tgi_state_pages_end(tgi_ctx* ctx, uint32_t turn, int slot, uint64_t first, const uint8_t* status,
+                        const uint64_t* n_done, tgi_state_end_t* out);
+int tgi_state_pages_close(tgi_ctx* ctx, const uint32_t* rows, uint32_t n_pages, const tgi_state_page* pages,
+                          const uint8_t* strs, uint64_t strs_len, uint32_t flags, tgi_state_pages_t* out);
+
 /* Snowball discovery — the outlinks of processed pages become the next layer's pages (crawl/runner.go:1199-1244 outside
  * random-walk, then standalone/runner.go:835-850 or dapr/standalone.go:612-616, 645-688), read straight from a slot's
  * resident Telegram result: nothing is read back before the dedup, so it works after TGI_RUN_JSONL_DEVICE and
