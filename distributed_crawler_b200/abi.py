@@ -225,6 +225,20 @@ class StateAddedC(C.Structure):  # tgi_state_added_t
                 ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+STATE_NO_BATCH = 0xFFFFFFFF  # tgi_state_pending_edges: a span without edges (the crawler's forced walkback)
+STATE_EDGE = np.dtype([("destination", "u1", (32,)), ("record", "<u8"), ("batch", "<u4"), ("dest_len", "u1"),
+                       ("source_type", "u1"), ("status", "u1"), ("reserved", "u1")])  # tgi_state_edge
+STATE_EDGE_BATCH = np.dtype([("batch_id", "S36"), ("span", "<u4"), ("first_edge", "<u4"),
+                             ("n_edges", "<u4")])  # tgi_state_edge_batch
+assert STATE_EDGE.itemsize == 48 and STATE_EDGE_BATCH.itemsize == 48
+
+
+class StateEdgesC(C.Structure):  # tgi_state_edges_t
+    _fields_ = [("n_candidates", C.c_uint64), ("n_edges", C.c_uint64), ("n_batches", C.c_uint32), ("reserved", C.c_uint32),
+                ("edges", C.c_void_p), ("batches", C.c_void_p), ("span_batch", C.c_void_p), ("kernel_ms", C.c_float),
+                ("gpu_launches", C.c_uint32)]
+
+
 STATE_EXPORT_DAPR, STATE_EXPORT_LOCAL = 0, 1
 STATE_EXPORT_CHUNK_DEFAULT = 100 * 1024 * 1024  # exportChunkSizeBytes (state/daprstate.go:2909)
 

@@ -881,22 +881,121 @@ DEVI void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
   }
 }
 
-// ids n0 .. n0+n-1 of the seed as version-4 uuid strings, 36 bytes each
+// id ctr of the seed in counter domain `domain` (word 2: 0 = pages, 1 = pending-edge batches) as a version-4 uuid
+// string of 36 bytes
+DEVI void st_uuid(uint64_t seed, uint64_t ctr, uint32_t domain, uint8_t* o) {
+  uint32_t c[4] = {(uint32_t)ctr, (uint32_t)(ctr >> 32), domain, 0u};
+  philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+  uint8_t b[16];
+  for (int q = 0; q < 16; q++) b[q] = (uint8_t)(c[q >> 2] >> (8 * (q & 3)));
+  b[6] = (b[6] & 0x0F) | 0x40;
+  b[8] = (b[8] & 0x3F) | 0x80;
+  for (int q = 0, p = 0; q < 16; q++) {
+    if (q == 4 || q == 6 || q == 8 || q == 10) o[p++] = '-';
+    o[p++] = "0123456789abcdef"[b[q] >> 4];
+    o[p++] = "0123456789abcdef"[b[q] & 15];
+  }
+}
+
+// page ids n0 .. n0+n-1 of the seed, 36 bytes each
 __global__ void st_uuid_kernel(uint64_t seed, uint64_t n0, uint64_t n, uint8_t* out) {
-  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t ctr = n0 + k;
-    uint32_t c[4] = {(uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u};
-    philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
-    uint8_t b[16];
-    for (int q = 0; q < 16; q++) b[q] = (uint8_t)(c[q >> 2] >> (8 * (q & 3)));
-    b[6] = (b[6] & 0x0F) | 0x40;
-    b[8] = (b[8] & 0x3F) | 0x80;
-    uint8_t* o = out + 36 * k;
-    for (int q = 0, p = 0; q < 16; q++) {
-      if (q == 4 || q == 6 || q == 8 || q == 10) o[p++] = '-';
-      o[p++] = "0123456789abcdef"[b[q] >> 4];
-      o[p++] = "0123456789abcdef"[b[q] & 15];
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x)
+    st_uuid(seed, n0 + k, 0u, out + 36 * k);
+}
+
+// ---- tandem hand-off (crawl/runner.go:1129, 1229-1306, 1414-1455): every page's pending-edge batch -------------------
+// The candidates of the discovery gather (owner-URL skip, status, n_done), deduplicated per span by st_first_kernel
+// (seenInBatch), then cut by FilterUsername and the invalid set's TTL.  Those two tests depend on the name only, so
+// the first occurrence of a name survives exactly when every occurrence in its span would: the order against the
+// dedup does not change the edges.
+struct StEdges {
+  const StCand* c;           // the gather's candidates in (span, record, link) order
+  const uint32_t* link;      // [bound] the link row in the result of every candidate
+  const uint64_t* coff;      // [n_spans+1] first candidate of every span; coff[n_spans] = the count
+  uint64_t bound;            // threads: at least the count
+  const uint32_t* bfirst;    // st_first_kernel's batch table (per span) and every candidate's slot in it
+  const uint32_t* slot_of;
+  const tgi_state_span* spans;
+  uint32_t n_spans;
+  const uint32_t* link_off;  // the slot's resident result
+  const tgi_link* links;
+  ExclusionDev x;            // TGI_SET_INVALID with the call's clock, TGI_SET_DISCOVERED
+  unsigned long long* n_cand;  // candidates that pass both name tests, before the dedup
+  uint32_t* flag;            // [bound] 1: candidate j is an edge
+  uint64_t* pos;             // [bound+1] scan of flag: the edge's index
+  uint32_t* has;             // [n_spans] 1: the span has an edge
+  uint64_t* bpos;            // [n_spans+1] scan of has: the span's batch
+  uint64_t seed, batch0;     // the id key, and the counter of the call's first batch
+  tgi_state_edge* edges;
+  tgi_state_edge_batch* batches;
+  uint32_t* span_batch;      // [n_spans]
+};
+
+// the link row of every candidate, from the gather's flags and offsets
+__global__ void st_edge_link_kernel(StDisc g, uint32_t* link) {
+  const uint64_t total = g.soff[g.n_spans];
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x)
+    if (g.flag[i]) link[g.pos[i]] = g.lnk[i];
+}
+
+__global__ void st_edge_keep_kernel(StEdges e) {
+  const uint64_t n = e.coff[e.n_spans];
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < e.bound; j += (uint64_t)gridDim.x * blockDim.x) {
+    bool pass = false, f = false;
+    if (j < n) {
+      const StCand& c = e.c[j];
+      const Key32 k = load_key(c.name);
+      pass = (e.links[e.link[j]].flags & TGI_LF_FILTER_OK) && !set_invalid_hit(e.x, k, key_hash(k), e.x.now_sec);  // :1247, :1261
+      f = pass && e.bfirst[e.slot_of[j]] == (uint32_t)j;  // :1267-1272
     }
+    const unsigned am = __activemask(), m = __ballot_sync(am, pass);
+    if (m && (threadIdx.x & 31) == (unsigned)__ffs(am) - 1) atomicAdd(e.n_cand, (unsigned long long)__popc(m));
+    e.flag[j] = f;
+  }
+}
+
+__global__ void st_edge_spans_kernel(StEdges e) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < e.n_spans; k += (uint64_t)gridDim.x * blockDim.x)
+    e.has[k] = e.pos[e.coff[k + 1]] > e.pos[e.coff[k]];
+}
+
+// the edges: destination, the record and source of the name's first occurrence in the page, the validator's discovered
+// look-up (validator.go:214-226); the batches: one per span with an edge (runner.go:1275-1291), in span order
+__global__ void st_edge_emit_kernel(StEdges e) {
+  const uint64_t n = e.coff[e.n_spans];
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!e.flag[j]) continue;
+    const StCand& c = e.c[j];
+    const uint32_t L = e.link[j];
+    const tgi_state_span s = e.spans[c.span];
+    uint64_t a = s.first, b = s.first + s.n_done - 1;  // the record that holds link row L
+    while (a < b) {
+      const uint64_t mid = (a + b + 1) >> 1;
+      if (e.link_off[mid] <= L) a = mid;
+      else b = mid - 1;
+    }
+    const Key32 k = load_key(c.name);
+    tgi_state_edge& o = e.edges[e.pos[j]];
+    store_key(o.destination, k);
+    o.record = a;
+    o.batch = (uint32_t)e.bpos[c.span];
+    o.dest_len = (uint8_t)c.len;
+    o.source_type = e.links[L].src;
+    o.status = set_lookup(e.x.discovered, k, key_hash(k)) >= 0 ? TGI_EDGE_DUPLICATE : TGI_EDGE_PENDING;
+    o.reserved = 0;
+  }
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < e.n_spans; k += (uint64_t)gridDim.x * blockDim.x) {
+    if (!e.has[k]) {
+      e.span_batch[k] = TGI_STATE_NO_BATCH;
+      continue;
+    }
+    const uint64_t q = e.bpos[k], f0 = e.pos[e.coff[k]];
+    e.span_batch[k] = (uint32_t)q;
+    tgi_state_edge_batch& bt = e.batches[q];
+    st_uuid(e.seed, e.batch0 + q, 1u, bt.batch_id);
+    bt.span = (uint32_t)k;
+    bt.first_edge = (uint32_t)f0;
+    bt.n_edges = (uint32_t)(e.pos[e.coff[k + 1]] - f0);
   }
 }
 

@@ -244,6 +244,10 @@ struct CrawlState {
   uint64_t id_seed = 0, id_next = 0;
   bool seeded = false;
   HostBuf h_surv, h_coff, h_ids, h_rows, h_json_off;
+  // tandem hand-off (tgi_state_pending_edges): the batch-id counter (ids under id_seed) and the call's outputs
+  uint64_t batch_next = 0;
+  DevBuf clink, edges, ebatches, span_batch;
+  HostBuf h_edges, h_ebatches, h_span_batch;
 };
 
 struct Slot {
@@ -4914,6 +4918,85 @@ int disc_json_empty(tgi_ctx* c, CrawlState& S, tgi_state_added_t* out) {
   return TGI_OK;
 }
 
+// What the span calls (tgi_state_discover, tgi_state_pending_edges) need of slot s, under its lock: a finished
+// Telegram result with its link rows
+int disc_slot(tgi_ctx* c, const Slot& s, int slot, const char* who) {
+  if (in_flight(s)) { set_err(c, "%s: slot %d is in flight", who, slot); return TGI_E_STATE; }
+  if (!s.busy || s.last.kind == REC_NONE) { set_err(c, "%s: slot %d holds no result (released or none)", who, slot); return TGI_E_STATE; }
+  if (s.last.kind != REC_TG) { set_err(c, "%s: slot %d's result is not a Telegram one", who, slot); return TGI_E_STATE; }
+  if (!s.last.dev.link_off || !s.last.dev.links) { set_err(c, "%s: slot %d's result has no links (run it with TGI_RUN_LINKS)", who, slot); return TGI_E_STATE; }
+  return TGI_OK;
+}
+
+// The spans' checks against slot s's result, and the gather's bound: the result's link rows times the largest number
+// of spans that share a processed record (no read-back)
+int disc_bound(tgi_ctx* c, const CrawlState& S, const Slot& s, const tgi_state_span* spans, uint32_t n_spans,
+               const char* who, uint64_t* bound) {
+  const uint64_t n = s.last.n;
+  std::vector<std::pair<uint64_t, int>> ev;  // the processed records' intervals
+  for (uint32_t k = 0; k < n_spans; k++) {
+    const tgi_state_span& sp = spans[k];
+    if (sp.row >= S.rows.size()) { set_err(c, "%s: span %u: no row %u", who, k, sp.row); return TGI_E_ARG; }
+    if (sp.first > n || sp.n_records > n - sp.first) { set_err(c, "%s: span %u lies outside the result's %llu records", who, k, (unsigned long long)n); return TGI_E_ARG; }
+    if (sp.n_done > sp.n_records) { set_err(c, "%s: span %u: n_done %llu > n_records %llu", who, k, (unsigned long long)sp.n_done, (unsigned long long)sp.n_records); return TGI_E_ARG; }
+    if (sp.n_done) {
+      ev.emplace_back(sp.first, 1);
+      ev.emplace_back(sp.first + sp.n_done, -1);
+    }
+  }
+  std::sort(ev.begin(), ev.end(), [](const auto& a, const auto& b) { return a.first != b.first ? a.first < b.first : a.second < b.second; });
+  int64_t cover = 0, most = 0;
+  for (const auto& e : ev) most = std::max(most, cover += e.second);
+  *bound = (uint64_t)most * s.last.n_links;  // link rows over the spans' processed records, at most
+  return TGI_OK;
+}
+
+// The discovery gather on the state stream, behind the slot's work: the spans' candidates (status, n_done, owner URL)
+// into out in (span, record, link row) order, every span's first candidate in gd.coff (the count at [n_spans]).  The
+// device time runs from S.t0; no synchronise.
+int disc_gather(tgi_ctx* c, CrawlState& S, Slot& s, const tgi_state_span* spans, uint32_t n_spans, uint64_t bound,
+                StCand* out, bool tiled, StDisc& gd, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  CK(S.spans.ensure(n_spans * sizeof(tgi_state_span)));
+  CK(S.cnt.ensure(n_spans * 4));
+  CK(S.soff.ensure((n_spans + 1) * 8));
+  CK(S.coff.ensure((n_spans + 1) * 8));
+  CK(S.lnk.ensure(bound * 4));
+  CK(S.spn.ensure(bound * 4));
+  CK(S.flag.ensure(bound * 4));
+  CK(S.pos.ensure((bound + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  gd = StDisc{};
+  gd.spans = S.spans.as<tgi_state_span>();
+  gd.n_spans = n_spans;
+  gd.status = s.last.dev.status;
+  gd.link_off = s.last.dev.link_off;
+  gd.links = s.last.dev.links;
+  gd.soff = S.soff.as<uint64_t>();
+  gd.bound = bound;
+  gd.flag = S.flag.as<uint32_t>();
+  gd.lnk = S.lnk.as<uint32_t>();
+  gd.spn = S.spn.as<uint32_t>();
+  gd.pos = S.pos.as<uint64_t>();
+  gd.out = out;
+  gd.coff = S.coff.as<uint64_t>();
+  int rc;
+  CK(cudaMemcpyAsync(S.spans.p, spans, n_spans * sizeof(tgi_state_span), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(S.ev_slot, s.stream));  // the result is complete on the slot's stream
+  CK(cudaStreamWaitEvent(st, S.ev_slot, 0));
+  CK(cudaEventRecord(S.t0, st));
+  st_disc_count_kernel<<<st_grid(c, n_spans), ST_THREADS, 0, st>>>(gd, S.cnt.as<uint32_t>());
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, S.cnt.as<uint32_t>(), n_spans, S.soff.as<uint64_t>(), S.sc.as<uint64_t>() + 1, launches, tiled))) return rc;
+  st_disc_flag_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(st_dev(S), gd);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, gd.flag, bound, gd.pos, S.sc.as<uint64_t>() + 2, launches, tiled))) return rc;
+  st_disc_emit_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(gd);
+  launches++;
+  CK(cudaGetLastError());
+  return TGI_OK;
+}
+
 // First occurrences (per span, or over the list) and Dapr's urlCache test over the candidates at d_cands (count d_n on
 // the device, at most bound), compacted into S.surv; the survivors come back to S.h_surv with one id each from counter
 // id_next on (S.h_ids).  Two synchronises: the survivors' count, then their rows and ids.
@@ -5177,77 +5260,27 @@ int tgi_state_discover(tgi_ctx* c, int slot, const tgi_state_span* spans, uint32
   if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
   Slot& s = c->slots[slot];
   std::lock_guard<std::mutex> sl(s.mu);
-  if (in_flight(s)) { set_err(c, "%s: slot %d is in flight", who, slot); return TGI_E_STATE; }
-  if (!s.busy || s.last.kind == REC_NONE) { set_err(c, "%s: slot %d holds no result (released or none)", who, slot); return TGI_E_STATE; }
-  if (s.last.kind != REC_TG) { set_err(c, "%s: slot %d's result is not a Telegram one", who, slot); return TGI_E_STATE; }
-  if (!s.last.dev.link_off || !s.last.dev.links) { set_err(c, "%s: slot %d's result has no links (run it with TGI_RUN_LINKS)", who, slot); return TGI_E_STATE; }
+  int rc;
+  if ((rc = disc_slot(c, s, slot, who))) return rc;
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
-  int rc;
   if ((rc = st_init(c, S))) return rc;
   memset(out, 0, sizeof *out);
   if ((rc = disc_args(c, flags, TGI_DISCOVER_NOW | TGI_DISCOVER_DAPR | TGI_DISCOVER_PAGE_JSON, now_sec, now_nsec, who))) return rc;
   if ((flags & TGI_DISCOVER_PAGE_JSON) && (rc = disc_json_empty(c, S, out))) return rc;
-  const uint64_t n = s.last.n;
-  std::vector<std::pair<uint64_t, int>> ev;  // the processed records' intervals: the gather's bound
-  for (uint32_t k = 0; k < n_spans; k++) {
-    const tgi_state_span& sp = spans[k];
-    if (sp.row >= S.rows.size()) { set_err(c, "%s: span %u: no row %u", who, k, sp.row); return TGI_E_ARG; }
-    if (sp.first > n || sp.n_records > n - sp.first) { set_err(c, "%s: span %u lies outside the result's %llu records", who, k, (unsigned long long)n); return TGI_E_ARG; }
-    if (sp.n_done > sp.n_records) { set_err(c, "%s: span %u: n_done %llu > n_records %llu", who, k, (unsigned long long)sp.n_done, (unsigned long long)sp.n_records); return TGI_E_ARG; }
-    if (sp.n_done) {
-      ev.emplace_back(sp.first, 1);
-      ev.emplace_back(sp.first + sp.n_done, -1);
-    }
-  }
-  std::sort(ev.begin(), ev.end(), [](const auto& a, const auto& b) { return a.first != b.first ? a.first < b.first : a.second < b.second; });
-  int64_t cover = 0, most = 0;
-  for (const auto& e : ev) most = std::max(most, cover += e.second);
-  const uint64_t bound = (uint64_t)most * s.last.n_links;  // link rows over the spans' processed records, at most
+  uint64_t bound = 0;
+  if ((rc = disc_bound(c, S, s, spans, n_spans, who, &bound))) return rc;
   const bool now = flags & TGI_DISCOVER_NOW, dapr = flags & TGI_DISCOVER_DAPR, json = flags & TGI_DISCOVER_PAGE_JSON;
   if (!bound) return TGI_OK;  // no candidate: no AddLayer call, nothing pending
   if (!now && (rc = st_grow(c, S, S.pend, S.n_pend * sizeof(StCand), (S.n_pend + bound) * sizeof(StCand)))) return rc;
   cudaStream_t st = S.stream;
-  CK(S.spans.ensure(n_spans * sizeof(tgi_state_span)));
-  CK(S.cnt.ensure(n_spans * 4));
-  CK(S.soff.ensure((n_spans + 1) * 8));
-  CK(S.coff.ensure((n_spans + 1) * 8));
-  CK(S.lnk.ensure(bound * 4));
-  CK(S.spn.ensure(bound * 4));
-  CK(S.flag.ensure(bound * 4));
-  CK(S.pos.ensure((bound + 1) * 8));
   if (now) CK(S.cand.ensure(bound * sizeof(StCand)));
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
   CK(S.h_coff.ensure((n_spans + 1) * 8));
-  StDisc gd{};
-  gd.spans = S.spans.as<tgi_state_span>();
-  gd.n_spans = n_spans;
-  gd.status = s.last.dev.status;
-  gd.link_off = s.last.dev.link_off;
-  gd.links = s.last.dev.links;
-  gd.soff = S.soff.as<uint64_t>();
-  gd.bound = bound;
-  gd.flag = S.flag.as<uint32_t>();
-  gd.lnk = S.lnk.as<uint32_t>();
-  gd.spn = S.spn.as<uint32_t>();
-  gd.pos = S.pos.as<uint64_t>();
-  gd.out = now ? S.cand.as<StCand>() : S.pend.as<StCand>() + S.n_pend;
-  gd.coff = S.coff.as<uint64_t>();
+  StDisc gd;
   uint32_t launches = 0;
   float ms = 0;
-  CK(cudaMemcpyAsync(S.spans.p, spans, n_spans * sizeof(tgi_state_span), cudaMemcpyHostToDevice, st));
-  CK(cudaEventRecord(S.ev_slot, s.stream));  // the result is complete on the slot's stream
-  CK(cudaStreamWaitEvent(st, S.ev_slot, 0));
-  CK(cudaEventRecord(S.t0, st));
-  st_disc_count_kernel<<<st_grid(c, n_spans), ST_THREADS, 0, st>>>(gd, S.cnt.as<uint32_t>());
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, S.cnt.as<uint32_t>(), n_spans, S.soff.as<uint64_t>(), S.sc.as<uint64_t>() + 1, launches))) return rc;
-  st_disc_flag_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(st_dev(S), gd);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, gd.flag, bound, gd.pos, S.sc.as<uint64_t>() + 2, launches))) return rc;
-  st_disc_emit_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(gd);
-  launches++;
-  CK(cudaGetLastError());
+  if ((rc = disc_gather(c, S, s, spans, n_spans, bound, now ? S.cand.as<StCand>() : S.pend.as<StCand>() + S.n_pend, false,
+                        gd, launches))) return rc;
   CK(cudaEventRecord(S.t1, st));
   CK(cudaMemcpyAsync(S.h_coff.p, gd.coff, (n_spans + 1) * 8, cudaMemcpyDeviceToHost, st));
   const uint64_t* coff = S.h_coff.as<uint64_t>();
@@ -5333,6 +5366,122 @@ int tgi_state_next_layer(tgi_ctx* c, int64_t layer_depth, uint32_t flags, int64_
   if ((rc = st_discover_apply(c, S, G, dapr, json, now_sec, now_nsec, max_pages, who, out, &ms, launches))) return rc;
   S.n_pend = 0;
   out->n_candidates = m;
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The discovery gather, st_first_kernel per span (seenInBatch), the name tests and the keep scan, the per-span batch
+// scan and one kernel for the edges and batches; one synchronise for the totals, one for the read-back.  Lock order: the
+// slot, then the state, then the sets.
+int tgi_state_pending_edges(tgi_ctx* c, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
+                            tgi_state_edges_t* out) {
+  static const char* const who = "tgi_state_pending_edges";
+  if (!c || !out || (n_spans && !spans)) return TGI_E_ARG;
+  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
+  Slot& s = c->slots[slot];
+  std::lock_guard<std::mutex> sl(s.mu);
+  int rc;
+  if ((rc = disc_slot(c, s, slot, who))) return rc;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  uint64_t bound = 0;
+  if ((rc = disc_bound(c, S, s, spans, n_spans, who, &bound))) return rc;
+  CK(S.h_span_batch.ensure(std::max<uint64_t>(n_spans, 1) * 4));
+  out->span_batch = S.h_span_batch.as<uint32_t>();
+  if (!bound) {  // no processed link row: no edge, no batch
+    std::fill_n(S.h_span_batch.as<uint32_t>(), n_spans, TGI_STATE_NO_BATCH);
+    return TGI_OK;
+  }
+  cudaStream_t st = S.stream;
+  const bool tiled = n_spans > 1;  // launches that do not depend on the number of pages
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * bound, 64));
+  CK(S.cand.ensure(bound * sizeof(StCand)));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.slot_of.ensure(bound * 4));
+  CK(S.clink.ensure(bound * 4));
+  CK(S.edges.ensure(bound * sizeof(tgi_state_edge)));
+  CK(S.ebatches.ensure(n_spans * sizeof(tgi_state_edge_batch)));
+  CK(S.span_batch.ensure(n_spans * 4));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  StDisc gd;
+  uint32_t launches = 0;
+  if ((rc = disc_gather(c, S, s, spans, n_spans, bound, S.cand.as<StCand>(), tiled, gd, launches))) return rc;
+  st_edge_link_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(gd, S.clink.as<uint32_t>());
+  launches++;
+  // seenInBatch: the first occurrence of every name within its span
+  StFirst w{};
+  w.c = S.cand.as<StCand>();
+  w.n = gd.coff + n_spans;
+  w.bound = bound;
+  w.per_span = true;
+  w.dedup = true;
+  w.bfirst = S.bfirst.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.slot_of.as<uint32_t>();
+  CK(cudaMemsetAsync(w.bfirst, 0xFF, bslots * 4, st));
+  st_first_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(w);
+  launches++;
+  // the gather is done with its flags, offsets and counts: the edges' keep flags and scans reuse them
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [3] candidates, [4] edges, [5] batches
+  StEdges e{};
+  e.c = S.cand.as<StCand>();
+  e.link = S.clink.as<uint32_t>();
+  e.coff = gd.coff;
+  e.bound = bound;
+  e.bfirst = w.bfirst;
+  e.slot_of = w.slot_of;
+  e.spans = gd.spans;
+  e.n_spans = n_spans;
+  e.link_off = gd.link_off;
+  e.links = gd.links;
+  e.n_cand = (unsigned long long*)(dsc + 3);
+  e.flag = gd.flag;
+  e.pos = gd.pos;
+  e.has = S.cnt.as<uint32_t>();
+  e.bpos = S.soff.as<uint64_t>();
+  e.seed = S.id_seed;
+  e.batch0 = S.batch_next;
+  e.edges = S.edges.as<tgi_state_edge>();
+  e.batches = S.ebatches.as<tgi_state_edge_batch>();
+  e.span_batch = S.span_batch.as<uint32_t>();
+  CK(cudaMemsetAsync(dsc + 3, 0, 8, st));
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);  // the exclusion sets: probed by the kernels below, not changed
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    e.x = exclusion(c, now_sec);
+    st_edge_keep_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(e);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, e.flag, bound, e.pos, dsc + 4, launches, tiled))) return rc;
+    st_edge_spans_kernel<<<st_grid(c, n_spans), ST_THREADS, 0, st>>>(e);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, e.has, n_spans, e.bpos, dsc + 5, launches, tiled))) return rc;
+    st_edge_emit_kernel<<<st_grid(c, std::max<uint64_t>(bound, n_spans)), ST_THREADS, 0, st>>>(e);
+    launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t1, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  const uint64_t* hs = S.h_sc.as<uint64_t>();
+  const uint64_t n_edges = hs[4], n_batches = hs[5];
+  if (n_batches && !S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
+  float ms = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  CK(S.h_edges.ensure(std::max<uint64_t>(n_edges, 1) * sizeof(tgi_state_edge)));
+  CK(S.h_ebatches.ensure(std::max<uint64_t>(n_batches, 1) * sizeof(tgi_state_edge_batch)));
+  if (n_edges) CK(cudaMemcpyAsync(S.h_edges.p, S.edges.p, n_edges * sizeof(tgi_state_edge), cudaMemcpyDeviceToHost, st));
+  if (n_batches) CK(cudaMemcpyAsync(S.h_ebatches.p, S.ebatches.p, n_batches * sizeof(tgi_state_edge_batch), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_span_batch.p, S.span_batch.p, n_spans * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  S.batch_next += n_batches;
+  out->n_candidates = hs[3];
+  out->n_edges = n_edges;
+  out->n_batches = (uint32_t)n_batches;
+  out->edges = S.h_edges.as<tgi_state_edge>();
+  out->batches = S.h_ebatches.as<tgi_state_edge_batch>();
   out->kernel_ms = ms;
   out->gpu_launches = launches;
   return TGI_OK;

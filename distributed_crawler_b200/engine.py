@@ -40,7 +40,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
-    "tgi_state_pages_end", "tgi_state_pages_close",
+    "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges",
 ]
 
 
@@ -127,6 +127,7 @@ def lib() -> C.CDLL:
         L.tgi_state_id_seed.argtypes = [vp, u64]
         L.tgi_state_discover.argtypes = [vp, i32, vp, u32, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         L.tgi_state_next_layer.argtypes = [vp, C.c_int64, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
+        L.tgi_state_pending_edges.argtypes = [vp, i32, vp, u32, C.c_int64, C.POINTER(abi.StateEdgesC)]
         _LIB = L
     return _LIB
 
@@ -825,6 +826,24 @@ class Engine:
         out = abi.StateAddedC()
         self._check(lib().tgi_state_next_layer(self.h, layer_depth, flags, now[0], now[1], max_pages, C.byref(out)))
         return self._st_added(out, bool(flags & abi.DISCOVER_PAGE_JSON))
+
+    # --- tandem hand-off: every page's pending-edge batch --------------------------------------------------------
+    def state_pending_edges(self, slot: int, spans, now_sec: int = 0) -> dict:
+        """the pending edges of the slot's last Telegram result, deduplicated per page: spans = (row, first, n_records,
+        n_done) per owner page, now_sec = the clock of the invalid set's TTL.  Returns {"edges" (abi.STATE_EDGE rows),
+        "batches" (abi.STATE_EDGE_BATCH rows), "span_batch" (per span, abi.STATE_NO_BATCH without edges),
+        "n_candidates"}.  The device time is left in self.state_edges_ms"""
+        sp = np.zeros(max(len(spans), 1), abi.STATE_SPAN)
+        for k, (row, first, n_records, n_done) in enumerate(spans):
+            sp[k] = (row, 0, first, n_records, n_done)
+        out = abi.StateEdgesC()
+        self._check(lib().tgi_state_pending_edges(self.h, slot, sp.ctypes.data, len(spans), now_sec, C.byref(out)))
+        self.state_edges_ms = float(out.kernel_ms)
+        self.state_edges_launches = int(out.gpu_launches)
+        return {"edges": _view(out.edges, int(out.n_edges), abi.STATE_EDGE).copy(),
+                "batches": _view(out.batches, int(out.n_batches), abi.STATE_EDGE_BATCH).copy(),
+                "span_batch": _view(out.span_batch, len(spans), np.uint32).copy(),
+                "n_candidates": int(out.n_candidates)}
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

@@ -412,6 +412,15 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return a;
   }
+  // Tandem hand-off: every span's pending-edge batch from the slot's Telegram result, seenInBatch per page; a span with
+  // span_batch[k] == TGI_STATE_NO_BATCH made no batch (the forced walkback).  The arrays stay valid until the next
+  // state call.
+  tgi_state_edges_t StatePendingEdges(int slot, const std::vector<tgi_state_span>& spans, int64_t now_sec) {
+    tgi_state_edges_t a{};
+    if (tgi_state_pending_edges(ctx_, slot, spans.data(), (uint32_t)spans.size(), now_sec, &a) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return a;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

@@ -1070,6 +1070,63 @@ int tgi_state_discover(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint
 int tgi_state_next_layer(tgi_ctx* ctx, int64_t layer_depth, uint32_t flags, int64_t now_sec, int32_t now_nsec,
                          int64_t max_pages, tgi_state_added_t* out);
 
+/* Tandem hand-off — the random-walk tandem branch of processAllMessagesWithProcessor (crawl/runner.go:1129, 1229-1306,
+ * 1414-1455): every page's pending-edge batch for the validator, read straight from a slot's resident Telegram result,
+ * with seenInBatch per page.  tgi_pending_edges stays the single-batch form, deduplicated by the global set.
+ *   Spans    as tgi_state_discover's: the owner row, its records [first, first + n_records) of the slot's last result,
+ *            the first n_done of them processed.  Spans may share records.
+ *   Candidates  every link row of a processed record whose status is TGI_ST_EMITTED or TGI_ST_NOLINE, except names
+ *            byte-equal to the owner row's URL at the call (`o == owner.URL`), names FilterUsername refuses
+ *            (tgi_link.flags without TGI_LF_FILTER_OK) and names in TGI_SET_INVALID still live at now_sec (the TTL
+ *            predicate of TGI_RUN_SKIP_INVALID; an empty or unallocated set drops nothing).  The run flags FILTER /
+ *            SKIP_SELF / SKIP_INVALID / FRONTIER play no part; the result needs TGI_RUN_LINKS only.
+ *   Edges    per span, the first occurrence of every candidate name in (record, link row) order (seenInBatch), with the
+ *            record and source_type of that occurrence; status TGI_EDGE_DUPLICATE for a name in TGI_SET_DISCOVERED,
+ *            else TGI_EDGE_PENDING (the validator's cache look-ups; invalid names were dropped).  Edge order is (span,
+ *            record, link row): Go ranges over a per-message map, so every order inside a message is valid.
+ *   Batches  one per span with at least one edge, in span order: PendingEdgeBatch{SourceChannel: owner.URL,
+ *            SourcePageID: owner.ID, SourceDepth: owner.Depth, SequenceID: owner.SequenceID} of row spans[span].row.
+ *            A span without edges has span_batch = TGI_STATE_NO_BATCH: the crawler's forced walkback.  The n-th batch
+ *            made under the context takes the id of tgi_state_discover's page ids with counter (n_lo, n_hi, 1, 0): word
+ *            2 = 1 keeps batch ids apart from page ids under one seed.  n counts batches only, and tgi_state_set does
+ *            not reset it.  Without tgi_state_id_seed a call that would make a batch is TGI_E_STATE.
+ *   Cost     scratch is sized as tgi_state_discover's, without a read-back: pass all spans of one result in one call.
+ *            One synchronise for the totals, one for the read-back; from n_spans = 2 on the launches do not depend on
+ *            n_spans.
+ *   Errors   every check runs before anything changes; a rejected call leaves the state, the sets and the batch counter
+ *            as they were, and a successful one changes only the batch counter.  TGI_E_ARG: an unknown row, a span
+ *            outside the result, n_done > n_records.  TGI_E_STATE: no, a released or a non-Telegram result, a result
+ *            run without TGI_RUN_LINKS, a job in flight on the slot, no seed while a batch is due.  Lock order: the
+ *            slot, then the state.  All of out lives until the next state call.                                        */
+#define TGI_STATE_NO_BATCH 0xFFFFFFFFu
+typedef struct tgi_state_edge {        /* 48 bytes: one pending_edges row                                              */
+  uint8_t destination[32];             /* destination_channel, lower-cased, zero padded                               */
+  uint64_t record;                     /* the result record of its first occurrence in the page                       */
+  uint32_t batch;                      /* index into batches                                                          */
+  uint8_t dest_len;
+  uint8_t source_type;                 /* TGI_SRC_*                                                                   */
+  uint8_t status;                      /* TGI_EDGE_PENDING | TGI_EDGE_DUPLICATE                                       */
+  uint8_t reserved;
+} tgi_state_edge;
+typedef struct tgi_state_edge_batch {  /* 48 bytes: one pending_edge_batches row                                      */
+  uint8_t batch_id[36];                /* version-4 uuid string                                                       */
+  uint32_t span;                       /* owner = spans[span].row: source_channel / _page_id / _depth, sequence_id   */
+  uint32_t first_edge, n_edges;        /* its edges are edges[first_edge .. first_edge + n_edges)                     */
+} tgi_state_edge_batch;
+typedef struct tgi_state_edges_t {
+  uint64_t n_candidates;               /* candidates before seenInBatch                                               */
+  uint64_t n_edges;
+  uint32_t n_batches;
+  uint32_t reserved;
+  const tgi_state_edge* edges;         /* [n_edges] (pinned)                                                          */
+  const tgi_state_edge_batch* batches; /* [n_batches] (pinned)                                                        */
+  const uint32_t* span_batch;          /* [n_spans] batch index of every span, or TGI_STATE_NO_BATCH (pinned)         */
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies between them)   */
+  uint32_t gpu_launches;
+} tgi_state_edges_t;
+int tgi_state_pending_edges(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
+                            tgi_state_edges_t* out);
+
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
                          uint8_t* reason);
