@@ -383,6 +383,9 @@ void trace_slot(const Slot& s, const char* what) {
     }                                                                                   \
   } while (0)
 
+// the nanoseconds of a time.Time: every entry point that takes a (sec, nsec) time refuses anything else (TGI_E_ARG)
+bool nsec_ok(int32_t nsec) { return nsec >= 0 && nsec < 1000000000; }
+
 // ---- host-side rendering of the injected clock (same rules as render_time on the device) --------
 int host_render_time(char* dst, int64_t sec, int32_t nsec, int32_t tz) {
   int64_t t = sec + tz;
@@ -1442,20 +1445,33 @@ int upload_yt(tgi_ctx* c, Slot& s, const tgi_yt_batch* in) {
   if (!in) { set_err(c, "null batch"); return TGI_E_ARG; }
   if (in->n && (!in->recs || !in->chans)) { set_err(c, "youtube batch: recs/chans must be non-null"); return TGI_E_ARG; }
   if (in->n >= (1ull << 40)) { set_err(c, "youtube batch: too many records"); return TGI_E_ARG; }
-  {  // every offset the kernels will follow stays inside its array (O(n) on the host: 80-byte records, no side arrays)
+  {  // every offset the kernels will follow stays inside its array (O(n) on the host: 80-byte records, no side arrays), and
+     // every time is a time.Time's (0 <= nsec < 1e9)
     int e = 0;
+    uint64_t bad_rec = 0;
+    uint32_t bad_chan = 0;
     for (uint64_t i = 0; i < in->n; i++) {
       const tgi_yt_rec& r = in->recs[i];
       uint64_t end = r.str_off + (uint64_t)r.id_len + r.title_len + r.desc_len + r.duration_len + r.lang_len;
       for (int k = 0; k < 5; k++) end += r.thumb_len[k] == TGI_YT_THUMB_ABSENT ? 0u : r.thumb_len[k];
       if (end > in->strs_len || end < r.str_off) e |= 1;
       if (r.chan_idx >= in->n_chans) e |= 2;
+      if (!nsec_ok(r.published_nsec)) {
+        if (!(e & 4)) bad_rec = i;
+        e |= 4;
+      }
     }
     for (uint32_t i = 0; i < in->n_chans; i++) {
       const tgi_yt_chan& ch = in->chans[i];
       if ((uint64_t)ch.str_off + ch.id_len + ch.title_len + ch.desc_len + ch.thumb_len + ch.country_len > in->chan_strs_len) e |= 512;
+      if (!nsec_ok(ch.published_nsec)) {
+        if (!(e & 1024)) bad_chan = i;
+        e |= 1024;
+      }
     }
-    if (e) { set_err(c, "youtube batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
+    if (e & ~(4 | 1024)) { set_err(c, "youtube batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
+    if (e & 4) { set_err(c, "youtube batch: published_nsec %d of video %llu is outside [0, 1e9)", in->recs[bad_rec].published_nsec, (unsigned long long)bad_rec); return TGI_E_ARG; }
+    if (e) { set_err(c, "youtube batch: published_nsec %d of channel %u is outside [0, 1e9)", in->chans[bad_chan].published_nsec, bad_chan); return TGI_E_ARG; }
   }
   s.in_bytes = 0;
   InArrays a;
@@ -1558,17 +1574,23 @@ int upload_gm(tgi_ctx* c, Slot& s, const tgi_gm_batch* in) {
   if (!in) { set_err(c, "null batch"); return TGI_E_ARG; }
   if (in->n && !in->recs) { set_err(c, "generic batch: recs must be non-null"); return TGI_E_ARG; }
   if (in->n >= (1ull << 40)) { set_err(c, "generic batch: too many records"); return TGI_E_ARG; }
-  {
+  {  // offsets inside their arrays, and GetTimestamp() a time.Time (0 <= nsec < 1e9)
     int e = 0;
+    uint64_t bad = 0;
     for (uint64_t i = 0; i < in->n; i++) {
       const tgi_gm_rec& r = in->recs[i];
       const uint64_t end = r.str_off + (uint64_t)r.id_len + r.channel_len + r.text_len + r.sender_len;
       if (end > in->strs_len || end < r.str_off) e |= 1;
       if (in->react_off && (in->react_off[i] > in->react_off[i + 1] || in->react_off[i + 1] > in->n_reacts)) e |= 8;
+      if (!nsec_ok(r.ts_nsec)) {
+        if (!(e & 16)) bad = i;
+        e |= 16;
+      }
     }
     for (uint64_t i = 0; i < in->n_reacts; i++)
       if ((uint64_t)in->reacts[i].key_off + in->reacts[i].key_len > in->aux_len) e |= 64;
-    if (e) { set_err(c, "generic batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
+    if (e & ~16) { set_err(c, "generic batch: offsets outside their arrays (mask 0x%x)", e); return TGI_E_ARG; }
+    if (e) { set_err(c, "generic batch: ts_nsec %d of record %llu is outside [0, 1e9)", in->recs[bad].ts_nsec, (unsigned long long)bad); return TGI_E_ARG; }
   }
   const uint64_t n = in->n;
   s.in_bytes = 0;
@@ -1911,6 +1933,11 @@ int tgi_create(const tgi_config* cfg, tgi_ctx** out) {
   tgi_ctx* c = nullptr;
   if (!cfg || !out) { set_err(nullptr, "null argument"); return TGI_E_ARG; }
   if (cfg->abi_version != TGI_ABI_VERSION) { set_err(nullptr, "ABI version mismatch: library %d, caller %u", TGI_ABI_VERSION, cfg->abi_version); return TGI_E_ARG; }
+  if (!nsec_ok(cfg->created_at_nsec) || !nsec_ok(cfg->capture_nsec)) {
+    set_err(nullptr, "created_at_nsec %d / capture_nsec %d: outside [0, 1e9)", cfg->created_at_nsec, cfg->capture_nsec);
+    return TGI_E_ARG;
+  }
+  if (cfg->tz_offset_sec <= -86400 || cfg->tz_offset_sec >= 86400) { set_err(nullptr, "tz_offset_sec %d is a day or more", cfg->tz_offset_sec); return TGI_E_ARG; }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     set_err(nullptr, "no CUDA device visible: libtgingest has no CPU fallback");
@@ -2012,6 +2039,10 @@ void tgi_get_stats(tgi_ctx* c, tgi_stats* out) {
 
 int tgi_set_clock(tgi_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec, int32_t capture_nsec) {
   if (!c) return TGI_E_ARG;
+  if (!nsec_ok(created_at_nsec) || !nsec_ok(capture_nsec)) {  // the previous clock stays in effect
+    set_err(c, "tgi_set_clock: created_at_nsec %d / capture_nsec %d: outside [0, 1e9)", created_at_nsec, capture_nsec);
+    return TGI_E_ARG;
+  }
   cudaSetDevice(c->device);
   if (const int i = slot_in_flight(c); i >= 0) { set_err(c, "tgi_set_clock while slot %d is in flight", i); return TGI_E_STATE; }
   std::lock_guard<std::mutex> g(c->cfg_mu);

@@ -260,7 +260,7 @@ class MessageProcessor {
     return Result(ctx_, r);
   }
   void SetClock(int64_t created_sec, int32_t created_nsec, int64_t capture_sec, int32_t capture_nsec) {
-    tgi_set_clock(ctx_, created_sec, created_nsec, capture_sec, capture_nsec);
+    if (tgi_set_clock(ctx_, created_sec, created_nsec, capture_sec, capture_nsec) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
   }
   // time.Local as transitions (tgi_set_zone): instant t takes offset_sec[i] of the last start_sec[i] <= t; empty
   // vectors go back to Config::TzOffsetSec.

@@ -197,7 +197,7 @@ typedef struct tgi_yt_rec { /* 80 bytes, 16-byte aligned */
   uint16_t lang_len;
   uint16_t thumb_len[5]; /* default, medium, high, standard, maxres; TGI_YT_THUMB_ABSENT = no key */
   uint16_t reserved;
-  int32_t published_nsec;
+  int32_t published_nsec; /* 0 <= nsec < 1e9, as Time.Nanosecond(); anything else: the batch is TGI_E_ARG   */
   uint64_t reserved2;
 } tgi_yt_rec;
 
@@ -212,7 +212,7 @@ typedef struct tgi_yt_chan { /* 64 bytes; cached == 0 -> fallback branch youtube
   int64_t view_count;
   int64_t video_count;
   int64_t published_sec;
-  int32_t published_nsec;
+  int32_t published_nsec; /* 0 <= nsec < 1e9, as Time.Nanosecond(); anything else: the batch is TGI_E_ARG   */
   uint8_t cached;
   uint8_t reserved[11];
 } tgi_yt_chan;
@@ -249,7 +249,7 @@ typedef struct tgi_gm_rec { /* 48 bytes */
   uint64_t str_off;   /* in `strs`: id | channel_id | text | sender_name                            */
   int64_t ts_sec;     /* GetTimestamp(): time.Unix(sec, nsec) shown in the context's zone           */
   int64_t views;      /* GetViews()                                                                  */
-  int32_t ts_nsec;
+  int32_t ts_nsec;    /* 0 <= ts_nsec < 1e9, as Time.Nanosecond(); anything else: the batch is TGI_E_ARG */
   uint32_t text_len;
   uint16_t id_len;
   uint16_t channel_len;
@@ -280,13 +280,13 @@ typedef struct tgi_config {
   uint32_t abi_version;    /* TGI_ABI_VERSION                                                     */
   int32_t device;          /* CUDA ordinal                                                        */
   uint32_t flags;          /* TGI_CFG_*                                                           */
-  int32_t tz_offset_sec;   /* fixed offset of the process-local zone (time.Unix -> Local)         */
+  int32_t tz_offset_sec;   /* fixed offset of the process-local zone (time.Unix -> Local); |offset| < 86400 */
   int64_t min_post_date;   /* unix seconds                                                        */
   int64_t created_at_sec;  /* injected time.Now(): Telegram uses .UTC().Truncate(time.Second)
                               (tdutils.go:611); YouTube keeps zone + nanoseconds (youtube_crawler.go:704) */
   int64_t capture_sec;     /* injected time.Now() (tdutils.go:715, youtube_crawler.go:769)        */
-  int32_t capture_nsec;
-  int32_t created_at_nsec;
+  int32_t capture_nsec;    /* 0 <= nsec < 1e9 (both), as Time.Nanosecond()                       */
+  int32_t created_at_nsec; /* tgi_create refuses anything else, and |tz_offset_sec| >= 86400, with TGI_E_ARG */
   uint32_t crawl_label_len;
   uint32_t reserved;
   const char* crawl_label; /* Post.CrawlLabel as the sink would see it (daprstate.go:1113-1115)   */
@@ -359,7 +359,8 @@ void tgi_destroy(tgi_ctx* ctx);
 const char* tgi_last_error(tgi_ctx* ctx); /* ctx may be NULL: last create error                   */
 void tgi_get_stats(tgi_ctx* ctx, tgi_stats* out);
 /* injected clock can change per channel batch (tdutils.go:611,715 call time.Now per message).    */
-/* must not be called while a job is in flight on any slot (returns TGI_E_STATE)                  */
+/* must not be called while a job is in flight on any slot (returns TGI_E_STATE).  0 <= nsec < 1e9  */
+/* for both, else TGI_E_ARG; a rejected call leaves the previous clock in effect.                  */
 int tgi_set_clock(tgi_ctx* ctx, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec,
                   int32_t capture_nsec);
 

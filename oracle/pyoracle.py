@@ -39,8 +39,7 @@ def lib() -> C.CDLL:
     global _LIB
     if _LIB is None:
         L = C.CDLL(build())
-        L.orc_create.restype = C.c_void_p
-        L.orc_create.argtypes = [C.POINTER(abi.ConfigC)]
+        L.orc_create.argtypes = [C.POINTER(abi.ConfigC), C.POINTER(C.c_void_p)]
         L.orc_destroy.argtypes = [C.c_void_p]
         L.orc_set_clock.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32]
         L.orc_telegram_batch.argtypes = [C.c_void_p, C.POINTER(abi.TgBatchC), C.c_uint32, C.c_int,
@@ -108,23 +107,41 @@ def result_from_c(r) -> Result:
                   _copy(r.links, int(r.n_links), abi.LINK), int(r.n_new), int(r.frontier_size))
 
 
+class OracleError(RuntimeError):
+    """a call the library refuses with the same code (abi.E_ARG)"""
+
+    def __init__(self, code: int, what: str):
+        super().__init__(f"{what}: {code}")
+        self.code = code
+
+
+def _check(rc: int, what: str):
+    if rc != 0:
+        raise OracleError(rc, what)
+
+
 class Oracle:
     def __init__(self, cfg: abi.ConfigC | None = None, **kw):
         self.cfg = cfg or abi.make_config(**kw)
-        self.h = lib().orc_create(C.byref(self.cfg))
+        self.h = None
+        h = C.c_void_p()
+        _check(lib().orc_create(C.byref(self.cfg), C.byref(h)), "orc_create")
+        self.h = h.value
 
     def close(self):
-        if self.h:
+        if getattr(self, "h", None):
             lib().orc_destroy(self.h)
             self.h = None
 
     __del__ = close
 
+    def set_clock(self, created_at_sec, created_at_nsec, capture_sec, capture_nsec):
+        _check(lib().orc_set_clock(self.h, created_at_sec, created_at_nsec, capture_sec, capture_nsec), "orc_set_clock")
+
     def telegram(self, batch, run_flags=abi.RUN_JSONL | abi.RUN_LINKS, nthreads=1, copy=True):
         d = batch.descriptor()
         r = OrcResultC()
-        rc = lib().orc_telegram_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r))
-        assert rc == 0
+        _check(lib().orc_telegram_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r)), "orc_telegram_batch")
         out = result_from_c(r) if copy else (int(r.n), int(r.jsonl_len), int(r.n_links))
         self._last = (r, batch)  # the arrays stay valid until the next batch call (pending_edges reads them)
         return out
@@ -149,8 +166,7 @@ class Oracle:
     def youtube(self, batch, run_flags=abi.RUN_JSONL | abi.RUN_LINKS, nthreads=1, copy=True):
         d = batch.descriptor()
         r = OrcResultC()
-        rc = lib().orc_youtube_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r))
-        assert rc == 0
+        _check(lib().orc_youtube_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r)), "orc_youtube_batch")
         out = result_from_c(r) if copy else (int(r.n), int(r.jsonl_len), int(r.n_links))
         lib().orc_result_free(C.byref(r))
         return out
@@ -166,8 +182,7 @@ class Oracle:
     def generic(self, batch, run_flags=abi.RUN_JSONL, nthreads=1, copy=True):
         d = batch.descriptor()
         r = OrcResultC()
-        rc = lib().orc_generic_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r))
-        assert rc == 0
+        _check(lib().orc_generic_batch(self.h, C.byref(d), run_flags, nthreads, C.byref(r)), "orc_generic_batch")
         out = result_from_c(r) if copy else (int(r.n), int(r.jsonl_len), int(r.n_links))
         lib().orc_result_free(C.byref(r))
         return out

@@ -539,13 +539,21 @@ struct orc_ctx {
   buf_t r_status, r_jsonl, r_line_off, r_link_off, r_links;
 };
 
-orc_ctx* orc_create(const tgi_config* cfg) {
+/* time.Time's nanoseconds, and time.FixedZone offsets under a day: what tgi_create / tgi_set_clock and the batch
+ * uploads of the library accept (anything else is TGI_E_ARG there and here) */
+static int nsec_ok(int32_t nsec) { return nsec >= 0 && nsec < 1000000000; }
+
+int orc_create(const tgi_config* cfg, orc_ctx** out) {
+  *out = NULL;
+  if (!nsec_ok(cfg->created_at_nsec) || !nsec_ok(cfg->capture_nsec)) return TGI_E_ARG;
+  if (cfg->tz_offset_sec <= -86400 || cfg->tz_offset_sec >= 86400) return TGI_E_ARG;
   orc_ctx* c = (orc_ctx*)calloc(1, sizeof(*c));
   c->cfg = *cfg;
   c->label = (char*)malloc(cfg->crawl_label_len + 1);
   if (cfg->crawl_label_len) memcpy(c->label, cfg->crawl_label, cfg->crawl_label_len);
   c->cfg.crawl_label = c->label;
-  return c;
+  *out = c;
+  return TGI_OK;
 }
 void orc_destroy(orc_ctx* c) {
   if (!c) return;
@@ -562,11 +570,13 @@ void orc_destroy(orc_ctx* c) {
   for (int i = 0; i < 2; i++) { free(c->xset[i].keys); free(c->xset[i].seq); free(c->xset[i].slots); }
   free(c);
 }
-void orc_set_clock(orc_ctx* c, int64_t cs, int32_t cn, int64_t ps, int32_t pn) {
+int orc_set_clock(orc_ctx* c, int64_t cs, int32_t cn, int64_t ps, int32_t pn) {
+  if (!nsec_ok(cn) || !nsec_ok(pn)) return TGI_E_ARG; /* the previous clock stays */
   c->cfg.created_at_sec = cs;
   c->cfg.created_at_nsec = cn;
   c->cfg.capture_sec = ps;
   c->cfg.capture_nsec = pn;
+  return TGI_OK;
 }
 int orc_frontier_insert(orc_ctx* c, const uint8_t* keys32, uint64_t n, uint8_t* is_new) {
   for (uint64_t i = 0; i < n; i++) {
@@ -1373,6 +1383,10 @@ int orc_telegram_batch(orc_ctx* c, const tgi_tg_batch* in, uint32_t run_flags, i
 }
 int orc_youtube_batch(orc_ctx* c, const tgi_yt_batch* in, uint32_t run_flags, int nthreads,
                       orc_result* out) {
+  for (uint64_t i = 0; i < in->n; i++)
+    if (!nsec_ok(in->recs[i].published_nsec)) return TGI_E_ARG;
+  for (uint32_t i = 0; i < in->n_chans; i++)
+    if (!nsec_ok(in->chans[i].published_nsec)) return TGI_E_ARG;
   return run_batch(c, NULL, in, NULL, run_flags, nthreads, out);
 }
 /* crawl/runner.go:1580-1584,1667-1671 build map["%d_%d"]bool and :1171-1176 scans linearly; both are "is / where is
@@ -1404,6 +1418,8 @@ void orc_key_join(const int64_t* a, uint64_t na, const int64_t* b, uint64_t nb, 
 }
 
 int orc_generic_batch(orc_ctx* c, const tgi_gm_batch* in, uint32_t run_flags, int nthreads, orc_result* out) {
+  for (uint64_t i = 0; i < in->n; i++)
+    if (!nsec_ok(in->recs[i].ts_nsec)) return TGI_E_ARG;
   return run_batch(c, NULL, NULL, in, run_flags, nthreads, out);
 }
 void orc_result_free(orc_result* r) { /* arrays are context-owned; valid until the next batch call */

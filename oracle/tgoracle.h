@@ -40,10 +40,13 @@ typedef struct orc_result { /* arrays are owned by the orc_ctx, valid until its 
   uint64_t frontier_size;
 } orc_result;
 
-orc_ctx* orc_create(const tgi_config* cfg);
+/* TGI_E_ARG (and *out = NULL) for a configuration tgi_create refuses: a clock nsec outside [0, 1e9), |tz_offset_sec| >=
+ * 86400.  TGI_E_ARG from orc_set_clock (the previous clock stays) and from the batch calls (nothing is run) for an nsec
+ * outside [0, 1e9), as the library's tgi_set_clock and batch uploads.                                                  */
+int orc_create(const tgi_config* cfg, orc_ctx** out);
 void orc_destroy(orc_ctx* c);
-void orc_set_clock(orc_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec,
-                   int32_t capture_nsec);
+int orc_set_clock(orc_ctx* c, int64_t created_at_sec, int32_t created_at_nsec, int64_t capture_sec,
+                  int32_t capture_nsec);
 
 /* oracle-only run flags (beside TGI_RUN_*): how the timed CPU arm is run */
 #define ORC_RUN_SLICES 0x10000u /* leave the lines in the worker threads' own buffers (result.jsonl == NULL, jsonl_len and

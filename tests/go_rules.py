@@ -4,6 +4,7 @@ cross-checked by a second implementation.  Pure-Python loops: small inputs only.
 from __future__ import annotations
 
 import datetime as _dt
+import functools
 import re
 
 
@@ -25,10 +26,18 @@ def go_decode_rune(b: bytes, i: int):
     return 0xFFFD, 1
 
 
+_PLAIN = re.compile(rb'[\x20\x21\x23-\x25\x27-\x3b\x3d\x3f-\x5b\x5d-\x7f]+')  # ASCII that encoding/json copies as is
+
+
 def go_json_string(b: bytes) -> bytes:
     out = bytearray(b'"')
     i = 0
     while i < len(b):
+        m = _PLAIN.match(b, i)
+        if m:  # a run of bytes copied unchanged (long texts: one slice instead of a loop per byte)
+            out += m.group()
+            i = m.end()
+            continue
         c = b[i]
         if c < 0x80:
             if c >= 0x20 and c not in b'"\\<>&':
@@ -173,6 +182,12 @@ class _Raw(bytes):
     """already JSON"""
 
 
+@functools.lru_cache(maxsize=None)
+def _json_key(k: str) -> bytes:
+    """a struct field's JSON key (a fixed set of names)"""
+    return go_json_string(k.encode()) + b":"
+
+
 def _marshal(v) -> bytes:
     if isinstance(v, _Raw):
         return bytes(v)
@@ -188,7 +203,7 @@ def _marshal(v) -> bytes:
         return b"{" + b",".join(go_json_string(k) + b":" + _marshal(v[k]) for k in sorted(v)) + b"}"
     if isinstance(v, list):
         if v and isinstance(v[0], tuple) and len(v[0]) == 2 and isinstance(v[0][0], str):  # struct: [(json key, value)]
-            return b"{" + b",".join(go_json_string(k.encode()) + b":" + _marshal(x) for k, x in v) + b"}"
+            return b"{" + b",".join(_json_key(k) + _marshal(x) for k, x in v) + b"}"
         return b"[" + b",".join(_marshal(x) for x in v) + b"]"
     raise TypeError(type(v))
 
@@ -404,3 +419,53 @@ def youtube_post_line(v, ch, *, crawl_label=b"", created=(1_750_000_000, 0), cap
         ("outlinks", urls), ("capture_time", cap), ("handle", chid),
     ]
     return _marshal(post) + b"\n", urls, ids
+
+
+# ---- the whole generic Post line, a second time ----------------------------------------------------------------------------
+# From crawler/telegram/telegram_crawler.go:179-262 (convertMessageToPost over client.Message), model/data.go (field order and
+# types: a nil map and nil slices marshal as null, zero structs with their zero fields, a zero time.Time as
+# "0001-01-01T00:00:00Z") and time.Time.MarshalJSON: published_at = GetTimestamp(), created_at = capture_time = time.Now(),
+# all three in time.Local.  zone = (starts, offsets) is time.Local as a transition table (tests/zone_oracle.py's rule);
+# without one time.Local is the fixed offset tz.
+def generic_post_line(m, *, created, capture, tz=0, zone=None):
+    """-> the line of one pack.GenericMessage, or None when json.Marshal fails (a time outside year [0, 9999])"""
+    if zone is None:
+        when = lambda sec, nsec: _go_time_checked(sec, nsec, tz)
+    else:
+        from zone_oracle import go_json_time, go_offset
+        when = lambda sec, nsec: _Raw(go_json_time(sec, nsec, go_offset(zone, sec))) or None
+    pub, cre, cap = when(m.ts_sec, m.ts_nsec), when(*created), when(*capture)
+    if None in (pub, cre, cap):
+        return None
+    reactions = {}
+    for k, cnt in m.reactions:  # map assignment: a later entry of a key overwrites
+        reactions[_bs(k)] = cnt
+    chan, text = _bs(m.channel_id), _Raw(go_json_string(_bs(m.text)))  # the text is marshalled three times: escape it once
+    nil = None
+    post = [
+        ("post_link", b""), ("channel_id", chan), ("post_uid", _bs(m.id)), ("url", b""), ("published_at", pub),
+        ("created_at", cre), ("language_code", b""), ("engagement", 0), ("view_count", m.views), ("like_count", 0),
+        ("share_count", 0), ("comment_count", 0), ("crawl_label", b""), ("list_ids", nil), ("channel_name", chan),
+        ("search_terms", nil), ("search_term_ids", nil), ("project_ids", nil), ("exercise_ids", nil), ("label_data", nil),
+        ("labels_metadata", nil), ("project_labeled_post_ids", nil), ("labeler_ids", nil), ("all_labels", nil),
+        ("label_ids", nil), ("is_ad", False), ("transcript_text", b""), ("image_text", b""), ("video_length", nil),
+        ("is_verified", nil),
+        ("channel_data", [("channel_id", b""), ("channel_name", b""), ("channel_description", b""),
+                          ("channel_profile_image", b""),
+                          ("channel_engagement_data", [("follower_count", 0), ("following_count", 0), ("like_count", 0),
+                                                       ("post_count", 0), ("views_count", 0), ("comment_count", 0),
+                                                       ("share_count", 0)]),
+                          ("channel_url_external", b""), ("channel_url", b""), ("country_code", b""),
+                          ("published_at", _Raw(b'"0001-01-01T00:00:00Z"'))]),
+        ("platform_name", b"telegram"), ("shared_id", nil), ("quoted_id", nil), ("replied_id", nil), ("ai_label", nil),
+        ("root_post_id", nil), ("engagement_steps_count", 0), ("ocr_data", nil),
+        ("performance_scores", [("likes", nil), ("shares", nil), ("comments", nil), ("views", 0)]),
+        ("has_embed_media", nil), ("description", text), ("repost_channel_data", nil), ("post_type", nil),
+        ("inner_link", _Raw(b"{}")), ("post_title", nil), ("media_data", [("document_name", b"")]), ("is_reply", nil),
+        ("ad_fields", nil), ("likes_count", 0), ("shares_count", 0), ("comments_count", 0), ("views_count", m.views),
+        ("searchable_text", text), ("all_text", text), ("contrast_agent_project_ids", nil), ("agent_ids", nil),
+        ("segment_ids", nil), ("thumb_url", b""), ("media_url", b""), ("comments", nil),
+        ("reactions", reactions or None),  # :250: the map only if it has entries, else nil
+        ("outlinks", nil), ("capture_time", cap), ("handle", _bs(m.sender_name)),
+    ]
+    return _marshal(post) + b"\n"

@@ -313,6 +313,7 @@ def test_oracle_generic_message_sparse_post():
                       "contrast_agent_project_ids", "agent_ids", "segment_ids", "comments", "outlinks"]
     for i, m in enumerate(msgs):
         line = r.line(i)
+        assert line == go_rules.generic_post_line(m, created=(cs, cn), capture=(ps, pn), tz=tz), i  # the whole line
         assert line.endswith(b"}\n")
         js = lambda b: go_rules.go_json_string(b if isinstance(b, bytes) else b.encode())
         # the variable parts, byte for byte

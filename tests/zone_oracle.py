@@ -64,8 +64,8 @@ class ZonedOracle:
         self.clock = (c.created_at_sec, c.created_at_nsec, c.capture_sec, c.capture_nsec)
 
     def set_clock(self, created_sec, created_nsec, capture_sec, capture_nsec):
+        self.o.set_clock(created_sec, created_nsec, capture_sec, capture_nsec)
         self.clock = (created_sec, created_nsec, capture_sec, capture_nsec)
-        pyoracle.lib().orc_set_clock(self.o.h, *self.clock)
 
     def telegram(self, batch, run_flags=abi.RUN_JSONL | abi.RUN_LINKS):
         pub = [(int(d), 0) for d in batch.recs["date"]]
