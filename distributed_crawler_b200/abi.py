@@ -92,6 +92,10 @@ GM_REC = np.dtype([  # tgi_gm_rec: one client.Message (SURVEY a12)
     ("id_len", "<u2"), ("channel_len", "<u2"), ("sender_len", "<u2"), ("reserved", "<u2"), ("reserved2", "<u4"), ("reserved3", "<u4")])
 GM_REACTION = np.dtype([("key_off", "<u4"), ("key_len", "<u2"), ("reserved", "<u2"), ("count", "<i8")])
 assert YT_CHAN.itemsize == 64 and LINK.itemsize == 36 and GM_REC.itemsize == 48 and GM_REACTION.itemsize == 16
+CH_REC = np.dtype([  # tgi_ch_rec: one channel page's StoreChannelData record
+    ("chat_id", "<i8"), ("str_off", "<u8"), ("member_count", "<i4"), ("message_count", "<i4"), ("total_views", "<i4"),
+    ("title_len", "<u4"), ("image_len", "<u4"), ("url_len", "<u4")])
+assert CH_REC.itemsize == 40
 
 
 # ---- ctypes structs ---------------------------------------------------------------------------
@@ -117,6 +121,10 @@ class GmBatchC(C.Structure):
         ("n", C.c_uint64), ("recs", C.c_void_p), ("strs", C.c_void_p), ("strs_len", C.c_uint64),
         ("react_off", C.c_void_p), ("reacts", C.c_void_p), ("n_reacts", C.c_uint64), ("aux", C.c_void_p),
         ("aux_len", C.c_uint64)]
+
+
+class ChBatchC(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("recs", C.c_void_p), ("strs", C.c_void_p), ("strs_len", C.c_uint64)]
 
 
 class ConfigC(C.Structure):

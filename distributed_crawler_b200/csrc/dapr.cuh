@@ -4,6 +4,8 @@
 // For every record with status TGI_ST_EMITTED the reference sends
 //   Data     = base64.StdEncoding.EncodeToString(json.Marshal(post) + "\n")          (daprstate.go:1159)
 //   Metadata = the blob path <prefix><channelID>/posts/<PostUID>.jsonl                (:1150-1153, format :2689-2698)
+// and for every channel record of a tgi_channel_batch result StoreChannelData (:3113-3137) sends the same Data with the
+// path <prefix><p.URL>/channel_data.jsonl.
 // Two kernels: dapr_size_kernel measures both per record (the host scans them into u64 offsets with launch_scan),
 // dapr_write_kernel encodes each line once, a warp per record, and writes its path.
 #pragma once
@@ -16,6 +18,7 @@ constexpr int DAPR_VECS = DAPR_CHUNK / 16 + 1;  // aligned 16-byte loads that co
 constexpr int DAPR_ERR_TOO_LONG = 1;        // a payload or a path of 2^32 bytes or more
 // the path's literals, little-endian in immediates (no device globals: the other kernels' SASS stays as it was)
 constexpr uint64_t DAPR_POSTS = 0x2f7374736f702full;  // "/posts/"
+constexpr uint64_t DAPR_CHANNEL = 0x6c656e6e6168632full, DAPR_DATA = 0x617461645full;  // "/channel", "_data"
 constexpr uint64_t DAPR_JSONL = 0x6c6e6f736a2eull;    // ".jsonl"
 
 struct DaprOut {
@@ -33,16 +36,34 @@ struct DaprOut {
 struct DaprPath {
   const uint8_t* chan;  // channelID
   uint32_t chan_len;
+  uint64_t dir[2];      // the literal after it, up to 16 bytes: "/posts/" or "/channel_data"
+  uint32_t dir_len;
   const uint8_t* uid;   // PostUID, or (Telegram) its tail after the number and the '-'
   uint32_t uid_len;
   int64_t num;          // Telegram: id / 1048576, Go's truncating division (tdutils.go:1008)
   uint32_t num_len;     // digits of num, 0 for YouTube
 };
 
-// PostUID: Telegram id/2^20 "-" channel name (tdutils.go:1008), YouTube the video id (youtube_crawler.go:701)
+// PostUID: Telegram id/2^20 "-" channel name (tdutils.go:1008), YouTube the video id (youtube_crawler.go:701).  A channel
+// record's path is generateCrawlExecutableStoragePath(p.URL, "channel_data.jsonl") (daprstate.go:3113-3116): channelID =
+// its url, the literal "/channel_data", no PostUID.
 DEVI DaprPath dapr_path(const SinkSrc& s, uint64_t i) {
   DaprPath p;
-  if (s.yt) {
+  p.dir[0] = DAPR_POSTS;
+  p.dir[1] = 0;
+  p.dir_len = 7;
+  if (s.ch) {
+    const tgi_ch_rec& r = s.ch_recs[i];
+    p.chan = s.strs + r.str_off + r.title_len + r.image_len;
+    p.chan_len = r.url_len;
+    p.dir[0] = DAPR_CHANNEL;
+    p.dir[1] = DAPR_DATA;
+    p.dir_len = 13;
+    p.uid = p.chan;
+    p.uid_len = 0;
+    p.num = 0;
+    p.num_len = 0;
+  } else if (s.yt) {
     const tgi_yt_rec& r = s.yt_recs[i];
     p.chan = sink_chan_id(s, r.chan_idx, p.chan_len);
     p.uid = s.strs + r.str_off;
@@ -60,7 +81,7 @@ DEVI DaprPath dapr_path(const SinkSrc& s, uint64_t i) {
   return p;
 }
 DEVI uint64_t dapr_path_len(const DaprOut& o, const DaprPath& p) {
-  return (uint64_t)o.prefix_len + p.chan_len + 7 + p.num_len + p.uid_len + 6;  // "/posts/" ... ".jsonl"
+  return (uint64_t)o.prefix_len + p.chan_len + p.dir_len + p.num_len + p.uid_len + 6;  // "/posts/" ... ".jsonl"
 }
 
 // one thread per record: base64 length 4*ceil(len/3) of its line and the length of its path; 0 for records without a
@@ -129,7 +150,8 @@ __global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(SinkSrc s, D
       }
       __syncwarp();
     }
-    // the path: prefix | channelID | "/posts/" | [number "-"] PostUID | ".jsonl", one byte per lane and step
+    // the path: prefix | channelID | "/posts/" | [number "-"] PostUID | ".jsonl" (a channel record: prefix | url |
+    // "/channel_data" | ".jsonl"), one byte per lane and step
     const DaprPath p = dapr_path(s, i);
     if (p.num_len && l == 0) {
       const int k = render_i64(sh.num[w], p.num);
@@ -137,13 +159,13 @@ __global__ void __launch_bounds__(CTA_THREADS, 5) dapr_write_kernel(SinkSrc s, D
     }
     __syncwarp();
     uint8_t* dp = o.path + o.path_off[i];
-    const uint64_t e0 = o.prefix_len, e1 = e0 + p.chan_len, e2 = e1 + 7, e3 = e2 + p.num_len, e4 = e3 + p.uid_len,
+    const uint64_t e0 = o.prefix_len, e1 = e0 + p.chan_len, e2 = e1 + p.dir_len, e3 = e2 + p.num_len, e4 = e3 + p.uid_len,
                    e5 = e4 + 6;
     for (uint64_t j = l; j < e5; j += 32) {
       uint32_t c;
       if (j < e0) c = ldb(o.prefix + j);
       else if (j < e1) c = ldb(p.chan + (j - e0));
-      else if (j < e2) c = (uint32_t)(DAPR_POSTS >> (8 * (j - e1))) & 0xFF;
+      else if (j < e2) c = (uint32_t)(j - e1 < 8 ? p.dir[0] >> (8 * (j - e1)) : p.dir[1] >> (8 * (j - e1 - 8))) & 0xFF;
       else if (j < e3) c = sh.num[w][j - e2];
       else if (j < e4) c = ldb(p.uid + (j - e3));
       else c = (uint32_t)(DAPR_JSONL >> (8 * (j - e4))) & 0xFF;

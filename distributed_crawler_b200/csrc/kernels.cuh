@@ -8,6 +8,7 @@
 //   tg_emit_esc / tg_emit_maps             what the lane emitter leaves: strings that need escaping, comment lists ...
 //   frontier_*                             exact open-addressed hash set over 32-byte keys
 //   yt_* / gm_*                            YouTube (config 4) and generic-message (a12) lines
+//   ch_*                                   random-walk channel records (StoreChannelData)
 //   join_*                                 message-status join (SURVEY 8f)
 // yt_size_kernel is the warp-per-record predecessor of the YouTube lane sizer, kept as an A/B reference (TGI_YT_WARP).
 #pragma once
@@ -16,6 +17,7 @@
 #include "tg_lane.cuh"
 #include "yt_walk.cuh"
 #include "gm_walk.cuh"
+#include "ch_walk.cuh"
 #include "yt_lane.cuh"
 
 namespace tgi {
@@ -801,6 +803,39 @@ __global__ void __launch_bounds__(CTA_THREADS, 4) gm_emit_kernel(GmBatchDev b, C
     w.sc = &scs[wid];
     w.p = out + line_off[r];
     walk_gm_record(w, b, cfg, r);
+    if (l == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, ERR_LINE_MISMATCH);
+  }
+}
+
+// ---- channel records -> ChannelData lines (StoreChannelData) -------------------------------------------
+// big batches only (small ones are checked by the host): bad[0] gets the lowest record whose ranges leave strs
+__global__ void ch_validate_kernel(ChBatchDev b, uint64_t strs_len, unsigned long long* bad) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < b.n; i += (uint64_t)gridDim.x * blockDim.x)
+    if (!ch_rec_ok(b.recs[i], strs_len)) atomicMin(bad, (unsigned long long)i);
+}
+__global__ void __launch_bounds__(CTA_THREADS, 4) ch_size_kernel(ChBatchDev b, uint8_t* status, uint32_t* linelen) {
+  __shared__ YtScratch scs[WARPS_PER_CTA];
+  int wid = threadIdx.x >> 5, l = lane_id();
+  uint64_t nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
+  for (uint64_t r = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; r < b.n; r += nwarps) {
+    YtSizer z;
+    z.sc = &scs[wid];
+    walk_ch_record(z, b, r);
+    if (l == 0) {
+      status[r] = TGI_ST_EMITTED;  // json.Marshal of a ChannelData cannot fail
+      linelen[r] = (uint32_t)z.total;
+    }
+  }
+}
+__global__ void __launch_bounds__(CTA_THREADS, 4) ch_emit_kernel(ChBatchDev b, const uint64_t* line_off, uint8_t* out, int* err) {
+  __shared__ YtScratch scs[WARPS_PER_CTA];
+  int wid = threadIdx.x >> 5, l = lane_id();
+  uint64_t nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
+  for (uint64_t r = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; r < b.n; r += nwarps) {
+    YtWriter w;
+    w.sc = &scs[wid];
+    w.p = out + line_off[r];
+    walk_ch_record(w, b, r);
     if (l == 0 && (uint64_t)(w.p - out) != line_off[r + 1]) atomicOr(err, ERR_LINE_MISMATCH);
   }
 }

@@ -1,5 +1,5 @@
-// sink_src.cuh — what the result sinks (dapr.cuh, local_appends.cuh, combine.cuh) read of a slot's last Telegram or
-// YouTube result that is still resident on the device, and the rules they share (sm_90a).
+// sink_src.cuh — what the result sinks (dapr.cuh, local_appends.cuh, combine.cuh) read of a slot's last Telegram,
+// YouTube or channel-record result that is still resident on the device, and the rules they share (sm_90a).
 #pragma once
 #include "kernels.cuh"
 
@@ -11,6 +11,8 @@ struct SinkSrc {
   const uint64_t* line_off;
   const uint8_t* jsonl;
   bool yt;
+  bool ch;                    // a channel-record result (tgi_channel_batch): the Dapr sinks only
+  const tgi_ch_rec* ch_recs;
   const tgi_tg_rec* tg_recs;  // the resident batch: records, channel rows and their strings
   const tgi_tg_chan* tg_chans;
   const tgi_yt_rec* yt_recs;

@@ -91,14 +91,14 @@ struct HostBuf {  // pinned
   T* as() const { return (T*)p; }
 };
 
-enum RecKind { REC_NONE, REC_TG, REC_YT, REC_GM };
+enum RecKind { REC_NONE, REC_TG, REC_YT, REC_GM, REC_CH };
 
 // One job on a staging slot: upload a batch (which becomes the slot's resident batch), run the resident batch, or both.
 enum JobStages : uint32_t { JOB_UPLOAD = 1, JOB_RUN = 2 };
 struct Job {
   RecKind kind;
   uint32_t stages;    // JOB_UPLOAD | JOB_RUN
-  const void* batch;  // JOB_UPLOAD: the tgi_tg_batch / tgi_yt_batch / tgi_gm_batch of `kind`
+  const void* batch;  // JOB_UPLOAD: the tgi_tg_batch / tgi_yt_batch / tgi_gm_batch / tgi_ch_batch of `kind`
   uint32_t flags;     // JOB_RUN: TGI_RUN_*
 };
 
@@ -271,6 +271,7 @@ struct Slot {
   TgBatchDev tg{};
   YtBatchDev yt{};
   GmBatchDev gm{};
+  ChBatchDev ch{};
   uint64_t yt_desc_bytes = 0;
   uint64_t n_ents = 0, n_reacts = 0, n_comments = 0, in_bytes = 0, chan_strs_len = 0;
   RecKind resident = REC_NONE;  // REC_TG / REC_YT: tg / yt describes the batch of the last successful upload
@@ -1651,6 +1652,89 @@ int run_gm(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
   return finish_batch(c, s, REC_GM, n, flags, t.line_total, 0, 1024, launches, out);
 }
 
+// channel records (StoreChannelData): upload, range check (host for small batches, device above), size, scan, emit
+int upload_ch(tgi_ctx* c, Slot& s, const tgi_ch_batch* in) {
+  if (!in) { set_err(c, "null batch"); return TGI_E_ARG; }
+  if (in->n && !in->recs) { set_err(c, "channel batch: recs must be non-null"); return TGI_E_ARG; }
+  if (in->strs_len && !in->strs) { set_err(c, "channel batch: a non-empty strs has a null pointer"); return TGI_E_ARG; }
+  if (in->n >= (1ull << 40)) { set_err(c, "channel batch: too many records"); return TGI_E_ARG; }
+  const uint64_t n = in->n;
+  const bool host_checked = n <= HOST_VALIDATE_MAX;
+  if (host_checked) {
+    for (uint64_t i = 0; i < n; i++)
+      if (!ch_rec_ok(in->recs[i], in->strs_len)) {
+        set_err(c, "channel batch: record %llu: title | image | url outside strs, or a string of 16 MiB or more", (unsigned long long)i);
+        return TGI_E_ARG;
+      }
+  }
+  s.in_bytes = 0;
+  InArrays a;
+  a.add(s.d_recs, in->recs, n * sizeof(tgi_ch_rec));
+  a.add(s.d_strs, in->strs, in->strs_len);
+  const int rc = upload_arrays(c, s, a, false);
+  if (rc) return rc;
+  ChBatchDev& b = s.ch;
+  b.n = n;
+  b.recs = (const tgi_ch_rec*)a.dev[0];
+  b.strs = a.dev[1];
+  if (!host_checked) {
+    CK(s.d_scalars.ensure(SC_COUNT * 8));
+    CK(s.h_scalars.ensure(SC_COUNT * 8));
+    unsigned long long* bad = (unsigned long long*)s.d_scalars.p;
+    CK(cudaMemsetAsync(bad, 0xFF, 8, s.stream));
+    const unsigned vg = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)c->sms * 16);
+    ch_validate_kernel<<<vg, 256, 0, s.stream>>>(b, in->strs_len, bad);
+    CK(cudaGetLastError());
+    const int prc = publish(c, bad, s.h_scalars, 1, s.stream);
+    if (prc) return prc;
+    CK(cudaStreamSynchronize(s.stream));
+    const unsigned long long hbad = *s.h_scalars.as<unsigned long long>();
+    if (hbad != ~0ull) {
+      set_err(c, "channel batch: record %llu: title | image | url outside strs, or a string of 16 MiB or more", hbad);
+      return TGI_E_ARG;
+    }
+  }
+  return TGI_OK;
+}
+
+int run_ch(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
+  const ChBatchDev& b = s.ch;
+  const uint64_t n = b.n;
+  cudaStream_t st = s.stream;
+  uint32_t launches = 0;
+  const bool want_json = flags & TGI_RUN_JSONL;
+  CK(s.d_arena.ensure(1024 * sizeof(tgi_link)));
+  int rc = bulk_prologue(c, s, n);
+  if (rc) return rc;
+  if (n) {
+    CK(cudaMemsetAsync(s.d_link_start.p, 0, n * 4, st));
+    CK(cudaMemsetAsync(s.d_link_count.p, 0, n * 4, st));
+  }
+  int* derr = (int*)(s.d_scalars.as<uint64_t>() + SC_CURSOR) + 1;
+  unsigned g = (unsigned)std::min<uint64_t>((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
+  CK(cudaEventRecord(s.ev_p0, st));
+  if (n) {  // the status does not depend on TGI_RUN_JSONL: the size pass always runs
+    ch_size_kernel<<<g, CTA_THREADS, 0, st>>>(b, s.d_status.as<uint8_t>(), s.d_linelen.as<uint32_t>());
+    launches++;
+  }
+  CK(cudaEventRecord(s.ev_p1, st));
+  Totals t{};
+  if (want_json) {
+    rc = bulk_totals(c, s, n, want_json, launches, t);
+    if (rc) return rc;
+    CK(s.d_jsonl.ensure(t.line_total));
+    CK(cudaEventRecord(s.ev_e0, st));
+    if (n) {
+      ch_emit_kernel<<<g, CTA_THREADS, 0, st>>>(b, s.d_line_off.as<uint64_t>(), s.d_jsonl.as<uint8_t>(), derr);
+      launches++;
+    }
+    CK(cudaEventRecord(s.ev_f1, st));
+    CK(cudaEventRecord(s.ev_e1, st));
+    CK(cudaGetLastError());
+  }
+  return finish_batch(c, s, REC_CH, n, flags, t.line_total, 0, 1024, launches, out);
+}
+
 // ---- jobs -------------------------------------------------------------------------------------------------------------
 // Upload if the job uploads (an upload-only job waits for the copy to land), run if it runs.
 int run_job(tgi_ctx* c, Slot& s) {
@@ -1658,18 +1742,20 @@ int run_job(tgi_ctx* c, Slot& s) {
   if (j.stages & JOB_UPLOAD) {
     const int rc = j.kind == REC_TG   ? upload_tg(c, s, (const tgi_tg_batch*)j.batch)
                    : j.kind == REC_YT ? upload_yt(c, s, (const tgi_yt_batch*)j.batch)
-                                      : upload_gm(c, s, (const tgi_gm_batch*)j.batch);
+                   : j.kind == REC_GM ? upload_gm(c, s, (const tgi_gm_batch*)j.batch)
+                                      : upload_ch(c, s, (const tgi_ch_batch*)j.batch);
     if (rc != TGI_OK) return rc;
     if (!(j.stages & JOB_RUN)) {
       const cudaError_t e = cudaStreamSynchronize(s.stream);
       if (e != cudaSuccess) { set_err(c, "upload sync: %s", cudaGetErrorString(e)); return TGI_E_CUDA; }
     }
-    if (j.kind != REC_GM) s.resident = j.kind;  // generic batches are not run resident
+    if (j.kind == REC_TG || j.kind == REC_YT) s.resident = j.kind;  // generic and channel batches are not run resident
   }
   if (!(j.stages & JOB_RUN)) return TGI_OK;
   return j.kind == REC_TG   ? run_tg(c, s, j.flags, &s.res)
          : j.kind == REC_YT ? run_yt(c, s, j.flags, &s.res)
-                            : run_gm(c, s, j.flags, &s.res);
+         : j.kind == REC_GM ? run_gm(c, s, j.flags, &s.res)
+                            : run_ch(c, s, j.flags, &s.res);
 }
 
 // runs the slot's claimed job to its end, on the worker thread or the caller's
@@ -1815,12 +1901,15 @@ int slot_result(tgi_ctx* c, int slot, const char* who, LastResult* r) {
   return TGI_OK;
 }
 
-// The sinks' view of slot `slot`: its last result, which must be a Telegram or YouTube one with lines; with src, also
-// the device arrays the sink kernels read (sink_src.cuh).  Selects the context's device.
-int sink_source(tgi_ctx* c, int slot, const char* who, LastResult& r, SinkSrc* src) {
+// The sinks' view of slot `slot`: its last result, which must be a Telegram, YouTube or (Dapr sinks only, `dapr`)
+// channel-record one with lines; with src, also the device arrays the sink kernels read (sink_src.cuh).  Selects the
+// context's device.
+int sink_source(tgi_ctx* c, int slot, const char* who, LastResult& r, SinkSrc* src, bool dapr) {
   const int rc = slot_result(c, slot, who, &r);
   if (rc != TGI_OK) return rc;
   if (r.kind == REC_GM) { set_err(c, "%s: generic posts go to SavePost, not to the StorePost sinks", who); return TGI_E_STATE; }
+  // StoreChannelData: Dapr appends or combine files (daprstate.go:3088-3148); BaseStateManager's is a no-op (base.go:530)
+  if (r.kind == REC_CH && !dapr) { set_err(c, "%s: the local manager stores no channel data", who); return TGI_E_STATE; }
   if (!r.dev.line_off) { set_err(c, "%s: the slot's last result has no lines (run it with TGI_RUN_JSONL)", who); return TGI_E_STATE; }
   cudaSetDevice(c->device);
   if (!src) return TGI_OK;
@@ -1831,8 +1920,11 @@ int sink_source(tgi_ctx* c, int slot, const char* who, LastResult& r, SinkSrc* s
   src->line_off = r.dev.line_off;
   src->jsonl = r.dev.jsonl;
   src->yt = r.kind == REC_YT;
+  src->ch = r.kind == REC_CH;
   // the resident batch descriptor, not the upload buffers: a page-sized batch lives in the slot's one-block upload
-  if (src->yt) {
+  if (src->ch) {
+    src->ch_recs = s.ch.recs, src->strs = s.ch.strs;
+  } else if (src->yt) {
     src->yt_recs = s.yt.recs, src->yt_chans = s.yt.chans, src->strs = s.yt.strs, src->chan_strs = s.yt.chan_strs;
     src->n_chans = s.yt.n_chans;
   } else {
@@ -2226,6 +2318,14 @@ int tgi_generic_batch(tgi_ctx* c, const tgi_gm_batch* in, uint32_t run_flags, tg
   // generic messages have no links: no frontier phase, no frontier turn
   return run_blocking(c, {REC_GM, JOB_UPLOAD | JOB_RUN, in, run_flags & ~(uint32_t)TGI_RUN_FRONTIER}, out);
 }
+int tgi_channel_batch(tgi_ctx* c, const tgi_ch_batch* in, uint32_t run_flags, tgi_result* out) {
+  if (!c) return TGI_E_ARG;
+  if (run_flags & ~(uint32_t)(TGI_RUN_JSONL | TGI_RUN_JSONL_DEVICE)) {
+    set_err(c, "channel batch: run flags 0x%x (only TGI_RUN_JSONL and TGI_RUN_JSONL_DEVICE)", run_flags);
+    return TGI_E_ARG;
+  }
+  return run_blocking(c, {REC_CH, JOB_UPLOAD | JOB_RUN, in, run_flags}, out);
+}
 int tgi_youtube_upload(tgi_ctx* c, int slot, const tgi_yt_batch* in) {
   return submit_wait(c, slot, {REC_YT, JOB_UPLOAD, in, 0}, nullptr);
 }
@@ -2480,7 +2580,7 @@ int tgi_dapr_payloads(tgi_ctx* c, int slot, const char* path_prefix, uint32_t pr
   if (!c || !out || !path_prefix) return TGI_E_ARG;
   LastResult r;
   SinkSrc src;
-  int rc = sink_source(c, slot, "tgi_dapr_payloads", r, &src);
+  int rc = sink_source(c, slot, "tgi_dapr_payloads", r, &src, true);
   if (rc != TGI_OK) return rc;
   Slot& s = c->slots[slot];
   DaprBufs& z = s.dapr;
@@ -2562,7 +2662,7 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   if (!c || !out) return TGI_E_ARG;
   LastResult r;
   SinkSrc src;
-  int rc = sink_source(c, slot, "tgi_channel_appends", r, &src);
+  int rc = sink_source(c, slot, "tgi_channel_appends", r, &src, false);
   if (rc != TGI_OK) return rc;
   memset(out, 0, sizeof *out);
   const uint64_t n = r.n, total = r.jsonl_len;  // every byte of the JSONL belongs to a line that takes part
@@ -2811,7 +2911,7 @@ int tgi_combine_open(tgi_ctx* c, uint64_t trigger, uint64_t hard_cap, const char
 int tgi_combine_add(tgi_ctx* c, int slot, int64_t unix_nano, tgi_combined_t* out) {
   if (!c || !out) return TGI_E_ARG;
   LastResult r;
-  int rc = sink_source(c, slot, "tgi_combine_add", r, nullptr);
+  int rc = sink_source(c, slot, "tgi_combine_add", r, nullptr, true);
   if (rc != TGI_OK) return rc;
   Combiner& z = c->cb;
   std::lock_guard<std::mutex> g(z.mu);

@@ -40,7 +40,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_update_page", "tgi_state_update_messages", "tgi_state_read_page", "tgi_state_render", "tgi_state_layer_map",
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
-    "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges",
+    "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
 ]
 
 
@@ -71,6 +71,7 @@ def lib() -> C.CDLL:
         L.tgi_telegram_upload.argtypes = [vp, i32, C.POINTER(abi.TgBatchC)]
         L.tgi_telegram_run_resident.argtypes = [vp, i32, u32, C.POINTER(abi.ResultC)]
         L.tgi_generic_batch.argtypes = [vp, C.POINTER(abi.GmBatchC), u32, C.POINTER(abi.ResultC)]
+        L.tgi_channel_batch.argtypes = [vp, C.POINTER(abi.ChBatchC), u32, C.POINTER(abi.ResultC)]
         L.tgi_key_join.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, vp]
         L.tgi_plan_chunks.argtypes = [vp, C.c_uint64, C.c_uint64, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), vp]
         L.tgi_youtube_upload.argtypes = [vp, i32, C.POINTER(abi.YtBatchC)]
@@ -479,7 +480,8 @@ class Engine:
 
     def dapr_payloads(self, slot: int, prefix: bytes) -> "DaprPayloads":
         """host copies of the StorePost binding payloads of the slot's last Telegram / YouTube result (call before
-        release): the base64 of every line, and its blob path prefix | channelID | /posts/ | PostUID | .jsonl"""
+        release): the base64 of every line, and its blob path prefix | channelID | /posts/ | PostUID | .jsonl; for a
+        channel_batch result the StoreChannelData payloads, path prefix | url | /channel_data.jsonl"""
         out = abi.DaprPayloadsC()
         self._check(lib().tgi_dapr_payloads(self.h, slot, prefix, len(prefix), C.byref(out)))
         return DaprPayloads(out)
@@ -513,6 +515,18 @@ class Engine:
         d = batch.descriptor()
         r = abi.ResultC()
         self._check(lib().tgi_generic_batch(self.h, C.byref(d), run_flags, C.byref(r)))
+        out = Result(r, copy)
+        lib().tgi_result_release(self.h, r.slot)
+        return out
+
+    # --- random-walk channel records -> ChannelData lines (StoreChannelData) ----------------------
+    def channel_batch(self, batch, run_flags=abi.RUN_JSONL, copy=True) -> Result:
+        """the ChannelData line of every record (pack.pack_channels).  The slot's result stays readable after the
+        release: Engine.dapr_payloads(result.slot, prefix) and combine_add(result.slot, ns) take it until the next job on
+        that slot"""
+        d = batch.descriptor()
+        r = abi.ResultC()
+        self._check(lib().tgi_channel_batch(self.h, C.byref(d), run_flags, C.byref(r)))
         out = Result(r, copy)
         lib().tgi_result_release(self.h, r.slot)
         return out

@@ -186,6 +186,35 @@ class Batch {
   std::vector<tgi_tg_chan> chans_;
 };
 
+// The channel records of one random-walk step (tgi_ch_batch): what RunForChannel puts in model.ChannelData for each
+// channel page it holds (crawl/runner.go:587-607), packed for MessageProcessor::StoreChannelData.
+class ChannelBatch {
+ public:
+  // chat.Id, chat.Title, chat.Photo.Extra ("" when Photo == nil), p.URL and the int32 counts (runner.go:980-982)
+  void Add(int64_t chat_id, std::string_view title, std::string_view image, std::string_view url, int32_t member_count,
+           int32_t message_count, int32_t total_views) {
+    tgi_ch_rec r{};
+    r.chat_id = chat_id;
+    r.str_off = strs_.size();
+    r.member_count = member_count;
+    r.message_count = message_count;
+    r.total_views = total_views;
+    r.title_len = (uint32_t)title.size();
+    r.image_len = (uint32_t)image.size();
+    r.url_len = (uint32_t)url.size();
+    strs_.append(title).append(image).append(url);
+    recs_.push_back(r);
+  }
+  size_t Size() const { return recs_.size(); }
+  tgi_ch_batch Descriptor() const {
+    return tgi_ch_batch{recs_.size(), recs_.data(), (const uint8_t*)strs_.data(), strs_.size()};
+  }
+
+ private:
+  std::vector<tgi_ch_rec> recs_;
+  std::string strs_;
+};
+
 // One processed batch: views into library-owned pinned memory, released by the destructor.
 class Result {
  public:
@@ -257,6 +286,14 @@ class MessageProcessor {
     const tgi_tg_batch d = b.Descriptor();
     tgi_result r{};
     if (tgi_telegram_batch(ctx_, &d, run_flags, &r) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return Result(ctx_, r);
+  }
+  // The random-walk StoreChannelData lines (daprstate.go:3089-3094) of a step's channel pages; feed the result to
+  // Result::DaprPayloads (paths prefix|url|/channel_data.jsonl) or to the combiner.
+  Result StoreChannelData(const ChannelBatch& b, uint32_t run_flags = TGI_RUN_JSONL) {
+    const tgi_ch_batch d = b.Descriptor();
+    tgi_result r{};
+    if (tgi_channel_batch(ctx_, &d, run_flags, &r) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
     return Result(ctx_, r);
   }
   void SetClock(int64_t created_sec, int32_t created_nsec, int64_t capture_sec, int32_t capture_nsec) {

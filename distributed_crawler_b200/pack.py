@@ -443,3 +443,46 @@ def pack_generic(msgs: list[GenericMessage]) -> GmBatch:
         react_off[i + 1] = len(reacts)
     ra = np.array(reacts, abi.GM_REACTION) if reacts else np.zeros(0, abi.GM_REACTION)
     return GmBatch(recs=recs, strs=_blob(strs), react_off=react_off, reacts=ra, aux=_blob(aux))
+
+
+# ---- channel records: the random-walk StoreChannelData line ----------------------------------------------------------
+@dataclass
+class ChannelRecord:  # what RunForChannel puts in model.ChannelData (crawl/runner.go:592-610)
+    chat_id: int = 0                 # chat.Id
+    title: str | bytes = ""          # chat.Title
+    image: str | bytes = ""          # chat.Photo.Extra ("" when chat.Photo == nil)
+    url: str | bytes = ""            # p.URL
+    member_count: int = 0            # int32(memberCount), int32(messageCount), int32(totalViews) (runner.go:980-982)
+    message_count: int = 0
+    total_views: int = 0
+
+
+class ChBatch:
+    FIELDS = ("recs", "strs")
+
+    def __init__(self, **arrays):
+        for k in self.FIELDS:
+            setattr(self, k, arrays[k])
+        self.n = len(self.recs)
+
+    def descriptor(self) -> abi.ChBatchC:
+        d = abi.ChBatchC()
+        d.n = self.n
+        d.recs = abi.ptr(self.recs)
+        d.strs = abi.ptr(self.strs)
+        d.strs_len = self.strs.size
+        return d
+
+
+def pack_channels(recs_in: list[ChannelRecord]) -> ChBatch:
+    """one tgi_ch_rec per channel page; title | image | url of each record back to back in one blob"""
+    recs = np.zeros(len(recs_in), abi.CH_REC)
+    strs = bytearray()
+    for i, c in enumerate(recs_in):
+        parts = [_b(c.title), _b(c.image), _b(c.url)]
+        r = recs[i]
+        r["chat_id"], r["str_off"] = c.chat_id, len(strs)
+        r["member_count"], r["message_count"], r["total_views"] = c.member_count, c.message_count, c.total_views
+        r["title_len"], r["image_len"], r["url_len"] = (len(p) for p in parts)
+        strs += b"".join(parts)
+    return ChBatch(recs=recs, strs=_blob(strs))

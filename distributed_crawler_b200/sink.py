@@ -152,7 +152,8 @@ def store_posts_dapr(invoke, payloads, binding: str, naming_key: str) -> int:
     invoke(binding, "create", data, metadata) per post, in record order, with data = the base64 of its line and metadata
     {naming_key: blob path, "operation": "append"}; the path is raw bytes, as a Go string holds it.  `payloads` is Engine.dapr_payloads(slot, prefix); naming_key is
     fetchFileNamingComponent's answer for the binding, resolved once per crawl.  Records without a post are skipped.
-    Returns the number of requests."""
+    The payloads of an Engine.channel_batch result are StoreChannelData's requests (daprstate.go:3113-3144), of the
+    same shape.  Returns the number of requests."""
     k = 0
     for i in range(payloads.n):
         if payloads.data_off[i + 1] == payloads.data_off[i]:

@@ -272,6 +272,30 @@ typedef struct tgi_gm_batch {
   uint64_t aux_len;
 } tgi_gm_batch;
 
+/* ---- channel records: the random-walk StoreChannelData line ----------------------------------------
+ * A random-walk crawl stores no posts (DaprStateManager.StorePost returns early, state/daprstate.go:1109-1111); its
+ * one stored line per channel page is the model.ChannelData that RunForChannel builds (crawl/runner.go:592-610) and
+ * passes to sm.StoreChannelData(p.URL, channelData) (:620-626) before the activity check, marshalled with json.Marshal
+ * + '\n' (daprstate.go:3088-3148).  One record per channel page, filled by the shim from TDLib's chat and the counts
+ * of getChannelInfo (runner.go:975-983).                                                                            */
+typedef struct tgi_ch_rec { /* 40 bytes */
+  int64_t chat_id;        /* chat.Id: channel_id = strconv.FormatInt(chat_id, 10)                              */
+  uint64_t str_off;       /* in `strs`: title | image | url                                                     */
+  int32_t member_count;   /* int32(memberCount) (runner.go:982): follower_count                                 */
+  int32_t message_count;  /* int32(messageCount) (:981): post_count                                              */
+  int32_t total_views;    /* int32(totalViews) (:980): views_count                                               */
+  uint32_t title_len;     /* chat.Title: channel_name                                                           */
+  uint32_t image_len;     /* chat.Photo.Extra, 0 when chat.Photo == nil: channel_profile_image                  */
+  uint32_t url_len;       /* p.URL: channel_url_external = channel_url = "https://t.me/" + p.URL                */
+} tgi_ch_rec;
+
+typedef struct tgi_ch_batch {
+  uint64_t n;
+  const tgi_ch_rec* recs;
+  const uint8_t* strs;
+  uint64_t strs_len;
+} tgi_ch_batch;
+
 /* ---- configuration -------------------------------------------------------------------------- */
 #define TGI_CFG_HAS_MIN_POST_DATE 0x01 /* !cfg.MinPostDate.IsZero()                               */
 #define TGI_CFG_SKIP_MEDIA 0x02        /* cfg.SkipMediaDownload; REQUIRED (media download is RPC) */
@@ -469,7 +493,8 @@ int tgi_plan_chunks_carry(const uint64_t* line_off, uint64_t n, uint64_t trigger
  *   Path     path_prefix verbatim, then "combined-posts/combined_<ns>.jsonl" (generateCrawlExecutableStoragePath,
  *            daprstate.go:2689-2698, :3743-3746): path[path_off, path_off + path_len).  <ns> = max(unix_nano, previous
  *            <ns> + 1) for every blob, so names are unique and increase when one call closes several blobs.
- *   Inputs   tgi_combine_add takes the slot's last result (Telegram or YouTube, bulk or page) like tgi_dapr_payloads,
+ *   Inputs   tgi_combine_add takes the slot's last result (Telegram or YouTube, bulk or page, or tgi_channel_batch: its
+ *            channel_<id>_<ns>.jsonl files land in the same watch directory) like tgi_dapr_payloads,
  *            also after TGI_RUN_JSONL_DEVICE and TGI_RUN_NO_D2H.  TGI_E_STATE: no combiner is open, the slot holds no
  *            result, the result ran without TGI_RUN_JSONL, or it is a tgi_generic_batch one (SavePost has no Dapr
  *            implementation).  The open group never points into the slot: once tgi_combine_add returns, the slot may
@@ -531,7 +556,8 @@ int tgi_plan_channel_appends(const uint64_t* line_off, const void* chan_idx, uin
  *   Order    inside a group, lines in record order: what the per-post appends leave in the file.  Groups are ordered by
  *            their first line.  order[] lists the record index of every grouped line, group after group.
  *   Errors   TGI_E_STATE: the slot holds no result (see tgi_result_read_jsonl), the result ran without TGI_RUN_JSONL,
- *            or it is a tgi_generic_batch one (its posts go to SavePost).  TGI_E_ARG: bad slot or NULL out.
+ *            or it is a tgi_generic_batch one (its posts go to SavePost) or a tgi_channel_batch one (the local manager
+ *            stores no channel data).  TGI_E_ARG: bad slot or NULL out.
  *            TGI_E_NOMEM: allocation failed (the batch result stays valid).  TGI_E_CAPACITY: 2^32 - 16 records or more.
  * The call synchronises once.  Outputs live in library-owned pinned memory and stay valid until the release or the
  * next call on that slot.  The batch's tgi_result is not changed.                                                     */
@@ -563,7 +589,8 @@ int tgi_channel_appends(tgi_ctx* ctx, int slot, tgi_channel_appends_t* out);
  *                path[path_off[i], path_off[i+1]).  Telegram: channelID = the channel row's name (the channelName
  *                argument, tdutils.go:725), PostUID = FormatInt(id / 1048576) + "-" + channelName (tdutils.go:416,636,
  *                1008; truncating division).  YouTube: channelID = the channel row's id (video.ChannelID,
- *                youtube_crawler.go:396), PostUID = the record's id (video.ID, :701).
+ *                youtube_crawler.go:396), PostUID = the record's id (video.ID, :701).  A tgi_channel_batch result
+ *                (StoreChannelData, daprstate.go:3114-3117): prefix | url | "/channel_data.jsonl".
  * Only records with status TGI_ST_EMITTED get a payload; the others get empty ranges: a date-skipped message never
  * reaches StorePost (tdutils.go:419-421), a failed one panicked before it, and a TGI_ST_NOLINE one failed json.Marshal
  * before any binding call (daprstate.go:1141-1144).
@@ -594,6 +621,26 @@ int tgi_key_join(tgi_ctx* ctx, const int64_t* a_keys, uint64_t na, const int64_t
  * crawler/telegram/telegram_crawler.go:148-156 (convertMessageToPost :179-262) + json.Marshal+'\n'.
  * Blocking; picks a free slot.  status[] is TGI_ST_EMITTED or TGI_ST_NOLINE; no links.             */
 int tgi_generic_batch(tgi_ctx* ctx, const tgi_gm_batch* in, uint32_t run_flags, tgi_result* out);
+
+/* Channel records -> model.ChannelData lines: replaces the random-walk branch of RunForChannel (crawl/runner.go:592-626)
+ * up to json.Marshal+'\n' in StoreChannelData (state/daprstate.go:3089-3094), for the channel pages of a whole step.
+ * Blocking; picks a free slot, like tgi_generic_batch.
+ *   Line     {"channel_id":"<chat_id>","channel_name":<title>,"channel_description":"","channel_profile_image":<image>,
+ *            "channel_engagement_data":{"follower_count":<member_count>,"following_count":0,"like_count":0,
+ *            "post_count":<message_count>,"views_count":<total_views>,"comment_count":0,"share_count":0},
+ *            "channel_url_external":"https://t.me/<url>","channel_url":"https://t.me/<url>","country_code":"",
+ *            "published_at":"0001-01-01T00:00:00Z"} and '\n' (model/data.go:89-111).  Strings in encoding/json's
+ *            HTML-safe escaping, invalid UTF-8 as �.  json.Marshal cannot fail here: every status is
+ *            TGI_ST_EMITTED.  No links.
+ *   Flags    TGI_RUN_JSONL and TGI_RUN_JSONL_DEVICE only; any other flag is TGI_E_ARG.
+ *   Sinks    the result feeds tgi_dapr_payloads (Data = base64 of each line, path = path_prefix | url |
+ *            "/channel_data.jsonl", generateCrawlExecutableStoragePath daprstate.go:2689-2698 with channelID = p.URL) and
+ *            tgi_combine_add (the channel_<id>_<ns>.jsonl files enter the chunker's watch directory beside the post files,
+ *            daprstate.go:3096-3111).  tgi_channel_appends refuses it with TGI_E_STATE: the local manager stores no
+ *            channel data (state/base.go:530-532).
+ *   Errors   TGI_E_ARG, naming the first bad record: a range title | image | url outside strs, or a string of 16 MiB or
+ *            more.  Small batches are checked on the host, big ones on the device, before any kernel reads a string. */
+int tgi_channel_batch(tgi_ctx* ctx, const tgi_ch_batch* in, uint32_t run_flags, tgi_result* out);
 
 void tgi_result_release(tgi_ctx* ctx, int slot);
 
