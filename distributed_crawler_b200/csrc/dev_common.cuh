@@ -11,6 +11,7 @@
 
 #define FULL 0xffffffffu
 #define DEVI __device__ __forceinline__
+#define HDI __host__ __device__ __forceinline__  // pure SWAR helpers that tests/text_classes_check.cu runs on the host
 
 namespace tgi {
 
@@ -165,7 +166,7 @@ DEVI uint32_t swar_has_byte(uint32_t w, uint32_t c) {  // bit7 of each byte equa
 
 // exact per-byte equality: bit 7 of every byte of w that equals c (swar_has_byte above is exact only
 // as an "any" test: its borrow can flag the byte above a match)
-DEVI uint32_t swar_eq(uint32_t w, uint32_t c) {
+HDI uint32_t swar_eq(uint32_t w, uint32_t c) {
   const uint32_t x = w ^ (c * 0x01010101u);
   return ~(((x & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | x) & 0x80808080u;
 }
@@ -294,11 +295,20 @@ __device__ __noinline__ uint32_t warp_esc_len(const uint8_t* s, int64_t n, bool*
 // escaped length is n + #('"', '\\', \b \t \n \f \r) + 5 * #(other bytes < 0x20, '<', '>', '&').  The test is
 // stricter than warp_load_strip (it also rejects valid F4 sequences and every E2 80 xx), never looser.
 
+// w shifted up by k = 8, 16 or 24 bits with the top bytes of pw shifted in: byte i = the byte k / 8 places in front
+HDI uint32_t shift_in(uint32_t pw, uint32_t w, uint32_t k) {
+#ifdef __CUDA_ARCH__
+  return __funnelshift_l(pw, w, k);
+#else
+  return (w << k) | (pw >> (32 - k));
+#endif
+}
+
 // bit 7 of every byte of w that makes the text not clean; pw = the 4 bytes in front of w (bytes past the text's end
 // are read as ' ', so a sequence left open at the end is a mismatch)
-DEVI uint32_t utf8_unclean4(uint32_t pw, uint32_t w) {
+HDI uint32_t utf8_unclean4(uint32_t pw, uint32_t w) {
   const uint32_t M = 0x80808080u;
-  const uint32_t p1 = __funnelshift_l(pw, w, 8), p2 = __funnelshift_l(pw, w, 16), p3 = __funnelshift_l(pw, w, 24);
+  const uint32_t p1 = shift_in(pw, w, 8), p2 = shift_in(pw, w, 16), p3 = shift_in(pw, w, 24);
   const uint32_t cont = w & ~(w << 1);  // 10xxxxxx
   const uint32_t due = (p1 & (p1 << 1)) | (p2 & (p2 << 1) & (p2 << 2)) | (p3 & (p3 << 1) & (p3 << 2) & (p3 << 3));
   uint32_t bad = (cont ^ due) | (((w & 0x7F7F7F7Fu) + 0x0C0C0C0Cu) & w) | swar_eq(w & 0xFEFEFEFEu, 0xC0);  // >= F4, C0/C1
@@ -308,19 +318,23 @@ DEVI uint32_t utf8_unclean4(uint32_t pw, uint32_t w) {
   return bad & M;
 }
 
-// escaped length minus 1 summed over the ASCII bytes of w (the other bytes of a clean text are copied as they are)
-DEVI uint32_t esc_extra4(uint32_t w) {
-  // an "any" test: < 0x20, '<' / '>' (0x3C | 2 = 0x3E), '"' / '&' (0x22 | 4 = 0x26), '\\'
-  const uint32_t special = ((w - 0x20202020u) & ~w & 0x80808080u) | swar_has_byte(w | 0x02020202u, 0x3E) |
-                           swar_has_byte(w | 0x04040404u, 0x26) | swar_has_byte(w, 0x5C);
-  if (!special) return 0;
-  uint32_t x = 0;
-#pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const uint32_t b = (w >> (8 * k)) & 0xFF;
-    x += b < 0x80 ? ascii_esc_len(b) - 1u : 0u;
-  }
-  return x;
+// bit 7 of every byte >= 0xE0: the lead of a 3- or 4-byte sequence (or a byte no clean text holds)
+HDI uint32_t utf8_lead3(uint32_t w) { return ((w & 0x7F7F7F7Fu) + 0x20202020u) & w & 0x80808080u; }
+
+// utf8_unclean4 for a w whose bytes and pw's last three bytes hold no utf8_lead3: only a 2-byte sequence can be open in
+// front of a byte of w, so the 3- and 4-byte dues, the >= F4 test and the E0 / ED / F0 / E2 ranges drop out.  The same
+// bits as utf8_unclean4 (tests/text_classes_check.cu compares them).
+HDI uint32_t utf8_unclean2(uint32_t pw, uint32_t w) {
+  const uint32_t p1 = shift_in(pw, w, 8), ws = w << 1;
+  const uint32_t c0c1 = w & ws & ~((w & 0x3E3E3E3Eu) + 0x7E7E7E7Eu);  // 11xxxxxx with bits 5..1 clear: C0 or C1
+  return (((w & ~ws) ^ (p1 & (p1 << 1))) | c0c1) & 0x80808080u;
+}
+
+// bit 7 of every byte of w that may need escaping: < 0x20, '<' / '>' (0x3C | 2 = 0x3E), '"' / '&' (0x22 | 4 = 0x26),
+// '\\'.  Every such byte is flagged; a borrow can flag an ASCII byte above one as well, never a byte >= 0x80.
+DEVI uint32_t esc_special4(uint32_t w) {
+  return ((w - 0x20202020u) & ~w & 0x80808080u) | swar_has_byte(w | 0x02020202u, 0x3E) |
+         swar_has_byte(w | 0x04040404u, 0x26) | swar_has_byte(w, 0x5C);
 }
 
 // w with its bytes k.. read as ' '

@@ -148,7 +148,9 @@ DEVI uint32_t warp_count_tme(const uint8_t* s, int64_t n) {
 
 // The same count, and the text measured from the same 16 bytes per lane (JSONL runs): esc_len = its JSON-escaped length
 // if it is clean (utf8_unclean4), 0 if not (or if n == 0).  The lane's 4 bytes in front come from the lane below, or
-// for lane 0 from the previous strip's last lane.
+// for lane 0 from the previous strip's last lane.  The lane classifies its 16 bytes once: ASCII needs no clean test,
+// bytes without a 3- or 4-byte lead (Latin, Cyrillic, Arabic) take utf8_unclean2, the rest utf8_unclean4 word by
+// word; the escape count looks only at the bytes the special-byte test (esc_special4) flags.
 DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len) {
   const int l = lane_id();
   const uint32_t SP = 0x20202020u;
@@ -164,16 +166,31 @@ DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len)
     const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
     uint32_t pw = l == 0 ? tail : below;
     tail = __shfl_sync(FULL, w.w, 31);
-    const bool ascii = ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) == 0;
+    if ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) {  // not ASCII
+      // pw's first byte governs no byte of w: a lead there covers at most pw's other three
+      if ((utf8_lead3(w.x) | utf8_lead3(w.y) | utf8_lead3(w.z) | utf8_lead3(w.w) | utf8_lead3(pw & 0xFFFFFF00u)) == 0) {
+        bad |= utf8_unclean2(pw, w.x) | utf8_unclean2(w.x, w.y) | utf8_unclean2(w.y, w.z) | utf8_unclean2(w.z, w.w);
+      } else {
+        uint4 v = w;
 #pragma unroll 1
-    for (int k = 0; k < 4; k++) {  // a word at a time: the parse kernels' code has to stay small (instruction cache)
-      if (!ascii) bad |= utf8_unclean4(pw, w.x);
-      extra += esc_extra4(w.x);
-      pw = w.x;
-      w = make_uint4(w.y, w.z, w.w, w.x);
+        for (int k = 0; k < 4; k++) {  // a word at a time: the parse kernels' code has to stay small (instruction cache)
+          bad |= utf8_unclean4(pw, v.x);
+          pw = v.x;
+          v = make_uint4(v.y, v.z, v.w, v.x);
+        }
+      }
+    }
+    // bit 8j + k: byte j of word k may need escaping (line breaks, quotes, '<', '&': few lanes have one)
+    uint32_t sp = (esc_special4(w.x) >> 7) | (esc_special4(w.y) >> 6) | (esc_special4(w.z) >> 5) | (esc_special4(w.w) >> 4);
+    while (sp) {
+      const int b = __ffs(sp) - 1, k = b & 7;
+      sp &= sp - 1;
+      const uint32_t x = k == 0 ? w.x : (k == 1 ? w.y : (k == 2 ? w.z : w.w));
+      extra += ascii_esc_len((x >> (b & ~7)) & 0xFFu) - 1u;  // a flagged byte is ASCII; the text copies the others as they are
     }
   }
-  bad |= utf8_unclean4(tail, SP);  // a text that ends with its last strip: a sequence open at the end
+  // a text that ends with its last strip: a sequence open at the end (one needs a high bit in tail's last three bytes)
+  if (tail & 0x80808000u) bad |= utf8_unclean4(tail, SP);
   const uint32_t e = (uint32_t)n + warp_sum(extra);
   esc_len = __any_sync(FULL, bad != 0) ? 0u : e;
   return warp_sum(cnt);
