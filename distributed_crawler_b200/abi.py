@@ -247,6 +247,22 @@ class StateEdgesC(C.Structure):  # tgi_state_edges_t
                 ("gpu_launches", C.c_uint32)]
 
 
+READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
+# tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
+SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3
+
+
+class StateReadC(C.Structure):  # tgi_state_read_t
+    _fields_ = [("n_pages", C.c_uint64), ("rows", C.c_void_p), ("pages", C.c_void_p), ("strs", C.c_void_p), ("strs_len", C.c_uint64),
+                ("msgs", C.c_void_p), ("msg_first", C.c_void_p), ("n_msgs", C.c_uint64), ("select", C.c_void_p),
+                ("n_selected", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
+class StateLayersC(C.Structure):  # tgi_state_layers_t
+    _fields_ = [("n_layers", C.c_uint64), ("depth", C.c_void_p), ("n_pages", C.c_void_p), ("max_depth", C.c_int64),
+                ("has_max_depth", C.c_uint32), ("reserved", C.c_uint32), ("n_incomplete", C.c_uint64)]
+
+
 STATE_EXPORT_DAPR, STATE_EXPORT_LOCAL = 0, 1
 STATE_EXPORT_CHUNK_DEFAULT = 100 * 1024 * 1024  # exportChunkSizeBytes (state/daprstate.go:2909)
 

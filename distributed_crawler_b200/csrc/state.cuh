@@ -23,6 +23,9 @@
 // records the first fetched index of its message id; the new keys become the row's next generation, and the one page
 // renders through the export's line passes over that fresh contiguous segment.  Nothing reads another row's messages.
 // The turn's owner keys stay as the row's owner view; the close appends the view as the row's next generation.
+//
+// Page reads: the rows' fields come from the host mirror; their lists are the live messages of the distinct rows,
+// flagged in one pass, grouped by row with the render's radix passes and written out in that order.
 #pragma once
 #include "local_appends.cuh"
 
@@ -416,7 +419,7 @@ __global__ void st_row_starts_kernel(const uint32_t* rows, const uint64_t* n, ui
     if (q == 0 || rows[q - 1] != rows[q]) row_base[rows[q]] = base + q;
 }
 
-// ---- compaction / read-back -------------------------------------------------------------------------------------
+// ---- compaction -------------------------------------------------------------------------------------------------
 // flag[i] = message i is live (row == ST_NONE) or a live message of `row`
 __global__ void st_live_flag_kernel(StDev d, uint64_t n, uint32_t row, uint32_t* flag) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -428,17 +431,25 @@ __global__ void st_compact_kernel(StDev d, uint64_t n, const uint32_t* flag, con
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
     if (flag[i]) out[pos[i]] = d.msgs[i];
 }
-__global__ void st_read_kernel(StDev d, uint64_t n, const uint32_t* flag, const uint64_t* pos, tgi_state_msg* out) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    if (!flag[i]) continue;
-    const StMsg m = d.msgs[i];
+
+// ---- page reads (tgi_state_read_pages / _read_layer): the message lists of a set of rows -----------------------------
+// the live message count of every row of the read set (ascending)
+__global__ void st_set_counts_kernel(const uint32_t* row_cnt, const uint32_t* set, uint32_t n_set, uint32_t* cnt) {
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < n_set; k += (uint64_t)gridDim.x * blockDim.x)
+    cnt[k] = row_cnt[set[k]];
+}
+// the set's live messages grouped by row (sorted = their message indices, *n of them) as tgi_state_msg, in that order
+__global__ void st_gather_kernel(StDev d, const uint32_t* sorted, const uint64_t* n, tgi_state_msg* out) {
+  const uint64_t m = *n;
+  for (uint64_t q = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; q < m; q += (uint64_t)gridDim.x * blockDim.x) {
+    const StMsg s = d.msgs[sorted[q]];
     tgi_state_msg o;
-    o.chat_id = m.chat;
-    o.message_id = m.msg;
-    o.page_id = m.pid;
-    o.status = m.status;
-    o.platform = m.platform;
-    out[pos[i]] = o;
+    o.chat_id = s.chat;
+    o.message_id = s.msg;
+    o.page_id = s.pid;
+    o.status = s.status;
+    o.platform = s.platform;
+    out[q] = o;
   }
 }
 

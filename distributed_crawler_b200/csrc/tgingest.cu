@@ -248,6 +248,10 @@ struct CrawlState {
   uint64_t batch_next = 0;
   DevBuf clink, edges, ebatches, span_batch;
   HostBuf h_edges, h_ebatches, h_span_batch;
+  // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
+  // device and its staging, and the pinned outputs
+  DevBuf rset;
+  HostBuf h_rset, h_rrows, h_rpages, h_rstrs, h_rmsgs, h_rfirst, h_rsel, h_rdepth, h_rcount;
 };
 
 struct Slot {
@@ -3889,6 +3893,140 @@ int st_apply_updates(tgi_ctx* c, CrawlState& S, uint64_t m, uint32_t& launches, 
   return TGI_OK;
 }
 
+std::string_view st_view(const CrawlState& S, const tgi_state_page& p, int f) {
+  uint64_t o = p.str_off;
+  for (int k = 0; k < f; k++) o += p.str_len[k];
+  return std::string_view(S.blob.data() + o, p.str_len[f]);
+}
+
+// GetPage of n known rows into the pinned read buffers: the records and strings from the host mirror, and with `lists`
+// the rows' message lists from the device.  One pass over the message rows flags the live messages of the distinct
+// rows, the render's stable radix passes group them by row (storage order inside a row) and one gather writes them out;
+// the rows' counts, scanned, place each row's list.  The launches follow the state's row count, not n; two
+// synchronises: the lists' lengths, then the lists.
+int st_read_rows(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint64_t n, bool lists, const char* who, tgi_state_read_t* out) {
+  uint64_t sl = 0;
+  for (uint64_t k = 0; k < n; k++) sl += page_str_bytes(S.rows[rows[k]]);
+  CK(S.h_rrows.ensure(std::max<uint64_t>(n, 1) * 4));
+  CK(S.h_rpages.ensure(std::max<uint64_t>(n, 1) * sizeof(tgi_state_page)));
+  if (n) memcpy(S.h_rrows.p, rows, n * 4);
+  CK(S.h_rstrs.ensure(std::max<uint64_t>(sl, 1)));
+  tgi_state_page* pg = S.h_rpages.as<tgi_state_page>();
+  uint8_t* hs = S.h_rstrs.as<uint8_t>();
+  for (uint64_t k = 0, o = 0; k < n; k++) {
+    pg[k] = S.rows[rows[k]];
+    const uint64_t b = page_str_bytes(pg[k]);
+    if (b) memcpy(hs + o, S.blob.data() + pg[k].str_off, b);
+    pg[k].str_off = o;
+    pg[k].n_msgs = 0;
+    o += b;
+  }
+  out->n_pages = n;
+  out->rows = S.h_rrows.as<uint32_t>();
+  out->pages = pg;
+  out->strs = hs;
+  out->strs_len = sl;
+  if (!lists) return TGI_OK;
+  CK(S.h_rfirst.ensure(std::max<uint64_t>(n, 1) * 8));
+  CK(S.h_rmsgs.ensure(sizeof(tgi_state_msg)));
+  uint64_t* first = S.h_rfirst.as<uint64_t>();
+  out->msg_first = first;
+  out->msgs = S.h_rmsgs.as<tgi_state_msg>();
+  std::vector<uint32_t> set(rows, rows + n);  // the distinct rows, ascending
+  std::sort(set.begin(), set.end());
+  set.erase(std::unique(set.begin(), set.end()), set.end());
+  const uint32_t ns = (uint32_t)set.size();
+  const uint64_t nm = S.n_msgs, live = nm - S.n_dead, nr = S.rows.size();
+  if (!n || !live) {
+    for (uint64_t k = 0; k < n; k++) first[k] = 0;
+    return TGI_OK;
+  }
+  cudaStream_t st = S.stream;
+  int rc;
+  // S.rset: the set [ns] | its counts [ns] | their scan [ns+1]; h_rset stages the set and takes the scan back
+  const size_t o_cnt = 4ull * ns, o_off = 8ull * ns, rbytes = o_off + 8ull * (ns + 1);
+  CK(S.rset.ensure(rbytes));
+  CK(S.h_rset.ensure(rbytes));
+  uint32_t bits = 0;
+  while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
+  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
+  const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
+  CK(S.flag.ensure(nm * 4));
+  CK(S.pos.ensure((nm + 1) * 8));
+  CK(S.keys.ensure(2 * live * 4));
+  CK(S.vals.ensure(2 * live * 4));
+  CK(S.counts.ensure(radix * ntiles * 4));
+  CK(S.roff.ensure((radix * ntiles + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.spare.ensure(live * sizeof(tgi_state_msg)));
+  StRender g{};
+  g.flag = S.flag.as<uint32_t>();
+  g.pos = S.pos.as<uint64_t>();
+  g.keys[0] = S.keys.as<uint32_t>();
+  g.keys[1] = g.keys[0] + live;
+  g.vals[0] = S.vals.as<uint32_t>();
+  g.vals[1] = g.vals[0] + live;
+  uint8_t* dr = S.rset.as<uint8_t>();
+  const uint32_t* d_set = (const uint32_t*)dr;
+  uint32_t* d_cnt = (uint32_t*)(dr + o_cnt);
+  uint64_t* d_off = (uint64_t*)(dr + o_off);
+  uint64_t* sc = S.sc.as<uint64_t>();
+  memcpy(S.h_rset.p, set.data(), 4ull * ns);
+  CK(cudaMemcpyAsync(dr, S.h_rset.p, 4ull * ns, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+  const StDev d = st_dev(S);
+  uint32_t launches = 0;
+  CK(cudaEventRecord(S.t0, st));
+  st_rows_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, d_set, ns, g.flag);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, g.flag, nm, g.pos, sc + ST_SC_LIVE, launches))) return rc;
+  st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, g);
+  launches++;
+  int cur = 0;
+  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
+    const uint32_t shift = p * width;
+    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                   S.counts.as<uint32_t>());
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), sc + ST_SC_RADIX, launches)))
+      return rc;
+    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], g.vals[cur], g.keys[cur ^ 1], g.vals[cur ^ 1],
+                                                                      sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
+                                                                      S.roff.as<uint64_t>());
+    launches++;
+  }
+  st_set_counts_kernel<<<st_grid(c, ns), ST_THREADS, 0, st>>>(d.row_cnt, d_set, ns, d_cnt);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, d_cnt, ns, d_off, sc + ST_SC_ROWS, launches, true))) return rc;
+  st_gather_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, g.vals[cur], sc + ST_SC_LIVE, S.spare.as<tgi_state_msg>());
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_rset.as<uint8_t>() + o_off, d_off, 8ull * (ns + 1), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t* off = (const uint64_t*)(S.h_rset.as<uint8_t>() + o_off);
+  const uint64_t total = S.h_sc.as<uint64_t>()[ST_SC_LIVE];
+  if (total != off[ns]) {
+    set_err(c, "%s: %llu live messages flagged, the rows count %llu", who, (unsigned long long)total, (unsigned long long)off[ns]);
+    return TGI_E_CUDA;
+  }
+  CK(S.h_rmsgs.ensure(std::max<uint64_t>(total, 1) * sizeof(tgi_state_msg)));
+  if (total) CK(cudaMemcpyAsync(S.h_rmsgs.p, S.spare.p, total * sizeof(tgi_state_msg), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&out->kernel_ms, S.t0, S.t1);
+  for (uint64_t k = 0; k < n; k++) {
+    const uint64_t j = std::lower_bound(set.begin(), set.end(), rows[k]) - set.begin();
+    first[k] = off[j];
+    pg[k].n_msgs = (uint32_t)(off[j + 1] - off[j]);
+  }
+  out->msgs = S.h_rmsgs.as<tgi_state_msg>();
+  out->n_msgs = total;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -4111,20 +4249,87 @@ int tgi_state_read_page(tgi_ctx* c, uint32_t row, tgi_state_msg* out, uint64_t c
   if ((rc = st_row_count(c, S, row, &cnt))) return rc;
   *n = cnt;
   if (!out || cap < cnt || !cnt) return TGI_OK;
-  cudaStream_t st = S.stream;
-  const uint64_t nm = S.n_msgs;
-  CK(S.flag.ensure(nm * 4));
-  CK(S.pos.ensure((nm + 1) * 8));
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.spare.ensure(cnt * sizeof(tgi_state_msg)));
-  const StDev d = st_dev(S);
-  uint32_t launches = 0;
-  st_live_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, row, S.flag.as<uint32_t>());
-  if ((rc = launch_scan(c, st, S.tiles, S.flag.as<uint32_t>(), nm, S.pos.as<uint64_t>(), S.sc.as<uint64_t>(), launches))) return rc;
-  st_read_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, S.flag.as<uint32_t>(), S.pos.as<uint64_t>(), S.spare.as<tgi_state_msg>());
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, S.spare.p, cnt * sizeof(tgi_state_msg), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  tgi_state_read_t r{};
+  if ((rc = st_read_rows(c, S, &row, 1, true, "tgi_state_read_page", &r))) return rc;
+  memcpy(out, r.msgs + r.msg_first[0], r.pages[0].n_msgs * sizeof(tgi_state_msg));
+  return TGI_OK;
+}
+
+int tgi_state_read_pages(tgi_ctx* c, const uint32_t* rows, uint64_t n, uint32_t flags, tgi_state_read_t* out) {
+  if (!c || !out || (n && !rows)) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  if (flags & ~TGI_READ_MESSAGES) { set_err(c, "tgi_state_read_pages: unknown flags 0x%x", flags); return TGI_E_ARG; }
+  for (uint64_t k = 0; k < n; k++)
+    if (rows[k] >= S.rows.size()) { set_err(c, "tgi_state_read_pages: no row %u (rows[%llu])", rows[k], (unsigned long long)k); return TGI_E_ARG; }
+  return st_read_rows(c, S, rows, n, flags & TGI_READ_MESSAGES, "tgi_state_read_pages", out);
+}
+
+int tgi_state_read_layer(tgi_ctx* c, int64_t depth, int select, uint32_t flags, tgi_state_read_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  if (flags & ~TGI_READ_MESSAGES) { set_err(c, "tgi_state_read_layer: unknown flags 0x%x", flags); return TGI_E_ARG; }
+  if (select < TGI_SELECT_NONE || select > TGI_SELECT_DAPR) { set_err(c, "tgi_state_read_layer: unknown selection %d", select); return TGI_E_ARG; }
+  const auto it = S.layers.find(depth);  // base.go:329-332: no layer, no pages
+  const uint32_t* rows = it == S.layers.end() ? nullptr : it->second.data();
+  const uint64_t n = it == S.layers.end() ? 0 : it->second.size();
+  if ((rc = st_read_rows(c, S, rows, n, flags & TGI_READ_MESSAGES, "tgi_state_read_layer", out))) return rc;
+  if (select == TGI_SELECT_NONE) return TGI_OK;
+  CK(S.h_rsel.ensure(std::max<uint64_t>(n, 1)));
+  uint8_t* sel = S.h_rsel.as<uint8_t>();
+  std::unordered_set<std::string_view> seen;  // processLayerInParallel's uniquePages
+  uint64_t picked = 0;
+  for (uint64_t k = 0; k < n; k++) {
+    const tgi_state_page& p = S.rows[rows[k]];
+    const std::string_view status = st_view(S, p, TGI_PS_STATUS);
+    bool on = true;  // TGI_SELECT_STANDALONE: a new execution processes every page (standalone/runner.go:636-694)
+    if (select == TGI_SELECT_STANDALONE_RESUME) {
+      on = status != "fetched";  // the startIndex scan and the in-loop skip (:636-671, 672-694)
+    } else if (select == TGI_SELECT_DAPR) {
+      // dapr/standalone.go:459-463 records the URL before the status test at :477-497 (resuming: :420)
+      on = seen.insert(st_view(S, p, TGI_PS_URL)).second && status != "fetched" && status != "error";
+    }
+    sel[k] = on;
+    picked += on;
+  }
+  out->select = sel;
+  out->n_selected = picked;
+  return TGI_OK;
+}
+
+int tgi_state_layers(tgi_ctx* c, tgi_state_layers_t* out) {
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  const uint64_t nl = S.layers.size();
+  CK(S.h_rdepth.ensure(std::max<uint64_t>(nl, 1) * 8));
+  CK(S.h_rcount.ensure(std::max<uint64_t>(nl, 1) * 8));
+  int64_t* depth = S.h_rdepth.as<int64_t>();
+  uint64_t* count = S.h_rcount.as<uint64_t>();
+  int64_t max_depth = -1;  // base.go:450-455: only a depth above -1 counts
+  uint64_t k = 0, incomplete = 0;
+  for (const auto& [dp, L] : S.layers) {
+    depth[k] = dp;
+    count[k++] = L.size();
+    max_depth = std::max<int64_t>(max_depth, dp);
+    for (uint32_t r : L) incomplete += st_view(S, S.rows[r], TGI_PS_STATUS) != "fetched";  // base.go:485-495
+  }
+  out->n_layers = nl;
+  out->depth = depth;
+  out->n_pages = count;
+  out->max_depth = max_depth;
+  out->has_max_depth = max_depth != -1;
+  out->n_incomplete = incomplete;
   return TGI_OK;
 }
 

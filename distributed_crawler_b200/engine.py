@@ -41,6 +41,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
+    "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers",
 ]
 
 
@@ -129,6 +130,9 @@ def lib() -> C.CDLL:
         L.tgi_state_discover.argtypes = [vp, i32, vp, u32, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         L.tgi_state_next_layer.argtypes = [vp, C.c_int64, u32, C.c_int64, i32, C.c_int64, C.POINTER(abi.StateAddedC)]
         L.tgi_state_pending_edges.argtypes = [vp, i32, vp, u32, C.c_int64, C.POINTER(abi.StateEdgesC)]
+        L.tgi_state_read_pages.argtypes = [vp, vp, u64, u32, C.POINTER(abi.StateReadC)]
+        L.tgi_state_read_layer.argtypes = [vp, C.c_int64, i32, u32, C.POINTER(abi.StateReadC)]
+        L.tgi_state_layers.argtypes = [vp, C.POINTER(abi.StateLayersC)]
         _LIB = L
     return _LIB
 
@@ -646,6 +650,81 @@ class Engine:
         return [{"chatId": int(m["chat_id"]), "messageId": int(m["message_id"]), "status": names[int(m["status"])],
                  "pageId": ids[int(m["page_id"])], "platform": names[int(m["platform"])]}
                 for m in self.state_read_page_arrays(row)]
+
+    # --- layer reads: GetPage / GetLayerByDepth of many rows, GetMaxDepth, FindIncompleteCrawl's page test ---------------
+    def _st_read_arrays(self, out: abi.StateReadC) -> dict:
+        n = int(out.n_pages)
+        self.state_read_ms = float(out.kernel_ms)
+        self.state_read_launches = int(out.gpu_launches)
+        res = {"rows": _view(out.rows, n, np.uint32).copy(), "pages": _view(out.pages, n, abi.STATE_PAGE).copy(),
+               "strs": C.string_at(out.strs, out.strs_len) if out.strs_len else b"",
+               "msgs": _view(out.msgs, int(out.n_msgs), abi.STATE_MSG).copy() if out.msgs else None,
+               "msg_first": _view(out.msg_first, n, np.uint64).copy() if out.msg_first else None,
+               "select": _view(out.select, n, np.uint8).copy() if out.select else None,
+               "n_selected": int(out.n_selected)}
+        return res
+
+    def state_read_pages_arrays(self, rows, flags: int = abi.READ_MESSAGES) -> dict:
+        """tgi_state_read_pages as arrays: {"rows", "pages" (abi.STATE_PAGE, n_msgs = the list's length), "strs", "msgs"
+        (abi.STATE_MSG) and "msg_first" (None without abi.READ_MESSAGES), "select" (None), "n_selected"}"""
+        rows = np.ascontiguousarray(rows, np.uint32)
+        out = abi.StateReadC()
+        self._check(lib().tgi_state_read_pages(self.h, rows.ctypes.data if len(rows) else None, len(rows), flags,
+                                               C.byref(out)))
+        return self._st_read_arrays(out)
+
+    def state_read_layer_arrays(self, depth: int, select: int = abi.SELECT_NONE, flags: int = abi.READ_MESSAGES) -> dict:
+        """tgi_state_read_layer as arrays, as state_read_pages_arrays returns them ("select": 1 per processed page)"""
+        out = abi.StateReadC()
+        self._check(lib().tgi_state_read_layer(self.h, depth, select, flags, C.byref(out)))
+        return self._st_read_arrays(out)
+
+    def _st_pages(self, a: dict) -> list[dict]:
+        """the read's pages as state_pack dicts: every string, depth, timestamp (offset None for time.Local) and, when
+        the lists were read, "messages" (pageIds by the rows this engine has seen)"""
+        names = {v: k for k, v in self.__dict__.get("_st_codes", {}).items()}
+        names.update({i: c.encode() for i, c in enumerate(abi.STATE_CODES)})
+        ids = self.__dict__.get("_st_ids", [])
+        strs, pages = a["strs"], []
+        for k, r in enumerate(a["pages"]):
+            o, p = int(r["str_off"]), {}
+            for f, name in enumerate(abi.STATE_STRINGS):
+                ln = int(r["str_len"][f])
+                p[name] = strs[o:o + ln]
+                o += ln
+            off = int(r["ts_off"])
+            p["depth"] = int(r["depth"])
+            p["timestamp"] = (int(r["ts_sec"]), int(r["ts_nsec"]), None if off == abi.STATE_TS_LOCAL else off)
+            if a["msgs"] is not None:
+                f0 = int(a["msg_first"][k])
+                p["messages"] = [{"chatId": int(m["chat_id"]), "messageId": int(m["message_id"]),
+                                  "status": names[int(m["status"])], "pageId": ids[int(m["page_id"])],
+                                  "platform": names[int(m["platform"])]}
+                                 for m in a["msgs"][f0:f0 + int(r["n_msgs"])]]
+            pages.append(p)
+        return pages
+
+    def state_read_pages(self, rows, messages: bool = True) -> list[dict]:
+        """GetPage of every row, in order (a row listed twice comes back twice)"""
+        return self._st_pages(self.state_read_pages_arrays(rows, abi.READ_MESSAGES if messages else 0))
+
+    def state_read_layer(self, depth: int, select: int = abi.SELECT_NONE, messages: bool = True):
+        """GetLayerByDepth(depth) -> (pages, selected): selected = one bool per page under the runner's selection
+        (abi.SELECT_*), None with abi.SELECT_NONE; the pages' rows are left in self.state_read_rows"""
+        a = self.state_read_layer_arrays(depth, select, abi.READ_MESSAGES if messages else 0)
+        self.state_read_rows = [int(r) for r in a["rows"]]
+        return self._st_pages(a), None if a["select"] is None else [bool(x) for x in a["select"]]
+
+    def state_layers(self) -> dict:
+        """{"layers": [(depth, listed pages)] in ascending depth, "max_depth": GetMaxDepth or None for "no layers found",
+        "n_incomplete": listed pages whose status is not "fetched"}"""
+        out = abi.StateLayersC()
+        self._check(lib().tgi_state_layers(self.h, C.byref(out)))
+        n = int(out.n_layers)
+        depth = _view(out.depth, n, np.int64).tolist() if n else []
+        count = _view(out.n_pages, n, np.uint64).tolist() if n else []
+        return {"layers": [(int(d), int(c)) for d, c in zip(depth, count)],
+                "max_depth": int(out.max_depth) if out.has_max_depth else None, "n_incomplete": int(out.n_incomplete)}
 
     def state_render(self, metadata: bytes, last_updated: bytes, copy: bool = True):
         """json.Marshal(GetState()) with the shim's marshalled metadata and lastUpdated spliced in (copy=False: a view of

@@ -458,6 +458,33 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return a;
   }
+  // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
+  // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
+  // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.
+  tgi_state_read_t ReadLayer(int64_t depth, int select, bool messages) {
+    tgi_state_read_t o{};
+    if (tgi_state_read_layer(ctx_, depth, select, messages ? TGI_READ_MESSAGES : 0u, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  tgi_state_read_t ReadPages(const std::vector<uint32_t>& rows, bool messages) {
+    tgi_state_read_t o{};
+    if (tgi_state_read_pages(ctx_, rows.data(), rows.size(), messages ? TGI_READ_MESSAGES : 0u, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  // the rows the read's selection processes, in layer order (every row without a selection)
+  static std::vector<uint32_t> SelectedRows(const tgi_state_read_t& r) {
+    std::vector<uint32_t> out;
+    for (uint64_t k = 0; k < r.n_pages; k++)
+      if (!r.select || r.select[k]) out.push_back(r.rows[k]);
+    return out;
+  }
+  tgi_state_layers_t Layers() {
+    tgi_state_layers_t o{};
+    if (tgi_state_layers(ctx_, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   tgi_ctx* Raw() { return ctx_; }
 
  private:

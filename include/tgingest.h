@@ -815,7 +815,7 @@ int tgi_set_info(tgi_ctx* ctx, int which, tgi_set_info_t* out);
  *            status, pageId = the page} and later updates of it hit the appended message.  An update whose row is
  *            TGI_STATE_NO_PAGE is skipped and counted in *skipped (the reference returns an error its caller ignores).
  *   Read     tgi_state_read_page = GetPage(id).Messages: *n = the row's message count; the messages are written
- *            when cap >= *n.
+ *            when cap >= *n, gathered as tgi_state_read_pages gathers them (its n = 1 case).
  *   Render   tgi_state_render = json.Marshal(GetState()) (base.go:345-372), byte for byte: {"layers":[...],
  *            "metadata":<metadata>,"lastUpdated":<last_updated>} where the two spliced values are the shim's own
  *            json.Marshal of CrawlMetadata and of the time.  Layers in ascending depth (Go iterates layerMap in
@@ -1174,6 +1174,73 @@ typedef struct tgi_state_edges_t {
 } tgi_state_edges_t;
 int tgi_state_pending_edges(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
                             tgi_state_edges_t* out);
+
+/* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
+ * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on
+ * the device never holds a copy of the page table: layer read, tgi_state_pages_begin of the selected rows, one bulk
+ * batch, tgi_state_pages_end, tgi_state_discover, tgi_state_pages_close, tgi_state_next_layer, next layer read.
+ *   Pages    tgi_state_read_pages = GetPage(id) (base.go:110-120) of rows[0 .. n) in one call.  out->pages[k] is row
+ *            out->rows[k] = rows[k]'s record as stored, its strings at out->strs + pages[k].str_off (a TGI_STATE_TS_LOCAL timestamp
+ *            stays TGI_STATE_TS_LOCAL).  TGI_READ_MESSAGES: page k's list is msgs[msg_first[k] .. msg_first[k] +
+ *            pages[k].n_msgs), the row's live messages in list order, page_id as tgi_state_read_page gives it; a row
+ *            requested twice is returned twice and its list may be stored once, so msg_first need not increase.
+ *            Without the flag n_msgs is 0, msgs and msg_first are NULL and nothing is launched.
+ *   Layer    tgi_state_read_layer = GetLayerByDepth(depth) (base.go:325-342): the rows of the layer in list order, as
+ *            tgi_state_read_pages returns them, out->rows naming them; a row the layer lists twice is returned twice.  A depth without a
+ *            layer gives 0 pages, as Base returns [].  DaprStateManager's override (daprstate.go:3014-3074) differs only
+ *            when a listed id is missing from pageMap, which a row of the device state never is.  select fills
+ *            out->select[k] (1: the runner processes page k) and out->n_selected:
+ *            TGI_SELECT_NONE   nothing (select NULL).
+ *            TGI_SELECT_STANDALONE  a new execution: every page (standalone/runner.go:636-694).
+ *            TGI_SELECT_STANDALONE_RESUME  the same execution resumed: every page whose status is not "fetched" (the
+ *                              startIndex scan and the in-loop skip together).
+ *            TGI_SELECT_DAPR   processLayerInParallel (dapr/standalone.go:454-498, which always resumes: :420): the first
+ *                              page of every URL, byte for byte, and only if its status is neither "fetched" nor
+ *                              "error".  The URL is recorded before the status test, so a fetched first page hides a
+ *                              later unfetched page with the same URL.
+ *            The selected rows go to tgi_state_pages_begin as they are.
+ *   Layers   tgi_state_layers: every layer's depth and listed pages in ascending depth; GetMaxDepth (base.go:446-462):
+ *            max_depth = the largest depth above -1, has_max_depth = 0 when there is none (its "no layers found": a
+ *            state whose layers all lie at depth -1 or below has none); n_incomplete = the listed pages whose status is
+ *            not "fetched", a row listed twice counted twice (FindIncompleteCrawl's in-memory test, base.go:482-502, is
+ *            n_incomplete > 0).  Host mirror only: nothing is launched.
+ *   Cost     with TGI_READ_MESSAGES, one pass over the message rows per call whatever n: flags of the live messages of
+ *            the distinct rows, a scan, the render's stable radix passes (their number set by the state's row count),
+ *            the rows' counts and their scan, one gather.  The launches do not depend on n; two synchronises (the
+ *            lists' lengths, then the lists).  tgi_state_read_page is its n = 1 case.
+ *   Errors   TGI_E_ARG, the state unchanged: an unknown row, unknown flags or selection, rows NULL with n > 0.  The
+ *            state lock only (no slot is read).  All of out lives in pinned memory until the next state call.       */
+#define TGI_READ_MESSAGES 1u
+#define TGI_SELECT_NONE 0
+#define TGI_SELECT_STANDALONE 1
+#define TGI_SELECT_STANDALONE_RESUME 2
+#define TGI_SELECT_DAPR 3
+typedef struct tgi_state_read_t {
+  uint64_t n_pages;
+  const uint32_t* rows;          /* [n_pages] each page's row (pinned)                                               */
+  const tgi_state_page* pages;   /* [n_pages] the rows' records; str_off into strs, n_msgs = the list's length (pinned) */
+  const uint8_t* strs;           /* the pages' strings (pinned)                                                     */
+  uint64_t strs_len;
+  const tgi_state_msg* msgs;     /* [n_msgs] with TGI_READ_MESSAGES: the distinct rows' lists (pinned), else NULL   */
+  const uint64_t* msg_first;     /* [n_pages] page k's list starts at msgs[msg_first[k]] (pinned), else NULL        */
+  uint64_t n_msgs;
+  const uint8_t* select;         /* [n_pages] tgi_state_read_layer with a selection: 1 = processed (pinned), else NULL */
+  uint64_t n_selected;
+  float kernel_ms;               /* device time of the call's kernels and scans (not the copies)                   */
+  uint32_t gpu_launches;
+} tgi_state_read_t;
+typedef struct tgi_state_layers_t {
+  uint64_t n_layers;
+  const int64_t* depth;          /* [n_layers] ascending (pinned)                                                   */
+  const uint64_t* n_pages;       /* [n_layers] the ids each layer lists (pinned)                                     */
+  int64_t max_depth;             /* GetMaxDepth: the largest depth above -1, else -1                                 */
+  uint32_t has_max_depth;        /* 0: GetMaxDepth's "no layers found"                                               */
+  uint32_t reserved;
+  uint64_t n_incomplete;         /* listed pages whose status is not "fetched"                                       */
+} tgi_state_layers_t;
+int tgi_state_read_pages(tgi_ctx* ctx, const uint32_t* rows, uint64_t n, uint32_t flags, tgi_state_read_t* out);
+int tgi_state_read_layer(tgi_ctx* ctx, int64_t depth, int select, uint32_t flags, tgi_state_read_t* out);
+int tgi_state_layers(tgi_ctx* ctx, tgi_state_layers_t* out);
 
 /* pure helpers exposed for host code and tests (each runs the device code path on tiny inputs) */
 int tgi_filter_usernames(tgi_ctx* ctx, const uint8_t* names, const uint32_t* off, uint64_t n,
