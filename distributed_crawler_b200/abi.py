@@ -247,6 +247,20 @@ class StateEdgesC(C.Structure):  # tgi_state_edges_t
                 ("gpu_launches", C.c_uint32)]
 
 
+# tgi_state_edge_sql: the statement kinds (CreatePendingBatch, InsertPendingEdge, ClosePendingBatch) and the largest
+# rows_per_stmt (8 bind parameters per edge row, at most 65535 per Postgres statement)
+SQL_BATCH_INSERT, SQL_EDGE_INSERT, SQL_BATCH_CLOSE = 0, 1, 2
+SQL_MAX_ROWS = 8191
+STATE_EDGE_STMT = np.dtype([("kind", "<u4"), ("rows", "<u4"), ("sql_off", "<u8"), ("sql_len", "<u8"),
+                            ("params_off", "<u8"), ("params_len", "<u8")])  # tgi_state_edge_stmt
+assert STATE_EDGE_STMT.itemsize == 40
+
+
+class StateEdgeSqlC(C.Structure):  # tgi_state_edge_sql_t
+    _fields_ = [("n_stmts", C.c_uint64), ("stmts", C.c_void_p), ("data", C.c_void_p), ("data_len", C.c_uint64),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
 # tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
 SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3

@@ -1010,6 +1010,118 @@ __global__ void st_edge_emit_kernel(StEdges e) {
   }
 }
 
+// ---- tandem hand-off SQL (state/daprstate.go:3643-3678, 3896-3941): the params of every binding call ----------------
+// Rows are numbered batch inserts [0, nb), edge inserts [nb, nb + ne), batch closes [nb + ne, 2 nb + ne); a statement
+// holds k consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names, URLs),
+// which the sequential escaper handles without the warp's 128-byte strips idling most lanes.
+struct StSql {
+  const tgi_state_edge* edges;          // the hand-off, as tgi_state_pending_edges left it on the device
+  const tgi_state_edge_batch* batches;
+  const tgi_state_span* spans;
+  uint64_t ne, nb, n_rows;
+  uint32_t k;                           // rows per statement
+  uint32_t crawl_len, time_len;
+  const uint8_t* crawl;                 // crawl_id as given, then discovery_time rendered with its quotes
+  const uint8_t* time;
+  uint32_t* size;                       // [n_rows] bytes of row r
+  uint64_t* off;                        // [n_rows+1] their scan
+  uint8_t* out;
+  tgi_state_edge_stmt* stmts;           // [n_stmts]
+  uint64_t n_stmts, m[3];               // statements in all and of each kind
+  uint64_t sql_off[6], sql_len[6];      // the texts of kind i: [2i] k rows, [2i+1] the kind's last, shorter statement
+  uint64_t base;                        // the params' offset in the output
+};
+
+// one row's values, sized (dst == nullptr) or written, with the statement's "[" before its first row, "," before the
+// others and "]" after its last
+template <bool EMIT>
+DEVI uint32_t st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* dst) {
+  uint32_t o = 0;
+  auto lit = [&](const char* s, uint32_t n) {
+    if (EMIT)
+      for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
+    o += n;
+  };
+  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len(s, n); };
+  auto str = [&](const uint8_t* s, uint32_t n) {
+    lit("\"", 1);
+    esc(s, n);
+    lit("\"", 1);
+  };
+  auto field = [&](const tgi_state_page& p, int f) {
+    uint32_t n;
+    const uint8_t* s = st_str(d, p, f, n);
+    str(s, n);
+  };
+  const uint32_t kind = r < q.nb ? 0u : r < q.nb + q.ne ? 1u : 2u;
+  const uint64_t i = kind == 0 ? r : kind == 1 ? r - q.nb : r - q.nb - q.ne;  // the row within its kind
+  const uint64_t n = kind == 1 ? q.ne : q.nb;
+  lit(i % q.k ? "," : "[", 1);
+  const tgi_state_edge* e = kind == 1 ? q.edges + i : nullptr;
+  const tgi_state_edge_batch& b = q.batches[e ? e->batch : (uint32_t)i];
+  str(b.batch_id, 36);
+  if (kind != 2) {
+    const tgi_state_page& p = d.pages[q.spans[b.span].row];  // the owner
+    lit(",", 1);
+    str(q.crawl, q.crawl_len);
+    lit(",", 1);
+    if (kind == 0) {  // CreatePendingBatch (daprstate.go:3897-3906)
+      field(p, TGI_PS_URL);
+      lit(",", 1);
+      field(p, TGI_PS_ID);
+      lit(",", 1);
+      o += EMIT ? (uint32_t)render_i64(dst + o, p.depth) : ndigits_i64(p.depth);
+      lit(",", 1);
+      field(p, TGI_PS_SEQ);
+      lit(",\"open\"", 7);
+    } else {  // InsertPendingEdge (:3915-3926)
+      str(e->destination, e->dest_len);
+      lit(",", 1);
+      field(p, TGI_PS_URL);
+      lit(",", 1);
+      field(p, TGI_PS_SEQ);
+      lit(",", 1);
+      if (EMIT)
+        for (uint32_t k = 0; k < q.time_len; k++) dst[o + k] = q.time[k];
+      o += q.time_len;
+      switch (e->source_type) {  // tdutils.go:978-987
+        case TGI_SRC_MENTION: lit(",\"mention\"", 10); break;
+        case TGI_SRC_TEXT_URL: lit(",\"text_url\"", 11); break;
+        case TGI_SRC_URL: lit(",\"url\"", 6); break;
+        default: lit(",\"plaintext\"", 12); break;
+      }
+      lit(",\"pending\"", 10);
+    }
+  }
+  if (i % q.k == q.k - 1 || i == n - 1) lit("]", 1);
+  return o;
+}
+
+__global__ void st_sql_size_kernel(StDev d, StSql q) {
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    q.size[r] = st_sql_row<false>(d, q, r, nullptr);
+}
+
+// the rows at their scanned offsets, then every statement's entry: its rows, its kind's text, its params' span
+__global__ void st_sql_emit_kernel(StDev d, StSql q) {
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    st_sql_row<true>(d, q, r, q.out + q.off[r]);
+  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < q.n_stmts; s += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t kind = s < q.m[0] ? 0u : s < q.m[0] + q.m[1] ? 1u : 2u;
+    const uint64_t j = kind == 0 ? s : kind == 1 ? s - q.m[0] : s - q.m[0] - q.m[1];
+    const uint64_t n = kind == 1 ? q.ne : q.nb, first = (kind == 0 ? 0 : kind == 1 ? q.nb : q.nb + q.ne) + j * q.k;
+    const uint32_t rows = (uint32_t)min((uint64_t)q.k, n - j * q.k);
+    const uint32_t t = 2 * kind + (rows != q.k);
+    tgi_state_edge_stmt& st = q.stmts[s];
+    st.kind = kind;
+    st.rows = rows;
+    st.sql_off = q.sql_off[t];
+    st.sql_len = q.sql_len[t];
+    st.params_off = q.base + q.off[first];
+    st.params_len = q.off[first + rows] - q.off[first];
+  }
+}
+
 // ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------
 struct StLmEntry {  // one id of a layer, or an empty layer (row == ST_NONE)
   uint32_t row;

@@ -7,6 +7,7 @@
 #include <nccl.h>  // types only: the library itself is loaded with dlopen at tgi_comm_init
 
 #include <algorithm>
+#include <charconv>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -248,6 +249,12 @@ struct CrawlState {
   uint64_t batch_next = 0;
   DevBuf clink, edges, ebatches, span_batch;
   HostBuf h_edges, h_ebatches, h_span_batch;
+  // tandem hand-off SQL (tgi_state_edge_sql): whether the last state call was an accepted hand-off, whose edges,
+  // batches and spans above then still hold it; the rows' sizes and offsets, and the pinned output
+  bool handoff_live = false;
+  uint64_t handoff_ne = 0, handoff_nb = 0;
+  DevBuf sql_in, sql_size, sql_off, sql_out, sql_stmts;
+  HostBuf h_sql, h_sql_stmts;
   // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
   // device and its staging, and the pinned outputs
   DevBuf rset;
@@ -3439,9 +3446,11 @@ bool page_ok(tgi_ctx* c, const tgi_state_page& p, const uint8_t* strs, uint64_t 
   return true;
 }
 
-// the state's stream, events, preset codes and minimal buffers, on first use (under S.mu)
+// the state's stream, events, preset codes and minimal buffers, on first use (under S.mu).  Every state call but
+// tgi_state_edge_sql passes here, so this is also where the hand-off it renders ends.
 int st_init(tgi_ctx* c, CrawlState& S) {
   cudaSetDevice(c->device);
+  S.handoff_live = false;
   if (S.stream) return TGI_OK;
   CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
   CK(cudaEventCreate(&S.t0));
@@ -5570,6 +5579,45 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
   return TGI_OK;
 }
 
+// The SQL text of a statement of `rows` rows (TGI_SQL_*): for one row the literal of CreatePendingBatch,
+// InsertPendingEdge or ClosePendingBatch (state/daprstate.go:3897, 3915, 3935); for more the VALUES tuple repeated with
+// the placeholders numbered on, or the close's WHERE batch_id IN (...)
+void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
+  static const char* const head[3] = {
+      "INSERT INTO pending_edge_batches (batch_id, crawl_id, source_channel, source_page_id, source_depth, sequence_id, "
+      "status) VALUES ",
+      "INSERT INTO pending_edges (batch_id, crawl_id, destination_channel, source_channel, sequence_id, discovery_time, "
+      "source_type, validation_status) VALUES ",
+      "UPDATE pending_edge_batches SET status = 'closed', closed_at = NOW() WHERE batch_id "};
+  const uint32_t per = kind == TGI_SQL_BATCH_INSERT ? 7 : kind == TGI_SQL_EDGE_INSERT ? 8 : 1;
+  s = head[kind];
+  s.reserve(s.size() + (size_t)rows * (per * 8 + 4) + 8);
+  char num[16] = {'$'};
+  auto param = [&](uint32_t p) { s.append(num, (size_t)(std::to_chars(num + 1, num + sizeof num, p).ptr - num)); };
+  if (kind == TGI_SQL_BATCH_CLOSE) {
+    if (rows == 1) {
+      s += "= $1;";
+      return;
+    }
+    s += "IN (";
+    for (uint32_t r = 0; r < rows; r++) {
+      if (r) s += ", ";
+      param(r + 1);
+    }
+    s += ");";
+    return;
+  }
+  for (uint32_t r = 0; r < rows; r++) {
+    s += r ? ", (" : "(";
+    for (uint32_t k = 0; k < per; k++) {
+      if (k) s += ", ";
+      param(r * per + k + 1);
+    }
+    s += ")";
+  }
+  s += ";";
+}
+
 }  // namespace
 
 extern "C" {
@@ -5729,6 +5777,8 @@ int tgi_state_pending_edges(tgi_ctx* c, int slot, const tgi_state_span* spans, u
   out->span_batch = S.h_span_batch.as<uint32_t>();
   if (!bound) {  // no processed link row: no edge, no batch
     std::fill_n(S.h_span_batch.as<uint32_t>(), n_spans, TGI_STATE_NO_BATCH);
+    S.handoff_live = true;
+    S.handoff_ne = S.handoff_nb = 0;
     return TGI_OK;
   }
   cudaStream_t st = S.stream;
@@ -5813,12 +5863,124 @@ int tgi_state_pending_edges(tgi_ctx* c, int slot, const tgi_state_span* spans, u
   CK(cudaMemcpyAsync(S.h_span_batch.p, S.span_batch.p, n_spans * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   S.batch_next += n_batches;
+  S.handoff_live = true;  // S.edges, S.ebatches and S.spans hold it until the next state call
+  S.handoff_ne = n_edges;
+  S.handoff_nb = n_batches;
   out->n_candidates = hs[3];
   out->n_edges = n_edges;
   out->n_batches = (uint32_t)n_batches;
   out->edges = S.h_edges.as<tgi_state_edge>();
   out->batches = S.h_ebatches.as<tgi_state_edge_batch>();
   out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The binding calls of the last hand-off: the texts on the host (one per kind and row count), the params on the device
+// (a thread per row sizes it, a scan, a thread per row writes it and the emit also fills the statement table); one
+// synchronise for the params' length, one for the read-back
+int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                       uint32_t rows_per_stmt, tgi_state_edge_sql_t* out) {
+  static const char* const who = "tgi_state_edge_sql";
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  cudaSetDevice(c->device);  // not st_init: that would end the hand-off
+  const uint32_t k = rows_per_stmt;
+  if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
+  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
+  if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
+  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off to render (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  const uint64_t nb = S.handoff_nb, ne = S.handoff_ne;
+  char tb[48];
+  uint32_t tl = 0;
+  if (ne) {
+    std::lock_guard<std::mutex> zg(c->cfg_mu);
+    tl = (uint32_t)host_render_zone_time(tb, now_sec, now_nsec, c->zone, c->cfgdev.tz);
+    if (!tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  }
+  memset(out, 0, sizeof *out);
+  if (!nb) return TGI_OK;
+  // the statements: ceil(n / k) per kind, and the texts of their row counts (a kind's last statement may be shorter)
+  const uint64_t m[3] = {(nb + k - 1) / k, (ne + k - 1) / k, (nb + k - 1) / k};
+  const uint64_t n_stmts = m[0] + m[1] + m[2], n_rows = 2 * nb + ne;
+  StSql q{};
+  std::string texts, t;
+  for (uint32_t kind = 0; kind < 3; kind++) {
+    const uint64_t n = kind == TGI_SQL_EDGE_INSERT ? ne : nb;
+    const uint32_t rows[2] = {n >= k ? k : 0u, (uint32_t)(n % k)};
+    for (int j = 0; j < 2; j++) {
+      if (!rows[j]) continue;
+      edge_sql_text(kind, rows[j], t);
+      q.sql_off[2 * kind + j] = texts.size();
+      q.sql_len[2 * kind + j] = t.size();
+      texts += t;
+    }
+  }
+  cudaStream_t st = S.stream;
+  const size_t t_at = (crawl_id_len + 15) & ~(size_t)15;
+  CK(S.sql_in.ensure(t_at + sizeof tb));
+  CK(S.sql_size.ensure(n_rows * 4));
+  CK(S.sql_off.ensure((n_rows + 1) * 8));
+  CK(S.sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  std::vector<uint8_t> in(t_at + tl);
+  if (crawl_id_len) memcpy(in.data(), crawl_id, crawl_id_len);
+  if (tl) memcpy(in.data() + t_at, tb, tl);
+  if (!in.empty()) CK(cudaMemcpyAsync(S.sql_in.p, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  q.edges = S.edges.as<tgi_state_edge>();
+  q.batches = S.ebatches.as<tgi_state_edge_batch>();
+  q.spans = S.spans.as<tgi_state_span>();
+  q.ne = ne;
+  q.nb = nb;
+  q.n_rows = n_rows;
+  q.k = k;
+  q.crawl = S.sql_in.as<uint8_t>();
+  q.crawl_len = crawl_id_len;
+  q.time = q.crawl + t_at;
+  q.time_len = tl;
+  q.size = S.sql_size.as<uint32_t>();
+  q.off = S.sql_off.as<uint64_t>();
+  q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
+  q.n_stmts = n_stmts;
+  for (int j = 0; j < 3; j++) q.m[j] = m[j];
+  q.base = texts.size();
+  const StDev d = st_dev(S);
+  const unsigned grid = sink_grid(c, std::max(n_rows, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
+  uint32_t launches = 0;
+  int rc;
+  CK(cudaEventRecord(S.t0, st));
+  st_sql_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, q.size, n_rows, q.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
+  CK(S.sql_out.ensure(body));
+  CK(S.h_sql.ensure(texts.size() + body));
+  CK(S.h_sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
+  q.out = S.sql_out.as<uint8_t>();
+  CK(cudaEventRecord(S.t2, st));
+  st_sql_emit_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  uint8_t* h = S.h_sql.as<uint8_t>();
+  CK(cudaMemcpyAsync(h + texts.size(), S.sql_out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_sql_stmts.p, S.sql_stmts.p, n_stmts * sizeof(tgi_state_edge_stmt), cudaMemcpyDeviceToHost, st));
+  memcpy(h, texts.data(), texts.size());  // beside the copies: another part of the buffer
+  CK(cudaStreamSynchronize(st));
+  float ms = 0, t2 = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  cudaEventElapsedTime(&t2, S.t2, S.t3);
+  out->n_stmts = n_stmts;
+  out->stmts = S.h_sql_stmts.as<tgi_state_edge_stmt>();
+  out->data = h;
+  out->data_len = texts.size() + body;
+  out->kernel_ms = ms + t2;
   out->gpu_launches = launches;
   return TGI_OK;
 }

@@ -41,7 +41,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_add_pages", "tgi_state_export", "tgi_state_page_begin", "tgi_state_page_end",
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
-    "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers",
+    "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers", "tgi_state_edge_sql",
 ]
 
 
@@ -133,6 +133,7 @@ def lib() -> C.CDLL:
         L.tgi_state_read_pages.argtypes = [vp, vp, u64, u32, C.POINTER(abi.StateReadC)]
         L.tgi_state_read_layer.argtypes = [vp, C.c_int64, i32, u32, C.POINTER(abi.StateReadC)]
         L.tgi_state_layers.argtypes = [vp, C.POINTER(abi.StateLayersC)]
+        L.tgi_state_edge_sql.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateEdgeSqlC)]
         _LIB = L
     return _LIB
 
@@ -937,6 +938,20 @@ class Engine:
                 "batches": _view(out.batches, int(out.n_batches), abi.STATE_EDGE_BATCH).copy(),
                 "span_batch": _view(out.span_batch, len(spans), np.uint32).copy(),
                 "n_candidates": int(out.n_candidates)}
+
+    def state_edge_sql(self, crawl_id: bytes, now=(0, 0), rows_per_stmt: int = 1) -> list:
+        """the Postgres binding calls that store the last state_pending_edges (nothing but it since among the state
+        calls): every batch insert, every edge insert, every batch close, rows_per_stmt rows per statement.  Returns
+        [(kind (abi.SQL_*), rows, sql, params)]; the device time and launches are left in self.state_sql_ms and
+        self.state_sql_launches"""
+        out = abi.StateEdgeSqlC()
+        self._check(lib().tgi_state_edge_sql(self.h, crawl_id, len(crawl_id), now[0], now[1], rows_per_stmt, C.byref(out)))
+        self.state_sql_ms = float(out.kernel_ms)
+        self.state_sql_launches = int(out.gpu_launches)
+        st = _view(out.stmts, int(out.n_stmts), abi.STATE_EDGE_STMT)
+        data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
+        return [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
+                for k, r, so, sl, po, pl in st.tolist()]
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

@@ -458,6 +458,15 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return a;
   }
+  // Tandem hand-off SQL: the Postgres binding calls that store the last StatePendingEdges, rows_per_stmt rows per
+  // statement; statement k is an exec with metadata {"sql": data[sql_off, +sql_len), "params": data[params_off,
+  // +params_len)}.  The arrays stay valid until the next state call.
+  tgi_state_edge_sql_t StateEdgeSql(std::string_view crawl_id, int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt) {
+    tgi_state_edge_sql_t o{};
+    if (tgi_state_edge_sql(ctx_, crawl_id.data(), (uint32_t)crawl_id.size(), now_sec, now_nsec, rows_per_stmt, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
   // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
   // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.

@@ -1145,7 +1145,8 @@ int tgi_state_next_layer(tgi_ctx* ctx, int64_t layer_depth, uint32_t flags, int6
  *            as they were, and a successful one changes only the batch counter.  TGI_E_ARG: an unknown row, a span
  *            outside the result, n_done > n_records.  TGI_E_STATE: no, a released or a non-Telegram result, a result
  *            run without TGI_RUN_LINKS, a job in flight on the slot, no seed while a batch is due.  Lock order: the
- *            slot, then the state.  All of out lives until the next state call.                                        */
+ *            slot, then the state.  All of out lives until the next state call; the device-side edges, batches and
+ *            spans live as long, for tgi_state_edge_sql.                                                               */
 #define TGI_STATE_NO_BATCH 0xFFFFFFFFu
 typedef struct tgi_state_edge {        /* 48 bytes: one pending_edges row                                              */
   uint8_t destination[32];             /* destination_channel, lower-cased, zero padded                               */
@@ -1174,6 +1175,61 @@ typedef struct tgi_state_edges_t {
 } tgi_state_edges_t;
 int tgi_state_pending_edges(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
                             tgi_state_edges_t* out);
+
+/* Tandem hand-off SQL — the Postgres binding calls that store a hand-off: CreatePendingBatch, InsertPendingEdge and
+ * ClosePendingBatch (state/daprstate.go:3896-3941), each sent by ExecuteDatabaseOperation (:3643-3678) as an `exec`
+ * InvokeBinding with metadata {"sql": the text, "params": json.Marshal of its []any}.  The call renders them from the
+ * device-side edges, batches and spans of the context's last successful tgi_state_pending_edges; nothing is uploaded
+ * again but crawl_id and the clock.
+ *   Input    the last tgi_state_pending_edges.  Any other state call since (tgi_state_*, accepted or refused) ends it;
+ *            tgi_state_edge_sql does not, so one hand-off may be rendered many times, and the hand-off's own output
+ *            stays valid.  No hand-off to render is TGI_E_STATE.
+ *   Order    every batch insert, then every edge insert, then every batch close: a batch row exists before its edges
+ *            (pending_edges.batch_id REFERENCES pending_edge_batches) and is closed only after all of them are written
+ *            (crawl/runner.go:1414-1421).  Within a kind the hand-off's order: batches in span order, edges in (span,
+ *            record, link row) order, so the SERIAL pending_id comes out as with the reference's per-edge inserts.
+ *   Rows     rows_per_stmt = k rows per statement for each kind, the last statement of a kind holding the rest.
+ *            1 <= k <= 8191 (8 * 8191 bind parameters fit Postgres's 65535).  A statement's text depends only on its
+ *            kind and row count: one row is the reference's literal, byte for byte; more rows repeat the VALUES tuple
+ *            joined by ", " with the placeholders numbered on ("($1, ..., $8), ($9, ..., $16)"), and a close of more
+ *            rows is "WHERE batch_id IN ($1, $2, ...)".  Statements of one (kind, rows) share one copy of the text in
+ *            data.  params is one JSON array of the rows' values in order: cut into runs of 7 / 8 / 1 values it gives
+ *            json.Marshal of each row's []any, exactly what k = 1 sends.
+ *   Values   batch insert [batch_id, crawl_id, owner.URL, owner.ID, owner.Depth, owner.SequenceID, "open"]; edge insert
+ *            [batch_id, crawl_id, destination, owner.URL, owner.SequenceID, discovery_time, source_type, "pending"]
+ *            (crawl/runner.go:1276-1300; "pending" is InsertPendingEdge's literal, so a TGI_EDGE_DUPLICATE edge writes
+ *            it too); batch close [batch_id].  The owner is the batch's span row as the device state holds it; strings
+ *            take encoding/json's HTML-safe escaping, six characters \ufffd per invalid UTF-8 byte; Depth is a decimal int64;
+ *            source_type is "mention" | "text_url" | "url" | "plaintext" (TGI_SRC_*).
+ *   Clock    discovery_time = json.Marshal(time.Time) of (now_sec, now_nsec) in time.Local (tgi_set_zone, else
+ *            tz_offset_sec), RFC3339Nano with trailing zeros trimmed.  The reference reads time.Now() per edge; the
+ *            library reads the clock once per call, as discovery does, so every edge of a call has the same time.
+ *   Cost     a thread per row sizes it, a scan places it, a thread per row writes it and each statement's entry; two
+ *            launches and a scan, two synchronises.  A hand-off without batches gives 0 statements and launches nothing.
+ *   Errors   every check runs before anything is written: a refused call leaves the state, the batch counter and the
+ *            hand-off as they were.  TGI_E_ARG: k outside [1, 8191], now_nsec outside [0, 1e9), crawl_id NULL with a
+ *            length, and when the hand-off has edges a clock whose local year leaves [0, 9999] (json.Marshal fails).
+ *            TGI_E_STATE: no hand-off to render.  All of out lives in pinned memory until the next state call.        */
+#define TGI_SQL_BATCH_INSERT 0     /* CreatePendingBatch                                                              */
+#define TGI_SQL_EDGE_INSERT 1      /* InsertPendingEdge                                                               */
+#define TGI_SQL_BATCH_CLOSE 2      /* ClosePendingBatch                                                               */
+#define TGI_SQL_MAX_ROWS 8191u     /* 8 bind parameters per edge row, at most 65535 per statement                    */
+typedef struct tgi_state_edge_stmt {   /* 40 bytes: one exec InvokeBinding                                            */
+  uint32_t kind;                       /* TGI_SQL_*                                                                   */
+  uint32_t rows;
+  uint64_t sql_off, sql_len;           /* metadata "sql": data[sql_off .. sql_off + sql_len)                          */
+  uint64_t params_off, params_len;     /* metadata "params": data[params_off .. params_off + params_len)             */
+} tgi_state_edge_stmt;
+typedef struct tgi_state_edge_sql_t {
+  uint64_t n_stmts;
+  const tgi_state_edge_stmt* stmts;    /* [n_stmts] in execution order (pinned)                                       */
+  const uint8_t* data;                 /* the texts, then the params (pinned)                                         */
+  uint64_t data_len;
+  float kernel_ms;                     /* device time of the call's kernels and scan (not the copies)                 */
+  uint32_t gpu_launches;
+} tgi_state_edge_sql_t;
+int tgi_state_edge_sql(tgi_ctx* ctx, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                       uint32_t rows_per_stmt, tgi_state_edge_sql_t* out);
 
 /* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
  * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on
