@@ -261,6 +261,22 @@ class StateEdgeSqlC(C.Structure):  # tgi_state_edge_sql_t
                 ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+# tgi_state_walkback: its statement kinds (AddPageToPageBuffer, SaveEdgeRecords of one record), each edge-less span's
+# outcome (a channel picked; 10 draws of the owner's URL; no discovered channel) and pickWalkbackChannel's draws
+SQL_PAGE_BUFFER_INSERT, SQL_EDGE_RECORD_INSERT = 3, 4
+WALK_OK, WALK_EXHAUSTED, WALK_EMPTY = 0, 1, 2
+WALK_MAX_DRAWS = 10
+STATE_WALKBACK_SPAN = np.dtype([("span", "<u4"), ("status", "<u4"), ("draws", "<u4"), ("url_len", "<u4"),
+                                ("url", "u1", 32), ("page_id", "S36"), ("sequence_id", "S36")])  # tgi_state_walkback_span
+assert STATE_WALKBACK_SPAN.itemsize == 120
+
+
+class StateWalkbackC(C.Structure):  # tgi_state_walkback_t
+    _fields_ = [("n_walkbacks", C.c_uint32), ("reserved", C.c_uint32), ("walkbacks", C.c_void_p),
+                ("n_stmts", C.c_uint64), ("stmts", C.c_void_p), ("data", C.c_void_p), ("data_len", C.c_uint64),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
 # tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
 SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3

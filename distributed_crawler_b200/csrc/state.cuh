@@ -1122,6 +1122,172 @@ __global__ void st_sql_emit_kernel(StDev d, StSql q) {
   }
 }
 
+// ---- tandem forced walkback (crawl/runner.go:115-139, 1425-1455): the pick and the two rows of every edge-less span ---
+struct StWalk {
+  const uint32_t* spans;           // [n][2] every edge-less span's index and row, in span order
+  uint64_t n;
+  FrontierDev disc;                // TGI_SET_DISCOVERED (table == nullptr: never allocated)
+  uint64_t seed, w0;               // the id key, and the walkback counter of the first span
+  tgi_state_walkback_span* out;    // [n]
+  uint32_t* ok;                    // [n] 1: TGI_WALK_OK
+};
+
+// one span's pickWalkbackChannel(sm, owner.URL, nil) over the set's keys in first-occurrence order (Random() is
+// keys[rand.Intn(len(keys))], state/datamodels.go:152-162), and its two ids
+__global__ void st_walk_pick_kernel(StDev d, StWalk w) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < w.n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t wi = w.w0 + i, N = w.disc.table ? *w.disc.count : 0;
+    uint32_t ul;
+    const uint8_t* u = st_str(d, d.pages[w.spans[2 * i + 1]], TGI_PS_URL, ul);
+    tgi_state_walkback_span& o = w.out[i];
+    Key32 key{};
+    uint32_t status = TGI_WALK_EMPTY, draws = 0, klen = 0;
+    if (N) {
+      // the draw stream: word 2j and 2j + 1 are Philox block (w_lo, w_hi, 2, j)'s x0 | x1 << 32 and x2 | x3 << 32
+      uint32_t c[4];
+      uint64_t next = 0;
+      auto word = [&]() -> uint64_t {
+        if (!(next & 1)) {
+          c[0] = (uint32_t)wi, c[1] = (uint32_t)(wi >> 32), c[2] = 2u, c[3] = (uint32_t)(next >> 1);
+          philox4x32_10(c, (uint32_t)w.seed, (uint32_t)(w.seed >> 32));
+        }
+        return (next++ & 1) ? (c[2] | (uint64_t)c[3] << 32) : (c[0] | (uint64_t)c[1] << 32);
+      };
+      status = TGI_WALK_EXHAUSTED;
+      while (draws < TGI_WALK_MAX_DRAWS) {
+        draws++;
+        // Lemire's multiply-and-reject: exactly uniform on [0, N)
+        uint64_t x = word(), l = x * N;
+        if (l < N) {
+          const uint64_t t = (0 - N) % N;
+          while (l < t) l = (x = word()) * N;
+        }
+        key = load_key(w.disc.pool + 32 * __umul64hi(x, N));
+        klen = 32;
+        while (klen && !((key.w[(klen - 1) >> 2] >> (8 * ((klen - 1) & 3))) & 0xFF)) klen--;
+        bool self = klen == ul;  // url == sourceURL, byte for byte
+        for (uint32_t k = 0; self && k < ul; k++) self = ((key.w[k >> 2] >> (8 * (k & 3))) & 0xFF) == u[k];
+        if (!self) {
+          status = TGI_WALK_OK;
+          break;
+        }
+      }
+    }
+    if (status != TGI_WALK_OK) key = Key32{}, klen = 0;
+    o.span = w.spans[2 * i];
+    o.status = status;
+    o.draws = draws;
+    o.url_len = klen;
+    store_key(o.url, key);
+    st_uuid(w.seed, wi, 3u, o.page_id);
+    st_uuid(w.seed, wi, 4u, o.sequence_id);
+    w.ok[i] = status == TGI_WALK_OK;
+  }
+}
+
+// The SQL of the picks: rows page_buffer [0, n_ok), edge_records [n_ok, 2 n_ok) in span order, a statement k consecutive
+// rows of one kind, as StSql.  Thread t of [0, 2 n) stands for span t % n's row of kind t / n, which it has when the
+// span is TGI_WALK_OK; rank[i] is its place among those.
+struct StWalkSql {
+  const uint32_t* spans;               // StWalk's
+  const tgi_state_walkback_span* wb;   // [n] the picks
+  const uint64_t* rank;                // [n+1] scan of StWalk::ok
+  uint64_t n, n_ok;
+  uint32_t k;                          // rows per statement
+  uint32_t crawl_len, time_len;
+  const uint8_t* crawl;                // crawl_id as given, then discovery_time rendered with its quotes
+  const uint8_t* time;
+  uint32_t* size;                      // [2 n_ok] bytes of row r
+  uint64_t* off;                       // [2 n_ok + 1] their scan
+  uint8_t* out;
+  tgi_state_edge_stmt* stmts;          // [2 m]
+  uint64_t m;                          // statements of each kind
+  uint64_t sql_off[4], sql_len[4];     // the texts of kind i: [2i] k rows, [2i+1] the kind's last, shorter statement
+  uint64_t base;                       // the params' offset in the output
+};
+
+// one row's values, sized (dst == nullptr) or written, with the statement's "[" / "," / "]" as st_sql_row
+template <bool EMIT>
+DEVI uint32_t st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, uint64_t i, uint64_t j, uint8_t* dst) {
+  uint32_t o = 0;
+  auto lit = [&](const char* s, uint32_t n) {
+    if (EMIT)
+      for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
+    o += n;
+  };
+  auto str = [&](const uint8_t* s, uint32_t n) {
+    lit("\"", 1);
+    o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len(s, n);
+    lit("\"", 1);
+  };
+  auto field = [&](const tgi_state_page& p, int f) {
+    uint32_t n;
+    const uint8_t* s = st_str(d, p, f, n);
+    str(s, n);
+  };
+  const tgi_state_walkback_span& b = q.wb[i];
+  const tgi_state_page& p = d.pages[q.spans[2 * i + 1]];  // the owner
+  lit(j % q.k ? "," : "[", 1);
+  if (kind == 0) {  // AddPageToPageBuffer (daprstate.go:3620-3633)
+    str(b.page_id, 36);
+    lit(",", 1);
+    field(p, TGI_PS_ID);
+    lit(",", 1);
+    const int64_t depth = (int64_t)((uint64_t)p.depth + 1);  // owner.Depth + 1 wraps as Go's int
+    o += EMIT ? (uint32_t)render_i64(dst + o, depth) : ndigits_i64(depth);
+    lit(",", 1);
+    str(b.url, b.url_len);
+    lit(",", 1);
+    str(q.crawl, q.crawl_len);
+    lit(",", 1);
+    str(b.sequence_id, 36);
+  } else {  // SaveEdgeRecords of the walkback edge (:3176-3184)
+    str(b.url, b.url_len);
+    lit(",", 1);
+    field(p, TGI_PS_URL);
+    lit(",true,false,", 12);
+    if (EMIT)
+      for (uint32_t k = 0; k < q.time_len; k++) dst[o + k] = q.time[k];
+    o += q.time_len;
+    lit(",", 1);
+    str(q.crawl, q.crawl_len);
+    lit(",", 1);
+    field(p, TGI_PS_SEQ);
+  }
+  if (j % q.k == q.k - 1 || j == q.n_ok - 1) lit("]", 1);
+  return o;
+}
+
+__global__ void st_walk_size_kernel(StDev d, StWalkSql q) {
+  for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < 2 * q.n; t += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t kind = t >= q.n;
+    const uint64_t i = t - kind * q.n, j = q.rank[i];
+    if (q.rank[i + 1] > j) q.size[kind * q.n_ok + j] = st_walk_row<false>(d, q, kind, i, j, nullptr);
+  }
+}
+
+// the rows at their scanned offsets, then every statement's entry
+__global__ void st_walk_emit_kernel(StDev d, StWalkSql q) {
+  for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < 2 * q.n; t += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t kind = t >= q.n;
+    const uint64_t i = t - kind * q.n, j = q.rank[i];
+    if (q.rank[i + 1] > j) st_walk_row<true>(d, q, kind, i, j, q.out + q.off[kind * q.n_ok + j]);
+  }
+  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < 2 * q.m; s += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t kind = s >= q.m;
+    const uint64_t j = s - kind * q.m, first = kind * q.n_ok + j * q.k;
+    const uint32_t rows = (uint32_t)min((uint64_t)q.k, q.n_ok - j * q.k);
+    const uint32_t t = 2 * kind + (rows != q.k);
+    tgi_state_edge_stmt& st = q.stmts[s];
+    st.kind = TGI_SQL_PAGE_BUFFER_INSERT + kind;
+    st.rows = rows;
+    st.sql_off = q.sql_off[t];
+    st.sql_len = q.sql_len[t];
+    st.params_off = q.base + q.off[first];
+    st.params_len = q.off[first + rows] - q.off[first];
+  }
+}
+
 // ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------
 struct StLmEntry {  // one id of a layer, or an empty layer (row == ST_NONE)
   uint32_t row;

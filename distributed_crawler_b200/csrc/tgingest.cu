@@ -255,6 +255,14 @@ struct CrawlState {
   uint64_t handoff_ne = 0, handoff_nb = 0;
   DevBuf sql_in, sql_size, sql_off, sql_out, sql_stmts;
   HostBuf h_sql, h_sql_stmts;
+  // tandem forced walkback (tgi_state_walkback): the hand-off's edge-less spans as (span, row) pairs, whether its picks
+  // are made (then wb / wb_rank hold them and n_ok counts the usable ones), the counter of edge-less spans handled, the
+  // picks on the device and the pinned outputs
+  std::vector<uint32_t> wb_spans;
+  bool wb_picked = false;
+  uint64_t wb_n_ok = 0, walk_next = 0;
+  DevBuf wb_in, wb, wb_ok, wb_rank;
+  HostBuf h_wb, h_wb_sql, h_wb_stmts;
   // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
   // device and its staging, and the pinned outputs
   DevBuf rset;
@@ -5580,16 +5588,21 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
 }
 
 // The SQL text of a statement of `rows` rows (TGI_SQL_*): for one row the literal of CreatePendingBatch,
-// InsertPendingEdge or ClosePendingBatch (state/daprstate.go:3897, 3915, 3935); for more the VALUES tuple repeated with
-// the placeholders numbered on, or the close's WHERE batch_id IN (...)
+// InsertPendingEdge, ClosePendingBatch, AddPageToPageBuffer or SaveEdgeRecords (state/daprstate.go:3897, 3915, 3935,
+// 3620, 3167); for more the VALUES tuple repeated with the placeholders numbered on, or the close's WHERE batch_id IN
+// (...)
 void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
-  static const char* const head[3] = {
+  static const char* const head[5] = {
       "INSERT INTO pending_edge_batches (batch_id, crawl_id, source_channel, source_page_id, source_depth, sequence_id, "
       "status) VALUES ",
       "INSERT INTO pending_edges (batch_id, crawl_id, destination_channel, source_channel, sequence_id, discovery_time, "
       "source_type, validation_status) VALUES ",
-      "UPDATE pending_edge_batches SET status = 'closed', closed_at = NOW() WHERE batch_id "};
-  const uint32_t per = kind == TGI_SQL_BATCH_INSERT ? 7 : kind == TGI_SQL_EDGE_INSERT ? 8 : 1;
+      "UPDATE pending_edge_batches SET status = 'closed', closed_at = NOW() WHERE batch_id ",
+      "INSERT INTO page_buffer (page_id, parent_id, depth, url, crawl_id, sequence_id) VALUES ",
+      "INSERT INTO edge_records (destination_channel, source_channel, walkback, skipped, discovery_time, crawl_id, "
+      "sequence_id) VALUES "};
+  static const uint32_t per_row[5] = {7, 8, 1, 6, 7};
+  const uint32_t per = per_row[kind];
   s = head[kind];
   s.reserve(s.size() + (size_t)rows * (per * 8 + 4) + 8);
   char num[16] = {'$'};
@@ -5616,6 +5629,20 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
     s += ")";
   }
   s += ";";
+}
+
+// An accepted hand-off's edge-less spans (tgi_state_walkback's input) from its span_batch, read back already; its
+// walkbacks are not picked yet
+void handoff_walkbacks(CrawlState& S, const tgi_state_span* spans, uint32_t n_spans) {
+  const uint32_t* sb = S.h_span_batch.as<uint32_t>();
+  S.wb_spans.clear();
+  for (uint32_t k = 0; k < n_spans; k++)
+    if (sb[k] == TGI_STATE_NO_BATCH) {
+      S.wb_spans.push_back(k);
+      S.wb_spans.push_back(spans[k].row);
+    }
+  S.wb_picked = false;
+  S.wb_n_ok = 0;
 }
 
 }  // namespace
@@ -5779,6 +5806,7 @@ int tgi_state_pending_edges(tgi_ctx* c, int slot, const tgi_state_span* spans, u
     std::fill_n(S.h_span_batch.as<uint32_t>(), n_spans, TGI_STATE_NO_BATCH);
     S.handoff_live = true;
     S.handoff_ne = S.handoff_nb = 0;
+    handoff_walkbacks(S, spans, n_spans);
     return TGI_OK;
   }
   cudaStream_t st = S.stream;
@@ -5866,6 +5894,7 @@ int tgi_state_pending_edges(tgi_ctx* c, int slot, const tgi_state_span* spans, u
   S.handoff_live = true;  // S.edges, S.ebatches and S.spans hold it until the next state call
   S.handoff_ne = n_edges;
   S.handoff_nb = n_batches;
+  handoff_walkbacks(S, spans, n_spans);
   out->n_candidates = hs[3];
   out->n_edges = n_edges;
   out->n_batches = (uint32_t)n_batches;
@@ -5981,6 +6010,161 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   out->data = h;
   out->data_len = texts.size() + body;
   out->kernel_ms = ms + t2;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The forced walkbacks of the last hand-off.  The first call on a hand-off picks (a thread per edge-less span, a scan
+// that ranks the usable ones, one synchronise for the picks and their count); every call renders the rows as
+// tgi_state_edge_sql does (a thread per row sizes it, a scan, a thread per row writes it and the statement table; one
+// synchronise for the params' length, one for the read-back)
+int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                       uint32_t rows_per_stmt, tgi_state_walkback_t* out) {
+  static const char* const who = "tgi_state_walkback";
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  cudaSetDevice(c->device);  // not st_init: that would end the hand-off
+  const uint32_t k = rows_per_stmt;
+  if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
+  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
+  if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
+  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  const uint64_t n = S.wb_spans.size() / 2;
+  if (!n) {  // every span has a batch: nothing to pick, no launch
+    memset(out, 0, sizeof *out);
+    return TGI_OK;
+  }
+  if (!S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
+  char tb[48];
+  uint32_t tl = 0;
+  {
+    std::lock_guard<std::mutex> zg(c->cfg_mu);
+    tl = (uint32_t)host_render_zone_time(tb, now_sec, now_nsec, c->zone, c->cfgdev.tz);
+  }
+  cudaStream_t st = S.stream;
+  uint32_t launches = 0;
+  float ms = 0;
+  int rc;
+  uint64_t n_ok = S.wb_n_ok;
+  if (!S.wb_picked) {  // the hand-off's picks: made here, kept only once the call is accepted
+    CK(S.wb_in.ensure(n * 8));
+    CK(S.wb.ensure(n * sizeof(tgi_state_walkback_span)));
+    CK(S.wb_ok.ensure(n * 4));
+    CK(S.wb_rank.ensure((n + 1) * 8));
+    CK(S.sc.ensure(ST_SC_COUNT * 8));
+    CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+    CK(S.h_wb.ensure(n * sizeof(tgi_state_walkback_span)));
+    CK(cudaMemcpyAsync(S.wb_in.p, S.wb_spans.data(), n * 8, cudaMemcpyHostToDevice, st));
+    StWalk w{};
+    w.spans = S.wb_in.as<uint32_t>();
+    w.n = n;
+    w.seed = S.id_seed;
+    w.w0 = S.walk_next;
+    w.out = S.wb.as<tgi_state_walkback_span>();
+    w.ok = S.wb_ok.as<uint32_t>();
+    {
+      std::lock_guard<std::mutex> fg(c->fr_mu);  // the discovered set: read by the pick, not changed
+      if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+      w.disc = c->sets[TGI_SET_DISCOVERED].dev;
+      CK(cudaEventRecord(S.t0, st));
+      st_walk_pick_kernel<<<sink_grid(c, n, ST_THREADS, 4), ST_THREADS, 0, st>>>(st_dev(S), w);
+      launches++;
+      if ((rc = launch_scan(c, st, S.tiles, w.ok, n, S.wb_rank.as<uint64_t>(), S.sc.as<uint64_t>() + ST_SC_ROWS, launches))) return rc;
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(S.t1, st));
+      CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(S.h_wb.p, w.out, n * sizeof(tgi_state_walkback_span), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    }
+    cudaEventElapsedTime(&ms, S.t0, S.t1);
+    n_ok = S.h_sc.as<uint64_t>()[ST_SC_ROWS];
+  }
+  if (n_ok && !tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  if (!S.wb_picked) {
+    S.wb_picked = true;
+    S.wb_n_ok = n_ok;
+    S.walk_next += n;
+  }
+  memset(out, 0, sizeof *out);
+  out->n_walkbacks = (uint32_t)n;
+  out->walkbacks = S.h_wb.as<tgi_state_walkback_span>();
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  if (!n_ok) return TGI_OK;
+  // the statements: ceil(n_ok / k) per kind, and the texts of their row counts
+  const uint64_t m = (n_ok + k - 1) / k, n_stmts = 2 * m, n_rows = 2 * n_ok;
+  StWalkSql q{};
+  std::string texts, t;
+  for (uint32_t kind = 0; kind < 2; kind++) {
+    const uint32_t rows[2] = {n_ok >= k ? k : 0u, (uint32_t)(n_ok % k)};
+    for (int j = 0; j < 2; j++) {
+      if (!rows[j]) continue;
+      edge_sql_text(TGI_SQL_PAGE_BUFFER_INSERT + kind, rows[j], t);
+      q.sql_off[2 * kind + j] = texts.size();
+      q.sql_len[2 * kind + j] = t.size();
+      texts += t;
+    }
+  }
+  const size_t t_at = (crawl_id_len + 15) & ~(size_t)15;
+  CK(S.sql_in.ensure(t_at + sizeof tb));
+  CK(S.sql_size.ensure(n_rows * 4));
+  CK(S.sql_off.ensure((n_rows + 1) * 8));
+  CK(S.sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  std::vector<uint8_t> in(t_at + tl);
+  if (crawl_id_len) memcpy(in.data(), crawl_id, crawl_id_len);
+  memcpy(in.data() + t_at, tb, tl);
+  CK(cudaMemcpyAsync(S.sql_in.p, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  q.spans = S.wb_in.as<uint32_t>();
+  q.wb = S.wb.as<tgi_state_walkback_span>();
+  q.rank = S.wb_rank.as<uint64_t>();
+  q.n = n;
+  q.n_ok = n_ok;
+  q.k = k;
+  q.crawl = S.sql_in.as<uint8_t>();
+  q.crawl_len = crawl_id_len;
+  q.time = q.crawl + t_at;
+  q.time_len = tl;
+  q.size = S.sql_size.as<uint32_t>();
+  q.off = S.sql_off.as<uint64_t>();
+  q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
+  q.m = m;
+  q.base = texts.size();
+  const StDev d = st_dev(S);
+  const unsigned grid = sink_grid(c, std::max(2 * n, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
+  CK(cudaEventRecord(S.t0, st));
+  st_walk_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, q.size, n_rows, q.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
+  CK(S.sql_out.ensure(body));
+  CK(S.h_wb_sql.ensure(texts.size() + body));
+  CK(S.h_wb_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
+  q.out = S.sql_out.as<uint8_t>();
+  CK(cudaEventRecord(S.t2, st));
+  st_walk_emit_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  uint8_t* h = S.h_wb_sql.as<uint8_t>();
+  CK(cudaMemcpyAsync(h + texts.size(), S.sql_out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_wb_stmts.p, S.sql_stmts.p, n_stmts * sizeof(tgi_state_edge_stmt), cudaMemcpyDeviceToHost, st));
+  memcpy(h, texts.data(), texts.size());  // beside the copies: another part of the buffer
+  CK(cudaStreamSynchronize(st));
+  float t1 = 0, t2 = 0;
+  cudaEventElapsedTime(&t1, S.t0, S.t1);
+  cudaEventElapsedTime(&t2, S.t2, S.t3);
+  out->n_stmts = n_stmts;
+  out->stmts = S.h_wb_stmts.as<tgi_state_edge_stmt>();
+  out->data = h;
+  out->data_len = texts.size() + body;
+  out->kernel_ms = ms + t1 + t2;
   out->gpu_launches = launches;
   return TGI_OK;
 }

@@ -42,6 +42,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
     "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers", "tgi_state_edge_sql",
+    "tgi_state_walkback",
 ]
 
 
@@ -134,6 +135,7 @@ def lib() -> C.CDLL:
         L.tgi_state_read_layer.argtypes = [vp, C.c_int64, i32, u32, C.POINTER(abi.StateReadC)]
         L.tgi_state_layers.argtypes = [vp, C.POINTER(abi.StateLayersC)]
         L.tgi_state_edge_sql.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateEdgeSqlC)]
+        L.tgi_state_walkback.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateWalkbackC)]
         _LIB = L
     return _LIB
 
@@ -952,6 +954,26 @@ class Engine:
         data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
         return [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
                 for k, r, so, sl, po, pl in st.tolist()]
+
+    def state_walkback(self, crawl_id: bytes, now=(0, 0), rows_per_stmt: int = 1) -> tuple:
+        """the forced walkbacks of the last state_pending_edges (nothing but it, state_edge_sql and this since among the
+        state calls): a channel picked from the discovered set for every span without edges, and the Postgres binding
+        calls that store them, every page_buffer insert then every edge_records insert.  Returns (walkbacks, stmts):
+        per edge-less span {"span", "status" (abi.WALK_*), "draws", "url", "page_id", "sequence_id"}, and
+        [(kind (abi.SQL_*), rows, sql, params)]; the device time and launches are left in self.state_walk_ms and
+        self.state_walk_launches"""
+        out = abi.StateWalkbackC()
+        self._check(lib().tgi_state_walkback(self.h, crawl_id, len(crawl_id), now[0], now[1], rows_per_stmt, C.byref(out)))
+        self.state_walk_ms = float(out.kernel_ms)
+        self.state_walk_launches = int(out.gpu_launches)
+        wb = _view(out.walkbacks, int(out.n_walkbacks), abi.STATE_WALKBACK_SPAN)
+        walkbacks = [{"span": int(w["span"]), "status": int(w["status"]), "draws": int(w["draws"]),
+                      "url": bytes(w["url"][:int(w["url_len"])]), "page_id": bytes(w["page_id"]),
+                      "sequence_id": bytes(w["sequence_id"])} for w in wb]
+        st = _view(out.stmts, int(out.n_stmts), abi.STATE_EDGE_STMT)
+        data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
+        return walkbacks, [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
+                           for k, r, so, sl, po, pl in st.tolist()]
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:

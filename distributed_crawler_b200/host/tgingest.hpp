@@ -467,6 +467,16 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return o;
   }
+  // Tandem forced walkback: for every span of the last StatePendingEdges without edges, a channel picked from the
+  // discovered set (walkbacks[k].status TGI_WALK_*), and the exec calls that store the TGI_WALK_OK ones as StateEdgeSql's
+  // are read.  A span that is not OK is the reference's random-walk-walkback error for its page.  The arrays stay valid
+  // until the next state call.
+  tgi_state_walkback_t StateWalkback(std::string_view crawl_id, int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt) {
+    tgi_state_walkback_t o{};
+    if (tgi_state_walkback(ctx_, crawl_id.data(), (uint32_t)crawl_id.size(), now_sec, now_nsec, rows_per_stmt, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
   // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
   // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.

@@ -1182,8 +1182,8 @@ int tgi_state_pending_edges(tgi_ctx* ctx, int slot, const tgi_state_span* spans,
  * device-side edges, batches and spans of the context's last successful tgi_state_pending_edges; nothing is uploaded
  * again but crawl_id and the clock.
  *   Input    the last tgi_state_pending_edges.  Any other state call since (tgi_state_*, accepted or refused) ends it;
- *            tgi_state_edge_sql does not, so one hand-off may be rendered many times, and the hand-off's own output
- *            stays valid.  No hand-off to render is TGI_E_STATE.
+ *            tgi_state_edge_sql and tgi_state_walkback do not, so one hand-off may be rendered many times, and the
+ *            hand-off's own output and tgi_state_walkback's stay valid.  No hand-off to render is TGI_E_STATE.
  *   Order    every batch insert, then every edge insert, then every batch close: a batch row exists before its edges
  *            (pending_edges.batch_id REFERENCES pending_edge_batches) and is closed only after all of them are written
  *            (crawl/runner.go:1414-1421).  Within a kind the hand-off's order: batches in span order, edges in (span,
@@ -1230,6 +1230,70 @@ typedef struct tgi_state_edge_sql_t {
 } tgi_state_edge_sql_t;
 int tgi_state_edge_sql(tgi_ctx* ctx, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
                        uint32_t rows_per_stmt, tgi_state_edge_sql_t* out);
+
+/* Tandem forced walkback — the branch of a tandem step for a page without edges (crawl/runner.go:1425-1455): pick a
+ * walkback channel (pickWalkbackChannel, :115-139, exclude = nil), start a new chain at it with AddPageToPageBuffer
+ * (state/daprstate.go:3619-3641) and store the step with SaveEdgeRecords of one EdgeRecord{Walkback: true}
+ * (:3150-3204), each sent by ExecuteDatabaseOperation as an `exec` InvokeBinding.  The pick draws from the resident
+ * TGI_SET_DISCOVERED, so a shim keeps no copy of the discovered channels.
+ *   Input    the last tgi_state_pending_edges, as for tgi_state_edge_sql: every span with TGI_STATE_NO_BATCH, in span
+ *            order.  tgi_state_walkback and tgi_state_edge_sql both leave the hand-off in place and have their own
+ *            outputs, so either may come first and either may be called again; any other state call ends it.  No
+ *            hand-off is TGI_E_STATE.
+ *   Pick     the set's N keys in first-occurrence order (DiscoveredChannels.keys); key i is pool entry i without its
+ *            zero padding.  Up to 10 draws: a draw equal to the owner row's URL (byte for byte, case-sensitive, as
+ *            url == sourceURL) is skipped; TGI_WALK_EXHAUSTED after 10 such draws, TGI_WALK_EMPTY when N = 0 (also a
+ *            set never allocated), else TGI_WALK_OK with the first usable key.  N is the set as it is at the call.
+ *   Random   the w-th edge-less span the context has handled (w is not reset by tgi_state_set) draws from the 64-bit
+ *            words of Philox4x32-10 blocks (w_lo, w_hi, 2, j), j = 0, 1, ... under the page-id seed: x0 | x1 << 32,
+ *            then x2 | x3 << 32.  A draw is Lemire's multiply-and-reject over those words (m = x * N; when low64(m) <
+ *            (2^64 - N) mod N take the next word; the index is high64(m)), exactly uniform on [0, N) as rand.Intn.
+ *            The page ID and its new SequenceID are ids of the page-id construction with counter (w, 3) and (w, 4).
+ *            Without tgi_state_id_seed a hand-off with an edge-less span is TGI_E_STATE.
+ *   Once     the first accepted call on a hand-off makes its picks and ids and advances w; later calls on the same
+ *            hand-off return the same picks and ids (with any clock or rows_per_stmt), so a retried render cannot
+ *            start a second walkback page for a span.
+ *   Rows     each TGI_WALK_OK span gives a page_buffer row [ID, owner.ID, owner.Depth + 1, url, crawl_id, SequenceID]
+ *            and an edge_records row [url, owner.URL, true, false, discovery_time, crawl_id, owner.SequenceID]; the
+ *            records' empty CrawlID falls back to the configured one, so crawl_id is the call's.  Depth + 1 is a
+ *            decimal int64 and wraps as Go's int.  Strings, the clock and the year check are tgi_state_edge_sql's.
+ *   Order    every page_buffer insert (TGI_SQL_PAGE_BUFFER_INSERT), then every edge_records insert
+ *            (TGI_SQL_EDGE_RECORD_INSERT), rows_per_stmt = k rows per statement by tgi_state_edge_sql's rule: k = 1
+ *            gives the reference's literals and json.Marshal of each []any byte for byte.
+ *   Cost     a thread per edge-less span picks, a scan ranks the usable ones, a thread per row sizes it, a scan, a
+ *            thread per row writes it and the statement table.  A hand-off without edge-less spans launches nothing.
+ *   Errors   every check runs before anything changes: a refused call leaves the state, w and the hand-off as they
+ *            were.  TGI_E_ARG: k outside [1, 8191], now_nsec outside [0, 1e9), crawl_id NULL with a length, and when
+ *            there is a row a clock whose local year leaves [0, 9999].  TGI_E_STATE: no hand-off, no seed.  All of out
+ *            lives in pinned memory until the next state call.                                                      */
+#define TGI_SQL_PAGE_BUFFER_INSERT 3  /* AddPageToPageBuffer                                                          */
+#define TGI_SQL_EDGE_RECORD_INSERT 4  /* SaveEdgeRecords, one record                                                  */
+#define TGI_WALK_OK 0                 /* a walkback channel was picked                                                */
+#define TGI_WALK_EXHAUSTED 1          /* 10 draws, all the owner's URL (ErrWalkbackExhausted)                         */
+#define TGI_WALK_EMPTY 2              /* no discovered channel to pull from                                           */
+#define TGI_WALK_MAX_DRAWS 10         /* maxWalkbackAttempts                                                          */
+typedef struct tgi_state_walkback_span { /* 120 bytes: one edge-less span                                             */
+  uint32_t span;                       /* its index in the hand-off's spans                                           */
+  uint32_t status;                     /* TGI_WALK_*                                                                  */
+  uint32_t draws;                      /* draws made, 0 for TGI_WALK_EMPTY                                            */
+  uint32_t url_len;
+  uint8_t url[32];                     /* the walkback channel (TGI_WALK_OK), zero padded                            */
+  uint8_t page_id[36];                 /* the new page's ID                                                           */
+  uint8_t sequence_id[36];             /* its SequenceID: the new chain                                               */
+} tgi_state_walkback_span;
+typedef struct tgi_state_walkback_t {
+  uint32_t n_walkbacks;                /* the hand-off's edge-less spans                                              */
+  uint32_t reserved;
+  const tgi_state_walkback_span* walkbacks; /* [n_walkbacks] in span order (pinned)                                   */
+  uint64_t n_stmts;
+  const tgi_state_edge_stmt* stmts;    /* [n_stmts] in execution order (pinned)                                       */
+  const uint8_t* data;                 /* the texts, then the params (pinned)                                         */
+  uint64_t data_len;
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies)               */
+  uint32_t gpu_launches;
+} tgi_state_walkback_t;
+int tgi_state_walkback(tgi_ctx* ctx, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                       uint32_t rows_per_stmt, tgi_state_walkback_t* out);
 
 /* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
  * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on

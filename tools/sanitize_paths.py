@@ -64,4 +64,18 @@ for b, flags in ((Corpus(100, profile=2, nthreads=4).batch, abi.RUN_JSONL), (Cor
     print("combine", e.combine_add(0, 1).n_blobs)
     e.release(0)
 print("combine flush", e.combine_flush(2).n_blobs)
+# tandem hand-off, its SQL and the forced walkbacks of its edge-less spans (one over the owner's URL only)
+w = Engine(set_growth=1 << 20)
+w.state_id_seed(7)
+w.state_set([(0, [{"id": b"p%d" % k, "url": b"chan%05d" % k, "sequenceId": b"s"} for k in range(4)])])
+w.set_add(abi.SET_DISCOVERED, names_to_keys32([b"chan00000"] + [b"disc%04d" % i for i in range(2000)]))
+w.telegram_submit(0, pack_telegram([msg("messageText", "t.me/chan%05d t.me/other%d" % (k, k), id=(k + 1) << 20,
+                                        chat_id=-1, date=1_700_000_000) for k in range(8)]), abi.RUN_LINKS)
+w.telegram_wait(0)
+print("handoff", w.state_pending_edges(0, [(0, 0, 2, 0), (1, 0, 4, 4), (2, 2, 2, 0), (3, 4, 4, 4)], 1_700_000_100)["span_batch"])
+print("edge sql", len(w.state_edge_sql(b"c", (1_700_000_100, 0), 2)))
+print("walkback", [r["status"] for r in w.state_walkback(b"c", (1_700_000_100, 0), 1)[0]],
+      len(w.state_walkback(b"c", (1_700_000_100, 5), 7)[1]))
+w.release(0)
+w.close()
 print("done")
