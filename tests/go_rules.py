@@ -212,9 +212,27 @@ _LINK_CARRIERS = ("messageText", "messagePhoto", "messageVideo", "messageDocumen
                   "messageVoiceNote")
 
 
+def go_div(a: int, b: int) -> int:
+    """Go's integer `/`: the quotient truncated toward zero (Python's // floors)"""
+    q = abs(a) // abs(b)
+    return q if (a < 0) == (b < 0) else -q
+
+
+# the channel strings repeat in every line of the channel: escape each once (a 65 535-byte title of '<' costs a
+# per-byte loop)
+_chan_json = functools.lru_cache(maxsize=256)(go_json_string)
+
+
+def _chan_str(prefix: bytes, s: bytes, suffix: bytes = b"") -> _Raw:
+    """go_json_string(prefix + s + suffix) for ASCII prefix / suffix: an ASCII byte never joins a UTF-8 sequence, so the
+    escaper treats the three parts alike apart"""
+    return _Raw(go_json_string(prefix)[:-1] + _chan_json(s)[1:-1] + go_json_string(suffix)[1:])
+
+
 def telegram_post_line(m, ch, *, crawl_label=b"", created=(1_750_000_000, 0), capture=(1_750_000_001, 0), tz=0,
-                       min_post_date=None):
-    """-> ("skipped" | "failed" | "emitted", line or None, outlinks) for one pack.Message in channel `ch`"""
+                       min_post_date=None, zone=None):
+    """-> ("skipped" | "failed" | "emitted", line or None, outlinks) for one pack.Message in channel `ch`.  zone =
+    (starts, offsets): time.Local as a transition table (tests/zone_oracle.py's rule) instead of the fixed offset tz."""
     if min_post_date is not None and m.date < min_post_date:  # tdutils.go:419-421
         return "skipped", None, []
     if m.panics or (m.content_type == "messageVideo" and m.video_shape == "broken"):  # :395-405 recovered panic
@@ -246,22 +264,30 @@ def telegram_post_line(m, ch, *, crawl_label=b"", created=(1_750_000_000, 0), ca
                      ("reactions", None if c.reactions is None else {_bs(k): v for k, v in c.reactions}),
                      ("view_count", c.view_count), ("reply_count", c.reply_count), ("handle", _bs(c.handle))] for c in m.comments]
     ncomments = 0 if comments is None else len(comments)
-    msgno = int(m.id / 1048576) if m.id >= 0 else -((-m.id) // 1048576)  # Go integer division truncates toward zero (:1008)
+    msgno = go_div(m.id, 1048576)  # message.Id/1048576 on an int64 (:1008): exact, truncated toward zero
     user, name, title = _bs(ch.username), _bs(ch.name), _bs(ch.title)
     link = b""
     if user:
-        link = b"https://t.me/" + user + b"/" + str(msgno).encode() + (b"?single" if m.media_album_id != 0 else b"")
+        link = _chan_str(b"https://t.me/", user, b"/" + str(msgno).encode() + (b"?single" if m.media_album_id != 0 else b""))
+    uid = _chan_str(str(msgno).encode() + b"-", name)
+    churl = _chan_str(b"https://t.me/c/", name)
+    title = _Raw(_chan_json(title))
     chat = str(m.chat_id).encode()
     known = ("messageText", "messageVideo", "messagePhoto", "messageAnimation", "messageAnimatedEmoji", "messagePoll",
              "messageGiveaway", "messagePaidMedia", "messageSticker", "messageGiveawayWinners", "messageGiveawayCompleted",
              "messageVideoNote", "messageDocument", "messageAudio", "messageVoiceNote")
     # MessageContentType() of a type ParseMessage has no case for travels in Message.alt (pack.py); nil content -> "unknown"
     post_type = ["unknown"] if ct == "none" else [ct] if ct in known else [_bs(m.alt) or _bs(ct)]
-    tm = lambda s, ns, z: _Raw(go_time_json(s, ns, z))
+    if zone is None:
+        local = lambda s, ns: _Raw(go_time_json(s, ns, tz))
+    else:  # zone_oracle's rendering, which ZonedOracle uses as well: not a second check of the zone rule, which
+        # tests/test_zones.py pins against the oracle's fixed-offset rendering at every offset of real zones
+        from zone_oracle import go_json_time, go_offset
+        local = lambda s, ns: _Raw(go_json_time(s, ns, go_offset(zone, s)))
     nil = None
     post = [
-        ("post_link", link), ("channel_id", chat), ("post_uid", str(msgno).encode() + b"-" + name), ("url", link),
-        ("published_at", tm(m.date, 0, tz)), ("created_at", tm(created[0], 0, 0)),  # time.Now().UTC().Truncate(time.Second)
+        ("post_link", link), ("channel_id", chat), ("post_uid", uid), ("url", link),
+        ("published_at", local(m.date, 0)), ("created_at", _Raw(go_time_json(created[0], 0, 0))),  # time.Now().UTC().Truncate(time.Second)
         ("language_code", b""), ("engagement", m.view_count), ("view_count", m.view_count), ("like_count", 0),
         ("share_count", m.share_count), ("comment_count", ncomments), ("crawl_label", _bs(crawl_label)), ("list_ids", nil),
         ("channel_name", title), ("search_terms", nil), ("search_term_ids", nil), ("project_ids", nil), ("exercise_ids", nil),
@@ -273,7 +299,7 @@ def telegram_post_line(m, ch, *, crawl_label=b"", created=(1_750_000_000, 0), ca
                           ("channel_engagement_data", [("follower_count", ch.member_count), ("following_count", 0),
                                                        ("like_count", 0), ("post_count", ch.post_count),
                                                        ("views_count", ch.view_count), ("comment_count", 0), ("share_count", 0)]),
-                          ("channel_url_external", b"https://t.me/c/" + name), ("channel_url", b"https://t.me/c/" + name),
+                          ("channel_url_external", churl), ("channel_url", churl),
                           ("country_code", b""), ("published_at", _Raw(b'"0001-01-01T00:00:00Z"'))]),
         ("platform_name", b"Telegram"), ("shared_id", nil), ("quoted_id", nil), ("replied_id", nil), ("ai_label", nil),
         ("root_post_id", nil), ("engagement_steps_count", 0), ("ocr_data", nil),
@@ -284,7 +310,7 @@ def telegram_post_line(m, ch, *, crawl_label=b"", created=(1_750_000_000, 0), ca
         ("views_count", m.view_count), ("searchable_text", b""), ("all_text", b""), ("contrast_agent_project_ids", nil),
         ("agent_ids", nil), ("segment_ids", nil), ("thumb_url", b""),  # fetchAndUploadMedia returns "" under SkipMediaDownload (:233-239)
         ("media_url", media), ("comments", comments), ("reactions", reactions), ("outlinks", [_bs(x) for x in links]),
-        ("capture_time", tm(capture[0], capture[1], tz)), ("handle", _bs(m.handle)),
+        ("capture_time", local(*capture)), ("handle", _bs(m.handle)),
     ]
     return "emitted", _marshal(post) + b"\n", links
 
