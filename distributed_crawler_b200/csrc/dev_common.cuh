@@ -288,6 +288,22 @@ __device__ __noinline__ uint32_t warp_esc_len(const uint8_t* s, int64_t n, bool*
   if (needs_exact) *needs_exact = ex;
   return warp_sum(tot);
 }
+// The same length summed in 64 bits, for the state writers, which refuse a page of 4 GiB or more: one string of ~716 MB
+// of '<' already wraps warp_esc_len.  A lane's share is at most 24 bytes per strip, under 2^32 for any n below 2^32.
+// (Its own loop rather than a shared one: sharing it changed the register allocation of the Post-line kernels.)
+__device__ __noinline__ uint64_t warp_esc_len64(const uint8_t* s, int64_t n) {
+  uint32_t lane = 0, carry = 0;
+  for (int64_t base = 0; base < n; base += 128) {
+    Strip st = warp_load_strip(s, base, n, carry);
+    uint32_t e, u;
+    strip_lane_totals(st, s, base, n, e, u);
+    lane += e;
+  }
+  uint64_t tot = lane;
+#pragma unroll
+  for (int d = 16; d; d >>= 1) tot += __shfl_xor_sync(FULL, tot, d);
+  return tot;
+}
 
 // ---- a message text measured 16 bytes per lane (the link count of the parse kernels, tg_links.cuh) ----------------
 // A text is "clean" when it is valid UTF-8 without C0/C1, bytes >= 0xF4 or E2 80 (U+2000..U+203F, which holds
@@ -521,10 +537,14 @@ DEVI uint4 lds128(uint32_t a) {
 }
 
 // ---- single-thread JSON escaping (Go's sequential algorithm, for short strings such as map keys) --
-DEVI uint32_t thread_esc_len(const uint8_t* s, uint32_t n) {
-  uint32_t o = 0;
+// W: the width of the count.  uint64_t for a string that may escape past 4 GiB (the state writers' size passes).
+template <class W = uint32_t>
+DEVI W thread_esc_len(const uint8_t* s, uint32_t n) {
+  W o = 0;
   for (uint32_t i = 0; i < n;) {
-    if (i + 4 <= n) {  // four plain ASCII bytes at once (ids, handles and file names are mostly that)
+    // four plain ASCII bytes at once (ids, handles and file names are mostly that).  i + 4 wraps for i within 3 bytes of
+    // 2^32, which only a state string (up to 2^32 - 1 bytes) reaches; the 32-bit form keeps the Post-line kernels' code
+    if (sizeof(W) == 8 ? n - i >= 4 : i + 4 <= n) {
       const uint32_t w = ld_u32_unaligned(s + i);
       const uint32_t odd = (w & 0x80808080u) | ((w - 0x20202020u) & ~w & 0x80808080u) | swar_has_byte(w, 0x22) |
                            swar_has_byte(w, 0x5C) | swar_has_byte(w, 0x3C) | swar_has_byte(w, 0x3E) | swar_has_byte(w, 0x26);

@@ -27,6 +27,8 @@
 // Page reads: the rows' fields come from the host mirror; their lists are the live messages of the distinct rows,
 // flagged in one pass, grouped by row with the render's radix passes and written out in that order.
 #pragma once
+#include <type_traits>
+
 #include "local_appends.cuh"
 
 namespace tgi {
@@ -483,9 +485,18 @@ struct StRender {
   uint32_t* esz;       // [entries] entry sizes with messages (the scan's input)
   uint8_t* out;        // the layers' bytes
 };
-// the scalars block: live messages, body bytes, message slots, a timestamp that does not render, an entry of 4 GiB or
-// more, message bytes, rows, radix counts
+// the scalars block: live messages, body bytes, message slots, a timestamp that does not render, an entry, message,
+// row or id of 4 GiB or more, message bytes, rows, radix counts
 enum { ST_SC_LIVE, ST_SC_BYTES, ST_SC_SLOTS, ST_SC_ERR, ST_SC_BIG, ST_SC_MBYTES, ST_SC_ROWS, ST_SC_RADIX, ST_SC_COUNT };
+
+// The 4 GiB rule: every writer sizes a piece (an entry with its messages, a SQL row, a layer-map id) in 64 bits and flags
+// one of 4 GiB or more in ST_SC_BIG, which refuses the call before anything is written; a written piece is under 4 GiB,
+// so the emits keep 32-bit offsets within it.
+template <bool EMIT>
+using StLen = std::conditional_t<EMIT, uint32_t, uint64_t>;
+DEVI void st_flag_big(uint64_t* sc, uint64_t bytes) {
+  if (bytes > 0xFFFFFFFFull) atomicMax((unsigned long long*)sc + ST_SC_BIG, 1ull);
+}
 
 // JSON escape of a short string by one thread (Go's sequential rule, as thread_esc_len measures it)
 DEVI uint32_t st_thread_esc(uint8_t* dst, const uint8_t* s, uint32_t n) {
@@ -527,14 +538,14 @@ DEVI const uint8_t* st_str(const StDev& d, const tgi_state_page& p, int f, uint3
 
 // one message, sized (dst == nullptr) or written: [,]{"chatId":N,"messageId":N,"status":"S","pageId":"P"[,"platform":"X"]}
 template <bool EMIT>
-DEVI uint32_t st_message(const StDev& d, const StMsg& m, bool comma, uint8_t* dst) {
-  uint32_t o = 0;
+DEVI StLen<EMIT> st_message(const StDev& d, const StMsg& m, bool comma, uint8_t* dst) {
+  StLen<EMIT> o = 0;
   auto lit = [&](const char* s, uint32_t n) {
     if (EMIT)
       for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
     o += n;
   };
-  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len(s, n); };
+  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n); };
   auto num = [&](long long v) { o += EMIT ? (uint32_t)render_i64(dst + o, v) : ndigits_i64(v); };
   if (comma) lit(",", 1);
   lit("{\"chatId\":", 10);
@@ -574,16 +585,21 @@ __global__ void st_render_pairs_kernel(StDev d, uint64_t n, StRender r) {
 }
 // size pass, a thread per grouped message k (sorted = the grouped message indices, sorted_rows their rows)
 __global__ void st_msg_size_kernel(StDev d, StRender r, const uint32_t* sorted, const uint32_t* sorted_rows, uint64_t live) {
-  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < live; k += (uint64_t)gridDim.x * blockDim.x)
-    r.msize[k] = st_message<false>(d, d.msgs[sorted[k]], k != r.row_base[sorted_rows[k]], nullptr);
+  for (uint64_t k = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; k < live; k += (uint64_t)gridDim.x * blockDim.x) {
+    // saturated, not flagged: a message of 4 GiB or more makes its entry one, and only the entries a call writes are
+    // checked (a message of a page in no layer list is sized by the render but never written)
+    const uint64_t sz = st_message<false>(d, d.msgs[sorted[k]], k != r.row_base[sorted_rows[k]], nullptr);
+    r.msize[k] = sz > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)sz;
+  }
 }
 
 // one entry, sized or written by a warp (lane 0 writes the literals, the warp escapes the strings).  Returns the bytes
-// of part A (framing and fields up to the first message) in *a and of the whole entry without messages.  LINE: the
+// of part A (framing and fields up to the first message) in *a and of the whole entry without messages, in 64 bits
+// (part A in 32: when it wraps, so does the whole).  LINE: the
 // page alone as one JSONL line, {page}\n, without layer framing (the exports).  A template parameter rather than an
 // entry flag: the flag cost the render's emit kernel 8 bytes of spills.
 template <bool EMIT, bool LINE = false>
-DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint32_t cnt, uint8_t* dst, uint64_t msg_bytes,
+DEVI uint64_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint32_t cnt, uint8_t* dst, uint64_t msg_bytes,
                        uint32_t* a, bool* bad) {
   const bool l0 = lane_id() == 0;
   uint64_t o = 0;
@@ -599,7 +615,7 @@ DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint
   auto str = [&](const tgi_state_page& p, int f) {
     uint32_t n;
     const uint8_t* s = st_str(d, p, f, n);
-    o += EMIT ? esc_to_global(dst + o, s, n) : warp_esc_len(s, n);
+    o += EMIT ? esc_to_global(dst + o, s, n) : warp_esc_len64(s, n);
   };
   if (LINE) {
   } else if (e.flags & ST_E_FIRST) {
@@ -660,7 +676,7 @@ DEVI uint32_t st_entry(const StDev& d, const StRender& r, const StEntry& e, uint
   }
   if (LINE) lit("\n", 1);
   else if (e.flags & ST_E_LAST) lit("]}", 2);
-  return (uint32_t)(o - msg_bytes);
+  return o - msg_bytes;
 }
 
 constexpr int ST_WARPS = 8;  // warps per CTA of the warp-per-entry kernels
@@ -680,13 +696,13 @@ DEVI void st_entry_size(const StDev& d, const StRender& r) {
     }
     uint32_t a;
     bool bad = false;
-    const uint32_t sz = st_entry<false, LINE>(d, r, en, cnt, nullptr, mb, &a, &bad);
+    const uint64_t sz = st_entry<false, LINE>(d, r, en, cnt, nullptr, mb, &a, &bad);
     if (lane_id() == 0) {
       r.esize_lo[e] = a;
-      r.ebytes[e] = sz;
+      r.ebytes[e] = (uint32_t)sz;
       r.ecnt[e] = cnt;
       r.esz[e] = (uint32_t)(sz + mb);
-      if (sz + mb > 0xFFFFFFFFull) atomicMax((unsigned long long*)r.sc + ST_SC_BIG, 1ull);
+      st_flag_big(r.sc, sz + mb);
       if (bad) atomicMax((unsigned long long*)r.sc + ST_SC_ERR, 1ull);
     }
   }
@@ -1025,6 +1041,7 @@ struct StSql {
   const uint8_t* time;
   uint32_t* size;                       // [n_rows] bytes of row r
   uint64_t* off;                        // [n_rows+1] their scan
+  uint64_t* sc;                         // ST_SC_*: ST_SC_BIG
   uint8_t* out;
   tgi_state_edge_stmt* stmts;           // [n_stmts]
   uint64_t n_stmts, m[3];               // statements in all and of each kind
@@ -1035,14 +1052,14 @@ struct StSql {
 // one row's values, sized (dst == nullptr) or written, with the statement's "[" before its first row, "," before the
 // others and "]" after its last
 template <bool EMIT>
-DEVI uint32_t st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* dst) {
-  uint32_t o = 0;
+DEVI StLen<EMIT> st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* dst) {
+  StLen<EMIT> o = 0;
   auto lit = [&](const char* s, uint32_t n) {
     if (EMIT)
       for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
     o += n;
   };
-  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len(s, n); };
+  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n); };
   auto str = [&](const uint8_t* s, uint32_t n) {
     lit("\"", 1);
     esc(s, n);
@@ -1098,8 +1115,11 @@ DEVI uint32_t st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* ds
 }
 
 __global__ void st_sql_size_kernel(StDev d, StSql q) {
-  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x)
-    q.size[r] = st_sql_row<false>(d, q, r, nullptr);
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_sql_row<false>(d, q, r, nullptr);
+    q.size[r] = (uint32_t)sz;
+    st_flag_big(q.sc, sz);
+  }
 }
 
 // the rows at their scanned offsets, then every statement's entry: its rows, its kind's text, its params' span
@@ -1199,6 +1219,7 @@ struct StWalkSql {
   const uint8_t* time;
   uint32_t* size;                      // [2 n_ok] bytes of row r
   uint64_t* off;                       // [2 n_ok + 1] their scan
+  uint64_t* sc;                        // ST_SC_*: ST_SC_BIG
   uint8_t* out;
   tgi_state_edge_stmt* stmts;          // [2 m]
   uint64_t m;                          // statements of each kind
@@ -1208,8 +1229,8 @@ struct StWalkSql {
 
 // one row's values, sized (dst == nullptr) or written, with the statement's "[" / "," / "]" as st_sql_row
 template <bool EMIT>
-DEVI uint32_t st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, uint64_t i, uint64_t j, uint8_t* dst) {
-  uint32_t o = 0;
+DEVI StLen<EMIT> st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, uint64_t i, uint64_t j, uint8_t* dst) {
+  StLen<EMIT> o = 0;
   auto lit = [&](const char* s, uint32_t n) {
     if (EMIT)
       for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
@@ -1217,7 +1238,7 @@ DEVI uint32_t st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, uin
   };
   auto str = [&](const uint8_t* s, uint32_t n) {
     lit("\"", 1);
-    o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len(s, n);
+    o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n);
     lit("\"", 1);
   };
   auto field = [&](const tgi_state_page& p, int f) {
@@ -1262,7 +1283,11 @@ __global__ void st_walk_size_kernel(StDev d, StWalkSql q) {
   for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < 2 * q.n; t += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t kind = t >= q.n;
     const uint64_t i = t - kind * q.n, j = q.rank[i];
-    if (q.rank[i + 1] > j) q.size[kind * q.n_ok + j] = st_walk_row<false>(d, q, kind, i, j, nullptr);
+    if (q.rank[i + 1] > j) {
+      const uint64_t sz = st_walk_row<false>(d, q, kind, i, j, nullptr);
+      q.size[kind * q.n_ok + j] = (uint32_t)sz;
+      st_flag_big(q.sc, sz);
+    }
   }
 }
 
@@ -1301,13 +1326,14 @@ struct StLm {
   const uint8_t* keys;
   uint32_t* size;  // [n] bytes of entry e
   uint64_t* off;   // [n+1] their scan
+  uint64_t* sc;    // ST_SC_*: ST_SC_BIG
   uint8_t* out;
 };
 
 // one entry, sized (EMIT false) or written: [opening][,]"<escaped id>"[]]
 template <bool EMIT>
-DEVI uint32_t st_lm_entry(const StDev& d, const StLm& L, const StLmEntry& e, uint8_t* dst) {
-  uint32_t o = 0;
+DEVI StLen<EMIT> st_lm_entry(const StDev& d, const StLm& L, const StLmEntry& e, uint8_t* dst) {
+  StLen<EMIT> o = 0;
   auto ch = [&](uint32_t c) {
     if (EMIT) dst[o] = (uint8_t)c;
     o++;
@@ -1320,7 +1346,7 @@ DEVI uint32_t st_lm_entry(const StDev& d, const StLm& L, const StLmEntry& e, uin
     ch('"');
     uint32_t il;
     const uint8_t* id = st_str(d, d.pages[e.row], TGI_PS_ID, il);
-    o += EMIT ? st_thread_esc(dst + o, id, il) : thread_esc_len(id, il);
+    o += EMIT ? st_thread_esc(dst + o, id, il) : thread_esc_len<StLen<EMIT>>(id, il);
     ch('"');
   }
   if (e.last) ch(']');
@@ -1328,8 +1354,11 @@ DEVI uint32_t st_lm_entry(const StDev& d, const StLm& L, const StLmEntry& e, uin
 }
 
 __global__ void st_lm_size_kernel(StDev d, StLm L) {
-  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < L.n; e += (uint64_t)gridDim.x * blockDim.x)
-    L.size[e] = st_lm_entry<false>(d, L, L.entries[e], nullptr);
+  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < L.n; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_lm_entry<false>(d, L, L.entries[e], nullptr);
+    L.size[e] = (uint32_t)sz;
+    st_flag_big(L.sc, sz);
+  }
 }
 __global__ void st_lm_emit_kernel(StDev d, StLm L) {
   for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < L.n; e += (uint64_t)gridDim.x * blockDim.x)

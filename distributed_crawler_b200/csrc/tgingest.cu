@@ -4475,18 +4475,21 @@ int tgi_state_layer_map(tgi_ctx* c, tgi_state_json_t* out) {
     L.keys = S.lm_keys.as<uint8_t>();
     L.size = S.e32.as<uint32_t>();
     L.off = S.e64.as<uint64_t>();
+    L.sc = S.sc.as<uint64_t>();
     const StDev d = st_dev(S);
     CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StLmEntry), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(S.lm_keys.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
     CK(cudaEventRecord(S.t0, st));
     st_lm_size_kernel<<<st_grid(c, ne), ST_THREADS, 0, st>>>(d, L);
     launches++;
     if ((rc = launch_scan(c, st, S.tiles, L.size, ne, L.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
     CK(cudaGetLastError());
     CK(cudaEventRecord(S.t1, st));
-    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.as<uint64_t>() + ST_SC_BYTES, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    body = *S.h_sc.as<uint64_t>();
+    if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "tgi_state_layer_map: an id renders to 4 GiB or more"); return TGI_E_CAPACITY; }
+    body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
     CK(S.out.ensure(body));
     CK(S.h_out.ensure(body + 2));
     L.out = S.out.as<uint8_t>();
@@ -5568,6 +5571,7 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
   cudaEventElapsedTime(&t, S.t4, S.t5);
   *ms += t;
   if (hs[ST_SC_ERR]) { set_err(c, "%s: a page timestamp's year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  if (hs[ST_SC_BIG]) { set_err(c, "%s: an added page renders to 4 GiB or more (its parentId)", who); return TGI_E_CAPACITY; }
   const uint64_t body = hs[ST_SC_BYTES];
   CK(S.out.ensure(body));
   CK(S.h_out.ensure(body));
@@ -5971,6 +5975,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   q.time_len = tl;
   q.size = S.sql_size.as<uint32_t>();
   q.off = S.sql_off.as<uint64_t>();
+  q.sc = S.sc.as<uint64_t>();
   q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
   q.n_stmts = n_stmts;
   for (int j = 0; j < 3; j++) q.m[j] = m[j];
@@ -5979,6 +5984,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   const unsigned grid = sink_grid(c, std::max(n_rows, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
   uint32_t launches = 0;
   int rc;
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
   CK(cudaEventRecord(S.t0, st));
   st_sql_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
   launches++;
@@ -5987,6 +5993,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CK(cudaEventRecord(S.t1, st));
   CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "tgi_state_edge_sql: a row renders to 4 GiB or more"); return TGI_E_CAPACITY; }
   const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
   CK(S.sql_out.ensure(body));
   CK(S.h_sql.ensure(texts.size() + body));
@@ -6081,17 +6088,21 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
     n_ok = S.h_sc.as<uint64_t>()[ST_SC_ROWS];
   }
   if (n_ok && !tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
-  if (!S.wb_picked) {
+  auto accept = [&]() {  // the picks are kept once the call is accepted: a refused first call picks the same again
+    if (S.wb_picked) return;
     S.wb_picked = true;
     S.wb_n_ok = n_ok;
     S.walk_next += n;
-  }
+  };
   memset(out, 0, sizeof *out);
   out->n_walkbacks = (uint32_t)n;
   out->walkbacks = S.h_wb.as<tgi_state_walkback_span>();
   out->kernel_ms = ms;
   out->gpu_launches = launches;
-  if (!n_ok) return TGI_OK;
+  if (!n_ok) {
+    accept();
+    return TGI_OK;
+  }
   // the statements: ceil(n_ok / k) per kind, and the texts of their row counts
   const uint64_t m = (n_ok + k - 1) / k, n_stmts = 2 * m, n_rows = 2 * n_ok;
   StWalkSql q{};
@@ -6129,11 +6140,13 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   q.time_len = tl;
   q.size = S.sql_size.as<uint32_t>();
   q.off = S.sql_off.as<uint64_t>();
+  q.sc = S.sc.as<uint64_t>();
   q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
   q.m = m;
   q.base = texts.size();
   const StDev d = st_dev(S);
   const unsigned grid = sink_grid(c, std::max(2 * n, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
   CK(cudaEventRecord(S.t0, st));
   st_walk_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
   launches++;
@@ -6142,6 +6155,8 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CK(cudaEventRecord(S.t1, st));
   CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "%s: a row renders to 4 GiB or more", who); return TGI_E_CAPACITY; }
+  accept();
   const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
   CK(S.sql_out.ensure(body));
   CK(S.h_wb_sql.ensure(texts.size() + body));

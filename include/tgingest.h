@@ -825,7 +825,10 @@ int tgi_set_info(tgi_ctx* ctx, int which, tgi_set_info_t* out);
  *            memory until the next state call.
  *   Errors   TGI_E_ARG: malformed input (string ranges, layer / message counts, an unknown code, a row that is
  *            neither a row nor TGI_STATE_NO_PAGE, nsec / offset out of range, messages in tgi_state_add_layer);
- *            TGI_E_NOMEM.  More than 2^32 - 2 message rows is TGI_E_CAPACITY.                                     */
+ *            TGI_E_NOMEM.  More than 2^32 - 2 message rows is TGI_E_CAPACITY.  Every writer of this state (render,
+ *            exports, page and discovery JSON, layer map, edge SQL, walkback) refuses a page, message, layer-map id or
+ *            SQL row that renders to 4 GiB or more with TGI_E_CAPACITY before writing it; the whole output may pass
+ *            4 GiB.  Calls whose page JSON fails after their update (Dapr's UpdatePage) fail so for this too.       */
 #define TGI_STATE_NO_PAGE 0xFFFFFFFFu
 #define TGI_STATE_TS_LOCAL 0x7FFFFFFF
 enum { TGI_PS_ID, TGI_PS_URL, TGI_PS_STATUS, TGI_PS_ERROR, TGI_PS_PLATFORM, TGI_PS_PARENT, TGI_PS_CONN, TGI_PS_SEQ,
