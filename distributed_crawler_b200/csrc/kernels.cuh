@@ -1,7 +1,9 @@
 // kernels.cuh — __global__ kernels of the ingest engine (sm_90a).  See DESIGN.md §4 for the data layout and the
 // roofline bookkeeping.  All of it is integer/byte work:
 //   tg_chan_size / tg_chan_emit            per-channel constant strings (once per batch, tiny)
-//   tg_parse / tg_ent_map / tg_parse_ent   status + link extraction, one warp per record (split by code footprint)
+//   tg_parse / tg_ent_map / tg_parse_ent   status + link extraction (split by code footprint): tg_parse scans 32
+//                                          records' texts per warp as one packed stream, the other two take one warp
+//                                          per record with entities
 //   tg_size_lane                           JSONL line length, one LANE per record (+ the warp for the message text)
 //   scan_*                                 exclusive scan u32 -> u64 offsets
 //   tg_emit_lane                           the line, one LANE per record (tg_lane.cuh)
@@ -201,26 +203,122 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
 // entities (lanes pick them out of groups of 32), tg_size_lane_kernel = line lengths.  Fusing them was tried twice
 // (one parse kernel; parse + size in ONE pass over the text, fewer instructions in all): both fused kernels stalled on
 // instruction fetch and were slower than the split ones.
+//
+// tg_parse_kernel takes the records 32 per warp, lane k owning record 32g + k, and scans their texts as ONE packed
+// stream: text j's 16-byte chunks (cut from the text's start) follow text j - 1's in one chunk index space, and the
+// warp walks that space 32 chunks per pass, each lane on the chunk of whichever record holds it.  A warp per record
+// left most lanes idle (the median text fills about 20 of a strip's 32 lanes, a caption 7) and paid a full warp
+// iteration for every record without text to scan.  Per chunk the lane does what warp_count_tme_esc does per strip
+// lane (tme16, measure16); the totals go to the owning lane through shared-memory atomics on the (rare) nonzero values.
+// Only the records with a "t.me/" hit then take the warp-wide extraction, one after the other.
 template <bool MEASURE>
 DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_flags, const ParseOut& o) {
-  int wid = threadIdx.x >> 5;
-  uint64_t nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
-  for (uint64_t r = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; r < b.n; r += nwarps) {
-    // The chain header -> string offset -> text is two DRAM round trips per record and this kernel has little else to
-    // do (long_scoreboard 9 cycles per issue): read the NEXT record's header now, touch its text at the bottom of
-    // the loop, when that load has long completed.
-    const uint64_t rn = r + nwarps;
-    unsigned long long nx_off = 0;
-    uint32_t nx_len = 0;
-    if (rn < b.n) {
-      asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(nx_off) : "l"(&b.recs[rn].str_off));
-      asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(nx_len) : "l"(&b.recs[rn].text_len));
+  __shared__ uint32_t acc[WARPS_PER_CTA][MEASURE ? 3 : 1][32];  // per record: "t.me/" hits, escape extras, not clean
+  const int wid = threadIdx.x >> 5, l = lane_id();
+  const uint32_t SP = 0x20202020u;
+  uint32_t* a_cnt = acc[wid][0];
+  uint32_t* a_extra = acc[wid][MEASURE ? 1 : 0];
+  uint32_t* a_bad = acc[wid][MEASURE ? 2 : 0];
+  const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
+  for (uint64_t g = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; g < ngroups; g += nwarps) {
+    const uint64_t r = g * 32 + l;
+    const bool mine = r < b.n && b.ent_off[r + 1] == b.ent_off[r];  // the others: tg_parse_ent_kernel
+    uint32_t status = TGI_ST_EMITTED, len = 0;                          // len: bytes of text to scan
+    const uint8_t* text = b.strs;
+    if (mine) {
+      const tgi_tg_rec* rec = &b.recs[r];
+      const uint32_t fl = rec->flags;
+      if ((cfg.flags & TGI_CFG_HAS_MIN_POST_DATE) && (int64_t)rec->date < cfg.min_post_date) {
+        status = TGI_ST_SKIPPED;  // tdutils.go:419-421
+      } else if (fl & TGI_RF_PANIC) {
+        status = TGI_ST_FAILED;
+      } else if (ct_carries_links(rec->content_type) && (fl & TGI_RF_HAS_TEXT)) {
+        text += rec->str_off;
+        len = rec->text_len;
+      }
     }
-    if (b.ent_off[r + 1] == b.ent_off[r])  // the others: tg_parse_ent_kernel
-      parse_one_record<false, MEASURE>(b, cfg, o, r, load_rec_view(b, r));
-    if (rn < b.n) {
-      const uint32_t off = (uint32_t)lane_id() * 128u;
-      if (off < nx_len + 127u && off < 2048u) asm volatile("prefetch.global.L1 [%0];" ::"l"(b.strs + nx_off + off));
+    // the group's chunks: this record's are [incl - nch, incl) (64 bits: 32 texts of up to 4 GiB)
+    const uint64_t nch = ((uint64_t)len + 15u) >> 4;
+    uint64_t incl = nch;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint64_t t = __shfl_up_sync(FULL, incl, d);
+      if (l >= d) incl += t;
+    }
+    const uint64_t total = __shfl_sync(FULL, incl, 31), first = incl - nch;
+    a_cnt[l] = 0;
+    if (MEASURE) a_extra[l] = a_bad[l] = 0;
+    __syncwarp();
+    uint32_t carry = SP;  // the last 4 bytes of lane 31's chunk in the previous pass
+    for (uint64_t base = 0; base < total; base += 32) {
+      // owner of chunk base + l = the number of records whose chunks end at or before it (5 steps of a binary search on
+      // the scan, clamped to the pass so that it fits 32 bits)
+      const uint32_t end = incl <= base ? 0u : (uint32_t)min(incl - base, (uint64_t)32);
+      int ow = 0;
+#pragma unroll
+      for (int s = 16; s; s >>= 1)
+        if (__shfl_sync(FULL, end, ow + s - 1) <= (uint32_t)l) ow += s;
+      const uint8_t* s = (const uint8_t*)__shfl_sync(FULL, (unsigned long long)text, ow);
+      const uint64_t j = base + l - __shfl_sync(FULL, first, ow);  // chunk of that record
+      const int64_t n = __shfl_sync(FULL, len, ow), p0 = (int64_t)(16 * j), rem = n - p0;
+      const bool act = base + l < total;
+      uint4 w = make_uint4(SP, SP, SP, SP);
+      uint32_t cnt = 0, extra = 0, bad = 0;
+      if (act) {
+        w = ld16_unaligned(s + p0);
+        cnt = __popc(tme16(s, p0, n, w));
+        if (rem < 16) w = make_uint4(blank_from(w.x, rem), blank_from(w.y, rem - 4), blank_from(w.z, rem - 8), blank_from(w.w, rem - 12));
+      }
+      const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
+      const uint32_t pw = j == 0 ? SP : (l == 0 ? carry : below);  // a chunk in front of the text's first is not its
+      carry = __shfl_sync(FULL, w.w, 31);
+      if (MEASURE && act) {
+        measure16(w, pw, bad, extra);
+        // the text's last chunk: a sequence open at its end (one needs a high bit in the last three bytes)
+        if (rem <= 16 && (w.w & 0x80808000u)) bad |= utf8_unclean4(w.w, SP);
+      }
+      if (cnt) atomicAdd(&a_cnt[ow], cnt);
+      if (MEASURE && extra) atomicAdd(&a_extra[ow], extra);
+      if (MEASURE && bad) a_bad[ow] = 1u;
+    }
+    __syncwarp();
+    uint32_t ub = a_cnt[l], text_esc = 0;
+    if (MEASURE) text_esc = a_bad[l] ? 0u : len + a_extra[l];
+    if (ub >= (1u << 20)) {  // seq packing of the frontier needs ordinal < 2^20 (SEQ_ORD_BITS)
+      atomicOr(o.err, ERR_TOO_MANY_LINKS);
+      ub = 0;
+    }
+    // one arena reservation for the group (links_compact puts the links in record order)
+    const uint32_t ub_incl = warp_incl_scan(ub), ub_total = __shfl_sync(FULL, ub_incl, 31);
+    uint32_t gstart = 0;
+    if (ub_total) {
+      if (l == 31) gstart = atomicAdd(o.cursor, ub_total);
+      gstart = __shfl_sync(FULL, gstart, 31);
+    }
+    const uint32_t lstart = ub ? gstart + (ub_incl - ub) : 0u;
+    const bool fits = (uint64_t)gstart + ub_incl <= o.arena_cap;
+    if (ub && !fits) atomicOr(o.err, ERR_ARENA_OVERFLOW);
+    uint32_t nlinks = 0;
+    for (uint32_t todo = __ballot_sync(FULL, ub && fits); todo; todo &= todo - 1) {
+      const int k = __ffs(todo) - 1;
+      const tgi_tg_chan* ch = &b.chans[b.recs[g * 32 + k].chan_idx];
+      LinkSink ls;
+      ls.out = o.arena + __shfl_sync(FULL, lstart, k);
+      ls.cap = __shfl_sync(FULL, ub, k);
+      ls.count = 0;
+      ls.name_bytes = 0;
+      ls.self = b.chan_strs + ch->str_off + ch->title_len;
+      ls.self_len = ch->name_len;
+      // a record without entities: warp_extract_links is the plaintext scan alone
+      warp_scan_channel_links(ls, (const uint8_t*)__shfl_sync(FULL, (unsigned long long)text, k), __shfl_sync(FULL, len, k),
+                              TGI_SRC_PLAINTEXT, true);
+      if (l == k) nlinks = ls.count;
+    }
+    if (mine) {
+      o.status[r] = (uint8_t)status;
+      o.linelen[r] = MEASURE && status == TGI_ST_EMITTED ? text_esc : 0u;  // the size pass overwrites the emitted ones
+      o.link_start[r] = lstart;
+      o.link_count[r] = nlinks;
     }
   }
 }

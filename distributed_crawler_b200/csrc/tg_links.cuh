@@ -146,11 +146,39 @@ DEVI uint32_t warp_count_tme(const uint8_t* s, int64_t n) {
   return warp_sum(cnt);
 }
 
+// 16 bytes of a text w (bytes past its end read as ' ') with the 4 bytes in front of them pw (' ' at its start), measured
+// for the JSONL line: bad |= the bits that make the text not clean (utf8_unclean4), extra += what JSON escaping adds.
+// The bytes are classified once: ASCII needs no clean test, bytes without a 3- or 4-byte lead (Latin, Cyrillic, Arabic)
+// take utf8_unclean2, the rest utf8_unclean4 word by word; the escape count looks only at the bytes the special-byte
+// test (esc_special4) flags.
+DEVI void measure16(const uint4 w, uint32_t pw, uint32_t& bad, uint32_t& extra) {
+  if ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) {  // not ASCII
+    // pw's first byte governs no byte of w: a lead there covers at most pw's other three
+    if ((utf8_lead3(w.x) | utf8_lead3(w.y) | utf8_lead3(w.z) | utf8_lead3(w.w) | utf8_lead3(pw & 0xFFFFFF00u)) == 0) {
+      bad |= utf8_unclean2(pw, w.x) | utf8_unclean2(w.x, w.y) | utf8_unclean2(w.y, w.z) | utf8_unclean2(w.z, w.w);
+    } else {
+      uint4 v = w;
+#pragma unroll 1
+      for (int k = 0; k < 4; k++) {  // a word at a time: the parse kernels' code has to stay small (instruction cache)
+        bad |= utf8_unclean4(pw, v.x);
+        pw = v.x;
+        v = make_uint4(v.y, v.z, v.w, v.x);
+      }
+    }
+  }
+  // bit 8j + k: byte j of word k may need escaping (line breaks, quotes, '<', '&': few lanes have one)
+  uint32_t sp = (esc_special4(w.x) >> 7) | (esc_special4(w.y) >> 6) | (esc_special4(w.z) >> 5) | (esc_special4(w.w) >> 4);
+  while (sp) {
+    const int b = __ffs(sp) - 1, k = b & 7;
+    sp &= sp - 1;
+    const uint32_t x = k == 0 ? w.x : (k == 1 ? w.y : (k == 2 ? w.z : w.w));
+    extra += ascii_esc_len((x >> (b & ~7)) & 0xFFu) - 1u;  // a flagged byte is ASCII; the text copies the others as they are
+  }
+}
+
 // The same count, and the text measured from the same 16 bytes per lane (JSONL runs): esc_len = its JSON-escaped length
 // if it is clean (utf8_unclean4), 0 if not (or if n == 0).  The lane's 4 bytes in front come from the lane below, or
-// for lane 0 from the previous strip's last lane.  The lane classifies its 16 bytes once: ASCII needs no clean test,
-// bytes without a 3- or 4-byte lead (Latin, Cyrillic, Arabic) take utf8_unclean2, the rest utf8_unclean4 word by
-// word; the escape count looks only at the bytes the special-byte test (esc_special4) flags.
+// for lane 0 from the previous strip's last lane.
 DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len) {
   const int l = lane_id();
   const uint32_t SP = 0x20202020u;
@@ -164,30 +192,9 @@ DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len)
       if (rem < 16) w = make_uint4(blank_from(w.x, rem), blank_from(w.y, rem - 4), blank_from(w.z, rem - 8), blank_from(w.w, rem - 12));
     }
     const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
-    uint32_t pw = l == 0 ? tail : below;
+    const uint32_t pw = l == 0 ? tail : below;
     tail = __shfl_sync(FULL, w.w, 31);
-    if ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) {  // not ASCII
-      // pw's first byte governs no byte of w: a lead there covers at most pw's other three
-      if ((utf8_lead3(w.x) | utf8_lead3(w.y) | utf8_lead3(w.z) | utf8_lead3(w.w) | utf8_lead3(pw & 0xFFFFFF00u)) == 0) {
-        bad |= utf8_unclean2(pw, w.x) | utf8_unclean2(w.x, w.y) | utf8_unclean2(w.y, w.z) | utf8_unclean2(w.z, w.w);
-      } else {
-        uint4 v = w;
-#pragma unroll 1
-        for (int k = 0; k < 4; k++) {  // a word at a time: the parse kernels' code has to stay small (instruction cache)
-          bad |= utf8_unclean4(pw, v.x);
-          pw = v.x;
-          v = make_uint4(v.y, v.z, v.w, v.x);
-        }
-      }
-    }
-    // bit 8j + k: byte j of word k may need escaping (line breaks, quotes, '<', '&': few lanes have one)
-    uint32_t sp = (esc_special4(w.x) >> 7) | (esc_special4(w.y) >> 6) | (esc_special4(w.z) >> 5) | (esc_special4(w.w) >> 4);
-    while (sp) {
-      const int b = __ffs(sp) - 1, k = b & 7;
-      sp &= sp - 1;
-      const uint32_t x = k == 0 ? w.x : (k == 1 ? w.y : (k == 2 ? w.z : w.w));
-      extra += ascii_esc_len((x >> (b & ~7)) & 0xFFu) - 1u;  // a flagged byte is ASCII; the text copies the others as they are
-    }
+    measure16(w, pw, bad, extra);
   }
   // a text that ends with its last strip: a sequence open at the end (one needs a high bit in tail's last three bytes)
   if (tail & 0x80808000u) bad |= utf8_unclean4(tail, SP);

@@ -1390,8 +1390,6 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
     }
     po = tg_parse_out(s, s.d_status.as<uint8_t>(), dsc, arena_cap);
     if (n) {
-      uint64_t want = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-      unsigned g = (unsigned)std::min<uint64_t>(want, (uint64_t)c->sms * grid_mult());
       CK(cudaEventRecord(s.ev_p0, st));
       const uint64_t groups = (n + 31) / 32;
       unsigned ge = (unsigned)std::min<uint64_t>((groups + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (uint64_t)c->sms * grid_mult());
@@ -1404,8 +1402,8 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
         else tg_parse_ent_kernel<false><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
         launches += 2;
       }
-      if (measure) tg_parse_kernel<true><<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, po);  // records without entities
-      else tg_parse_kernel<false><<<g, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
+      if (measure) tg_parse_kernel<true><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);  // records without entities
+      else tg_parse_kernel<false><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
       launches++;
       if (want_json) {
         tg_size_lane_kernel<<<ge, CTA_THREADS, 0, st>>>(b, cfg, po);
