@@ -1027,119 +1027,143 @@ __global__ void st_edge_emit_kernel(StEdges e) {
 }
 
 // ---- tandem hand-off SQL (state/daprstate.go:3643-3678, 3896-3941): the params of every binding call ----------------
-// Rows are numbered batch inserts [0, nb), edge inserts [nb, nb + ne), batch closes [nb + ne, 2 nb + ne); a statement
-// holds k consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names, URLs),
-// which the sequential escaper handles without the warp's 128-byte strips idling most lanes.
-struct StSql {
-  const tgi_state_edge* edges;          // the hand-off, as tgi_state_pending_edges left it on the device
-  const tgi_state_edge_batch* batches;
-  const tgi_state_span* spans;
-  uint64_t ne, nb, n_rows;
-  uint32_t k;                           // rows per statement
+// A SQL call's statements: kind i (TGI_SQL_* kind0 + i) has rows[i] rows, numbered after the kinds before it; a
+// statement holds k consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names,
+// URLs), which the sequential escaper handles without the warp's 128-byte strips idling most lanes.
+struct StSqlPlan {
+  uint32_t kind0, k;                    // the first kind, rows per statement
+  uint64_t rows[3], m[3];               // rows and statements of each kind
+  uint64_t n_stmts;
   uint32_t crawl_len, time_len;
   const uint8_t* crawl;                 // crawl_id as given, then discovery_time rendered with its quotes
   const uint8_t* time;
-  uint32_t* size;                       // [n_rows] bytes of row r
-  uint64_t* off;                        // [n_rows+1] their scan
+  uint32_t* size;                       // [rows] bytes of row r
+  uint64_t* off;                        // [rows+1] their scan
   uint64_t* sc;                         // ST_SC_*: ST_SC_BIG
   uint8_t* out;
   tgi_state_edge_stmt* stmts;           // [n_stmts]
-  uint64_t n_stmts, m[3];               // statements in all and of each kind
   uint64_t sql_off[6], sql_len[6];      // the texts of kind i: [2i] k rows, [2i+1] the kind's last, shorter statement
   uint64_t base;                        // the params' offset in the output
 };
 
-// one row's values, sized (dst == nullptr) or written, with the statement's "[" before its first row, "," before the
-// others and "]" after its last
+// one row's values, sized (EMIT false) or written at dst: the statement's "[" before its first row and "," before the
+// others, quoted escaped strings, page fields, numbers, raw bytes (the rendered clock), "]" after its last row
 template <bool EMIT>
-DEVI StLen<EMIT> st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* dst) {
-  StLen<EMIT> o = 0;
-  auto lit = [&](const char* s, uint32_t n) {
+struct StSqlRow {
+  uint8_t* dst;
+  StLen<EMIT> o;
+  DEVI void lit(const void* s, uint32_t n) {
     if (EMIT)
-      for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
+      for (uint32_t k = 0; k < n; k++) dst[o + k] = ((const uint8_t*)s)[k];
     o += n;
-  };
-  auto esc = [&](const uint8_t* s, uint32_t n) { o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n); };
-  auto str = [&](const uint8_t* s, uint32_t n) {
+  }
+  DEVI void str(const uint8_t* s, uint32_t n) {
     lit("\"", 1);
-    esc(s, n);
+    o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n);
     lit("\"", 1);
-  };
-  auto field = [&](const tgi_state_page& p, int f) {
+  }
+  DEVI void field(const StDev& d, const tgi_state_page& p, int f) {
     uint32_t n;
     const uint8_t* s = st_str(d, p, f, n);
     str(s, n);
-  };
-  const uint32_t kind = r < q.nb ? 0u : r < q.nb + q.ne ? 1u : 2u;
-  const uint64_t i = kind == 0 ? r : kind == 1 ? r - q.nb : r - q.nb - q.ne;  // the row within its kind
-  const uint64_t n = kind == 1 ? q.ne : q.nb;
-  lit(i % q.k ? "," : "[", 1);
-  const tgi_state_edge* e = kind == 1 ? q.edges + i : nullptr;
-  const tgi_state_edge_batch& b = q.batches[e ? e->batch : (uint32_t)i];
-  str(b.batch_id, 36);
-  if (kind != 2) {
-    const tgi_state_page& p = d.pages[q.spans[b.span].row];  // the owner
-    lit(",", 1);
-    str(q.crawl, q.crawl_len);
-    lit(",", 1);
-    if (kind == 0) {  // CreatePendingBatch (daprstate.go:3897-3906)
-      field(p, TGI_PS_URL);
-      lit(",", 1);
-      field(p, TGI_PS_ID);
-      lit(",", 1);
-      o += EMIT ? (uint32_t)render_i64(dst + o, p.depth) : ndigits_i64(p.depth);
-      lit(",", 1);
-      field(p, TGI_PS_SEQ);
-      lit(",\"open\"", 7);
-    } else {  // InsertPendingEdge (:3915-3926)
-      str(e->destination, e->dest_len);
-      lit(",", 1);
-      field(p, TGI_PS_URL);
-      lit(",", 1);
-      field(p, TGI_PS_SEQ);
-      lit(",", 1);
-      if (EMIT)
-        for (uint32_t k = 0; k < q.time_len; k++) dst[o + k] = q.time[k];
-      o += q.time_len;
-      switch (e->source_type) {  // tdutils.go:978-987
-        case TGI_SRC_MENTION: lit(",\"mention\"", 10); break;
-        case TGI_SRC_TEXT_URL: lit(",\"text_url\"", 11); break;
-        case TGI_SRC_URL: lit(",\"url\"", 6); break;
-        default: lit(",\"plaintext\"", 12); break;
-      }
-      lit(",\"pending\"", 10);
-    }
   }
-  if (i % q.k == q.k - 1 || i == n - 1) lit("]", 1);
-  return o;
-}
-
-__global__ void st_sql_size_kernel(StDev d, StSql q) {
-  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t sz = st_sql_row<false>(d, q, r, nullptr);
-    q.size[r] = (uint32_t)sz;
-    st_flag_big(q.sc, sz);
+  DEVI void num(long long v) { o += EMIT ? (uint32_t)render_i64(dst + o, v) : ndigits_i64(v); }
+  DEVI void open(uint64_t j, uint32_t k) { lit(j % k ? "," : "[", 1); }  // row j of its kind
+  DEVI void close(uint64_t j, uint32_t k, uint64_t n) {
+    if (j % k == k - 1 || j == n - 1) lit("]", 1);
   }
-}
+};
 
-// the rows at their scanned offsets, then every statement's entry: its rows, its kind's text, its params' span
-__global__ void st_sql_emit_kernel(StDev d, StSql q) {
-  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < q.n_rows; r += (uint64_t)gridDim.x * blockDim.x)
-    st_sql_row<true>(d, q, r, q.out + q.off[r]);
+// every statement's entry: its kind, rows, text and params' span
+DEVI void st_sql_stmts(const StSqlPlan& q) {
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < q.n_stmts; s += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t kind = s < q.m[0] ? 0u : s < q.m[0] + q.m[1] ? 1u : 2u;
-    const uint64_t j = kind == 0 ? s : kind == 1 ? s - q.m[0] : s - q.m[0] - q.m[1];
-    const uint64_t n = kind == 1 ? q.ne : q.nb, first = (kind == 0 ? 0 : kind == 1 ? q.nb : q.nb + q.ne) + j * q.k;
-    const uint32_t rows = (uint32_t)min((uint64_t)q.k, n - j * q.k);
+    uint32_t kind = 0;
+    uint64_t j = s, first = 0;
+    for (; j >= q.m[kind]; kind++) {
+      j -= q.m[kind];
+      first += q.rows[kind];
+    }
+    first += j * q.k;
+    const uint32_t rows = (uint32_t)min((uint64_t)q.k, q.rows[kind] - j * q.k);
     const uint32_t t = 2 * kind + (rows != q.k);
     tgi_state_edge_stmt& st = q.stmts[s];
-    st.kind = kind;
+    st.kind = q.kind0 + kind;
     st.rows = rows;
     st.sql_off = q.sql_off[t];
     st.sql_len = q.sql_len[t];
     st.params_off = q.base + q.off[first];
     st.params_len = q.off[first + rows] - q.off[first];
   }
+}
+
+// the hand-off's rows: batch inserts [0, nb), edge inserts [nb, nb + ne), batch closes [nb + ne, 2 nb + ne)
+struct StSql {
+  StSqlPlan p;                          // rows {nb, ne, nb} from TGI_SQL_BATCH_INSERT
+  const tgi_state_edge* edges;          // the hand-off, as tgi_state_pending_edges left it on the device
+  const tgi_state_edge_batch* batches;
+  const tgi_state_span* spans;
+};
+
+template <bool EMIT>
+DEVI StLen<EMIT> st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t* dst) {
+  StSqlRow<EMIT> w{dst, 0};
+  const uint64_t nb = q.p.rows[0], ne = q.p.rows[1];
+  const uint32_t kind = r < nb ? 0u : r < nb + ne ? 1u : 2u;
+  const uint64_t i = kind == 0 ? r : kind == 1 ? r - nb : r - nb - ne;  // the row within its kind
+  w.open(i, q.p.k);
+  const tgi_state_edge* e = kind == 1 ? q.edges + i : nullptr;
+  const tgi_state_edge_batch& b = q.batches[e ? e->batch : (uint32_t)i];
+  w.str(b.batch_id, 36);
+  if (kind != 2) {
+    const tgi_state_page& p = d.pages[q.spans[b.span].row];  // the owner
+    w.lit(",", 1);
+    w.str(q.p.crawl, q.p.crawl_len);
+    w.lit(",", 1);
+    if (kind == 0) {  // CreatePendingBatch (daprstate.go:3897-3906)
+      w.field(d, p, TGI_PS_URL);
+      w.lit(",", 1);
+      w.field(d, p, TGI_PS_ID);
+      w.lit(",", 1);
+      w.num(p.depth);
+      w.lit(",", 1);
+      w.field(d, p, TGI_PS_SEQ);
+      w.lit(",\"open\"", 7);
+    } else {  // InsertPendingEdge (:3915-3926)
+      w.str(e->destination, e->dest_len);
+      w.lit(",", 1);
+      w.field(d, p, TGI_PS_URL);
+      w.lit(",", 1);
+      w.field(d, p, TGI_PS_SEQ);
+      w.lit(",", 1);
+      w.lit(q.p.time, q.p.time_len);
+      switch (e->source_type) {  // tdutils.go:978-987
+        case TGI_SRC_MENTION: w.lit(",\"mention\"", 10); break;
+        case TGI_SRC_TEXT_URL: w.lit(",\"text_url\"", 11); break;
+        case TGI_SRC_URL: w.lit(",\"url\"", 6); break;
+        default: w.lit(",\"plaintext\"", 12); break;
+      }
+      w.lit(",\"pending\"", 10);
+    }
+  }
+  w.close(i, q.p.k, kind == 1 ? ne : nb);
+  return w.o;
+}
+
+__global__ void st_sql_size_kernel(StDev d, StSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_sql_row<false>(d, q, r, nullptr);
+    q.p.size[r] = (uint32_t)sz;
+    st_flag_big(q.p.sc, sz);
+  }
+}
+
+// the rows at their scanned offsets, then the statement table
+__global__ void st_sql_emit_kernel(StDev d, StSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    st_sql_row<true>(d, q, r, q.p.out + q.p.off[r]);
+  st_sql_stmts(q.p);
 }
 
 // ---- tandem forced walkback (crawl/runner.go:115-139, 1425-1455): the pick and the two rows of every edge-less span ---
@@ -1205,78 +1229,47 @@ __global__ void st_walk_pick_kernel(StDev d, StWalk w) {
   }
 }
 
-// The SQL of the picks: rows page_buffer [0, n_ok), edge_records [n_ok, 2 n_ok) in span order, a statement k consecutive
-// rows of one kind, as StSql.  Thread t of [0, 2 n) stands for span t % n's row of kind t / n, which it has when the
-// span is TGI_WALK_OK; rank[i] is its place among those.
+// The SQL of the picks: rows page_buffer [0, n_ok), edge_records [n_ok, 2 n_ok) in span order.  Thread t of [0, 2 n)
+// stands for span t % n's row of kind t / n, which it has when the span is TGI_WALK_OK; rank[i] is its place among those.
 struct StWalkSql {
+  StSqlPlan p;                         // rows {n_ok, n_ok} from TGI_SQL_PAGE_BUFFER_INSERT
   const uint32_t* spans;               // StWalk's
   const tgi_state_walkback_span* wb;   // [n] the picks
   const uint64_t* rank;                // [n+1] scan of StWalk::ok
-  uint64_t n, n_ok;
-  uint32_t k;                          // rows per statement
-  uint32_t crawl_len, time_len;
-  const uint8_t* crawl;                // crawl_id as given, then discovery_time rendered with its quotes
-  const uint8_t* time;
-  uint32_t* size;                      // [2 n_ok] bytes of row r
-  uint64_t* off;                       // [2 n_ok + 1] their scan
-  uint64_t* sc;                        // ST_SC_*: ST_SC_BIG
-  uint8_t* out;
-  tgi_state_edge_stmt* stmts;          // [2 m]
-  uint64_t m;                          // statements of each kind
-  uint64_t sql_off[4], sql_len[4];     // the texts of kind i: [2i] k rows, [2i+1] the kind's last, shorter statement
-  uint64_t base;                       // the params' offset in the output
+  uint64_t n;
 };
 
-// one row's values, sized (dst == nullptr) or written, with the statement's "[" / "," / "]" as st_sql_row
 template <bool EMIT>
 DEVI StLen<EMIT> st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, uint64_t i, uint64_t j, uint8_t* dst) {
-  StLen<EMIT> o = 0;
-  auto lit = [&](const char* s, uint32_t n) {
-    if (EMIT)
-      for (uint32_t k = 0; k < n; k++) dst[o + k] = (uint8_t)s[k];
-    o += n;
-  };
-  auto str = [&](const uint8_t* s, uint32_t n) {
-    lit("\"", 1);
-    o += EMIT ? st_thread_esc(dst + o, s, n) : thread_esc_len<StLen<EMIT>>(s, n);
-    lit("\"", 1);
-  };
-  auto field = [&](const tgi_state_page& p, int f) {
-    uint32_t n;
-    const uint8_t* s = st_str(d, p, f, n);
-    str(s, n);
-  };
+  StSqlRow<EMIT> w{dst, 0};
   const tgi_state_walkback_span& b = q.wb[i];
   const tgi_state_page& p = d.pages[q.spans[2 * i + 1]];  // the owner
-  lit(j % q.k ? "," : "[", 1);
+  w.open(j, q.p.k);
   if (kind == 0) {  // AddPageToPageBuffer (daprstate.go:3620-3633)
-    str(b.page_id, 36);
-    lit(",", 1);
-    field(p, TGI_PS_ID);
-    lit(",", 1);
-    const int64_t depth = (int64_t)((uint64_t)p.depth + 1);  // owner.Depth + 1 wraps as Go's int
-    o += EMIT ? (uint32_t)render_i64(dst + o, depth) : ndigits_i64(depth);
-    lit(",", 1);
-    str(b.url, b.url_len);
-    lit(",", 1);
-    str(q.crawl, q.crawl_len);
-    lit(",", 1);
-    str(b.sequence_id, 36);
+    w.str(b.page_id, 36);
+    w.lit(",", 1);
+    w.field(d, p, TGI_PS_ID);
+    w.lit(",", 1);
+    w.num((int64_t)((uint64_t)p.depth + 1));  // owner.Depth + 1 wraps as Go's int
+    w.lit(",", 1);
+    w.str(b.url, b.url_len);
+    w.lit(",", 1);
+    w.str(q.p.crawl, q.p.crawl_len);
+    w.lit(",", 1);
+    w.str(b.sequence_id, 36);
   } else {  // SaveEdgeRecords of the walkback edge (:3176-3184)
-    str(b.url, b.url_len);
-    lit(",", 1);
-    field(p, TGI_PS_URL);
-    lit(",true,false,", 12);
-    if (EMIT)
-      for (uint32_t k = 0; k < q.time_len; k++) dst[o + k] = q.time[k];
-    o += q.time_len;
-    lit(",", 1);
-    str(q.crawl, q.crawl_len);
-    lit(",", 1);
-    field(p, TGI_PS_SEQ);
+    w.str(b.url, b.url_len);
+    w.lit(",", 1);
+    w.field(d, p, TGI_PS_URL);
+    w.lit(",true,false,", 12);
+    w.lit(q.p.time, q.p.time_len);
+    w.lit(",", 1);
+    w.str(q.p.crawl, q.p.crawl_len);
+    w.lit(",", 1);
+    w.field(d, p, TGI_PS_SEQ);
   }
-  if (j % q.k == q.k - 1 || j == q.n_ok - 1) lit("]", 1);
-  return o;
+  w.close(j, q.p.k, q.p.rows[0]);
+  return w.o;
 }
 
 __global__ void st_walk_size_kernel(StDev d, StWalkSql q) {
@@ -1285,32 +1278,20 @@ __global__ void st_walk_size_kernel(StDev d, StWalkSql q) {
     const uint64_t i = t - kind * q.n, j = q.rank[i];
     if (q.rank[i + 1] > j) {
       const uint64_t sz = st_walk_row<false>(d, q, kind, i, j, nullptr);
-      q.size[kind * q.n_ok + j] = (uint32_t)sz;
-      st_flag_big(q.sc, sz);
+      q.p.size[kind * q.p.rows[0] + j] = (uint32_t)sz;
+      st_flag_big(q.p.sc, sz);
     }
   }
 }
 
-// the rows at their scanned offsets, then every statement's entry
+// the rows at their scanned offsets, then the statement table
 __global__ void st_walk_emit_kernel(StDev d, StWalkSql q) {
   for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < 2 * q.n; t += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t kind = t >= q.n;
     const uint64_t i = t - kind * q.n, j = q.rank[i];
-    if (q.rank[i + 1] > j) st_walk_row<true>(d, q, kind, i, j, q.out + q.off[kind * q.n_ok + j]);
+    if (q.rank[i + 1] > j) st_walk_row<true>(d, q, kind, i, j, q.p.out + q.p.off[kind * q.p.rows[0] + j]);
   }
-  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < 2 * q.m; s += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t kind = s >= q.m;
-    const uint64_t j = s - kind * q.m, first = kind * q.n_ok + j * q.k;
-    const uint32_t rows = (uint32_t)min((uint64_t)q.k, q.n_ok - j * q.k);
-    const uint32_t t = 2 * kind + (rows != q.k);
-    tgi_state_edge_stmt& st = q.stmts[s];
-    st.kind = TGI_SQL_PAGE_BUFFER_INSERT + kind;
-    st.rows = rows;
-    st.sql_off = q.sql_off[t];
-    st.sql_len = q.sql_len[t];
-    st.params_off = q.base + q.off[first];
-    st.params_len = q.off[first + rows] - q.off[first];
-  }
+  st_sql_stmts(q.p);
 }
 
 // ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------

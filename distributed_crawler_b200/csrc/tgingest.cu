@@ -3664,22 +3664,14 @@ int st_drop_messages(tgi_ctx* c, CrawlState& S, uint32_t r) {
   return TGI_OK;
 }
 
-// json.Marshal(page) of the P rows by the export's line passes: their cnt messages are sorted[0, cnt) (message indices
-// grouped by row, each row's in list order; srows[] holds the row of each), and the caller has set row_base[row] for
-// every listed row (its first grouped message; any value for a row without messages).  The size pass is enqueued into
-// r (no synchronise); once the host has S.sc in hs, st_page_json_emit writes the lines and brings them back.  tiled:
-// the scans take their multi-launch form whatever their length, so the launch count does not depend on P.
-int st_page_json_size(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, const uint32_t* sorted, const uint32_t* srows,
-                      uint64_t cnt, bool tiled, StRender& r, uint32_t& launches) {
-  cudaStream_t st = S.stream;
-  int rc;
-  CK(S.entries.ensure(P * sizeof(StEntry)));
-  CK(S.msize.ensure(cnt * 4));
-  CK(S.moff.ensure((cnt + 1) * 8));
-  CK(S.e32.ensure(4 * P * 4));
-  CK(S.e64.ensure(2 * (P + 1) * 8));
+// r over the state's render buffers for ne entries: the zone, S.sc, row_base, msize and moff as the caller sized them,
+// and the per-entry arrays in S.entries, S.e32 and S.e64, sized here
+int st_render_bind(tgi_ctx* c, CrawlState& S, uint64_t ne, StRender& r) {
+  CK(S.entries.ensure(ne * sizeof(StEntry)));
+  CK(S.e32.ensure(4 * ne * 4));
+  CK(S.e64.ensure(2 * (ne + 1) * 8));
   r.entries = S.entries.as<StEntry>();
-  r.n_entries = P;
+  r.n_entries = ne;
   r.zone = c->cfgdev.zone;
   r.zone_n = c->cfgdev.zone_n;
   r.tz = c->cfgdev.tz;
@@ -3688,11 +3680,27 @@ int st_page_json_size(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t 
   r.msize = S.msize.as<uint32_t>();
   r.moff = S.moff.as<uint64_t>();
   r.esize_lo = S.e32.as<uint32_t>();
-  r.ebytes = r.esize_lo + P;
-  r.ecnt = r.ebytes + P;
-  r.esz = r.ecnt + P;
+  r.ebytes = r.esize_lo + ne;
+  r.ecnt = r.ebytes + ne;
+  r.esz = r.ecnt + ne;
   r.eoff = S.e64.as<uint64_t>();
-  r.eslot = r.eoff + P + 1;
+  r.eslot = r.eoff + ne + 1;
+  return TGI_OK;
+}
+
+// json.Marshal(page) of the P rows by the export's line passes: their cnt messages are sorted[0, cnt) (message indices
+// grouped by row, each row's in list order; srows[] holds the row of each), and the caller has set row_base[row] for
+// every listed row (its first grouped message; with cnt = 0, 0 for every row, as st_entry_size reads moff[row_base[row]]).
+// The size pass is enqueued into r (no synchronise); once the host has S.sc in hs, st_page_json_emit writes the lines
+// and brings them back.  tiled: the scans take their multi-launch form whatever their length, so the launch count does
+// not depend on P.
+int st_page_json_size(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, const uint32_t* sorted, const uint32_t* srows,
+                      uint64_t cnt, bool tiled, StRender& r, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  int rc;
+  CK(S.msize.ensure(cnt * 4));
+  CK(S.moff.ensure((cnt + 1) * 8));
+  if ((rc = st_render_bind(c, S, P, r))) return rc;
   const StDev d = st_dev(S);
   std::vector<StEntry> E(P);
   for (uint32_t k = 0; k < P; k++) E[k] = StEntry{(long long)S.rows[rows[k]].depth, rows[k], 0};
@@ -3707,7 +3715,8 @@ int st_page_json_size(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t 
   st_line_size_kernel<<<sink_grid(c, P, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
   launches++;
   if ((rc = launch_scan(c, st, S.tiles, r.esz, P, r.eoff, r.sc + ST_SC_BYTES, launches, tiled))) return rc;
-  if ((rc = launch_scan(c, st, S.tiles, r.ecnt, P, r.eslot, r.sc + ST_SC_SLOTS, launches, tiled))) return rc;
+  // the message slots: read only by st_msg_emit_kernel, which runs only when there are messages
+  if (cnt && (rc = launch_scan(c, st, S.tiles, r.ecnt, P, r.eslot, r.sc + ST_SC_SLOTS, launches, tiled))) return rc;
   CK(cudaGetLastError());
   return TGI_OK;
 }
@@ -3767,31 +3776,14 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
   CK(S.row_base.ensure((nr + 1) * 8));
   CK(S.msize.ensure(live * 4));
   CK(S.moff.ensure((live + 1) * 8));
-  CK(S.entries.ensure(ne * sizeof(StEntry)));
-  CK(S.e32.ensure(4 * ne * 4));
-  CK(S.e64.ensure(2 * (ne + 1) * 8));
   StRender r{};
-  r.entries = S.entries.as<StEntry>();
-  r.n_entries = ne;
-  r.zone = c->cfgdev.zone;
-  r.zone_n = c->cfgdev.zone_n;
-  r.tz = c->cfgdev.tz;
-  r.sc = S.sc.as<uint64_t>();
+  if ((rc = st_render_bind(c, S, ne, r))) return rc;
   r.flag = S.flag.as<uint32_t>();
   r.pos = S.pos.as<uint64_t>();
   r.keys[0] = S.keys.as<uint32_t>();
   r.keys[1] = r.keys[0] + live;
   r.vals[0] = S.vals.as<uint32_t>();
   r.vals[1] = r.vals[0] + live;
-  r.row_base = S.row_base.as<uint64_t>();
-  r.msize = S.msize.as<uint32_t>();
-  r.moff = S.moff.as<uint64_t>();
-  r.esize_lo = S.e32.as<uint32_t>();
-  r.ebytes = r.esize_lo + ne;
-  r.ecnt = r.ebytes + ne;
-  r.esz = r.ecnt + ne;
-  r.eoff = S.e64.as<uint64_t>();
-  r.eslot = r.eoff + ne + 1;
   // radix passes over the bits of the largest row
   uint32_t bits = 0;
   while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
@@ -3848,6 +3840,50 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
   CK(cudaGetLastError());
   CK(cudaEventRecord(S.t3, st));
   return TGI_OK;
+}
+
+// The two passes of a writer with a thread per piece (a layer-map id, a SQL row) and block ST_THREADS: size writes the n
+// pieces' sizes to sz, which the scan turns into off and their total in ST_SC_BYTES, read back with one synchronise.  A
+// piece of 4 GiB or more refuses the call (noun names it) before anything is written; else *body is the output's
+// length, and st_rows_emit sizes out for it, points *dst at it and enqueues emit.  Once the emit has finished,
+// st_rows_ms is the device time of both passes.
+template <class A>
+int st_rows_size(tgi_ctx* c, CrawlState& S, void (*size)(StDev, A), const A& a, unsigned grid, const uint32_t* sz, uint64_t n,
+                 uint64_t* off, const char* who, const char* noun, uint64_t* body, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  int rc;
+  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
+  CK(cudaEventRecord(S.t0, st));
+  size<<<grid, ST_THREADS, 0, st>>>(st_dev(S), a);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, sz, n, off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t* hs = S.h_sc.as<uint64_t>();
+  if (hs[ST_SC_BIG]) { set_err(c, "%s: %s renders to 4 GiB or more", who, noun); return TGI_E_CAPACITY; }
+  *body = hs[ST_SC_BYTES];
+  return TGI_OK;
+}
+template <class A>
+int st_rows_emit(tgi_ctx* c, CrawlState& S, void (*emit)(StDev, A), A& a, uint8_t** dst, DevBuf& out, uint64_t body,
+                 unsigned grid, uint32_t& launches) {
+  cudaStream_t st = S.stream;
+  CK(out.ensure(body));
+  *dst = out.as<uint8_t>();
+  CK(cudaEventRecord(S.t2, st));
+  emit<<<grid, ST_THREADS, 0, st>>>(st_dev(S), a);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t3, st));
+  return TGI_OK;
+}
+float st_rows_ms(const CrawlState& S) {
+  float size_ms = 0, emit_ms = 0;
+  cudaEventElapsedTime(&size_ms, S.t0, S.t1);
+  cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
+  return size_ms + emit_ms;
 }
 
 // the m UpdateMessage calls in S.upd, in order (rows valid, st_reserve(m) done): the batch table, one probe per distinct
@@ -4474,34 +4510,16 @@ int tgi_state_layer_map(tgi_ctx* c, tgi_state_json_t* out) {
     L.size = S.e32.as<uint32_t>();
     L.off = S.e64.as<uint64_t>();
     L.sc = S.sc.as<uint64_t>();
-    const StDev d = st_dev(S);
     CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StLmEntry), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(S.lm_keys.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-    CK(cudaEventRecord(S.t0, st));
-    st_lm_size_kernel<<<st_grid(c, ne), ST_THREADS, 0, st>>>(d, L);
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, L.size, ne, L.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(S.t1, st));
-    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "tgi_state_layer_map: an id renders to 4 GiB or more"); return TGI_E_CAPACITY; }
-    body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
-    CK(S.out.ensure(body));
+    const unsigned grid = st_grid(c, ne);
+    if ((rc = st_rows_size(c, S, st_lm_size_kernel, L, grid, L.size, ne, L.off, "tgi_state_layer_map", "an id", &body, launches)))
+      return rc;
     CK(S.h_out.ensure(body + 2));
-    L.out = S.out.as<uint8_t>();
-    CK(cudaEventRecord(S.t2, st));
-    st_lm_emit_kernel<<<st_grid(c, ne), ST_THREADS, 0, st>>>(d, L);
-    launches++;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(S.t3, st));
+    if ((rc = st_rows_emit(c, S, st_lm_emit_kernel, L, &L.out, S.out, body, grid, launches))) return rc;
     CK(cudaMemcpyAsync(S.h_out.as<uint8_t>() + 1, S.out.p, body, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    float size_ms = 0, emit_ms = 0;
-    cudaEventElapsedTime(&size_ms, S.t0, S.t1);
-    cudaEventElapsedTime(&emit_ms, S.t2, S.t3);
-    out->kernel_ms = size_ms + emit_ms;
+    out->kernel_ms = st_rows_ms(S);
   } else {
     CK(S.h_out.ensure(2));
   }
@@ -5351,12 +5369,20 @@ int disc_gather(tgi_ctx* c, CrawlState& S, Slot& s, const tgi_state_span* spans,
   return TGI_OK;
 }
 
-// First occurrences (per span, or over the list) and Dapr's urlCache test over the candidates at d_cands (count d_n on
-// the device, at most bound), compacted into S.surv; the survivors come back to S.h_surv with one id each from counter
-// id_next on (S.h_ids).  Two synchronises: the survivors' count, then their rows and ids.
+// First occurrences (per span, or over the list) and, with url_test, Dapr's urlCache test over the candidates at d_cands
+// (count d_n on the device, at most bound), compacted into S.surv; the survivors come back to S.h_surv with one id each
+// from counter id_next on (S.h_ids).  Two synchronises: the survivors' count, then their rows and ids.  The urlCache is
+// read under fr_mu, behind its last change.
 int st_survivors(tgi_ctx* c, CrawlState& S, const StCand* d_cands, const uint64_t* d_n, uint64_t bound, bool per_span,
-                 bool dedup, const FrontierDev& urls, uint64_t* n_surv, float* ms, uint32_t& launches) {
+                 bool dedup, bool url_test, uint64_t* n_surv, float* ms, uint32_t& launches) {
   cudaStream_t st = S.stream;
+  std::unique_lock<std::mutex> fg(c->fr_mu, std::defer_lock);
+  FrontierDev urls{};
+  if (url_test) {
+    fg.lock();
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    urls = c->sets[TGI_SET_URLS].dev;
+  }
   const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * bound, 64));
   CK(S.bfirst.ensure(bslots * 4));
   CK(S.slot_of.ensure(bound * 4));
@@ -5519,73 +5545,25 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
   out->rows = hr;
   out->ids = ids;
   if (!json) return TGI_OK;
-  // 4. json.Marshal of every added page: the export's line passes over the added rows, which hold no messages
+  // 4. json.Marshal of every added page by the page turns' line passes over the added rows, which hold no messages
   if (!n_add) return disc_json_empty(c, S, out);
-  CK(S.h_json_off.ensure((n_add + 1) * 8));
   if ((rc = st_upload_codes(c, S))) return rc;
   std::lock_guard<std::mutex> zg(c->cfg_mu);  // the zone table, as in tgi_state_render
   cudaStream_t st = S.stream;
-  const uint64_t ne = n_add, nr = S.rows.size();
-  CK(S.entries.ensure(ne * sizeof(StEntry)));
+  const uint64_t nr = S.rows.size();
   CK(S.row_base.ensure((nr + 1) * 8));
-  CK(S.moff.ensure(8));
-  CK(S.msize.ensure(4));
-  CK(S.e32.ensure(4 * ne * 4));
-  CK(S.e64.ensure(2 * (ne + 1) * 8));
+  CK(cudaMemsetAsync(S.row_base.p, 0, (nr + 1) * 8, st));
   StRender r{};
-  r.entries = S.entries.as<StEntry>();
-  r.n_entries = ne;
-  r.zone = c->cfgdev.zone;
-  r.zone_n = c->cfgdev.zone_n;
-  r.tz = c->cfgdev.tz;
-  r.sc = S.sc.as<uint64_t>();
-  r.row_base = S.row_base.as<uint64_t>();  // every row at 0: the added rows count no messages
-  r.msize = S.msize.as<uint32_t>();
-  r.moff = S.moff.as<uint64_t>();
-  r.esize_lo = S.e32.as<uint32_t>();
-  r.ebytes = r.esize_lo + ne;
-  r.ecnt = r.ebytes + ne;
-  r.esz = r.ecnt + ne;
-  r.eoff = S.e64.as<uint64_t>();
-  r.eslot = r.eoff + ne + 1;
-  std::vector<StEntry> E(ne);
-  for (uint64_t q = 0; q < ne; q++) E[q] = StEntry{(long long)S.rows[hr[q]].depth, hr[q], 0};
-  const StDev d = st_dev(S);
   uint64_t* hs = S.h_sc.as<uint64_t>();
-  CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(r.row_base, 0, (nr + 1) * 8, st));
-  CK(cudaMemsetAsync(r.moff, 0, 8, st));
-  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-  const unsigned grid = sink_grid(c, ne, ST_WARPS, 16);
   CK(cudaEventRecord(S.t4, st));
-  st_line_size_kernel<<<grid, ST_WARPS * 32, 0, st>>>(d, r);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, r.esz, ne, r.eoff, r.sc + ST_SC_BYTES, launches))) return rc;
-  CK(cudaGetLastError());
+  if ((rc = st_page_json_size(c, S, hr, (uint32_t)n_add, nullptr, nullptr, 0, false, r, launches))) return rc;
   CK(cudaEventRecord(S.t5, st));
   CK(cudaMemcpyAsync(hs, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  float t = 0;
-  cudaEventElapsedTime(&t, S.t4, S.t5);
-  *ms += t;
-  if (hs[ST_SC_ERR]) { set_err(c, "%s: a page timestamp's year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
-  if (hs[ST_SC_BIG]) { set_err(c, "%s: an added page renders to 4 GiB or more (its parentId)", who); return TGI_E_CAPACITY; }
-  const uint64_t body = hs[ST_SC_BYTES];
-  CK(S.out.ensure(body));
-  CK(S.h_out.ensure(body));
-  r.out = S.out.as<uint8_t>();
-  CK(cudaEventRecord(S.t4, st));
-  st_line_emit_kernel<<<grid, ST_WARPS * 32, 0, st>>>(d, r);
-  launches++;
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(S.t5, st));
-  CK(cudaMemcpyAsync(S.h_out.p, S.out.p, body, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(S.h_json_off.p, r.eoff, (ne + 1) * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&t, S.t4, S.t5);
-  *ms += t;
-  out->page_json = S.h_out.as<uint8_t>();
-  out->json_off = S.h_json_off.as<uint64_t>();
+  float size_ms = 0, emit_ms = 0;
+  cudaEventElapsedTime(&size_ms, S.t4, S.t5);
+  if ((rc = st_page_json_emit(c, S, r, nullptr, 0, hs, who, &out->page_json, &out->json_off, &emit_ms, launches))) return rc;
+  *ms += size_ms + emit_ms;
   return TGI_OK;
 }
 
@@ -5645,6 +5623,93 @@ void handoff_walkbacks(CrawlState& S, const tgi_state_span* spans, uint32_t n_sp
     }
   S.wb_picked = false;
   S.wb_n_ok = 0;
+}
+
+// the checks both SQL calls make, in order: rows_per_stmt, now_nsec, crawl_id, a live hand-off
+int sql_args(tgi_ctx* c, const CrawlState& S, uint32_t k, int32_t now_nsec, const char* crawl_id, uint32_t crawl_id_len,
+             const char* who) {
+  if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
+  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
+  if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
+  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  return TGI_OK;
+}
+
+// discovery_time: the clock in time.Local, rendered with its quotes into tb[0, *tl); a year outside [0, 9999] refuses
+int sql_clock(tgi_ctx* c, int64_t now_sec, int32_t now_nsec, const char* who, char (&tb)[48], uint32_t* tl) {
+  std::lock_guard<std::mutex> zg(c->cfg_mu);
+  *tl = (uint32_t)host_render_zone_time(tb, now_sec, now_nsec, c->zone, c->cfgdev.tz);
+  if (!*tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  return TGI_OK;
+}
+
+// The statements of q.p (kind0, k and rows set) over `threads` row threads: their texts on the host (one per kind and
+// row count, a kind's last statement maybe shorter), crawl_id and the clock tb[0, tl) uploaded, the params by the
+// two-pass writer (accepted() once the size pass has passed), and the texts, params and statement table read back into
+// h and hst.  Adds its device time and launches to out's.
+template <class Q, class Out, class F>
+int sql_render(tgi_ctx* c, CrawlState& S, Q& q, void (*size)(StDev, Q), void (*emit)(StDev, Q), uint64_t threads,
+               const char* crawl_id, uint32_t crawl_id_len, const char* tb, uint32_t tl, const char* who, F&& accepted,
+               HostBuf& h, HostBuf& hst, Out* out) {
+  StSqlPlan& p = q.p;
+  const uint32_t k = p.k;
+  uint64_t n_rows = 0;
+  std::string texts, t;
+  for (uint32_t i = 0; i < 3; i++) {
+    p.m[i] = (p.rows[i] + k - 1) / k;
+    p.n_stmts += p.m[i];
+    n_rows += p.rows[i];
+    const uint32_t rows[2] = {p.rows[i] >= k ? k : 0u, (uint32_t)(p.rows[i] % k)};
+    for (int j = 0; j < 2; j++) {
+      if (!rows[j]) continue;
+      edge_sql_text(p.kind0 + i, rows[j], t);
+      p.sql_off[2 * i + j] = texts.size();
+      p.sql_len[2 * i + j] = t.size();
+      texts += t;
+    }
+  }
+  cudaStream_t st = S.stream;
+  const size_t t_at = (crawl_id_len + 15) & ~(size_t)15;
+  CK(S.sql_in.ensure(t_at + 48));
+  CK(S.sql_size.ensure(n_rows * 4));
+  CK(S.sql_off.ensure((n_rows + 1) * 8));
+  CK(S.sql_stmts.ensure(p.n_stmts * sizeof(tgi_state_edge_stmt)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  std::vector<uint8_t> in(t_at + tl);
+  if (crawl_id_len) memcpy(in.data(), crawl_id, crawl_id_len);
+  if (tl) memcpy(in.data() + t_at, tb, tl);
+  if (!in.empty()) CK(cudaMemcpyAsync(S.sql_in.p, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  p.crawl = S.sql_in.as<uint8_t>();
+  p.crawl_len = crawl_id_len;
+  p.time = p.crawl + t_at;
+  p.time_len = tl;
+  p.size = S.sql_size.as<uint32_t>();
+  p.off = S.sql_off.as<uint64_t>();
+  p.sc = S.sc.as<uint64_t>();
+  p.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
+  p.base = texts.size();
+  const unsigned grid = sink_grid(c, std::max(threads, p.n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
+  uint32_t launches = 0;
+  uint64_t body = 0;
+  int rc;
+  if ((rc = st_rows_size(c, S, size, q, grid, p.size, n_rows, p.off, who, "a row", &body, launches))) return rc;
+  accepted();
+  CK(h.ensure(texts.size() + body));
+  CK(hst.ensure(p.n_stmts * sizeof(tgi_state_edge_stmt)));
+  if ((rc = st_rows_emit(c, S, emit, q, &p.out, S.sql_out, body, grid, launches))) return rc;
+  uint8_t* o = h.as<uint8_t>();
+  CK(cudaMemcpyAsync(o + texts.size(), S.sql_out.p, body, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(hst.p, S.sql_stmts.p, p.n_stmts * sizeof(tgi_state_edge_stmt), cudaMemcpyDeviceToHost, st));
+  memcpy(o, texts.data(), texts.size());  // beside the copies: another part of the buffer
+  CK(cudaStreamSynchronize(st));
+  out->n_stmts = p.n_stmts;
+  out->stmts = hst.as<tgi_state_edge_stmt>();
+  out->data = o;
+  out->data_len = texts.size() + body;
+  out->kernel_ms += st_rows_ms(S);
+  out->gpu_launches += launches;
+  return TGI_OK;
 }
 
 }  // namespace
@@ -5708,16 +5773,7 @@ int tgi_state_discover(tgi_ctx* c, int slot, const tgi_state_span* spans, uint32
   }
   // per span: first occurrences under Base's rules (none under Dapr's) and Dapr's urlCache test
   uint64_t n_surv = 0;
-  {
-    std::unique_lock<std::mutex> fg(c->fr_mu, std::defer_lock);
-    FrontierDev urls{};
-    if (dapr) {
-      fg.lock();
-      if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-      urls = c->sets[TGI_SET_URLS].dev;
-    }
-    if ((rc = st_survivors(c, S, S.cand.as<StCand>(), gd.coff + n_spans, bound, true, !dapr, urls, &n_surv, &ms, launches))) return rc;
-  }
+  if ((rc = st_survivors(c, S, S.cand.as<StCand>(), gd.coff + n_spans, bound, true, !dapr, dapr, &n_surv, &ms, launches))) return rc;
   float gather_ms = 0;
   cudaEventElapsedTime(&gather_ms, S.t0, S.t1);
   ms += gather_ms;
@@ -5765,16 +5821,7 @@ int tgi_state_next_layer(tgi_ctx* c, int64_t layer_depth, uint32_t flags, int64_
   uint32_t launches = 0;
   float ms = 0;
   uint64_t n_surv = 0;
-  {
-    std::unique_lock<std::mutex> fg(c->fr_mu, std::defer_lock);
-    FrontierDev urls{};
-    if (dapr) {
-      fg.lock();
-      if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
-      urls = c->sets[TGI_SET_URLS].dev;
-    }
-    if ((rc = st_survivors(c, S, S.pend.as<StCand>(), S.coff.as<uint64_t>(), m, false, true, urls, &n_surv, &ms, launches))) return rc;
-  }
+  if ((rc = st_survivors(c, S, S.pend.as<StCand>(), S.coff.as<uint64_t>(), m, false, true, dapr, &n_surv, &ms, launches))) return rc;
   const std::vector<DiscGroup> G(1, DiscGroup{layer_depth + 1, true, 0, n_surv});
   if ((rc = st_discover_apply(c, S, G, dapr, json, now_sec, now_nsec, max_pages, who, out, &ms, launches))) return rc;
   S.n_pend = 0;
@@ -5917,106 +5964,24 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
   cudaSetDevice(c->device);  // not st_init: that would end the hand-off
-  const uint32_t k = rows_per_stmt;
-  if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
-  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
-  if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
-  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off to render (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  int rc;
+  if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who))) return rc;
   const uint64_t nb = S.handoff_nb, ne = S.handoff_ne;
   char tb[48];
   uint32_t tl = 0;
-  if (ne) {
-    std::lock_guard<std::mutex> zg(c->cfg_mu);
-    tl = (uint32_t)host_render_zone_time(tb, now_sec, now_nsec, c->zone, c->cfgdev.tz);
-    if (!tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
-  }
+  if (ne && (rc = sql_clock(c, now_sec, now_nsec, who, tb, &tl))) return rc;
   memset(out, 0, sizeof *out);
   if (!nb) return TGI_OK;
-  // the statements: ceil(n / k) per kind, and the texts of their row counts (a kind's last statement may be shorter)
-  const uint64_t m[3] = {(nb + k - 1) / k, (ne + k - 1) / k, (nb + k - 1) / k};
-  const uint64_t n_stmts = m[0] + m[1] + m[2], n_rows = 2 * nb + ne;
   StSql q{};
-  std::string texts, t;
-  for (uint32_t kind = 0; kind < 3; kind++) {
-    const uint64_t n = kind == TGI_SQL_EDGE_INSERT ? ne : nb;
-    const uint32_t rows[2] = {n >= k ? k : 0u, (uint32_t)(n % k)};
-    for (int j = 0; j < 2; j++) {
-      if (!rows[j]) continue;
-      edge_sql_text(kind, rows[j], t);
-      q.sql_off[2 * kind + j] = texts.size();
-      q.sql_len[2 * kind + j] = t.size();
-      texts += t;
-    }
-  }
-  cudaStream_t st = S.stream;
-  const size_t t_at = (crawl_id_len + 15) & ~(size_t)15;
-  CK(S.sql_in.ensure(t_at + sizeof tb));
-  CK(S.sql_size.ensure(n_rows * 4));
-  CK(S.sql_off.ensure((n_rows + 1) * 8));
-  CK(S.sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
-  std::vector<uint8_t> in(t_at + tl);
-  if (crawl_id_len) memcpy(in.data(), crawl_id, crawl_id_len);
-  if (tl) memcpy(in.data() + t_at, tb, tl);
-  if (!in.empty()) CK(cudaMemcpyAsync(S.sql_in.p, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  q.p.kind0 = TGI_SQL_BATCH_INSERT;
+  q.p.k = rows_per_stmt;
+  q.p.rows[0] = q.p.rows[2] = nb;
+  q.p.rows[1] = ne;
   q.edges = S.edges.as<tgi_state_edge>();
   q.batches = S.ebatches.as<tgi_state_edge_batch>();
   q.spans = S.spans.as<tgi_state_span>();
-  q.ne = ne;
-  q.nb = nb;
-  q.n_rows = n_rows;
-  q.k = k;
-  q.crawl = S.sql_in.as<uint8_t>();
-  q.crawl_len = crawl_id_len;
-  q.time = q.crawl + t_at;
-  q.time_len = tl;
-  q.size = S.sql_size.as<uint32_t>();
-  q.off = S.sql_off.as<uint64_t>();
-  q.sc = S.sc.as<uint64_t>();
-  q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
-  q.n_stmts = n_stmts;
-  for (int j = 0; j < 3; j++) q.m[j] = m[j];
-  q.base = texts.size();
-  const StDev d = st_dev(S);
-  const unsigned grid = sink_grid(c, std::max(n_rows, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
-  uint32_t launches = 0;
-  int rc;
-  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-  CK(cudaEventRecord(S.t0, st));
-  st_sql_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, q.size, n_rows, q.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(S.t1, st));
-  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "tgi_state_edge_sql: a row renders to 4 GiB or more"); return TGI_E_CAPACITY; }
-  const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
-  CK(S.sql_out.ensure(body));
-  CK(S.h_sql.ensure(texts.size() + body));
-  CK(S.h_sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
-  q.out = S.sql_out.as<uint8_t>();
-  CK(cudaEventRecord(S.t2, st));
-  st_sql_emit_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
-  launches++;
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(S.t3, st));
-  uint8_t* h = S.h_sql.as<uint8_t>();
-  CK(cudaMemcpyAsync(h + texts.size(), S.sql_out.p, body, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(S.h_sql_stmts.p, S.sql_stmts.p, n_stmts * sizeof(tgi_state_edge_stmt), cudaMemcpyDeviceToHost, st));
-  memcpy(h, texts.data(), texts.size());  // beside the copies: another part of the buffer
-  CK(cudaStreamSynchronize(st));
-  float ms = 0, t2 = 0;
-  cudaEventElapsedTime(&ms, S.t0, S.t1);
-  cudaEventElapsedTime(&t2, S.t2, S.t3);
-  out->n_stmts = n_stmts;
-  out->stmts = S.h_sql_stmts.as<tgi_state_edge_stmt>();
-  out->data = h;
-  out->data_len = texts.size() + body;
-  out->kernel_ms = ms + t2;
-  out->gpu_launches = launches;
-  return TGI_OK;
+  return sql_render(c, S, q, st_sql_size_kernel, st_sql_emit_kernel, 2 * nb + ne, crawl_id, crawl_id_len, tb, tl, who, [] {},
+                    S.h_sql, S.h_sql_stmts, out);
 }
 
 // The forced walkbacks of the last hand-off.  The first call on a hand-off picks (a thread per edge-less span, a scan
@@ -6030,27 +5995,17 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
   cudaSetDevice(c->device);  // not st_init: that would end the hand-off
-  const uint32_t k = rows_per_stmt;
-  if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
-  if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
-  if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
-  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  int rc;
+  if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who))) return rc;
   const uint64_t n = S.wb_spans.size() / 2;
   if (!n) {  // every span has a batch: nothing to pick, no launch
     memset(out, 0, sizeof *out);
     return TGI_OK;
   }
   if (!S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
-  char tb[48];
-  uint32_t tl = 0;
-  {
-    std::lock_guard<std::mutex> zg(c->cfg_mu);
-    tl = (uint32_t)host_render_zone_time(tb, now_sec, now_nsec, c->zone, c->cfgdev.tz);
-  }
   cudaStream_t st = S.stream;
   uint32_t launches = 0;
   float ms = 0;
-  int rc;
   uint64_t n_ok = S.wb_n_ok;
   if (!S.wb_picked) {  // the hand-off's picks: made here, kept only once the call is accepted
     CK(S.wb_in.ensure(n * 8));
@@ -6085,7 +6040,9 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
     cudaEventElapsedTime(&ms, S.t0, S.t1);
     n_ok = S.h_sc.as<uint64_t>()[ST_SC_ROWS];
   }
-  if (n_ok && !tl) { set_err(c, "%s: the clock's local year is outside [0, 9999] (json.Marshal fails)", who); return TGI_E_ARG; }
+  char tb[48];
+  uint32_t tl = 0;
+  if (n_ok && (rc = sql_clock(c, now_sec, now_nsec, who, tb, &tl))) return rc;
   auto accept = [&]() {  // the picks are kept once the call is accepted: a refused first call picks the same again
     if (S.wb_picked) return;
     S.wb_picked = true;
@@ -6101,85 +6058,16 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
     accept();
     return TGI_OK;
   }
-  // the statements: ceil(n_ok / k) per kind, and the texts of their row counts
-  const uint64_t m = (n_ok + k - 1) / k, n_stmts = 2 * m, n_rows = 2 * n_ok;
   StWalkSql q{};
-  std::string texts, t;
-  for (uint32_t kind = 0; kind < 2; kind++) {
-    const uint32_t rows[2] = {n_ok >= k ? k : 0u, (uint32_t)(n_ok % k)};
-    for (int j = 0; j < 2; j++) {
-      if (!rows[j]) continue;
-      edge_sql_text(TGI_SQL_PAGE_BUFFER_INSERT + kind, rows[j], t);
-      q.sql_off[2 * kind + j] = texts.size();
-      q.sql_len[2 * kind + j] = t.size();
-      texts += t;
-    }
-  }
-  const size_t t_at = (crawl_id_len + 15) & ~(size_t)15;
-  CK(S.sql_in.ensure(t_at + sizeof tb));
-  CK(S.sql_size.ensure(n_rows * 4));
-  CK(S.sql_off.ensure((n_rows + 1) * 8));
-  CK(S.sql_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
-  CK(S.sc.ensure(ST_SC_COUNT * 8));
-  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
-  std::vector<uint8_t> in(t_at + tl);
-  if (crawl_id_len) memcpy(in.data(), crawl_id, crawl_id_len);
-  memcpy(in.data() + t_at, tb, tl);
-  CK(cudaMemcpyAsync(S.sql_in.p, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  q.p.kind0 = TGI_SQL_PAGE_BUFFER_INSERT;
+  q.p.k = rows_per_stmt;
+  q.p.rows[0] = q.p.rows[1] = n_ok;
   q.spans = S.wb_in.as<uint32_t>();
   q.wb = S.wb.as<tgi_state_walkback_span>();
   q.rank = S.wb_rank.as<uint64_t>();
   q.n = n;
-  q.n_ok = n_ok;
-  q.k = k;
-  q.crawl = S.sql_in.as<uint8_t>();
-  q.crawl_len = crawl_id_len;
-  q.time = q.crawl + t_at;
-  q.time_len = tl;
-  q.size = S.sql_size.as<uint32_t>();
-  q.off = S.sql_off.as<uint64_t>();
-  q.sc = S.sc.as<uint64_t>();
-  q.stmts = S.sql_stmts.as<tgi_state_edge_stmt>();
-  q.m = m;
-  q.base = texts.size();
-  const StDev d = st_dev(S);
-  const unsigned grid = sink_grid(c, std::max(2 * n, n_stmts), ST_THREADS, 4);  // one pass: SMs x 1024 rows
-  CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
-  CK(cudaEventRecord(S.t0, st));
-  st_walk_size_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, q.size, n_rows, q.off, S.sc.as<uint64_t>() + ST_SC_BYTES, launches))) return rc;
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(S.t1, st));
-  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (S.h_sc.as<uint64_t>()[ST_SC_BIG]) { set_err(c, "%s: a row renders to 4 GiB or more", who); return TGI_E_CAPACITY; }
-  accept();
-  const uint64_t body = S.h_sc.as<uint64_t>()[ST_SC_BYTES];
-  CK(S.sql_out.ensure(body));
-  CK(S.h_wb_sql.ensure(texts.size() + body));
-  CK(S.h_wb_stmts.ensure(n_stmts * sizeof(tgi_state_edge_stmt)));
-  q.out = S.sql_out.as<uint8_t>();
-  CK(cudaEventRecord(S.t2, st));
-  st_walk_emit_kernel<<<grid, ST_THREADS, 0, st>>>(d, q);
-  launches++;
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(S.t3, st));
-  uint8_t* h = S.h_wb_sql.as<uint8_t>();
-  CK(cudaMemcpyAsync(h + texts.size(), S.sql_out.p, body, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(S.h_wb_stmts.p, S.sql_stmts.p, n_stmts * sizeof(tgi_state_edge_stmt), cudaMemcpyDeviceToHost, st));
-  memcpy(h, texts.data(), texts.size());  // beside the copies: another part of the buffer
-  CK(cudaStreamSynchronize(st));
-  float t1 = 0, t2 = 0;
-  cudaEventElapsedTime(&t1, S.t0, S.t1);
-  cudaEventElapsedTime(&t2, S.t2, S.t3);
-  out->n_stmts = n_stmts;
-  out->stmts = S.h_wb_stmts.as<tgi_state_edge_stmt>();
-  out->data = h;
-  out->data_len = texts.size() + body;
-  out->kernel_ms = ms + t1 + t2;
-  out->gpu_launches = launches;
-  return TGI_OK;
+  return sql_render(c, S, q, st_walk_size_kernel, st_walk_emit_kernel, 2 * n, crawl_id, crawl_id_len, tb, tl, who, accept,
+                    S.h_wb_sql, S.h_wb_stmts, out);
 }
 
 }  // extern "C"

@@ -950,10 +950,7 @@ class Engine:
         self._check(lib().tgi_state_edge_sql(self.h, crawl_id, len(crawl_id), now[0], now[1], rows_per_stmt, C.byref(out)))
         self.state_sql_ms = float(out.kernel_ms)
         self.state_sql_launches = int(out.gpu_launches)
-        st = _view(out.stmts, int(out.n_stmts), abi.STATE_EDGE_STMT)
-        data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
-        return [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
-                for k, r, so, sl, po, pl in st.tolist()]
+        return self._st_stmts(out)
 
     def state_walkback(self, crawl_id: bytes, now=(0, 0), rows_per_stmt: int = 1) -> tuple:
         """the forced walkbacks of the last state_pending_edges (nothing but it, state_edge_sql and this since among the
@@ -970,10 +967,15 @@ class Engine:
         walkbacks = [{"span": int(w["span"]), "status": int(w["status"]), "draws": int(w["draws"]),
                       "url": bytes(w["url"][:int(w["url_len"])]), "page_id": bytes(w["page_id"]),
                       "sequence_id": bytes(w["sequence_id"])} for w in wb]
+        return walkbacks, self._st_stmts(out)
+
+    @staticmethod
+    def _st_stmts(out) -> list:
+        """the statement table of a state_edge_sql or state_walkback result: [(kind, rows, sql, params)]"""
         st = _view(out.stmts, int(out.n_stmts), abi.STATE_EDGE_STMT)
         data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
-        return walkbacks, [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
-                           for k, r, so, sl, po, pl in st.tolist()]
+        return [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])
+                for k, r, so, sl, po, pl in st.tolist()]
 
     # --- frontier -------------------------------------------------------------------------------
     def frontier_insert(self, keys32: np.ndarray) -> np.ndarray:
