@@ -1,7 +1,7 @@
 // kernels.cuh — __global__ kernels of the ingest engine (sm_90a).  See DESIGN.md §4 for the data layout and the
 // roofline bookkeeping.  All of it is integer/byte work:
 //   tg_chan_size / tg_chan_emit            per-channel constant strings (once per batch, tiny)
-//   tg_parse / tg_ent_map / tg_parse_ent   status + link extraction (split by code footprint): tg_parse scans 32
+//   tg_ent_map / tg_parse / tg_parse_ent   status + link extraction (split by code footprint): tg_parse scans 32
 //                                          records' texts per warp as one packed stream, the other two take one warp
 //                                          per record with entities
 //   tg_size_lane                           JSONL line length, one LANE per record (+ the warp for the message text)
@@ -128,6 +128,10 @@ struct ParseOut {
   int* err;
 };
 
+// link_count of a record with entities between tg_parse_kernel and tg_parse_ent_kernel: its reserved slots (< 2^20), with
+// this bit if tg_parse_kernel mapped its entities (tg_ent_map_kernel skips it)
+constexpr uint32_t LC_MAPPED = 1u << 31;
+
 DEVI TgRecView load_rec_view(const TgBatchDev& b, uint64_t r) {
   TgRecView v;
   const tgi_tg_rec* rec = &b.recs[r];
@@ -147,21 +151,19 @@ DEVI TgRecView load_rec_view(const TgBatchDev& b, uint64_t r) {
   return v;
 }
 
-// One record.  ENTITIES == false: the record has no entities, so the whole UTF-16 offset machinery
-// (warp_utf16_to_bytes, the exact UTF-8 path) is compiled out.  MEASURE (JSONL runs of the multi-kernel pipeline): the
-// link count also measures the message text, and linelen[r] carries its escaped length to tg_size_lane_body (0: not
-// measured, the size pass measures it itself).
-template <bool ENTITIES, bool MEASURE = false>
+// One record (the page kernel).  ENTITIES == false: the record has no entities, so the whole UTF-16 offset machinery
+// (warp_utf16_to_bytes, the exact UTF-8 path) is compiled out.
+template <bool ENTITIES>
 DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOut& o, uint64_t r, TgRecView v) {
   const int l = lane_id();
-  uint32_t status = TGI_ST_EMITTED, nlinks = 0, lstart = 0, text_esc = 0;
+  uint32_t status = TGI_ST_EMITTED, nlinks = 0, lstart = 0;
   if ((cfg.flags & TGI_CFG_HAS_MIN_POST_DATE) && (int64_t)v.rec->date < cfg.min_post_date) {
     status = TGI_ST_SKIPPED;  // tdutils.go:419-421
   } else if (v.flags & TGI_RF_PANIC) {
     status = TGI_ST_FAILED;
   } else {
     if (!ENTITIES) v.e1 = v.e0;
-    uint32_t ub = warp_link_upper_bound<MEASURE>(v, b.ents, text_esc);
+    uint32_t ub = warp_link_upper_bound(v, b.ents);
     if (ub >= (1u << 20)) {  // seq packing of the frontier needs ordinal < 2^20 (SEQ_ORD_BITS)
       if (l == 0) atomicOr(o.err, ERR_TOO_MANY_LINKS);
       ub = 0;
@@ -180,7 +182,7 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
         ls.name_bytes = 0;
         ls.self = b.chan_strs + ch->str_off + ch->title_len;
         ls.self_len = ch->name_len;
-        bool ok = warp_extract_links(v, b.ents, b.aux, o.ent_range, ls);
+        bool ok = warp_extract_links(v, b.ents, b.aux, o.ent_range, ls, true);
         nlinks = ls.count;
         if (!ok) {
           status = TGI_ST_FAILED;
@@ -191,16 +193,28 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
   }
   if (l == 0) {
     o.status[r] = (uint8_t)status;
-    o.linelen[r] = MEASURE && status == TGI_ST_EMITTED ? text_esc : 0u;  // the size pass overwrites the emitted ones
+    o.linelen[r] = 0u;  // the size pass measures the texts and overwrites the emitted ones
     o.link_start[r] = lstart;
     o.link_count[r] = nlinks;
   }
 }
 
+// The packed chunk stream of a group of 32 records (tg_parse_kernel, tg_ent_map_kernel): incl = the chunks of the lane's
+// record and the records below it.  Returns the owner of chunk base + lane = the number of records whose chunks end at
+// or before it (5 steps of a binary search on the scan, clamped to the pass so that it fits 32 bits).
+DEVI int packed_chunk_owner(uint64_t incl, uint64_t base) {
+  const uint32_t end = incl <= base ? 0u : (uint32_t)min(incl - base, (uint64_t)32);
+  int ow = 0;
+#pragma unroll
+  for (int s = 16; s; s >>= 1)
+    if (__shfl_sync(FULL, end, ow + s - 1) <= (uint32_t)lane_id()) ow += s;
+  return ow;
+}
+
 // The parse step is split by instruction footprint (the SM's instruction caches hold only a few thousand instructions):
-// tg_parse_kernel = status + links of the records WITHOUT entities (three quarters of the corpus; small code),
-// tg_ent_map_kernel = UTF-16 entity offsets -> byte ranges, tg_parse_ent_kernel = links of the records with
-// entities (lanes pick them out of groups of 32), tg_size_lane_kernel = line lengths.  Fusing them was tried twice
+// tg_ent_map_kernel = UTF-16 entity offsets -> byte ranges, tg_parse_kernel = status, link bounds and text measurement
+// of every record and the links of the records WITHOUT entities (small code), tg_parse_ent_kernel = links of the
+// records with entities (lanes pick them out of groups of 32), tg_size_lane_kernel = line lengths.  Fusing them was tried twice
 // (one parse kernel; parse + size in ONE pass over the text, fewer instructions in all): both fused kernels stalled on
 // instruction fetch and were slower than the split ones.
 //
@@ -208,26 +222,31 @@ DEVI void parse_one_record(const TgBatchDev& b, const CfgDev& cfg, const ParseOu
 // stream: text j's 16-byte chunks (cut from the text's start) follow text j - 1's in one chunk index space, and the
 // warp walks that space 32 chunks per pass, each lane on the chunk of whichever record holds it.  A warp per record
 // left most lanes idle (the median text fills about 20 of a strip's 32 lanes, a caption 7) and paid a full warp
-// iteration for every record without text to scan.  Per chunk the lane does what warp_count_tme_esc does per strip
-// lane (tme16, measure16); the totals go to the owning lane through shared-memory atomics on the (rare) nonzero values.
-// Only the records with a "t.me/" hit then take the warp-wide extraction, one after the other.
+// iteration for every record without text to scan.  Per chunk the lane counts "t.me/" (tme16) and measures the bytes
+// (measure16); the totals go to the owning lane through shared-memory atomics on the (rare) nonzero values.  Only the
+// records without entities and with a "t.me/" hit then take the warp-wide extraction, one after the other; a record
+// with entities gets its arena slots (the bound) and leaves the extraction to tg_parse_ent_kernel, which keeps the
+// entity code out of this kernel's instruction footprint.
 template <bool MEASURE>
 DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_flags, const ParseOut& o) {
-  __shared__ uint32_t acc[WARPS_PER_CTA][MEASURE ? 3 : 1][32];  // per record: "t.me/" hits, escape extras, not clean
+  // per record: "t.me/" hits, a byte >= 0x80, escape extras, not clean
+  __shared__ uint32_t acc[WARPS_PER_CTA][MEASURE ? 4 : 2][32];
   const int wid = threadIdx.x >> 5, l = lane_id();
   const uint32_t SP = 0x20202020u;
   uint32_t* a_cnt = acc[wid][0];
-  uint32_t* a_extra = acc[wid][MEASURE ? 1 : 0];
-  uint32_t* a_bad = acc[wid][MEASURE ? 2 : 0];
+  uint32_t* a_hi = acc[wid][1];
+  uint32_t* a_extra = acc[wid][MEASURE ? 2 : 0];
+  uint32_t* a_bad = acc[wid][MEASURE ? 3 : 0];
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
   for (uint64_t g = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; g < ngroups; g += nwarps) {
     const uint64_t r = g * 32 + l;
-    const bool mine = r < b.n && b.ent_off[r + 1] == b.ent_off[r];  // the others: tg_parse_ent_kernel
-    uint32_t status = TGI_ST_EMITTED, len = 0;                          // len: bytes of text to scan
+    uint32_t status = TGI_ST_EMITTED, len = 0, nents = 0;  // len: bytes of text to scan; nents: its link-kind entities
+    bool ents = false;                                       // the record has entities (tg_parse_ent_kernel extracts)
     const uint8_t* text = b.strs;
-    if (mine) {
+    if (r < b.n) {
       const tgi_tg_rec* rec = &b.recs[r];
-      const uint32_t fl = rec->flags;
+      const uint32_t fl = rec->flags, e0 = b.ent_off[r], e1 = b.ent_off[r + 1];
+      ents = e1 != e0;
       if ((cfg.flags & TGI_CFG_HAS_MIN_POST_DATE) && (int64_t)rec->date < cfg.min_post_date) {
         status = TGI_ST_SKIPPED;  // tdutils.go:419-421
       } else if (fl & TGI_RF_PANIC) {
@@ -235,6 +254,7 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
       } else if (ct_carries_links(rec->content_type) && (fl & TGI_RF_HAS_TEXT)) {
         text += rec->str_off;
         len = rec->text_len;
+        for (uint32_t e = e0; e < e1; e++) nents += b.ents[e].type != TGI_ENT_OTHER;
       }
     }
     // the group's chunks: this record's are [incl - nch, incl) (64 bits: 32 texts of up to 4 GiB)
@@ -246,18 +266,12 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
       if (l >= d) incl += t;
     }
     const uint64_t total = __shfl_sync(FULL, incl, 31), first = incl - nch;
-    a_cnt[l] = 0;
+    a_cnt[l] = a_hi[l] = 0;
     if (MEASURE) a_extra[l] = a_bad[l] = 0;
     __syncwarp();
     uint32_t carry = SP;  // the last 4 bytes of lane 31's chunk in the previous pass
     for (uint64_t base = 0; base < total; base += 32) {
-      // owner of chunk base + l = the number of records whose chunks end at or before it (5 steps of a binary search on
-      // the scan, clamped to the pass so that it fits 32 bits)
-      const uint32_t end = incl <= base ? 0u : (uint32_t)min(incl - base, (uint64_t)32);
-      int ow = 0;
-#pragma unroll
-      for (int s = 16; s; s >>= 1)
-        if (__shfl_sync(FULL, end, ow + s - 1) <= (uint32_t)l) ow += s;
+      const int ow = packed_chunk_owner(incl, base);
       const uint8_t* s = (const uint8_t*)__shfl_sync(FULL, (unsigned long long)text, ow);
       const uint64_t j = base + l - __shfl_sync(FULL, first, ow);  // chunk of that record
       const int64_t n = __shfl_sync(FULL, len, ow), p0 = (int64_t)(16 * j), rem = n - p0;
@@ -278,11 +292,12 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
         if (rem <= 16 && (w.w & 0x80808000u)) bad |= utf8_unclean4(w.w, SP);
       }
       if (cnt) atomicAdd(&a_cnt[ow], cnt);
+      if ((w.x | w.y | w.z | w.w) & 0x80808080u) a_hi[ow] = 1u;
       if (MEASURE && extra) atomicAdd(&a_extra[ow], extra);
       if (MEASURE && bad) a_bad[ow] = 1u;
     }
     __syncwarp();
-    uint32_t ub = a_cnt[l], text_esc = 0;
+    uint32_t ub = a_cnt[l] + nents, text_esc = 0;  // the link bound: "t.me/" hits + entities of the three kinds
     if (MEASURE) text_esc = a_bad[l] ? 0u : len + a_extra[l];
     if (ub >= (1u << 20)) {  // seq packing of the frontier needs ordinal < 2^20 (SEQ_ORD_BITS)
       atomicOr(o.err, ERR_TOO_MANY_LINKS);
@@ -299,7 +314,7 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
     const bool fits = (uint64_t)gstart + ub_incl <= o.arena_cap;
     if (ub && !fits) atomicOr(o.err, ERR_ARENA_OVERFLOW);
     uint32_t nlinks = 0;
-    for (uint32_t todo = __ballot_sync(FULL, ub && fits); todo; todo &= todo - 1) {
+    for (uint32_t todo = __ballot_sync(FULL, ub && fits && !ents); todo; todo &= todo - 1) {
       const int k = __ffs(todo) - 1;
       const tgi_tg_chan* ch = &b.chans[b.recs[g * 32 + k].chan_idx];
       LinkSink ls;
@@ -314,11 +329,25 @@ DEVI void tg_parse_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_fla
                               TGI_SRC_PLAINTEXT, true);
       if (l == k) nlinks = ls.count;
     }
-    if (mine) {
+    // a record with entities keeps its reservation until tg_parse_ent_kernel.  An ASCII text has its entities mapped
+    // here (a byte is a rune and a UTF-16 unit: utf16OffsetToBytes' loop meets unit i at byte i); tg_ent_map_kernel
+    // maps the others
+    const bool mapped = ents && ub && fits && a_hi[l] == 0;
+    if (mapped) {
+      for (uint32_t e = b.ent_off[r], e1 = b.ent_off[r + 1]; e < e1; e++) {
+        const tgi_entity en = b.ents[e];
+        if (en.type != TGI_ENT_MENTION && en.type != TGI_ENT_URL) continue;
+        const int32_t off = en.offset, stop = (int32_t)((uint32_t)en.offset + (uint32_t)en.length), n = (int32_t)len;
+        const bool s_in = off >= 0 && off < n;
+        o.ent_range[e] = stop >= 0 && stop < n ? make_int2(s_in && off <= stop ? off : -1, stop)
+                                               : (s_in ? make_int2(off, n) : make_int2(0, 0));
+      }
+    }
+    if (r < b.n) {
       o.status[r] = (uint8_t)status;
       o.linelen[r] = MEASURE && status == TGI_ST_EMITTED ? text_esc : 0u;  // the size pass overwrites the emitted ones
       o.link_start[r] = lstart;
-      o.link_count[r] = nlinks;
+      o.link_count[r] = ents && fits && ub ? ub | (mapped ? LC_MAPPED : 0u) : nlinks;
     }
   }
 }
@@ -326,38 +355,164 @@ template <bool MEASURE>
 __global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_kernel(TgBatchDev b, CfgDev cfg, uint32_t run_flags, ParseOut o) {
   tg_parse_body<MEASURE>(b, cfg, run_flags, o);
 }
+// utf16OffsetToBytes for every mention / url entity, 32 records per warp over one packed chunk stream as in
+// tg_parse_kernel (a warp per record walked a non-ASCII text from its start once per entity).  A clean text (unclean16)
+// decodes rune by rune the way Go's does, so a 16-byte chunk holds utf16_units16 units, and a scan over the pass (cut
+// at the records' first chunks) plus the record's units of the earlier passes places every rune start.  The lane on a
+// chunk looks for its record's entity offsets and ends in it and writes the byte index of the (one) rune start it finds
+// to ent_range[e].x / .y; after the walk the owning lane applies the end of utf16OffsetToBytes to them.  A record whose
+// text is not clean takes warp_map_entities, a warp each, which is exact on any bytes.
 DEVI void tg_ent_map_body(const TgBatchDev& b, const ParseOut& o) {
   const int wid = threadIdx.x >> 5, l = lane_id();
+  const uint32_t SP = 0x20202020u;
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
   for (uint64_t g = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; g < ngroups; g += nwarps) {
-    const uint64_t rl = g * 32 + l;
-    uint32_t todo = __ballot_sync(FULL, rl < b.n && b.ent_off[rl + 1] != b.ent_off[rl]);
-    while (todo) {
-      const uint64_t r = g * 32 + (uint32_t)(__ffs(todo) - 1);
-      todo &= todo - 1;
-      warp_map_entities(load_rec_view(b, r), b.ents, o.ent_range);
+    const uint64_t r = g * 32 + l;
+    uint32_t len = 0, e0 = 0, e1 = 0;  // [e0, e1): the entities to map (none: the record takes no part)
+    uint32_t t_lo = 0x7FFFFFFFu, t_hi = 0;  // the unit positions looked for (int32 >= 0) lie in [t_lo, t_hi]
+    bool any = false;
+    const uint8_t* text = b.strs;
+    if (r < b.n && o.status[r] == TGI_ST_EMITTED) {  // the records tg_parse_ent_kernel extracts, unless mapped
+      e0 = b.ent_off[r];
+      e1 = b.ent_off[r + 1];
+      const tgi_tg_rec* rec = &b.recs[r];
+      const uint32_t lc = o.link_count[r];
+      if (e1 != e0 && lc != 0 && !(lc & LC_MAPPED) && ct_carries_links(rec->content_type) && (rec->flags & TGI_RF_HAS_TEXT)) {
+        for (uint32_t e = e0; e < e1; e++) {
+          const tgi_entity en = b.ents[e];
+          if (en.type == TGI_ENT_MENTION || en.type == TGI_ENT_URL) {
+            o.ent_range[e] = make_int2(-1, -1);  // no rune start found yet at the offset / at the end
+            any = true;
+            const int32_t stop = (int32_t)((uint32_t)en.offset + (uint32_t)en.length);
+            if (en.offset >= 0) t_lo = min(t_lo, (uint32_t)en.offset), t_hi = max(t_hi, (uint32_t)en.offset);
+            if (stop >= 0) t_lo = min(t_lo, (uint32_t)stop), t_hi = max(t_hi, (uint32_t)stop);
+          }
+        }
+      }
+      if (any) {
+        text += rec->str_off;
+        len = rec->text_len;
+      } else {
+        e1 = e0;
+      }
     }
+    // a rune of a clean text has at most 3 bytes per unit, so the one at unit t starts before byte 3t + 1: the walk
+    // stops there (the chunks past it hold no position looked for, and Go's result does not depend on their bytes)
+    const uint64_t nch = min(((uint64_t)len + 15u) >> 4, t_lo <= t_hi ? (3 * (uint64_t)t_hi + 16u) >> 4 : 0u);
+    uint64_t incl = nch;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint64_t t = __shfl_up_sync(FULL, incl, d);
+      if (l >= d) incl += t;
+    }
+    const uint64_t total = __shfl_sync(FULL, incl, 31), first = incl - nch;
+    uint32_t units = 0;     // the record's units in the chunks of the passes so far
+    bool unclean = false;   // the record's text is not clean
+    uint32_t carry = SP;    // the last 4 bytes of lane 31's chunk in the previous pass
+    __syncwarp();
+    for (uint64_t base = 0; base < total; base += 32) {
+      const int ow = packed_chunk_owner(incl, base);
+      const uint8_t* s = (const uint8_t*)__shfl_sync(FULL, (unsigned long long)text, ow);
+      const uint64_t j = base + l - __shfl_sync(FULL, first, ow);  // chunk of that record
+      const int64_t n = __shfl_sync(FULL, len, ow), p0 = (int64_t)(16 * j), rem = n - p0;
+      const bool act = base + l < total;
+      uint4 w = make_uint4(SP, SP, SP, SP);
+      uint32_t u = 0, bad = 0;
+      if (act) {
+        w = ld16_unaligned(s + p0);
+        if (rem < 16) w = make_uint4(blank_from(w.x, rem), blank_from(w.y, rem - 4), blank_from(w.z, rem - 8), blank_from(w.w, rem - 12));
+        u = utf16_units16(w, rem < 16 ? (uint32_t)rem : 16u);
+      }
+      const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
+      const uint32_t pw = j == 0 ? SP : (l == 0 ? carry : below);
+      carry = __shfl_sync(FULL, w.w, 31);
+      if (act) {
+        unclean16(w, pw, bad);
+        if (rem <= 16 && (w.w & 0x80808000u)) bad |= utf8_unclean4(w.w, SP);
+      }
+      // the segmented scan: this lane's record holds the pass's lanes [lo, hi)
+      const uint32_t ui = warp_incl_scan(u), badm = __ballot_sync(FULL, bad != 0);
+      const uint32_t hi = incl <= base ? 0u : (uint32_t)min(incl - base, (uint64_t)32);
+      const uint32_t lo = first <= base ? 0u : (uint32_t)min(first - base, (uint64_t)32);
+      const uint32_t top = __shfl_sync(FULL, ui, hi ? hi - 1 : 0), bot = __shfl_sync(FULL, ui, lo ? lo - 1 : 0);
+      const uint32_t seg0 = lo ? bot : 0u;  // units of the pass in front of the record's chunks
+      const uint32_t pos = __shfl_sync(FULL, units, ow) + ui - u - __shfl_sync(FULL, seg0, ow);  // units before the chunk
+      const uint32_t me0 = __shfl_sync(FULL, e0, ow), me1 = __shfl_sync(FULL, e1, ow);
+      const uint32_t mlo = __shfl_sync(FULL, t_lo, ow), mhi = __shfl_sync(FULL, t_hi, ow);
+      if (hi > lo) {
+        units += top - seg0;
+        unclean = unclean || (badm & ((hi == 32 ? ~0u : (1u << hi) - 1u) & ~((1u << lo) - 1u)));
+      }
+      if (act && pos <= mhi && mlo < pos + u) {  // a position looked for can lie in this chunk
+        for (uint32_t e = me0; e < me1; e++) {
+          const tgi_entity en = b.ents[e];
+          if (en.type != TGI_ENT_MENTION && en.type != TGI_ENT_URL) continue;
+          // Go compares int32 unit positions: the end wraps as an int32 sum, a negative offset is never reached
+          const uint32_t t0 = (uint32_t)en.offset - pos, t1 = (uint32_t)en.offset + (uint32_t)en.length - pos;
+          if (t0 < u) {
+            const int k = rune_at_unit16(w, t0);
+            if (k >= 0) o.ent_range[e].x = (int)(p0 + k);
+          }
+          if (t1 < u) {
+            const int k = rune_at_unit16(w, t1);
+            if (k >= 0) o.ent_range[e].y = (int)(p0 + k);
+          }
+        }
+      }
+    }
+    __syncwarp();
+    if (!unclean) {  // the end of utf16OffsetToBytes
+      for (uint32_t e = e0; e < e1; e++) {
+        const uint32_t t = b.ents[e].type;
+        if (t != TGI_ENT_MENTION && t != TGI_ENT_URL) continue;
+        const int2 h = o.ent_range[e];
+        int2 rg;
+        if (h.y >= 0) rg = make_int2(h.x >= 0 && h.x <= h.y ? h.x : -1, h.y);  // a start past the end is never reached
+        else rg = h.x >= 0 ? make_int2(h.x, (int)len) : make_int2(0, 0);
+        o.ent_range[e] = rg;
+      }
+    }
+    for (uint32_t todo = __ballot_sync(FULL, unclean && e1 != e0); todo; todo &= todo - 1)
+      warp_map_entities(load_rec_view(b, g * 32 + (uint32_t)(__ffs(todo) - 1)), b.ents, o.ent_range);
   }
 }
 __global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_ent_map_kernel(TgBatchDev b, ParseOut o) { tg_ent_map_body(b, o); }
-template <bool MEASURE>
-DEVI void tg_parse_ent_body(const TgBatchDev& b, const CfgDev& cfg, uint32_t run_flags, const ParseOut& o) {
+// The links of the records with entities that tg_parse_kernel left: their slots are reserved (link_count) and their
+// entities mapped (ent_range), so the warp only extracts, record after record.  The plaintext scan is skipped when the
+// reservation is the entities alone: the count found no "t.me/" in the text.
+DEVI void tg_parse_ent_body(const TgBatchDev& b, const ParseOut& o) {
   const int wid = threadIdx.x >> 5, l = lane_id();
   const uint64_t ngroups = (b.n + 31) / 32, nwarps = (uint64_t)gridDim.x * WARPS_PER_CTA;
   for (uint64_t g = (uint64_t)blockIdx.x * WARPS_PER_CTA + wid; g < ngroups; g += nwarps) {
     const uint64_t rl = g * 32 + l;
-    uint32_t todo = __ballot_sync(FULL, rl < b.n && b.ent_off[rl + 1] != b.ent_off[rl]);
+    uint32_t todo = __ballot_sync(FULL, rl < b.n && b.ent_off[rl + 1] != b.ent_off[rl] && o.status[rl] == TGI_ST_EMITTED &&
+                                            o.link_count[rl] != 0);
     while (todo) {
       const uint64_t r = g * 32 + (uint32_t)(__ffs(todo) - 1);
       todo &= todo - 1;
-      parse_one_record<true, MEASURE>(b, cfg, o, r, load_rec_view(b, r));
+      const TgRecView v = load_rec_view(b, r);
+      const tgi_tg_chan* ch = &b.chans[v.rec->chan_idx];
+      LinkSink ls;
+      ls.out = o.arena + o.link_start[r];
+      ls.cap = o.link_count[r] & ~LC_MAPPED;
+      ls.count = 0;
+      ls.name_bytes = 0;
+      ls.self = b.chan_strs + ch->str_off + ch->title_len;
+      ls.self_len = ch->name_len;
+      uint32_t c = 0;
+      for (uint32_t e = v.e0 + l; e < v.e1; e += 32) c += b.ents[e].type != TGI_ENT_OTHER;
+      const bool ok = warp_extract_links(v, b.ents, b.aux, o.ent_range, ls, ls.cap != warp_sum(c));
+      if (l == 0) {
+        if (!ok) {  // the reference panics: the same result as parse_one_record's
+          o.status[r] = TGI_ST_FAILED;
+          o.linelen[r] = 0;
+        }
+        o.link_count[r] = ok ? ls.count : 0u;
+      }
     }
   }
 }
-template <bool MEASURE>
-__global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_ent_kernel(TgBatchDev b, CfgDev cfg, uint32_t run_flags, ParseOut o) {
-  tg_parse_ent_body<MEASURE>(b, cfg, run_flags, o);
-}
+__global__ void __launch_bounds__(CTA_THREADS, LB_PARSE) tg_parse_ent_kernel(TgBatchDev b, ParseOut o) { tg_parse_ent_body(b, o); }
 
 // The same sizes, 32 records per warp: every lane sizes the small pieces of its own record (numbers,
 // handle / media strings, comments, reactions, outlinks); the description, the one long string, is measured by the
@@ -387,7 +542,7 @@ DEVI void tg_size_lane_body(const TgBatchDev& b, const CfgDev& cfg, const ParseO
     uint32_t tot = 0;
     bool warp_comments = false, warp_map = false;
     const uint32_t r0 = b.react_off[r], nr = b.react_off[r + 1] - r0;
-    // the parse's measurement (parse_one_record), != 0 only for a text of >= 1 byte: then alt != text, and d.desc == text
+    // the parse's measurement (tg_parse_kernel), != 0 only for a text of >= 1 byte: then alt != text, and d.desc == text
     // says the description is the message text
     const uint32_t text_esc = active ? o.linelen[r] : 0u;
     const bool measured = text_esc != 0 && d.desc == a.v.text;

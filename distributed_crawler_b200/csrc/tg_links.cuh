@@ -146,12 +146,12 @@ DEVI uint32_t warp_count_tme(const uint8_t* s, int64_t n) {
   return warp_sum(cnt);
 }
 
-// 16 bytes of a text w (bytes past its end read as ' ') with the 4 bytes in front of them pw (' ' at its start), measured
-// for the JSONL line: bad |= the bits that make the text not clean (utf8_unclean4), extra += what JSON escaping adds.
+// 16 bytes of a text w (bytes past its end read as ' ') with the 4 bytes in front of them pw (' ' at its start): unclean16
+// ORs into bad the bits that make the text not clean (utf8_unclean4); measure16 also adds to extra what JSON escaping adds.
 // The bytes are classified once: ASCII needs no clean test, bytes without a 3- or 4-byte lead (Latin, Cyrillic, Arabic)
 // take utf8_unclean2, the rest utf8_unclean4 word by word; the escape count looks only at the bytes the special-byte
 // test (esc_special4) flags.
-DEVI void measure16(const uint4 w, uint32_t pw, uint32_t& bad, uint32_t& extra) {
+DEVI void unclean16(const uint4 w, uint32_t pw, uint32_t& bad) {
   if ((w.x | w.y | w.z | w.w | pw) & 0x80808080u) {  // not ASCII
     // pw's first byte governs no byte of w: a lead there covers at most pw's other three
     if ((utf8_lead3(w.x) | utf8_lead3(w.y) | utf8_lead3(w.z) | utf8_lead3(w.w) | utf8_lead3(pw & 0xFFFFFF00u)) == 0) {
@@ -166,6 +166,9 @@ DEVI void measure16(const uint4 w, uint32_t pw, uint32_t& bad, uint32_t& extra) 
       }
     }
   }
+}
+DEVI void measure16(const uint4 w, uint32_t pw, uint32_t& bad, uint32_t& extra) {
+  unclean16(w, pw, bad);
   // bit 8j + k: byte j of word k may need escaping (line breaks, quotes, '<', '&': few lanes have one)
   uint32_t sp = (esc_special4(w.x) >> 7) | (esc_special4(w.y) >> 6) | (esc_special4(w.z) >> 5) | (esc_special4(w.w) >> 4);
   while (sp) {
@@ -174,33 +177,6 @@ DEVI void measure16(const uint4 w, uint32_t pw, uint32_t& bad, uint32_t& extra) 
     const uint32_t x = k == 0 ? w.x : (k == 1 ? w.y : (k == 2 ? w.z : w.w));
     extra += ascii_esc_len((x >> (b & ~7)) & 0xFFu) - 1u;  // a flagged byte is ASCII; the text copies the others as they are
   }
-}
-
-// The same count, and the text measured from the same 16 bytes per lane (JSONL runs): esc_len = its JSON-escaped length
-// if it is clean (utf8_unclean4), 0 if not (or if n == 0).  The lane's 4 bytes in front come from the lane below, or
-// for lane 0 from the previous strip's last lane.
-DEVI uint32_t warp_count_tme_esc(const uint8_t* s, int64_t n, uint32_t& esc_len) {
-  const int l = lane_id();
-  const uint32_t SP = 0x20202020u;
-  uint32_t cnt = 0, extra = 0, bad = 0, tail = SP;  // tail: the last 4 bytes of the previous strip
-  for (int64_t base = 0; base < n; base += 512) {
-    const int64_t p0 = base + 16 * l, rem = n - p0;
-    uint4 w = make_uint4(SP, SP, SP, SP);
-    if (rem > 0) {
-      w = ld16_unaligned(s + p0);
-      cnt += __popc(tme16(s, p0, n, w));
-      if (rem < 16) w = make_uint4(blank_from(w.x, rem), blank_from(w.y, rem - 4), blank_from(w.z, rem - 8), blank_from(w.w, rem - 12));
-    }
-    const uint32_t below = __shfl_up_sync(FULL, w.w, 1);
-    const uint32_t pw = l == 0 ? tail : below;
-    tail = __shfl_sync(FULL, w.w, 31);
-    measure16(w, pw, bad, extra);
-  }
-  // a text that ends with its last strip: a sequence open at the end (one needs a high bit in tail's last three bytes)
-  if (tail & 0x80808000u) bad |= utf8_unclean4(tail, SP);
-  const uint32_t e = (uint32_t)n + warp_sum(extra);
-  esc_len = __any_sync(FULL, bad != 0) ? 0u : e;
-  return warp_sum(cnt);
 }
 
 // channelLinkRegex over s[0..n).  all == false: FindStringSubmatch (first match only, reserved names
@@ -315,6 +291,36 @@ __device__ __noinline__ void warp_utf16_to_bytes(const uint8_t* s, int64_t n, in
   }
 }
 
+// UTF-16 units of 16 bytes w of a clean text, nvalid of them in the text: bytes - continuation bytes + 4-byte leads
+// (each a surrogate pair)
+DEVI uint32_t utf16_units16(const uint4 w, uint32_t nvalid) {
+  const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+  uint32_t u = nvalid;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {  // bytes past the text are ' ': neither kind
+    const uint32_t x = ws[k];
+    u += __popc(x & (x << 1) & (x << 2) & (x << 3) & 0x80808080u) - __popc(x & ~(x << 1) & 0x80808080u);
+  }
+  return u;
+}
+
+// index of the rune start of w (16 bytes of a clean text) that sits t UTF-16 units after w's first byte, -1 if t falls
+// on the second unit of a surrogate pair.  t < utf16_units16(w, ...).
+DEVI int rune_at_unit16(uint4 w, uint32_t t) {
+  uint32_t pos = 0;
+#pragma unroll 1
+  for (int k = 0; k < 16; k++) {
+    const uint32_t x = w.x & 0xFFu;
+    if ((x & 0xC0u) != 0x80u) {
+      if (pos == t) return k;
+      pos += 1u + (x >= 0xF0u);
+      if (pos > t) return -1;
+    }
+    w = make_uint4(__funnelshift_r(w.x, w.y, 8), __funnelshift_r(w.y, w.z, 8), __funnelshift_r(w.z, w.w, 8), w.w >> 8);
+  }
+  return -1;
+}
+
 struct TgRecView {  // decoded view of one record, warp-uniform
   const tgi_tg_rec* rec;
   const uint8_t *text, *alt, *media, *handle;
@@ -328,20 +334,17 @@ DEVI bool ct_carries_links(uint32_t ct) {  // extractFormattedTextFromMessage td
          ct == TGI_CT_ANIMATION || ct == TGI_CT_AUDIO || ct == TGI_CT_VOICE_NOTE;
 }
 
-// upper bound on the number of links of this record (entities of the three kinds + "t.me/" hits).  MEASURE: text_esc =
-// the text's escaped length if the count found it clean, else 0 (warp_count_tme_esc); 0 for a record it does not scan.
-template <bool MEASURE>
-DEVI uint32_t warp_link_upper_bound(const TgRecView& v, const tgi_entity* ents, uint32_t& text_esc) {
-  text_esc = 0;
+// upper bound on the number of links of this record (entities of the three kinds + "t.me/" hits)
+DEVI uint32_t warp_link_upper_bound(const TgRecView& v, const tgi_entity* ents) {
   if (!ct_carries_links(v.ct) || !(v.flags & TGI_RF_HAS_TEXT)) return 0;
   uint32_t c = 0;
   for (uint32_t e = v.e0 + lane_id(); e < v.e1; e += 32) c += ents[e].type != TGI_ENT_OTHER;
-  return warp_sum(c) + (MEASURE ? warp_count_tme_esc(v.text, v.text_len, text_esc) : warp_count_tme(v.text, v.text_len));
+  return warp_sum(c) + warp_count_tme(v.text, v.text_len);
 }
 
 // utf16OffsetToBytes for every mention / url entity of the record -> ranges[e - v.e0... absolute e] = (start, end)
-// (tg_ent_map_kernel; a kernel of its own so that the UTF-8 machinery and the link scan never share an
-// instruction cache)
+// (the page kernel, and tg_ent_map_kernel for a text that is not clean; never in a kernel with the link scan, so that
+// the UTF-8 machinery and the link scan never share an instruction cache)
 DEVI void warp_map_entities(const TgRecView& v, const tgi_entity* ents, int2* ranges) {
   if (!ct_carries_links(v.ct) || !(v.flags & TGI_RF_HAS_TEXT)) return;
   int64_t ascii_prefix = -1;  // computed when the first offset has to be mapped
@@ -363,8 +366,10 @@ DEVI void warp_map_entities(const TgRecView& v, const tgi_entity* ents, int2* ra
   }
 }
 
-// returns false if the reference would panic (record FAILED).  ranges: warp_map_entities' output
-DEVI bool warp_extract_links(const TgRecView& v, const tgi_entity* ents, const uint8_t* aux, const int2* ranges, LinkSink& ls) {
+// returns false if the reference would panic (record FAILED).  ranges: warp_map_entities' output.  plaintext == false:
+// the text holds no "t.me/", so the plaintext scan would find nothing.
+DEVI bool warp_extract_links(const TgRecView& v, const tgi_entity* ents, const uint8_t* aux, const int2* ranges, LinkSink& ls,
+                             bool plaintext) {
   if (!ct_carries_links(v.ct) || !(v.flags & TGI_RF_HAS_TEXT)) return true;
   for (uint32_t e = v.e0; e < v.e1; e++) {
     tgi_entity en = ents[e];
@@ -380,7 +385,7 @@ DEVI bool warp_extract_links(const TgRecView& v, const tgi_entity* ents, const u
       }
     }
   }
-  warp_scan_channel_links(ls, v.text, v.text_len, TGI_SRC_PLAINTEXT, true);
+  if (plaintext) warp_scan_channel_links(ls, v.text, v.text_len, TGI_SRC_PLAINTEXT, true);
   return true;
 }
 

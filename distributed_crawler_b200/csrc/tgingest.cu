@@ -1396,15 +1396,17 @@ int run_tg(tgi_ctx* c, Slot& s, uint32_t flags, tgi_result* out) {
       // JSONL: the link count measures the message texts as well (the size pass then skips the clean ones); runs without
       // JSONL take the instances without that code
       const bool measure = want_json && size_text_in_parse();
-      if (s.n_ents) {  // records with entities first: status + links (two kernels by instruction footprint)
-        tg_ent_map_kernel<<<ge, CTA_THREADS, 0, st>>>(b, po);
-        if (measure) tg_parse_ent_kernel<true><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
-        else tg_parse_ent_kernel<false><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
-        launches += 2;
-      }
-      if (measure) tg_parse_kernel<true><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);  // records without entities
+      // status, link bounds, the entity offsets of ASCII texts and the links of the records without entities; then the
+      // entity offsets of the other texts; then the links of the records with entities (three kernels by instruction
+      // footprint)
+      if (measure) tg_parse_kernel<true><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
       else tg_parse_kernel<false><<<ge, CTA_THREADS, 0, st>>>(b, cfg, flags, po);
       launches++;
+      if (s.n_ents) {
+        tg_ent_map_kernel<<<ge, CTA_THREADS, 0, st>>>(b, po);
+        tg_parse_ent_kernel<<<ge, CTA_THREADS, 0, st>>>(b, po);
+        launches += 2;
+      }
       if (want_json) {
         tg_size_lane_kernel<<<ge, CTA_THREADS, 0, st>>>(b, cfg, po);
         launches++;
