@@ -277,6 +277,37 @@ class StateWalkbackC(C.Structure):  # tgi_state_walkback_t
                 ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+# tgi_state_validator_walkback: its three more statement kinds (CompletePendingBatch, FlushBatchStats' upsert and
+# delete), the validation classes of a claimed edge, the input rows (ClaimWalkbackBatch's batch and edges, strings as
+# (offset, length) into one blob) and each batch's outcome
+SQL_BATCH_COMPLETE, SQL_STATS_UPSERT, SQL_EDGES_DELETE = 5, 6, 7
+EDGE_CLASS_VALID, EDGE_CLASS_NOT_CHANNEL, EDGE_CLASS_INVALID, EDGE_CLASS_DUPLICATE, EDGE_CLASS_OTHER = 0, 1, 2, 3, 4
+EDGE_CLASS_OF = {b"valid": EDGE_CLASS_VALID, b"not_channel": EDGE_CLASS_NOT_CHANNEL, b"invalid": EDGE_CLASS_INVALID,
+                 b"duplicate": EDGE_CLASS_DUPLICATE}  # validation_status by exact match; anything else is OTHER
+CLAIMED_BATCH_STRINGS = ("batch_id", "crawl_id", "source_channel", "source_page_id", "sequence_id")  # TGI_CB_*
+VW_NO_EDGE = 0xFFFFFFFF
+CLAIMED_BATCH = np.dtype([("str_off", "<u8", 5), ("str_len", "<u4", 5), ("reserved", "<u4"),
+                          ("source_depth", "<i8")])  # tgi_claimed_batch
+CLAIMED_EDGE = np.dtype([("str_off", "<u8", 2), ("str_len", "<u4", 2), ("cls", "<u4"),
+                         ("reserved", "<u4")])  # tgi_claimed_edge
+STATE_VALIDATOR_BATCH = np.dtype([("status", "<u4"), ("walkback", "<u4"), ("rnd", "<i4"), ("draws", "<u4"),
+                                  ("n_valid", "<u4"), ("forward_edge", "<u4"), ("url_len", "<u4"), ("reserved", "<u4"),
+                                  ("url", "u1", 32), ("page_id", "S36"),
+                                  ("sequence_id", "S36")])  # tgi_state_validator_batch
+assert (CLAIMED_BATCH.itemsize, CLAIMED_EDGE.itemsize, STATE_VALIDATOR_BATCH.itemsize) == (72, 32, 136)
+
+
+class ClaimedBatchesC(C.Structure):  # tgi_claimed_batches
+    _fields_ = [("n_batches", C.c_uint32), ("reserved", C.c_uint32), ("batches", C.c_void_p), ("edge_off", C.c_void_p),
+                ("edges", C.c_void_p), ("n_edges", C.c_uint64), ("strs", C.c_void_p), ("strs_len", C.c_uint64)]
+
+
+class StateValidatorWalkbackC(C.Structure):  # tgi_state_validator_walkback_t
+    _fields_ = [("n_batches", C.c_uint32), ("reserved", C.c_uint32), ("batches", C.c_void_p),
+                ("n_stmts", C.c_uint64), ("stmts", C.c_void_p), ("data", C.c_void_p), ("data_len", C.c_uint64),
+                ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
 # tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
 SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3

@@ -1028,11 +1028,12 @@ __global__ void st_edge_emit_kernel(StEdges e) {
 
 // ---- tandem hand-off SQL (state/daprstate.go:3643-3678, 3896-3941): the params of every binding call ----------------
 // A SQL call's statements: kind i (TGI_SQL_* kind0 + i) has rows[i] rows, numbered after the kinds before it; a
-// statement holds k consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names,
+// statement holds k[i] consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names,
 // URLs), which the sequential escaper handles without the warp's 128-byte strips idling most lanes.
+constexpr uint32_t ST_SQL_KINDS = 5;  // the most kinds one call renders
 struct StSqlPlan {
-  uint32_t kind0, k;                    // the first kind, rows per statement
-  uint64_t rows[3], m[3];               // rows and statements of each kind
+  uint32_t kind0, k[ST_SQL_KINDS];      // the first kind, rows per statement of each kind
+  uint64_t rows[ST_SQL_KINDS], m[ST_SQL_KINDS];  // rows and statements of each kind (0 past the call's kinds)
   uint64_t n_stmts;
   uint32_t crawl_len, time_len;
   const uint8_t* crawl;                 // crawl_id as given, then discovery_time rendered with its quotes
@@ -1042,7 +1043,8 @@ struct StSqlPlan {
   uint64_t* sc;                         // ST_SC_*: ST_SC_BIG
   uint8_t* out;
   tgi_state_edge_stmt* stmts;           // [n_stmts]
-  uint64_t sql_off[6], sql_len[6];      // the texts of kind i: [2i] k rows, [2i+1] the kind's last, shorter statement
+  uint64_t sql_off[2 * ST_SQL_KINDS], sql_len[2 * ST_SQL_KINDS];  // kind i's texts: [2i] k[i] rows, [2i+1] its last,
+                                                                  // shorter statement
   uint64_t base;                        // the params' offset in the output
 };
 
@@ -1083,9 +1085,9 @@ DEVI void st_sql_stmts(const StSqlPlan& q) {
       j -= q.m[kind];
       first += q.rows[kind];
     }
-    first += j * q.k;
-    const uint32_t rows = (uint32_t)min((uint64_t)q.k, q.rows[kind] - j * q.k);
-    const uint32_t t = 2 * kind + (rows != q.k);
+    first += j * q.k[kind];
+    const uint32_t rows = (uint32_t)min((uint64_t)q.k[kind], q.rows[kind] - j * q.k[kind]);
+    const uint32_t t = 2 * kind + (rows != q.k[kind]);
     tgi_state_edge_stmt& st = q.stmts[s];
     st.kind = q.kind0 + kind;
     st.rows = rows;
@@ -1110,7 +1112,7 @@ DEVI StLen<EMIT> st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t*
   const uint64_t nb = q.p.rows[0], ne = q.p.rows[1];
   const uint32_t kind = r < nb ? 0u : r < nb + ne ? 1u : 2u;
   const uint64_t i = kind == 0 ? r : kind == 1 ? r - nb : r - nb - ne;  // the row within its kind
-  w.open(i, q.p.k);
+  w.open(i, q.p.k[kind]);
   const tgi_state_edge* e = kind == 1 ? q.edges + i : nullptr;
   const tgi_state_edge_batch& b = q.batches[e ? e->batch : (uint32_t)i];
   w.str(b.batch_id, 36);
@@ -1145,7 +1147,7 @@ DEVI StLen<EMIT> st_sql_row(const StDev& d, const StSql& q, uint64_t r, uint8_t*
       w.lit(",\"pending\"", 10);
     }
   }
-  w.close(i, q.p.k, kind == 1 ? ne : nb);
+  w.close(i, q.p.k[kind], kind == 1 ? ne : nb);
   return w.o;
 }
 
@@ -1176,48 +1178,73 @@ struct StWalk {
   uint32_t* ok;                    // [n] 1: TGI_WALK_OK
 };
 
-// one span's pickWalkbackChannel(sm, owner.URL, nil) over the set's keys in first-occurrence order (Random() is
-// keys[rand.Intn(len(keys))], state/datamodels.go:152-162), and its two ids
+// A walker's draw stream: word 2j and 2j + 1 are Philox block (ctr_lo, ctr_hi, domain, j)'s x0 | x1 << 32 and
+// x2 | x3 << 32 under the id key
+struct StDraws {
+  uint64_t seed, ctr;
+  uint32_t domain;
+  uint64_t next = 0;
+  uint32_t c[4];
+  DEVI uint64_t word() {
+    if (!(next & 1)) {
+      c[0] = (uint32_t)ctr, c[1] = (uint32_t)(ctr >> 32), c[2] = domain, c[3] = (uint32_t)(next >> 1);
+      philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+    }
+    return (next++ & 1) ? (c[2] | (uint64_t)c[3] << 32) : (c[0] | (uint64_t)c[1] << 32);
+  }
+  // Lemire's multiply-and-reject: exactly uniform on [0, N), N > 0, as rand.IntN
+  DEVI uint64_t below(uint64_t N) {
+    uint64_t x = word(), l = x * N;
+    if (l < N) {
+      const uint64_t t = (0 - N) % N;
+      while (l < t) l = (x = word()) * N;
+    }
+    return __umul64hi(x, N);
+  }
+};
+
+// key[0, klen) == s[0, n), byte for byte
+DEVI bool st_key_eq(const Key32& key, uint32_t klen, const uint8_t* s, uint32_t n) {
+  bool eq = klen == n;
+  for (uint32_t k = 0; eq && k < n; k++) eq = ((key.w[k >> 2] >> (8 * (k & 3))) & 0xFF) == s[k];
+  return eq;
+}
+
+// pickWalkbackChannel(sm, source, exclude) (crawl/runner.go:120-139) over the set's keys in first-occurrence order
+// (Random() is keys[rand.Intn(len(keys))], state/datamodels.go:152-162): up to 10 draws from r, a draw equal to
+// source[0, sl) or excluded(key, klen) retried.  Returns TGI_WALK_*; key / klen hold the pick when TGI_WALK_OK, else 0.
+template <class X>
+DEVI uint32_t st_pick_walkback(StDraws& r, const FrontierDev& disc, const uint8_t* src, uint32_t sl, X&& excluded,
+                               Key32& key, uint32_t& klen, uint32_t& draws) {
+  const uint64_t N = disc.table ? *disc.count : 0;
+  uint32_t status = N ? TGI_WALK_EXHAUSTED : TGI_WALK_EMPTY;
+  key = Key32{};
+  klen = draws = 0;
+  while (N && draws < TGI_WALK_MAX_DRAWS) {
+    draws++;
+    key = load_key(disc.pool + 32 * r.below(N));
+    klen = 32;
+    while (klen && !((key.w[(klen - 1) >> 2] >> (8 * ((klen - 1) & 3))) & 0xFF)) klen--;
+    if (!st_key_eq(key, klen, src, sl) && !excluded(key, klen)) {  // url == sourceURL || exclude[url]
+      status = TGI_WALK_OK;
+      break;
+    }
+  }
+  if (status != TGI_WALK_OK) key = Key32{}, klen = 0;
+  return status;
+}
+
+// one span's pickWalkbackChannel(sm, owner.URL, nil) and its two ids
 __global__ void st_walk_pick_kernel(StDev d, StWalk w) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < w.n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t wi = w.w0 + i, N = w.disc.table ? *w.disc.count : 0;
+    const uint64_t wi = w.w0 + i;
     uint32_t ul;
     const uint8_t* u = st_str(d, d.pages[w.spans[2 * i + 1]], TGI_PS_URL, ul);
     tgi_state_walkback_span& o = w.out[i];
-    Key32 key{};
-    uint32_t status = TGI_WALK_EMPTY, draws = 0, klen = 0;
-    if (N) {
-      // the draw stream: word 2j and 2j + 1 are Philox block (w_lo, w_hi, 2, j)'s x0 | x1 << 32 and x2 | x3 << 32
-      uint32_t c[4];
-      uint64_t next = 0;
-      auto word = [&]() -> uint64_t {
-        if (!(next & 1)) {
-          c[0] = (uint32_t)wi, c[1] = (uint32_t)(wi >> 32), c[2] = 2u, c[3] = (uint32_t)(next >> 1);
-          philox4x32_10(c, (uint32_t)w.seed, (uint32_t)(w.seed >> 32));
-        }
-        return (next++ & 1) ? (c[2] | (uint64_t)c[3] << 32) : (c[0] | (uint64_t)c[1] << 32);
-      };
-      status = TGI_WALK_EXHAUSTED;
-      while (draws < TGI_WALK_MAX_DRAWS) {
-        draws++;
-        // Lemire's multiply-and-reject: exactly uniform on [0, N)
-        uint64_t x = word(), l = x * N;
-        if (l < N) {
-          const uint64_t t = (0 - N) % N;
-          while (l < t) l = (x = word()) * N;
-        }
-        key = load_key(w.disc.pool + 32 * __umul64hi(x, N));
-        klen = 32;
-        while (klen && !((key.w[(klen - 1) >> 2] >> (8 * ((klen - 1) & 3))) & 0xFF)) klen--;
-        bool self = klen == ul;  // url == sourceURL, byte for byte
-        for (uint32_t k = 0; self && k < ul; k++) self = ((key.w[k >> 2] >> (8 * (k & 3))) & 0xFF) == u[k];
-        if (!self) {
-          status = TGI_WALK_OK;
-          break;
-        }
-      }
-    }
-    if (status != TGI_WALK_OK) key = Key32{}, klen = 0;
+    Key32 key;
+    uint32_t draws, klen;
+    StDraws r{w.seed, wi, 2u};
+    const uint32_t status = st_pick_walkback(r, w.disc, u, ul, [](const Key32&, uint32_t) { return false; }, key, klen, draws);
     o.span = w.spans[2 * i];
     o.status = status;
     o.draws = draws;
@@ -1244,7 +1271,7 @@ DEVI StLen<EMIT> st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, 
   StSqlRow<EMIT> w{dst, 0};
   const tgi_state_walkback_span& b = q.wb[i];
   const tgi_state_page& p = d.pages[q.spans[2 * i + 1]];  // the owner
-  w.open(j, q.p.k);
+  w.open(j, q.p.k[kind]);
   if (kind == 0) {  // AddPageToPageBuffer (daprstate.go:3620-3633)
     w.str(b.page_id, 36);
     w.lit(",", 1);
@@ -1268,7 +1295,7 @@ DEVI StLen<EMIT> st_walk_row(const StDev& d, const StWalkSql& q, uint32_t kind, 
     w.lit(",", 1);
     w.field(d, p, TGI_PS_SEQ);
   }
-  w.close(j, q.p.k, q.p.rows[0]);
+  w.close(j, q.p.k[kind], q.p.rows[0]);
   return w.o;
 }
 
@@ -1291,6 +1318,210 @@ __global__ void st_walk_emit_kernel(StDev d, StWalkSql q) {
     const uint64_t i = t - kind * q.n, j = q.rank[i];
     if (q.rank[i + 1] > j) st_walk_row<true>(d, q, kind, i, j, q.p.out + q.p.off[kind * q.p.rows[0] + j]);
   }
+  st_sql_stmts(q.p);
+}
+
+// ---- validator walkback (crawl/validator.go:360-489): processWalkbackBatch of every claimed batch -------------------
+struct StVw {
+  const tgi_claimed_batch* b;      // [n] the claimed batches, their edges and strings as uploaded
+  const uint64_t* eoff;            // [n+1]
+  const tgi_claimed_edge* e;
+  const uint8_t* s;
+  uint64_t n;
+  int64_t rate;                    // cfg.WalkbackRate
+  FrontierDev disc;                // TGI_SET_DISCOVERED (table == nullptr: never allocated)
+  uint64_t seed, v0;               // the id key, and the counter of the first batch
+  tgi_state_validator_batch* out;  // [n]
+  uint32_t* vlist;                 // [n_edges] batch i's valid edges (index within it) at [eoff[i], + n_valid)
+  uint32_t* tlist;                 // [n_edges] the first edge of each of its distinct source types at [eoff[i], + d)
+  uint32_t* cnt;                   // [3n] per batch: 1 when TGI_WALK_OK; its edge rows; its stats rows
+};
+
+// FlushBatchStats' key of an edge: its source_type, "unknown" when empty (daprstate.go:4140-4143)
+DEVI const uint8_t* st_vw_type(const StVw& v, const tgi_claimed_edge& e, uint32_t& n) {
+  n = e.str_len[TGI_CE_SOURCE_TYPE];
+  if (!n) {
+    n = 7;
+    return (const uint8_t*)"unknown";
+  }
+  return v.s + e.str_off[TGI_CE_SOURCE_TYPE];
+}
+DEVI bool st_bytes_eq(const uint8_t* a, uint32_t an, const uint8_t* b, uint32_t bn) {
+  bool eq = an == bn;
+  for (uint32_t k = 0; eq && k < an; k++) eq = a[k] == b[k];
+  return eq;
+}
+
+// one batch: its valid edges and distinct source types, the decision, the pick, the two ids and its row counts
+__global__ void st_vw_pick_kernel(StVw v) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < v.n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t e0 = v.eoff[i], m = v.eoff[i + 1] - e0, vi = v.v0 + i;
+    const tgi_claimed_edge* E = v.e + e0;
+    uint32_t nv = 0, nt = 0;
+    for (uint32_t q = 0; q < (uint32_t)m; q++) {
+      if (E[q].cls == TGI_EDGE_CLASS_VALID) v.vlist[e0 + nv++] = q;
+      uint32_t tl, ul;
+      const uint8_t* t = st_vw_type(v, E[q], tl);
+      bool first = true;
+      for (uint32_t r = 0; first && r < nt; r++) first = !st_bytes_eq(t, tl, st_vw_type(v, E[v.tlist[e0 + r]], ul), ul);
+      if (first) v.tlist[e0 + nt++] = q;
+    }
+    StDraws r{v.seed, vi, 5u};
+    const tgi_claimed_batch& b = v.b[i];
+    int32_t rnd = -1;
+    bool walkback = true;
+    if (nv) {
+      rnd = (int32_t)r.below(100) + 1;
+      walkback = v.rate >= rnd;
+    }
+    Key32 key{};
+    uint32_t status = TGI_WALK_OK, draws = 0, klen = 0, fwd = TGI_VW_NO_EDGE;
+    if (walkback) {
+      const uint32_t* vl = v.vlist + e0;
+      auto excluded = [&](const Key32& k, uint32_t kl) {  // exclude[url]: the batch's valid channels
+        for (uint32_t x = 0; x < nv; x++) {
+          const tgi_claimed_edge& c = E[vl[x]];
+          if (st_key_eq(k, kl, v.s + c.str_off[TGI_CE_DESTINATION], c.str_len[TGI_CE_DESTINATION])) return true;
+        }
+        return false;
+      };
+      status = st_pick_walkback(r, v.disc, v.s + b.str_off[TGI_CB_SOURCE_CHANNEL], b.str_len[TGI_CB_SOURCE_CHANNEL],
+                                excluded, key, klen, draws);
+    } else {
+      fwd = v.vlist[e0 + r.below(nv)];
+    }
+    tgi_state_validator_batch& o = v.out[i];
+    o.status = status;
+    o.walkback = walkback;
+    o.rnd = rnd;
+    o.draws = draws;
+    o.n_valid = nv;
+    o.forward_edge = fwd;
+    o.url_len = klen;
+    o.reserved = 0;
+    store_key(o.url, key);
+    st_uuid(v.seed, vi, 6u, o.page_id);
+    st_uuid(v.seed, vi, 7u, o.sequence_id);
+    const bool ok = status == TGI_WALK_OK;
+    v.cnt[i] = ok;
+    v.cnt[v.n + i] = ok ? 1 + nv - !walkback : 0;  // the primary, then the valid channels not followed
+    v.cnt[2 * v.n + i] = ok ? nt : 0;
+  }
+}
+
+// The SQL of the OK batches: rows of page_buffer, edge_records, complete, stats upsert, delete.  Row j of a kind
+// belongs to the batch whose rank range holds it: rank (one row per OK batch), erank or srank (scans of StVw::cnt).
+struct StVwSql {
+  StSqlPlan p;                     // rows {n_ok, edge rows, n_ok, stats rows, n_ok} from TGI_SQL_PAGE_BUFFER_INSERT
+  StVw v;
+  const uint64_t* rank;            // [3 (n+1)]: the scans of StVw::cnt's three parts
+};
+
+// the last batch i with rank[i] <= j: the batch of row j
+DEVI uint64_t st_vw_batch(const uint64_t* rank, uint64_t n, uint64_t j) {
+  uint64_t a = 0, b = n - 1;
+  while (a < b) {
+    const uint64_t mid = (a + b + 1) >> 1;
+    if (rank[mid] <= j) a = mid;
+    else b = mid - 1;
+  }
+  return a;
+}
+
+template <bool EMIT>
+DEVI StLen<EMIT> st_vw_row(const StVwSql& q, uint64_t r, uint8_t* dst) {
+  uint32_t kind = 0;
+  uint64_t j = r;
+  while (j >= q.p.rows[kind]) j -= q.p.rows[kind++];
+  const StVw& v = q.v;
+  const uint64_t* rank = q.rank + (kind == 1 ? 1 : kind == 3 ? 2 : 0) * (v.n + 1);
+  const uint64_t i = st_vw_batch(rank, v.n, j), x = j - rank[i];  // the batch, and the row within its rows of the kind
+  const tgi_claimed_batch& b = v.b[i];
+  const tgi_state_validator_batch& o = v.out[i];
+  const tgi_claimed_edge* E = v.e + v.eoff[i];
+  StSqlRow<EMIT> w{dst, 0};
+  auto bstr = [&](int f) { w.str(v.s + b.str_off[f], b.str_len[f]); };
+  auto crawl = [&]() {  // the batch's CrawlID, else the configured one (daprstate.go:3181-3183, 3623-3626)
+    if (b.str_len[TGI_CB_CRAWL_ID]) bstr(TGI_CB_CRAWL_ID);
+    else w.str(q.p.crawl, q.p.crawl_len);
+  };
+  auto edge = [&](uint32_t y) { w.str(v.s + E[y].str_off[TGI_CE_DESTINATION], E[y].str_len[TGI_CE_DESTINATION]); };
+  auto url = [&]() {  // nextURL
+    if (o.walkback) w.str(o.url, o.url_len);
+    else edge(o.forward_edge);
+  };
+  w.open(j, q.p.k[kind]);
+  if (kind == 0) {  // AddPageToPageBuffer (daprstate.go:3620-3633) of validator.go:430-438's page
+    w.str(o.page_id, 36);
+    w.lit(",", 1);
+    bstr(TGI_CB_SOURCE_PAGE_ID);
+    w.lit(",", 1);
+    w.num((int64_t)((uint64_t)b.source_depth + 1));  // SourceDepth + 1 wraps as Go's int
+    w.lit(",", 1);
+    url();
+    w.lit(",", 1);
+    crawl();
+    w.lit(",", 1);
+    if (o.walkback) w.str(o.sequence_id, 36);
+    else bstr(TGI_CB_SEQUENCE_ID);
+  } else if (kind == 1) {  // SaveEdgeRecords (:3176-3184) of the primary edge, then the skipped ones (validator.go:446-473)
+    if (x == 0) {
+      url();
+    } else {  // the valid channels in edge order without the followed one
+      const uint32_t* vl = v.vlist + v.eoff[i];
+      const uint32_t y = (uint32_t)x - 1;
+      edge(vl[y] < o.forward_edge ? vl[y] : vl[y + 1]);  // a walkback's forward_edge is past every edge
+    }
+    w.lit(",", 1);
+    bstr(TGI_CB_SOURCE_CHANNEL);
+    if (x) w.lit(",false,true,", 12);
+    else if (o.walkback) w.lit(",true,false,", 12);
+    else w.lit(",false,false,", 13);
+    w.lit(q.p.time, q.p.time_len);
+    w.lit(",", 1);
+    crawl();
+    w.lit(",", 1);
+    bstr(TGI_CB_SEQUENCE_ID);
+  } else if (kind == 3) {  // FlushBatchStats' upsert of one source_type (daprstate.go:4137-4166)
+    bstr(TGI_CB_CRAWL_ID);
+    w.lit(",", 1);
+    uint32_t tl, ul;
+    const uint8_t* t = st_vw_type(v, E[v.tlist[v.eoff[i] + x]], tl);
+    w.str(t, tl);
+    long long c[5] = {0, 0, 0, 0, 0};  // total, valid, not_channel, invalid, duplicate
+    const uint32_t m = (uint32_t)(v.eoff[i + 1] - v.eoff[i]);
+    for (uint32_t e = 0; e < m; e++)
+      if (st_bytes_eq(t, tl, st_vw_type(v, E[e], ul), ul)) {
+        c[0]++;
+#pragma unroll
+        for (uint32_t f = 0; f < 4; f++) c[1 + f] += E[e].cls == f;  // the switch's four cases; OTHER is in total only
+      }
+#pragma unroll
+    for (int f = 0; f < 5; f++) {
+      w.lit(",", 1);
+      w.num(c[f]);
+    }
+  } else {  // CompletePendingBatch (:4125-4130), FlushBatchStats' delete (:4170-4174)
+    bstr(TGI_CB_BATCH_ID);
+  }
+  w.close(j, q.p.k[kind], q.p.rows[kind]);
+  return w.o;
+}
+
+__global__ void st_vw_size_kernel(StDev, StVwSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3] + q.p.rows[4];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_vw_row<false>(q, r, nullptr);
+    q.p.size[r] = (uint32_t)sz;
+    st_flag_big(q.p.sc, sz);
+  }
+}
+
+// the rows at their scanned offsets, then the statement table
+__global__ void st_vw_emit_kernel(StDev, StVwSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3] + q.p.rows[4];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    st_vw_row<true>(q, r, q.p.out + q.p.off[r]);
   st_sql_stmts(q.p);
 }
 

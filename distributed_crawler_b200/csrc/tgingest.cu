@@ -263,6 +263,11 @@ struct CrawlState {
   uint64_t wb_n_ok = 0, walk_next = 0;
   DevBuf wb_in, wb, wb_ok, wb_rank;
   HostBuf h_wb, h_wb_sql, h_wb_stmts;
+  // validator walkback (tgi_state_validator_walkback): the counter of claimed batches handled, the uploaded batches,
+  // the per-batch outcomes, lists, counts and their scans, and the pinned outputs
+  uint64_t vw_next = 0;
+  DevBuf vw_b, vw_eoff, vw_e, vw_s, vw_out, vw_list, vw_cnt, vw_rank;
+  HostBuf h_vw, h_vw_sql, h_vw_stmts;
   // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
   // device and its staging, and the pinned outputs
   DevBuf rset;
@@ -5570,11 +5575,11 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
 }
 
 // The SQL text of a statement of `rows` rows (TGI_SQL_*): for one row the literal of CreatePendingBatch,
-// InsertPendingEdge, ClosePendingBatch, AddPageToPageBuffer or SaveEdgeRecords (state/daprstate.go:3897, 3915, 3935,
-// 3620, 3167); for more the VALUES tuple repeated with the placeholders numbered on, or the close's WHERE batch_id IN
-// (...)
+// InsertPendingEdge, ClosePendingBatch, AddPageToPageBuffer, SaveEdgeRecords, CompletePendingBatch or FlushBatchStats'
+// upsert and delete (state/daprstate.go:3897, 3915, 3935, 3620, 3167, 4126, 4163, 4170); for more the VALUES tuple
+// repeated with the placeholders numbered on, or WHERE batch_id IN (...).  The upsert always has one row.
 void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
-  static const char* const head[5] = {
+  static const char* const head[8] = {
       "INSERT INTO pending_edge_batches (batch_id, crawl_id, source_channel, source_page_id, source_depth, sequence_id, "
       "status) VALUES ",
       "INSERT INTO pending_edges (batch_id, crawl_id, destination_channel, source_channel, sequence_id, discovery_time, "
@@ -5582,14 +5587,22 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
       "UPDATE pending_edge_batches SET status = 'closed', closed_at = NOW() WHERE batch_id ",
       "INSERT INTO page_buffer (page_id, parent_id, depth, url, crawl_id, sequence_id) VALUES ",
       "INSERT INTO edge_records (destination_channel, source_channel, walkback, skipped, discovery_time, crawl_id, "
-      "sequence_id) VALUES "};
-  static const uint32_t per_row[5] = {7, 8, 1, 6, 7};
+      "sequence_id) VALUES ",
+      "UPDATE pending_edge_batches SET status = 'completed', completed_at = NOW() WHERE batch_id ",
+      "INSERT INTO source_type_stats (crawl_id, source_type, total, valid, not_channel, invalid, duplicate) VALUES ($1, "
+      "$2, $3, $4, $5, $6, $7) ON CONFLICT (crawl_id, source_type) DO UPDATE SET total = source_type_stats.total + "
+      "EXCLUDED.total, valid = source_type_stats.valid + EXCLUDED.valid, not_channel = source_type_stats.not_channel + "
+      "EXCLUDED.not_channel, invalid = source_type_stats.invalid + EXCLUDED.invalid, duplicate = "
+      "source_type_stats.duplicate + EXCLUDED.duplicate;",
+      "DELETE FROM pending_edges WHERE batch_id "};
+  static const uint32_t per_row[8] = {7, 8, 1, 6, 7, 1, 7, 1};
   const uint32_t per = per_row[kind];
   s = head[kind];
+  if (kind == TGI_SQL_STATS_UPSERT) return;
   s.reserve(s.size() + (size_t)rows * (per * 8 + 4) + 8);
   char num[16] = {'$'};
   auto param = [&](uint32_t p) { s.append(num, (size_t)(std::to_chars(num + 1, num + sizeof num, p).ptr - num)); };
-  if (kind == TGI_SQL_BATCH_CLOSE) {
+  if (kind == TGI_SQL_BATCH_CLOSE || kind == TGI_SQL_BATCH_COMPLETE || kind == TGI_SQL_EDGES_DELETE) {
     if (rows == 1) {
       s += "= $1;";
       return;
@@ -5627,13 +5640,13 @@ void handoff_walkbacks(CrawlState& S, const tgi_state_span* spans, uint32_t n_sp
   S.wb_n_ok = 0;
 }
 
-// the checks both SQL calls make, in order: rows_per_stmt, now_nsec, crawl_id, a live hand-off
+// the checks the SQL calls make, in order: rows_per_stmt, now_nsec, crawl_id, and for the hand-off's two a live hand-off
 int sql_args(tgi_ctx* c, const CrawlState& S, uint32_t k, int32_t now_nsec, const char* crawl_id, uint32_t crawl_id_len,
-             const char* who) {
+             const char* who, bool handoff = true) {
   if (k < 1 || k > TGI_SQL_MAX_ROWS) { set_err(c, "%s: rows_per_stmt %u outside [1, %u]", who, k, TGI_SQL_MAX_ROWS); return TGI_E_ARG; }
   if (now_nsec < 0 || now_nsec >= 1000000000) { set_err(c, "%s: now_nsec %d out of range", who, now_nsec); return TGI_E_ARG; }
   if (crawl_id_len && !crawl_id) { set_err(c, "%s: crawl_id is NULL", who); return TGI_E_ARG; }
-  if (!S.handoff_live) { set_err(c, "%s: no tandem hand-off (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
+  if (handoff && !S.handoff_live) { set_err(c, "%s: no tandem hand-off (tgi_state_pending_edges, then no other state call)", who); return TGI_E_STATE; }
   return TGI_OK;
 }
 
@@ -5645,7 +5658,7 @@ int sql_clock(tgi_ctx* c, int64_t now_sec, int32_t now_nsec, const char* who, ch
   return TGI_OK;
 }
 
-// The statements of q.p (kind0, k and rows set) over `threads` row threads: their texts on the host (one per kind and
+// The statements of q.p (kind0, k and rows of its kinds set) over `threads` row threads: their texts on the host (one per kind and
 // row count, a kind's last statement maybe shorter), crawl_id and the clock tb[0, tl) uploaded, the params by the
 // two-pass writer (accepted() once the size pass has passed), and the texts, params and statement table read back into
 // h and hst.  Adds its device time and launches to out's.
@@ -5654,10 +5667,10 @@ int sql_render(tgi_ctx* c, CrawlState& S, Q& q, void (*size)(StDev, Q), void (*e
                const char* crawl_id, uint32_t crawl_id_len, const char* tb, uint32_t tl, const char* who, F&& accepted,
                HostBuf& h, HostBuf& hst, Out* out) {
   StSqlPlan& p = q.p;
-  const uint32_t k = p.k;
   uint64_t n_rows = 0;
   std::string texts, t;
-  for (uint32_t i = 0; i < 3; i++) {
+  for (uint32_t i = 0; i < ST_SQL_KINDS; i++) {
+    const uint32_t k = p.k[i] ? p.k[i] : 1;  // a kind past the call's has no rows
     p.m[i] = (p.rows[i] + k - 1) / k;
     p.n_stmts += p.m[i];
     n_rows += p.rows[i];
@@ -5711,6 +5724,35 @@ int sql_render(tgi_ctx* c, CrawlState& S, Q& q, void (*size)(StDev, Q), void (*e
   out->data_len = texts.size() + body;
   out->kernel_ms += st_rows_ms(S);
   out->gpu_launches += launches;
+  return TGI_OK;
+}
+
+// The claimed batches' checks (TGI_E_ARG): every array, offset, length and class code, before anything is uploaded
+int vw_input(tgi_ctx* c, const tgi_claimed_batches* in, const char* who) {
+  const uint64_t n = in->n_batches, ne = in->n_edges, sl = in->strs_len;
+  if (n && (!in->batches || !in->edge_off)) { set_err(c, "%s: batches or edge_off is NULL", who); return TGI_E_ARG; }
+  if (ne && !in->edges) { set_err(c, "%s: edges is NULL", who); return TGI_E_ARG; }
+  if (sl && !in->strs) { set_err(c, "%s: strs is NULL", who); return TGI_E_ARG; }
+  if (!n) return TGI_OK;
+  if (in->edge_off[0] != 0 || in->edge_off[n] != ne) {
+    set_err(c, "%s: edge_off[0] must be 0 and edge_off[n] n_edges (%llu)", who, (unsigned long long)ne);
+    return TGI_E_ARG;
+  }
+  auto out_of = [&](uint64_t off, uint32_t len) { return off > sl || len > sl - off; };
+  for (uint64_t i = 0; i < n; i++) {
+    const uint64_t a = in->edge_off[i], b = in->edge_off[i + 1];
+    if (b < a) { set_err(c, "%s: edge_off decreases at batch %llu", who, (unsigned long long)i); return TGI_E_ARG; }
+    if (b - a >= TGI_VW_NO_EDGE) { set_err(c, "%s: batch %llu has 2^32 - 1 edges or more", who, (unsigned long long)i); return TGI_E_ARG; }
+    const tgi_claimed_batch& B = in->batches[i];
+    for (int f = 0; f < 5; f++)
+      if (out_of(B.str_off[f], B.str_len[f])) { set_err(c, "%s: batch %llu string %d outside strs", who, (unsigned long long)i, f); return TGI_E_ARG; }
+  }
+  for (uint64_t j = 0; j < ne; j++) {
+    const tgi_claimed_edge& E = in->edges[j];
+    if (E.cls > TGI_EDGE_CLASS_OTHER) { set_err(c, "%s: edge %llu has class %u", who, (unsigned long long)j, E.cls); return TGI_E_ARG; }
+    for (int f = 0; f < 2; f++)
+      if (out_of(E.str_off[f], E.str_len[f])) { set_err(c, "%s: edge %llu string %d outside strs", who, (unsigned long long)j, f); return TGI_E_ARG; }
+  }
   return TGI_OK;
 }
 
@@ -5976,7 +6018,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   if (!nb) return TGI_OK;
   StSql q{};
   q.p.kind0 = TGI_SQL_BATCH_INSERT;
-  q.p.k = rows_per_stmt;
+  std::fill_n(q.p.k, 3, rows_per_stmt);
   q.p.rows[0] = q.p.rows[2] = nb;
   q.p.rows[1] = ne;
   q.edges = S.edges.as<tgi_state_edge>();
@@ -6062,7 +6104,7 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   }
   StWalkSql q{};
   q.p.kind0 = TGI_SQL_PAGE_BUFFER_INSERT;
-  q.p.k = rows_per_stmt;
+  std::fill_n(q.p.k, 2, rows_per_stmt);
   q.p.rows[0] = q.p.rows[1] = n_ok;
   q.spans = S.wb_in.as<uint32_t>();
   q.wb = S.wb.as<tgi_state_walkback_span>();
@@ -6070,6 +6112,105 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   q.n = n;
   return sql_render(c, S, q, st_walk_size_kernel, st_walk_emit_kernel, 2 * n, crawl_id, crawl_id_len, tb, tl, who, accept,
                     S.h_wb_sql, S.h_wb_stmts, out);
+}
+
+// processWalkbackBatch for every claimed batch: the upload, a thread per batch decides and picks, three scans place its
+// rows (one synchronise for the outcomes and totals), then the rows as tgi_state_edge_sql renders them (a thread per row
+// sizes it, a scan, a thread per row writes it and the statement table; one synchronise for the params' length, one
+// for the read-back)
+int tgi_state_validator_walkback(tgi_ctx* c, const tgi_claimed_batches* in, int64_t walkback_rate, const char* crawl_id,
+                                 uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt,
+                                 tgi_state_validator_walkback_t* out) {
+  static const char* const who = "tgi_state_validator_walkback";
+  if (!c || !out || !in) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;  // a state call: a live hand-off ends here
+  if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who, false))) return rc;
+  if ((rc = vw_input(c, in, who))) return rc;
+  const uint64_t n = in->n_batches, ne = in->n_edges;
+  if (!n) {
+    memset(out, 0, sizeof *out);
+    return TGI_OK;
+  }
+  if (!S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
+  cudaStream_t st = S.stream;
+  CK(S.vw_b.ensure(n * sizeof(tgi_claimed_batch)));
+  CK(S.vw_eoff.ensure((n + 1) * 8));
+  CK(S.vw_e.ensure(ne * sizeof(tgi_claimed_edge)));
+  CK(S.vw_s.ensure(in->strs_len));
+  CK(S.vw_out.ensure(n * sizeof(tgi_state_validator_batch)));
+  CK(S.vw_list.ensure(2 * ne * 4));
+  CK(S.vw_cnt.ensure(3 * n * 4));
+  CK(S.vw_rank.ensure(3 * (n + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_vw.ensure(n * sizeof(tgi_state_validator_batch)));
+  CK(cudaMemcpyAsync(S.vw_b.p, in->batches, n * sizeof(tgi_claimed_batch), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(S.vw_eoff.p, in->edge_off, (n + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (ne) CK(cudaMemcpyAsync(S.vw_e.p, in->edges, ne * sizeof(tgi_claimed_edge), cudaMemcpyHostToDevice, st));
+  if (in->strs_len) CK(cudaMemcpyAsync(S.vw_s.p, in->strs, in->strs_len, cudaMemcpyHostToDevice, st));
+  StVw v{};
+  v.b = S.vw_b.as<tgi_claimed_batch>();
+  v.eoff = S.vw_eoff.as<uint64_t>();
+  v.e = S.vw_e.as<tgi_claimed_edge>();
+  v.s = S.vw_s.as<uint8_t>();
+  v.n = n;
+  v.rate = walkback_rate;
+  v.seed = S.id_seed;
+  v.v0 = S.vw_next;
+  v.out = S.vw_out.as<tgi_state_validator_batch>();
+  v.vlist = S.vw_list.as<uint32_t>();
+  v.tlist = v.vlist + ne;
+  v.cnt = S.vw_cnt.as<uint32_t>();
+  uint64_t* rank = S.vw_rank.as<uint64_t>();
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [ST_SC_ROWS] OK batches, [ST_SC_BYTES] edge rows, [ST_SC_SLOTS] stats rows
+  static const int tot[3] = {ST_SC_ROWS, ST_SC_BYTES, ST_SC_SLOTS};
+  uint32_t launches = 0;
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);  // the discovered set: read by the pick, not changed
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    v.disc = c->sets[TGI_SET_DISCOVERED].dev;
+    CK(cudaEventRecord(S.t0, st));
+    st_vw_pick_kernel<<<sink_grid(c, n, ST_THREADS, 4), ST_THREADS, 0, st>>>(v);
+    launches++;
+    for (int k = 0; k < 3; k++)
+      if ((rc = launch_scan(c, st, S.tiles, v.cnt + k * n, n, rank + k * (n + 1), dsc + tot[k], launches))) return rc;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t1, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(S.h_vw.p, v.out, n * sizeof(tgi_state_validator_batch), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  float ms = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  const uint64_t* hs = S.h_sc.as<uint64_t>();
+  const uint64_t n_ok = hs[ST_SC_ROWS], n_edge_rows = hs[ST_SC_BYTES], n_stats = hs[ST_SC_SLOTS];
+  char tb[48];
+  uint32_t tl = 0;
+  if (n_ok && (rc = sql_clock(c, now_sec, now_nsec, who, tb, &tl))) return rc;
+  auto accept = [&]() { S.vw_next += n; };  // a refused call leaves v where it was
+  memset(out, 0, sizeof *out);
+  out->n_batches = (uint32_t)n;
+  out->batches = S.h_vw.as<tgi_state_validator_batch>();
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  if (!n_ok) {
+    accept();
+    return TGI_OK;
+  }
+  StVwSql q{};
+  q.p.kind0 = TGI_SQL_PAGE_BUFFER_INSERT;
+  const uint64_t rows[5] = {n_ok, n_edge_rows, n_ok, n_stats, n_ok};
+  for (int k = 0; k < 5; k++) {
+    q.p.rows[k] = rows[k];
+    q.p.k[k] = k == TGI_SQL_STATS_UPSERT - TGI_SQL_PAGE_BUFFER_INSERT ? 1u : rows_per_stmt;  // upserts: one row each
+  }
+  q.v = v;
+  q.rank = rank;
+  return sql_render(c, S, q, st_vw_size_kernel, st_vw_emit_kernel, 3 * n_ok + n_edge_rows + n_stats, crawl_id,
+                    crawl_id_len, tb, tl, who, accept, S.h_vw_sql, S.h_vw_stmts, out);
 }
 
 }  // extern "C"

@@ -42,7 +42,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
     "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers", "tgi_state_edge_sql",
-    "tgi_state_walkback",
+    "tgi_state_walkback", "tgi_state_validator_walkback",
 ]
 
 
@@ -136,6 +136,8 @@ def lib() -> C.CDLL:
         L.tgi_state_layers.argtypes = [vp, C.POINTER(abi.StateLayersC)]
         L.tgi_state_edge_sql.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateEdgeSqlC)]
         L.tgi_state_walkback.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateWalkbackC)]
+        L.tgi_state_validator_walkback.argtypes = [vp, C.POINTER(abi.ClaimedBatchesC), C.c_int64, C.c_char_p, u32,
+                                                   C.c_int64, i32, u32, C.POINTER(abi.StateValidatorWalkbackC)]
         _LIB = L
     return _LIB
 
@@ -969,9 +971,37 @@ class Engine:
                       "sequence_id": bytes(w["sequence_id"])} for w in wb]
         return walkbacks, self._st_stmts(out)
 
+    def state_validator_walkback(self, batches, walkback_rate: int, crawl_id: bytes, now=(0, 0),
+                                 rows_per_stmt: int = 1) -> tuple:
+        """processWalkbackBatch for claimed batches (a list of dicts for state_pack.pack_claimed_batches, or its packed
+        tuple): each batch's decision and pick, and the Postgres binding calls of the OK ones, every page_buffer insert,
+        every edge_records insert, every complete, every stats upsert, every delete.  Returns (results, stmts): per
+        batch {"status" (abi.WALK_*), "walkback", "rnd", "draws", "n_valid", "forward_edge" (None for a walkback),
+        "url", "page_id", "sequence_id"}, and [(kind (abi.SQL_*), rows, sql, params)]; the device time and launches are
+        left in self.state_vw_ms and self.state_vw_launches"""
+        from .state_pack import pack_claimed_batches
+        recs, edge_off, edges, blob = batches if isinstance(batches, tuple) else pack_claimed_batches(batches)
+        recs, edges = np.ascontiguousarray(recs, abi.CLAIMED_BATCH), np.ascontiguousarray(edges, abi.CLAIMED_EDGE)
+        edge_off, blob = np.ascontiguousarray(edge_off, np.uint64), np.ascontiguousarray(blob, np.uint8)
+        cin = abi.ClaimedBatchesC(len(recs), 0, recs.ctypes.data, edge_off.ctypes.data, edges.ctypes.data, len(edges),
+                                  blob.ctypes.data, len(blob))
+        out = abi.StateValidatorWalkbackC()
+        self._check(lib().tgi_state_validator_walkback(self.h, C.byref(cin), walkback_rate, crawl_id, len(crawl_id),
+                                                       now[0], now[1], rows_per_stmt, C.byref(out)))
+        self.state_vw_ms = float(out.kernel_ms)
+        self.state_vw_launches = int(out.gpu_launches)
+        res = _view(out.batches, int(out.n_batches), abi.STATE_VALIDATOR_BATCH)
+        results = [{"status": int(r["status"]), "walkback": bool(r["walkback"]), "rnd": int(r["rnd"]),
+                    "draws": int(r["draws"]), "n_valid": int(r["n_valid"]),
+                    "forward_edge": None if r["forward_edge"] == abi.VW_NO_EDGE else int(r["forward_edge"]),
+                    "url": bytes(r["url"][:int(r["url_len"])]), "page_id": bytes(r["page_id"]),
+                    "sequence_id": bytes(r["sequence_id"])} for r in res]
+        return results, self._st_stmts(out)
+
     @staticmethod
     def _st_stmts(out) -> list:
-        """the statement table of a state_edge_sql or state_walkback result: [(kind, rows, sql, params)]"""
+        """the statement table of a state_edge_sql, state_walkback or state_validator_walkback result:
+        [(kind, rows, sql, params)]"""
         st = _view(out.stmts, int(out.n_stmts), abi.STATE_EDGE_STMT)
         data = C.string_at(out.data, int(out.data_len)) if out.data_len else b""
         return [(int(k), int(r), data[int(so):int(so + sl)], data[int(po):int(po + pl)])

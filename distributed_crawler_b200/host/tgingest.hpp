@@ -477,6 +477,18 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return o;
   }
+  // Validator walkback: processWalkbackBatch for n claimed batches (batches[k].status TGI_WALK_*; a batch that is not OK
+  // is the reference's random-walk-walkback error and stays claimed), and the exec calls of the OK ones as StateEdgeSql's
+  // are read.  Ends a live StatePendingEdges hand-off.  The arrays stay valid until the next state call.
+  tgi_state_validator_walkback_t StateValidatorWalkback(const tgi_claimed_batches& in, int64_t walkback_rate,
+                                                        std::string_view crawl_id, int64_t now_sec, int32_t now_nsec,
+                                                        uint32_t rows_per_stmt) {
+    tgi_state_validator_walkback_t o{};
+    if (tgi_state_validator_walkback(ctx_, &in, walkback_rate, crawl_id.data(), (uint32_t)crawl_id.size(), now_sec,
+                                     now_nsec, rows_per_stmt, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
   // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
   // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.

@@ -36,3 +36,38 @@ def pack_pages(pages, code, msg_page):
             msgs.append((m["chatId"], m["messageId"], msg_page(m.get("pageId", b""), i), code(m.get("status", b"")),
                          code(m.get("platform", b""))))
     return recs, np.frombuffer(bytes(blob) + b"\0" * 16, np.uint8).copy(), np.array(msgs, abi.STATE_MSG)
+
+
+def pack_claimed_batches(batches):
+    """-> (tgi_claimed_batch array, edge_off u64[n+1], tgi_claimed_edge array, string blob) of claimed batches, each a
+    dict with PendingEdgeBatch's strings as bytes (abi.CLAIMED_BATCH_STRINGS; missing = empty), "source_depth" and
+    "edges" = [(destination, source_type, validation_status)], all bytes; the status maps to abi.EDGE_CLASS_* by exact
+    match, anything else OTHER.  Equal strings are stored once."""
+    recs = np.zeros(len(batches), abi.CLAIMED_BATCH)
+    edge_off = np.zeros(len(batches) + 1, np.uint64)
+    blob = bytearray()
+    at = {}
+
+    def put(s):
+        o = at.get(s)
+        if o is None:
+            o = at[s] = len(blob)
+            blob.extend(s)
+        return o
+
+    rows = []
+    for i, b in enumerate(batches):
+        for k, name in enumerate(abi.CLAIMED_BATCH_STRINGS):
+            s = b.get(name, b"")
+            recs[i]["str_off"][k], recs[i]["str_len"][k] = put(s), len(s)
+        recs[i]["source_depth"] = b.get("source_depth", 0)
+        for dest, st, status in b.get("edges", ()):
+            rows.append((put(dest), put(st), len(dest), len(st), abi.EDGE_CLASS_OF.get(status, abi.EDGE_CLASS_OTHER)))
+        edge_off[i + 1] = len(rows)
+    edges = np.zeros(len(rows), abi.CLAIMED_EDGE)
+    if rows:
+        a = np.array(rows, np.uint64)
+        edges["str_off"] = a[:, 0:2]
+        edges["str_len"] = a[:, 2:4]
+        edges["cls"] = a[:, 4]
+    return recs, edge_off, edges, np.frombuffer(bytes(blob) + b"\0" * 16, np.uint8).copy()

@@ -1298,6 +1298,125 @@ typedef struct tgi_state_walkback_t {
 int tgi_state_walkback(tgi_ctx* ctx, const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
                        uint32_t rows_per_stmt, tgi_state_walkback_t* out);
 
+/* Validator walkback — the validator pod's walkback processor (crawl/validator.go:314-489) for n claimed batches in one
+ * call: processWalkbackBatch's decision, its forward or walkback pick (pickWalkbackChannel, crawl/runner.go:115-139,
+ * with the batch's valid channels excluded), AddPageToPageBuffer (state/daprstate.go:3619-3641), SaveEdgeRecords of
+ * the primary and skipped edges (:3150-3204), CompletePendingBatch and FlushBatchStats (:4124-4206), each sent by
+ * ExecuteDatabaseOperation as an `exec` InvokeBinding.  The walkback pick draws from the resident TGI_SET_DISCOVERED.
+ *   Input    what ClaimWalkbackBatch (:4016-4122) returns, per batch: tgi_claimed_batch (its five strings as (offset,
+ *            length) pairs into strs, source_depth) and its edges edges[edge_off[i] .. edge_off[i+1]) in the order the
+ *            database returned them, each with its destination, its source_type and its validation_status mapped to a
+ *            TGI_EDGE_CLASS_* by exact match ("valid", "not_channel", "invalid", "duplicate", anything else OTHER).
+ *            Nothing is read from a crawler hand-off.  It is a state call, so it ends a live tgi_state_pending_edges
+ *            hand-off (a following tgi_state_edge_sql or tgi_state_walkback is TGI_E_STATE).
+ *   Decide   per batch, in input order: validFirstClaimed = the destinations of its VALID edges, in edge order.  None:
+ *            walk back, rnd = -1.  Else rnd = IntN(100) + 1 and the batch walks back iff walkback_rate >= rnd.
+ *   Pick     walkback: pickWalkbackChannel(source_channel, exclude = validFirstClaimed) over the set's N keys in
+ *            first-occurrence order, as tgi_state_walkback's pick: up to 10 draws, a draw equal (byte for byte) to the
+ *            source channel or to any excluded name is retried; TGI_WALK_OK, TGI_WALK_EXHAUSTED after 10 such draws,
+ *            TGI_WALK_EMPTY when N = 0.  The page's SequenceID is a new id, the primary edge's the batch's.  Forward:
+ *            idx = IntN(n_valid); the page URL is that destination, which leaves the skipped list (order kept); the page
+ *            and the primary edge take the batch's SequenceID.  A batch whose pick fails writes nothing (the reference
+ *            returns the error before its first write) and keeps its result, so the shim can log it and leave the batch
+ *            claimed.
+ *   Random   the v-th batch the context handles (v is not reset by tgi_state_set, and tgi_state_walkback's counter is
+ *            separate) draws from the 64-bit words of Philox4x32-10 blocks (v_lo, v_hi, 5, j) under the page-id seed:
+ *            x0 | x1 << 32, then x2 | x3 << 32.  rnd, the forward index and the walkback draws are Lemire's
+ *            multiply-and-reject over that one stream, in that order.  The page ID and the new SequenceID are ids of the
+ *            page-id construction with counter (v, 6) and (v, 7).  v advances by n on an accepted call only.  Without
+ *            tgi_state_id_seed a call with batches is TGI_E_STATE.
+ *   Rows     per TGI_WALK_OK batch: page_buffer [ID, source_page_id, source_depth + 1, url, crawl_id, page SequenceID];
+ *            edge_records primary [url, source_channel, walkback, false, discovery_time, crawl_id, batch SequenceID],
+ *            then one skipped row [ch, source_channel, false, true, discovery_time, crawl_id, batch SequenceID] per
+ *            remaining valid channel; complete [batch_id]; one stats upsert [batch crawl_id, st, total, valid,
+ *            not_channel, invalid, duplicate] per distinct source_type of all its edges (empty is "unknown"), in
+ *            first-occurrence order; delete [batch_id].  crawl_id of the page and edge rows is the batch's, or the call's
+ *            when the batch's is empty; the stats rows take the batch's as it is (FlushBatchStats has no fallback).
+ *            source_depth + 1 wraps as Go's int.  OTHER counts in total only.  Strings, the clock and the year check
+ *            are tgi_state_edge_sql's; the clock is read once per call.
+ *   Order    every page_buffer insert (TGI_SQL_PAGE_BUFFER_INSERT), every edge_records insert (per batch: primary, then
+ *            skipped), every complete (TGI_SQL_BATCH_COMPLETE), every upsert (TGI_SQL_STATS_UPSERT), every delete
+ *            (TGI_SQL_EDGES_DELETE), each kind in batch order: a batch's page, edges, complete, stats and delete keep the
+ *            reference's order.  rows_per_stmt = k rows per statement by tgi_state_edge_sql's rule for every kind but
+ *            the upserts; complete and delete of more rows are "WHERE batch_id IN ($1, ...)".  A stats upsert is always
+ *            one row per statement: rows of two batches of one crawl share the key (crawl_id, source_type), and Postgres
+ *            refuses an ON CONFLICT DO UPDATE that touches one row twice.  k = 1 gives the reference's calls.
+ *   Cost     a thread per batch decides, picks, lists its valid edges and its distinct source types (a compare against
+ *            each type found so far, so m edges of d types cost m * d compares) and counts its rows; three scans place
+ *            them; a thread per row sizes it, a scan, a thread per row writes it and the statement table.  A stats row
+ *            counts its type over the batch's edges.  Three synchronises.  n = 0 launches nothing.
+ *   Errors   every check runs before anything changes: a refused call makes nothing and leaves v as it was.  TGI_E_ARG:
+ *            k outside [1, 8191], now_nsec outside [0, 1e9), crawl_id NULL with a length, a NULL array with a count,
+ *            edge_off[0] != 0, edge_off decreasing or edge_off[n] != n_edges, a batch of 2^32 - 1 edges or more, a
+ *            string outside strs, a class code past OTHER, and when there is a row a clock whose local year leaves
+ *            [0, 9999].  TGI_E_STATE: no seed.  TGI_E_CAPACITY: a row of 4 GiB or more.  All of out lives in pinned
+ *            memory until the next state call.                                                                       */
+#define TGI_SQL_BATCH_COMPLETE 5      /* CompletePendingBatch                                                         */
+#define TGI_SQL_STATS_UPSERT 6        /* FlushBatchStats: one source_type's upsert                                    */
+#define TGI_SQL_EDGES_DELETE 7        /* FlushBatchStats: the batch's pending_edges                                   */
+#define TGI_EDGE_CLASS_VALID 0        /* validation_status "valid"                                                    */
+#define TGI_EDGE_CLASS_NOT_CHANNEL 1  /* "not_channel"                                                                */
+#define TGI_EDGE_CLASS_INVALID 2      /* "invalid"                                                                    */
+#define TGI_EDGE_CLASS_DUPLICATE 3    /* "duplicate"                                                                  */
+#define TGI_EDGE_CLASS_OTHER 4        /* anything else: counted in total only                                         */
+#define TGI_CB_BATCH_ID 0             /* tgi_claimed_batch strings                                                    */
+#define TGI_CB_CRAWL_ID 1
+#define TGI_CB_SOURCE_CHANNEL 2
+#define TGI_CB_SOURCE_PAGE_ID 3
+#define TGI_CB_SEQUENCE_ID 4
+#define TGI_CE_DESTINATION 0          /* tgi_claimed_edge strings                                                     */
+#define TGI_CE_SOURCE_TYPE 1
+#define TGI_VW_NO_EDGE 0xFFFFFFFFu    /* tgi_state_validator_batch.forward_edge of a walkback                         */
+typedef struct tgi_claimed_batch {    /* 72 bytes: one PendingEdgeBatch                                               */
+  uint64_t str_off[5];                /* TGI_CB_*: strs[str_off[f] .. + str_len[f])                                   */
+  uint32_t str_len[5];
+  uint32_t reserved;
+  int64_t source_depth;
+} tgi_claimed_batch;
+typedef struct tgi_claimed_edge {     /* 32 bytes: one PendingEdge                                                    */
+  uint64_t str_off[2];                /* TGI_CE_*                                                                     */
+  uint32_t str_len[2];
+  uint32_t cls;                       /* TGI_EDGE_CLASS_*                                                             */
+  uint32_t reserved;
+} tgi_claimed_edge;
+typedef struct tgi_claimed_batches {
+  uint32_t n_batches;
+  uint32_t reserved;
+  const tgi_claimed_batch* batches;   /* [n_batches]                                                                  */
+  const uint64_t* edge_off;           /* [n_batches+1]: batch i's edges are edges[edge_off[i] .. edge_off[i+1])       */
+  const tgi_claimed_edge* edges;      /* [n_edges]                                                                    */
+  uint64_t n_edges;
+  const uint8_t* strs;                /* every string of the batches and edges                                        */
+  uint64_t strs_len;
+} tgi_claimed_batches;
+typedef struct tgi_state_validator_batch { /* 136 bytes: one batch's outcome                                          */
+  uint32_t status;                    /* TGI_WALK_* (a forward batch is TGI_WALK_OK)                                  */
+  uint32_t walkback;                  /* 1: walked back                                                               */
+  int32_t rnd;                        /* IntN(100) + 1, or -1 without a valid edge                                    */
+  uint32_t draws;                     /* walkback draws made                                                          */
+  uint32_t n_valid;                   /* len(validFirstClaimed)                                                       */
+  uint32_t forward_edge;              /* the followed edge's index within the batch, or TGI_VW_NO_EDGE                */
+  uint32_t url_len;
+  uint32_t reserved;
+  uint8_t url[32];                    /* the walkback channel (TGI_WALK_OK walkback), zero padded                     */
+  uint8_t page_id[36];                /* the new page's ID                                                            */
+  uint8_t sequence_id[36];            /* the new chain's SequenceID, which the page takes when it walks back          */
+} tgi_state_validator_batch;
+typedef struct tgi_state_validator_walkback_t {
+  uint32_t n_batches;
+  uint32_t reserved;
+  const tgi_state_validator_batch* batches; /* [n_batches] in input order (pinned)                                    */
+  uint64_t n_stmts;
+  const tgi_state_edge_stmt* stmts;   /* [n_stmts] in execution order (pinned)                                        */
+  const uint8_t* data;                /* the texts, then the params (pinned)                                          */
+  uint64_t data_len;
+  float kernel_ms;                    /* device time of the call's kernels and scans (not the copies)                */
+  uint32_t gpu_launches;
+} tgi_state_validator_walkback_t;
+int tgi_state_validator_walkback(tgi_ctx* ctx, const tgi_claimed_batches* in, int64_t walkback_rate, const char* crawl_id,
+                                 uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt,
+                                 tgi_state_validator_walkback_t* out);
+
 /* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
  * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on
  * the device never holds a copy of the page table: layer read, tgi_state_pages_begin of the selected rows, one bulk
