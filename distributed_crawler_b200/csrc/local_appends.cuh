@@ -10,21 +10,20 @@
 //      index of its first line (atomicMin);
 //   3. runs: maximal spans of consecutive lines of one canonical channel (flag + scan); groups: the lines that are
 //      their channel's first line (flag + scan), so a group's id is the rank of its first line;
-//   4. a stable LSD radix sort of the runs by group id, 8 bits or fewer per pass, with a block-local stable scatter;
+//   4. the stable LSD radix sort of radix.cuh orders the runs by group id;
 //   5. an exclusive scan of the run line counts in sorted order places every line in `order`, a scan of the line
 //      lengths in that order gives every run its destination byte, and the gather copies the bytes, mapped from the
 //      output side: a thread per 16-byte output vector.
 // Sizes the host does not know yet (lines, runs, groups) stay on the device: kernels are launched for their upper
 // bounds (records, channel rows) and read the exact counts from the scalars block.
 #pragma once
+#include "radix.cuh"
 #include "sink_src.cuh"
 
 namespace tgi {
 
 constexpr uint32_t LA_NONE = 0xFFFFFFFFu;
 constexpr int LA_THREADS = 256;
-// radix sort: a tile of RS_TILE runs per CTA; warp w owns RS_ROUNDS * 32 consecutive runs of it
-constexpr int RS_WARPS = 8, RS_ROUNDS = 8, RS_TILE = RS_WARPS * RS_ROUNDS * 32, RS_RADIX = 256;
 // gather: a CTA copies LA_GATHER_ITEMS * LA_THREADS consecutive output vectors per step (64 KiB)
 constexpr int LA_GATHER_ITEMS = 16;
 // the scalars block: counts the scans leave on the device
@@ -142,72 +141,6 @@ __global__ void la_runs_kernel(uint64_t n, LaWork w) {
     w.run_start[r] = (uint32_t)j;
     w.keys[0][r] = (uint32_t)w.gpos[w.first_line[w.lkey[j]]];
     w.vals[0][r] = r;
-  }
-}
-
-// 4a. digit counts of one tile of runs, digit-major: counts[d * ntiles + tile]
-__global__ void __launch_bounds__(RS_WARPS * 32) la_radix_hist_kernel(const uint32_t* keys, const uint64_t* count,
-                                                                      uint32_t shift, uint32_t radix, uint32_t ntiles,
-                                                                      uint32_t* counts) {
-  __shared__ uint32_t h[RS_RADIX];
-  for (uint32_t d = threadIdx.x; d < radix; d += blockDim.x) h[d] = 0;
-  __syncthreads();
-  const uint64_t n = *count, base = (uint64_t)blockIdx.x * RS_TILE;
-  for (uint32_t t = threadIdx.x; t < RS_TILE; t += blockDim.x)
-    if (base + t < n) atomicAdd(h + ((keys[base + t] >> shift) & (radix - 1)), 1u);
-  __syncthreads();
-  for (uint32_t d = threadIdx.x; d < radix; d += blockDim.x) counts[(uint64_t)d * ntiles + blockIdx.x] = h[d];
-}
-
-// 4b. stable scatter of one tile: off[d * ntiles + tile] (the scan of the counts) is where the tile's runs with digit d
-// start.  Warp w walks its runs in order, 32 at a time: __match_any_sync finds the lanes with the same digit, and a
-// run's rank is the number of such lanes below it plus the runs of that digit the warp already placed.  The first walk
-// counts per warp and digit, the prefix over the warps turns the counts into starts, the second walk places.
-__global__ void __launch_bounds__(RS_WARPS * 32) la_radix_scatter_kernel(const uint32_t* kin, const uint32_t* vin,
-                                                                         uint32_t* kout, uint32_t* vout,
-                                                                         const uint64_t* count, uint32_t shift,
-                                                                         uint32_t radix, uint32_t ntiles,
-                                                                         const uint64_t* off) {
-  __shared__ uint32_t wh[RS_WARPS][RS_RADIX];
-  const int l = lane_id(), w = threadIdx.x >> 5;
-  for (uint32_t d = threadIdx.x; d < RS_WARPS * RS_RADIX; d += blockDim.x) (&wh[0][0])[d] = 0;
-  __syncthreads();
-  const uint64_t n = *count, base = (uint64_t)blockIdx.x * RS_TILE + (uint64_t)w * (RS_ROUNDS * 32);
-  uint32_t kk[RS_ROUNDS], vv[RS_ROUNDS];
-#pragma unroll
-  for (int k = 0; k < RS_ROUNDS; k++) {
-    const uint64_t i = base + k * 32 + l;
-    const bool ok = i < n;
-    kk[k] = ok ? kin[i] : 0;
-    vv[k] = ok ? vin[i] : 0;
-    const uint32_t d = ok ? (kk[k] >> shift) & (radix - 1) : LA_NONE;
-    const uint32_t peers = __match_any_sync(FULL, d);
-    if (ok && l == __ffs(peers) - 1) wh[w][d] += __popc(peers);
-    __syncwarp();
-  }
-  __syncthreads();
-  for (uint32_t d = threadIdx.x; d < radix; d += blockDim.x) {
-    uint32_t run = (uint32_t)off[(uint64_t)d * ntiles + blockIdx.x];
-    for (int x = 0; x < RS_WARPS; x++) {
-      const uint32_t c = wh[x][d];
-      wh[x][d] = run;
-      run += c;
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < RS_ROUNDS; k++) {
-    const bool ok = base + k * 32 + l < n;
-    const uint32_t d = ok ? (kk[k] >> shift) & (radix - 1) : LA_NONE;
-    const uint32_t peers = __match_any_sync(FULL, d);
-    if (ok) {
-      const uint32_t dst = wh[w][d] + __popc(peers & ((1u << l) - 1));
-      kout[dst] = kk[k];
-      vout[dst] = vv[k];
-    }
-    __syncwarp();
-    if (ok && l == __ffs(peers) - 1) wh[w][d] += __popc(peers);
-    __syncwarp();
   }
 }
 

@@ -11,8 +11,8 @@
 //   table       open-addressed (row, gen, chat_id, message_id) -> lowest message index: the gen in the key keeps
 //               tombstones out of every lookup; the table is rebuilt from the live rows when the messages compact.
 //
-// Render: live messages are compacted and grouped by row with the stable radix passes of local_appends.cuh (order
-// inside a row = storage order); a thread per message sizes it, a warp per entry (a page of a layer, or an empty layer)
+// Render: live messages are compacted and grouped by row with the stable radix sort of radix.cuh (order inside a
+// row = storage order); a thread per message sizes it, a warp per entry (a page of a layer, or an empty layer)
 // sizes the page around its messages, scans place both, and the emit writes every byte at its final offset: a warp per
 // entry for the page's fields, a thread per (entry, message) slot for the messages.
 //
@@ -25,11 +25,12 @@
 // The turn's owner keys stay as the row's owner view; the close appends the view as the row's next generation.
 //
 // Page reads: the rows' fields come from the host mirror; their lists are the live messages of the distinct rows,
-// flagged in one pass, grouped by row with the render's radix passes and written out in that order.
+// flagged in one pass, grouped by row like the render's and written out in that order.
 #pragma once
 #include <type_traits>
 
-#include "local_appends.cuh"
+#include "kernels.cuh"
+#include "radix.cuh"
 
 namespace tgi {
 
@@ -470,10 +471,6 @@ struct StRender {
   uint32_t zone_n;
   int32_t tz;
   uint64_t* sc;        // ST_SC_*
-  uint32_t* flag;      // [n_msgs] live flags
-  uint64_t* pos;       // [n_msgs+1] their scan
-  uint32_t* keys[2];   // radix ping-pong: row, message index
-  uint32_t* vals[2];
   uint64_t* row_base;  // [rows+1] scan of row_cnt: first grouped message of every row
   uint32_t* msize;     // [live] bytes of grouped message k (its leading comma included)
   uint64_t* moff;      // [live+1] their scan
@@ -569,18 +566,19 @@ DEVI StLen<EMIT> st_message(const StDev& d, const StMsg& m, bool comma, uint8_t*
   return o;
 }
 
-// live flags of every message row
-__global__ void st_render_flag_kernel(StDev d, uint64_t n, StRender r) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-    r.flag[i] = st_live(d, d.msgs[i]);
-}
-// the live messages compacted in storage order: the radix sort's input pairs (row, message index)
-__global__ void st_render_pairs_kernel(StDev d, uint64_t n, StRender r) {
+struct StGroup {       // live messages grouped by row (the render, the page reads, the page close)
+  const uint32_t* flag;  // [n_msgs] flags of the messages taken
+  const uint64_t* pos;   // [n_msgs+1] their scan
+  uint32_t* keys[2];     // radix ping-pong: row, message index
+  uint32_t* vals[2];
+};
+// the flagged messages compacted in storage order: the radix sort's input pairs (row, message index)
+__global__ void st_render_pairs_kernel(StDev d, uint64_t n, StGroup g) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    if (!r.flag[i]) continue;
-    const uint64_t k = r.pos[i];
-    r.keys[0][k] = d.msgs[i].row;
-    r.vals[0][k] = (uint32_t)i;
+    if (!g.flag[i]) continue;
+    const uint64_t k = g.pos[i];
+    g.keys[0][k] = d.msgs[i].row;
+    g.vals[0][k] = (uint32_t)i;
   }
 }
 // size pass, a thread per grouped message k (sorted = the grouped message indices, sorted_rows their rows)

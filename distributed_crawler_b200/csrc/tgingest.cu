@@ -543,6 +543,45 @@ int launch_scan(tgi_ctx* c, Slot& s, const uint32_t* in, uint64_t n, uint64_t* o
   return launch_scan(c, s.stream, s.d_tiles, in, n, out, d_total, launches);
 }
 
+// The passes of a radix sort of keys up to kmax: over the bits of kmax, 8 bits or fewer each.  The sorted pairs end in
+// side `out` of the ping-pong, so a caller that needs them in a given place puts that place there before the sort.
+struct RadixPlan {
+  uint32_t passes, width;
+  int out;
+  explicit RadixPlan(uint64_t kmax) {
+    uint32_t bits = 0;
+    while (bits < 32 && kmax >> bits) bits++;
+    passes = (bits + 7) / 8;
+    width = passes ? (bits + passes - 1) / passes : 0;
+    out = passes & 1;
+  }
+};
+
+// The stable LSD radix sort (radix.cuh) of the *d_n pairs (keys[0], vals[0]) by key, by plan's passes, the pairs
+// ping-ponging between sides 0 and 1; n_max >= *d_n sizes the tiles, counts and roff hold the digit counts and their
+// scan, whose total goes to *d_total.  tiled: the scans take their multi-launch form.  Nothing is waited for.
+int radix_sort(tgi_ctx* c, cudaStream_t st, DevBuf& tiles, uint32_t* const keys[2], uint32_t* const vals[2], const uint64_t* d_n,
+               uint64_t n_max, const RadixPlan& plan, DevBuf& counts, DevBuf& roff, uint64_t* d_total, bool tiled,
+               uint32_t& launches) {
+  const uint32_t radix = 1u << plan.width;
+  const uint64_t ntiles = std::max<uint64_t>((n_max + RS_TILE - 1) / RS_TILE, 1);
+  CK(counts.ensure(radix * ntiles * 4));
+  CK(roff.ensure((radix * ntiles + 1) * 8));
+  int rc;
+  for (uint32_t p = 0, cur = 0; p < plan.passes; p++, cur ^= 1) {
+    const uint32_t shift = p * plan.width;
+    radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(keys[cur], d_n, shift, radix, (uint32_t)ntiles,
+                                                                   counts.as<uint32_t>());
+    launches++;
+    if ((rc = launch_scan(c, st, tiles, counts.as<uint32_t>(), radix * ntiles, roff.as<uint64_t>(), d_total, launches, tiled)))
+      return rc;
+    radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(keys[cur], vals[cur], keys[cur ^ 1], vals[cur ^ 1], d_n,
+                                                                      shift, radix, (uint32_t)ntiles, roff.as<uint64_t>());
+    launches++;
+  }
+  return TGI_OK;
+}
+
 // Sizes the frontier scratch for a batch of n records and `links` links (the hash table holds at least twice as many
 // slots, the per-link state covers `lstate_rows`) and returns the kernels' view of it.  The table is not zeroed.
 int frontier_scratch(tgi_ctx* c, FrontierScratch& z, uint64_t n, uint64_t links, uint64_t lstate_rows, FrontierBatch& fb) {
@@ -2698,17 +2737,10 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   const uint64_t nc = src.n_chans, n2 = n + 2;
   const uint64_t gmax = std::min<uint64_t>(n, nc);  // groups: at most one per record and one per row
   const uint64_t tslots = next_pow2(std::max<uint64_t>(2 * nc, 64));
-  // radix passes over the bits of the largest group id, 8 bits or fewer each
-  uint32_t bits = 0;
-  while (bits < 32 && (gmax - 1) >> bits) bits++;
-  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
-  const uint64_t ntiles = (n + RS_TILE - 1) / RS_TILE;
   CK(z.table.ensure(tslots * 4));
   CK(z.rows.ensure(2 * nc * 4));
   CK(z.u32s.ensure(11 * n2 * 4));
   CK(z.u64s.ensure(7 * n2 * 8));
-  CK(z.counts.ensure(radix * ntiles * 4));
-  CK(z.roff.ensure((radix * ntiles + 1) * 8));
   CK(z.groups.ensure(gmax * sizeof(tgi_channel_group)));
   CK(z.order.ensure(n * 8));
   CK(z.data.ensure(total));
@@ -2750,19 +2782,11 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   if ((rc = launch_scan(c, s, w.gflag, n, w.gpos, w.sc + LA_SC_GROUPS, launches))) return rc;
   la_runs_kernel<<<grid(n), LA_THREADS, 0, st>>>(n, w);
   launches++;
-  int cur = 0;  // the ping-pong side that holds the sorted pairs
-  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
-    const uint32_t shift = p * width;
-    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(w.keys[cur], w.sc + LA_SC_RUNS, shift, radix,
-                                                                     (uint32_t)ntiles, z.counts.as<uint32_t>());
-    launches++;
-    if ((rc = launch_scan(c, s, z.counts.as<uint32_t>(), radix * ntiles, z.roff.as<uint64_t>(), w.sc + LA_SC_RADIX, launches))) return rc;
-    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(w.keys[cur], w.vals[cur], w.keys[cur ^ 1],
-                                                                        w.vals[cur ^ 1], w.sc + LA_SC_RUNS, shift, radix,
-                                                                        (uint32_t)ntiles, z.roff.as<uint64_t>());
-    launches++;
-  }
-  const uint32_t* sorted = w.vals[cur];
+  const RadixPlan plan(gmax - 1);  // by group id
+  if ((rc = radix_sort(c, st, s.d_tiles, w.keys, w.vals, w.sc + LA_SC_RUNS, n, plan, z.counts, z.roff, w.sc + LA_SC_RADIX, false,
+                       launches)))
+    return rc;
+  const uint32_t* sorted = w.vals[plan.out];
   la_sorted_counts_kernel<<<grid(n), LA_THREADS, 0, st>>>(n, sorted, w);
   launches++;
   if ((rc = launch_scan(c, s, w.cnt, n, w.lpos, w.sc + LA_SC_SORTED_LINES, launches))) return rc;
@@ -2770,7 +2794,7 @@ int tgi_channel_appends(tgi_ctx* c, int slot, tgi_channel_appends_t* out) {
   la_order_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w);
   launches += 2;
   if ((rc = launch_scan(c, s, w.cnt, n, w.goff, w.sc + LA_SC_BYTES, launches))) return rc;
-  la_tables_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w.keys[cur], sorted, w);
+  la_tables_kernel<<<grid(n), LA_THREADS, 0, st>>>(src, w.keys[plan.out], sorted, w);
   la_gather_kernel<<<sink_grid(c, (total + 15) / 16, LA_GATHER_ITEMS * LA_THREADS, 8), LA_THREADS, 0, st>>>(src, w, total);
   launches += 2;
   CK(cudaGetLastError());
@@ -3767,6 +3791,39 @@ int st_page_json_emit(tgi_ctx* c, CrawlState& S, StRender& r, const uint32_t* so
   return TGI_OK;
 }
 
+// The live messages of every row (set == nullptr) or of the rows set[0, ns) (ascending), grouped by row in storage order:
+// their message indices in S.vals[at, at + live) and their rows in S.keys[at, at + live), live (<= bound) in ST_SC_LIVE.
+// S.keys and S.vals are sized for at + 2 * bound here; a caller with pairs below `at` sizes them first, since a buffer
+// that grows does not keep its contents.  tiled: the scans take their multi-launch form.  Nothing is waited for.
+int st_group_rows(tgi_ctx* c, CrawlState& S, const uint32_t* set, uint32_t ns, uint64_t bound, uint64_t at, bool tiled,
+                  uint32_t& launches) {
+  const uint64_t nm = S.n_msgs, nr = S.rows.size();
+  cudaStream_t st = S.stream;
+  int rc;
+  CK(S.flag.ensure(nm * 4));
+  CK(S.pos.ensure((nm + 1) * 8));
+  CK(S.keys.ensure((at + 2 * bound) * 4));
+  CK(S.vals.ensure((at + 2 * bound) * 4));
+  const RadixPlan plan(std::max<uint64_t>(nr, 1) - 1);  // by row
+  uint32_t* flag = S.flag.as<uint32_t>();
+  uint64_t* pos = S.pos.as<uint64_t>();
+  StGroup g{flag, pos};
+  g.keys[plan.out] = S.keys.as<uint32_t>() + at;
+  g.keys[plan.out ^ 1] = S.keys.as<uint32_t>() + at + bound;
+  g.vals[plan.out] = S.vals.as<uint32_t>() + at;
+  g.vals[plan.out ^ 1] = S.vals.as<uint32_t>() + at + bound;
+  const StDev d = st_dev(S);
+  uint64_t* live = S.sc.as<uint64_t>() + ST_SC_LIVE;
+  if (set) st_rows_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, set, ns, flag);
+  else st_live_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, ST_NONE, flag);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, flag, nm, pos, live, launches, tiled))) return rc;
+  st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, g);
+  launches++;
+  return radix_sort(c, st, S.tiles, g.keys, g.vals, live, bound, plan, S.counts, S.roff, S.sc.as<uint64_t>() + ST_SC_RADIX, tiled,
+                    launches);
+}
+
 // the entries' bytes in S.out by the render's two passes, their offsets in S.e64 ([ne+1]); *body = their length,
 // *size_ms = the size pass.  The emit is enqueued behind S.t2 and ends at S.t3, not waited for.
 int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bool lines, const char* who, uint64_t* body,
@@ -3776,51 +3833,19 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
   int rc;
   CK(S.sc.ensure(ST_SC_COUNT * 8));
   CK(S.h_sc.ensure(ST_SC_COUNT * 8));
-  CK(S.flag.ensure(nm * 4));
-  CK(S.pos.ensure((nm + 1) * 8));
-  CK(S.keys.ensure(2 * live * 4));
-  CK(S.vals.ensure(2 * live * 4));
   CK(S.row_base.ensure((nr + 1) * 8));
   CK(S.msize.ensure(live * 4));
   CK(S.moff.ensure((live + 1) * 8));
   StRender r{};
   if ((rc = st_render_bind(c, S, ne, r))) return rc;
-  r.flag = S.flag.as<uint32_t>();
-  r.pos = S.pos.as<uint64_t>();
-  r.keys[0] = S.keys.as<uint32_t>();
-  r.keys[1] = r.keys[0] + live;
-  r.vals[0] = S.vals.as<uint32_t>();
-  r.vals[1] = r.vals[0] + live;
-  // radix passes over the bits of the largest row
-  uint32_t bits = 0;
-  while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
-  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
-  const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
-  CK(S.counts.ensure(radix * ntiles * 4));
-  CK(S.roff.ensure((radix * ntiles + 1) * 8));
   const StDev d = st_dev(S);
   CK(cudaMemcpyAsync(S.entries.p, E.data(), ne * sizeof(StEntry), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(S.sc.p, 0, ST_SC_COUNT * 8, st));
   CK(cudaEventRecord(S.t0, st));
-  st_render_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, r.flag, nm, r.pos, r.sc + ST_SC_LIVE, launches))) return rc;
-  st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, r);
-  launches++;
-  int cur = 0;
-  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
-    const uint32_t shift = p * width;
-    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                   S.counts.as<uint32_t>());
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), r.sc + ST_SC_RADIX, launches))) return rc;
-    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(r.keys[cur], r.vals[cur], r.keys[cur ^ 1], r.vals[cur ^ 1],
-                                                                      r.sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                      S.roff.as<uint64_t>());
-    launches++;
-  }
+  if ((rc = st_group_rows(c, S, nullptr, 0, live, 0, false, launches))) return rc;
+  const uint32_t* sorted = S.vals.as<uint32_t>();
   if ((rc = launch_scan(c, st, S.tiles, d.row_cnt, nr, r.row_base, r.sc + ST_SC_ROWS, launches))) return rc;
-  st_msg_size_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, r, r.vals[cur], r.keys[cur], live);
+  st_msg_size_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, r, sorted, S.keys.as<uint32_t>(), live);
   launches++;
   if ((rc = launch_scan(c, st, S.tiles, r.msize, live, r.moff, r.sc + ST_SC_MBYTES, launches))) return rc;
   (lines ? st_line_size_kernel : st_entry_size_kernel)<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
@@ -3842,7 +3867,7 @@ int st_emit_entries(tgi_ctx* c, CrawlState& S, const std::vector<StEntry>& E, bo
   r.out = S.out.as<uint8_t>();
   CK(cudaEventRecord(S.t2, st));
   (lines ? st_line_emit_kernel : st_entry_emit_kernel)<<<sink_grid(c, ne, ST_WARPS, 16), ST_WARPS * 32, 0, st>>>(d, r);
-  if (slots) st_msg_emit_kernel<<<st_grid(c, slots), ST_THREADS, 0, st>>>(d, r, r.vals[cur]);
+  if (slots) st_msg_emit_kernel<<<st_grid(c, slots), ST_THREADS, 0, st>>>(d, r, sorted);
   launches += 1 + (slots != 0);
   CK(cudaGetLastError());
   CK(cudaEventRecord(S.t3, st));
@@ -3958,8 +3983,8 @@ std::string_view st_view(const CrawlState& S, const tgi_state_page& p, int f) {
 }
 
 // GetPage of n known rows into the pinned read buffers: the records and strings from the host mirror, and with `lists`
-// the rows' message lists from the device.  One pass over the message rows flags the live messages of the distinct
-// rows, the render's stable radix passes group them by row (storage order inside a row) and one gather writes them out;
+// the rows' message lists from the device.  st_group_rows groups the live messages of the distinct rows by row (storage
+// order inside a row) and one gather writes them out;
 // the rows' counts, scanned, place each row's list.  The launches follow the state's row count, not n; two
 // synchronises: the lists' lengths, then the lists.
 int st_read_rows(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint64_t n, bool lists, const char* who, tgi_state_read_t* out) {
@@ -3994,7 +4019,7 @@ int st_read_rows(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint64_t n, bo
   std::sort(set.begin(), set.end());
   set.erase(std::unique(set.begin(), set.end()), set.end());
   const uint32_t ns = (uint32_t)set.size();
-  const uint64_t nm = S.n_msgs, live = nm - S.n_dead, nr = S.rows.size();
+  const uint64_t live = S.n_msgs - S.n_dead;
   if (!n || !live) {
     for (uint64_t k = 0; k < n; k++) first[k] = 0;
     return TGI_OK;
@@ -4005,26 +4030,9 @@ int st_read_rows(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint64_t n, bo
   const size_t o_cnt = 4ull * ns, o_off = 8ull * ns, rbytes = o_off + 8ull * (ns + 1);
   CK(S.rset.ensure(rbytes));
   CK(S.h_rset.ensure(rbytes));
-  uint32_t bits = 0;
-  while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
-  const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0, radix = 1u << width;
-  const uint64_t ntiles = std::max<uint64_t>((live + RS_TILE - 1) / RS_TILE, 1);
-  CK(S.flag.ensure(nm * 4));
-  CK(S.pos.ensure((nm + 1) * 8));
-  CK(S.keys.ensure(2 * live * 4));
-  CK(S.vals.ensure(2 * live * 4));
-  CK(S.counts.ensure(radix * ntiles * 4));
-  CK(S.roff.ensure((radix * ntiles + 1) * 8));
   CK(S.sc.ensure(ST_SC_COUNT * 8));
   CK(S.h_sc.ensure(ST_SC_COUNT * 8));
   CK(S.spare.ensure(live * sizeof(tgi_state_msg)));
-  StRender g{};
-  g.flag = S.flag.as<uint32_t>();
-  g.pos = S.pos.as<uint64_t>();
-  g.keys[0] = S.keys.as<uint32_t>();
-  g.keys[1] = g.keys[0] + live;
-  g.vals[0] = S.vals.as<uint32_t>();
-  g.vals[1] = g.vals[0] + live;
   uint8_t* dr = S.rset.as<uint8_t>();
   const uint32_t* d_set = (const uint32_t*)dr;
   uint32_t* d_cnt = (uint32_t*)(dr + o_cnt);
@@ -4036,28 +4044,11 @@ int st_read_rows(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint64_t n, bo
   const StDev d = st_dev(S);
   uint32_t launches = 0;
   CK(cudaEventRecord(S.t0, st));
-  st_rows_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, d_set, ns, g.flag);
-  launches++;
-  if ((rc = launch_scan(c, st, S.tiles, g.flag, nm, g.pos, sc + ST_SC_LIVE, launches))) return rc;
-  st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, g);
-  launches++;
-  int cur = 0;
-  for (uint32_t p = 0; p < passes; p++, cur ^= 1) {
-    const uint32_t shift = p * width;
-    la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                   S.counts.as<uint32_t>());
-    launches++;
-    if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), sc + ST_SC_RADIX, launches)))
-      return rc;
-    la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], g.vals[cur], g.keys[cur ^ 1], g.vals[cur ^ 1],
-                                                                      sc + ST_SC_LIVE, shift, radix, (uint32_t)ntiles,
-                                                                      S.roff.as<uint64_t>());
-    launches++;
-  }
+  if ((rc = st_group_rows(c, S, d_set, ns, live, 0, false, launches))) return rc;
   st_set_counts_kernel<<<st_grid(c, ns), ST_THREADS, 0, st>>>(d.row_cnt, d_set, ns, d_cnt);
   launches++;
   if ((rc = launch_scan(c, st, S.tiles, d_cnt, ns, d_off, sc + ST_SC_ROWS, launches, true))) return rc;
-  st_gather_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, g.vals[cur], sc + ST_SC_LIVE, S.spare.as<tgi_state_msg>());
+  st_gather_kernel<<<st_grid(c, live), ST_THREADS, 0, st>>>(d, S.vals.as<uint32_t>(), sc + ST_SC_LIVE, S.spare.as<tgi_state_msg>());
   launches++;
   CK(cudaGetLastError());
   CK(cudaEventRecord(S.t1, st));
@@ -5123,43 +5114,11 @@ int st_pages_close(tgi_ctx* c, CrawlState& S, const uint32_t* rows, uint32_t P, 
   std::unique_lock<std::mutex> zg(c->cfg_mu, std::defer_lock);  // the zone table, as in tgi_state_render
   if (json) {
     // the rows without a view render their lists as they are: their live messages, found by a scan of the message rows
-    // and grouped by row with the render's stable radix passes, follow the views' K messages
+    // and grouped by row like the render's, follow the views' K messages
     if (M) {
-      const uint64_t nm = S.n_msgs, nr = S.rows.size();
-      uint32_t bits = 0;
-      while (bits < 32 && nr > 1 && (nr - 1) >> bits) bits++;
-      const uint32_t passes = (bits + 7) / 8, width = passes ? (bits + passes - 1) / passes : 0,
-                     radix = 1u << width;
-      const uint64_t ntiles = std::max<uint64_t>((M + RS_TILE - 1) / RS_TILE, 1);
-      CK(S.flag.ensure(nm * 4));
-      CK(S.pos.ensure((nm + 1) * 8));
-      CK(S.counts.ensure(radix * ntiles * 4));
-      CK(S.roff.ensure((radix * ntiles + 1) * 8));
-      StRender g{};
-      g.flag = S.flag.as<uint32_t>();
-      g.pos = S.pos.as<uint64_t>();
-      const int fin = passes & 1;  // the buffer the last pass writes: right behind the views' messages
-      g.keys[fin] = S.keys.as<uint32_t>() + K;
-      g.keys[fin ^ 1] = S.keys.as<uint32_t>() + K + M;
-      g.vals[fin] = S.vals.as<uint32_t>() + K;
-      g.vals[fin ^ 1] = S.vals.as<uint32_t>() + K + M;
-      uint64_t* cnt = S.sc.as<uint64_t>() + ST_SC_LIVE;
-      st_rows_flag_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, (const uint32_t*)(dseg + o_bare), (uint32_t)bare.size(), g.flag);
-      launches++;
-      if ((rc = launch_scan(c, st, S.tiles, g.flag, nm, g.pos, cnt, launches, tiled))) return rc;
-      st_render_pairs_kernel<<<st_grid(c, nm), ST_THREADS, 0, st>>>(d, nm, g);
-      launches++;
-      for (uint32_t p = 0, cur = 0; p < passes; p++, cur ^= 1) {
-        const uint32_t shift = p * width;
-        la_radix_hist_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], cnt, shift, radix, (uint32_t)ntiles,
-                                                                       S.counts.as<uint32_t>());
-        launches++;
-        if ((rc = launch_scan(c, st, S.tiles, S.counts.as<uint32_t>(), radix * ntiles, S.roff.as<uint64_t>(), S.sc.as<uint64_t>() + ST_SC_RADIX, launches, tiled))) return rc;
-        la_radix_scatter_kernel<<<(unsigned)ntiles, RS_WARPS * 32, 0, st>>>(g.keys[cur], g.vals[cur], g.keys[cur ^ 1], g.vals[cur ^ 1], cnt,
-                                                                          shift, radix, (uint32_t)ntiles, S.roff.as<uint64_t>());
-        launches++;
-      }
-      st_row_starts_kernel<<<st_grid(c, M), ST_THREADS, 0, st>>>(g.keys[fin], cnt, K, S.row_base.as<uint64_t>());
+      if ((rc = st_group_rows(c, S, (const uint32_t*)(dseg + o_bare), (uint32_t)bare.size(), M, K, tiled, launches))) return rc;
+      st_row_starts_kernel<<<st_grid(c, M), ST_THREADS, 0, st>>>(S.keys.as<uint32_t>() + K, S.sc.as<uint64_t>() + ST_SC_LIVE, K,
+                                                                 S.row_base.as<uint64_t>());
       launches++;
       CK(cudaGetLastError());
     }

@@ -57,7 +57,7 @@ def measure(label, batch, yt, n, reps, tmp):
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             appends_call(e, 0)
         for ev in sorted(prof.key_averages(), key=lambda ev: -(getattr(ev, "device_time_total", 0) or 0)):
-            if "la_" not in ev.key and "scan_" not in ev.key:
+            if not any(s in ev.key for s in ("la_", "radix_", "scan_")):
                 continue
             t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
             line = f"  {ev.key[:48]:48s} {t / 1e3:8.3f} ms ({ev.count} launch)"
