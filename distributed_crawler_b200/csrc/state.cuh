@@ -850,11 +850,16 @@ DEVI bool st_same_cand(const StFirst& w, const StCand& a, const StCand& b) {
   return (!w.per_span || a.span == b.span) && key_eq(load_key(a.name), load_key(b.name));
 }
 
+// a candidate's batch-table hash: its key's, mixed with its span when the candidates of each span are kept apart
+DEVI uint64_t st_cand_hash(const Key32& k, uint32_t span, bool per_span) {
+  return key_hash(k) ^ (per_span ? span * 0x9E3779B97F4A7C15ull : 0ull);
+}
+
 __global__ void st_first_kernel(StFirst w) {
   const uint64_t n = *w.n;
   for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const StCand& c = w.c[j];
-    const uint64_t h = key_hash(load_key(c.name)) ^ (w.per_span ? c.span * 0x9E3779B97F4A7C15ull : 0ull);
+    const uint64_t h = st_cand_hash(load_key(c.name), c.span, w.per_span);
     uint64_t s = (h >> 7) & w.bmask;
     for (;; s = (s + 1) & w.bmask) {
       const uint32_t cur = atomicCAS(w.bfirst + s, ST_NONE, (uint32_t)j);
