@@ -308,6 +308,33 @@ class StateValidatorWalkbackC(C.Structure):  # tgi_state_validator_walkback_t
                 ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+# tgi_state_rw_lookups / tgi_state_rw_step: the standard random walk.  Dapr's chatIDCache set, the SearchPublicChat
+# outcome codes, the span statuses past WALK_*, the two upsert kinds, a lookup row, an outcome and a span's step
+SET_SEEDS = 5
+RW_FOUND, RW_NOT_SUPERGROUP, RW_NOT_FOUND, RW_RETIRE = 0, 1, 2, 3
+RW_RETIRED, RW_DEFERRED = 3, 4
+RW_NO_FORWARD = 0xFFFFFFFF
+SQL_SEED_UPSERT, SQL_INVALID_UPSERT = 8, 9
+RW_LOOKUP = np.dtype([("name", "u1", 32), ("record", "<u8"), ("span", "<u4"), ("name_len", "u1"), ("source_type", "u1"),
+                      ("reserved", "<u2")])  # tgi_rw_lookup
+RW_OUTCOME = np.dtype([("chat_id", "<i8"), ("code", "<u4"), ("reserved", "<u4")])  # tgi_rw_outcome
+RW_SPAN = np.dtype([("status", "<u4"), ("walkback", "<u4"), ("rnd", "<i4"), ("draws", "<u4"), ("n_new", "<u4"),
+                    ("forward", "<u4"), ("url_len", "<u4"), ("reserved", "<u4"), ("url", "u1", 32), ("page_id", "S36"),
+                    ("sequence_id", "S36")])  # tgi_rw_span
+assert (RW_LOOKUP.itemsize, RW_OUTCOME.itemsize, RW_SPAN.itemsize) == (48, 16, 136)
+
+
+class StateRwLookupsC(C.Structure):  # tgi_state_rw_lookups_t
+    _fields_ = [("n_candidates", C.c_uint64), ("n_lookups", C.c_uint64), ("lookups", C.c_void_p),
+                ("span_candidates", C.c_void_p), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
+class StateRwStepC(C.Structure):  # tgi_state_rw_step_t
+    _fields_ = [("n_spans", C.c_uint32), ("reserved", C.c_uint32), ("spans", C.c_void_p), ("hits", C.c_uint64 * 4),
+                ("misses", C.c_uint64 * 4), ("n_stmts", C.c_uint64), ("stmts", C.c_void_p), ("data", C.c_void_p),
+                ("data_len", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
 # tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
 SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3

@@ -1030,12 +1030,12 @@ __global__ void st_edge_emit_kernel(StEdges e) {
 }
 
 // ---- tandem hand-off SQL (state/daprstate.go:3643-3678, 3896-3941): the params of every binding call ----------------
-// A SQL call's statements: kind i (TGI_SQL_* kind0 + i) has rows[i] rows, numbered after the kinds before it; a
+// A SQL call's statements: kind i (TGI_SQL_* kind[i]) has rows[i] rows, numbered after the kinds before it; a
 // statement holds k[i] consecutive rows of one kind.  A thread per row: a row is ~200 bytes of short strings (uuids, names,
 // URLs), which the sequential escaper handles without the warp's 128-byte strips idling most lanes.
 constexpr uint32_t ST_SQL_KINDS = 5;  // the most kinds one call renders
 struct StSqlPlan {
-  uint32_t kind0, k[ST_SQL_KINDS];      // the first kind, rows per statement of each kind
+  uint32_t kind[ST_SQL_KINDS], k[ST_SQL_KINDS];  // each kind's TGI_SQL_* code and rows per statement
   uint64_t rows[ST_SQL_KINDS], m[ST_SQL_KINDS];  // rows and statements of each kind (0 past the call's kinds)
   uint64_t n_stmts;
   uint32_t crawl_len, time_len;
@@ -1092,7 +1092,7 @@ DEVI void st_sql_stmts(const StSqlPlan& q) {
     const uint32_t rows = (uint32_t)min((uint64_t)q.k[kind], q.rows[kind] - j * q.k[kind]);
     const uint32_t t = 2 * kind + (rows != q.k[kind]);
     tgi_state_edge_stmt& st = q.stmts[s];
-    st.kind = q.kind0 + kind;
+    st.kind = q.kind[kind];
     st.rows = rows;
     st.sql_off = q.sql_off[t];
     st.sql_len = q.sql_len[t];
@@ -1215,11 +1215,12 @@ DEVI bool st_key_eq(const Key32& key, uint32_t klen, const uint8_t* s, uint32_t 
 
 // pickWalkbackChannel(sm, source, exclude) (crawl/runner.go:120-139) over the set's keys in first-occurrence order
 // (Random() is keys[rand.Intn(len(keys))], state/datamodels.go:152-162): up to 10 draws from r, a draw equal to
-// source[0, sl) or excluded(key, klen) retried.  Returns TGI_WALK_*; key / klen hold the pick when TGI_WALK_OK, else 0.
+// source[0, sl) or excluded(key, klen) retried, over the set's first N keys (N = 0: the set is empty or was never
+// allocated).  Returns TGI_WALK_*; key / klen hold the pick when TGI_WALK_OK, else 0.
+DEVI uint64_t st_set_count(const FrontierDev& disc) { return disc.table ? *disc.count : 0; }
 template <class X>
-DEVI uint32_t st_pick_walkback(StDraws& r, const FrontierDev& disc, const uint8_t* src, uint32_t sl, X&& excluded,
+DEVI uint32_t st_pick_walkback(StDraws& r, const FrontierDev& disc, uint64_t N, const uint8_t* src, uint32_t sl, X&& excluded,
                                Key32& key, uint32_t& klen, uint32_t& draws) {
-  const uint64_t N = disc.table ? *disc.count : 0;
   uint32_t status = N ? TGI_WALK_EXHAUSTED : TGI_WALK_EMPTY;
   key = Key32{};
   klen = draws = 0;
@@ -1247,7 +1248,8 @@ __global__ void st_walk_pick_kernel(StDev d, StWalk w) {
     Key32 key;
     uint32_t draws, klen;
     StDraws r{w.seed, wi, 2u};
-    const uint32_t status = st_pick_walkback(r, w.disc, u, ul, [](const Key32&, uint32_t) { return false; }, key, klen, draws);
+    const uint32_t status = st_pick_walkback(r, w.disc, st_set_count(w.disc), u, ul, [](const Key32&, uint32_t) { return false; },
+                                             key, klen, draws);
     o.span = w.spans[2 * i];
     o.status = status;
     o.draws = draws;
@@ -1388,7 +1390,7 @@ __global__ void st_vw_pick_kernel(StVw v) {
         }
         return false;
       };
-      status = st_pick_walkback(r, v.disc, v.s + b.str_off[TGI_CB_SOURCE_CHANNEL], b.str_len[TGI_CB_SOURCE_CHANNEL],
+      status = st_pick_walkback(r, v.disc, st_set_count(v.disc), v.s + b.str_off[TGI_CB_SOURCE_CHANNEL], b.str_len[TGI_CB_SOURCE_CHANNEL],
                                 excluded, key, klen, draws);
     } else {
       fwd = v.vlist[e0 + r.below(nv)];
@@ -1525,6 +1527,298 @@ __global__ void st_vw_emit_kernel(StDev, StVwSql q) {
   const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3] + q.p.rows[4];
   for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x)
     st_vw_row<true>(q, r, q.p.out + q.p.off[r]);
+  st_sql_stmts(q.p);
+}
+
+// ---- standard random walk (crawl/runner.go:1218-1227, 1245-1384, 1458-1540): lookups, then the replay of a step -----
+// Every name's candidates depend only on its own history, so only its first candidate of the call acts: skipped when
+// the name is invalid or discovered, a seed hit, or a lookup; every later candidate is skipped (the first left the name
+// discovered or invalid, or retired the replay).
+enum : uint32_t { ST_RW_SKIP = 0, ST_RW_SEED = 1, ST_RW_LOOKUP = 2 };
+
+struct StRw {
+  const StCand* c;           // the gather's candidates in (span, record, link) order
+  const uint32_t* link;      // [bound] each candidate's link row in the result
+  const uint64_t* coff;      // [n_spans+1]; coff[n_spans] = the count
+  uint64_t bound;
+  const uint32_t* bfirst;    // st_first_kernel's batch table over the call, and every candidate's slot in it
+  const uint32_t* slot_of;
+  const tgi_state_span* spans;
+  uint32_t n_spans;
+  const uint32_t* link_off;  // the slot's resident result
+  const tgi_link* links;
+  ExclusionDev x;            // TGI_SET_INVALID with the call's clock, TGI_SET_DISCOVERED
+  FrontierDev seeds;         // TGI_SET_SEEDS
+  uint32_t* cls;             // [bound] ST_RW_*
+  uint32_t* flag;            // [bound] 1: a lookup
+  uint64_t* pos;             // [bound+1] scan of flag: each candidate's lookup index
+  tgi_rw_lookup* out;
+};
+
+__global__ void st_rw_class_kernel(StRw r) {
+  const uint64_t n = r.coff[r.n_spans];
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < r.bound; j += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t cl = ST_RW_SKIP;
+    if (j < n && r.bfirst[r.slot_of[j]] == (uint32_t)j) {
+      const Key32 k = load_key(r.c[j].name);
+      const uint64_t h = key_hash(k);
+      if (!set_invalid_hit(r.x, k, h, r.x.now_sec) && set_lookup(r.x.discovered, k, h) < 0)  // :1247, :1310
+        cl = set_lookup(r.seeds, k, h) >= 0 ? ST_RW_SEED : ST_RW_LOOKUP;                      // :1312
+    }
+    r.cls[j] = cl;
+    r.flag[j] = cl == ST_RW_LOOKUP;
+  }
+}
+
+// the lookup rows: name, span, the record that holds the link row, its source
+__global__ void st_rw_lookup_kernel(StRw r) {
+  const uint64_t n = r.coff[r.n_spans];
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (!r.flag[j]) continue;
+    const StCand& c = r.c[j];
+    const uint32_t L = r.link[j];
+    const tgi_state_span s = r.spans[c.span];
+    uint64_t a = s.first, b = s.first + s.n_done - 1;  // the record that holds link row L
+    while (a < b) {
+      const uint64_t mid = (a + b + 1) >> 1;
+      if (r.link_off[mid] <= L) a = mid;
+      else b = mid - 1;
+    }
+    tgi_rw_lookup& o = r.out[r.pos[j]];
+    store_key(o.name, load_key(c.name));
+    o.record = a;
+    o.span = c.span;
+    o.name_len = (uint8_t)c.len;
+    o.source_type = r.links[L].src;
+    o.reserved = 0;
+  }
+}
+
+// The step over the lists of the lookups: lookups [0, nl) apply and so do the candidates before the retiring lookup's
+// (of [0, cut)); spans [0, n_dec) decide, and span n_dec is retired when a lookup retires.
+struct StRwStep {
+  const StCand* c;           // the lookups' lists
+  const uint32_t* cls;
+  const uint64_t* lpos;
+  const uint64_t* coff;
+  const tgi_state_span* spans;
+  uint32_t n_spans, n_dec;
+  const tgi_rw_lookup* lk;
+  const tgi_rw_outcome* oc;
+  uint64_t nl, cut;          // the lookups before the first retire; the candidates
+  uint32_t* flag;            // [2 nl + cut]: found, failed (lookups), discovered insert (candidates)
+  uint64_t* pos;             // [3][...+1] their scans: seed upsert rows, invalid upsert rows, discovered inserts
+  uint64_t* pos_i;
+  uint64_t* pos_d;
+  uint32_t* flist;           // [found] the lookup of every seed upsert row = the newChannels of every span
+  uint32_t* ilist;           // [failed] the lookup of every invalid upsert row
+  uint8_t* fkeys;            // [found][32], [failed][32], [inserts][32]: the three sets' keys in candidate order
+  uint8_t* ikeys;
+  uint8_t* dkeys;
+  const uint32_t* dnew;      // [inserts] 1: the discovered insert added its key
+  const uint64_t* npos;      // [inserts+1] its scan
+  const uint64_t* n0;        // TGI_SET_DISCOVERED's count before the inserts
+  FrontierDev disc;          // TGI_SET_DISCOVERED after them
+  int64_t rate;              // cfg.WalkbackRate
+  uint64_t seed, u0;         // the id key, and the counter of the first deciding span
+  tgi_rw_span* out;          // [n_spans]
+  uint32_t* cnt;             // [2 n_spans]: 1 when the span writes its page; its edge rows
+};
+
+// every lookup's and applied candidate's effects as flags
+__global__ void st_rw_flags_kernel(StRwStep w) {
+  const uint64_t m = max(w.nl, w.cut);
+  for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < m; t += (uint64_t)gridDim.x * blockDim.x) {
+    if (t < w.nl) {
+      const uint32_t o = w.oc[t].code;
+      w.flag[t] = o == TGI_RW_FOUND;
+      w.flag[w.nl + t] = o == TGI_RW_NOT_FOUND || o == TGI_RW_NOT_SUPERGROUP;
+    }
+    if (t < w.cut) {  // candidate t applies when it comes before the retiring lookup: lpos[t + 1] <= nl
+      const uint32_t cl = w.cls[t];
+      const bool applies = w.lpos[t] + (cl == ST_RW_LOOKUP) <= w.nl;
+      w.flag[2 * w.nl + t] = applies && (cl == ST_RW_SEED || (cl == ST_RW_LOOKUP && w.oc[w.lpos[t]].code == TGI_RW_FOUND));
+    }
+  }
+}
+
+// the flagged rows and keys compacted in candidate order
+__global__ void st_rw_compact_kernel(StRwStep w) {
+  const uint64_t m = max(w.nl, w.cut);
+  for (uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t < m; t += (uint64_t)gridDim.x * blockDim.x) {
+    if (t < w.nl && w.flag[t]) {
+      w.flist[w.pos[t]] = (uint32_t)t;
+      store_key(w.fkeys + 32 * w.pos[t], load_key(w.lk[t].name));
+    }
+    if (t < w.nl && w.flag[w.nl + t]) {
+      w.ilist[w.pos_i[t]] = (uint32_t)t;
+      store_key(w.ikeys + 32 * w.pos_i[t], load_key(w.lk[t].name));
+    }
+    if (t < w.cut && w.flag[2 * w.nl + t]) store_key(w.dkeys + 32 * w.pos_d[t], load_key(w.c[t].name));
+  }
+}
+
+// MarkChannelInvalid's stamp of every failed lookup's name, the new ones' and the expired ones' alike
+__global__ void st_rw_stamp_kernel(FrontierDev inv, const uint8_t* keys, uint64_t n, long long now_sec) {
+  for (uint64_t q = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; q < n; q += (uint64_t)gridDim.x * blockDim.x) {
+    const Key32 k = load_key(keys + 32 * q);
+    const int64_t pi = set_lookup(inv, k, key_hash(k));
+    if (pi >= 0) inv.payload[pi] = (uint64_t)now_sec;
+  }
+}
+
+// the discovered insert's NEW flags as scan input
+__global__ void st_rw_new_kernel(const uint8_t* is_new, uint64_t n, uint32_t* out) {
+  for (uint64_t q = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; q < n; q += (uint64_t)gridDim.x * blockDim.x)
+    out[q] = is_new[q];
+}
+
+DEVI const uint8_t* st_rw_name(const StRwStep& w, uint64_t f, uint32_t& len) {  // seed upsert row f's name
+  const tgi_rw_lookup& l = w.lk[w.flist[f]];
+  len = l.name_len;
+  return l.name;
+}
+
+// one span: its newChannels, the decision, the pick, the two ids and its row counts
+__global__ void st_rw_span_kernel(StDev d, StRwStep w) {
+  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < w.n_spans; s += (uint64_t)gridDim.x * blockDim.x) {
+    tgi_rw_span& o = w.out[s];
+    Key32 key{};
+    uint32_t status = s == w.n_dec ? TGI_RW_RETIRED : TGI_RW_DEFERRED, draws = 0, klen = 0, fwd = TGI_RW_NO_FORWARD;
+    uint32_t n_new = 0;
+    int32_t rnd = -1;
+    bool walkback = false;
+    if (s < w.n_dec) {
+      const uint64_t ui = w.u0 + s, c1 = w.coff[s + 1];
+      const uint64_t f0 = w.pos[w.lpos[w.coff[s]]], f1 = w.pos[w.lpos[c1]];
+      n_new = (uint32_t)(f1 - f0);
+      StDraws r{w.seed, ui, 8u};
+      if (n_new) rnd = (int32_t)r.below(100) + 1;
+      walkback = !n_new || w.rate >= rnd;  // :1471-1482
+      if (walkback) {
+        uint32_t ul;
+        const uint8_t* u = st_str(d, d.pages[w.spans[s].row], TGI_PS_URL, ul);
+        auto excluded = [&](const Key32& k, uint32_t kl) {  // exclude = newChannels
+          for (uint64_t f = f0; f < f1; f++) {
+            uint32_t nl;
+            const uint8_t* nm = st_rw_name(w, f, nl);
+            if (st_key_eq(k, kl, nm, nl)) return true;
+          }
+          return false;
+        };
+        const uint64_t N = *w.n0 + w.npos[w.pos_d[c1]];  // the set after this span's candidates
+        status = st_pick_walkback(r, w.disc, N, u, ul, excluded, key, klen, draws);
+      } else {
+        fwd = (uint32_t)r.below(n_new);
+        const tgi_rw_lookup& l = w.lk[w.flist[f0 + fwd]];
+        key = load_key(l.name);
+        klen = l.name_len;
+        status = TGI_WALK_OK;
+      }
+      st_uuid(w.seed, ui, 9u, o.page_id);
+      st_uuid(w.seed, ui, 10u, o.sequence_id);
+    } else {
+      for (int q = 0; q < 36; q++) o.page_id[q] = o.sequence_id[q] = 0;
+    }
+    o.status = status;
+    o.walkback = walkback;
+    o.rnd = rnd;
+    o.draws = draws;
+    o.n_new = n_new;
+    o.forward = fwd;
+    o.url_len = klen;
+    o.reserved = 0;
+    store_key(o.url, key);
+    const bool ok = status == TGI_WALK_OK;
+    w.cnt[s] = ok;
+    w.cnt[w.n_spans + s] = ok ? 1 + n_new - !walkback : 0;  // the primary, then the new channels not followed
+  }
+}
+
+// The SQL of the step: rows of seed upserts, invalid upserts, page_buffer, edge_records.  A page or edge row belongs to
+// the span whose rank range holds it (scans of StRwStep::cnt's two parts).
+struct StRwSql {
+  StSqlPlan p;               // rows {found, failed, pages, edge rows}
+  StRwStep w;
+  const uint64_t* rank;      // [2 (n_spans+1)]
+};
+
+template <bool EMIT>
+DEVI StLen<EMIT> st_rw_row(const StDev& d, const StRwSql& q, uint64_t r, uint8_t* dst) {
+  uint32_t kind = 0;
+  uint64_t j = r;
+  while (j >= q.p.rows[kind]) j -= q.p.rows[kind++];
+  const StRwStep& w = q.w;
+  StSqlRow<EMIT> o{dst, 0};
+  o.open(j, q.p.k[kind]);
+  if (kind == 0) {  // UpsertSeedChannelChatID (daprstate.go:3395-3402)
+    uint32_t nl;
+    const uint8_t* nm = st_rw_name(w, j, nl);
+    o.str(nm, nl);
+    o.lit(",", 1);
+    o.num(w.oc[w.flist[j]].chat_id);
+  } else if (kind == 1) {  // MarkChannelInvalid (:3569-3578)
+    const tgi_rw_lookup& l = w.lk[w.ilist[j]];
+    o.str(l.name, l.name_len);
+    if (w.oc[w.ilist[j]].code == TGI_RW_NOT_FOUND) o.lit(",\"not_found\"", 12);
+    else o.lit(",\"not_supergroup\"", 17);
+  } else {
+    const uint64_t* rank = q.rank + (kind == 3) * (w.n_spans + 1);
+    const uint64_t s = st_vw_batch(rank, w.n_spans, j), x = j - rank[s];  // the span, and the row within its rows
+    const tgi_state_page& p = d.pages[w.spans[s].row];  // the owner
+    const tgi_rw_span& b = w.out[s];
+    if (kind == 2) {  // AddPageToPageBuffer (:3620-3633) of runner.go:1459-1504's page
+      o.str(b.page_id, 36);
+      o.lit(",", 1);
+      o.field(d, p, TGI_PS_ID);
+      o.lit(",", 1);
+      o.num((int64_t)((uint64_t)p.depth + 1));  // owner.Depth + 1 wraps as Go's int
+      o.lit(",", 1);
+      o.str(b.url, b.url_len);
+      o.lit(",", 1);
+      o.str(q.p.crawl, q.p.crawl_len);
+      o.lit(",", 1);
+      if (b.walkback) o.str(b.sequence_id, 36);
+      else o.field(d, p, TGI_PS_SEQ);
+    } else {  // SaveEdgeRecords (:3176-3184): the primary edge, then the skipped ones (runner.go:1505-1535)
+      if (x == 0) {
+        o.str(b.url, b.url_len);
+      } else {
+        const uint64_t f0 = w.pos[w.lpos[w.coff[s]]], y = x - 1;
+        uint32_t nl;
+        const uint8_t* nm = st_rw_name(w, f0 + (y < b.forward ? y : y + 1), nl);  // a walkback's forward is past all
+        o.str(nm, nl);
+      }
+      o.lit(",", 1);
+      o.field(d, p, TGI_PS_URL);
+      if (x) o.lit(",false,true,", 12);
+      else if (b.walkback) o.lit(",true,false,", 12);
+      else o.lit(",false,false,", 13);
+      o.lit(q.p.time, q.p.time_len);
+      o.lit(",", 1);
+      o.str(q.p.crawl, q.p.crawl_len);
+      o.lit(",", 1);
+      o.field(d, p, TGI_PS_SEQ);
+    }
+  }
+  o.close(j, q.p.k[kind], q.p.rows[kind]);
+  return o.o;
+}
+
+__global__ void st_rw_size_kernel(StDev d, StRwSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_rw_row<false>(d, q, r, nullptr);
+    q.p.size[r] = (uint32_t)sz;
+    st_flag_big(q.p.sc, sz);
+  }
+}
+
+// the rows at their scanned offsets, then the statement table
+__global__ void st_rw_emit_kernel(StDev d, StRwSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    st_rw_row<true>(d, q, r, q.p.out + q.p.off[r]);
   st_sql_stmts(q.p);
 }
 

@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstring>
 #include <mutex>
+#include <numeric>
 #include <map>
 #include <memory>
 #include <string>
@@ -268,6 +269,15 @@ struct CrawlState {
   uint64_t vw_next = 0;
   DevBuf vw_b, vw_eoff, vw_e, vw_s, vw_out, vw_list, vw_cnt, vw_rank;
   HostBuf h_vw, h_vw_sql, h_vw_stmts;
+  // standard random walk (tgi_state_rw_lookups / _step): whether the lookups' lists are live (cand, coff and spans
+  // above then hold them, with each candidate's class and lookup index and the lookup rows), their sizes, the counter of
+  // deciding spans, the step's scratch and the pinned outputs
+  bool rw_live = false;
+  uint32_t rw_n_spans = 0;
+  uint64_t rw_n_cand = 0, rw_n_lk = 0, rw_next = 0;
+  DevBuf rw_cls, rw_lpos, rw_lk, rw_oc, rw_flag, rw_pos, rw_list, rw_keys, rw_new, rw_nflag, rw_npos, rw_n0, rw_out,
+      rw_cnt, rw_rank;
+  HostBuf h_rw_lk, h_rw_cand, h_rw_out, h_rw_sql, h_rw_stmts;
   // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
   // device and its staging, and the pinned outputs
   DevBuf rset;
@@ -334,8 +344,8 @@ struct tgi_ctx {
   DevBuf d_zone;
   // the resident key sets, indexed by TGI_SET_*: the dedup set (every key this GPU has seen), the exclusion sets of the
   // frontier -> validator hand-off (tgi_set_add), this rank's partition of the multi-GPU set (tgi_comm_init) and Dapr's
-  // urlCache (tgi_state_discover)
-  KeySet sets[5];
+  // urlCache (tgi_state_discover), Dapr's chatIDCache (tgi_state_rw_step)
+  KeySet sets[6];
   int64_t now_sec = 0;     // tgi_set_now: the clock the TTL of the invalid set is checked against
   uint64_t fr_cap0 = 0;    // tgi_config.frontier_capacity: the size the dedup set started at
   uint64_t grow_max = 0;   // tgi_set_growth: sets grow up to this many keys (0: fixed size)
@@ -598,9 +608,10 @@ int frontier_scratch(tgi_ctx* c, FrontierScratch& z, uint64_t n, uint64_t links,
 }
 
 // The set `which` (TGI_SET_*) names, or nullptr.  With exclusion_only, only the sets the caller fills are named (the
-// tgi_set_add / _clear / _size family: the exclusion sets and the urlCache).
+// tgi_set_add / _clear / _size / _export family: the exclusion sets, the urlCache and the chatIDCache).
 KeySet* key_set(tgi_ctx* c, int which, bool exclusion_only) {
-  if (which == TGI_SET_INVALID || which == TGI_SET_DISCOVERED || which == TGI_SET_URLS) return &c->sets[which];
+  if (which == TGI_SET_INVALID || which == TGI_SET_DISCOVERED || which == TGI_SET_URLS || which == TGI_SET_SEEDS)
+    return &c->sets[which];
   if (!exclusion_only && (which == TGI_SET_FRONTIER || which == TGI_SET_OWNED)) return &c->sets[which];
   return nullptr;
 }
@@ -2578,6 +2589,23 @@ int tgi_set_size(tgi_ctx* c, int which, uint64_t* n) {
   std::lock_guard<std::mutex> g(c->fr_mu);
   return set_count(c, *k, n);
 }
+int tgi_set_export(tgi_ctx* c, int which, uint8_t* keys32, int64_t* stamps_sec, uint64_t cap, uint64_t* n) {
+  if (!c || !n) return TGI_E_ARG;
+  KeySet* k = key_set(c, which, true);
+  if (!k) { set_err(c, "tgi_set_export: unknown set %d", which); return TGI_E_ARG; }
+  if (stamps_sec && which != TGI_SET_INVALID) { set_err(c, "tgi_set_export: only TGI_SET_INVALID has stamps"); return TGI_E_ARG; }
+  cudaSetDevice(c->device);
+  std::lock_guard<std::mutex> g(c->fr_mu);
+  uint64_t sz = 0;
+  if (const int rc = set_count(c, *k, &sz)) return rc;
+  const uint64_t m = std::min(sz, cap);
+  cudaStream_t st = c->slots[0].stream;
+  if (m && keys32) CK(cudaMemcpyAsync(keys32, k->dev.pool, m * 32, cudaMemcpyDeviceToHost, st));
+  if (m && stamps_sec) CK(cudaMemcpyAsync(stamps_sec, k->dev.payload, m * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  *n = sz;
+  return TGI_OK;
+}
 int tgi_set_now(tgi_ctx* c, int64_t now_sec) {
   if (!c) return TGI_E_ARG;
   std::lock_guard<std::mutex> g(c->fr_mu);
@@ -3484,10 +3512,12 @@ bool page_ok(tgi_ctx* c, const tgi_state_page& p, const uint8_t* strs, uint64_t 
 }
 
 // the state's stream, events, preset codes and minimal buffers, on first use (under S.mu).  Every state call but
-// tgi_state_edge_sql passes here, so this is also where the hand-off it renders ends.
+// tgi_state_edge_sql, tgi_state_walkback and tgi_state_rw_step passes here, so this is also where the hand-off and the
+// lookups' lists end.
 int st_init(tgi_ctx* c, CrawlState& S) {
   cudaSetDevice(c->device);
   S.handoff_live = false;
+  S.rw_live = false;
   if (S.stream) return TGI_OK;
   CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
   CK(cudaEventCreate(&S.t0));
@@ -5535,10 +5565,11 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
 
 // The SQL text of a statement of `rows` rows (TGI_SQL_*): for one row the literal of CreatePendingBatch,
 // InsertPendingEdge, ClosePendingBatch, AddPageToPageBuffer, SaveEdgeRecords, CompletePendingBatch or FlushBatchStats'
-// upsert and delete (state/daprstate.go:3897, 3915, 3935, 3620, 3167, 4126, 4163, 4170); for more the VALUES tuple
-// repeated with the placeholders numbered on, or WHERE batch_id IN (...).  The upsert always has one row.
+// upsert and delete, UpsertSeedChannelChatID or MarkChannelInvalid (state/daprstate.go:3897, 3915, 3935, 3620, 3167,
+// 4126, 4163, 4170, 3400, 3576); for more the VALUES tuple repeated with the placeholders numbered on (before the ON
+// CONFLICT clause of the last two), or WHERE batch_id IN (...).  The stats upsert always has one row.
 void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
-  static const char* const head[8] = {
+  static const char* const head[10] = {
       "INSERT INTO pending_edge_batches (batch_id, crawl_id, source_channel, source_page_id, source_depth, sequence_id, "
       "status) VALUES ",
       "INSERT INTO pending_edges (batch_id, crawl_id, destination_channel, source_channel, sequence_id, discovery_time, "
@@ -5553,8 +5584,10 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
       "EXCLUDED.total, valid = source_type_stats.valid + EXCLUDED.valid, not_channel = source_type_stats.not_channel + "
       "EXCLUDED.not_channel, invalid = source_type_stats.invalid + EXCLUDED.invalid, duplicate = "
       "source_type_stats.duplicate + EXCLUDED.duplicate;",
-      "DELETE FROM pending_edges WHERE batch_id "};
-  static const uint32_t per_row[8] = {7, 8, 1, 6, 7, 1, 7, 1};
+      "DELETE FROM pending_edges WHERE batch_id ",
+      "INSERT INTO seed_channels (channel_username, chat_id) VALUES ",
+      "INSERT INTO invalid_channels (channel_username, reason, invalidated_at) VALUES "};
+  static const uint32_t per_row[10] = {7, 8, 1, 6, 7, 1, 7, 1, 2, 2};
   const uint32_t per = per_row[kind];
   s = head[kind];
   if (kind == TGI_SQL_STATS_UPSERT) return;
@@ -5580,8 +5613,11 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
       if (k) s += ", ";
       param(r * per + k + 1);
     }
-    s += ")";
+    s += kind == TGI_SQL_INVALID_UPSERT ? ", NOW())" : ")";
   }
+  if (kind == TGI_SQL_SEED_UPSERT) s += " ON CONFLICT (channel_username) DO UPDATE SET chat_id = EXCLUDED.chat_id";
+  if (kind == TGI_SQL_INVALID_UPSERT)
+    s += " ON CONFLICT (channel_username) DO UPDATE SET reason = EXCLUDED.reason, invalidated_at = NOW()";
   s += ";";
 }
 
@@ -5617,7 +5653,7 @@ int sql_clock(tgi_ctx* c, int64_t now_sec, int32_t now_nsec, const char* who, ch
   return TGI_OK;
 }
 
-// The statements of q.p (kind0, k and rows of its kinds set) over `threads` row threads: their texts on the host (one per kind and
+// The statements of q.p (kind, k and rows of its kinds set) over `threads` row threads: their texts on the host (one per kind and
 // row count, a kind's last statement maybe shorter), crawl_id and the clock tb[0, tl) uploaded, the params by the
 // two-pass writer (accepted() once the size pass has passed), and the texts, params and statement table read back into
 // h and hst.  Adds its device time and launches to out's.
@@ -5636,7 +5672,7 @@ int sql_render(tgi_ctx* c, CrawlState& S, Q& q, void (*size)(StDev, Q), void (*e
     const uint32_t rows[2] = {p.rows[i] >= k ? k : 0u, (uint32_t)(p.rows[i] % k)};
     for (int j = 0; j < 2; j++) {
       if (!rows[j]) continue;
-      edge_sql_text(p.kind0 + i, rows[j], t);
+      edge_sql_text(p.kind[i], rows[j], t);
       p.sql_off[2 * i + j] = texts.size();
       p.sql_len[2 * i + j] = t.size();
       texts += t;
@@ -5967,6 +6003,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
   cudaSetDevice(c->device);  // not st_init: that would end the hand-off
+  S.rw_live = false;
   int rc;
   if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who))) return rc;
   const uint64_t nb = S.handoff_nb, ne = S.handoff_ne;
@@ -5976,7 +6013,7 @@ int tgi_state_edge_sql(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   memset(out, 0, sizeof *out);
   if (!nb) return TGI_OK;
   StSql q{};
-  q.p.kind0 = TGI_SQL_BATCH_INSERT;
+  std::iota(q.p.kind, q.p.kind + ST_SQL_KINDS, (uint32_t)TGI_SQL_BATCH_INSERT);
   std::fill_n(q.p.k, 3, rows_per_stmt);
   q.p.rows[0] = q.p.rows[2] = nb;
   q.p.rows[1] = ne;
@@ -5998,6 +6035,7 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
   CrawlState& S = c->state;
   std::lock_guard<std::mutex> g(S.mu);
   cudaSetDevice(c->device);  // not st_init: that would end the hand-off
+  S.rw_live = false;
   int rc;
   if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who))) return rc;
   const uint64_t n = S.wb_spans.size() / 2;
@@ -6062,7 +6100,7 @@ int tgi_state_walkback(tgi_ctx* c, const char* crawl_id, uint32_t crawl_id_len, 
     return TGI_OK;
   }
   StWalkSql q{};
-  q.p.kind0 = TGI_SQL_PAGE_BUFFER_INSERT;
+  std::iota(q.p.kind, q.p.kind + ST_SQL_KINDS, (uint32_t)TGI_SQL_PAGE_BUFFER_INSERT);
   std::fill_n(q.p.k, 2, rows_per_stmt);
   q.p.rows[0] = q.p.rows[1] = n_ok;
   q.spans = S.wb_in.as<uint32_t>();
@@ -6160,7 +6198,7 @@ int tgi_state_validator_walkback(tgi_ctx* c, const tgi_claimed_batches* in, int6
     return TGI_OK;
   }
   StVwSql q{};
-  q.p.kind0 = TGI_SQL_PAGE_BUFFER_INSERT;
+  std::iota(q.p.kind, q.p.kind + ST_SQL_KINDS, (uint32_t)TGI_SQL_PAGE_BUFFER_INSERT);
   const uint64_t rows[5] = {n_ok, n_edge_rows, n_ok, n_stats, n_ok};
   for (int k = 0; k < 5; k++) {
     q.p.rows[k] = rows[k];
@@ -6170,6 +6208,302 @@ int tgi_state_validator_walkback(tgi_ctx* c, const tgi_claimed_batches* in, int6
   q.rank = rank;
   return sql_render(c, S, q, st_vw_size_kernel, st_vw_emit_kernel, 3 * n_ok + n_edge_rows + n_stats, crawl_id,
                     crawl_id_len, tb, tl, who, accept, S.h_vw_sql, S.h_vw_stmts, out);
+}
+
+// The standard random walk's lookups: the discovery gather, st_first_kernel over the call, the classes under the
+// three sets, a scan and the lookup rows; one synchronise for the totals, one for the read-back.  Lock order: the
+// slot, then the state, then the sets.
+int tgi_state_rw_lookups(tgi_ctx* c, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
+                         tgi_state_rw_lookups_t* out) {
+  static const char* const who = "tgi_state_rw_lookups";
+  if (!c || !out || (n_spans && !spans)) return TGI_E_ARG;
+  if (slot < 0 || slot >= TGI_SLOTS) { set_err(c, "%s: bad slot %d", who, slot); return TGI_E_ARG; }
+  Slot& s = c->slots[slot];
+  std::lock_guard<std::mutex> sl(s.mu);
+  int rc;
+  if ((rc = disc_slot(c, s, slot, who))) return rc;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  if ((rc = st_init(c, S))) return rc;
+  memset(out, 0, sizeof *out);
+  uint64_t bound = 0;
+  if ((rc = disc_bound(c, S, s, spans, n_spans, who, &bound))) return rc;
+  CK(S.h_rw_cand.ensure(std::max<uint64_t>(n_spans, 1) * 8));
+  out->span_candidates = S.h_rw_cand.as<uint64_t>();
+  S.rw_n_spans = n_spans;
+  S.rw_n_cand = S.rw_n_lk = 0;
+  if (!n_spans) {
+    S.rw_live = true;
+    return TGI_OK;
+  }
+  bound = std::max<uint64_t>(bound, 1);  // the step reads the spans and their (empty) offsets from the gather
+  cudaStream_t st = S.stream;
+  const bool tiled = n_spans > 1;  // launches that do not depend on the number of pages
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * bound, 64));
+  CK(S.cand.ensure(bound * sizeof(StCand)));
+  CK(S.bfirst.ensure(bslots * 4));
+  CK(S.slot_of.ensure(bound * 4));
+  CK(S.clink.ensure(bound * 4));
+  CK(S.rw_cls.ensure(bound * 4));
+  CK(S.rw_lpos.ensure((bound + 1) * 8));
+  CK(S.rw_lk.ensure(bound * sizeof(tgi_rw_lookup)));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_coff.ensure((n_spans + 1) * 8));
+  StDisc gd;
+  uint32_t launches = 0;
+  if ((rc = disc_gather(c, S, s, spans, n_spans, bound, S.cand.as<StCand>(), tiled, gd, launches))) return rc;
+  st_edge_link_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(gd, S.clink.as<uint32_t>());
+  launches++;
+  // the first candidate of every name over the whole call
+  StFirst w{};
+  w.c = S.cand.as<StCand>();
+  w.n = gd.coff + n_spans;
+  w.bound = bound;
+  w.dedup = true;
+  w.bfirst = S.bfirst.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.slot_of.as<uint32_t>();
+  CK(cudaMemsetAsync(w.bfirst, 0xFF, bslots * 4, st));
+  st_first_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(w);
+  launches++;
+  StRw r{};  // the gather is done with its flags: the lookups' flags reuse them
+  r.c = w.c;
+  r.link = S.clink.as<uint32_t>();
+  r.coff = gd.coff;
+  r.bound = bound;
+  r.bfirst = w.bfirst;
+  r.slot_of = w.slot_of;
+  r.spans = gd.spans;
+  r.n_spans = n_spans;
+  r.link_off = gd.link_off;
+  r.links = gd.links;
+  r.cls = S.rw_cls.as<uint32_t>();
+  r.flag = gd.flag;
+  r.pos = S.rw_lpos.as<uint64_t>();
+  r.out = S.rw_lk.as<tgi_rw_lookup>();
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [3] lookups
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);  // the three sets: probed by the kernels below, not changed
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    r.x = exclusion(c, now_sec);
+    r.seeds = c->sets[TGI_SET_SEEDS].dev;
+    st_rw_class_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(r);
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, r.flag, bound, r.pos, dsc + 3, launches, tiled))) return rc;
+    st_rw_lookup_kernel<<<st_grid(c, bound), ST_THREADS, 0, st>>>(r);
+    launches++;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t1, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(S.h_coff.p, gd.coff, (n_spans + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  const uint64_t nl = S.h_sc.as<uint64_t>()[3];
+  const uint64_t* coff = S.h_coff.as<uint64_t>();
+  float ms = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  CK(S.h_rw_lk.ensure(std::max<uint64_t>(nl, 1) * sizeof(tgi_rw_lookup)));
+  if (nl) {
+    CK(cudaMemcpyAsync(S.h_rw_lk.p, r.out, nl * sizeof(tgi_rw_lookup), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  for (uint32_t k = 0; k < n_spans; k++) S.h_rw_cand.as<uint64_t>()[k] = coff[k + 1] - coff[k];
+  S.rw_live = true;  // cand, coff, spans, rw_cls, rw_lpos and rw_lk hold the lists until the next state call
+  S.rw_n_cand = coff[n_spans];
+  S.rw_n_lk = nl;
+  out->n_candidates = coff[n_spans];
+  out->n_lookups = nl;
+  out->lookups = S.h_rw_lk.as<tgi_rw_lookup>();
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The standard random walk's step over the last lookups' lists: the outcomes' checks and the retire point on the host;
+// a thread per lookup and candidate flags the effects, three scans, one compaction (one synchronise); the three ordered
+// set inserts on the sets' stream; a thread per span decides and picks over the discovered set as the replay leaves it,
+// two scans place its rows (one synchronise); then the rows as tgi_state_edge_sql renders them.
+int tgi_state_rw_step(tgi_ctx* c, const tgi_rw_outcome* outcomes, uint64_t n_outcomes, int64_t walkback_rate,
+                      const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                      uint32_t rows_per_stmt, tgi_state_rw_step_t* out) {
+  static const char* const who = "tgi_state_rw_step";
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  cudaSetDevice(c->device);  // not st_init: that would end the lists this call reads
+  S.handoff_live = false;    // a state call: a live tandem hand-off ends here
+  int rc;
+  if ((rc = sql_args(c, S, rows_per_stmt, now_nsec, crawl_id, crawl_id_len, who, false))) return rc;
+  if (!S.rw_live) { set_err(c, "%s: no lookups (tgi_state_rw_lookups, then no other state call)", who); return TGI_E_STATE; }
+  const uint64_t n = S.rw_n_lk, nc = S.rw_n_cand;
+  const uint32_t n_spans = S.rw_n_spans;
+  if (n_outcomes != n) { set_err(c, "%s: %llu outcomes for %llu lookups", who, (unsigned long long)n_outcomes, (unsigned long long)n); return TGI_E_ARG; }
+  if (n && !outcomes) { set_err(c, "%s: outcomes is NULL", who); return TGI_E_ARG; }
+  uint64_t nl = n;  // the lookups that apply: those before the first retire
+  for (uint64_t q = 0; q < n; q++) {
+    if (outcomes[q].code > TGI_RW_RETIRE) { set_err(c, "%s: outcome %llu has code %u", who, (unsigned long long)q, outcomes[q].code); return TGI_E_ARG; }
+    if (outcomes[q].code == TGI_RW_RETIRE && nl == n) nl = q;
+  }
+  const tgi_rw_lookup* L = S.h_rw_lk.as<tgi_rw_lookup>();
+  const uint32_t n_dec = nl < n ? L[nl].span : n_spans;  // the deciding spans; span n_dec retired
+  if (n_dec && !S.seeded) { set_err(c, "%s: no id seed (tgi_state_id_seed)", who); return TGI_E_STATE; }
+  char tb[48];
+  uint32_t tl = 0;
+  if (n_dec && (rc = sql_clock(c, now_sec, now_nsec, who, tb, &tl))) return rc;
+  memset(out, 0, sizeof *out);
+  for (uint64_t q = 0; q < nl; q++) {  // lookupStats.record
+    const uint32_t src = L[q].source_type & 3;
+    if (outcomes[q].code == TGI_RW_FOUND) out->hits[src]++;
+    else out->misses[src]++;
+  }
+  out->n_spans = n_spans;
+  if (!n_spans) {
+    S.rw_live = false;
+    return TGI_OK;
+  }
+  cudaStream_t st = S.stream;
+  CK(S.rw_oc.ensure(std::max<uint64_t>(n, 1) * sizeof(tgi_rw_outcome)));
+  CK(S.rw_flag.ensure((2 * nl + nc + 1) * 4));
+  CK(S.rw_pos.ensure((2 * (nl + 1) + nc + 1) * 8));
+  CK(S.rw_list.ensure((2 * nl + 1) * 4));
+  CK(S.rw_keys.ensure((2 * nl + nc + 1) * 32));
+  CK(S.rw_new.ensure(nc + 1));
+  CK(S.rw_nflag.ensure((nc + 1) * 4));
+  CK(S.rw_npos.ensure((nc + 1) * 8));
+  CK(S.rw_n0.ensure(8));
+  CK(S.rw_out.ensure(n_spans * sizeof(tgi_rw_span)));
+  CK(S.rw_cnt.ensure(2 * n_spans * 4));
+  CK(S.rw_rank.ensure(2 * (n_spans + 1) * 8));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_rw_out.ensure(n_spans * sizeof(tgi_rw_span)));
+  if (n) CK(cudaMemcpyAsync(S.rw_oc.p, outcomes, n * sizeof(tgi_rw_outcome), cudaMemcpyHostToDevice, st));
+  StRwStep w{};
+  w.c = S.cand.as<StCand>();
+  w.cls = S.rw_cls.as<uint32_t>();
+  w.lpos = S.rw_lpos.as<uint64_t>();
+  w.coff = S.coff.as<uint64_t>();
+  w.spans = S.spans.as<tgi_state_span>();
+  w.n_spans = n_spans;
+  w.n_dec = n_dec;
+  w.lk = S.rw_lk.as<tgi_rw_lookup>();
+  w.oc = S.rw_oc.as<tgi_rw_outcome>();
+  w.nl = nl;
+  w.cut = nc;  // a candidate applies when the lookups up to it are before the retire: lpos[j + 1] <= nl
+  w.flag = S.rw_flag.as<uint32_t>();
+  w.pos = S.rw_pos.as<uint64_t>();
+  w.pos_i = w.pos + nl + 1;
+  w.pos_d = w.pos_i + nl + 1;
+  w.flist = S.rw_list.as<uint32_t>();
+  w.ilist = w.flist + nl;
+  w.fkeys = S.rw_keys.as<uint8_t>();
+  w.ikeys = w.fkeys + 32 * nl;
+  w.dkeys = w.ikeys + 32 * nl;
+  w.dnew = S.rw_nflag.as<uint32_t>();
+  w.npos = S.rw_npos.as<uint64_t>();
+  w.n0 = S.rw_n0.as<uint64_t>();
+  w.rate = walkback_rate;
+  w.seed = S.id_seed;
+  w.u0 = S.rw_next;
+  w.out = S.rw_out.as<tgi_rw_span>();
+  w.cnt = S.rw_cnt.as<uint32_t>();
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [3] seed upserts, [4] invalid upserts, [5] discovered inserts, [6] pages, [7] edges
+  const uint64_t* hs = S.h_sc.as<uint64_t>();
+  uint32_t launches = 0;
+  const bool tiled = true;  // launches that do not depend on the sizes
+  CK(cudaEventRecord(S.t0, st));
+  st_rw_flags_kernel<<<st_grid(c, std::max(nl, nc)), ST_THREADS, 0, st>>>(w);
+  launches++;
+  if ((rc = launch_scan(c, st, S.tiles, w.flag, nl, w.pos, dsc + 3, launches, tiled))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, w.flag + nl, nl, w.pos_i, dsc + 4, launches, tiled))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, w.flag + 2 * nl, nc, w.pos_d, dsc + 5, launches, tiled))) return rc;
+  st_rw_compact_kernel<<<st_grid(c, std::max(nl, nc)), ST_THREADS, 0, st>>>(w);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0, t = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  const uint64_t n_found = hs[3], n_fail = hs[4], n_ins = hs[5];
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);
+    cudaStream_t st0 = c->slots[0].stream;
+    KeySet& SD = c->sets[TGI_SET_DISCOVERED];
+    KeySet& SI = c->sets[TGI_SET_INVALID];
+    KeySet& SS = c->sets[TGI_SET_SEEDS];
+    // AddDiscoveredChannel of the seed hits and found names in candidate order, after the set's count is kept as N0
+    if (n_ins && (rc = set_first_use(c, SD, false))) return rc;
+    if (SD.dev.table) CK(cudaMemcpyAsync(S.rw_n0.p, SD.dev.count, 8, cudaMemcpyDeviceToDevice, st0));
+    else CK(cudaMemsetAsync(S.rw_n0.p, 0, 8, st0));
+    if (n_ins) {
+      if ((rc = frontier_insert_enqueue(c, SD, w.dkeys, nullptr, n_ins, S.rw_new.p))) return rc;
+      CK(cudaStreamSynchronize(st0));
+      if ((rc = frontier_insert_check(c, SD))) return rc;
+    }
+    // MarkChannelInvalid: the failed names in, then every one of them stamped with the call's clock
+    if (n_fail) {
+      if ((rc = set_first_use(c, SI, true))) return rc;
+      if ((rc = frontier_insert_enqueue(c, SI, w.ikeys, nullptr, n_fail, nullptr))) return rc;
+      CK(cudaStreamSynchronize(st0));
+      if ((rc = frontier_insert_check(c, SI))) return rc;
+      st_rw_stamp_kernel<<<st_grid(c, n_fail), ST_THREADS, 0, st0>>>(SI.dev, w.ikeys, n_fail, (long long)now_sec);
+      launches++;
+    }
+    // UpsertSeedChannelChatID fills chatIDCache
+    if (n_found) {
+      if ((rc = set_first_use(c, SS, false))) return rc;
+      if ((rc = frontier_insert_enqueue(c, SS, w.fkeys, nullptr, n_found, nullptr))) return rc;
+      CK(cudaStreamSynchronize(st0));
+      if ((rc = frontier_insert_check(c, SS))) return rc;
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st0));
+    w.disc = SD.dev;
+    CK(cudaEventRecord(S.t2, st));
+    st_rw_new_kernel<<<st_grid(c, n_ins), ST_THREADS, 0, st>>>(S.rw_new.as<uint8_t>(), n_ins, S.rw_nflag.as<uint32_t>());
+    launches++;
+    if ((rc = launch_scan(c, st, S.tiles, w.dnew, n_ins, S.rw_npos.as<uint64_t>(), dsc + 5, launches, tiled))) return rc;
+    st_rw_span_kernel<<<sink_grid(c, n_spans, ST_THREADS, 4), ST_THREADS, 0, st>>>(st_dev(S), w);
+    launches++;
+    uint64_t* rank = S.rw_rank.as<uint64_t>();
+    for (int k = 0; k < 2; k++)
+      if ((rc = launch_scan(c, st, S.tiles, w.cnt + k * n_spans, n_spans, rank + k * (n_spans + 1), dsc + 6 + k, launches, tiled)))
+        return rc;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(S.t3, st));
+    CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(S.h_rw_out.p, w.out, n_spans * sizeof(tgi_rw_span), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  cudaEventElapsedTime(&t, S.t2, S.t3);
+  ms += t;
+  const uint64_t n_pages = hs[6], n_edges = hs[7];
+  auto accept = [&]() {  // the lists are spent once the call is accepted
+    S.rw_next += n_dec;
+    S.rw_live = false;
+  };
+  out->spans = S.h_rw_out.as<tgi_rw_span>();
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  if (!(n_found + n_fail + n_pages)) {
+    accept();
+    return TGI_OK;
+  }
+  StRwSql q{};
+  q.p.kind[0] = TGI_SQL_SEED_UPSERT;
+  q.p.kind[1] = TGI_SQL_INVALID_UPSERT;
+  q.p.kind[2] = TGI_SQL_PAGE_BUFFER_INSERT;
+  q.p.kind[3] = TGI_SQL_EDGE_RECORD_INSERT;
+  const uint64_t rows[4] = {n_found, n_fail, n_pages, n_edges};
+  for (int k = 0; k < 4; k++) {
+    q.p.rows[k] = rows[k];
+    q.p.k[k] = rows_per_stmt;
+  }
+  q.w = w;
+  q.rank = S.rw_rank.as<uint64_t>();
+  return sql_render(c, S, q, st_rw_size_kernel, st_rw_emit_kernel, n_found + n_fail + n_pages + n_edges, crawl_id,
+                    crawl_id_len, tb, tl, who, accept, S.h_rw_sql, S.h_rw_stmts, out);
 }
 
 }  // extern "C"

@@ -42,7 +42,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_page_close", "tgi_state_id_seed", "tgi_state_discover", "tgi_state_next_layer", "tgi_state_pages_begin",
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
     "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers", "tgi_state_edge_sql",
-    "tgi_state_walkback", "tgi_state_validator_walkback",
+    "tgi_state_walkback", "tgi_state_validator_walkback", "tgi_state_rw_lookups", "tgi_state_rw_step", "tgi_set_export",
 ]
 
 
@@ -138,6 +138,10 @@ def lib() -> C.CDLL:
         L.tgi_state_walkback.argtypes = [vp, C.c_char_p, u32, C.c_int64, i32, u32, C.POINTER(abi.StateWalkbackC)]
         L.tgi_state_validator_walkback.argtypes = [vp, C.POINTER(abi.ClaimedBatchesC), C.c_int64, C.c_char_p, u32,
                                                    C.c_int64, i32, u32, C.POINTER(abi.StateValidatorWalkbackC)]
+        L.tgi_state_rw_lookups.argtypes = [vp, i32, vp, u32, C.c_int64, C.POINTER(abi.StateRwLookupsC)]
+        L.tgi_state_rw_step.argtypes = [vp, vp, u64, C.c_int64, C.c_char_p, u32, C.c_int64, i32, u32,
+                                        C.POINTER(abi.StateRwStepC)]
+        L.tgi_set_export.argtypes = [vp, i32, vp, vp, u64, C.POINTER(u64)]
         _LIB = L
     return _LIB
 
@@ -463,6 +467,17 @@ class Engine:
         n = C.c_uint64()
         self._check(lib().tgi_set_size(self.h, which, C.byref(n)))
         return n.value
+
+    def set_export(self, which: int) -> tuple:
+        """a caller-filled set's keys in first-occurrence order, [n, 32] uint8, and for abi.SET_INVALID their stamps
+        (else None)"""
+        n = C.c_uint64()
+        self._check(lib().tgi_set_export(self.h, which, None, None, 0, C.byref(n)))
+        keys = np.zeros((n.value, 32), np.uint8)
+        stamps = np.zeros(n.value, np.int64) if which == abi.SET_INVALID else None
+        self._check(lib().tgi_set_export(self.h, which, keys.ctypes.data, None if stamps is None else stamps.ctypes.data,
+                                         n.value, C.byref(n)))
+        return keys, stamps
 
     def set_now(self, now_sec: int):
         self._check(lib().tgi_set_now(self.h, now_sec))
@@ -997,6 +1012,49 @@ class Engine:
                     "url": bytes(r["url"][:int(r["url_len"])]), "page_id": bytes(r["page_id"]),
                     "sequence_id": bytes(r["sequence_id"])} for r in res]
         return results, self._st_stmts(out)
+
+    # --- standard random walk: SearchPublicChat lookups, then the step ------------------------------------------------
+    def state_rw_lookups(self, slot: int, spans, now_sec: int = 0) -> dict:
+        """the SearchPublicChat calls of the standard random walk over the slot's last Telegram result: spans = (row,
+        first, n_records, n_done) per owner page, now_sec = the clock of the invalid set's TTL.  Returns {"lookups"
+        (abi.RW_LOOKUP rows), "span_candidates", "n_candidates"}.  The device time is left in self.state_rw_lookups_ms"""
+        sp = np.zeros(max(len(spans), 1), abi.STATE_SPAN)
+        for k, (row, first, n_records, n_done) in enumerate(spans):
+            sp[k] = (row, 0, first, n_records, n_done)
+        out = abi.StateRwLookupsC()
+        self._check(lib().tgi_state_rw_lookups(self.h, slot, sp.ctypes.data, len(spans), now_sec, C.byref(out)))
+        self.state_rw_lookups_ms = float(out.kernel_ms)
+        self.state_rw_lookups_launches = int(out.gpu_launches)
+        return {"lookups": _view(out.lookups, int(out.n_lookups), abi.RW_LOOKUP).copy(),
+                "span_candidates": _view(out.span_candidates, len(spans), np.uint64).copy(),
+                "n_candidates": int(out.n_candidates)}
+
+    def state_rw_step(self, outcomes, walkback_rate: int, crawl_id: bytes, now=(0, 0), rows_per_stmt: int = 1) -> tuple:
+        """the step of the last state_rw_lookups: outcomes = one (code (abi.RW_*), chat_id) per lookup row, or an
+        abi.RW_OUTCOME array.  Returns (spans, stats, stmts): per span {"status" (abi.WALK_* / RW_RETIRED /
+        RW_DEFERRED), "walkback", "rnd", "draws", "n_new", "forward" (None for a walkback), "url", "page_id",
+        "sequence_id"}, {"hits", "misses"} per abi.SRC_NAMES, and [(kind (abi.SQL_*), rows, sql, params)]; the device
+        time and launches are left in self.state_rw_ms and self.state_rw_launches"""
+        if not isinstance(outcomes, np.ndarray):
+            oc = np.zeros(len(outcomes), abi.RW_OUTCOME)
+            for q, (code, chat_id) in enumerate(outcomes):
+                oc[q] = (chat_id, code, 0)
+            outcomes = oc
+        outcomes = np.ascontiguousarray(outcomes, abi.RW_OUTCOME)
+        out = abi.StateRwStepC()
+        self._check(lib().tgi_state_rw_step(self.h, outcomes.ctypes.data if len(outcomes) else None, len(outcomes),
+                                            walkback_rate, crawl_id, len(crawl_id), now[0], now[1], rows_per_stmt,
+                                            C.byref(out)))
+        self.state_rw_ms = float(out.kernel_ms)
+        self.state_rw_launches = int(out.gpu_launches)
+        res = _view(out.spans, int(out.n_spans), abi.RW_SPAN)
+        spans = [{"status": int(r["status"]), "walkback": bool(r["walkback"]), "rnd": int(r["rnd"]),
+                  "draws": int(r["draws"]), "n_new": int(r["n_new"]),
+                  "forward": None if r["forward"] == abi.RW_NO_FORWARD else int(r["forward"]),
+                  "url": bytes(r["url"][:int(r["url_len"])]), "page_id": bytes(r["page_id"]),
+                  "sequence_id": bytes(r["sequence_id"])} for r in res]
+        stats = {"hits": list(out.hits), "misses": list(out.misses)}
+        return spans, stats, self._st_stmts(out)
 
     @staticmethod
     def _st_stmts(out) -> list:

@@ -489,6 +489,24 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return o;
   }
+  // Standard random walk: the SearchPublicChat calls of many pages (RwLookups), then, with one outcome per lookup, the
+  // step (RwStep): the sets' updates, every page's walkback decision and pick (spans[k].status TGI_WALK_*, or
+  // TGI_RW_RETIRED / TGI_RW_DEFERRED past a retiring FLOOD_WAIT) and the exec calls as StateEdgeSql's are read.  The
+  // arrays stay valid until the next state call.
+  tgi_state_rw_lookups_t RwLookups(int slot, const std::vector<tgi_state_span>& spans, int64_t now_sec) {
+    tgi_state_rw_lookups_t o{};
+    if (tgi_state_rw_lookups(ctx_, slot, spans.data(), (uint32_t)spans.size(), now_sec, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  tgi_state_rw_step_t RwStep(const std::vector<tgi_rw_outcome>& outcomes, int64_t walkback_rate, std::string_view crawl_id,
+                             int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt) {
+    tgi_state_rw_step_t o{};
+    if (tgi_state_rw_step(ctx_, outcomes.data(), outcomes.size(), walkback_rate, crawl_id.data(), (uint32_t)crawl_id.size(),
+                          now_sec, now_nsec, rows_per_stmt, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
   // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
   // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.

@@ -1097,6 +1097,7 @@ int tgi_state_pages_close(tgi_ctx* ctx, const uint32_t* rows, uint32_t n_pages, 
  *            result, a result run without TGI_RUN_LINKS, a job in flight on the slot, no seed.  Lock order: the slot,
  *            then the state (as tgi_state_page_end).                                                                */
 #define TGI_SET_URLS 4              /* Dapr's urlCache (daprstate.go:646-658): seeded with tgi_set_add            */
+/* TGI_SET_SEEDS 5, Dapr's chatIDCache, is with tgi_state_rw_lookups below */
 #define TGI_DISCOVER_NOW 1u         /* AddLayer per span now (standalone/runner.go:835-850); else append to pending */
 #define TGI_DISCOVER_DAPR 2u        /* DaprStateManager.AddLayer's rules instead of BaseStateManager's            */
 #define TGI_DISCOVER_PAGE_JSON 4u   /* json.Marshal of every added page (Dapr's per-page SaveState value)         */
@@ -1416,6 +1417,143 @@ typedef struct tgi_state_validator_walkback_t {
 int tgi_state_validator_walkback(tgi_ctx* ctx, const tgi_claimed_batches* in, int64_t walkback_rate, const char* crawl_id,
                                  uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec, uint32_t rows_per_stmt,
                                  tgi_state_validator_walkback_t* out);
+
+/* Standard random walk — the random-walk branch of processAllMessagesWithProcessor without TandemCrawl
+ * (crawl/runner.go:1218-1227, 1245-1384, 1458-1540) for many pages in two calls: tgi_state_rw_lookups lists the
+ * SearchPublicChat calls the pages make; the caller makes them; tgi_state_rw_step applies their outcomes to the three
+ * resident sets, makes every page's walkback decision and pick, and renders the binding calls.  Only the RPC stays with
+ * the caller.
+ *   Spans    as tgi_state_pending_edges's: the owner row, its records of the slot's last result (run with
+ *            TGI_RUN_LINKS), the first n_done processed.  Spans may share records.  They are replayed as if they ran one
+ *            after another in span order (Go runs pages on concurrent goroutines: this is one valid serialisation).
+ *   Candidates  every link row of a processed record with status TGI_ST_EMITTED or TGI_ST_NOLINE, except names
+ *            byte-equal to the owner row's URL (`o == owner.URL`), in (span, record, link row) order.  No FilterUsername.
+ *   Classes  a name's candidates depend only on its own history.  Its first candidate of the call is skipped when the
+ *            name is in TGI_SET_INVALID live at now_sec (IsInvalidChannel) or in TGI_SET_DISCOVERED
+ *            (IsDiscoveredChannel); else it is a seed hit when TGI_SET_SEEDS holds it (GetCachedChatID: Dapr's
+ *            chatIDCache, seeded by the shim from LoadSeedChannels), which only adds it to the discovered set; else it
+ *            is a lookup.  Every later candidate of the name is skipped: after a seed hit or a found lookup the name is
+ *            discovered, after a failed one it is invalid, and a retiring one ends the replay.
+ *   Lookups  tgi_state_rw_lookups: one row per lookup in candidate order, with the name, its span, its record and its
+ *            source_type (msgSourceMap's value: the link row's source), and every span's candidate count.  It changes
+ *            nothing, not even a counter.  Its lists stay on the device for tgi_state_rw_step; any other state call
+ *            ends them, and so does an accepted tgi_state_rw_step.  The classes use the sets as they are at this call.
+ *   Outcomes one per lookup row: TGI_RW_FOUND (a chatTypeSupergroup, with its chat id), TGI_RW_NOT_SUPERGROUP,
+ *            TGI_RW_NOT_FOUND (any non-flood search error), TGI_RW_RETIRE (a FLOOD_WAIT at or above the retire
+ *            threshold).  The caller sleeps and retries short FLOOD_WAITs itself and reports the final outcome.
+ *   Replay   tgi_state_rw_step, in span order: a seed hit does AddDiscoveredChannel; FOUND does AddDiscoveredChannel,
+ *            adds the name to the span's newChannels, emits a seed_channels upsert [name, chat_id] and inserts the name
+ *            into TGI_SET_SEEDS (UpsertSeedChannelChatID fills chatIDCache too); NOT_FOUND / NOT_SUPERGROUP emit an
+ *            invalid_channels upsert [name, "not_found" | "not_supergroup"] and stamp the name into TGI_SET_INVALID at
+ *            now_sec (MarkChannelInvalid: a stamp that expired is replaced).  The first RETIRE ends its span: the
+ *            effects of the span's earlier candidates stand, the span is TGI_RW_RETIRED and writes no page or edge rows.
+ *            Every later span is TGI_RW_DEFERRED: no change and no rows, for the caller to submit again; the outcomes
+ *            of its lookups are not used.  The sets' inserts keep candidate order, so TGI_SET_DISCOVERED's
+ *            first-occurrence order is the replay's.
+ *   Decide   per span that is neither (runner.go:1458-1504): newChannels in first-occurrence order, n_new of them.  With
+ *            n_new = 0 it walks back and rnd = -1; else rnd = IntN(100) + 1 and it walks back iff walkback_rate >= rnd.
+ *            Walkback: pickWalkbackChannel(owner.URL, exclude = newChannels) over the first N_s keys of
+ *            TGI_SET_DISCOVERED, N_s = the set as the replay leaves it after this span's candidates (earlier spans'
+ *            inserts and its own included), with tgi_state_walkback's rule (10 draws; TGI_WALK_EXHAUSTED,
+ *            TGI_WALK_EMPTY); the page takes a new SequenceID.  Forward: idx = IntN(n_new), the page URL is
+ *            newChannels[idx], which leaves the list (order kept); the page takes owner.SequenceID.
+ *   Random   the u-th deciding span under the context (u is not reset by tgi_state_set, and no other call shares its
+ *            counter) draws rnd, the forward index and the walkback draws, in that order, by Lemire's rule from the
+ *            64-bit words of Philox4x32-10 blocks (u_lo, u_hi, 8, j) under the page-id seed.  The page ID and the new
+ *            SequenceID are ids of the page-id construction with counter (u, 9) and (u, 10).  u advances by the
+ *            deciding spans of an accepted call.  Without tgi_state_id_seed a call with a deciding span is TGI_E_STATE.
+ *   Rows     per span: its upserts in candidate order; then, when its pick is TGI_WALK_OK, page_buffer [ID, owner.ID,
+ *            owner.Depth + 1, url, crawl_id, SequenceID] and edge_records: the primary [url, owner.URL, walkback, false,
+ *            discovery_time, crawl_id, owner.SequenceID], then [ch, owner.URL, false, true, discovery_time, crawl_id,
+ *            owner.SequenceID] per remaining new channel in order.  A span whose pick fails keeps its upserts and set
+ *            changes and writes no page or edge rows (Go returns the error after those effects).  The page and its edges
+ *            leave CrawlID empty, so crawl_id is the call's.  Strings, Depth + 1, the clock and the year check are
+ *            tgi_state_walkback's.
+ *   Order    every seed_channels upsert (TGI_SQL_SEED_UPSERT), every invalid_channels upsert (TGI_SQL_INVALID_UPSERT),
+ *            every page_buffer insert, every edge_records insert, each kind in candidate / span order, rows_per_stmt =
+ *            k rows per statement by tgi_state_edge_sql's rule for every kind (the upserts' names are distinct within a
+ *            call, so no ON CONFLICT touches a row twice): "VALUES ($1, $2), ($3, $4) ON CONFLICT ...", an invalid
+ *            tuple "($1, $2, NOW())".  k = 1 gives the reference's calls byte for byte.
+ *   Stats    per TGI_SRC_* the hits (FOUND) and misses (NOT_FOUND, NOT_SUPERGROUP) of the applied lookups:
+ *            lookupStats' counts, for the shim's log lines.
+ *   Cost     lookups: the discovery gather, one first-occurrence table over the call, a thread per candidate classifies
+ *            it, a scan, a thread per lookup writes its row; one synchronise for the totals, one for the read-back.
+ *            step: a thread per lookup and candidate flags the effects, three scans, one compaction (one synchronise);
+ *            the three ordered set inserts; a thread per span decides and picks, two scans (one synchronise); then the
+ *            rows as tgi_state_edge_sql renders them.
+ *   Errors   every check runs before anything changes: a refused call leaves the sets, u and the lists as they were.
+ *            lookups: TGI_E_ARG for an unknown row, a span outside the result, n_done > n_records; TGI_E_STATE for no,
+ *            a released or a non-Telegram result, a result run without TGI_RUN_LINKS, a job in flight on the slot.
+ *            step: TGI_E_ARG for k outside [1, 8191], now_nsec outside [0, 1e9), crawl_id NULL with a length,
+ *            outcomes NULL with lookups, n_outcomes other than the lookups' count, an unknown outcome code, and when a
+ *            span decides a clock whose local year leaves [0, 9999]; TGI_E_STATE for no lists or no seed.  After
+ *            TGI_E_CAPACITY (a set past its capacity or growth limit: each set's insert is all or nothing) or
+ *            TGI_E_CUDA the sets inserted before may hold their keys.  Lock order: the slot, then the state, then the
+ *            sets.  All of out lives in pinned memory until the next state call.                                      */
+#define TGI_SET_SEEDS 5                /* Dapr's chatIDCache (daprstate.go:3375-3411): seeded with tgi_set_add      */
+#define TGI_RW_FOUND 0                 /* SearchPublicChat found a chatTypeSupergroup                                 */
+#define TGI_RW_NOT_SUPERGROUP 1        /* found, another chat type                                                    */
+#define TGI_RW_NOT_FOUND 2             /* any non-flood search error                                                  */
+#define TGI_RW_RETIRE 3                /* FLOOD_WAIT at or above floodWaitRetireThresholdSecs                         */
+#define TGI_RW_RETIRED 3               /* tgi_rw_span.status past TGI_WALK_*: the span met the retiring lookup        */
+#define TGI_RW_DEFERRED 4              /* a span after it: submit it again                                           */
+#define TGI_RW_NO_FORWARD 0xFFFFFFFFu  /* tgi_rw_span.forward of a walkback                                           */
+#define TGI_SQL_SEED_UPSERT 8          /* UpsertSeedChannelChatID                                                    */
+#define TGI_SQL_INVALID_UPSERT 9       /* MarkChannelInvalid                                                          */
+typedef struct tgi_rw_lookup {         /* 48 bytes: one SearchPublicChat call                                         */
+  uint8_t name[32];                    /* the username, zero padded                                                   */
+  uint64_t record;                     /* the result record of the candidate                                          */
+  uint32_t span;
+  uint8_t name_len;
+  uint8_t source_type;                 /* TGI_SRC_*                                                                   */
+  uint16_t reserved;
+} tgi_rw_lookup;
+typedef struct tgi_rw_outcome {        /* 16 bytes                                                                    */
+  int64_t chat_id;                     /* TGI_RW_FOUND: chat.Id                                                       */
+  uint32_t code;                       /* TGI_RW_*                                                                    */
+  uint32_t reserved;
+} tgi_rw_outcome;
+typedef struct tgi_state_rw_lookups_t {
+  uint64_t n_candidates;
+  uint64_t n_lookups;
+  const tgi_rw_lookup* lookups;        /* [n_lookups] in candidate order (pinned)                                     */
+  const uint64_t* span_candidates;     /* [n_spans] (pinned)                                                          */
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies)               */
+  uint32_t gpu_launches;
+} tgi_state_rw_lookups_t;
+typedef struct tgi_rw_span {           /* 136 bytes: one page's step                                                  */
+  uint32_t status;                     /* TGI_WALK_* (a forward pick is TGI_WALK_OK), TGI_RW_RETIRED, TGI_RW_DEFERRED */
+  uint32_t walkback;                   /* 1: walked back                                                              */
+  int32_t rnd;                         /* IntN(100) + 1, or -1 without new channels                                   */
+  uint32_t draws;                      /* walkback draws made                                                         */
+  uint32_t n_new;                      /* len(newChannels)                                                            */
+  uint32_t forward;                    /* the followed channel's index in newChannels, or TGI_RW_NO_FORWARD           */
+  uint32_t url_len;
+  uint32_t reserved;
+  uint8_t url[32];                     /* the next page's URL (TGI_WALK_OK), zero padded                              */
+  uint8_t page_id[36];                 /* the next page's ID                                                          */
+  uint8_t sequence_id[36];             /* the new chain's SequenceID, which the page takes when it walks back         */
+} tgi_rw_span;
+typedef struct tgi_state_rw_step_t {
+  uint32_t n_spans;
+  uint32_t reserved;
+  const tgi_rw_span* spans;            /* [n_spans] (pinned)                                                          */
+  uint64_t hits[4], misses[4];         /* per TGI_SRC_*                                                               */
+  uint64_t n_stmts;
+  const tgi_state_edge_stmt* stmts;    /* [n_stmts] in execution order (pinned)                                       */
+  const uint8_t* data;                 /* the texts, then the params (pinned)                                         */
+  uint64_t data_len;
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies)               */
+  uint32_t gpu_launches;
+} tgi_state_rw_step_t;
+int tgi_state_rw_lookups(tgi_ctx* ctx, int slot, const tgi_state_span* spans, uint32_t n_spans, int64_t now_sec,
+                         tgi_state_rw_lookups_t* out);
+int tgi_state_rw_step(tgi_ctx* ctx, const tgi_rw_outcome* outcomes, uint64_t n_outcomes, int64_t walkback_rate,
+                      const char* crawl_id, uint32_t crawl_id_len, int64_t now_sec, int32_t now_nsec,
+                      uint32_t rows_per_stmt, tgi_state_rw_step_t* out);
+/* tgi_set_export: the first min(count, cap) keys of a caller-filled set (TGI_SET_INVALID, _DISCOVERED, _URLS, _SEEDS)
+ * in first-occurrence order, and with stamps_sec (TGI_SET_INVALID only) their stamps; *n = the set's count. */
+int tgi_set_export(tgi_ctx* ctx, int which, uint8_t* keys32, int64_t* stamps_sec, uint64_t cap, uint64_t* n);
 
 /* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
  * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on
