@@ -335,6 +335,46 @@ class StateRwStepC(C.Structure):  # tgi_state_rw_step_t
                 ("data_len", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
 
 
+# tgi_state_validator_lookups / tgi_state_validator_edges: the validator's edge pass.  A claimed PendingEdge (strings as
+# (offset, length) into one blob), a lookup row, a row's outcome and attempts, an edge's result, and their codes
+VE_STRINGS = ("destination", "crawl_id", "source_type")  # TGI_VE_*
+VA_VALID, VA_NOT_CHANNEL, VA_INVALID, VA_OTHER, VA_TRANSIENT, VA_BLOCKED = 0, 1, 2, 3, 4, 5
+VR_NONE, VR_NOT_SUPERGROUP, VR_NOT_FOUND, VR_CACHED_INVALID, VR_UNKNOWN_STATUS = 0, 1, 2, 3, 4
+VS_PENDING, VS_VALID, VS_DUPLICATE, VS_INVALID, VS_NOT_CHANNEL = 0, 1, 2, 3, 4
+VK_DEFINITIVE, VK_TRANSIENT, VK_BLOCKED = 0, 1, 2
+VR_NAMES = (b"", b"not_supergroup", b"not_found", b"cached_invalid", b"unknown_status")
+VS_NAMES = (b"pending", b"valid", b"duplicate", b"invalid", b"not_channel")
+VE_BLOCKED_THRESHOLD = 5
+VE_NOT_CROSSED = 0xFFFFFFFFFFFFFFFF
+SQL_ACCESS_EVENT, SQL_EDGE_UPDATE = 10, 11
+PENDING_CLAIM_EDGE = np.dtype([("pending_id", "<i8"), ("str_off", "<u8", 3), ("str_len", "<u4", 3),
+                               ("reserved", "<u4")])  # tgi_pending_claim_edge
+VALIDATOR_LOOKUP = np.dtype([("name", "u1", 32), ("occ_off", "<u8"), ("m", "<u4"), ("name_len", "u1"),
+                             ("reserved", "u1", 3)])  # tgi_validator_lookup
+VALIDATOR_OUTCOME = np.dtype([("discovered", "<u4"), ("claimed", "<u4"), ("n_attempts", "<u4"),
+                              ("reserved", "<u4")])  # tgi_validator_outcome
+VALIDATOR_ATTEMPT = np.dtype([("kind", "<u4"), ("reason", "<u4")])  # tgi_validator_attempt
+VALIDATOR_EDGE_RESULT = np.dtype([("blocked_count", "<i8"), ("status", "u1"), ("reason", "u1"), ("kind", "u1"),
+                                  ("reserved", "u1", 5)])  # tgi_validator_edge_result
+assert (PENDING_CLAIM_EDGE.itemsize, VALIDATOR_LOOKUP.itemsize, VALIDATOR_OUTCOME.itemsize, VALIDATOR_ATTEMPT.itemsize,
+        VALIDATOR_EDGE_RESULT.itemsize) == (48, 48, 16, 8, 16)
+
+
+class PendingClaimC(C.Structure):  # tgi_pending_claim
+    _fields_ = [("edges", C.c_void_p), ("n_edges", C.c_uint64), ("strs", C.c_void_p), ("strs_len", C.c_uint64)]
+
+
+class StateValidatorLookupsC(C.Structure):  # tgi_state_validator_lookups_t
+    _fields_ = [("n_edges", C.c_uint64), ("n_cached", C.c_uint64), ("n_lookups", C.c_uint64), ("lookups", C.c_void_p),
+                ("occurrences", C.c_void_p), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
+class StateValidatorEdgesC(C.Structure):  # tgi_state_validator_edges_t
+    _fields_ = [("n_edges", C.c_uint64), ("edges", C.c_void_p), ("blocked_count_out", C.c_int64),
+                ("crossed_at", C.c_uint64), ("n_stmts", C.c_uint64), ("stmts", C.c_void_p), ("data", C.c_void_p),
+                ("data_len", C.c_uint64), ("kernel_ms", C.c_float), ("gpu_launches", C.c_uint32)]
+
+
 READ_MESSAGES = 1  # tgi_state_read_pages / _read_layer: also each page's message list, gathered on the device
 # tgi_state_read_layer's page selection: none, standalone (new execution / resumed), Dapr's processLayerInParallel
 SELECT_NONE, SELECT_STANDALONE, SELECT_STANDALONE_RESUME, SELECT_DAPR = 0, 1, 2, 3

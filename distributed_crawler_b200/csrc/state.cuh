@@ -1822,6 +1822,326 @@ __global__ void st_rw_emit_kernel(StDev d, StRwSql q) {
   st_sql_stmts(q.p);
 }
 
+// ---- validator edge pass (crawl/validator.go:94-309): the lookups of a claim, then its edges' outcomes --------------
+// A name's occurrences share their invalid-cache test, so the claim is grouped by name: a stable sort of the edges by
+// their name's first occurrence puts every name's edges together, in edge order, and the names in first-occurrence
+// order; the names the invalid set decides sort last (key n).
+struct StVe {
+  const tgi_pending_claim_edge* e;  // [n] the claim and its strings as uploaded
+  const uint8_t* s;
+  uint64_t n;
+  uint64_t* d_n;             // n on the device, for the first-occurrence table and the sort
+  StCand* c;                 // [n] every destination as a key
+  const uint32_t* bfirst;    // st_first_kernel's batch table over the claim, and every edge's slot in it
+  const uint32_t* slot_of;
+  ExclusionDev x;            // TGI_SET_INVALID with the call's clock
+  uint32_t* flag;            // [n] 1: the first occurrence of a name the invalid set does not decide
+  uint64_t* lpos;            // [n+1] scan of flag: the name's lookup row
+  const uint64_t* nl;        // its total
+  uint32_t* keys;            // [n] the name's first occurrence, n when the invalid set decides it
+  uint32_t* vals;            // [n] the edge
+  const uint32_t* skeys;     // the sorted pairs
+  const uint32_t* svals;
+  uint64_t* loff;            // [n+1] each lookup row's first sorted edge; loff[nl] = the edges of all rows
+  uint64_t* n_occ;           // that count
+  uint32_t* elk;             // [n] each edge's lookup row, ST_NONE for a cached one
+  uint32_t* rank;            // [n] its occurrence within the row
+  tgi_validator_lookup* out;
+};
+
+DEVI Key32 st_ve_key(const tgi_pending_claim_edge& E, const uint8_t* s) {  // the destination, zero padded
+  const uint8_t* p = s + E.str_off[TGI_VE_DESTINATION];
+  const uint32_t len = E.str_len[TGI_VE_DESTINATION];
+  Key32 k;
+#pragma unroll
+  for (uint32_t i = 0; i < 8; i++) {
+    uint32_t w = 0;
+#pragma unroll
+    for (uint32_t b = 0; b < 4; b++)
+      if (4 * i + b < len) w |= (uint32_t)p[4 * i + b] << (8 * b);
+    k.w[i] = w;
+  }
+  return k;
+}
+
+__global__ void st_ve_key_kernel(StVe v) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < v.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    StCand& c = v.c[j];
+    store_key(c.name, st_ve_key(v.e[j], v.s));
+    c.len = v.e[j].str_len[TGI_VE_DESTINATION];
+    c.parent = c.span = c.reserved = 0;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *v.d_n = v.n;
+}
+
+// IsInvalidChannel (validator.go:206) per edge, the lookup flags and the sort's pairs
+__global__ void st_ve_class_kernel(StVe v) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < v.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const Key32 k = load_key(v.c[j].name);
+    const uint32_t f = v.bfirst[v.slot_of[j]];
+    const bool inv = set_invalid_hit(v.x, k, key_hash(k), v.x.now_sec);
+    v.flag[j] = f == (uint32_t)j && !inv;
+    v.keys[j] = inv ? (uint32_t)v.n : f;
+    v.vals[j] = (uint32_t)j;
+  }
+}
+
+// the first sorted edge of every lookup row, and the end of the rows' edges
+__global__ void st_ve_group_kernel(StVe v) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < v.n; p += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t k = v.skeys[p];
+    if (k == (uint32_t)v.n) continue;
+    if (p == 0 || v.skeys[p - 1] != k) v.loff[v.lpos[k]] = p;
+    if (p + 1 == v.n || v.skeys[p + 1] == (uint32_t)v.n) {
+      v.loff[*v.nl] = p + 1;
+      *v.n_occ = p + 1;
+    }
+  }
+}
+
+// every edge's lookup row and occurrence, and every row from its first occurrence
+__global__ void st_ve_rows_kernel(StVe v) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < v.n; p += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t k = v.skeys[p], j = v.svals[p];
+    if (k == (uint32_t)v.n) {
+      v.elk[j] = ST_NONE;
+      v.rank[j] = 0;
+      continue;
+    }
+    const uint32_t l = (uint32_t)v.lpos[k];
+    const uint64_t r = p - v.loff[l];
+    v.elk[j] = l;
+    v.rank[j] = (uint32_t)r;
+    if (r == 0) {
+      tgi_validator_lookup& o = v.out[l];
+      store_key(o.name, load_key(v.c[j].name));
+      o.occ_off = p;
+      o.m = (uint32_t)(v.loff[l + 1] - p);
+      o.name_len = (uint8_t)v.c[j].len;
+      o.reserved[0] = o.reserved[1] = o.reserved[2] = 0;
+    }
+  }
+}
+
+// The outcomes of the lookup rows applied to every edge of the plan
+struct StVeApply {
+  const tgi_pending_claim_edge* e;  // the plan: the claim, each edge's lookup row and occurrence
+  const uint8_t* s;
+  uint64_t n;
+  const uint32_t* elk;
+  const uint32_t* rank;
+  const tgi_validator_outcome* oc;  // [lookups]
+  const uint64_t* aoff;             // [lookups] each row's first attempt
+  const tgi_validator_attempt* at;
+  int64_t count_in;
+  tgi_validator_edge_result* res;   // [n]
+  uint32_t* flag;                   // [2n] 1: the edge's attempt is a claimed VALID; a NOT_CHANNEL or INVALID
+  uint64_t* pos;                    // [n+1] scan of the first half: the seed upsert rows
+  uint64_t* pos_i;                  // [n+1] of the second: the invalid upsert rows
+  uint32_t* list;                   // [2n] the edge of every seed row, then of every invalid row at n
+  uint8_t* keys;                    // [2n][32] their names, the same way
+  uint64_t* sc;                     // [2] the counter after the claim, the crossing edge
+};
+
+// validateSingleEdge's update and outcome kind of every edge
+__global__ void st_ve_edge_kernel(StVeApply a) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < a.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t st = TGI_VS_INVALID, rs = TGI_VR_CACHED_INVALID, kd = TGI_VK_DEFINITIVE;  // :206-213
+    bool seed = false, inv = false;
+    const uint32_t l = a.elk[j];
+    if (l != ST_NONE) {
+      const tgi_validator_outcome o = a.oc[l];
+      const uint32_t r = a.rank[j];
+      if (o.discovered) {  // :216-226
+        st = TGI_VS_DUPLICATE;
+        rs = TGI_VR_NONE;
+      } else if (r < o.n_attempts) {
+        const tgi_validator_attempt t = a.at[a.aoff[l] + r];
+        rs = TGI_VR_NONE;
+        switch (t.kind) {
+          case TGI_VA_VALID: st = o.claimed ? TGI_VS_VALID : TGI_VS_DUPLICATE; seed = o.claimed; break;  // :260-280
+          case TGI_VA_NOT_CHANNEL: st = TGI_VS_NOT_CHANNEL; rs = t.reason; inv = true; break;             // :282-290
+          case TGI_VA_INVALID: st = TGI_VS_INVALID; rs = t.reason; inv = true; break;                     // :292-300
+          case TGI_VA_OTHER: st = TGI_VS_INVALID; rs = TGI_VR_UNKNOWN_STATUS; break;                      // :304-308
+          case TGI_VA_TRANSIENT: st = TGI_VS_PENDING; kd = TGI_VK_TRANSIENT; break;                        // :229-235, 248-252
+          default: st = TGI_VS_PENDING; kd = TGI_VK_BLOCKED; break;                                        // :241-247
+        }
+      } else if (a.at[a.aoff[l] + o.n_attempts - 1].kind == TGI_VA_VALID) {  // the database has the name now
+        st = TGI_VS_DUPLICATE;
+        rs = TGI_VR_NONE;
+      }  // else MarkChannelInvalid left it in the invalid cache: invalid / cached_invalid
+    }
+    tgi_validator_edge_result& o = a.res[j];
+    o.blocked_count = 0;
+    o.status = (uint8_t)st;
+    o.reason = (uint8_t)rs;
+    o.kind = (uint8_t)kd;
+#pragma unroll
+    for (int q = 0; q < 5; q++) o.reserved[q] = 0;
+    a.flag[j] = seed;
+    a.flag[a.n + j] = inv;
+  }
+}
+
+// The blocked counter's step x -> max(x + a, b) (validator.go:153-176); "f then g" is one such map, so the steps scan.
+// Counts stay within [0, 2^62 + n]; ST_VE_NEG stands for minus infinity and keeps every sum clear of overflow.
+constexpr long long ST_VE_NEG = -(1ll << 61);
+constexpr int ST_VE_THREADS = 1024, ST_VE_ITEMS = 8;
+struct StVeMap {
+  long long a, b;
+};
+DEVI StVeMap st_ve_then(const StVeMap& f, const StVeMap& g) {
+  return {max(f.a + g.a, ST_VE_NEG), max(max(f.b + g.a, g.b), ST_VE_NEG)};
+}
+DEVI StVeMap st_ve_step(uint32_t kind) {
+  return kind == TGI_VK_BLOCKED ? StVeMap{1, ST_VE_NEG} : kind == TGI_VK_TRANSIENT ? StVeMap{-1, 0} : StVeMap{ST_VE_NEG, 0};
+}
+DEVI StVeMap st_ve_shfl_up(const StVeMap& f, int d) {
+  return {(long long)__shfl_up_sync(FULL, f.a, d), (long long)__shfl_up_sync(FULL, f.b, d)};
+}
+
+// One block: every edge's count after it, the first blocked edge that reaches the threshold, and the final count.
+// A pass covers ST_VE_ITEMS consecutive edges per thread; the count before a pass carries to the next.
+__global__ void __launch_bounds__(ST_VE_THREADS) st_ve_counter_kernel(StVeApply a) {
+  __shared__ StVeMap wsum[32];
+  __shared__ long long carry;
+  __shared__ unsigned long long crossed;
+  const int l = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    carry = a.count_in;
+    crossed = TGI_VE_NOT_CROSSED;
+  }
+  __syncthreads();
+  const StVeMap id{0, ST_VE_NEG};
+  for (uint64_t base = 0; base < a.n; base += (uint64_t)ST_VE_THREADS * ST_VE_ITEMS) {
+    const uint64_t j0 = base + (uint64_t)threadIdx.x * ST_VE_ITEMS;
+    StVeMap f = id;
+    for (int q = 0; q < ST_VE_ITEMS; q++)
+      if (j0 + q < a.n) f = st_ve_then(f, st_ve_step(a.res[j0 + q].kind));
+    StVeMap x = f;  // inclusive over the warp
+    for (int d = 1; d < 32; d <<= 1) {
+      const StVeMap t = st_ve_shfl_up(x, d);
+      if (l >= d) x = st_ve_then(t, x);
+    }
+    if (l == 31) wsum[w] = x;
+    __syncthreads();
+    if (w == 0) {
+      StVeMap y = wsum[l];
+      for (int d = 1; d < 32; d <<= 1) {
+        const StVeMap t = st_ve_shfl_up(y, d);
+        if (l >= d) y = st_ve_then(t, y);
+      }
+      wsum[l] = y;
+    }
+    __syncthreads();
+    StVeMap ex = st_ve_shfl_up(x, 1);  // the threads before this one
+    if (l == 0) ex = id;
+    if (w) ex = st_ve_then(wsum[w - 1], ex);
+    const long long c0 = carry;
+    long long cnt = max(c0 + ex.a, ex.b);
+    for (int q = 0; q < ST_VE_ITEMS && j0 + q < a.n; q++) {
+      const uint32_t kd = a.res[j0 + q].kind;
+      const StVeMap s = st_ve_step(kd);
+      cnt = max(cnt + s.a, s.b);
+      a.res[j0 + q].blocked_count = cnt;
+      if (kd == TGI_VK_BLOCKED && cnt >= TGI_VE_BLOCKED_THRESHOLD) atomicMin(&crossed, (unsigned long long)(j0 + q));
+    }
+    __syncthreads();
+    if (threadIdx.x == ST_VE_THREADS - 1) carry = max(c0 + wsum[31].a, wsum[31].b);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    a.sc[0] = (uint64_t)carry;
+    a.sc[1] = crossed;
+  }
+}
+
+// the seed and invalid upsert rows' edges and names, in edge order
+__global__ void st_ve_compact_kernel(StVeApply a) {
+  for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j < a.n; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (a.flag[j]) {
+      a.list[a.pos[j]] = (uint32_t)j;
+      store_key(a.keys + 32 * a.pos[j], st_ve_key(a.e[j], a.s));
+    }
+    if (a.flag[a.n + j]) {
+      a.list[a.n + a.pos_i[j]] = (uint32_t)j;
+      store_key(a.keys + 32 * (a.n + a.pos_i[j]), st_ve_key(a.e[j], a.s));
+    }
+  }
+}
+
+// The SQL of the pass: rows of seed upserts, invalid upserts, the access event, pending_edges updates
+struct StVeSql {
+  StSqlPlan p;
+  StVeApply a;
+};
+
+template <bool EMIT>
+DEVI void st_ve_reason(StSqlRow<EMIT>& o, uint32_t r) {  // a TGI_VR_* as its JSON string
+  switch (r) {
+    case TGI_VR_NOT_SUPERGROUP: o.lit("\"not_supergroup\"", 16); break;
+    case TGI_VR_NOT_FOUND: o.lit("\"not_found\"", 11); break;
+    case TGI_VR_CACHED_INVALID: o.lit("\"cached_invalid\"", 16); break;
+    case TGI_VR_UNKNOWN_STATUS: o.lit("\"unknown_status\"", 16); break;
+    default: o.lit("\"\"", 2); break;
+  }
+}
+
+template <bool EMIT>
+DEVI StLen<EMIT> st_ve_row(const StVeSql& q, uint64_t r, uint8_t* dst) {
+  uint32_t kind = 0;
+  uint64_t j = r;
+  while (j >= q.p.rows[kind]) j -= q.p.rows[kind++];
+  const StVeApply& a = q.a;
+  StSqlRow<EMIT> o{dst, 0};
+  o.open(j, q.p.k[kind]);
+  if (kind < 2) {  // UpsertSeedChannelChatID(name, 0) (daprstate.go:3395-3402), MarkChannelInvalid (:3569-3578)
+    const uint32_t e = a.list[kind * a.n + j];
+    const tgi_pending_claim_edge& E = a.e[e];
+    o.str(a.s + E.str_off[TGI_VE_DESTINATION], E.str_len[TGI_VE_DESTINATION]);
+    if (kind == 0) {
+      o.lit(",0", 2);
+    } else {
+      o.lit(",", 1);
+      st_ve_reason(o, a.res[e].reason);
+    }
+  } else if (kind == 2) {  // InsertAccessEvent("ip_blocked") (:4385-4391)
+    o.lit("\"ip_blocked\"", 12);
+  } else {  // UpdatePendingEdge (:3999-4006): [status, reason, pending_id]
+    const tgi_validator_edge_result& x = a.res[j];
+    switch (x.status) {
+      case TGI_VS_VALID: o.lit("\"valid\"", 7); break;
+      case TGI_VS_DUPLICATE: o.lit("\"duplicate\"", 11); break;
+      case TGI_VS_INVALID: o.lit("\"invalid\"", 9); break;
+      case TGI_VS_NOT_CHANNEL: o.lit("\"not_channel\"", 13); break;
+      default: o.lit("\"pending\"", 9); break;
+    }
+    o.lit(",", 1);
+    st_ve_reason(o, x.reason);
+    o.lit(",", 1);
+    o.num(a.e[j].pending_id);
+  }
+  o.close(j, q.p.k[kind], q.p.rows[kind]);
+  return o.o;
+}
+
+__global__ void st_ve_size_kernel(StDev, StVeSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t sz = st_ve_row<false>(q, r, nullptr);
+    q.p.size[r] = (uint32_t)sz;
+    st_flag_big(q.p.sc, sz);
+  }
+}
+
+// the rows at their scanned offsets, then the statement table
+__global__ void st_ve_emit_kernel(StDev, StVeSql q) {
+  const uint64_t n_rows = q.p.rows[0] + q.p.rows[1] + q.p.rows[2] + q.p.rows[3];
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_rows; r += (uint64_t)gridDim.x * blockDim.x)
+    st_ve_row<true>(q, r, q.p.out + q.p.off[r]);
+  st_sql_stmts(q.p);
+}
+
 // ---- json.Marshal(map[int][]string) of the layer map ----------------------------------------------------------------
 struct StLmEntry {  // one id of a layer, or an empty layer (row == ST_NONE)
   uint32_t row;

@@ -278,6 +278,14 @@ struct CrawlState {
   DevBuf rw_cls, rw_lpos, rw_lk, rw_oc, rw_flag, rw_pos, rw_list, rw_keys, rw_new, rw_nflag, rw_npos, rw_n0, rw_out,
       rw_cnt, rw_rank;
   HostBuf h_rw_lk, h_rw_cand, h_rw_out, h_rw_sql, h_rw_stmts;
+  // validator edge pass (tgi_state_validator_lookups / _edges): whether a plan is live (only the next lookups or an
+  // accepted pass ends it, so its buffers are its own), its claim, lookup rows and each edge's row and occurrence on the
+  // device, the lookup rows on the host, the pass's scratch and the pinned outputs
+  bool ve_live = false;
+  uint64_t ve_n = 0, ve_nl = 0;
+  DevBuf ve_e, ve_s, ve_cand, ve_bfirst, ve_slot, ve_flag, ve_lpos, ve_keys, ve_vals, ve_loff, ve_elk, ve_rank, ve_lk;
+  DevBuf ve_oc, ve_aoff, ve_at, ve_res, ve_pos, ve_list, ve_names;
+  HostBuf h_ve_lk, h_ve_occ, h_ve_aoff, h_ve_res, h_ve_sql, h_ve_stmts;
   // page reads (tgi_state_read_pages / _read_layer, tgi_state_layers): the read set with its counts and offsets on the
   // device and its staging, and the pinned outputs
   DevBuf rset;
@@ -5565,11 +5573,25 @@ int st_discover_apply(tgi_ctx* c, CrawlState& S, const std::vector<DiscGroup>& G
 
 // The SQL text of a statement of `rows` rows (TGI_SQL_*): for one row the literal of CreatePendingBatch,
 // InsertPendingEdge, ClosePendingBatch, AddPageToPageBuffer, SaveEdgeRecords, CompletePendingBatch or FlushBatchStats'
-// upsert and delete, UpsertSeedChannelChatID or MarkChannelInvalid (state/daprstate.go:3897, 3915, 3935, 3620, 3167,
-// 4126, 4163, 4170, 3400, 3576); for more the VALUES tuple repeated with the placeholders numbered on (before the ON
-// CONFLICT clause of the last two), or WHERE batch_id IN (...).  The stats upsert always has one row.
+// upsert and delete, UpsertSeedChannelChatID, MarkChannelInvalid, InsertAccessEvent or UpdatePendingEdge
+// (state/daprstate.go:3897, 3915, 3935, 3620, 3167, 4126, 4163, 4170, 3400, 3576, 4386, 4001); for more the VALUES tuple
+// repeated with the placeholders numbered on (before the ON CONFLICT clause of the upserts), WHERE batch_id IN (...), or
+// the update's join on a VALUES list.  The stats upsert and the access event always have one row.
 void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
-  static const char* const head[10] = {
+  if (kind == TGI_SQL_EDGE_UPDATE) {  // UpdatePendingEdge (daprstate.go:4001); more rows join a VALUES list on the id
+    if (rows == 1) {
+      s = "UPDATE pending_edges SET validation_status = $1, validation_reason = $2, validated_at = NOW() WHERE pending_id = $3;";
+      return;
+    }
+    s = "UPDATE pending_edges AS e SET validation_status = v.s, validation_reason = v.r, validated_at = NOW() FROM (VALUES ";
+    for (uint32_t r = 0; r < rows; r++) {
+      s += r ? ", ($" : "($";
+      s += std::to_string(3 * r + 1) + ", $" + std::to_string(3 * r + 2) + ", $" + std::to_string(3 * r + 3) + "::integer)";
+    }
+    s += ") AS v(s, r, id) WHERE e.pending_id = v.id;";
+    return;
+  }
+  static const char* const head[11] = {
       "INSERT INTO pending_edge_batches (batch_id, crawl_id, source_channel, source_page_id, source_depth, sequence_id, "
       "status) VALUES ",
       "INSERT INTO pending_edges (batch_id, crawl_id, destination_channel, source_channel, sequence_id, discovery_time, "
@@ -5586,8 +5608,9 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
       "source_type_stats.duplicate + EXCLUDED.duplicate;",
       "DELETE FROM pending_edges WHERE batch_id ",
       "INSERT INTO seed_channels (channel_username, chat_id) VALUES ",
-      "INSERT INTO invalid_channels (channel_username, reason, invalidated_at) VALUES "};
-  static const uint32_t per_row[10] = {7, 8, 1, 6, 7, 1, 7, 1, 2, 2};
+      "INSERT INTO invalid_channels (channel_username, reason, invalidated_at) VALUES ",
+      "INSERT INTO access_events (reason, occurred_at) VALUES "};
+  static const uint32_t per_row[11] = {7, 8, 1, 6, 7, 1, 7, 1, 2, 2, 1};
   const uint32_t per = per_row[kind];
   s = head[kind];
   if (kind == TGI_SQL_STATS_UPSERT) return;
@@ -5613,7 +5636,7 @@ void edge_sql_text(uint32_t kind, uint32_t rows, std::string& s) {
       if (k) s += ", ";
       param(r * per + k + 1);
     }
-    s += kind == TGI_SQL_INVALID_UPSERT ? ", NOW())" : ")";
+    s += kind == TGI_SQL_INVALID_UPSERT || kind == TGI_SQL_ACCESS_EVENT ? ", NOW())" : ")";
   }
   if (kind == TGI_SQL_SEED_UPSERT) s += " ON CONFLICT (channel_username) DO UPDATE SET chat_id = EXCLUDED.chat_id";
   if (kind == TGI_SQL_INVALID_UPSERT)
@@ -5748,6 +5771,61 @@ int vw_input(tgi_ctx* c, const tgi_claimed_batches* in, const char* who) {
     for (int f = 0; f < 2; f++)
       if (out_of(E.str_off[f], E.str_len[f])) { set_err(c, "%s: edge %llu string %d outside strs", who, (unsigned long long)j, f); return TGI_E_ARG; }
   }
+  return TGI_OK;
+}
+
+// A claim's checks (TGI_E_ARG): its arrays, strings, destinations and pending_ids, before anything is uploaded
+int ve_input(tgi_ctx* c, const tgi_pending_claim* in, const char* who) {
+  const uint64_t n = in->n_edges, sl = in->strs_len;
+  if (n && !in->edges) { set_err(c, "%s: edges is NULL", who); return TGI_E_ARG; }
+  if (sl && !in->strs) { set_err(c, "%s: strs is NULL", who); return TGI_E_ARG; }
+  if (n >= ST_NONE) { set_err(c, "%s: a claim of 2^32 - 1 edges or more", who); return TGI_E_ARG; }
+  std::vector<int64_t> ids(n);
+  for (uint64_t j = 0; j < n; j++) {
+    const tgi_pending_claim_edge& E = in->edges[j];
+    for (int f = 0; f < 3; f++)
+      if (E.str_off[f] > sl || E.str_len[f] > sl - E.str_off[f]) {
+        set_err(c, "%s: edge %llu string %d outside strs", who, (unsigned long long)j, f);
+        return TGI_E_ARG;
+      }
+    const uint32_t dl = E.str_len[TGI_VE_DESTINATION];
+    if (dl < 1 || dl > 32) { set_err(c, "%s: edge %llu has a destination of %u bytes (1 to 32)", who, (unsigned long long)j, dl); return TGI_E_ARG; }
+    ids[j] = E.pending_id;
+  }
+  std::sort(ids.begin(), ids.end());
+  const auto d = std::adjacent_find(ids.begin(), ids.end());
+  if (d != ids.end()) { set_err(c, "%s: pending_id %lld twice in the claim", who, (long long)*d); return TGI_E_ARG; }
+  return TGI_OK;
+}
+
+// The outcomes' checks (TGI_E_ARG) against the plan's lookup rows L; aoff[l] = row l's first attempt
+int ve_outcomes(tgi_ctx* c, const tgi_validator_lookup* L, const tgi_validator_outcome* oc, uint64_t n,
+                const tgi_validator_attempt* at, uint64_t n_at, uint64_t* aoff, const char* who) {
+  uint64_t a = 0;
+  auto bad = [&](uint64_t l, const char* what) {
+    set_err(c, "%s: lookup %llu: %s", who, (unsigned long long)l, what);
+    return TGI_E_ARG;
+  };
+  auto final_kind = [](uint32_t k) { return k == TGI_VA_VALID || k == TGI_VA_NOT_CHANNEL || k == TGI_VA_INVALID; };
+  for (uint64_t l = 0; l < n; l++) {
+    const tgi_validator_outcome& o = oc[l];
+    const uint32_t na = o.n_attempts;
+    if (o.discovered > 1 || o.claimed > 1) return bad(l, "discovered or claimed past 1");
+    if (na > n_at - a) return bad(l, "more attempts than n_attempts holds");
+    aoff[l] = a;
+    if (o.discovered && na) return bad(l, "discovered with attempts");
+    if (!o.discovered && (!na || na > L[l].m)) return bad(l, "no attempt, or more attempts than occurrences");
+    for (uint32_t q = 0; q < na; q++) {
+      const tgi_validator_attempt& t = at[a + q];
+      if (t.kind > TGI_VA_BLOCKED || t.reason > TGI_VR_NOT_FOUND) return bad(l, "an unknown attempt kind or reason");
+      if (final_kind(t.kind) && q + 1 < na) return bad(l, "a final attempt before the last one");
+    }
+    const bool last_final = na && final_kind(at[a + na - 1].kind);
+    if (na && !last_final && na < L[l].m) return bad(l, "a last attempt that is not final while fewer than m were made");
+    if (o.claimed && !(na && at[a + na - 1].kind == TGI_VA_VALID)) return bad(l, "claimed without a final VALID");
+    a += na;
+  }
+  if (a != n_at) { set_err(c, "%s: the rows make %llu attempts, n_attempts is %llu", who, (unsigned long long)a, (unsigned long long)n_at); return TGI_E_ARG; }
   return TGI_OK;
 }
 
@@ -6504,6 +6582,252 @@ int tgi_state_rw_step(tgi_ctx* c, const tgi_rw_outcome* outcomes, uint64_t n_out
   q.rank = S.rw_rank.as<uint64_t>();
   return sql_render(c, S, q, st_rw_size_kernel, st_rw_emit_kernel, n_found + n_fail + n_pages + n_edges, crawl_id,
                     crawl_id_len, tb, tl, who, accept, S.h_rw_sql, S.h_rw_stmts, out);
+}
+
+// The validator edge pass's lookups: the upload, a thread per edge builds its key, st_first_kernel over the claim, a
+// thread per edge classifies it against the invalid set, a scan, the stable radix sort by first occurrence, a thread
+// per sorted edge places the rows and occurrences; one synchronise for the totals, one for the read-back.  Lock order:
+// the state, then the sets.
+int tgi_state_validator_lookups(tgi_ctx* c, const tgi_pending_claim* claim, int64_t now_sec,
+                                tgi_state_validator_lookups_t* out) {
+  static const char* const who = "tgi_state_validator_lookups";
+  if (!c || !out || !claim) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if ((rc = ve_input(c, claim, who))) return rc;
+  const uint64_t n = claim->n_edges;
+  memset(out, 0, sizeof *out);
+  S.ve_live = false;  // the plan before is gone from here
+  S.ve_n = n;
+  S.ve_nl = 0;
+  if (!n) {
+    S.ve_live = true;
+    return TGI_OK;
+  }
+  cudaStream_t st = S.stream;
+  const uint64_t bslots = next_pow2(std::max<uint64_t>(2 * n, 64));
+  CK(S.ve_e.ensure(n * sizeof(tgi_pending_claim_edge)));
+  CK(S.ve_s.ensure(std::max<uint64_t>(claim->strs_len, 1)));
+  CK(S.ve_cand.ensure(n * sizeof(StCand)));
+  CK(S.ve_bfirst.ensure(bslots * 4));
+  CK(S.ve_slot.ensure(n * 4));
+  CK(S.ve_flag.ensure(2 * n * 4));
+  CK(S.ve_lpos.ensure((n + 1) * 8));
+  CK(S.ve_keys.ensure(2 * n * 4));
+  CK(S.ve_vals.ensure(2 * n * 4));
+  CK(S.ve_loff.ensure((n + 1) * 8));
+  CK(S.ve_elk.ensure(n * 4));
+  CK(S.ve_rank.ensure(n * 4));
+  CK(S.ve_lk.ensure(n * sizeof(tgi_validator_lookup)));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(cudaMemcpyAsync(S.ve_e.p, claim->edges, n * sizeof(tgi_pending_claim_edge), cudaMemcpyHostToDevice, st));
+  if (claim->strs_len) CK(cudaMemcpyAsync(S.ve_s.p, claim->strs, claim->strs_len, cudaMemcpyHostToDevice, st));
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [3] lookup rows, [4] their edges, [5] the sort's digit total, [6] n
+  StVe v{};
+  v.e = S.ve_e.as<tgi_pending_claim_edge>();
+  v.s = S.ve_s.as<uint8_t>();
+  v.n = n;
+  v.d_n = dsc + 6;
+  v.c = S.ve_cand.as<StCand>();
+  v.flag = S.ve_flag.as<uint32_t>();
+  v.lpos = S.ve_lpos.as<uint64_t>();
+  v.nl = dsc + 3;
+  v.n_occ = dsc + 4;
+  v.loff = S.ve_loff.as<uint64_t>();
+  v.elk = S.ve_elk.as<uint32_t>();
+  v.rank = S.ve_rank.as<uint32_t>();
+  v.out = S.ve_lk.as<tgi_validator_lookup>();
+  const RadixPlan plan(n);  // by first occurrence; n for the names the invalid set decides
+  uint32_t* keys[2] = {S.ve_keys.as<uint32_t>(), S.ve_keys.as<uint32_t>() + n};
+  uint32_t* vals[2] = {S.ve_vals.as<uint32_t>(), S.ve_vals.as<uint32_t>() + n};
+  v.keys = keys[0];
+  v.vals = vals[0];
+  v.skeys = keys[plan.out];
+  v.svals = vals[plan.out];
+  uint32_t launches = 0;
+  CK(cudaEventRecord(S.t0, st));
+  st_ve_key_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(v);
+  launches++;
+  StFirst w{};  // the first occurrence of every name over the claim
+  w.c = v.c;
+  w.n = v.d_n;
+  w.bound = n;
+  w.dedup = true;
+  w.bfirst = S.ve_bfirst.as<uint32_t>();
+  w.bmask = bslots - 1;
+  w.slot_of = S.ve_slot.as<uint32_t>();
+  CK(cudaMemsetAsync(w.bfirst, 0xFF, bslots * 4, st));
+  st_first_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(w);
+  launches++;
+  v.bfirst = w.bfirst;
+  v.slot_of = w.slot_of;
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);  // the invalid set: probed, not changed
+    if (c->fr_event_valid) CK(cudaStreamWaitEvent(st, c->fr_event, 0));
+    v.x = exclusion(c, now_sec);
+    st_ve_class_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(v);
+    launches++;
+    CK(cudaGetLastError());
+  }
+  if ((rc = launch_scan(c, st, S.tiles, v.flag, n, v.lpos, dsc + 3, launches, true))) return rc;
+  if ((rc = radix_sort(c, st, S.tiles, keys, vals, v.d_n, n, plan, S.counts, S.roff, dsc + 5, true, launches))) return rc;
+  CK(cudaMemsetAsync(v.loff, 0, 8, st));  // no row: loff[0] = 0 ends them
+  CK(cudaMemsetAsync(v.n_occ, 0, 8, st));
+  st_ve_group_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(v);
+  st_ve_rows_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(v);
+  launches += 2;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const uint64_t nl = S.h_sc.as<uint64_t>()[3], n_occ = S.h_sc.as<uint64_t>()[4];
+  float ms = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  CK(S.h_ve_lk.ensure(std::max<uint64_t>(nl, 1) * sizeof(tgi_validator_lookup)));
+  CK(S.h_ve_occ.ensure(std::max<uint64_t>(n_occ, 1) * 4));
+  if (nl) CK(cudaMemcpyAsync(S.h_ve_lk.p, v.out, nl * sizeof(tgi_validator_lookup), cudaMemcpyDeviceToHost, st));
+  if (n_occ) CK(cudaMemcpyAsync(S.h_ve_occ.p, v.svals, n_occ * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  S.ve_live = true;  // ve_e, ve_s, ve_elk, ve_rank and h_ve_lk hold the plan
+  S.ve_nl = nl;
+  out->n_edges = n;
+  out->n_cached = n - n_occ;
+  out->n_lookups = nl;
+  out->lookups = S.h_ve_lk.as<tgi_validator_lookup>();
+  out->occurrences = S.h_ve_occ.as<uint32_t>();
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  return TGI_OK;
+}
+
+// The validator edge pass over the plan: the outcomes' checks on the host; a thread per edge derives its update, one
+// block scans the counter, two scans and a compaction place the upsert rows (one synchronise); the two ordered set
+// inserts on the sets' stream; then the rows as tgi_state_edge_sql renders them.
+int tgi_state_validator_edges(tgi_ctx* c, const tgi_validator_outcome* outcomes, uint64_t n_outcomes,
+                              const tgi_validator_attempt* attempts, uint64_t n_attempts, int64_t blocked_count_in,
+                              int64_t now_sec, uint32_t rows_per_stmt, tgi_state_validator_edges_t* out) {
+  static const char* const who = "tgi_state_validator_edges";
+  if (!c || !out) return TGI_E_ARG;
+  CrawlState& S = c->state;
+  std::lock_guard<std::mutex> g(S.mu);
+  int rc;
+  if ((rc = st_init(c, S))) return rc;
+  if ((rc = sql_args(c, S, rows_per_stmt, 0, nullptr, 0, who, false))) return rc;
+  if (!S.ve_live) { set_err(c, "%s: no plan (tgi_state_validator_lookups)", who); return TGI_E_STATE; }
+  if (blocked_count_in < 0 || blocked_count_in > (1ll << 62)) { set_err(c, "%s: blocked_count_in %lld outside [0, 2^62]", who, (long long)blocked_count_in); return TGI_E_ARG; }
+  const uint64_t n = S.ve_n, nl = S.ve_nl;
+  if (n_outcomes != nl) { set_err(c, "%s: %llu outcomes for %llu lookups", who, (unsigned long long)n_outcomes, (unsigned long long)nl); return TGI_E_ARG; }
+  if ((nl && !outcomes) || (n_attempts && !attempts)) { set_err(c, "%s: outcomes or attempts is NULL", who); return TGI_E_ARG; }
+  CK(S.h_ve_aoff.ensure(std::max<uint64_t>(nl, 1) * 8));
+  if ((rc = ve_outcomes(c, S.h_ve_lk.as<tgi_validator_lookup>(), outcomes, nl, attempts, n_attempts, S.h_ve_aoff.as<uint64_t>(), who)))
+    return rc;
+  memset(out, 0, sizeof *out);
+  out->blocked_count_out = blocked_count_in;
+  out->crossed_at = TGI_VE_NOT_CROSSED;
+  if (!n) {
+    S.ve_live = false;
+    return TGI_OK;
+  }
+  cudaStream_t st = S.stream;
+  CK(S.ve_oc.ensure(std::max<uint64_t>(nl, 1) * sizeof(tgi_validator_outcome)));
+  CK(S.ve_aoff.ensure(std::max<uint64_t>(nl, 1) * 8));
+  CK(S.ve_at.ensure(std::max<uint64_t>(n_attempts, 1) * sizeof(tgi_validator_attempt)));
+  CK(S.ve_res.ensure(n * sizeof(tgi_validator_edge_result)));
+  CK(S.ve_flag.ensure(2 * n * 4));
+  CK(S.ve_pos.ensure(2 * (n + 1) * 8));
+  CK(S.ve_list.ensure(2 * n * 4));
+  CK(S.ve_names.ensure(2 * n * 32));
+  CK(S.sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_sc.ensure(ST_SC_COUNT * 8));
+  CK(S.h_ve_res.ensure(n * sizeof(tgi_validator_edge_result)));
+  if (nl) {
+    CK(cudaMemcpyAsync(S.ve_oc.p, outcomes, nl * sizeof(tgi_validator_outcome), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(S.ve_aoff.p, S.h_ve_aoff.p, nl * 8, cudaMemcpyHostToDevice, st));
+  }
+  if (n_attempts) CK(cudaMemcpyAsync(S.ve_at.p, attempts, n_attempts * sizeof(tgi_validator_attempt), cudaMemcpyHostToDevice, st));
+  uint64_t* dsc = S.sc.as<uint64_t>();  // [0] the count after the claim, [1] the crossing, [3] seed rows, [4] invalid rows
+  StVeApply a{};
+  a.e = S.ve_e.as<tgi_pending_claim_edge>();
+  a.s = S.ve_s.as<uint8_t>();
+  a.n = n;
+  a.elk = S.ve_elk.as<uint32_t>();
+  a.rank = S.ve_rank.as<uint32_t>();
+  a.oc = S.ve_oc.as<tgi_validator_outcome>();
+  a.aoff = S.ve_aoff.as<uint64_t>();
+  a.at = S.ve_at.as<tgi_validator_attempt>();
+  a.count_in = blocked_count_in;
+  a.res = S.ve_res.as<tgi_validator_edge_result>();
+  a.flag = S.ve_flag.as<uint32_t>();
+  a.pos = S.ve_pos.as<uint64_t>();
+  a.pos_i = a.pos + n + 1;
+  a.list = S.ve_list.as<uint32_t>();
+  a.keys = S.ve_names.as<uint8_t>();
+  a.sc = dsc;
+  uint32_t launches = 0;
+  CK(cudaEventRecord(S.t0, st));
+  st_ve_edge_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(a);
+  st_ve_counter_kernel<<<1, ST_VE_THREADS, 0, st>>>(a);
+  launches += 2;
+  if ((rc = launch_scan(c, st, S.tiles, a.flag, n, a.pos, dsc + 3, launches, true))) return rc;
+  if ((rc = launch_scan(c, st, S.tiles, a.flag + n, n, a.pos_i, dsc + 4, launches, true))) return rc;
+  st_ve_compact_kernel<<<st_grid(c, n), ST_THREADS, 0, st>>>(a);
+  launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(S.t1, st));
+  CK(cudaMemcpyAsync(S.h_sc.p, S.sc.p, ST_SC_COUNT * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(S.h_ve_res.p, a.res, n * sizeof(tgi_validator_edge_result), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, S.t0, S.t1);
+  const uint64_t* hs = S.h_sc.as<uint64_t>();
+  const uint64_t n_seed = hs[3], n_inv = hs[4], crossed = hs[1];
+  const int64_t count_out = (int64_t)hs[0];
+  {
+    std::lock_guard<std::mutex> fg(c->fr_mu);
+    cudaStream_t st0 = c->slots[0].stream;
+    KeySet& SI = c->sets[TGI_SET_INVALID];
+    KeySet& SS = c->sets[TGI_SET_SEEDS];
+    if (n_seed) {  // UpsertSeedChannelChatID fills chatIDCache
+      if ((rc = set_first_use(c, SS, false))) return rc;
+      if ((rc = frontier_insert_enqueue(c, SS, a.keys, nullptr, n_seed, nullptr))) return rc;
+      CK(cudaStreamSynchronize(st0));
+      if ((rc = frontier_insert_check(c, SS))) return rc;
+    }
+    if (n_inv) {  // MarkChannelInvalid: the names in, then every one of them stamped with the call's clock
+      const uint8_t* ikeys = a.keys + 32 * n;
+      if ((rc = set_first_use(c, SI, true))) return rc;
+      if ((rc = frontier_insert_enqueue(c, SI, ikeys, nullptr, n_inv, nullptr))) return rc;
+      CK(cudaStreamSynchronize(st0));
+      if ((rc = frontier_insert_check(c, SI))) return rc;
+      st_rw_stamp_kernel<<<st_grid(c, n_inv), ST_THREADS, 0, st0>>>(SI.dev, ikeys, n_inv, (long long)now_sec);
+      launches++;
+      CK(cudaGetLastError());
+      CK(cudaStreamSynchronize(st0));
+    }
+  }
+  out->n_edges = n;
+  out->edges = S.h_ve_res.as<tgi_validator_edge_result>();
+  out->blocked_count_out = count_out;
+  out->crossed_at = crossed;
+  out->kernel_ms = ms;
+  out->gpu_launches = launches;
+  StVeSql q{};
+  q.p.kind[0] = TGI_SQL_SEED_UPSERT;
+  q.p.kind[1] = TGI_SQL_INVALID_UPSERT;
+  q.p.kind[2] = TGI_SQL_ACCESS_EVENT;
+  q.p.kind[3] = TGI_SQL_EDGE_UPDATE;
+  const uint64_t rows[4] = {n_seed, n_inv, crossed != TGI_VE_NOT_CROSSED ? 1u : 0u, n};
+  for (int k = 0; k < 4; k++) {
+    q.p.rows[k] = rows[k];
+    q.p.k[k] = k == 2 ? 1u : rows_per_stmt;
+  }
+  q.a = a;
+  auto accept = [&]() { S.ve_live = false; };
+  return sql_render(c, S, q, st_ve_size_kernel, st_ve_emit_kernel, n_seed + n_inv + rows[2] + n, nullptr, 0, nullptr, 0,
+                    who, accept, S.h_ve_sql, S.h_ve_stmts, out);
 }
 
 }  // extern "C"

@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = [
     "tgi_state_pages_end", "tgi_state_pages_close", "tgi_state_pending_edges", "tgi_channel_batch",
     "tgi_state_read_pages", "tgi_state_read_layer", "tgi_state_layers", "tgi_state_edge_sql",
     "tgi_state_walkback", "tgi_state_validator_walkback", "tgi_state_rw_lookups", "tgi_state_rw_step", "tgi_set_export",
+    "tgi_state_validator_lookups", "tgi_state_validator_edges",
 ]
 
 
@@ -142,6 +143,10 @@ def lib() -> C.CDLL:
         L.tgi_state_rw_step.argtypes = [vp, vp, u64, C.c_int64, C.c_char_p, u32, C.c_int64, i32, u32,
                                         C.POINTER(abi.StateRwStepC)]
         L.tgi_set_export.argtypes = [vp, i32, vp, vp, u64, C.POINTER(u64)]
+        L.tgi_state_validator_lookups.argtypes = [vp, C.POINTER(abi.PendingClaimC), C.c_int64,
+                                                  C.POINTER(abi.StateValidatorLookupsC)]
+        L.tgi_state_validator_edges.argtypes = [vp, vp, u64, vp, u64, C.c_int64, C.c_int64, u32,
+                                                C.POINTER(abi.StateValidatorEdgesC)]
         _LIB = L
     return _LIB
 
@@ -1055,6 +1060,51 @@ class Engine:
                   "sequence_id": bytes(r["sequence_id"])} for r in res]
         stats = {"hits": list(out.hits), "misses": list(out.misses)}
         return spans, stats, self._st_stmts(out)
+
+    # --- validator edge pass: lookups of a claim, then the edges' outcomes ---------------------------------------------
+    def state_validator_lookups(self, edges, now_sec: int = 0) -> dict:
+        """the names of a ClaimPendingEdges result that need IsChannelDiscovered and t.me: edges = a list of dicts for
+        state_pack.pack_claimed_edges, or its packed tuple; now_sec = the clock of the invalid set's TTL.  Returns
+        {"lookups" (abi.VALIDATOR_LOOKUP rows), "occurrences" (u32 edge indices), "n_cached"}.  The device time is left
+        in self.state_ve_lookups_ms"""
+        from .state_pack import pack_claimed_edges
+        recs, blob = edges if isinstance(edges, tuple) else pack_claimed_edges(edges)
+        recs, blob = np.ascontiguousarray(recs, abi.PENDING_CLAIM_EDGE), np.ascontiguousarray(blob, np.uint8)
+        cin = abi.PendingClaimC(recs.ctypes.data, len(recs), blob.ctypes.data, len(blob))
+        out = abi.StateValidatorLookupsC()
+        self._check(lib().tgi_state_validator_lookups(self.h, C.byref(cin), now_sec, C.byref(out)))
+        self.state_ve_lookups_ms = float(out.kernel_ms)
+        self.state_ve_lookups_launches = int(out.gpu_launches)
+        return {"lookups": _view(out.lookups, int(out.n_lookups), abi.VALIDATOR_LOOKUP).copy(),
+                "occurrences": _view(out.occurrences, int(out.n_edges - out.n_cached), np.uint32).copy(),
+                "n_cached": int(out.n_cached)}
+
+    def state_validator_edges(self, outcomes, attempts, blocked_count_in: int = 0, now_sec: int = 0,
+                              rows_per_stmt: int = 1) -> tuple:
+        """the edge pass of the last state_validator_lookups: outcomes = one (discovered, claimed, n_attempts) per lookup
+        row, attempts = the rows' (kind (abi.VA_*), reason (abi.VR_*)) in row order, or abi.VALIDATOR_OUTCOME /
+        VALIDATOR_ATTEMPT arrays.  Returns (edges, counter, stmts): per edge {"status", "reason", "kind",
+        "blocked_count"} (abi.VS_*, VR_*, VK_*), {"out", "crossed_at" (None when not crossed)}, and [(kind (abi.SQL_*),
+        rows, sql, params)]; the device time and launches are left in self.state_ve_ms and self.state_ve_launches"""
+        if not isinstance(outcomes, np.ndarray):
+            outcomes = np.array([(d, c, n, 0) for d, c, n in outcomes], abi.VALIDATOR_OUTCOME)
+        if not isinstance(attempts, np.ndarray):
+            attempts = np.array(list(attempts), abi.VALIDATOR_ATTEMPT)
+        outcomes = np.ascontiguousarray(outcomes, abi.VALIDATOR_OUTCOME)
+        attempts = np.ascontiguousarray(attempts, abi.VALIDATOR_ATTEMPT)
+        out = abi.StateValidatorEdgesC()
+        self._check(lib().tgi_state_validator_edges(self.h, outcomes.ctypes.data if len(outcomes) else None,
+                                                    len(outcomes), attempts.ctypes.data if len(attempts) else None,
+                                                    len(attempts), blocked_count_in, now_sec, rows_per_stmt,
+                                                    C.byref(out)))
+        self.state_ve_ms = float(out.kernel_ms)
+        self.state_ve_launches = int(out.gpu_launches)
+        res = _view(out.edges, int(out.n_edges), abi.VALIDATOR_EDGE_RESULT)
+        edges = [{"status": int(r["status"]), "reason": int(r["reason"]), "kind": int(r["kind"]),
+                  "blocked_count": int(r["blocked_count"])} for r in res]
+        counter = {"out": int(out.blocked_count_out),
+                   "crossed_at": None if out.crossed_at == abi.VE_NOT_CROSSED else int(out.crossed_at)}
+        return edges, counter, self._st_stmts(out)
 
     @staticmethod
     def _st_stmts(out) -> list:

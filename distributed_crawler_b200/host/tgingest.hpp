@@ -507,6 +507,26 @@ class MessageProcessor {
       throw std::runtime_error(tgi_last_error(ctx_));
     return o;
   }
+  // Validator edge pass: the names of one ClaimPendingEdges result to ask (ValidatorLookups), then, with one outcome per
+  // lookup row and the rows' attempts in order, every edge's update, the blocked counter and the exec calls as
+  // StateEdgeSql's are read (ValidatorEdges).  The lookups' plan lives until the next ValidatorLookups or an accepted
+  // ValidatorEdges; the arrays stay valid until the next call of the pair.
+  tgi_state_validator_lookups_t ValidatorLookups(const std::vector<tgi_pending_claim_edge>& edges, std::string_view strs,
+                                                 int64_t now_sec) {
+    const tgi_pending_claim in{edges.data(), edges.size(), (const uint8_t*)strs.data(), strs.size()};
+    tgi_state_validator_lookups_t o{};
+    if (tgi_state_validator_lookups(ctx_, &in, now_sec, &o) != TGI_OK) throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
+  tgi_state_validator_edges_t ValidatorEdges(const std::vector<tgi_validator_outcome>& outcomes,
+                                             const std::vector<tgi_validator_attempt>& attempts, int64_t blocked_count_in,
+                                             int64_t now_sec, uint32_t rows_per_stmt) {
+    tgi_state_validator_edges_t o{};
+    if (tgi_state_validator_edges(ctx_, outcomes.data(), outcomes.size(), attempts.data(), attempts.size(), blocked_count_in,
+                                  now_sec, rows_per_stmt, &o) != TGI_OK)
+      throw std::runtime_error(tgi_last_error(ctx_));
+    return o;
+  }
   // Layer reads: GetLayerByDepth with a runner's selection (TGI_SELECT_*), GetPage of many rows, and the layer summary
   // (GetMaxDepth, FindIncompleteCrawl's page test).  ReadLayer's selected rows go to StatePagesBegin as they are; with
   // messages each page's list is msgs[msg_first[k] .. + pages[k].n_msgs).  The arrays stay valid until the next state call.

@@ -71,3 +71,21 @@ def pack_claimed_batches(batches):
         edges["str_len"] = a[:, 2:4]
         edges["cls"] = a[:, 4]
     return recs, edge_off, edges, np.frombuffer(bytes(blob) + b"\0" * 16, np.uint8).copy()
+
+
+def pack_claimed_edges(edges):
+    """-> (tgi_pending_claim_edge array, string blob) of a ClaimPendingEdges result: each edge a dict with "pending_id"
+    and its strings as bytes (abi.VE_STRINGS; missing = empty), in claim order.  Equal strings are stored once."""
+    recs = np.zeros(len(edges), abi.PENDING_CLAIM_EDGE)
+    blob = bytearray()
+    at = {}
+    for i, e in enumerate(edges):
+        recs[i]["pending_id"] = e["pending_id"]
+        for k, name in enumerate(abi.VE_STRINGS):
+            s = e.get(name, b"")
+            o = at.get(s)
+            if o is None:
+                o = at[s] = len(blob)
+                blob.extend(s)
+            recs[i]["str_off"][k], recs[i]["str_len"][k] = o, len(s)
+    return recs, np.frombuffer(bytes(blob) + b"\0" * 16, np.uint8).copy()

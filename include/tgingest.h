@@ -1555,6 +1555,157 @@ int tgi_state_rw_step(tgi_ctx* ctx, const tgi_rw_outcome* outcomes, uint64_t n_o
  * in first-occurrence order, and with stamps_sec (TGI_SET_INVALID only) their stamps; *n = the set's count. */
 int tgi_set_export(tgi_ctx* ctx, int which, uint8_t* keys32, int64_t* stamps_sec, uint64_t cap, uint64_t* n);
 
+/* Validator edge pass — the edge validator of a validator pod (runEdgeValidation + validateSingleEdge,
+ * crawl/validator.go:94-309) for one ClaimPendingEdges result in two calls: tgi_state_validator_lookups lists the names
+ * that need the database and t.me; the caller asks them; tgi_state_validator_edges applies the outcomes to the resident
+ * sets, replays the blocked-state counter and renders every binding call.  The caller keeps no copy of
+ * invalidChannelCache (TGI_SET_INVALID) or chatIDCache (TGI_SET_SEEDS).
+ *   Input    the claimed edges in the order ClaimPendingEdges returned them: pending_id and the destination, crawl_id
+ *            and source_type as (offset, length) pairs into strs.  crawl_id and source_type are checked, not read.
+ *   Classes  an edge whose destination is in TGI_SET_INVALID live at now_sec (IsInvalidChannel, daprstate.go:3556-3564)
+ *            is invalid / cached_invalid.  Every other name is one lookup row, in first-occurrence order, with its
+ *            occurrences' edge indices in edge order (m of them): names are grouped by the first-occurrence table of
+ *            tgi_state_rw_lookups, so every occurrence of a name shares its row.
+ *   Lookups  tgi_state_validator_lookups changes nothing.  Its plan stays on the device until the next
+ *            tgi_state_validator_lookups or an accepted tgi_state_validator_edges; other state calls (the walkback
+ *            processor's tgi_state_validator_walkback runs beside the HTTP phase) leave it.
+ *   Shim     per lookup row: one IsChannelDiscovered; discovered stops there.  Else up to m HTTP attempts, the j-th for
+ *            occurrence j, stopping at the first final one (TGI_VA_VALID, _NOT_CHANNEL, _INVALID): a transient, blocked or
+ *            unknown-status attempt goes on to the next occurrence, which in the reference validates again.  After VALID
+ *            one ClaimDiscoveredChannel with that occurrence's crawl_id.  Deviation from the reference: IsChannelDiscovered
+ *            is asked once per name, not per occurrence, and a name's attempts are made together instead of interleaved
+ *            with other names'.  The outcomes are the reference's unless another pod claims the name during the claim or
+ *            t.me answers differently over time.
+ *   Outcomes one tgi_validator_outcome per lookup row ({discovered, claimed, n_attempts}) and the rows' attempts in
+ *            row order, each {kind TGI_VA_*, reason TGI_VR_NONE / _NOT_SUPERGROUP / _NOT_FOUND (what ValidateChannelHTTP
+ *            returns, channelvalidator.go:136-149)}.  The reason is read for NOT_CHANNEL and INVALID only.
+ *   Edges    per edge in claim order, status / reason / kind: a discovered name's occurrences are duplicate.  Occurrence
+ *            j < n_attempts takes attempt j: VALID is valid when claimed, else duplicate; NOT_CHANNEL / INVALID are that
+ *            status with the attempt's reason; OTHER is invalid / unknown_status; TRANSIENT and BLOCKED are pending.  A
+ *            later occurrence follows the final attempt: duplicate after VALID (the database has the name, claimed or
+ *            not), invalid / cached_invalid after NOT_CHANNEL or INVALID.  Every kind is TGI_VK_DEFINITIVE but
+ *            TRANSIENT's and BLOCKED's.
+ *   Replay   the counter from blocked_count_in over the edges' kinds (:153-176): blocked x + 1, transient max(x - 1, 0),
+ *            definitive 0.  Each is the map x -> max(x + a, b), and their composition is associative, so a scan computes
+ *            every edge's count.  crossed_at = the first blocked edge whose count reaches TGI_VE_BLOCKED_THRESHOLD (the
+ *            state becomes active and InsertAccessEvent runs), else TGI_VE_NOT_CROSSED.  The caller keeps active and
+ *            lastProbeAt and claims only while not active, so every call starts from a state that is not active.
+ *   Sets     TGI_SET_INVALID: each NOT_CHANNEL / INVALID name stamped at now_sec (MarkChannelInvalid; an expired stamp is
+ *            replaced).  TGI_SET_SEEDS: each claimed VALID name (UpsertSeedChannelChatID).  Both in edge order.
+ *            TGI_SET_DISCOVERED is not touched: the validator never calls AddDiscoveredChannel.
+ *   Rows     seed_channels upserts [name, 0] (TGI_SQL_SEED_UPSERT), invalid_channels upserts [name, reason]
+ *            (TGI_SQL_INVALID_UPSERT), at most one access event ["ip_blocked"] (TGI_SQL_ACCESS_EVENT), then one
+ *            pending_edges update [status, reason, pending_id] per edge (TGI_SQL_EDGE_UPDATE, daprstate.go:3999-4006).
+ *   Order    the four kinds in that order, each in edge order, so each edge's own calls keep the reference's order.
+ *            rows_per_stmt = k rows per statement for the upserts and updates by tgi_state_edge_sql's rule; k = 1 gives
+ *            the reference's calls byte for byte.  The update of k > 1 rows is "UPDATE pending_edges AS e SET
+ *            validation_status = v.s, validation_reason = v.r, validated_at = NOW() FROM (VALUES ($1, $2, $3::integer),
+ *            ...) AS v(s, r, id) WHERE e.pending_id = v.id;", which has not been run against Postgres.  No row takes a
+ *            crawl_id or the clock, so the call takes neither.
+ *   Cost     lookups: the upload, a thread per edge builds its key, the first-occurrence table, a thread per edge
+ *            classifies it, a scan, a stable radix sort by first occurrence, a thread per sorted edge places its row and
+ *            occurrence; two synchronises.  edges: a thread per edge derives its outcome, one block scans the counter
+ *            maps (8 edges per thread per pass), two scans and a compaction (one synchronise), the two ordered set
+ *            inserts, then the rows as tgi_state_edge_sql renders them.  An empty claim launches nothing.
+ *   Errors   every check runs before anything changes: a refused call leaves the sets and the plan as they were.
+ *            TGI_E_ARG: lookups: claim or a NULL array with a count, 2^32 - 1 edges or more, a string outside strs, a
+ *            destination that is empty or longer than 32 bytes (the hand-off never writes one), a pending_id twice.
+ *            edges: k outside [1, 8191], blocked_count_in < 0, a NULL array with a count, n_outcomes other than the
+ *            lookup count, the attempts' total other than n_attempts, an unknown code (discovered or claimed past 1, a
+ *            kind past TGI_VA_BLOCKED, a reason past TGI_VR_NOT_FOUND), discovered with attempts, an undiscovered row
+ *            with no attempt or more than m, a final attempt before the last one, a last attempt that is not final while
+ *            fewer than m were made, claimed without a final VALID.  TGI_E_STATE: edges without a plan.  After
+ *            TGI_E_CAPACITY or TGI_E_CUDA the set inserted first may hold its keys.  Lock order: the state, then the
+ *            sets.  All of out lives in pinned memory until the next call of the pair.                                 */
+#define TGI_VE_DESTINATION 0           /* tgi_pending_claim_edge strings                                              */
+#define TGI_VE_CRAWL_ID 1
+#define TGI_VE_SOURCE_TYPE 2
+#define TGI_VA_VALID 0                 /* attempt kinds: ValidateChannelHTTP's status "valid"                         */
+#define TGI_VA_NOT_CHANNEL 1           /* "not_channel"                                                               */
+#define TGI_VA_INVALID 2               /* "invalid"                                                                   */
+#define TGI_VA_OTHER 3                 /* any other status                                                            */
+#define TGI_VA_TRANSIENT 4             /* an error other than ErrBlocked, or a cancelled rate-limit wait              */
+#define TGI_VA_BLOCKED 5               /* ErrBlocked                                                                  */
+#define TGI_VR_NONE 0                  /* validation reasons: ""                                                      */
+#define TGI_VR_NOT_SUPERGROUP 1
+#define TGI_VR_NOT_FOUND 2
+#define TGI_VR_CACHED_INVALID 3        /* results only                                                                */
+#define TGI_VR_UNKNOWN_STATUS 4        /* results only                                                                */
+#define TGI_VS_PENDING 0               /* validation statuses: "pending"                                              */
+#define TGI_VS_VALID 1
+#define TGI_VS_DUPLICATE 2
+#define TGI_VS_INVALID 3
+#define TGI_VS_NOT_CHANNEL 4
+#define TGI_VK_DEFINITIVE 0            /* edgeOutcomeKind                                                             */
+#define TGI_VK_TRANSIENT 1
+#define TGI_VK_BLOCKED 2
+#define TGI_VE_BLOCKED_THRESHOLD 5     /* blockedThreshold (validator.go:35)                                          */
+#define TGI_VE_NOT_CROSSED 0xFFFFFFFFFFFFFFFFull
+#define TGI_SQL_ACCESS_EVENT 10        /* InsertAccessEvent (daprstate.go:4385-4391)                                  */
+#define TGI_SQL_EDGE_UPDATE 11         /* UpdatePendingEdge                                                           */
+typedef struct tgi_pending_claim_edge { /* 48 bytes: one PendingEdge                                                  */
+  int64_t pending_id;
+  uint64_t str_off[3];                 /* TGI_VE_*: strs[str_off[f] .. + str_len[f])                                  */
+  uint32_t str_len[3];
+  uint32_t reserved;
+} tgi_pending_claim_edge;
+typedef struct tgi_pending_claim {
+  const tgi_pending_claim_edge* edges; /* [n_edges] in claim order                                                    */
+  uint64_t n_edges;
+  const uint8_t* strs;
+  uint64_t strs_len;
+} tgi_pending_claim;
+typedef struct tgi_validator_lookup {  /* 48 bytes: one name to ask                                                   */
+  uint8_t name[32];                    /* zero padded                                                                 */
+  uint64_t occ_off;                    /* its edges: occurrences[occ_off .. + m), ascending                           */
+  uint32_t m;
+  uint8_t name_len;
+  uint8_t reserved[3];
+} tgi_validator_lookup;
+typedef struct tgi_state_validator_lookups_t {
+  uint64_t n_edges;
+  uint64_t n_cached;                   /* edges decided by TGI_SET_INVALID                                            */
+  uint64_t n_lookups;
+  const tgi_validator_lookup* lookups; /* [n_lookups] in first-occurrence order (pinned)                              */
+  const uint32_t* occurrences;         /* [n_edges - n_cached] edge indices (pinned)                                  */
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies)               */
+  uint32_t gpu_launches;
+} tgi_state_validator_lookups_t;
+typedef struct tgi_validator_outcome { /* 16 bytes: one lookup row                                                    */
+  uint32_t discovered;                 /* IsChannelDiscovered said true                                               */
+  uint32_t claimed;                    /* ClaimDiscoveredChannel inserted the name                                    */
+  uint32_t n_attempts;                 /* HTTP attempts, the next n_attempts entries of attempts                      */
+  uint32_t reserved;
+} tgi_validator_outcome;
+typedef struct tgi_validator_attempt { /* 8 bytes                                                                     */
+  uint32_t kind;                       /* TGI_VA_*                                                                    */
+  uint32_t reason;                     /* TGI_VR_NONE, _NOT_SUPERGROUP, _NOT_FOUND                                    */
+} tgi_validator_attempt;
+typedef struct tgi_validator_edge_result { /* 16 bytes: one edge's UpdatePendingEdge                                  */
+  int64_t blocked_count;               /* consecutiveCount after the edge                                             */
+  uint8_t status;                      /* TGI_VS_*                                                                    */
+  uint8_t reason;                      /* TGI_VR_*                                                                    */
+  uint8_t kind;                        /* TGI_VK_*                                                                    */
+  uint8_t reserved[5];
+} tgi_validator_edge_result;
+typedef struct tgi_state_validator_edges_t {
+  uint64_t n_edges;
+  const tgi_validator_edge_result* edges; /* [n_edges] in claim order (pinned)                                        */
+  int64_t blocked_count_out;
+  uint64_t crossed_at;                 /* the edge that entered the blocked state, or TGI_VE_NOT_CROSSED              */
+  uint64_t n_stmts;
+  const tgi_state_edge_stmt* stmts;    /* [n_stmts] in execution order (pinned)                                       */
+  const uint8_t* data;                 /* the texts, then the params (pinned)                                         */
+  uint64_t data_len;
+  float kernel_ms;                     /* device time of the call's kernels and scans (not the copies)               */
+  uint32_t gpu_launches;
+} tgi_state_validator_edges_t;
+int tgi_state_validator_lookups(tgi_ctx* ctx, const tgi_pending_claim* claim, int64_t now_sec,
+                                tgi_state_validator_lookups_t* out);
+int tgi_state_validator_edges(tgi_ctx* ctx, const tgi_validator_outcome* outcomes, uint64_t n_outcomes,
+                              const tgi_validator_attempt* attempts, uint64_t n_attempts, int64_t blocked_count_in,
+                              int64_t now_sec, uint32_t rows_per_stmt, tgi_state_validator_edges_t* out);
+
 /* Layer reads — the reads that begin every depth of both runners (standalone/runner.go:594-700,
  * dapr/standalone.go:948-1021 and 454-498) and FindIncompleteCrawl's page test, by row, so a shim that runs discovery on
  * the device never holds a copy of the page table: layer read, tgi_state_pages_begin of the selected rows, one bulk
